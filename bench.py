@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- images/sec of the MapNet/PoseNet ResNet-34 training step on B200.
+"""bench.py -- images/sec of the MapNet/PoseNet ResNet-34 training step on H100.
 
-    python bench.py --gpus N --steps K --warmup W [--workload posenet_bs64|mapnet_n32t3]
+    python bench.py --gpus N --steps K --warmup W [--workload posenet_bs64|mapnet_n32t3] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference ...      # the reference's CPU path (oracle port) on host cores
 
@@ -10,6 +10,15 @@ allreduce of the flat gradient buffer], Adam.  `value` = whole-job images/sec
 with inputs resident in HBM; `e2e` = the same step through the reference-facing
 nn.Module surface with HOST (pinned) inputs, H2D copies and loss.item() inside
 the timed region.  Prints ONE JSON line on rank 0.
+
+--dump-outputs DIR writes what the LAST timed step computed, as the caller of the step receives it, to DIR/<name>.npy:
+loss (float64), pred (the model output, float32), crit_params (the criterion's learned scalars after the step) and a
+fixed seeded sample of 2^20 entries each of the updated parameters and of their gradients (float32).  Inputs,
+initial weights and dropout masks are seeded, so two builds run with the same arguments can be compared output for
+output.  Split-K partial sums (conv wgrad, head GEMMs) are added in a fixed order, so the fp32 arithmetic of a step
+does not depend on CTA timing; the BatchNorm statistics are accumulated with fp64 atomics, whose order does vary, but
+their rounding (~1e-16 relative) only reaches the fp32 values in rare ties.  Two runs with the same arguments wrote
+bit-identical outputs on one H100.  Nothing is written anywhere else.
 """
 import argparse
 import json
@@ -88,12 +97,13 @@ def _peaks():
         d = json.load(open(p))
         return dict(hbm=float(d["hbm_gbs"]), tc_burst=float(d["bf16_tflops"]),
                     tc_sustained=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), src="measured")
-    return dict(hbm=6650.0, tc_burst=1590.0, tc_sustained=1400.0, src="fallback")
+    # NVIDIA data sheet, H100 SXM at 700 W: 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s (a bound, not a measured rate)
+    return dict(hbm=3350.0, tc_burst=989.0, tc_sustained=989.0, src="datasheet")
 
 
 def _ncu_traffic():
     """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant conv kernel, from the committed
-    `ncu --set full` capture (profiles/ncu_traffic.json, written from the CSV export by tools/ncu_summary.py).
+    `ncu --set full` capture (ncu_traffic.json under profiles/, written from the CSV export by tools/ncu_summary.py).
     The capture records the digest of the kernel sources it was taken with; a capture of OTHER sources than the ones
     this run was built from is reported as stale (traffic = None) instead of being passed off as a measurement of
     this build.  None when no capture is committed."""
@@ -232,7 +242,7 @@ def run_reference(args, cfg, rank, world):
 
 
 # --------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # --------------------------------------------------------------------------------
 def run_b200(args, cfg, rank, local_rank, world):
     import torch
@@ -246,7 +256,7 @@ def run_b200(args, cfg, rank, local_rank, world):
     from oracle import mapnet_oracle as O      # FLOP model only (roofline denominator)
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device -- the B200 arm has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device -- the GPU arm has no CPU fallback")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -271,8 +281,11 @@ def run_b200(args, cfg, rank, local_rank, world):
     model.cuda(); crit.cuda(); model.train()
     dp = None
 
+    last_out = [None]
+
     def eager_step(x, targ):
         out = model(x)
+        last_out[0] = out.detach()
         loss = crit(out, targ)
         opt.learner.zero_grad()
         loss.backward()
@@ -325,10 +338,13 @@ def run_b200(args, cfg, rank, local_rank, world):
     t_wall0 = time.time()
     e0.record()
     for i in range(args.steps):
-        step(*dev_batches[i % nb])
+        last_loss = step(*dev_batches[i % nb])
     e1.record()
     barrier()
     t_wall1 = time.time()
+    dump = None
+    if args.dump_outputs and rank == 0:
+        dump = snapshot_outputs(last_loss, step.out if args.graph else last_out[0], model, crit)
     launches = (L.mapnet_launch_count() - lc0) // max(1, args.steps)
     if args.graph:
         launches = graph_launches       # kernels inside the replayed graphs (counted while capturing)
@@ -414,8 +430,8 @@ def run_b200(args, cfg, rank, local_rank, world):
     # steps are enqueued first WITHOUT a sync, so the device is busy while the host runs ahead and the
     # profiled launches are already queued when the device reaches them: no host-side gap lands
     # inside a bracket.  What remains is the isolation itself: a bracketed launch cannot overlap its prologue /
-    # pipeline fill / tail with its neighbours as it does in the CUDA-graph step, +5-7 us per launch
-    # (profiles/r01d_conv_microbench.txt, block 3 vs block 2) -- `achieved` is therefore a LOWER bound.
+    # pipeline fill / tail with its neighbours as it does in the CUDA-graph step -- `achieved` is therefore a
+    # LOWER bound.
     for i in range(2):
         step(*dev_batches[i % nb])
     if rank == 0:
@@ -437,13 +453,13 @@ def run_b200(args, cfg, rank, local_rank, world):
                 per_class[nm] = {"tflops": fl3[k] / (ms3[k] * 1e-3) / 1e12, "ms_per_step": ms3[k] / psteps,
                                  "launches_per_step": n3[k] // psteps}
         peak = peaks["tc_burst"]      # every bracketed launch runs alone for 10-50 us at full clocks: the burst figure
-        kname = {"bf16": "k_tc_conv / k_tc_conv2 / k_tc_conv_halo / k_tc_wgrad(2) (all conv launches of a step, bf16 operands)",
-                 "tc_split": "k_tc_conv / k_tc_conv2 / k_tc_wgrad(2) (all conv launches of a step; fp16 hi/lo operand planes, "
-                             "4 tcgen05 MMAs per algorithmic product: the tensor pipe executes 4x the algorithmic FLOPs)"}
+        kname = {"bf16": "k_tc_conv / k_tc_wgrad (all conv launches of a step, bf16 operands)",
+                 "tc_split": "k_tc_conv / k_tc_wgrad (all conv launches of a step; fp16 hi/lo operand planes, "
+                             "4 wgmma products per algorithmic product: the tensor cores execute 4x the algorithmic FLOPs)"}
         nt = _ncu_traffic()
         roof = {"bound": "tensor", "kernel": kname.get(args.precision, "k_conv_simt (fp32 CUDA-core engine)"),
                 "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                "peak_source": "%s (MEASURED_PEAKS.json bf16_tflops, burst)" % peaks["src"],
+                "peak_source": "%s (MEASURED_PEAKS.json bf16_tflops if present, else the H100 SXM data sheet)" % peaks["src"],
                 "frac_of_sustained_peak": achieved / peaks["tc_sustained"],
                 "mma_flops_per_algorithmic_flop": 4 if args.precision == "tc_split" else 1,
                 "traffic": (None if (nt is None or nt.get("stale")) else nt.get("dram_bytes_per_launch")),
@@ -456,7 +472,7 @@ def run_b200(args, cfg, rank, local_rank, world):
 
     # ---------------- side by side: (img/s, parity) of the two tensor-core modes, N=1 only ----------------
     # bf16 operands: the throughput mode (pose ~5e-2 off the fp32 reference: the format, not the kernels).
-    # tc_split: the same tcgen05 engines on fp16 hi/lo operand planes, 4 MMAs per product -- meets the north-star
+    # tc_split: the same wgmma engines on fp16 hi/lo operand planes, 4 MMAs per product -- meets the north-star
     # 1e-4 bar (tests/test_gpu_step.py::test_step_tc_split_strict*).  Both are measured here, in this run.
     modes = None
     if rank == 0 and world == 1 and not args.no_modes and args.precision in ("bf16", "tc_split"):
@@ -489,8 +505,7 @@ def run_b200(args, cfg, rank, local_rank, world):
         modes = {args.precision: {"images_per_s": value, "ms_per_step": ms_step, "parity_vs_reference": parity[args.precision]},
                  other: {"images_per_s": frames(cfg) / (oms / 1000.0), "ms_per_step": oms, "steps": nsteps,
                          "parity_vs_reference": parity[other]},
-                 "note": "same workload, same run, CUDA-graph step, inputs resident in HBM; fp32 CUDA-core engine "
-                         "(precision fp32, also 1e-4): 957 img/s (profiles/r02c_bench_posenet_bs64_fp32.json)"}
+                 "note": "same workload, same run, CUDA-graph step, inputs resident in HBM"}
         del g2, model2, net2
 
     # ---------------- cpu baseline: oracle port on the host cores (rank 0, N=1 only) -------------
@@ -528,7 +543,7 @@ def run_b200(args, cfg, rank, local_rank, world):
                        "criterion": cfg["kind"], "optimizer": "adam (fused, flat)", "droprate": args.droprate,
                        "parallelism": "dp%d" % world, "precision": args.precision,
                        "cuda_graph": bool(args.graph), "eager_ms_per_step": eager_ms,
-                       "l2": "per-step working set (activations + gradients, >3 GB) exceeds the 126 MB L2; "
+                       "l2": "per-step working set (activations + gradients, >3 GB) exceeds the 50 MB L2; "
                              "%d distinct input batches rotate" % nb},
             "e2e": {"value": e2e_val, "unit": "images/s", "ms_per_step": e2e_ms, "h2d_bytes_per_step": h2d,
                     "d2h_bytes_per_step": 4},
@@ -538,17 +553,8 @@ def run_b200(args, cfg, rank, local_rank, world):
             "cpu_baseline": cpu,
             "precision_modes": modes,
         }
-        if world > 1 and args.workload != "posenet_bs64":
-            # the default workload differs between N = 1 (posenet_bs64, BASELINE configs[1]) and N > 1 (configs[3]): the
-            # weak-scaling baseline of THIS workload is its own one-GPU line, not the N = 1 default line
-            n1 = {"mapnet_n32t3": (19172.4, "profiles/r02c_bench_mapnet_n32t3.json"),
-                  "mapnetpp_n16t10": (20499.1, "profiles/r02c_bench_mapnetpp_n16t10.json")}.get(args.workload)
-            if n1 is not None and args.precision == "bf16":
-                line["config"]["one_gpu_same_workload"] = {
-                    "images_per_s": n1[0], "source": n1[1],
-                    "note": "bench.py --gpus 1 defaults to posenet_bs64; weak-scaling efficiency of this line = "
-                            "value / (n_gpus x images_per_s), with `python bench.py --workload %s` as the N = 1 run"
-                            % args.workload}
+        if dump is not None:
+            write_outputs(args.dump_outputs, dump)
         print(json.dumps(line), flush=True)
     if world > 1:
         # the measurement is complete and printed: a communicator teardown that stalls (CUDA graphs holding captured NCCL
@@ -564,6 +570,36 @@ def run_b200(args, cfg, rank, local_rank, world):
         torch.cuda.synchronize()
         dist.barrier()
         dist.destroy_process_group()
+
+
+DUMP_SAMPLE = 1 << 20
+
+
+def snapshot_outputs(loss, pred, model, crit):
+    """Host copies of what one training step hands its caller (see the module docstring)."""
+    import numpy as np
+    import torch
+    with torch.no_grad():
+        params = [p for p in model.parameters()]
+        flat_p = torch.cat([p.detach().reshape(-1).float() for p in params])
+        flat_g = torch.cat([(p.grad.reshape(-1).float() if p.grad is not None else torch.zeros(p.numel(), device=p.device))
+                            for p in params])
+        idx = np.sort(np.random.default_rng(0).choice(flat_p.numel(), size=min(DUMP_SAMPLE, flat_p.numel()), replace=False))
+        it = torch.from_numpy(idx).to(flat_p.device)
+        out = {"loss": np.array([float(loss)], dtype=np.float64),
+               "pred": pred.float().cpu().numpy(),
+               "crit_params": np.array([float(p) for p in crit.parameters()], dtype=np.float32),
+               "params_sample": flat_p[it].cpu().numpy(),
+               "grads_sample": flat_g[it].cpu().numpy(),
+               "sample_index": idx.astype(np.float64)}
+    return out
+
+
+def write_outputs(d, arrays):
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), a)
 
 
 def main():
@@ -583,7 +619,13 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", dest="graph", action="store_false",
                     help="run the step eagerly instead of replaying it as CUDA graphs")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step to DIR/<name>.npy (see the module docstring)")
     args = ap.parse_args()
+    if args.steps is not None and args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.warmup is not None and args.warmup < 0:
+        ap.error("--warmup must not be negative")
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

@@ -9,9 +9,7 @@ import os
 from ctypes import c_char_p, c_float, c_int, c_int64, c_uint64, c_void_p, POINTER
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# MAPNET_LIB_VARIANT=e8: a library built with MAPNET_BUILD_EPI_WARPS=8 (geomapnet_b200/build.py), for A/B measurements
-_VARIANT = os.environ.get("MAPNET_LIB_VARIANT", "")
-LIB_PATH = os.path.join(_HERE, "csrc", "libmapnet_b200%s.so" % (("_" + _VARIANT) if _VARIANT else ""))
+LIB_PATH = os.path.join(_HERE, "csrc", "libmapnet_b200.so")
 
 PREC = {"fp32": 0, "bf16": 1, "bf16_simt": 2, "tc_split": 3}
 LOSS_MODE = {"posenet": 0, "mapnet": 1, "online": 2, "online_gps": 3}
@@ -30,7 +28,7 @@ def lib():
     if not os.path.exists(LIB_PATH):
         raise MapNetLibError(
             "geomapnet_b200: %s is missing -- build it with `python -m geomapnet_b200.build` "
-            "(nvcc, sm_100a).  There is no fallback path." % LIB_PATH)
+            "(nvcc, sm_90a).  There is no fallback path." % LIB_PATH)
     L = ctypes.CDLL(LIB_PATH)
     L.mapnet_last_error.restype = c_char_p
     L.mapnet_abi_version.restype = c_int

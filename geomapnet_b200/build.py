@@ -1,10 +1,10 @@
-"""Builds geomapnet_b200/csrc/libmapnet_b200.so in-tree with nvcc for sm_100a.
+"""Builds geomapnet_b200/csrc/libmapnet_b200.so in-tree with nvcc for sm_90a (H100).
 
     python -m geomapnet_b200.build [--force]
 
 The shared library is a plain C ABI (include/mapnet_b200.h): no torch, no
-pybind -- Python binds it with ctypes (geomapnet_b200/_lib.py).  It is git-ignored
-but travels to the GPU box with the gpurun snapshot.
+pybind -- Python binds it with ctypes (geomapnet_b200/_lib.py).  It is a build
+product and git-ignored.
 """
 import hashlib
 import os
@@ -14,19 +14,13 @@ from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-# MAPNET_BUILD_EPI_WARPS=4|8: epilogue warps per CTA of the tcgen05 conv engines (conv_tc.cu, MN_EPI_WARPS).  The
-# non-default value builds a SECOND library (libmapnet_b200_e<N>.so, loaded with MAPNET_LIB_VARIANT=e<N>) so both
-# can be measured in one GPU session; the default is what the package loads.
-DEFAULT_EPI_WARPS = 4
-EPI_WARPS = int(os.environ.get("MAPNET_BUILD_EPI_WARPS", DEFAULT_EPI_WARPS))
-_SUFFIX = "" if EPI_WARPS == DEFAULT_EPI_WARPS else "_e%d" % EPI_WARPS
-OUT = os.path.join(CSRC, "libmapnet_b200%s.so" % _SUFFIX)
-OBJ = os.path.join(CSRC, "_obj" + _SUFFIX)
+OUT = os.path.join(CSRC, "libmapnet_b200.so")
+OBJ = os.path.join(CSRC, "_obj")
 SOURCES = ["api.cu", "net.cu", "bn.cu", "conv_simt.cu", "conv_tc.cu", "layout.cu", "head.cu", "loss.cu", "adam.cu",
            "preprocess.cu", "pgo.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
-         "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v", "-DMN_EPI_WARPS=%d" % EPI_WARPS]
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
+         "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
 def _digest():

@@ -1,4 +1,4 @@
-"""Fused B200 criteria behind the reference's nn.Module surface.
+"""Fused GPU criteria behind the reference's nn.Module surface.
 
 Host-side mirror of /root/reference/common/criterion.py: PoseNetCriterion
 (:33-52), MapNetCriterion (:54-109), MapNetOnlineCriterion (:111-184) with the

@@ -123,7 +123,7 @@ int launch_adam(float* p, const float* g, float* m, float* v, long long n, float
                 float eps, float wd, float bc1, float bc2, float gscale, const float* sqnorm_or_null,
                 float max_norm, int* step_dev, cudaStream_t st) {
   long long grid = ((n >> 2) + 255) / 256;
-  if (grid > 148LL * 8) grid = 148LL * 8;
+  if (grid > kNumSMs * 8LL) grid = kNumSMs * 8LL;
   if (grid < 1) grid = 1;
   if (step_dev != nullptr) {
     MN_LAUNCH(k_inc_i32, 1, 1, 0, st, step_dev);

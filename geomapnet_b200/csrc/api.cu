@@ -228,7 +228,7 @@ int mapnet_test_dgrad_shortcut(int B, int Hi, int Wi, int Ci, int Co, const void
   return r;
 }
 
-// One tcgen05 conv launch WITH its fused epilogue, as the training step runs it (bf16 mode):
+// One wgmma conv launch WITH its fused epilogue, as the training step runs it (bf16 mode):
 //   kind 0 (fprop):  out = conv(in0, wmat);  sums[0..1][c] = (sum out, sum out^2) over the stored bf16 values
 //                    -- the BatchNorm batch statistics the step takes from the conv epilogue;
 //   kind 1 (dgrad):  g = conv_dgrad(in0, wmat) [+ residual], gated by the consumer BatchNorm's ReLU
@@ -317,7 +317,7 @@ int mapnet_test_stem(int B, int H, int W, const float* x_nchw, const float* w_oi
   return r;
 }
 
-// micro-benchmark of one tcgen05 conv launch configuration (plan built once, CUDA-event timing)
+// micro-benchmark of one wgmma conv launch configuration (plan built once, CUDA-event timing)
 int mapnet_bench_conv(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* in0,
                       const void* in1, const void* wmat, void* out, int iters, float* host_ms) {
   MN_TRY(require_device());

@@ -127,7 +127,7 @@ k_channel_sums(const T* __restrict__ a, const TZ* __restrict__ zmask, const T* _
 static int sums_grid(long long M, int C) {
   const int rows_par = kEwThreads / (C >> 3);
   long long want = (M + (long long)rows_par * 8 - 1) / ((long long)rows_par * 8);   // >= 8 rows per thread
-  const long long cap = 148LL * 4;
+  const long long cap = (long long)kNumSMs * 4;
   if (want < 1) want = 1;
   return (int)(want < cap ? want : cap);
 }
@@ -147,7 +147,7 @@ static int launch_sums(int mode, const T* a, const TZ* zmask, const T* y, const 
   return 0;
 }
 
-// finalize for statistics accumulated by the tcgen05 conv epilogue (conv_tc.cu): sum the
+// finalize for statistics accumulated by the wgmma conv epilogue (conv_tc.cu): sum the
 // replicas, produce mean / invstd / scale / shift, update the running stats, reset the replicas
 // block = 32 channels x 32 replicas: coalesced replica loads, shared-memory reduction over replicas
 __global__ void __launch_bounds__(1024)
@@ -377,7 +377,7 @@ static int slice_grid_x(long long M, int C) {
   if (per_sm == 0) { const char* e = getenv("MAPNET_EW_BLOCKS_PER_SM"); per_sm = e ? atoi(e) : 8; if (per_sm < 1 || per_sm > 8) per_sm = 8; }
   const long long slices = C >> 6;
   long long gx = (M + 31) / 32;
-  long long cap = (148LL * per_sm) / slices;
+  long long cap = ((long long)kNumSMs * per_sm) / slices;
   if (cap < 1) cap = 1;
   if (gx > cap) gx = cap;
   return (int)(gx < 1 ? 1 : gx);
@@ -462,11 +462,10 @@ k_bn_apply_lazy(const T* __restrict__ y, const void* __restrict__ res, TZ* __res
 static int ew_grid(long long n) {
   long long g = (n + kEwThreads - 1) / kEwThreads;
   // few fat threads: the per-thread channel-parameter prologue is amortised over several vectors and
-  // 148*8 blocks x 256 threads (full occupancy) x 4 loads in flight cover the HBM latency-bandwidth product.
-  // Measured on B200 (posenet_bs64 step, two A/B pairs): 8 blocks per SM 4.135 / 4.156 ms, 4 per SM 4.150 / 4.178 ms.
+  // 132*8 blocks x 256 threads (full occupancy) x 4 loads in flight cover the HBM latency-bandwidth product.
   static int per_sm = 0;
   if (per_sm == 0) { const char* e = getenv("MAPNET_EW_BLOCKS_PER_SM"); per_sm = e ? atoi(e) : 8; if (per_sm < 1 || per_sm > 8) per_sm = 8; }
-  const long long cap = 148LL * per_sm;
+  const long long cap = (long long)kNumSMs * per_sm;
   return (int)(g < cap ? (g < 1 ? 1 : g) : cap);
 }
 

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the MapNet B200 hot path (sm_100a only).
+// Shared device/host helpers for the MapNet hot path (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -48,12 +48,15 @@ extern unsigned long long g_launch_count;   // kernels launched by this library 
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// SMs of the target GPU (H100 SXM): persistent grids and split-K factors are sized for it
+static constexpr int kNumSMs = 132;
+
 // ---- programmatic dependent launch -------------------------------------------
 // Every kernel of the library starts with pdl_prologue(): it lets the NEXT kernel in the stream be
 // scheduled early (its blocks then sit in griddepcontrol.wait) and itself waits until the PREVIOUS
 // kernel has completed and flushed.  Nothing touches global memory before the wait, so the
 // semantics are those of a serialized stream; what overlaps is launch latency, block scheduling
-// and per-block setup (barrier init, TMEM allocation, descriptor prefetch) -- worth it because a
+// and per-block setup (barrier init, descriptor prefetch) -- worth it because a
 // training step is ~290 launches of 2-40 us each.  MAPNET_PDL=0 disables the launch attribute.
 #if defined(__CUDACC__)
 __device__ __forceinline__ void pdl_prologue() {
@@ -127,7 +130,7 @@ template <> struct Vec8<bf16> {
 // consecutive channels: 8 x hi (16 B) then 8 x lo (16 B) -- one logical element is 4 bytes, so the NHWC
 // indexing of the element-wise kernels (pointer + 8*i) is unchanged, and the conv engines see a 16-bit tensor
 // with 2C "channels" whose K order is (c/8, plane, c%8); the packed weight matrices use the same K order
-// (layout.cu), so every hi/lo cross product is formed by ordinary tcgen05 MMAs.  Only Vec8 access is defined.
+// (layout.cu), so every hi/lo cross product is formed by ordinary wgmma MMAs.  Only Vec8 access is defined.
 struct hsplit { uint32_t raw; };
 
 __device__ __forceinline__ void split_f16(float v, __half& hi, __half& lo) {

@@ -3,7 +3,7 @@
 // This is the STRICT-PARITY path (precision="fp32"): every product and sum is
 // fp32 like the reference's cuDNN fp32 convs, so loss/pose match the reference
 // PyTorch path to <=1e-4 (BASELINE.json north_star).  It is also the on-GPU
-// cross-check for the tcgen05 kernels in conv_tc.cu.  It is not a CPU fallback
+// cross-check for the wgmma kernels in conv_tc.cu.  It is not a CPU fallback
 // and not the benchmarked path: the bf16 tensor-core path is.
 //
 // Replaces cuDNN conv fwd / bwd-data / bwd-filter behind torchvision resnet34
@@ -12,7 +12,7 @@
 // GEMM views (NHWC activations, weights [N][K] K-major):
 //   fprop: C[m=(b,oh,ow)][n=co] = sum_k A[m][k=(kh,kw,ci)] * Wk[n][k]
 //   dgrad: C[m=(b,ih,iw)][n=ci] = sum_k dY[..][k=(kh,kw,co)] * Wd[n][k]
-//   wgrad: C[m=co][n=(kh,kw,ci)] = sum_{k=pixel} dY[k][m] * X[k@tap][n]   (split-K, atomics)
+//   wgrad: C[m=co][n=(kh,kw,ci)] = sum_{k=pixel} dY[k][m] * X[k@tap][n]   (split-K, fixed-order reduction)
 #include "kernels.h"
 
 namespace mapnet {
@@ -127,7 +127,7 @@ k_conv_simt(ConvGeom g, const T* __restrict__ src, const float* __restrict__ wma
 template <typename T>
 __global__ void __launch_bounds__(NT)
 k_conv_simt_wgrad(ConvGeom g, const T* __restrict__ x, const T* __restrict__ dy, float* __restrict__ dw,
-                  long long kchunk) {
+                  float* __restrict__ part, long long kchunk) {
   pdl_prologue();
   __shared__ float As[BK][BM + 4];   // [pixel][co]
   __shared__ float Bs[BK][BN + 4];   // [pixel][(tap,ci)]
@@ -179,6 +179,10 @@ k_conv_simt_wgrad(ConvGeom g, const T* __restrict__ x, const T* __restrict__ dy,
     }
     __syncthreads();
   }
+  // one writer per element: split z STORES into its workspace slice (launch_split_reduce adds the slices up in a
+  // fixed order), a single split adds into dw directly
+  const bool split = part != nullptr;
+  float* out = split ? part + (long long)blockIdx.z * M * N : dw;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int m = m0 + ty * 4 + i;
@@ -187,7 +191,7 @@ k_conv_simt_wgrad(ConvGeom g, const T* __restrict__ x, const T* __restrict__ dy,
     for (int j = 0; j < 4; ++j) {
       const int n = n0 + tx * 4 + j;
       if (n >= N) continue;
-      atomicAdd(dw + (long long)m * N + n, acc[i][j]);
+      out[(long long)m * N + n] = split ? acc[i][j] : out[(long long)m * N + n] + acc[i][j];
     }
   }
 }
@@ -213,15 +217,22 @@ int launch_conv_simt_wgrad(const ConvGeom& g, const T* x, const T* dy, float* dw
   MN_CHECK(g.Ci % 4 == 0 && g.Co % 4 == 0, "conv_simt wgrad: channels %% 4 != 0");
   const int gm = cdiv(g.Co, BM), gn = cdiv(g.KH * g.KW * g.Ci, BN);
   const long long Kt = g.M_out();
-  long long splits = (148LL * 4) / ((long long)gm * gn);
+  long long splits = ((long long)kNumSMs * 4) / ((long long)gm * gn);
   if (splits < 1) splits = 1;
   long long kchunk = (Kt + splits - 1) / splits;
   kchunk = ((kchunk + BK - 1) / BK) * BK;
   if (kchunk < 256) kchunk = 256;
   splits = (Kt + kchunk - 1) / kchunk;
   dim3 grid(gm, gn, (unsigned)splits);
-  MN_LAUNCH(k_conv_simt_wgrad<T>, grid, NT, 0, st, g, x, dy, dw, kchunk);
+  const long long n = (long long)g.Co * g.KH * g.KW * g.Ci;
+  float* part = nullptr;
+  if (splits > 1) MN_CUDA(cudaMallocAsync((void**)&part, (size_t)splits * n * sizeof(float), st));   // stream-ordered
+  MN_LAUNCH(k_conv_simt_wgrad<T>, grid, NT, 0, st, g, x, dy, dw, part, kchunk);
   MN_LAUNCH_CHECK();
+  if (part != nullptr) {
+    MN_TRY(launch_split_reduce(part, (int)splits, n, dw, st));
+    MN_CUDA(cudaFreeAsync(part, st));
+  }
   return 0;
 }
 

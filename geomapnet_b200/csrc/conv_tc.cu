@@ -1,23 +1,24 @@
-// tcgen05 / TMA implicit-GEMM convolution engines for sm_100a (bf16 operands,
-// fp32 accumulation in TMEM): fprop, dgrad, wgrad of every ResNet-34 conv.
+// wgmma / TMA implicit-GEMM convolution engines for sm_90a (bf16 operands,
+// fp32 accumulation in registers): fprop, dgrad, wgrad of every ResNet-34 conv.
 //
 // Replaces cuDNN conv fwd / bwd-data / bwd-filter behind torchvision resnet34
-// (/root/reference/models/posenet.py:66; SURVEY.md section 2c) with hand-written kernels:
+// (reference models/posenet.py:66; SURVEY.md section 2c) with hand-written kernels:
 //
 //  k_tc_conv  (fprop, dgrad)  D[pixel][cout] = sum_{tap,c} A_tap[pixel][c] * W[cout][tap][c]
 //     * im2col is done ON THE FLY by TMA: the A tile of one (tap, 64-channel block)
 //       is a 4-D box {64 ch, TW, TH, TN} of the NHWC activation tensor at the tap's
 //       spatial offset; out-of-bounds pixels (padding, ragged edges) are zero-filled
 //       by the TMA unit.  Stride-2 convs read parity views of the tensor (4 maps).
-//     * warp-specialised, persistent CTAs: warp0 = TMA producer, warp1 = MMA issuer
-//       (single elected thread, tcgen05.mma cta_group::1, M=128, N=64/128, K=16),
-//       warps2-5 = epilogue (tcgen05.ld -> +residual -> bf16 -> global), with a
-//       double-buffered TMEM accumulator so the epilogue of tile i overlaps the
-//       mainloop of tile i+1.
+//     * warp-specialised, persistent CTAs: warp 8 = TMA producer, warps 0-7 = two
+//       consumer warpgroups, each issuing wgmma m64nBNk16 for 64 of the tile's 128
+//       pixel rows (N = 64/128, K = 16) and then running the epilogue on its own
+//       rows (registers -> shared memory -> +residual -> bf16 -> global) while the
+//       producer already streams the next tile's operands.
 //  k_tc_wgrad  dW[cout][tap][c] += sum_pixels dY[pixel][cout] * X_tap[pixel][c]
 //     * both operands are MN-major (pixels = K): two 64-channel X chunks form the
-//       128 rows of A, dY supplies up to 256 columns of B; split-K over pixel tiles
-//       with fp32 red.global.add into the flat wgrad buffer.
+//       128 rows of A (one per consumer warpgroup), dY supplies up to 128 columns of B;
+//       split-K over pixel tiles, the splits' partial dW added up in a fixed order into the flat
+//       wgrad buffer (k_wgrad_reduce).
 #include <cudaTypedefs.h>
 
 #include <stdarg.h>
@@ -125,7 +126,7 @@ struct ConvParams {
   // output tensor [Nimg, Hout, Wout, Cout]; pixel (n, jh*os+oa, jw*os+ob)
   int Hout, Wout, Cout, os;
   int debug;     // micro-benchmark only: 1 = skip the MMAs, 2 = skip the TMA loads (results are garbage)
-  int fmt_a, fmt_b;        // UMMA operand element formats: 0 = fp16, 1 = bf16
+  int fmt_a, fmt_b;        // wgmma operand element formats (equal): 0 = fp16, 1 = bf16
   int out32;               // strict mode: output (and residual) are fp32 tensors
   int epi_prefetch;        // epilogue warps pull the NEXT tile's residual / y / zmask / yd rows into L2 (env MAPNET_TC_EPI_PREFETCH)
 };
@@ -155,8 +156,10 @@ struct WgradParams {
   int Ci, Co, KK;          // dW layout [Co][KK][Ci] (real channels)
   int debug;               // micro-benchmark only: 3 = skip the atomic epilogue
   int split;               // strict mode: X and dY are split 16-bit planes, the four hi/lo products are summed
-  int fmt_a, fmt_b;        // UMMA operand element formats: 0 = fp16, 1 = bf16
-  const float* oscale;     // device scalar multiplied into the accumulators before the atomics, or null
+  int fmt_a, fmt_b;        // wgmma operand element formats (equal): 0 = fp16, 1 = bf16
+  const float* oscale;     // device scalar multiplied into the accumulators before they are stored, or null
+  float* partial;          // splits > 1: split s stores its dW slice at partial + s * part_stride (no atomics), or null
+  long long part_stride;   // Co * KK * Ci
   WgradTap taps[16];
 };
 // chunk c = (tap c / cpt, 64-element block c % cpt)
@@ -198,29 +201,20 @@ __device__ __forceinline__ void warp_transpose_reduce(float (&x)[32], int lane) 
 //                                                         (and downsample BN) that consumes g
 // which removes the separate reduction pass over dY and Y of every BatchNorm backward.
 //
-// tcgen05.ld hands lane L the 32 fp32 columns of accumulator row L: touching global memory in that
-// layout costs one L1 wavefront per lane per 16 bytes (measured: with three extra tensors the
-// epilogue, not the MMAs, bounded the dgrad).  The accumulator chunk is therefore transposed once
-// through a per-warp shared-memory scratch (row stride 36 floats: conflict-free both ways) into the
-// COALESCED layout -- lane L owns 8 consecutive columns (16 bytes of bf16) p = L&3 of rows
-// 8i + (L>>2), i = 0..3 -- in which every global load and store instruction covers 8 rows x 64
-// contiguous bytes, and everything else (residual, gate, statistics) happens in that layout.
+// The wgmma accumulator fragment scatters a row over four lanes in 8-byte pieces: touching global memory in
+// that layout costs a wavefront per lane per 8 bytes.  Each warpgroup therefore stages its 64 accumulator rows
+// once in shared memory (row stride BN + 4 floats: conflict-free reads) and re-reads them in the COALESCED
+// layout -- lane L owns 8 consecutive columns (16 bytes of bf16) p = L&3 of rows 8i + (L>>2), i = 0..3, of a
+// 32-row quarter -- in which every global load and store instruction covers 8 rows x 64 contiguous bytes, and
+// everything else (residual, gate, statistics) happens in that layout.
 // ---------------------------------------------------------------------------------
-static constexpr int kEpiRowStride = 36;                 // floats per scratch row (32 + 4 pad)
-static constexpr int kEpiScratchFloats = 32 * kEpiRowStride;
-
-// Epilogue warps per CTA of the fprop / dgrad engines.  TMEM lane quarter q = warp % 4 is fixed by the hardware;
-// with 8 warps the two warps of a quarter split the 32-column chunks of the accumulator (even / odd chunks).
-// Most launches of the network are ONE wave of one tile per CTA, where the epilogue is not hidden behind the
-// next tile's MMAs but sits at the end of the kernel: halving it is worth one pipeline stage of shared memory.
-#ifndef MN_EPI_WARPS
-#define MN_EPI_WARPS 4
-#endif
-static constexpr int kEpiWarps = MN_EPI_WARPS;
-static_assert(kEpiWarps == 4 || kEpiWarps == 8, "MN_EPI_WARPS must be 4 or 8");
-static constexpr int kEpiSplit = kEpiWarps / 4;          // warps per TMEM lane quarter
+// Two consumer warpgroups (warps 0-7) and one TMA producer warp (warp 8).  In the epilogue the two warps that
+// share a 32-row quarter of the tile split its 32-column chunks (even / odd chunks).
+static constexpr int kEpiWarps = 8;
+static constexpr int kEpiSplit = 2;                      // warps per 32-row quarter
 static constexpr int kEpiThreads = 32 * kEpiWarps;
-static constexpr int kConvThreads = 64 + kEpiThreads;    // warp 0 TMA producer, warp 1 MMA issuer, then the epilogue
+static constexpr int kProducerWarp = kEpiWarps;
+static constexpr int kConvThreads = kEpiThreads + 32;
 
 // Epilogue variants (template flags): the flags are launch-uniform, and specialising on them keeps every
 // variant's chunk body straight-line code (runtime flags cost ~3x: branches fence the scheduler and the
@@ -318,26 +312,30 @@ __device__ __forceinline__ void epi_prefetch_next(const ConvParams& P, const int
   }
 }
 
-// stage this lane's accumulator row (32 fp32) into the warp's scratch
-__device__ __forceinline__ void epi_stage(const uint32_t (&v)[32], float* __restrict__ scr, const int lane) {
-  float4* dst = reinterpret_cast<float4*>(scr + lane * kEpiRowStride);
+// write this thread's wgmma accumulator fragment (rows 16*wq + lane/4 (+8), columns 8j + 2*(lane%4) (+1)) into
+// the warpgroup's staging rows
+template <int BN>
+__device__ __forceinline__ void acc_to_stage(const float (&d)[BN / 2], float* __restrict__ stg, const int wq, const int lane) {
+  constexpr int RS = BN + 4;
+  float* r0 = stg + (16 * wq + (lane >> 2)) * RS + 2 * (lane & 3);
 #pragma unroll
-  for (int j = 0; j < 8; ++j)
-    dst[j] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                         __uint_as_float(v[4 * j + 3]));
+  for (int j = 0; j < BN / 8; ++j) {
+    *reinterpret_cast<float2*>(r0 + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(r0 + 8 * RS + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
 }
 
-template <int F>
-__device__ __forceinline__ void epi_chunk(float* __restrict__ scr, const EpiRegs& G,
+// one 32-column chunk of a warp's 32 staged rows (row stride RS floats)
+template <int F, int RS>
+__device__ __forceinline__ void epi_chunk(const float* __restrict__ scr, const EpiRegs& G,
                                           const long long (&rowoff)[4], const bool (&rstore)[4], const float (&rw)[4],
                                           const int coff, const int col0, bf16* out, const EpiBwd& E, const int lane,
                                           float& s0, float& s1, float& s2) {
-  __syncwarp();                                // the staged rows are visible to the whole warp
   const int p = lane & 3, rr = lane >> 2;
   float4 lo[4], hi[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    const float4* src = reinterpret_cast<const float4*>(scr + (8 * i + rr) * kEpiRowStride + 8 * p);
+    const float4* src = reinterpret_cast<const float4*>(scr + (8 * i + rr) * RS + 8 * p);
     lo[i] = src[0]; hi[i] = src[1];
   }
   float msc[8], msh[8];
@@ -419,7 +417,6 @@ __device__ __forceinline__ void epi_chunk(float* __restrict__ scr, const EpiRegs
       }
     }
   }
-  __syncwarp();                                // scratch may be overwritten by the next chunk
   if (F & (EPI_STATS | EPI_BWD)) {
     group_reduce8(c0, lane);
     group_reduce8(c1, lane);
@@ -429,56 +426,32 @@ __device__ __forceinline__ void epi_chunk(float* __restrict__ scr, const EpiRegs
   }
 }
 
-// One accumulator tile (this warp's 32 rows x BN columns): wait for the MMAs, walk the 32-column chunks,
-// hand the TMEM stage back after the last TMEM read.  `release` performs the tempty arrive.
-template <int F, int BN, typename Release>
-__device__ __forceinline__ void epi_tile(const uint32_t tmem_addr, const bool has_acc, const uint32_t tfull_bar,
-                                         const uint32_t tfull_phase, Release release, float* __restrict__ scr,
-                                         float (*stw)[BN / 32][32], const long long (&rowoff)[4],
-                                         const bool (&rvalid)[4], const bool do_store, const int tn,
-                                         const bf16* residual, bf16* out, const EpiBwd& E, const int lane,
+// One accumulator tile (this warp's 32 staged rows x BN columns): walk the warp's 32-column chunks.
+template <int F, int BN>
+__device__ __forceinline__ void epi_tile(const float* __restrict__ rows, float (*stw)[BN / 32][32],
+                                         const long long (&rowoff)[4], const bool (&rvalid)[4], const bool do_store,
+                                         const int tn, const bf16* residual, bf16* out, const EpiBwd& E, const int lane,
                                          const int half) {
   bool rstore[4]; float rw[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) { rstore[i] = rvalid[i] && do_store; rw[i] = rvalid[i] ? 1.f : 0.f; }
-  // the first chunk's operand loads are in flight while the MMAs finish
-  // this warp's chunks: half, half + kEpiSplit, ...  (kEpiSplit == 1: all of them)
-  EpiRegs G;
-  epi_issue_loads<F>(G, rowoff, half * 32, residual, E, lane);
-  mbar_wait(tfull_bar, tfull_phase);
-  tc_fence_after();
-  uint32_t v[32];
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = 0u;      // has_acc == false: no filter tap reaches this output class, D = 0
-  if (has_acc) tmem_ld32(tmem_addr + half * 32, v);
 #pragma unroll 1
   for (int cc = half; cc < BN / 32; cc += kEpiSplit) {
-    if (cc > half) epi_issue_loads<F>(G, rowoff, cc * 32, residual, E, lane);
-    if (has_acc) tmem_ld_wait();
-    if (cc + kEpiSplit >= BN / 32) {
-      // all of this warp's TMEM reads of this accumulator stage are complete: hand it back
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) release();
-    }
-    epi_stage(v, scr, lane);
-    // the next chunk's TMEM read overlaps this chunk's processing
-    if (has_acc && cc + kEpiSplit < BN / 32) tmem_ld32(tmem_addr + (cc + kEpiSplit) * 32, v);
-    epi_chunk<F>(scr, G, rowoff, rstore, rw, cc * 32, tn * BN + cc * 32, out, E, lane, stw[0][cc][lane],
-                 stw[1][cc][lane], stw[2][cc][lane]);
+    EpiRegs G;
+    epi_issue_loads<F>(G, rowoff, cc * 32, residual, E, lane);
+    epi_chunk<F, BN + 4>(rows + cc * 32, G, rowoff, rstore, rw, cc * 32, tn * BN + cc * 32, out, E, lane,
+                         stw[0][cc][lane], stw[1][cc][lane], stw[2][cc][lane]);
   }
 }
 
 // launch-uniform dispatch over the variants the network uses
-template <int BN, typename Release>
-__device__ __forceinline__ void epi_tile_dispatch(const int mode, const uint32_t tmem_addr, const bool has_acc,
-                                                  const uint32_t tfull_bar, const uint32_t tfull_phase, Release release,
-                                                  float* __restrict__ scr, float (*stw)[BN / 32][32],
-                                                  const long long (&rowoff)[4], const bool (&rvalid)[4],
-                                                  const bool do_store, const int tn, const bf16* residual, bf16* out,
-                                                  const EpiBwd& E, const int lane, const int half) {
-#define MN_EPI_CASE(Fv) case (Fv): epi_tile<(Fv), BN>(tmem_addr, has_acc, tfull_bar, tfull_phase, release, scr, stw, rowoff, \
-                                                      rvalid, do_store, tn, residual, out, E, lane, half); break;
+template <int BN>
+__device__ __forceinline__ void epi_tile_dispatch(const int mode, const float* __restrict__ rows,
+                                                  float (*stw)[BN / 32][32], const long long (&rowoff)[4],
+                                                  const bool (&rvalid)[4], const bool do_store, const int tn,
+                                                  const bf16* residual, bf16* out, const EpiBwd& E, const int lane,
+                                                  const int half) {
+#define MN_EPI_CASE(Fv) case (Fv): epi_tile<(Fv), BN>(rows, stw, rowoff, rvalid, do_store, tn, residual, out, E, lane, half); break;
   switch (mode) {
     MN_EPI_CASE(0)
     MN_EPI_CASE(EPI_RES)
@@ -560,60 +533,102 @@ __device__ __forceinline__ void epi_finalize(const EpiFin& Fin, double* __restri
   if (etid == 0) *Fin.counter = 0u;
 }
 
-// as many stages as fit in 227 KB: the engines are bound by bytes in flight x L2 latency
-static constexpr int conv_stages(int BN) {      // + 18 KB (4 epilogue warps) / 37 KB (8) of epilogue scratch
-  return kEpiWarps == 4 ? (BN <= 64 ? 8 : (BN <= 128 ? 6 : 4)) : (BN <= 64 ? 7 : (BN <= 128 ? 5 : 3));
+// as many stages as fit in 227 KB next to the accumulator staging rows: the engines are bound by bytes in flight
+static constexpr int conv_stages(int BN) { return BN <= 64 ? 7 : 4; }
+static constexpr size_t conv_smem_bytes(int BN) {
+  return (size_t)conv_stages(BN) * (128 * 128 + BN * 128) + (size_t)128 * (BN + 4) * 4 + 1024;
 }
-static constexpr int wgrad_stages(int BN) { return BN <= 64 ? 9 : (BN <= 128 ? 6 : 4); }
-static constexpr int kOcc2Stages = 3;          // BN = 64, two CTAs per SM: 3 x 24 KB + 18 KB scratch per CTA
+static constexpr int wgrad_stages(int BN) { return BN <= 64 ? 9 : 6; }
+
+// named barrier of one consumer warpgroup (barrier 0 is __syncthreads, 1 is epi_bar)
+__device__ __forceinline__ void wg_bar(const int wg) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); }
+
+// release a pipeline stage: one thread per consumer warpgroup arrives on the stage's empty barrier in every CTA of
+// the cluster (each CTA's producer multicasts its slice of the weight tile into all of them)
+template <int CL>
+__device__ __forceinline__ void release_stage(const uint32_t empty_bar, const bool arriver) {
+  if (!arriver) return;
+  if (CL == 1) mbar_arrive(empty_bar);
+  else {
+#pragma unroll
+    for (int r = 0; r < CL; ++r) mbar_arrive_cluster(mapa(empty_bar, (uint32_t)r));
+  }
+}
+
+// Mainloop of one tile for one consumer warpgroup: kblocks k-blocks of 64, each four wgmma K=16 steps.  A stage is
+// handed back as soon as the wgmma group that read it has retired (one group stays in flight behind the next).
+// a_off / a_step: this warpgroup's A rows inside a stage and the byte step per K=16; b_step likewise for B.
+template <int BN, int CL, int FMT, int TA, int TB>
+__device__ __forceinline__ void mma_tile(float (&d)[BN / 2], const int kblocks, int& stage, uint32_t& phase,
+                                         const int STAGES, const uint32_t stage_bytes, const uint32_t smem_base,
+                                         const uint32_t a_off, const uint32_t a_step, const uint32_t b_off,
+                                         const uint32_t b_step, const uint64_t adesc, const uint64_t bdesc,
+                                         const uint32_t full0, const uint32_t empty0, const bool arriver,
+                                         const bool skip_mma) {
+  int prev = -1;
+  for (int kb = 0; kb < kblocks; ++kb) {
+    mbar_wait(full0 + 8 * stage, phase);
+    if (!skip_mma) {
+      const uint32_t sa = smem_base + stage * stage_bytes + a_off;
+      const uint32_t sb = smem_base + stage * stage_bytes + b_off;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_k16<TA, TB>(WgmmaTag<BN, FMT>(), d, smem_desc(adesc, sa + k * a_step), smem_desc(bdesc, sb + k * b_step),
+                          (kb > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      wgmma_fence_acc(d);
+    }
+    if (prev >= 0) release_stage<CL>(empty0 + 8 * prev, arriver);
+    prev = stage;
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_acc(d);
+  if (prev >= 0) release_stage<CL>(empty0 + 8 * prev, arriver);
+  if (kblocks == 0 || skip_mma) {         // no filter tap reaches this output class (or MMAs skipped): D = 0
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+  }
+}
 
 // ---------------------------------------------------------------------------------
 // fprop / dgrad kernel
 // ---------------------------------------------------------------------------------
 // CL = thread-block cluster size along M: the CL CTAs of a cluster work on CL consecutive
 // M tiles of the same N tile and share the weight tile -- each loads 1/CL of it and TMA-
-// multicasts it to all (the engines are L2-bandwidth bound, this cuts the B traffic by CL).
-// OCC = CTAs per SM.  The Cout = 64 launches (layer1, the stem, the layer2.0 dgrad) are EPILOGUE-bound: 8 192 outputs per
-// tile but only K = 576 (ncu r02a: the four epilogue warps issue or sit in short-scoreboard stalls for all of their
-// samples while the producer and MMA warps wait; skipping the MMAs or the TMA loads does not shorten the kernel).  Two CTAs
-// per SM (3 pipeline stages each instead of 8) put eight epilogue warps on the SM, each tile's epilogue on its own.
-template <int BN, int CL, int OCC = 1>
-__global__ void __launch_bounds__(kConvThreads, OCC)
+// multicasts it to all (cuts the B traffic from L2 by CL).
+template <int BN, int CL>
+__global__ void __launch_bounds__(kConvThreads, 1)
 k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
           const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapA3,
           const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapB2,
           const __grid_constant__ ConvParams P, const bf16* __restrict__ residual,
           bf16* __restrict__ out, double* __restrict__ stats, const EpiBwd E, const EpiFin Fin) {
-  constexpr int STAGES = (OCC == 2) ? kOcc2Stages : conv_stages(BN);
+  constexpr int STAGES = conv_stages(BN);
   constexpr uint32_t A_BYTES = 128 * 128;        // 128 pixels x 64 ch bf16
   constexpr uint32_t B_BYTES = BN * 128;
   constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  constexpr uint32_t TMEM_COLS = 2 * BN;         // double-buffered accumulator: 128 / 256 / 512 columns
+  constexpr int RS = BN + 4;                     // floats per accumulator staging row
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment for the 128B swizzle atoms
   const uint32_t smem_base = __shfl_sync(0xffffffffu, (smem_u32(smem_raw) + 1023u) & ~1023u, 0);
-  __shared__ __align__(8) uint64_t bars[2 * STAGES + 4];
-  __shared__ uint32_t tmem_base_smem;
+  __shared__ __align__(8) uint64_t bars[2 * STAGES];
   const uint32_t full0 = __shfl_sync(0xffffffffu, smem_u32(&bars[0]), 0), empty0 = smem_u32(&bars[STAGES]);
-  const uint32_t tfull0 = __shfl_sync(0xffffffffu, smem_u32(&bars[2 * STAGES]), 0), tempty0 = smem_u32(&bars[2 * STAGES + 2]);
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform for the compiler
   const int lane = threadIdx.x & 31;
 
   const uint32_t crank = (CL > 1) ? cluster_ctarank() : 0u;
   constexpr uint16_t CMASK = (uint16_t)((1u << CL) - 1u);
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     prefetch_tmap(&mapA0); prefetch_tmap(&mapB);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(full0 + 8 * i, 1); mbar_init(empty0 + 8 * i, CL); }
-    for (int i = 0; i < 2; ++i) { mbar_init(tfull0 + 8 * i, 1); mbar_init(tempty0 + 8 * i, kEpiWarps); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(full0 + 8 * i, 1); mbar_init(empty0 + 8 * i, 2 * CL); }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(smem_u32(&tmem_base_smem), TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
   if (CL > 1) cluster_sync();          // peers' barriers are initialised before any multicast
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, tmem_base_smem, 0);
   pdl_prologue();      // nothing above touches global memory: setup overlaps the previous kernel's tail
 
   // work items: (group of CL consecutive M tiles, N tile); every CTA of a cluster walks the
@@ -625,7 +640,7 @@ k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
   const int first_tile = blockIdx.x / CL;
   const int tile_step = gridDim.x / CL;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===================== TMA producer =====================
     if (elect_one()) {
       int stage = 0; uint32_t phase = 0;
@@ -661,68 +676,39 @@ k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const uint32_t IDESC = make_idesc_fmt(128, BN, 0, 0, (uint32_t)P.fmt_a, (uint32_t)P.fmt_b);
+  } else {
+    // ===================== consumer warpgroups: MMAs, then the epilogue of their own 64 rows =====================
+    const int wg = warp >> 2;               // accumulator rows 64*wg .. 64*wg + 63 of the tile
+    const int wq = warp & 3;
+    const int q = 2 * wg + (wq >> 1);       // the 32-row quarter this warp's epilogue walks
+    const int half = wq & 1;                // which of the quarter's chunk subsets
+    const bool arriver = (threadIdx.x & 127) == 0;
+    float* stg = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)) + STAGES * STAGE_BYTES);
+    const int epi_mode = epi_mode_of(residual, stats, E, P.out32);
     constexpr uint64_t DESC_BASE = make_smem_desc_base(16, 1024);
     int stage = 0; uint32_t phase = 0;
-    int as = 0; uint32_t aphase = 0;
-    for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
-      const int kblocks = P.cls[tile / per_class].num_taps * P.cblocks;
-      mbar_wait(tempty0 + 8 * as, aphase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + as * BN;
-      for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait(full0 + 8 * stage, phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t sa = smem_base + stage * STAGE_BYTES;
-          const uint32_t sb = sa + A_BYTES;
-          if (P.debug == 1) {
-            mbar_arrive(empty0 + 8 * stage);
-            if (kb == kblocks - 1) mbar_arrive(tfull0 + 8 * as);
-          } else {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              mma_bf16(d_tmem, smem_desc(DESC_BASE, sa + k * 32), smem_desc(DESC_BASE, sb + k * 32), IDESC,
-                       (kb > 0 || k > 0) ? 1u : 0u);
-            }
-            if (CL == 1) mma_commit(empty0 + 8 * stage); else mma_commit_mc(empty0 + 8 * stage, CMASK);
-            if (kb == kblocks - 1) mma_commit(tfull0 + 8 * as);
-          }
-        }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (kblocks == 0 && elect_one()) mbar_arrive(tfull0 + 8 * as);
-      if (++as == 2) { as = 0; aphase ^= 1; }
-    }
-  } else {
-    // ===================== epilogue (warps 2..5 -> TMEM lane quarters 2,3,0,1) =====================
-    const int q = warp & 3;                 // TMEM lane quarter
-    const int ew = warp - 2;                // epilogue warp index, 0 .. kEpiWarps-1
-    const int half = ew >> 2;               // which of the quarter's chunk subsets (0 when kEpiWarps == 4)
-    // per-warp transpose scratch: dynamic shared memory behind the pipeline stages (static is capped at 48 KB)
-    float* scr = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)) + STAGES * STAGE_BYTES) + ew * kEpiScratchFloats;
-    const int epi_mode = epi_mode_of(residual, stats, E, P.out32);
-    int as = 0; uint32_t aphase = 0;
-    // fused BatchNorm statistics (fprop only): lane L keeps the running column sums of column
-    // cc*32+L over all rows this warp has stored, flushed with fp64 atomics per N tile
     // running column sums of this warp, [statistic][chunk][lane] (lane <-> column epi_stat_col(lane)); kept in
-    // shared memory so that the chunk loop can stay ROLLED: unrolled, the epilogue alone was > 100 KB of
-    // SASS and the four epilogue warps stalled on instruction fetch (ncu: stall_no_inst dominant)
+    // shared memory so that the chunk loop can stay ROLLED (unrolled, the epilogue's code size stalls the
+    // epilogue warps on instruction fetch)
     __shared__ float epi_stats[4][3][BN / 32][32];
     float (*stw)[BN / 32][32] = epi_stats[q];
 #pragma unroll 1
     for (int i = half; i < BN / 32; i += kEpiSplit) { stw[0][i][lane] = 0.f; stw[1][i][lane] = 0.f; stw[2][i][lane] = 0.f; }
     int st_tn = -1;
-    const int etid = ew * 32 + lane;
+    const int etid = warp * 32 + lane;
     auto flush_stats = [&](int tn_flush) { epi_flush<BN>(epi_stats, stats, P.Cout, tn_flush, E.yd != nullptr, etid); };
     for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
       const TileCoord tc = decode_tile(tile, per_class, P.n_tiles_n);
       const ClassDesc cd = P.cls[tc.cls];
       const int kblocks = cd.num_taps * P.cblocks;
       const int tn = tc.tn;
+      float d[BN / 2];
+      if (P.fmt_a)
+        mma_tile<BN, CL, 1, 0, 0>(d, kblocks, stage, phase, STAGES, STAGE_BYTES, smem_base, wg * 64 * 128, 32, A_BYTES, 32,
+                                  DESC_BASE, DESC_BASE, full0, empty0, arriver, P.debug == 1);
+      else
+        mma_tile<BN, CL, 0, 0, 0>(d, kblocks, stage, phase, STAGES, STAGE_BYTES, smem_base, wg * 64 * 128, 32, A_BYTES, 32,
+                                  DESC_BASE, DESC_BASE, full0, empty0, arriver, P.debug == 1);
       if (stats != nullptr && tn != st_tn) { if (st_tn >= 0) flush_stats(st_tn); st_tn = tn; }
       int tm = tc.group * CL + (int)crank;
       const int tw = tm % P.tiles_w; tm /= P.tiles_w;
@@ -743,19 +729,12 @@ k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
       }
       if (P.epi_prefetch && tile + tile_step < total_tiles)
         epi_prefetch_next<BN>(P, tile + tile_step, per_class, CL, (int)crank, q, lane, residual, E);
-      if (P.debug == 3) {           // micro-benchmark: no epilogue work at all
-        mbar_wait(tfull0 + 8 * as, aphase);
-        tc_fence_after();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty0 + 8 * as);
-        if (++as == 2) { as = 0; aphase ^= 1; }
-        continue;
-      }
-      epi_tile_dispatch<BN>(epi_mode, tmem_base + ((uint32_t)(q * 32) << 16) + as * BN, kblocks > 0, tfull0 + 8 * as,
-                            aphase, [&]() { mbar_arrive(tempty0 + 8 * as); }, scr, stw, rowoff, rvalid, P.debug != 4, tn,
-                            residual, out, E, lane, half);
-      if (++as == 2) { as = 0; aphase ^= 1; }
+      if (P.debug == 3) continue;            // micro-benchmark: no epilogue work at all
+      wg_bar(wg);                             // the previous tile's staged rows have been read
+      acc_to_stage<BN>(d, stg + wg * 64 * RS, wq, lane);
+      wg_bar(wg);
+      epi_tile_dispatch<BN>(epi_mode, stg + q * 32 * RS, stw, rowoff, rvalid, P.debug != 4, tn, residual, out, E, lane,
+                            half);
     }
     if (stats != nullptr && st_tn >= 0) flush_stats(st_tn);
     if (Fin.mode != 0) {
@@ -764,466 +743,63 @@ k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
     }
   }
   // ---- teardown ----
-  tc_fence_before();
-  __syncthreads();
-  if (CL > 1) cluster_sync();          // no CTA exits while a peer may still multicast into it
-  tc_fence_after();
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
+  if (CL > 1) {
+    __syncthreads();
+    cluster_sync();                    // no CTA exits while a peer may still multicast into it or arrive on it
+  }
 }
 
 // ---------------------------------------------------------------------------------
-// 2-SM variant (tcgen05 cta_group::2): a CTA pair computes a 256 x BN tile.  Each CTA
-// stages its own 128 pixel rows of A and only HALF of the weight tile; one MMA issued by
-// the leader spans both CTAs' shared memory and TMEM.  Per-SM bytes per FLOP drop to what
-// a 256x256 GEMM tile needs -- the engines are bound by shared-memory ingest, not by math.
-// ---------------------------------------------------------------------------------
-static constexpr int conv2_stages(int BN) { return kEpiWarps == 4 ? (BN <= 128 ? 8 : 6) : (BN <= 128 ? 7 : 5); }
-
-template <int BN>
-__global__ void __launch_bounds__(kConvThreads, 1)
-k_tc_conv2(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
-           const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapA3,
-           const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapB2,
-           const __grid_constant__ ConvParams P, const bf16* __restrict__ residual,
-           bf16* __restrict__ out, double* __restrict__ stats, const EpiBwd E, const EpiFin Fin) {
-  constexpr int STAGES = conv2_stages(BN);
-  constexpr uint32_t A_BYTES = 128 * 128;
-  constexpr uint32_t BH_BYTES = (BN / 2) * 128;      // this CTA's half of the weight tile
-  constexpr uint32_t STAGE_BYTES = A_BYTES + BH_BYTES;
-  constexpr uint32_t TMEM_COLS = 2 * BN;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = __shfl_sync(0xffffffffu, (smem_u32(smem_raw) + 1023u) & ~1023u, 0);
-  __shared__ __align__(8) uint64_t bars[2 * STAGES + 4];
-  __shared__ uint32_t tmem_base_smem;
-  const uint32_t full0 = __shfl_sync(0xffffffffu, smem_u32(&bars[0]), 0), empty0 = smem_u32(&bars[STAGES]);
-  const uint32_t tfull0 = __shfl_sync(0xffffffffu, smem_u32(&bars[2 * STAGES]), 0), tempty0 = smem_u32(&bars[2 * STAGES + 2]);
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform for the compiler
-  const int lane = threadIdx.x & 31;
-  const uint32_t crank = cluster_ctarank();
-  const bool leader = (crank == 0);
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&mapA0); prefetch_tmap(&mapB);
-    // full: leader's arrive.expect_tx + peer's remote arrive; empty / tfull: one multicast commit;
-    // tempty: the epilogue warps of each CTA arrive on the LEADER's barrier
-    for (int i = 0; i < STAGES; ++i) { mbar_init(full0 + 8 * i, 2); mbar_init(empty0 + 8 * i, 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(tfull0 + 8 * i, 1); mbar_init(tempty0 + 8 * i, 2 * kEpiWarps); }
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc_2sm(smem_u32(&tmem_base_smem), TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, tmem_base_smem, 0);
-  pdl_prologue();      // nothing above touches global memory: setup overlaps the previous kernel's tail
-
-  const int n_groups = (P.n_tiles_m + 1) / 2;
-  const int per_class = n_groups * P.n_tiles_n;
-  const int total_tiles = per_class * P.n_classes;
-  const int first_tile = blockIdx.x / 2;
-  const int tile_step = gridDim.x / 2;
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    if (elect_one()) {
-      int stage = 0; uint32_t phase = 0;
-      for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
-        const TileCoord tc = decode_tile(tile, per_class, P.n_tiles_n);
-        const ClassDesc cd = P.cls[tc.cls];
-        const int tn = tc.tn;
-        int tm = tc.group * 2 + (int)crank;
-        const int tw = tm % P.tiles_w; tm /= P.tiles_w;
-        const int th = tm % P.tiles_h;
-        const int tb = tm / P.tiles_h;
-        const int jw0 = tw * P.TW, jh0 = th * P.TH, n0 = tb * P.TN;
-        for (int t = cd.tap0; t < cd.tap0 + cd.num_taps; ++t) {
-          const TapDesc tap = P.taps[t];
-          const int am = tap.map & 3;
-          const CUtensorMap* mA = (am == 0) ? &mapA0 : (am == 1) ? &mapA1 : (am == 2) ? &mapA2 : &mapA3;
-          const CUtensorMap* mB = (tap.map & 4) ? &mapB2 : &mapB;
-          for (int cb = 0; cb < P.cblocks; ++cb) {
-            mbar_wait(empty0 + 8 * stage, phase ^ 1);
-            const uint32_t sa = smem_base + stage * STAGE_BYTES;
-            const uint32_t lfull = mapa(full0 + 8 * stage, 0);      // the LEADER's full barrier
-            if (leader) mbar_expect_tx(full0 + 8 * stage, 2 * STAGE_BYTES);
-            else mbar_arrive_cluster(lfull);
-            tma_load_4d_2sm(sa, mA, lfull, cb * 64, jw0 + tap.dw, jh0 + tap.dh, n0);
-            tma_load_2d_2sm(sa + A_BYTES, mB, lfull, tap.kidx * P.Cs + cb * 64, tn * BN + (int)crank * (BN / 2));
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (leader) {
-      const uint32_t IDESC = make_idesc_fmt(256, BN, 0, 0, (uint32_t)P.fmt_a, (uint32_t)P.fmt_b);
-      constexpr uint64_t DESC_BASE = make_smem_desc_base(16, 1024);
-      int stage = 0; uint32_t phase = 0;
-      int as = 0; uint32_t aphase = 0;
-      for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
-        const int kblocks = P.cls[tile / per_class].num_taps * P.cblocks;
-        mbar_wait(tempty0 + 8 * as, aphase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * BN;
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(full0 + 8 * stage, phase);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t sa = smem_base + stage * STAGE_BYTES;
-            const uint32_t sb = sa + A_BYTES;
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              mma_bf16_2sm(d_tmem, smem_desc(DESC_BASE, sa + k * 32), smem_desc(DESC_BASE, sb + k * 32), IDESC,
-                           (kb > 0 || k > 0) ? 1u : 0u);
-            }
-            mma_commit_2sm(empty0 + 8 * stage, 3);
-            if (kb == kblocks - 1) mma_commit_2sm(tfull0 + 8 * as, 3);
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        if (kblocks == 0 && elect_one()) {       // no filter tap reaches this output class: D = 0
-          mbar_arrive(tfull0 + 8 * as);
-          mbar_arrive_cluster(mapa(tfull0 + 8 * as, 1));
-        }
-        if (++as == 2) { as = 0; aphase ^= 1; }
-      }
-    }
-  } else {
-    // ===================== epilogue (both CTAs; own TMEM half) =====================
-    const int q = warp & 3;                 // TMEM lane quarter
-    const int ew = warp - 2;                // epilogue warp index, 0 .. kEpiWarps-1
-    const int half = ew >> 2;               // which of the quarter's chunk subsets (0 when kEpiWarps == 4)
-    // per-warp transpose scratch: dynamic shared memory behind the pipeline stages (static is capped at 48 KB)
-    float* scr = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)) + STAGES * STAGE_BYTES) + ew * kEpiScratchFloats;
-    const int epi_mode = epi_mode_of(residual, stats, E, P.out32);
-    int as = 0; uint32_t aphase = 0;
-    // running column sums of this warp, [statistic][chunk][lane] (lane <-> column epi_stat_col(lane)); kept in
-    // shared memory so that the chunk loop can stay ROLLED: unrolled, the epilogue alone was > 100 KB of
-    // SASS and the four epilogue warps stalled on instruction fetch (ncu: stall_no_inst dominant)
-    __shared__ float epi_stats[4][3][BN / 32][32];
-    float (*stw)[BN / 32][32] = epi_stats[q];
-#pragma unroll 1
-    for (int i = half; i < BN / 32; i += kEpiSplit) { stw[0][i][lane] = 0.f; stw[1][i][lane] = 0.f; stw[2][i][lane] = 0.f; }
-    int st_tn = -1;
-    const int etid = ew * 32 + lane;
-    auto flush_stats = [&](int tn_flush) { epi_flush<BN>(epi_stats, stats, P.Cout, tn_flush, E.yd != nullptr, etid); };
-    for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
-      const TileCoord tc = decode_tile(tile, per_class, P.n_tiles_n);
-      const ClassDesc cd = P.cls[tc.cls];
-      const int kblocks = cd.num_taps * P.cblocks;
-      const int tn = tc.tn;
-      if (stats != nullptr && tn != st_tn) { if (st_tn >= 0) flush_stats(st_tn); st_tn = tn; }
-      int tm = tc.group * 2 + (int)crank;
-      const int tw = tm % P.tiles_w; tm /= P.tiles_w;
-      const int th = tm % P.tiles_h;
-      const int tb = tm / P.tiles_h;
-      // the 4 rows this lane owns in the coalesced layout: tile row q*32 + 8i + (lane>>2)
-      long long rowoff[4]; bool rvalid[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int m = q * 32 + 8 * i + (lane >> 2);
-        const int lw = m % P.TW;
-        const int lh = (m / P.TW) % P.TH;
-        const int ln = m / (P.TW * P.TH);
-        const int jw = tw * P.TW + lw, jh = th * P.TH + lh, n = tb * P.TN + ln;
-        rvalid[i] = (jw < cd.Ws) && (jh < cd.Hs) && (n < P.Nimg);
-        const long long pix = ((long long)n * P.Hout + (jh * P.os + cd.oa)) * P.Wout + (jw * P.os + cd.ob);
-        rowoff[i] = (rvalid[i] ? pix * P.Cout : 0) + tn * BN;     // outside rows: clamped, loads stay in bounds
-      }
-      if (P.epi_prefetch && tile + tile_step < total_tiles)
-        epi_prefetch_next<BN>(P, tile + tile_step, per_class, 2, (int)crank, q, lane, residual, E);
-      epi_tile_dispatch<BN>(epi_mode, tmem_base + ((uint32_t)(q * 32) << 16) + as * BN, kblocks > 0, tfull0 + 8 * as,
-                            aphase, [&]() { mbar_arrive_cluster(mapa(tempty0 + 8 * as, 0)); }, scr, stw, rowoff, rvalid, true, tn,
-                            residual, out, E, lane, half);
-      if (++as == 2) { as = 0; aphase ^= 1; }
-    }
-    if (stats != nullptr && st_tn >= 0) flush_stats(st_tn);
-    if (Fin.mode != 0) {
-      __shared__ unsigned int s_fin_flag;
-      epi_finalize(Fin, stats, P.Cout, etid, &s_fin_flag);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync();
-  tc_fence_after();
-  if (warp == 1) tmem_dealloc_2sm(tmem_base, TMEM_COLS);
-}
-
-// ---------------------------------------------------------------------------------
-// Halo-resident 3x3 / stride-1 engine (fprop and dgrad of 29 of the 36 convs).
-//
-// Measured (profiles/): the 4-D im2col TMA box costs ~4 cycles per 128-byte pixel row, and the
-// per-tap engine above re-stages the same pixels 9 times -- the tensor pipe idles 2/3 of the
-// time.  Here the activation tile is staged ONCE per 64-channel block together with its halo:
-// pixels are addressed in a padded linear space q = h*P + (w+1), P = W+2 (TMA's out-of-bounds
-// zero fill provides the halo columns / rows), an M tile is 128 consecutive q, and the nine
-// filter taps are nine SHIFTED shared-memory matrix descriptors into the same patch
-// (row m of tap (kh,kw) = patch row m + (kh-1)*P + (kw-1)).  Rows that fall on halo columns
-// compute garbage that is never stored (W/(W+2) of the MMA rows are useful).
-// For Cin=64 the whole weight matrix (72 KB) stays resident in shared memory.
-// ---------------------------------------------------------------------------------
-struct HaloParams {
-  int Nimg, H, W, P, tiles_per_img, n_tiles_m, n_tiles_n;
-  int cblocks, Cs, Cout;
-  int R, patch_bytes;           // patch box rows, bytes per patch buffer (multiple of 1024)
-  int NP, NB;                   // patch / weight ring depths
-  int b_stationary;             // weights loaded once per CTA (9*cblocks tiles)
-  int dq[9], kidx[9];           // per tap: shift in padded-linear space, K index of its weight slice
-  int use_base_offset;
-  int row_boxes;                // patch staged as R per-image-row boxes {64 ch, W, 1} (halo columns pre-zeroed) instead of one {64, W+2, R} box
-  int scr_off;                  // byte offset (from the 1024-aligned base) of the epilogue warps' transpose scratch
-  int debug;                    // micro-benchmark only: 1 = skip MMAs, 2 = skip TMA loads
-};
-
-template <int BN>
-__global__ void __launch_bounds__(kConvThreads, 1)
-k_tc_conv_halo(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-               const __grid_constant__ HaloParams P, const bf16* __restrict__ residual, bf16* __restrict__ out,
-               double* __restrict__ stats, const EpiBwd E, const EpiFin Fin) {
-  constexpr uint32_t B_BYTES = BN * 128;
-  constexpr uint32_t TMEM_COLS = 2 * BN;
-  constexpr int MAXNP = 4, MAXNB = 12;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = __shfl_sync(0xffffffffu, (smem_u32(smem_raw) + 1023u) & ~1023u, 0);
-  const uint32_t b_base = smem_base + P.NP * P.patch_bytes;
-  __shared__ __align__(8) uint64_t bars[2 * MAXNP + 2 * MAXNB + 5];
-  __shared__ uint32_t tmem_base_smem;
-  const uint32_t pfull0 = __shfl_sync(0xffffffffu, smem_u32(&bars[0]), 0), pempty0 = smem_u32(&bars[MAXNP]);
-  const uint32_t bfull0 = __shfl_sync(0xffffffffu, smem_u32(&bars[2 * MAXNP]), 0), bempty0 = smem_u32(&bars[2 * MAXNP + MAXNB]);
-  const uint32_t tfull0 = __shfl_sync(0xffffffffu, smem_u32(&bars[2 * MAXNP + 2 * MAXNB]), 0), tempty0 = tfull0 + 16;
-  const uint32_t bstat = tfull0 + 32;
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform for the compiler
-  const int lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&mapA); prefetch_tmap(&mapB);
-    for (int i = 0; i < MAXNP; ++i) { mbar_init(pfull0 + 8 * i, 1); mbar_init(pempty0 + 8 * i, 1); }
-    for (int i = 0; i < MAXNB; ++i) { mbar_init(bfull0 + 8 * i, 1); mbar_init(bempty0 + 8 * i, 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(tfull0 + 8 * i, 1); mbar_init(tempty0 + 8 * i, kEpiWarps); }
-    mbar_init(bstat, 1);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc(smem_u32(&tmem_base_smem), TMEM_COLS);
-  if (P.row_boxes && warp >= 2) {
-    // Per-row staging: every image row lands as ONE contiguous box of W pixels at patch row r*P + 1; the two halo
-    // pixels of each patch row (slots r*P and r*P + P-1) are never written by TMA and are zeroed here, once.
-    // (ncu r02a: the single {64, W+2, R} box made this engine TMA-bound -- 6 200 cycles per tile for 1 150 cycles of
-    // MMAs, tensor pipe 24 % active; 128-byte rows of an out-of-bounds-padded box cost ~4x a dense row.)
-    uint8_t* sb = smem_raw + (smem_base - smem_u32(smem_raw));
-    const int nslots = P.NP * P.R * 2;
-    for (int i = (int)threadIdx.x - 64; i < nslots * 8; i += kEpiThreads) {     // 8 x 16 B per 128-byte pixel row
-      const int slot = i >> 3, part = i & 7;
-      const int ps = slot / (P.R * 2), rr = (slot >> 1) % P.R, side = slot & 1;
-      uint4* dst = reinterpret_cast<uint4*>(sb + (size_t)ps * P.patch_bytes + ((size_t)rr * P.P + (side ? P.P - 1 : 0)) * 128) + part;
-      *dst = make_uint4(0u, 0u, 0u, 0u);
-    }
-    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");   // generic-proxy zeros -> visible to the UMMA reads
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, tmem_base_smem, 0);
-  pdl_prologue();      // nothing above touches global memory: setup overlaps the previous kernel's tail
-
-  const int total_tiles = P.n_tiles_m * P.n_tiles_n;
-  const int ntaps_total = 9 * P.cblocks;
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
-      if (P.b_stationary) {
-        // (stationary weights imply a single N tile)
-        mbar_expect_tx(bstat, (uint32_t)ntaps_total * B_BYTES);
-        for (int cb = 0; cb < P.cblocks; ++cb)
-          for (int t = 0; t < 9; ++t)
-            tma_load_2d(b_base + (cb * 9 + t) * B_BYTES, &mapB, bstat, P.kidx[t] * P.Cs + cb * 64, 0);
-      }
-      int ps = 0; uint32_t pphase = 0;
-      int bs = 0; uint32_t bphase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int tn = tile % P.n_tiles_n;
-        const int tm = tile / P.n_tiles_n;
-        const int n = tm / P.tiles_per_img, t = tm - n * P.tiles_per_img;
-        const int q0 = t * 128;
-        const int a = q0 - P.P - 1;
-        const int h_lo = (a >= 0) ? a / P.P : -((-a + P.P - 1) / P.P);
-        for (int cb = 0; cb < P.cblocks; ++cb) {
-          mbar_wait(pempty0 + 8 * ps, pphase ^ 1);
-          if (P.debug == 2) mbar_arrive(pfull0 + 8 * ps);
-          else if (P.row_boxes) {
-            mbar_expect_tx(pfull0 + 8 * ps, (uint32_t)(P.R * P.W * 128));
-            for (int r = 0; r < P.R; ++r)      // rows outside the image are zero-filled by TMA
-              tma_load_4d(smem_base + ps * P.patch_bytes + (uint32_t)(r * P.P + 1) * 128u, &mapA, pfull0 + 8 * ps, cb * 64, 0,
-                          h_lo + r, n);
-          } else {
-            mbar_expect_tx(pfull0 + 8 * ps, (uint32_t)(P.R * P.P * 128));
-            tma_load_4d(smem_base + ps * P.patch_bytes, &mapA, pfull0 + 8 * ps, cb * 64, -1, h_lo, n);
-          }
-          if (++ps == P.NP) { ps = 0; pphase ^= 1; }
-          if (!P.b_stationary) {
-            for (int tp = 0; tp < 9; ++tp) {
-              mbar_wait(bempty0 + 8 * bs, bphase ^ 1);
-              if (P.debug == 2) mbar_arrive(bfull0 + 8 * bs);
-              else {
-                mbar_expect_tx(bfull0 + 8 * bs, B_BYTES);
-                tma_load_2d(b_base + bs * B_BYTES, &mapB, bfull0 + 8 * bs, P.kidx[tp] * P.Cs + cb * 64, tn * BN);
-              }
-              if (++bs == P.NB) { bs = 0; bphase ^= 1; }
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t IDESC = make_idesc_bf16(128, BN, 0, 0);
-    constexpr uint64_t DESC_BASE = make_smem_desc_base(16, 1024);
-    int ps = 0; uint32_t pphase = 0;
-    int bs = 0; uint32_t bphase = 0;
-    int as = 0; uint32_t aphase = 0;
-    if (P.b_stationary) mbar_wait(bstat, 0);
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int tm = tile / P.n_tiles_n;
-      const int t = tm % P.tiles_per_img;
-      const int q0 = t * 128;
-      const int a = q0 - P.P - 1;
-      const int h_lo = (a >= 0) ? a / P.P : -((-a + P.P - 1) / P.P);
-      const int row0 = q0 - h_lo * P.P;          // patch row of tile row 0 for the centre tap
-      mbar_wait(tempty0 + 8 * as, aphase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + as * BN;
-      for (int cb = 0; cb < P.cblocks; ++cb) {
-        mbar_wait(pfull0 + 8 * ps, pphase);
-        tc_fence_after();
-        const uint32_t patch = smem_base + ps * P.patch_bytes;
-        for (int tp = 0; tp < 9; ++tp) {
-          uint32_t sb;
-          if (P.b_stationary) sb = b_base + (cb * 9 + tp) * B_BYTES;
-          else { mbar_wait(bfull0 + 8 * bs, bphase); tc_fence_after(); sb = b_base + bs * B_BYTES; }
-          if (elect_one()) {
-            const uint32_t sa = patch + (uint32_t)(row0 + P.dq[tp]) * 128u;
-            uint64_t abase = DESC_BASE;
-            if (P.use_base_offset) abase |= (uint64_t)((sa >> 7) & 7u) << 49;
-            if (P.debug == 1) {
-              if (!P.b_stationary) mbar_arrive(bempty0 + 8 * bs);
-              if (tp == 8) mbar_arrive(pempty0 + 8 * ps);
-              if (tp == 8 && cb == P.cblocks - 1) mbar_arrive(tfull0 + 8 * as);
-            } else {
-#pragma unroll
-              for (int k = 0; k < 4; ++k)
-                mma_bf16(d_tmem, smem_desc(abase, sa + k * 32), smem_desc(DESC_BASE, sb + k * 32), IDESC,
-                         (cb > 0 || tp > 0 || k > 0) ? 1u : 0u);
-              if (!P.b_stationary) mma_commit(bempty0 + 8 * bs);
-              if (tp == 8) mma_commit(pempty0 + 8 * ps);
-              if (tp == 8 && cb == P.cblocks - 1) mma_commit(tfull0 + 8 * as);
-            }
-          }
-          __syncwarp();
-          if (!P.b_stationary) { if (++bs == P.NB) { bs = 0; bphase ^= 1; } }
-        }
-        if (++ps == P.NP) { ps = 0; pphase ^= 1; }
-      }
-      if (++as == 2) { as = 0; aphase ^= 1; }
-    }
-  } else {
-    // ===================== epilogue =====================
-    const int q = warp & 3;                 // TMEM lane quarter
-    const int ew = warp - 2;                // epilogue warp index, 0 .. kEpiWarps-1
-    const int half = ew >> 2;               // which of the quarter's chunk subsets (0 when kEpiWarps == 4)
-    // per-warp transpose scratch: dynamic shared memory behind the patch / weight rings (static is capped at 48 KB)
-    float* scr = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)) + P.scr_off) + ew * kEpiScratchFloats;
-    const int epi_mode = epi_mode_of(residual, stats, E, 0);
-    int as = 0; uint32_t aphase = 0;
-    // running column sums of this warp, [statistic][chunk][lane] (lane <-> column epi_stat_col(lane)); kept in
-    // shared memory so that the chunk loop can stay ROLLED: unrolled, the epilogue alone was > 100 KB of
-    // SASS and the four epilogue warps stalled on instruction fetch (ncu: stall_no_inst dominant)
-    __shared__ float epi_stats[4][3][BN / 32][32];
-    float (*stw)[BN / 32][32] = epi_stats[q];
-#pragma unroll 1
-    for (int i = half; i < BN / 32; i += kEpiSplit) { stw[0][i][lane] = 0.f; stw[1][i][lane] = 0.f; stw[2][i][lane] = 0.f; }
-    int st_tn = -1;
-    const int etid = ew * 32 + lane;
-    auto flush_stats = [&](int tn_flush) { epi_flush<BN>(epi_stats, stats, P.Cout, tn_flush, E.yd != nullptr, etid); };
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int tn = tile % P.n_tiles_n;
-      if (stats != nullptr && tn != st_tn) { if (st_tn >= 0) flush_stats(st_tn); st_tn = tn; }
-      const int tm = tile / P.n_tiles_n;
-      const int n = tm / P.tiles_per_img, t = tm - n * P.tiles_per_img;
-      long long rowoff[4]; bool rvalid[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int qq = t * 128 + q * 32 + 8 * i + (lane >> 2);
-        const int h = qq / P.P, j = qq - h * P.P;
-        rvalid[i] = (j >= 1) && (j <= P.W) && (h < P.H);
-        const long long pix = ((long long)n * P.H + h) * P.W + (j - 1);
-        rowoff[i] = (rvalid[i] ? pix * P.Cout : 0) + tn * BN;     // outside rows: clamped, loads stay in bounds
-      }
-      epi_tile_dispatch<BN>(epi_mode, tmem_base + ((uint32_t)(q * 32) << 16) + as * BN, true, tfull0 + 8 * as,
-                            aphase, [&]() { mbar_arrive(tempty0 + 8 * as); }, scr, stw, rowoff, rvalid, true, tn,
-                            residual, out, E, lane, half);
-      if (++as == 2) { as = 0; aphase ^= 1; }
-    }
-    if (stats != nullptr && st_tn >= 0) flush_stats(st_tn);
-    if (Fin.mode != 0) {
-      __shared__ unsigned int s_fin_flag;
-      epi_finalize(Fin, stats, P.Cout, etid, &s_fin_flag);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
-}
-
-// ---------------------------------------------------------------------------------
-// wgrad epilogue: lane = accumulator row (one input channel of chunk `ch`), v = 32 consecutive output columns
-// starting at column col0.  fp32 red.global.add into dW[co][tap][ci].
+// wgrad epilogue: this thread's accumulator fragment -- rows r = 16*wq + lane/4 and r + 8 of X chunk `ch`
+// (input channels), columns 8j + 2*(lane%4) (+1) from col0 (output channels) -- into dW[co][tap][ci] at `dw`.
+// Every element has exactly one writer per launch (split): with one split it is added into the gradient buffer
+// (which may already hold a gradient to accumulate onto), with several it is STORED into the split's slice of the
+// workspace and k_wgrad_reduce adds the slices up in a fixed order -- the result does not depend on CTA timing.
 // Strict mode: rows and columns index the split planes -- row r of a 64-element chunk is channel
-// (r/16)*8 + r%8 of plane (r/8)%2, columns likewise -- and the four hi/lo products of one (co, ci) pair land in
-// four accumulator cells: the two planes of a column pair (i, i+8) are added in registers, the two planes of a
-// row pair (lane, lane^8) with one shuffle, and the lanes of plane 0 issue a quarter of the atomics.
+// (r/16)*8 + r%8 of plane (r/8)%2, columns likewise -- so the four hi/lo products of one (co, ci) pair are the
+// cells (r, c), (r+8, c), (r, c+8), (r+8, c+8), all held by the same thread: summed in registers, one atomic.
 // ---------------------------------------------------------------------------------
-__device__ __forceinline__ void wgrad_store(const WgradParams& P, float* __restrict__ dw, const uint32_t (&v)[32],
-                                            const bool valid, const WgradChunk& ch, const int ci_l, const int col0,
-                                            const int lane) {
+template <int BN>
+__device__ __forceinline__ void wgrad_store(const WgradParams& P, float* __restrict__ dw, const float (&d)[BN / 2],
+                                            const WgradChunk& ch, const int col0, const int wq, const int lane) {
+  const int r = 16 * wq + (lane >> 2);
+  const int c = 2 * (lane & 3);
+  const bool store = P.partial != nullptr;
+  auto put = [&](float* p, const float v) { if (store) *p = v; else *p += v; };
   if (!P.split) {
-    if (valid) {
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const int co = col0 + i;
-        if (co < P.Co)
-          atomicAdd(dw + ((long long)co * P.KK + ch.tap) * P.Ci + ch.c0 + ci_l, __uint_as_float(v[i]));
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int co = col0 + 8 * j + c + e;
+        if (co < P.Co) {
+          float* p = dw + ((long long)co * P.KK + ch.tap) * P.Ci + ch.c0 + r;
+          put(p, d[4 * j + e]);
+          put(p + 8, d[4 * j + 2 + e]);
+        }
       }
-    }
     return;
   }
   const float osc = (P.oscale != nullptr) ? __ldg(P.oscale) : 1.f;
-  // real input channel of this row: chunk offset c0 (in split elements) -> c0/2 real channels
-  const int ci = (ch.c0 >> 1) + ((ci_l >> 4) << 3) + (ci_l & 7);
-  const bool plane0 = (ci_l & 8) == 0;
+  // real input channel of rows r / r + 8: chunk offset c0 (in split elements) -> c0/2 real channels
+  const int ci = (ch.c0 >> 1) + ((r >> 4) << 3) + (r & 7);
 #pragma unroll
-  for (int g = 0; g < 2; ++g)
+  for (int g = 0; g < BN / 16; ++g)
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      float s = __uint_as_float(v[16 * g + k]) + __uint_as_float(v[16 * g + 8 + k]);
-      s += __shfl_xor_sync(0xffffffffu, s, 8);
-      const int co = ((col0 + 16 * g) >> 1) + k;
-      if (valid && plane0 && co < P.Co)
-        atomicAdd(dw + ((long long)co * P.KK + ch.tap) * P.Ci + ci, s * osc);
+    for (int e = 0; e < 2; ++e) {
+      const float s = d[8 * g + e] + d[8 * g + 2 + e] + d[8 * g + 4 + e] + d[8 * g + 6 + e];
+      const int co = ((col0 + 16 * g) >> 1) + c + e;
+      if (co < P.Co) put(dw + ((long long)co * P.KK + ch.tap) * P.Ci + ci, s * osc);
     }
 }
 
 // ---------------------------------------------------------------------------------
-// wgrad kernel: one CTA per (M-tile of 2 X chunks, N-tile of BN couts, K split)
+// wgrad kernel: one CTA per (M-tile of 2 X chunks, N-tile of BN couts, K split); consumer warpgroup j owns chunk j
 // ---------------------------------------------------------------------------------
 // OCC = CTAs per SM: with 2, each CTA gets half the stages and the fp32-atomic epilogue of one CTA
-// (~40% of a CTA's life) overlaps the other CTA's MMAs instead of idling the tensor pipe
+// overlaps the other CTA's MMAs instead of idling the tensor cores
 template <int BN, int OCC>
-__global__ void __launch_bounds__(192, OCC)
+__global__ void __launch_bounds__(kConvThreads, OCC)
 k_tc_wgrad(const __grid_constant__ CUtensorMap mapX0, const __grid_constant__ CUtensorMap mapX1,
            const __grid_constant__ CUtensorMap mapX2, const __grid_constant__ CUtensorMap mapX3,
            const __grid_constant__ CUtensorMap mapDY, const __grid_constant__ WgradParams P,
@@ -1233,13 +809,10 @@ k_tc_wgrad(const __grid_constant__ CUtensorMap mapX0, const __grid_constant__ CU
   constexpr uint32_t A_BYTES = 2 * CHUNK_BYTES;
   constexpr uint32_t B_BYTES = (BN / 64) * CHUNK_BYTES;
   constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  constexpr uint32_t TMEM_COLS = (BN <= 64) ? 64 : (BN <= 128 ? 128 : 256);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = __shfl_sync(0xffffffffu, (smem_u32(smem_raw) + 1023u) & ~1023u, 0);
-  __shared__ __align__(8) uint64_t bars[2 * STAGES + 1];
-  __shared__ uint32_t tmem_base_smem;
+  __shared__ __align__(8) uint64_t bars[2 * STAGES];
   const uint32_t full0 = __shfl_sync(0xffffffffu, smem_u32(&bars[0]), 0), empty0 = smem_u32(&bars[STAGES]);
-  const uint32_t tfull = __shfl_sync(0xffffffffu, smem_u32(&bars[2 * STAGES]), 0);
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform for the compiler
   const int lane = threadIdx.x & 31;
 
@@ -1254,20 +827,15 @@ k_tc_wgrad(const __grid_constant__ CUtensorMap mapX0, const __grid_constant__ CU
   int t_end = t_beg + P.tiles_per_split; if (t_end > P.n_pix_tiles) t_end = P.n_pix_tiles;
   const int ksteps = (t_end > t_beg) ? (t_end - t_beg) : 0;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     prefetch_tmap(&mapX0); prefetch_tmap(&mapDY);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(full0 + 8 * i, 1); mbar_init(empty0 + 8 * i, 1); }
-    mbar_init(tfull, 1);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(full0 + 8 * i, 1); mbar_init(empty0 + 8 * i, 2); }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(smem_u32(&tmem_base_smem), TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, tmem_base_smem, 0);
   pdl_prologue();      // nothing above touches global memory: setup overlaps the previous kernel's tail
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     if (elect_one()) {
       int stage = 0; uint32_t phase = 0;
       const WgradChunk ch0 = wgrad_chunk(P, c_lo);
@@ -1291,177 +859,46 @@ k_tc_wgrad(const __grid_constant__ CUtensorMap mapX0, const __grid_constant__ CU
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    const uint32_t IDESC = make_idesc_fmt(128, BN, 1, 1, (uint32_t)P.fmt_a, (uint32_t)P.fmt_b);
-    // MN-major, 128B swizzle: LBO = stride between 64-element MN chunks, SBO = 8-pixel group stride
+  } else {
+    const int wg = warp >> 2;                 // X chunk c_lo + wg = accumulator rows
+    // MN-major, 128B swizzle: LBO = stride between 64-element MN chunks, SBO = 8-pixel group stride;
+    // 64 pixels per stage = 4 x K16, 16 pixel rows = 2048 B
     constexpr uint64_t DESC_BASE = make_smem_desc_base(CHUNK_BYTES, 1024);
     int stage = 0; uint32_t phase = 0;
-    for (int ks = 0; ks < ksteps; ++ks) {
-      mbar_wait(full0 + 8 * stage, phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t sa = smem_base + stage * STAGE_BYTES;
-        const uint32_t sb = sa + A_BYTES;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {     // 64 pixels per stage = 4 x K16; 16 pixel rows = 2048 B
-          mma_bf16(tmem_base, smem_desc(DESC_BASE, sa + k * 2048), smem_desc(DESC_BASE, sb + k * 2048), IDESC,
-                   (ks > 0 || k > 0) ? 1u : 0u);
-        }
-        mma_commit(empty0 + 8 * stage);
-        if (ks == ksteps - 1) mma_commit(tfull);
-      }
-      __syncwarp();
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
-    }
-  } else if (ksteps > 0) {
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    const int j = m >> 6, ci_l = m & 63;
-    const bool valid = j < n_valid_chunks;
-    const WgradChunk ch = wgrad_chunk(P, valid ? c_lo + j : c_lo);
-    mbar_wait(tfull, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int cc = 0; cc < ((P.debug == 3) ? 0 : BN / 32); ++cc) {
-      uint32_t v[32];
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + cc * 32, v);
-      tmem_ld_wait();
-      wgrad_store(P, dw, v, valid, ch, ci_l, nt * BN + cc * 32, lane);
-    }
+    float d[BN / 2];
+    const bool arriver = (threadIdx.x & 127) == 0;
+    if (P.fmt_a)
+      mma_tile<BN, 1, 1, 1, 1>(d, ksteps, stage, phase, STAGES, STAGE_BYTES, smem_base, wg * CHUNK_BYTES, 2048, A_BYTES,
+                               2048, DESC_BASE, DESC_BASE, full0, empty0, arriver, false);
+    else
+      mma_tile<BN, 1, 0, 1, 1>(d, ksteps, stage, phase, STAGES, STAGE_BYTES, smem_base, wg * CHUNK_BYTES, 2048, A_BYTES,
+                               2048, DESC_BASE, DESC_BASE, full0, empty0, arriver, false);
+    float* dst = (P.partial != nullptr) ? P.partial + (long long)split * P.part_stride : dw;
+    if (ksteps > 0 && wg < n_valid_chunks && P.debug != 3)
+      wgrad_store<BN>(P, dst, d, wgrad_chunk(P, c_lo + wg), nt * BN, warp & 3, lane);
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
-// ---------------------------------------------------------------------------------
-// 2-SM wgrad: a CTA pair accumulates a 256 x BN block of dW (4 X chunks x BN couts); each CTA
-// stages 2 X chunks and half of the dY columns.
-// ---------------------------------------------------------------------------------
-static constexpr int wgrad2_stages(int BN) { return BN <= 128 ? 8 : 6; }
-
-template <int BN, int OCC>
-__global__ void __launch_bounds__(192, OCC)
-k_tc_wgrad2(const __grid_constant__ CUtensorMap mapX0, const __grid_constant__ CUtensorMap mapX1,
-            const __grid_constant__ CUtensorMap mapX2, const __grid_constant__ CUtensorMap mapX3,
-            const __grid_constant__ CUtensorMap mapDY, const __grid_constant__ WgradParams P,
-            float* __restrict__ dw) {
-  constexpr int STAGES = wgrad2_stages(BN) / OCC;
-  constexpr uint32_t CHUNK_BYTES = 64 * 128;
-  constexpr uint32_t A_BYTES = 2 * CHUNK_BYTES;
-  constexpr int NBCH = BN / 128;                       // dY chunks (64 couts) staged by this CTA
-  constexpr uint32_t B_BYTES = NBCH * CHUNK_BYTES;
-  constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  constexpr uint32_t TMEM_COLS = (BN <= 128) ? 128 : 256;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = __shfl_sync(0xffffffffu, (smem_u32(smem_raw) + 1023u) & ~1023u, 0);
-  __shared__ __align__(8) uint64_t bars[2 * STAGES + 1];
-  __shared__ uint32_t tmem_base_smem;
-  const uint32_t full0 = __shfl_sync(0xffffffffu, smem_u32(&bars[0]), 0), empty0 = smem_u32(&bars[STAGES]);
-  const uint32_t tfull = __shfl_sync(0xffffffffu, smem_u32(&bars[2 * STAGES]), 0);
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform for the compiler
-  const int lane = threadIdx.x & 31;
-  const uint32_t crank = cluster_ctarank();
-  const bool leader = (crank == 0);
-
-  int u = blockIdx.x / 2;
-  const int split = u % P.splits; u /= P.splits;
-  const int nt = u % P.n_ntiles;
-  const int mt = u / P.n_ntiles;
-  const int c_lo = mt * 4 + 2 * (int)crank;            // this CTA's first X chunk
-  const int n_valid = (c_lo + 1 < P.n_chunks) ? 2 : ((c_lo < P.n_chunks) ? 1 : 0);
-  const int t_beg = split * P.tiles_per_split;
-  int t_end = t_beg + P.tiles_per_split; if (t_end > P.n_pix_tiles) t_end = P.n_pix_tiles;
-  const int ksteps = (t_end > t_beg) ? (t_end - t_beg) : 0;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&mapX0); prefetch_tmap(&mapDY);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(full0 + 8 * i, 2); mbar_init(empty0 + 8 * i, 1); }
-    mbar_init(tfull, 1);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc_2sm(smem_u32(&tmem_base_smem), TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, tmem_base_smem, 0);
-  pdl_prologue();      // nothing above touches global memory: setup overlaps the previous kernel's tail
-
-  if (warp == 0) {
-    if (elect_one()) {
-      int stage = 0; uint32_t phase = 0;
-      const int ca = (n_valid >= 1) ? c_lo : 0;
-      const int cb2 = (n_valid == 2) ? c_lo + 1 : ca;
-      const WgradChunk ch0 = wgrad_chunk(P, ca);
-      const WgradChunk ch1 = wgrad_chunk(P, cb2);
-      const CUtensorMap* m0 = (ch0.map == 0) ? &mapX0 : (ch0.map == 1) ? &mapX1 : (ch0.map == 2) ? &mapX2 : &mapX3;
-      const CUtensorMap* m1 = (ch1.map == 0) ? &mapX0 : (ch1.map == 1) ? &mapX1 : (ch1.map == 2) ? &mapX2 : &mapX3;
-      for (int t = t_beg; t < t_end; ++t) {
-        int tt = t;
-        const int tw = tt % P.tiles_w; tt /= P.tiles_w;
-        const int th = tt % P.tiles_h;
-        const int tb = tt / P.tiles_h;
-        const int ow0 = tw * P.TW, oh0 = th * P.TH, n0 = tb * P.TN;
-        mbar_wait(empty0 + 8 * stage, phase ^ 1);
-        const uint32_t sa = smem_base + stage * STAGE_BYTES;
-        const uint32_t lfull = mapa(full0 + 8 * stage, 0);
-        if (leader) mbar_expect_tx(full0 + 8 * stage, 2 * STAGE_BYTES);
-        else mbar_arrive_cluster(lfull);
-        tma_load_4d_2sm(sa, m0, lfull, ch0.c0, ow0 + ch0.dw, oh0 + ch0.dh, n0);
-        tma_load_4d_2sm(sa + CHUNK_BYTES, m1, lfull, ch1.c0, ow0 + ch1.dw, oh0 + ch1.dh, n0);
+// dw[i] += sum over splits s = 0, 1, ... of part[s * stride + i], added in that order (4 elements per thread).  The
+// loads of 8 splits are issued together before their adds: one dependent DRAM round trip per split would make the
+// kernel latency-bound (tens of splits, few elements per thread).
+__global__ void k_wgrad_reduce(const float4* __restrict__ part, const long long stride4, const int splits,
+                               const long long n4, float4* __restrict__ dw) {
+  pdl_prologue();
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int k0 = 0; k0 < splits; k0 += 8) {
+      float4 v[8];
 #pragma unroll
-        for (int j = 0; j < NBCH; ++j)
-          tma_load_4d_2sm(sa + A_BYTES + j * CHUNK_BYTES, &mapDY, lfull,
-                          nt * BN + (int)crank * (BN / 2) + j * 64, ow0, oh0, n0);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    if (leader) {
-      const uint32_t IDESC = make_idesc_fmt(256, BN, 1, 1, (uint32_t)P.fmt_a, (uint32_t)P.fmt_b);
-      constexpr uint64_t DESC_BASE = make_smem_desc_base(CHUNK_BYTES, 1024);
-      int stage = 0; uint32_t phase = 0;
-      for (int ks = 0; ks < ksteps; ++ks) {
-        mbar_wait(full0 + 8 * stage, phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t sa = smem_base + stage * STAGE_BYTES;
-          const uint32_t sb = sa + A_BYTES;
+      for (int j = 0; j < 8; ++j)
+        v[j] = (k0 + j < splits) ? part[(long long)(k0 + j) * stride4 + i] : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            mma_bf16_2sm(tmem_base, smem_desc(DESC_BASE, sa + k * 2048), smem_desc(DESC_BASE, sb + k * 2048), IDESC,
-                         (ks > 0 || k > 0) ? 1u : 0u);
-          }
-          mma_commit_2sm(empty0 + 8 * stage, 3);
-          if (ks == ksteps - 1) mma_commit_2sm(tfull, 3);
-        }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
+      for (int j = 0; j < 8; ++j) { s.x += v[j].x; s.y += v[j].y; s.z += v[j].z; s.w += v[j].w; }
     }
-  } else if (ksteps > 0) {
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    const int j = m >> 6, ci_l = m & 63;
-    const bool valid = j < n_valid;
-    const WgradChunk ch = wgrad_chunk(P, valid ? c_lo + j : 0);
-    mbar_wait(tfull, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int cc = 0; cc < BN / 32; ++cc) {
-      uint32_t v[32];
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + cc * 32, v);
-      tmem_ld_wait();
-      wgrad_store(P, dw, v, valid, ch, ci_l, nt * BN + cc * 32, lane);
-    }
+    float4 o = dw[i];
+    o.x += s.x; o.y += s.y; o.z += s.z; o.w += s.w;
+    dw[i] = o;
   }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync();
-  tc_fence_after();
-  if (warp == 1) tmem_dealloc_2sm(tmem_base, TMEM_COLS);
 }
 
 // ---------------------------------------------------------------------------------
@@ -1481,12 +918,6 @@ struct TcConvPlan {
   const bf16* wmat;
   const bf16* wmat2;                    // dgrad weight matrix [Ci][Co2] of a folded 1x1/stride-2 shortcut conv, or null
   int BN, CL;
-  bool two_cta;                         // cta_group::2 kernel (256 x BN pair tiles)
-  bool occ2;                            // BN = 64 per-tap kernel with two CTAs per SM (epilogue-bound launches)
-  bool halo;                            // halo-resident 3x3/s1 engine
-  HaloParams HP;
-  CUtensorMap hmapA, hmapB;
-  size_t halo_smem;
   std::vector<ConvLaunch> launches;     // fprop: 1; dgrad: 1 (stride 1) or 4 (stride 2)
   // wgrad
   WgradParams WP;
@@ -1497,6 +928,7 @@ struct TcConvPlan {
   const void *c_in0, *c_in1;
   bool smem_attr_set;
   const float* out_scale;               // strict mode dgrad / wgrad: device scalar applied to the accumulators, or null
+  float* ws;                            // wgrad with split-K: per-split dW slices (allocated at the first run)
 };
 
 static void pick_box(int Wd, int Hd, int pixels, int* TW, int* TH, int* TN) {
@@ -1509,91 +941,56 @@ static void pick_box(int Wd, int Hd, int pixels, int* TW, int* TH, int* TN) {
   *TW = tw; *TH = th; *TN = tn;
 }
 
-// N-tile: wider tiles re-use the A operand more (the engines are L2-bandwidth bound), but
-// must still leave enough tiles to occupy the 148 SMs.
-static int pick_bn(int Cout, long long M) {
-  static int force = -1;
-  if (force < 0) { const char* e = getenv("MAPNET_TC_BN"); force = e ? atoi(e) : 0; }
-  if (force == 64 || (force == 128 && Cout % 128 == 0) || (force == 256 && Cout % 256 == 0)) return force;
-  if (Cout % 256 == 0 && (M / 128) * (Cout / 256) >= 120) return 256;
-  if (Cout % 128 == 0) return 128;
-  return 64;
-}
-
 static int pick_cl() {
   static int cl = -1;
   if (cl < 0) { const char* e = getenv("MAPNET_TC_CLUSTER"); cl = e ? atoi(e) : 1; if (cl != 1 && cl != 2 && cl != 4) cl = 1; }
   return cl;
 }
 
-static int use_2cta() {     // -1 auto (cost model), 0 never, 1 whenever the channel count allows
-  static int v = -2;
-  if (v == -2) { const char* e = getenv("MAPNET_TC_2CTA"); v = e ? atoi(e) : -1; }
-  return v;
+// N tile by a small cost model: wider tiles re-use the A operand more, but must still leave enough work items to
+// occupy the SMs.  A k-block costs max(bytes staged / ingest rate, MMA issue time) plus a fixed cost per work item
+// (prologue, epilogue).  The constants -- ~55 B per cycle of TMA ingest, 580 / 600 cycles of issue per k-block, ~2000
+// cycles per work item -- are carried over from a fit to an earlier tensor-memory engine on another GPU and have NOT
+// been measured for these wgmma engines on H100: treat the model as a ranking heuristic between BN = 64 and 128.
+// BN is 64 or 128 because a consumer warpgroup holds its 64 x BN fp32 accumulator in registers.  MAPNET_TC_BN=64|128
+// forces the choice (where Cout allows it).
+static int forced_bn() {
+  static int f = -1;
+  if (f < 0) { const char* e = getenv("MAPNET_TC_BN"); f = e ? atoi(e) : 0; }
+  return f;
 }
-
-// Tile configuration by a small cost model fitted to tools/bench_conv.py on B200
-// (profiles/r01_conv_microbench.txt): a k-block (4 MMAs + barrier round trip) costs the issuing
-// warp ~600 cycles for N <= 128 and ~980 for N = 256 on one CTA, ~490 / ~1075 on a CTA pair;
-// TMA alone sustains ~55 B/cycle per CTA; a kernel needs waves x (k-blocks x max(...) + ~2000).
-struct TileChoice { int BN; bool two_cta; };
+static double kblock_cycles(int bn) {
+  const double bytes = 16384.0 + bn * 128.0;
+  const double issue = bn <= 64 ? 580.0 : 600.0;
+  return (bytes / 55.0 > issue) ? bytes / 55.0 : issue;
+}
 // `ncls` classes of `mtiles` M tiles each, class c with kb[c] k-blocks per tile (a stride-2 dgrad launched as ONE
 // grid over its parity classes); work items are dealt round-robin to the persistent CTAs, heaviest class first
-static TileChoice choose_tiles_classes(int Cout, long long mtiles, int ncls, const int* kb) {
-  const int forced_bn = []() { const char* e = getenv("MAPNET_TC_BN"); return e ? atoi(e) : 0; }();
-  const int mode2 = use_2cta();
-  TileChoice best = {64, false};
+static int choose_bn_classes(int Cout, long long mtiles, int ncls, const int* kb) {
+  int best = 64;
   double best_t = 1e30;
-  for (int two = 0; two <= 1; ++two) {
-    if (two && mode2 == 0) continue;
-    if (!two && mode2 == 1 && Cout % 128 == 0) continue;
-    for (int bn = 64; bn <= 256; bn *= 2) {
-      if (Cout % bn != 0) continue;
-      if (two && bn < 128) continue;
-      if (forced_bn && bn != forced_bn && Cout % forced_bn == 0 && !(two && forced_bn < 128)) continue;
-      const long long per_class = (two ? (mtiles + 1) / 2 : mtiles) * (Cout / bn);
-      const int slots = two ? 74 : 148;
-      const double bytes = 16384.0 + (two ? bn * 64.0 : bn * 128.0);
-      const double issue = two ? (bn <= 128 ? 490.0 : 1075.0) : (bn <= 64 ? 580.0 : (bn <= 128 ? 600.0 : 980.0));
-      const double per_kb = (bytes / 55.0 > issue) ? bytes / 55.0 : issue;
-      // slot j gets items j, j + slots, ...: the busiest slot bounds the launch
-      double t = 0.0;
-      const long long total = per_class * ncls;
-      for (int j = 0; j < slots && j < total; ++j) {
-        double tj = 0.0;
-        for (long long it = j; it < total; it += slots) tj += kb[it / per_class] * per_kb + 2000.0;
-        if (tj > t) t = tj;
-      }
-      if (t < best_t) { best_t = t; best.BN = bn; best.two_cta = (two != 0); }
+  for (int bn = 64; bn <= 128; bn *= 2) {
+    if (Cout % bn != 0) continue;
+    if (forced_bn() && bn != forced_bn() && Cout % forced_bn() == 0) continue;
+    const long long per_class = mtiles * (Cout / bn);
+    const double per_kb = kblock_cycles(bn);
+    // slot j gets items j, j + slots, ...: the busiest slot bounds the launch
+    double t = 0.0;
+    const long long total = per_class * ncls;
+    for (int j = 0; j < kNumSMs && j < total; ++j) {
+      double tj = 0.0;
+      for (long long it = j; it < total; it += kNumSMs) tj += kb[it / per_class] * per_kb + 2000.0;
+      if (tj > t) t = tj;
     }
+    if (t < best_t) { best_t = t; best = bn; }
   }
   return best;
 }
 
-static TileChoice choose_tiles(int Cout, long long Mpix, int kblocks) {
-  const int forced_bn = []() { const char* e = getenv("MAPNET_TC_BN"); return e ? atoi(e) : 0; }();
-  const int mode2 = use_2cta();
+static int choose_bn(int Cout, long long Mpix, int kblocks) {
   const long long mtiles = (Mpix + 127) / 128;
-  TileChoice best = {64, false};
-  double best_t = 1e30;
-  for (int two = 0; two <= 1; ++two) {
-    if (two && mode2 == 0) continue;
-    if (!two && mode2 == 1 && Cout % 128 == 0) continue;
-    for (int bn = 64; bn <= 256; bn *= 2) {
-      if (Cout % bn != 0) continue;
-      if (two && bn < 128) continue;
-      if (forced_bn && bn != forced_bn && Cout % forced_bn == 0 && !(two && forced_bn < 128)) continue;
-      const long long items = (two ? (mtiles + 1) / 2 : mtiles) * (Cout / bn);
-      const int slots = two ? 74 : 148;
-      const long long waves = (items + slots - 1) / slots;
-      const double bytes = 16384.0 + (two ? bn * 64.0 : bn * 128.0);
-      const double issue = two ? (bn <= 128 ? 490.0 : 1075.0) : (bn <= 64 ? 580.0 : (bn <= 128 ? 600.0 : 980.0));
-      const double per_kb = (bytes / 55.0 > issue) ? bytes / 55.0 : issue;
-      const double t = (double)waves * (kblocks * per_kb + 2000.0);
-      if (t < best_t) { best_t = t; best.BN = bn; best.two_cta = (two != 0); }
-    }
-  }
-  return best;
+  const int kb[1] = {kblocks};
+  return choose_bn_classes(Cout, mtiles, 1, kb);
 }
 
 static int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
@@ -1608,82 +1005,15 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
   MN_CHECK(g.in_pix_stride == 0 || (g.stride == 1 && kind != 1), "tc conv: strided input views only for stride-1 fprop / wgrad");
   TcConvPlan* p = new TcConvPlan();
   p->g = g; p->kind = kind; p->wmat = wmat; p->wmat2 = nullptr; p->shortcut_flops_k = 0;
-  p->c_in0 = p->c_in1 = nullptr; p->smem_attr_set = false; p->out_scale = nullptr;
+  p->c_in0 = p->c_in1 = nullptr; p->smem_attr_set = false; p->out_scale = nullptr; p->ws = nullptr;
   p->CL = pick_cl();
-  p->two_cta = false;
-  p->occ2 = false;
-  p->halo = false;
   const int s = g.stride, pad = g.pad, KK = g.KH * g.KW;
   // strict mode: the engines see 2*C 16-bit channels per pixel and every filter tap twice (hi / lo weight planes)
   const int SP = g.split ? 2 : 1;
   MN_CHECK(!g.split || KK <= 9, "tc conv: strict mode supports up to 9 filter taps");
-  {
-    static int halo_mode = -1, halo_bo = -1;
-    // default OFF since round 2: the Cout = 64 launches are bound by per-CTA serial latency, and the per-tap engine with TWO
-    // CTAs per SM (OCC = 2 below) beats the halo engine on layer1 (31.6 vs 38.7 us fprop, 38.8 vs 47.5 us gated dgrad at B = 64,
-    // profiles/r02b_conv_microbench.txt); MAPNET_TC_HALO=1 selects the halo-resident engine again
-    if (halo_mode < 0) { const char* e = getenv("MAPNET_TC_HALO"); halo_mode = e ? atoi(e) : 0; }
-    if (halo_bo < 0) { const char* e = getenv("MAPNET_TC_HALO_BASEOFF"); halo_bo = e ? atoi(e) : 0; }   // measured: swizzle follows absolute smem address bits, base_offset must stay 0
-    if (halo_mode && !g.split && (kind == 0 || kind == 1) && g.KH == 3 && s == 1 && g.Wi + 2 <= 256) {
-      // fprop: gather x [B,H,W,Ci] -> y [.,Co]; dgrad: gather dy [B,H,W,Co] -> dx [.,Ci] (same spatial dims)
-      const int Cs = (kind == 0) ? g.Ci : g.Co, Cn = (kind == 0) ? g.Co : g.Ci;
-      HaloParams& H = p->HP; memset(&H, 0, sizeof(H));
-      H.Nimg = g.B; H.H = g.Hi; H.W = g.Wi; H.P = g.Wi + 2;
-      H.tiles_per_img = cdiv((long long)g.Hi * H.P, 128);
-      H.n_tiles_m = g.B * H.tiles_per_img;
-      H.cblocks = Cs / 64; H.Cs = Cs; H.Cout = Cn;
-      // rows needed: from floor((q0-P-1)/P) to floor((q0+127+P+1)/P) for any q0 = 128 t
-      H.R = (128 + 2 * H.P + 2 + H.P - 1) / H.P + 1;
-      if (H.R > g.Hi + 3) H.R = g.Hi + 3;
-      if (H.R <= 256) {
-        H.patch_bytes = (int)(((long long)H.R * H.P * 128 + 1023) / 1024 * 1024);
-        // N tile: the patch cost is per tile, so prefer wide N; keep >= ~120 tiles when possible
-        int bn = (Cn % 256 == 0 && H.n_tiles_m >= 120) ? 256 : ((Cn % 128 == 0) ? 128 : 64);
-        { const char* e = getenv("MAPNET_TC_BN"); int f = e ? atoi(e) : 0; if ((f == 64 || f == 128 || f == 256) && Cn % f == 0) bn = f; }
-        const long long wbytes = 9LL * H.cblocks * bn * 128;
-        // 227 KB per CTA minus the alignment slack and the kernel's static shared memory (epilogue scratch,
-        // per-warp statistics, barriers)
-        const long long budget = 227LL * 1024 - 1024 - ((long long)kEpiWarps * kEpiScratchFloats * 4 + 1536LL * (bn / 32) + 512);
-        H.b_stationary = (Cn == bn && wbytes + 2LL * H.patch_bytes <= budget) ? 1 : 0;
-        long long left = budget - (H.b_stationary ? wbytes : 0);
-        if (H.b_stationary) { H.NP = (int)(left / H.patch_bytes); H.NB = 0; }
-        else {
-          H.NP = 2; left -= 2LL * H.patch_bytes;
-          H.NB = (int)(left / (bn * 128));
-          while (H.NB > 12) { if (H.NP < 4 && left - H.patch_bytes >= 6LL * bn * 128) { H.NP++; left -= H.patch_bytes; H.NB = (int)(left / (bn * 128)); } else H.NB = 12; }
-        }
-        if (H.NP > 4) H.NP = 4;
-        static int halo_all = -1;
-        if (halo_all < 0) { const char* e = getenv("MAPNET_TC_HALO_ALL"); halo_all = e ? atoi(e) : 0; }
-        // measured (tools/bench_conv.py): the halo engine wins only with stationary weights (Cin = 64);
-        // elsewhere the big patch box is slower than per-tap boxes and the weights dominate
-        if (H.NP >= 2 && (H.b_stationary || (halo_all && H.NB >= 3))) {
-          p->halo = true; p->BN = bn;
-          H.n_tiles_n = Cn / bn;
-          H.use_base_offset = halo_bo;
-          { const char* e = getenv("MAPNET_TC_HALO_ROWS"); H.row_boxes = e ? (atoi(e) != 0) : 1; }
-          { const char* e = getenv("MAPNET_TC_DEBUG"); H.debug = e ? atoi(e) : 0; }
-          for (int kh = 0; kh < 3; ++kh)
-            for (int kw = 0; kw < 3; ++kw) {
-              const int t = kh * 3 + kw;
-              H.kidx[t] = t;
-              H.dq[t] = (kind == 0) ? ((kh - 1) * H.P + (kw - 1)) : ((1 - kh) * H.P + (1 - kw));
-            }
-          H.scr_off = H.NP * H.patch_bytes + (H.b_stationary ? 9 * H.cblocks : H.NB) * bn * 128;
-          p->halo_smem = (size_t)H.scr_off + (size_t)kEpiWarps * kEpiScratchFloats * 4 + 1024;
-          *out = p;
-          return 0;
-        }
-      }
-    }
-  }
   if (kind == 0) {
     // ---------------- fprop ----------------
-    {
-      const TileChoice tc = choose_tiles(g.Co, g.M_out(), SP * KK * (SP * g.Ci / 64));
-      p->BN = tc.BN; p->two_cta = tc.two_cta;
-      if (tc.two_cta) p->CL = 2;
-    }
+    p->BN = choose_bn(g.Co, g.M_out(), SP * KK * (SP * g.Ci / 64));
     ConvLaunch L; memset(&L, 0, sizeof(L));
     ConvParams& P = L.P;
     { const char* e = getenv("MAPNET_TC_DEBUG"); P.debug = e ? atoi(e) : 0; }
@@ -1740,8 +1070,7 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
     { const char* e = getenv("MAPNET_TC_DGRAD_MERGE"); if (e) merge = atoi(e); }
     if (s == 1 || merge) {
       // ONE launch over all classes, heaviest class first (the persistent CTAs take work items round-robin).
-      // Measured on B200 (profiles/r01b_launch_shares.csv): as four launches of 1..4 taps on 1/4 of the pixels
-      // the stride-2 dgrads of layer2.0/3.0/4.0 ran at 100-130 TFLOP/s -- each launch a single short wave.
+      // As four launches of 1..4 taps on 1/4 of the pixels each stride-2 dgrad would be four single short waves.
       for (int i = 1; i < ncls; ++i)              // stable insertion sort by tap count, descending
         for (int j = i; j > 0 && ct[j].n > ct[j - 1].n; --j) { ClassTaps tmp = ct[j]; ct[j] = ct[j - 1]; ct[j - 1] = tmp; }
       const int Hs0 = cdiv(g.Hi, s), Ws0 = cdiv(g.Wi, s);      // the largest class (a = b = 0)
@@ -1755,11 +1084,7 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
       P.n_tiles_m = P.tiles_w * P.tiles_h * P.tiles_n;
       int kbs[4];
       for (int i = 0; i < ncls; ++i) kbs[i] = ct[i].n * (SP * g.Co / 64);
-      {
-        const TileChoice tc = choose_tiles_classes(g.Ci, P.n_tiles_m, ncls, kbs);
-        p->BN = tc.BN; p->two_cta = tc.two_cta;
-        if (tc.two_cta) p->CL = 2;
-      }
+      p->BN = choose_bn_classes(g.Ci, P.n_tiles_m, ncls, kbs);
       P.n_tiles_n = g.Ci / p->BN;
       P.cblocks = SP * g.Co / 64; P.Cs = SP * g.Co;
       P.Hout = g.Hi; P.Wout = g.Wi; P.Cout = g.Ci; P.os = s;
@@ -1774,12 +1099,8 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
       L.n_maps = 1; L.pa[0] = L.pb[0] = 0;
       p->launches.push_back(L);
     } else {
-      {
-        // one launch per class: size the tiles for one class
-        const TileChoice tc = choose_tiles(g.Ci, g.M_in() / (s * s), SP * ((KK + s * s - 1) / (s * s)) * (SP * g.Co / 64));
-        p->BN = tc.BN; p->two_cta = tc.two_cta;
-        if (tc.two_cta) p->CL = 2;
-      }
+      // one launch per class: size the tiles for one class
+      p->BN = choose_bn(g.Ci, g.M_in() / (s * s), SP * ((KK + s * s - 1) / (s * s)) * (SP * g.Co / 64));
       for (int i = 0; i < ncls; ++i) {
         ConvLaunch L; memset(&L, 0, sizeof(L));
         ConvParams& P = L.P;
@@ -1804,9 +1125,9 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
     WgradParams& P = p->WP; memset(&P, 0, sizeof(P));
     { const char* e = getenv("MAPNET_TC_DEBUG"); P.debug = e ? atoi(e) : 0; }
     const int CoS = SP * g.Co, CiS = SP * g.Ci;      // GEMM N / M extents in 16-bit operand elements
-    p->BN = (CoS % 256 == 0) ? 256 : ((CoS % 128 == 0) ? 128 : 64);
-    MN_CHECK(p->BN == 64 || p->BN == 128 || p->BN == 256, "tc wgrad: Co=%d unsupported", g.Co);
+    p->BN = (CoS % 128 == 0) ? 128 : 64;      // 64 x BN fp32 accumulator per consumer warpgroup in registers
     P.split = g.split; P.fmt_a = g.split ? g.fmt_z : 1; P.fmt_b = g.split ? g.fmt_g : 1;
+    MN_CHECK(P.fmt_a == P.fmt_b, "tc wgrad: wgmma needs both operands in the same 16-bit format");
     P.BN = p->BN; P.Nimg = g.B; P.Ho = g.Ho; P.Wo = g.Wo; P.Ci = g.Ci; P.Co = g.Co; P.KK = KK;
     pick_box(g.Wo, g.Ho, 64, &P.TW, &P.TH, &P.TN);
     P.tiles_w = cdiv(g.Wo, P.TW); P.tiles_h = cdiv(g.Ho, P.TH); P.tiles_n = cdiv(g.B, P.TN);
@@ -1814,10 +1135,7 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
     P.cpt = CiS / 64;
     P.n_chunks = KK * P.cpt;
     MN_CHECK(KK <= 16, "tc wgrad: too many filter taps");
-    p->two_cta = (use_2cta() != 0) && (CoS % 128 == 0);
-    if (p->two_cta) p->BN = (CoS % 256 == 0) ? 256 : 128;
-    P.BN = p->BN;
-    P.n_mtiles = cdiv(P.n_chunks, p->two_cta ? 4 : 2); P.n_ntiles = CoS / p->BN;
+    P.n_mtiles = cdiv(P.n_chunks, 2); P.n_ntiles = CoS / p->BN;
     p->w_nmaps = 0;
     for (int kh = 0; kh < g.KH; ++kh)
       for (int kw = 0; kw < g.KW; ++kw) {
@@ -1833,7 +1151,7 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
         }
       }
     const int units = P.n_mtiles * P.n_ntiles;
-    int splits = (p->two_cta ? 74 * 2 : 148 * 2) / units; if (splits < 1) splits = 1;
+    int splits = (kNumSMs * 2) / units; if (splits < 1) splits = 1;
     if (splits > P.n_pix_tiles) splits = P.n_pix_tiles;
     P.tiles_per_split = cdiv(P.n_pix_tiles, splits);
     P.splits = cdiv(P.n_pix_tiles, P.tiles_per_split);
@@ -1842,7 +1160,10 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
   return 0;
 }
 
-void tc_plan_destroy(TcConvPlan* p) { delete p; }
+void tc_plan_destroy(TcConvPlan* p) {
+  if (p != nullptr && p->ws != nullptr) cudaFree(p->ws);
+  delete p;
+}
 void tc_plan_set_out_scale(TcConvPlan* p, const float* inv_scale) { if (p != nullptr) p->out_scale = inv_scale; }
 
 // Fold the dgrad of the block's 1x1 / stride-2 downsample conv into the (merged) dgrad of its 3x3 / stride-2 conv1:
@@ -1851,7 +1172,7 @@ void tc_plan_set_out_scale(TcConvPlan* p, const float* inv_scale) { if (p != nul
 // matrix wmat2 = [Ci][Co].  Replaces 4 launches, a zero-filled full-size tensor and its re-read as a residual.
 int tc_plan_add_shortcut(TcConvPlan* p, const bf16* wmat2) {
   MN_CHECK(p != nullptr && wmat2 != nullptr, "tc_plan_add_shortcut: null argument");
-  MN_CHECK(p->kind == 1 && !p->halo && !p->g.split && p->g.stride == 2 && p->g.KH == 3 && p->launches.size() == 1,
+  MN_CHECK(p->kind == 1 && !p->g.split && p->g.stride == 2 && p->g.KH == 3 && p->launches.size() == 1,
            "tc_plan_add_shortcut: needs a merged 3x3 stride-2 dgrad plan (bf16 mode)");
   ConvParams& P = p->launches[0].P;
   ClassDesc& c = P.cls[P.n_classes - 1];
@@ -1879,19 +1200,8 @@ int tc_plan_describe(const TcConvPlan* p, char* buf, int cap) {
     va_end(ap);
     if (w < 0 || w >= cap - n) ovf = true; else n += w;
   };
-  put("{\"kind\":%d,\"halo\":%d,\"BN\":%d,\"two_cta\":%d,\"CL\":%d,\"shortcut\":%d", p->kind, p->halo ? 1 : 0, p->BN,
-      p->two_cta ? 1 : 0, p->CL, p->wmat2 != nullptr ? 1 : 0);
-  if (p->halo) {
-    const HaloParams& H = p->HP;
-    put(",\"halo_params\":{\"Nimg\":%d,\"H\":%d,\"W\":%d,\"P\":%d,\"tiles_per_img\":%d,\"n_tiles_m\":%d,\"n_tiles_n\":%d,"
-        "\"cblocks\":%d,\"Cs\":%d,\"Cout\":%d,\"R\":%d,\"NP\":%d,\"NB\":%d,\"b_stationary\":%d,\"smem\":%lld,\"dq\":[",
-        H.Nimg, H.H, H.W, H.P, H.tiles_per_img, H.n_tiles_m, H.n_tiles_n, H.cblocks, H.Cs, H.Cout, H.R, H.NP, H.NB,
-        H.b_stationary, (long long)p->halo_smem);
-    for (int t = 0; t < 9; ++t) put("%s%d", t ? "," : "", H.dq[t]);
-    put("],\"kidx\":[");
-    for (int t = 0; t < 9; ++t) put("%s%d", t ? "," : "", H.kidx[t]);
-    put("]}");
-  } else if (p->kind == 2) {
+  put("{\"kind\":%d,\"BN\":%d,\"CL\":%d,\"shortcut\":%d", p->kind, p->BN, p->CL, p->wmat2 != nullptr ? 1 : 0);
+  if (p->kind == 2) {
     const WgradParams& P = p->WP;
     put(",\"wgrad\":{\"TW\":%d,\"TH\":%d,\"TN\":%d,\"tiles_w\":%d,\"tiles_h\":%d,\"tiles_n\":%d,\"n_pix_tiles\":%d,"
         "\"n_chunks\":%d,\"n_mtiles\":%d,\"n_ntiles\":%d,\"BN\":%d,\"splits\":%d,\"tiles_per_split\":%d,\"Ci\":%d,\"Co\":%d,"
@@ -1932,7 +1242,7 @@ int tc_plan_describe(const TcConvPlan* p, char* buf, int cap) {
   return 0;
 }
 
-int tc_plan_launches(const TcConvPlan* p) { return p->halo ? 1 : (p->kind == 2 ? 1 : (int)p->launches.size()); }
+int tc_plan_launches(const TcConvPlan* p) { return p->kind == 2 ? 1 : (int)p->launches.size(); }
 
 template <typename K>
 static int set_smem(K kernel, size_t bytes) {
@@ -1974,29 +1284,7 @@ int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* res
   E.oscale = p->out_scale;
   const ConvGeom& g = p->g;
   const int SP = g.split ? 2 : 1;
-  int nsm = 148;
-  if (p->halo) {
-    HaloParams& H = p->HP;
-    if (p->c_in0 != in0) {
-      const int Cs = H.Cs;
-      MN_TRY(encode_act_map(&p->hmapA, in0, Cs, H.W, H.H, H.Nimg, (long long)Cs * 2, (long long)H.W * Cs * 2,
-                            (long long)H.H * H.W * Cs * 2, H.row_boxes ? H.W : H.P, H.row_boxes ? 1 : H.R, 1));
-      MN_TRY(encode_w_map(&p->hmapB, p->wmat, 9 * Cs, H.Cout, p->BN));
-      p->c_in0 = in0;
-    }
-    void (*kern)(CUtensorMap, CUtensorMap, HaloParams, const bf16*, bf16*, double*, EpiBwd, EpiFin) =
-        (p->BN == 64) ? k_tc_conv_halo<64> : (p->BN == 128 ? k_tc_conv_halo<128> : k_tc_conv_halo<256>);
-    if (!p->smem_attr_set) {
-      MN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->halo_smem));
-      p->smem_attr_set = true;
-    }
-    const int total = H.n_tiles_m * H.n_tiles_n;
-    const int grid = total < nsm ? total : nsm;
-    F.expected = (unsigned int)grid;
-    MN_LAUNCH(kern, grid, kConvThreads, p->halo_smem, st, p->hmapA, p->hmapB, H, residual, (bf16*)out, stats, E, F);
-    MN_LAUNCH_CHECK();
-    return 0;
-  }
+  const int nsm = kNumSMs;
   if (p->kind == 0 || p->kind == 1) {
     MN_CHECK(p->wmat2 == nullptr || in1 != nullptr, "tc_conv_run: a dgrad plan with a folded shortcut needs the shortcut's gradient as in1");
     if (p->c_in0 != in0 || (p->wmat2 != nullptr && p->c_in1 != in1)) {
@@ -2019,31 +1307,16 @@ int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* res
       }
       p->c_in0 = in0; p->c_in1 = in1;
     }
-    const size_t scratch = (size_t)kEpiWarps * kEpiScratchFloats * 4;      // epilogue transpose scratch behind the stages
-    size_t smem = (size_t)conv_stages(p->BN) * (128 * 128 + p->BN * 128) + 1024 + scratch;
+    const size_t smem = conv_smem_bytes(p->BN);
     void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, ConvParams, const bf16*, bf16*, double*, EpiBwd, EpiFin) = nullptr;
-    if (p->two_cta) {
-      smem = (size_t)conv2_stages(p->BN) * (128 * 128 + (p->BN / 2) * 128) + 1024 + scratch;
-      kern = (p->BN == 256) ? k_tc_conv2<256> : k_tc_conv2<128>;
-    }
-#define PICK(BNv, CLv) if (!p->two_cta && p->BN == BNv && p->CL == CLv) kern = k_tc_conv<BNv, CLv>;
-    PICK(64, 1) PICK(128, 1) PICK(256, 1) PICK(64, 2) PICK(128, 2) PICK(256, 2) PICK(64, 4) PICK(128, 4) PICK(256, 4)
+#define PICK(BNv, CLv) if (p->BN == BNv && p->CL == CLv) kern = k_tc_conv<BNv, CLv>;
+    PICK(64, 1) PICK(128, 1) PICK(64, 2) PICK(128, 2) PICK(64, 4) PICK(128, 4)
 #undef PICK
-    {
-      static int occ2 = -1;
-      if (occ2 < 0) { const char* e = getenv("MAPNET_TC_OCC2"); occ2 = e ? atoi(e) : 1; }
-      p->occ2 = occ2 && !p->two_cta && p->BN == 64 && p->CL == 1 && kEpiWarps == 4;
-      if (p->occ2) {
-        kern = k_tc_conv<64, 1, 2>;
-        smem = (size_t)kOcc2Stages * (128 * 128 + 64 * 128) + 1024 + scratch;
-      }
-    }
     MN_CHECK(kern != nullptr, "tc conv: no kernel for BN=%d CL=%d", p->BN, p->CL);
     if (!p->smem_attr_set) {
       MN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
       p->smem_attr_set = true;
     }
-    if (p->occ2) nsm *= 2;
     F.expected = 0;
     for (auto& L : p->launches) {     // the sums of a stride-2 dgrad come from all its parity classes / launches
       const int groups = cdiv(L.P.n_tiles_m, p->CL) * L.P.n_tiles_n * L.P.n_classes;
@@ -2051,8 +1324,8 @@ int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* res
       F.expected += (unsigned int)((groups < max_clusters ? groups : max_clusters) * p->CL);
     }
     static int epi_pf = -1;
-    // measured on B200 (posenet_bs64): 3.911 ms/step without, 3.917 with -- the fused dgrad epilogues are not bound by
-    // the DRAM latency of their extra operands (most are L2 hits right behind their producers): opt-in experiment
+    // opt-in experiment: the fused dgrad epilogues read extra operands that are mostly L2 hits right behind their
+    // producers
     if (epi_pf < 0) { const char* e = getenv("MAPNET_TC_EPI_PREFETCH"); epi_pf = e ? atoi(e) : 0; }
     for (auto& L : p->launches) {
       const int groups = cdiv(L.P.n_tiles_m, p->CL) * L.P.n_tiles_n * L.P.n_classes;
@@ -2085,39 +1358,38 @@ int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* res
   }
   static int occ = -1;
   if (occ < 0) { const char* e = getenv("MAPNET_TC_WGRAD_OCC"); occ = (e && atoi(e) == 1) ? 1 : 2; }   // measured: 2 CTAs/SM = 587 -> 781 TF/s on layer3/4 wgrad
-  if (p->two_cta) {
-    const size_t smem2 = (size_t)(wgrad2_stages(p->BN) / occ) * (2 * 8192 + (p->BN / 128) * 8192) + 1024;
-    void (*k2)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, WgradParams, float*) =
-        (occ == 2) ? ((p->BN == 256) ? k_tc_wgrad2<256, 2> : k_tc_wgrad2<128, 2>)
-                   : ((p->BN == 256) ? k_tc_wgrad2<256, 1> : k_tc_wgrad2<128, 1>);
-    if (!p->smem_attr_set) {
-      MN_CUDA(cudaFuncSetAttribute(k2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-      p->smem_attr_set = true;
-    }
-    cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(P.n_mtiles * P.n_ntiles * P.splits * 2); cfg.blockDim = dim3(192);
-    cfg.dynamicSmemBytes = smem2; cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    MN_CUDA(cudaLaunchKernelEx(&cfg, k2, p->mapX[0], p->mapX[1], p->mapX[2], p->mapX[3], p->mapDY, P, (float*)out));
-    ++g_launch_count;
-    return 0;
-  }
   const int stages = wgrad_stages(p->BN) / occ;
   const size_t smem = (size_t)stages * (2 * 8192 + (p->BN / 64) * 8192) + 1024;
   void (*k1)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, WgradParams, float*) =
-      (occ == 2) ? ((p->BN == 64) ? k_tc_wgrad<64, 2> : (p->BN == 128 ? k_tc_wgrad<128, 2> : k_tc_wgrad<256, 2>))
-                 : ((p->BN == 64) ? k_tc_wgrad<64, 1> : (p->BN == 128 ? k_tc_wgrad<128, 1> : k_tc_wgrad<256, 1>));
+      (occ == 2) ? ((p->BN == 64) ? k_tc_wgrad<64, 2> : k_tc_wgrad<128, 2>)
+                 : ((p->BN == 64) ? k_tc_wgrad<64, 1> : k_tc_wgrad<128, 1>);
   if (!p->smem_attr_set) {
     MN_TRY(set_smem(k1, smem));
     p->smem_attr_set = true;
   }
   const int grid = P.n_mtiles * P.n_ntiles * P.splits;
-  MN_LAUNCH(k1, grid, 192, smem, st, p->mapX[0], p->mapX[1], p->mapX[2], p->mapX[3], p->mapDY, P, (float*)out);
+  P.part_stride = (long long)g.Co * P.KK * g.Ci;
+  P.partial = nullptr;
+  if (P.splits > 1) {
+    // split-K partial sums go through a workspace and a fixed-order reduction instead of float atomics, so that the
+    // gradient is bit-identical from run to run.  Allocated at the first (eager) run, before any graph capture.
+    if (p->ws == nullptr) MN_CUDA(cudaMalloc(&p->ws, (size_t)P.splits * P.part_stride * sizeof(float)));
+    P.partial = p->ws;
+  }
+  MN_LAUNCH(k1, grid, kConvThreads, smem, st, p->mapX[0], p->mapX[1], p->mapX[2], p->mapX[3], p->mapDY, P, (float*)out);
+  MN_LAUNCH_CHECK();
+  if (P.splits > 1) {
+    MN_TRY(launch_split_reduce(p->ws, P.splits, P.part_stride, (float*)out, st));
+  }
+  return 0;
+}
+
+int launch_split_reduce(const float* part, int splits, long long n, float* dst, cudaStream_t st) {
+  MN_CHECK(n % 4 == 0, "split reduce: %lld elements, not a multiple of 4", n);
+  MN_CHECK((((uintptr_t)part | (uintptr_t)dst) & 15) == 0, "split reduce: workspace / destination not 16-byte aligned");
+  const long long n4 = n / 4;
+  const long long grid = (n4 + 255) / 256 < kNumSMs * 8LL ? (n4 + 255) / 256 : kNumSMs * 8LL;
+  MN_LAUNCH(k_wgrad_reduce, (int)(grid > 0 ? grid : 1), 256, 0, st, (const float4*)part, n4, splits, n4, (float4*)dst);
   MN_LAUNCH_CHECK();
   return 0;
 }

@@ -71,7 +71,7 @@ __global__ void k_gap_bwd(const float* __restrict__ dfeat, T* __restrict__ dz, i
 template <typename T>
 int launch_gap_bwd(const float* dfeat, T* dz, int B, int HW, int C, cudaStream_t st) {
   const long long nvec = (long long)B * HW * (C >> 3);
-  long long grid = (nvec + 255) / 256; if (grid > 148 * 8) grid = 148 * 8;
+  long long grid = (nvec + 255) / 256; if (grid > kNumSMs * 8) grid = kNumSMs * 8;
   MN_LAUNCH(k_gap_bwd<T>, (int)grid, 256, 0, st, dfeat, dz, B, HW, C);
   MN_LAUNCH_CHECK();
   return 0;
@@ -121,7 +121,7 @@ __global__ void __launch_bounds__(256)
 k_small_gemm(const float* __restrict__ A, long long sam, long long sak, const float* __restrict__ Bm,
              long long sbn, long long sbk, float* __restrict__ C, int ldc, int M, int N, int K,
              const float* __restrict__ bias, float* __restrict__ aux, const float* __restrict__ mask,
-             int kchunk) {
+             int kchunk, float* __restrict__ part) {
   pdl_prologue();
   // 64-deep K tiles, the NEXT tile's 16 global loads per thread are in flight while the current one is
   // multiplied: these GEMMs are a few MFLOP, their cost is the chain of load latencies
@@ -131,10 +131,10 @@ k_small_gemm(const float* __restrict__ A, long long sam, long long sak, const fl
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   const int m0 = blockIdx.y * 32, n0 = blockIdx.x * 32;
   float acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
-  // split-K (EPI 0 only): blockIdx.z owns [kbeg, kend) and adds atomically into a zeroed C
+  // split-K (EPI 0 only): blockIdx.z owns [kbeg, kend) and stores its partial C into part[z] (k_split_sum adds them up)
   const int kbeg = blockIdx.z * kchunk;
   const int kend = (kbeg + kchunk < K) ? kbeg + kchunk : K;
-  const bool split = gridDim.z > 1;
+  const bool split = part != nullptr;
   float ra[KT * 32 / 256], rb[KT * 32 / 256];
   auto fetch = [&](int k0) {
 #pragma unroll
@@ -187,7 +187,7 @@ k_small_gemm(const float* __restrict__ A, long long sam, long long sak, const fl
       float v = acc[i][j];
       if (EPI == 0) {
         if (bias != nullptr && blockIdx.z == 0) v += bias[n];
-        if (split) { atomicAdd(C + o, v); continue; }
+        if (split) { part[((long long)blockIdx.z * M + m) * N + n] = v; continue; }
       } else if (EPI == 1) {
         v += bias[n];
         aux[o] = v;
@@ -201,24 +201,50 @@ k_small_gemm(const float* __restrict__ A, long long sam, long long sak, const fl
     }
 }
 
+// C[m*ldc+n] = part[0][m][n] + part[1][m][n] + ... (splits in order)
+__global__ void k_split_sum(const float* __restrict__ part, int splits, int M, int N, float* __restrict__ C, int ldc) {
+  pdl_prologue();
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= (long long)M * N) return;
+  // loads of 8 splits in flight at once, added in split order
+  float s = 0.f;
+  for (int z0 = 0; z0 < splits; z0 += 8) {
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = (z0 + j < splits) ? part[(long long)(z0 + j) * M * N + i] : 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) s += v[j];
+  }
+  C[(i / N) * ldc + i % N] = s;
+}
+
 int launch_small_gemm(int epi, const float* A, long long sam, long long sak, const float* Bm, long long sbn,
                       long long sbk, float* C, int ldc, int M, int N, int K, const float* bias, float* aux,
                       const float* mask, cudaStream_t st) {
   dim3 grid(cdiv(N, 32), cdiv(M, 32), 1);
   int kchunk = K;
-  if (epi == 0 && (int)(grid.x * grid.y) < 74 && K >= 256) {
-    int splits = 148 / (int)(grid.x * grid.y);
+  if (epi == 0 && (int)(grid.x * grid.y) < kNumSMs / 2 && K >= 256) {
+    int splits = kNumSMs / (int)(grid.x * grid.y);
     if (splits > K / 64) splits = K / 64;
     if (splits > 1) {
       kchunk = ((K + splits - 1) / splits + 63) / 64 * 64;
       grid.z = cdiv(K, kchunk);
-      MN_CUDA(cudaMemset2DAsync(C, (size_t)ldc * sizeof(float), 0, (size_t)N * sizeof(float), (size_t)M, st));
     }
   }
-  if (epi == 0) MN_LAUNCH(k_small_gemm<0>, grid, 256, 0, st, A, sam, sak, Bm, sbn, sbk, C, ldc, M, N, K, bias, aux, mask, kchunk);
-  else if (epi == 1) MN_LAUNCH(k_small_gemm<1>, grid, 256, 0, st, A, sam, sak, Bm, sbn, sbk, C, ldc, M, N, K, bias, aux, mask, kchunk);
-  else MN_LAUNCH(k_small_gemm<2>, grid, 256, 0, st, A, sam, sak, Bm, sbn, sbk, C, ldc, M, N, K, bias, aux, mask, kchunk);
+  // split-K: the splits store their partial C in a stream-ordered workspace, k_split_sum adds them in a fixed order
+  float* part = nullptr;
+  if (grid.z > 1) MN_CUDA(cudaMallocAsync((void**)&part, (size_t)grid.z * M * N * sizeof(float), st));
+  if (epi == 0) MN_LAUNCH(k_small_gemm<0>, grid, 256, 0, st, A, sam, sak, Bm, sbn, sbk, C, ldc, M, N, K, bias, aux, mask, kchunk, part);
+  else if (epi == 1) MN_LAUNCH(k_small_gemm<1>, grid, 256, 0, st, A, sam, sak, Bm, sbn, sbk, C, ldc, M, N, K, bias, aux, mask, kchunk, part);
+  else MN_LAUNCH(k_small_gemm<2>, grid, 256, 0, st, A, sam, sak, Bm, sbn, sbk, C, ldc, M, N, K, bias, aux, mask, kchunk, part);
   MN_LAUNCH_CHECK();
+  if (part != nullptr) {
+    const long long n = (long long)M * N;
+    const int g2 = (int)((n + 255) / 256);
+    MN_LAUNCH(k_split_sum, g2, 256, 0, st, part, (int)grid.z, M, N, C, ldc);
+    MN_LAUNCH_CHECK();
+    MN_CUDA(cudaFreeAsync(part, st));
+  }
   return 0;
 }
 

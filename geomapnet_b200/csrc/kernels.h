@@ -1,4 +1,4 @@
-// Internal launcher declarations for the MapNet B200 kernels.
+// Internal launcher declarations for the MapNet kernels.
 #pragma once
 #include "common.cuh"
 #include "bn_fin.cuh"
@@ -60,7 +60,7 @@ int launch_conv_simt_dgrad(const ConvGeom& g, const T* dy, const float* w_dg /*[
 template <typename T>
 int launch_conv_simt_wgrad(const ConvGeom& g, const T* x, const T* dy, float* dw_krsc /*zeroed, accumulated*/, cudaStream_t st);
 
-// ---- conv_tc.cu: tcgen05 / TMA implicit GEMM (bf16 tensor-core path) ------------
+// ---- conv_tc.cu: wgmma / TMA implicit GEMM (bf16 tensor-core path) ---------------
 struct TcConvPlan;   // opaque: tile shapes, tap tables and cached TMA tensor maps of one conv
 // kind 0 fprop (wmat = [Co][KH][KW][Ci]), 1 dgrad (wmat = [Ci][KH][KW][Co]), 2 wgrad (wmat unused)
 int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wmat);
@@ -140,6 +140,9 @@ template <typename T>
 int launch_gap(const T* z, float* feat, int B, int HW, int C, cudaStream_t st);
 template <typename T>
 int launch_gap_bwd(const float* dfeat, T* dz, int B, int HW, int C, cudaStream_t st);
+// dst[i] += part[i] + part[n + i] + ... + part[(splits - 1) * n + i], summed in that order (n % 4 == 0): the
+// deterministic second half of a split-K reduction whose splits STORE their partial results
+int launch_split_reduce(const float* part, int splits, long long n, float* dst, cudaStream_t st);
 int launch_small_gemm(int epi, const float* A, long long sam, long long sak, const float* Bm, long long sbn,
                       long long sbk, float* C, int ldc, int M, int N, int K, const float* bias, float* aux,
                       const float* mask, cudaStream_t st);

@@ -123,7 +123,7 @@ template int launch_pack_weights<bf16>(const WeightDesc*, int, const float*, bf1
 //   tap  t        holds hi(w) in BOTH plane slots of every 8-channel group,
 //   tap  KK + t   holds lo(w) in both,
 // so an activation row [xh xl] (the same 8-interleaved K order) against the two taps gives
-// xh*wh + xl*wh + xh*wl + xl*wl = (xh + xl) * (wh + wl): every hi/lo cross product, fp32-accumulated in TMEM.
+// xh*wh + xl*wh + xh*wl + xl*wl = (xh + xl) * (wh + wl): every hi/lo cross product, fp32-accumulated by the tensor cores.
 //   w_krsc2[co][2*KK][2*Ci]   (fprop; element format fmt_f: 0 fp16, 1 bf16)
 //   w_dg2  [ci][2*KK][2*Co]   (dgrad; element format fmt_g)
 // The stem's patch-matrix row (im2col_k, or 256 for the space-to-depth stem) is treated as ONE tap of that many channels.
@@ -227,7 +227,7 @@ __global__ void __launch_bounds__(256) k_split_tensor(const float* __restrict__ 
 int launch_split_tensor(const float* in, void* out, long long n, int fmt, cudaStream_t st) {
   MN_CHECK(n % 8 == 0, "split_tensor: element count must be a multiple of 8");
   const long long nvec = n / 8;
-  long long grid = (nvec + 255) / 256; if (grid > 148 * 8) grid = 148 * 8; if (grid < 1) grid = 1;
+  long long grid = (nvec + 255) / 256; if (grid > kNumSMs * 8) grid = kNumSMs * 8; if (grid < 1) grid = 1;
   MN_CHECK(fmt == 0, "split_tensor: only fp16 planes are built");
   MN_LAUNCH(k_split_tensor<hsplit>, (int)grid, 256, 0, st, in, (hsplit*)out, nvec);
   MN_LAUNCH_CHECK();
@@ -382,7 +382,7 @@ template <typename TZ>
 int launch_stem_s2d(const float* x_nchw, TZ* S, int B, int H, int W, int Hs, int Wsp, cudaStream_t st) {
   const long long n = (long long)B * Hs * Wsp;
   long long grid = (n + 255) / 256;
-  if (grid > 148LL * 8) grid = 148LL * 8;
+  if (grid > kNumSMs * 8LL) grid = kNumSMs * 8LL;
   MN_LAUNCH(k_stem_s2d<TZ>, (int)grid, 256, 0, st, x_nchw, S, B, H, W, Hs, Wsp);
   MN_LAUNCH_CHECK();
   return 0;

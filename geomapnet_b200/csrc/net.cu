@@ -145,8 +145,8 @@ int Net::init(int max_B_, int H_, int W_, int feat_dim_, int precision_) {
   MN_CHECK(max_B >= 0 && H >= 32 && W >= 32, "create: need max_B>=0 and H,W>=32 (got %d,%d,%d)", max_B, H, W);
   MN_CHECK(precision >= 0 && precision <= 3, "create: bad precision %d", precision);
   // strict tensor-core mode: forward AND backward conv operands are fp16 hi/lo planes.  (bf16 planes for the gradients
-  // would need no scaling, but wgrad multiplies activations by gradients and tcgen05.mma kind::f16 rejects mixed operand
-  // formats -- measured on B200: "illegal instruction", tools/experiments/mma_probe.cu.)
+  // would need no scaling, but wgrad multiplies activations by gradients and wgmma takes A and B in ONE element
+  // format: fp16 x bf16 does not exist.)
   split_fmt_z = 0; split_fmt_g = 0;
   MN_CHECK(feat_dim >= 8 && feat_dim % 4 == 0, "create: feat_dim must be a multiple of 4");
   last_B = 0; last_training = 0; last_has_mask = 0; tc_B = 0; profile_on = 0; prof_pool_used = 0;
@@ -158,12 +158,12 @@ int Net::init(int max_B_, int H_, int W_, int feat_dim_, int precision_) {
     stem_s2d = tc() && (e ? atoi(e) != 0 : 1) && (max_B == 0 || tc_overlapped_view_supported()); }
   Hc = conv_out(H, 7, 2, 3); Wc = conv_out(W, 7, 2, 3);        // (build_table sets them again)
   { const char* e = getenv("MAPNET_STEM_FUSE"); stem_fuse = (e ? atoi(e) != 0 : 1) && (Hc % 2 == 0) && (Wc % 2 == 0); }
-  // measured on B200 (posenet_bs64): finalizing inside the conv's last CTA costs every CTA a fence + counter round trip
-  // and the last one a serial tail -- 4.76 ms/step against 4.57 with the separate (PDL-overlapped) finalize launches: off
+  // finalizing inside the conv's last CTA costs every CTA a fence + counter round trip and the last one a serial tail;
+  // the separate (PDL-overlapped) finalize launches are the default
   { const char* e = getenv("MAPNET_TC_FUSE_FIN"); fuse_fin = (precision == PREC_BF16_TC) && (e ? atoi(e) != 0 : 0); }
   { const char* e = getenv("MAPNET_TC_FUSE_BWD"); fuse_bwd = (precision == PREC_BF16_TC) && (e ? atoi(e) != 0 : 1); }
-  // measured on B200 (posenet_bs64, bf16): the 68 finalize launches of a step cost 0.27 ms of 3.9 (timing experiment with
-  // the launches skipped); with the lazy finalize the consuming element-wise kernels do that work in their prologue
+  // with the lazy finalize the consuming element-wise kernels do the BatchNorm finalize work in their prologue instead
+  // of 68 separate finalize launches per step
   { const char* e = getenv("MAPNET_BN_LAZY_FIN"); lazy_fin = (fuse_stats && !fuse_fin && (e ? atoi(e) != 0 : 1)) ? 1 : 0; }
   stats_target = nullptr; bn_slots = nullptr; bn_slots_bytes = 0;
   { const char* e = getenv("MAPNET_TC_DS_FOLD"); ds_fold = (precision == PREC_BF16_TC) && (e ? atoi(e) != 0 : 1); }
@@ -647,7 +647,7 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
   }
 
   // ---- residual blocks, last to first ----
-  // fuse_bwd (tcgen05 path): the dgrad that PRODUCES a BatchNorm's incoming gradient gates it with that
+  // fuse_bwd (wgmma path): the dgrad that PRODUCES a BatchNorm's incoming gradient gates it with that
   // BN's ReLU and accumulates its backward reductions in the epilogue (conv_tc.cu, EpiBwd), so only a tiny
   // finalize and the apply pass remain.  `pre` = S0 arrives gated with the BN2 sums of this block pending.
   bool pre = bwd_pre;

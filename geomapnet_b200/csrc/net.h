@@ -10,7 +10,7 @@
 namespace mapnet {
 
 // PREC_TC_SPLIT: strict tensor-core mode -- fp32-stored conv outputs, conv operands as split fp16 hi/lo planes (22
-// significant bits), every product formed by 4 tcgen05 MMAs (hi*hi + hi*lo + lo*hi + lo*lo), fp32 accumulation in TMEM
+// significant bits), every product formed by 4 wgmma MMAs (hi*hi + hi*lo + lo*hi + lo*lo), fp32 accumulation
 enum Precision { PREC_FP32 = 0, PREC_BF16_TC = 1, PREC_BF16_SIMT = 2, PREC_TC_SPLIT = 3 };
 
 struct ParamEntry {
@@ -40,7 +40,7 @@ struct BlockL {
   int conv1, conv2, convd;       // indices into convs (convd = -1: identity)
   int Hi, Wi, Ho, Wo, Cin, Cout, stride;
   void *y1, *h, *y2, *yd, *out;  // activation buffers (T)
-  int ds_fold;                   // the downsample dgrad is folded into conv1's dgrad launch (tcgen05 path)
+  int ds_fold;                   // the downsample dgrad is folded into conv1's dgrad launch (wgmma path)
 };
 
 struct Net {
@@ -109,7 +109,7 @@ struct Net {
   int stem_fuse;                 // stem BN backward reductions inside the pool backward (env MAPNET_STEM_FUSE)
   int fuse_fin;                  // BN finalize inside the last CTA of the accumulating conv (env MAPNET_TC_FUSE_FIN)
   int fuse_bwd;                  // BN backward reductions accumulated in the dgrad epilogue (env MAPNET_TC_FUSE_BWD)
-  int fuse_stats;                // BN statistics accumulated in the tcgen05 conv epilogue (env MAPNET_TC_FUSE_STATS)
+  int fuse_stats;                // BN statistics accumulated in the wgmma conv epilogue (env MAPNET_TC_FUSE_STATS)
   int ds_fold;                   // fold each 1x1/s2 downsample dgrad into its block's conv1 dgrad (env MAPNET_TC_DS_FOLD)
   std::vector<ProfRec> prof;
   std::vector<cudaEvent_t> prof_pool; size_t prof_pool_used;

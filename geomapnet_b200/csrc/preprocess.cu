@@ -190,8 +190,8 @@ int mapnet_preprocess_run_ex(mapnet_preprocess_t* h, const void* img_nhwc_u8, in
   for (int c = 0; c < 3; ++c) MN_CHECK(std3[c] > 0.f, "preprocess_run: std[%d] = %f must be positive", c, std3[c]);
   cudaStream_t st = (cudaStream_t)stream;
   const long long t1 = (long long)n * p.Hin * p.Wout, t2 = (long long)n * p.Hout * p.Wout;
-  const int g1 = (int)((t1 + 255) / 256 < 148LL * 16 ? (t1 + 255) / 256 : 148LL * 16);
-  const int g2 = (int)((t2 + 255) / 256 < 148LL * 16 ? (t2 + 255) / 256 : 148LL * 16);
+  const int g1 = (int)((t1 + 255) / 256 < (long long)kNumSMs * 16 ? (t1 + 255) / 256 : (long long)kNumSMs * 16);
+  const int g2 = (int)((t2 + 255) / 256 < (long long)kNumSMs * 16 ? (t2 + 255) / 256 : (long long)kNumSMs * 16);
   MN_LAUNCH(k_pre_resize_h, g1, 256, 0, st, (const uint8_t*)img_nhwc_u8, (const int*)frame_index_dev, p.d_tmp, p.d_bh, p.d_kh,
             p.ksh, (long long)n * p.Hin, p.Hin, p.Win, p.Wout);
   MN_LAUNCH_CHECK();

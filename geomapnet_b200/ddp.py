@@ -15,10 +15,8 @@ gradients back to front.  The library runs it in three parts
 (mapnet_backward_part: head + layer4 = 64 % of the 89.4 MB after ~20 % of the
 backward FLOPs, then layer3, then the rest) and calls back after each one; the
 callback enqueues that slice's allreduce on a side stream, so that only the
-last 5 MB slice would be exposed.  MEASURED (round 2, 2 x B200, mapnet_n32t3,
-CUDA-graph step): 5.340 ms/step with the hook (high-priority NCCL communicator)
-vs 5.355 ms with one blocking allreduce, 5.132 ms on one GPU -- the 0.21 ms of
-NVLink time is NOT hidden.  The backward's kernels leave NCCL's CTAs no room: the
+last 5 MB slice would be exposed.  Whether that hides the NVLink time depends on
+the SMs NCCL gets (not measured on H100).  The backward's kernels leave NCCL's CTAs little room: the
 conv engines hold every SM with a persistent CTA of ~200 KB shared memory, the
 element-wise kernels fill every SM's 2048 thread slots, and programmatic
 dependent launch keeps the next kernel's CTAs queued ahead.  Hiding the

@@ -1,7 +1,7 @@
 """CUDA-graph capture of the training step (common/train.py:339-361).
 
 The step is ~200 short kernel launches; replaying it as two CUDA graphs removes the
-host launch cost and most of the inter-kernel gaps (Blackwell guideline 9).  Graph 1 =
+host launch cost and most of the inter-kernel gaps.  Graph 1 =
 forward + criterion + zero_grad + backward, graph 2 = [clip +] Adam.  Data parallel: the
 whole-buffer allreduce of FlatDataParallel sits between the two graphs (default).  With
 FlatDataParallel(overlap=True) the three slice allreduces issued from the backward-part hook
@@ -11,6 +11,7 @@ gain at 2 GPUs: 0.3 %, see geomapnet_b200/ddp.py).
 
     step = GraphedTrainStep(model, criterion, optimizer, x_example, targ_example)
     loss = step(x, targ)            # x, targ: CUDA tensors (copied into static buffers)
+    step.out                        # the step's prediction (a static buffer, overwritten by the next replay)
 
 Build it before (or without) keeping tensors of an earlier eager step alive: a live `loss` from a step that ran on the
 default stream pins the parameters' AccumulateGrad nodes to that stream and the capture then fails with
@@ -104,6 +105,7 @@ class GraphedTrainStep(object):
 
     def _fwd_bwd(self):
         out = self.model(self.x)
+        self.out = out.detach()
         loss = self.criterion(out, self.t)
         self.learner.zero_grad()
         loss.backward()

@@ -1,10 +1,10 @@
-"""B200-native PoseNet / MapNet behind the reference's nn.Module surface.
+"""H100-native PoseNet / MapNet behind the reference's nn.Module surface.
 
 Host-side mirror of /root/reference/models/posenet.py (PoseNet :36-73, MapNet
 :75-97, filter_hook :28-34): same constructor signatures, same parameter /
 state_dict key names and order (``feature_extractor.conv1.weight`` first; 222
 entries), same initialisation RNG consumption -- but ``forward`` runs the
-hand-written sm_100a kernels through the C ABI (include/mapnet_b200.h) instead
+hand-written sm_90a kernels through the C ABI (include/mapnet_b200.h) instead
 of a torchvision/cuDNN autograd graph, and the backward is one explicit call
 (no autograd inside the trunk).  PyTorch owns all parameter / gradient storage
 so torch.optim, clip_grad_norm_, state_dict, torch.save keep working
@@ -64,7 +64,7 @@ class PoseNet(nn.Module):
                  precision=None, seed=None):
         """feature_extractor: a torchvision-style ResNet-34 object.  It is NEVER run:
         only ``.fc.in_features`` is read and its state_dict harvested as initial trunk
-        weights (scripts/train.py:76-78).  precision: 'bf16' (tcgen05 tensor cores, bf16 operands,
+        weights (scripts/train.py:76-78).  precision: 'bf16' (wgmma tensor cores, bf16 operands,
         default), 'tc_split' (the same engines on fp16 hi/lo operand planes: 1e-4 parity on tensor cores),
         'fp32' (strict-parity CUDA-core path) or 'bf16_simt' (cross-check)."""
         super(PoseNet, self).__init__()
@@ -159,7 +159,7 @@ class PoseNet(nn.Module):
 
     def _pview(self, flat, name, off, n, shape):
         """The entry's tensor as a view of a flat buffer.  Conv weights (all but the stem) are stored in the order the
-        tcgen05 engines read and accumulate them, [Co][KH][KW][Ci] (mapnet_param_layout == 1): the view has the
+        wgmma engines read and accumulate them, [Co][KH][KW][Ci] (mapnet_param_layout == 1): the view has the
         reference's [Co,Ci,KH,KW] shape with torch.channels_last strides, so indexing, state_dict(), load_state_dict()
         and optimizers see the same tensor as in the reference while no kernel ever transposes a weight or a gradient."""
         if name in self._krsc:

@@ -1,4 +1,4 @@
-/* mapnet_b200.h -- C ABI of the B200-native MapNet/PoseNet training hot path.
+/* mapnet_b200.h -- C ABI of the H100-native MapNet/PoseNet training hot path.
  *
  * Drop-in boundary (SURVEY.md section 8b).  The reference (NVlabs/geomapnet) is pure
  * Python on PyTorch: it has NO native FFI for this path, so these entry points
@@ -37,9 +37,9 @@ typedef struct mapnet_trunk mapnet_trunk_t;
 
 /* precision of the conv engines / stored activations */
 #define MAPNET_PREC_FP32 0      /* fp32 CUDA-core implicit GEMM: strict 1e-4 parity mode            */
-#define MAPNET_PREC_BF16 1      /* tcgen05 tensor-core implicit GEMM, bf16 operands, fp32 accumulate */
+#define MAPNET_PREC_BF16 1      /* wgmma tensor-core implicit GEMM, bf16 operands, fp32 accumulate */
 #define MAPNET_PREC_BF16_SIMT 2 /* bf16 storage + CUDA-core fp32 math: cross-check of mode 1         */
-#define MAPNET_PREC_TC_SPLIT 3  /* tcgen05 strict mode: fp32 conv outputs, conv operands as split fp16 hi/lo planes,\
+#define MAPNET_PREC_TC_SPLIT 3  /* wgmma strict mode: fp32 conv outputs, conv operands as split fp16 hi/lo planes,\
                                    4 MMAs per product, fp32 accumulate -- meets the 1e-4 parity bar on tensor cores */
 
 /* criterion modes (common/criterion.py) */
@@ -63,7 +63,7 @@ int mapnet_param_count(mapnet_trunk_t* h);
 int mapnet_param_info(mapnet_trunk_t* h, int i, char* host_name, int name_cap, int* host_kind, int* host_ndim,
                       int64_t* host_shape4, int64_t* host_offset);
 /* Element order of entry i inside its flat buffer.  0: torch's contiguous order of the entry's shape.  1: a conv weight
- * of shape [Co,Ci,KH,KW] stored as [Co][KH][KW][Ci] -- the K-major order the tcgen05 engines read (fprop operand) and
+ * of shape [Co,Ci,KH,KW] stored as [Co][KH][KW][Ci] -- the K-major order the wgmma engines read (fprop operand) and
  * accumulate (wgrad), so neither direction needs a transposing pass per step.  To PyTorch that memory is the same
  * [Co,Ci,KH,KW] tensor in torch.channels_last strides: flat[off:off+n].view(Co,KH,KW,Ci).permute(0,3,1,2) -- logical
  * indexing, state_dict()/load_state_dict() and the reference's optimizer code are unaffected.  Every conv except the stem
@@ -174,7 +174,7 @@ int mapnet_test_plan_describe(int kind, int B, int Hi, int Wi, int Ci, int Co, i
 int mapnet_test_dgrad_shortcut(int B, int Hi, int Wi, int Ci, int Co, const void* dy1, const void* dy2,
                                const void* w1_dg, const void* w2_dg, void* dx, void* stream);
 
-/* one tcgen05 conv launch with the epilogue the training step fuses into it (bf16 mode; tensors bf16 NHWC):
+/* one wgmma conv launch with the epilogue the training step fuses into it (bf16 mode; tensors bf16 NHWC):
  * kind 0 fprop -> out + the BatchNorm batch statistics (sum, sum of squares per output channel) of the stored values;
  * kind 1 dgrad -> out = the gradient gated by the consumer BatchNorm's ReLU (+ residual) and that BatchNorm's backward
  * reductions (sum g, sum g*y [, sum g*yd]).  host_sums: [3][C] doubles.  Replaces cuDNN BN forward-training statistics

@@ -4,7 +4,7 @@ TEST INFRASTRUCTURE.  Usage:  python -m oracle.make_goldens [--full]
 
 Every golden holds the outputs of the reference's own modules
 (models/posenet.py, common/criterion.py, common/pose_utils.py, executed from
-/root/reference through oracle.ref_loader) on seed-generated inputs and
+the reference tree through oracle.ref_loader) on seed-generated inputs and
 seed-generated weights (oracle.weights).  Inputs/weights are NOT stored for the
 large configs -- they are regenerated from the seed on the test side; a
 checksum of each guards against generator drift.
@@ -119,8 +119,10 @@ def run_step_config(name, cfg, seed=7):
     for i, n in enumerate(FULL_GRAD_NAMES):
         t = by_name[n].detach().flatten()
         out["grad_full_%d" % i] = t[::sample_stride(t.numel())].numpy().copy()
-    if x.numel() <= 4 * 6 * 3 * 64 * 64:
+    if x.numel() <= 6 * 3 * 64 * 64:
         out["x"] = x.numpy()
+    elif x.numel() <= 4 * 6 * 3 * 64 * 64:       # keeps the file under 1 MB; the tail is covered by x_checksum
+        out["x_head"] = x.flatten()[:1 << 16].numpy().copy()
     np.savez_compressed(os.path.join(GOLD, "step_%s.npz" % name), **out)
     print("golden step_%s: loss=%.6f  ref time %.2fs" % (name, loss, dt), flush=True)
 
@@ -285,6 +287,138 @@ def run_keys():
     print("golden keys: %d state entries" % len(net.state_dict()), flush=True)
 
 
+LIVE_SAMPLE = 256       # entries per gradient tensor kept by run_live (fixed stride)
+INIT_SAMPLE = 64        # entries per initial state tensor kept by run_live (fixed stride)
+
+
+def _grad_samples(prefix, grads, out):
+    names = [k.replace("mapnet.", "", 1) for k in grads]
+    out[prefix + "grad_names"] = np.array(names)
+    out[prefix + "grad_norm"] = np.array([float(v.double().norm()) for v in grads.values()])
+    out[prefix + "grad_stride"] = np.array([max(1, v.numel() // LIVE_SAMPLE) for v in grads.values()], dtype=np.int64)
+    for i, v in enumerate(grads.values()):
+        out[prefix + "grad_%d" % i] = v.detach().flatten()[::max(1, v.numel() // LIVE_SAMPLE)].numpy().copy()
+
+
+def run_live():
+    """tests/golden/live_reference.npz: what the tests that once executed the reference live compared against --
+    training steps of the reference modules, its NaN-filter hook, the one-frame plumbing config, the PoseGraph
+    classes and numpy helpers, MF.get_indices, the reference PoseNet's seeded initialisation, and the reference
+    module's state_dict / criterion layout."""
+    import torchvision
+    from . import pgo_oracle as P
+    ns = ref_loader.load()
+    out = {}
+    for kind, cfg in (("posenet", dict(kind="posenet", N=2, H=64, W=64)),
+                      ("online", dict(kind="online", N=2, T=4, H=64, W=64))):
+        st = weights.make_state(3)
+        x, targ = weights.make_inputs(cfg, 3)
+        model = ref_loader.build_reference_model(st, "posenet" if kind == "posenet" else "mapnet")
+        model.train()
+        if kind == "posenet":
+            crit = ns.PoseNetCriterion(sax=0.0, saq=-3.0, learn_beta=True)
+        else:
+            crit = ns.MapNetOnlineCriterion(sax=0.0, saq=-3.0, srx=0.0, srq=-3.0, learn_beta=True, learn_gamma=True)
+        loss, o, grads, _ = ref_loader.reference_step(model, crit, x, targ)
+        out["step_%s_loss" % kind] = np.float64(loss)
+        out["step_%s_out" % kind] = o.numpy()
+        _grad_samples("step_%s_" % kind, grads, out)
+    # NaN filter hook (degenerate fc_wpqr = 0)
+    st = weights.make_state(3)
+    st["fc_wpqr.weight"] = torch.zeros_like(st["fc_wpqr.weight"])
+    st["fc_wpqr.bias"] = torch.zeros_like(st["fc_wpqr.bias"])
+    cfg = dict(kind="online", N=2, T=4, H=64, W=64)
+    x, targ = weights.make_inputs(cfg, 3)
+    model = ref_loader.build_reference_model(st, "mapnet", filter_nans=True)
+    model.train()
+    crit = ns.MapNetOnlineCriterion(sax=0.0, saq=-3.0, srx=0.0, srq=-3.0, learn_beta=True, learn_gamma=True)
+    import warnings
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore")
+        _, _, grads, _ = ref_loader.reference_step(model, crit, x, targ, do_step=False)
+    _grad_samples("nanfilter_", grads, out)
+    out["nanfilter_all_finite"] = np.array([bool(torch.isfinite(v).all()) for v in grads.values()])
+    out["nanfilter_fc_wpqr_weight"] = grads["mapnet.fc_wpqr.weight"].numpy()
+    # BASELINE configs[0]: one 256x256 frame
+    st = weights.make_state(7)
+    g = torch.Generator().manual_seed(7)
+    x = torch.randn(1, 3, 256, 256, generator=g)
+    targ = torch.randn(1, 6, generator=g)
+    model = ref_loader.build_reference_model(st, "posenet")
+    model.train()
+    loss, o, _, _ = ref_loader.reference_step(model, ns.PoseNetCriterion(sax=0.0, saq=-3.0, learn_beta=True), x, targ,
+                                              do_step=False)
+    out["config0_loss"] = np.float64(loss)
+    out["config0_out"] = o.numpy()
+    # PoseGraph classes and numpy helpers (common/pose_utils.py:306-804)
+    pns = P.load_reference()
+    rng = np.random.default_rng(11)
+    for ci, (N, fc) in enumerate([(3, False), (6, False), (5, True)]):
+        t = rng.normal(size=(N, 3)).cumsum(0) * 0.3
+        v = rng.normal(size=(N, 3)) * 0.4
+        q = np.stack([np.concatenate(([np.cos(np.linalg.norm(a))], np.sinc(np.linalg.norm(a) / np.pi) * a)) for a in v])
+        gt = np.hstack((t, q))
+        pred = gt + rng.normal(size=gt.shape) * 0.05
+        E = P.edges(N, fc)
+        vos = np.stack([np.concatenate((P.rotate_vector(gt[j, :3] - gt[i, :3], P.qinverse(gt[i, 3:])),
+                                        P.qmult(P.qinverse(gt[i, 3:]), gt[j, 3:]))) for i, j in E])
+        out["pgo%d_pred" % ci], out["pgo%d_vos" % ci], out["pgo%d_fc" % ci] = pred, vos, np.bool_(fc)
+        out["pgo%d_out" % ci] = pns["optimize_poses"](pred_poses=pred.copy(), vos=vos.copy(), fc_vos=fc, sax=1.5, saq=0.3,
+                                                     srx=0.7, srq=0.1)
+    for name in ("dpq_q", "dpsq_q", "dpsq_p", "dqstq_t", "m_rot"):
+        xx = rng.normal(size=(4, 1))
+        out["pgohelper_%s_in" % name], out["pgohelper_%s_out" % name] = xx, pns[name](xx)
+    # MF.get_indices (dataset_loaders/composite.py:60-75) on the cases tests/test_preprocess_host.py walks
+    get_indices = _reference_mf_get_indices()
+    from types import SimpleNamespace
+    rows = []
+    for steps, skip, L in [(3, 10, 1000), (5, 10, 47), (2, 1, 5), (4, 3, 30), (3, 10, 12)]:
+        for nodup in (False, True):
+            me = SimpleNamespace(variable_skip=False, skip=skip, steps=steps, no_duplicates=nodup, dset=range(L))
+            n = (L - (steps - 1) * skip) if nodup else L
+            for index in list(range(0, min(n, 40))) + [max(n - 1, 0)]:
+                rows.append([steps, skip, L, int(nodup), index] + list(get_indices(me, index)) + [-1] * (5 - steps))
+    out["mf_cases"] = np.array(rows, dtype=np.int64)
+    me = SimpleNamespace(variable_skip=True, skip=7, steps=5, no_duplicates=False, dset=range(500))
+    np.random.seed(3)
+    out["mf_variable_skip"] = np.asarray(get_indices(me, 250), dtype=np.int64)
+    # initialisation: the reference PoseNet's state_dict right after torch.manual_seed(11), without and with pretrained
+    # (models/posenet.py:50-66): per-tensor sums and a fixed-stride sample of the exact values
+    for pretrained in (False, True):
+        torch.manual_seed(11)
+        r = ns.PoseNet(torchvision.models.resnet34(weights=None), droprate=0.0, pretrained=pretrained)
+        sd = r.state_dict()
+        tag = "init_pre%d_" % int(pretrained)
+        out[tag + "keys"] = np.array(list(sd.keys()))
+        out[tag + "sum"] = np.array([float(v.double().sum()) for v in sd.values()])
+        out[tag + "stride"] = np.array([max(1, v.numel() // INIT_SAMPLE) for v in sd.values()], dtype=np.int64)
+        for i, v in enumerate(sd.values()):
+            out[tag + "%d" % i] = v.flatten()[::max(1, v.numel() // INIT_SAMPLE)].numpy().copy()
+    # state_dict layout of the reference MapNet and its criterion (strict load_state_dict checks names and shapes)
+    net = ns.PoseNet(torchvision.models.resnet34(weights=None), droprate=0.0, pretrained=False)
+    mp = ns.MapNet(mapnet=net)
+    out["mapnet_state_keys"] = np.array(list(mp.state_dict().keys()))
+    out["mapnet_state_shapes"] = np.array([repr(tuple(v.shape)) for v in mp.state_dict().values()])
+    rc = ns.MapNetCriterion(sax=1.0, saq=1.0, srx=1.0, srq=1.0, learn_beta=True, learn_gamma=True)
+    out["mapnet_criterion_state_keys"] = np.array(list(rc.state_dict().keys()))
+    np.savez_compressed(os.path.join(GOLD, "live_reference.npz"), **out)
+    print("golden live_reference: %d arrays" % len(out), flush=True)
+
+
+def _reference_mf_get_indices():
+    """MF.get_indices executed from the reference's own source text with the Python-2 integer divisions spelled `//`
+    (the module itself imports py2-only dataset code)."""
+    path = os.path.join(ref_loader.REF_ROOT, "dataset_loaders", "composite.py")
+    src = open(path).read().split("\n")
+    start = next(i for i, l in enumerate(src) if l.strip().startswith("def get_indices"))
+    end = next(i for i in range(start + 1, len(src)) if src[i].strip().startswith("def "))
+    body = "\n".join(l[2:] for l in src[start:end])
+    body = body.replace("len(offsets) / 2", "len(offsets) // 2").replace("self.steps/2", "self.steps//2").replace("np.int)", "int)")
+    ns = {"np": np}
+    exec(body, ns)
+    return ns["get_indices"]
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--full", action="store_true", help="also the BASELINE full-size configs (minutes)")
@@ -301,6 +435,9 @@ def main():
         return
     if a.only == "pgo":
         run_pgo()
+        return
+    if a.only == "live":
+        run_live()
         return
     if a.only is None:
         run_keys()

@@ -249,7 +249,7 @@ def _conv(x, w, stride, pad, emulate):
         y = F.conv2d(_RoundFwd.apply(x, _round_f16x2), _RoundFwd.apply(w, _round_f16x2), None, stride, pad)
         return _GradRound.apply(y)
     # operands rounded to bf16 (x already is when it is a stored activation);
-    # products exact in fp32, fp32 accumulate -- what tcgen05 kind::f16 does.
+    # products exact in fp32, fp32 accumulate -- what wgmma does.
     y = F.conv2d(_rb(x, emulate), _RoundFwd.apply(w, _round_bf16) if emulate == "bf16" else w, None, stride, pad)
     return _rb(y, emulate)      # conv output is stored (bf16) before BN reads it
 

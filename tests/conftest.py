@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "slow: takes more than a few seconds on CPU")
 
 
@@ -19,7 +19,7 @@ def _gpu_unavailable_reason():
     try:
         import torch
         if not torch.cuda.is_available():
-            return "no CUDA device on this host (gpu-marked tests run on the B200 box)"
+            return "no CUDA device on this host (gpu-marked tests need an H100)"
     except Exception as e:          # pragma: no cover
         return "torch unavailable: %r" % (e,)
     return None                     # GPU present: nothing is skipped, a missing library fails loudly

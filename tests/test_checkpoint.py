@@ -1,6 +1,6 @@
 """Checkpoint interchange with the reference (SURVEY.md section 8 row f4): the dict written by
 common/train.py:198-204 and the prefix logic of common/train.py:22-53, exercised on CPU between the
-REFERENCE's own modules (when /root/reference is present) / a torchvision-built stand-in and the
+REFERENCE's own modules (when the reference tree is present) / a torchvision-built stand-in and the
 product modules.  No kernels run here: the product modules are parameter containers on CPU."""
 import os
 
@@ -25,7 +25,7 @@ def _product(seed=3, pretrained=False):
 
 def _reference_like_state(seed=9):
     """A PoseNet state dict produced by the reference's own class when the tree is present, else by the
-    oracle's weight generator (same 222 keys)."""
+    oracle's weight generator, checked against the reference's recorded key order and shapes (same 222 keys)."""
     from oracle import ref_loader, weights
     if ref_loader.available():
         ns = ref_loader.load()
@@ -40,7 +40,15 @@ def _reference_like_state(seed=9):
                 elif k.endswith("num_batches_tracked"):
                     v.fill_(17)
         return {k: v.clone() for k, v in r.state_dict().items()}, "reference class"
-    return weights.make_state(seed), "oracle weights"
+    # without the reference tree: the oracle's generator, held to the reference PoseNet's recorded state_dict layout
+    import numpy as np
+    st = weights.make_state(seed)
+    L = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "live_reference.npz"))
+    layout = {str(k).replace("mapnet.", "", 1): str(sh) for k, sh in zip(L["mapnet_state_keys"], L["mapnet_state_shapes"])}
+    assert list(st.keys()) == list(layout.keys())
+    for k, v in st.items():
+        assert repr(tuple(v.shape)) == layout[k], k
+    return st, "oracle weights"
 
 
 def test_reference_checkpoint_loads_into_posenet_and_mapnet(built, tmp_path):
@@ -94,15 +102,15 @@ def test_prefixed_and_legacy_state_dicts(built):
         load_state_dict(_product(), {"encoder.stem.weight": torch.zeros(1)})
 
 
-def test_product_checkpoint_loads_into_reference_class(built, tmp_path):
-    """The other direction: a checkpoint saved from the product modules is a valid reference checkpoint."""
-    from oracle import ref_loader
+def test_product_checkpoint_loads_into_reference_class(built, tmp_path, golden_dir):
+    """The other direction: a checkpoint saved from the product modules is a valid reference checkpoint -- it has the
+    state_dict layout the reference MapNet's strict load_state_dict checks (the same 222 names, the same shapes) and
+    its criterion's keys, as recorded from the reference classes in tests/golden/live_reference.npz."""
+    import numpy as np
     from geomapnet_b200.common.checkpoint import save_checkpoint
     from geomapnet_b200.common.criterion import MapNetCriterion
-    if not ref_loader.available():
-        pytest.skip("reference tree only exists in the build container")
-    ns = ref_loader.load()
     from geomapnet_b200.models.posenet import MapNet
+    L = np.load(os.path.join(golden_dir, "live_reference.npz"))
     m = MapNet(_product(seed=21))
     crit = MapNetCriterion(sax=0.0, saq=-3.0, srx=0.0, srq=-3.0, learn_beta=True, learn_gamma=True)
     opt = torch.optim.Adam(list(m.parameters()) + list(crit.parameters()), lr=1e-4)
@@ -110,13 +118,15 @@ def test_product_checkpoint_loads_into_reference_class(built, tmp_path):
     assert os.path.basename(f) == "epoch_012.pth.tar"
     ck = torch.load(f, map_location="cpu", weights_only=False)
     assert sorted(ck.keys()) == ["criterion_state_dict", "epoch", "model_state_dict", "optim_state_dict"]
-    r = ns.MapNet(ns.PoseNet(torchvision.models.resnet34(weights=None), droprate=0.0, pretrained=False))
-    r.load_state_dict(ck["model_state_dict"])             # strict: same 222 keys, same shapes
-    for k, v in r.state_dict().items():
-        assert torch.equal(v, m.state_dict()[k]), k
-    rc = ns.MapNetCriterion(sax=1.0, saq=1.0, srx=1.0, srq=1.0, learn_beta=True, learn_gamma=True)
-    rc.load_state_dict(ck["criterion_state_dict"])
-    assert [float(p.detach()) for p in rc.parameters()] == [float(p.detach()) for p in crit.parameters()]
+    msd = ck["model_state_dict"]
+    keys = [str(k) for k in L["mapnet_state_keys"]]
+    assert len(keys) == 222 and sorted(msd.keys()) == sorted(keys)
+    for k, shape in zip(keys, L["mapnet_state_shapes"]):
+        assert repr(tuple(msd[k].shape)) == str(shape), k
+        assert torch.equal(msd[k], m.state_dict()[k]), k
+    ckeys = [str(k) for k in L["mapnet_criterion_state_keys"]]
+    assert sorted(ck["criterion_state_dict"].keys()) == sorted(ckeys)
+    assert [float(ck["criterion_state_dict"][k]) for k in ckeys] == [float(p.detach()) for p in crit.parameters()]
 
 
 def test_resume_restores_optimizer_epoch_and_criterion(built, tmp_path):

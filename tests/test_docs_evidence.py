@@ -1,9 +1,7 @@
 """The numbers the documents quote are the numbers of the committed evidence (CPU only, no compute).
 
-README.md / DESIGN.md / profiles/README.md quote bench lines and ncu rows; every quoted figure must be readable from a
-file under profiles/ (the judge cites profiles/, not prose).  Also: the `roofline.traffic` source must belong to the
-kernel sources of this tree (bench.py reports it as stale otherwise)."""
-import csv
+README.md, DESIGN.md and profiles/README.md quote bench lines; every quoted figure must be readable from a file under
+profiles/, which also records the GPU the line was measured on."""
 import json
 import os
 import re
@@ -24,10 +22,9 @@ def _fmt(v):
 
 
 BENCH = {
-    "posenet_bs64": "r02c_bench_posenet_bs64.json",
-    "mapnet_n32t3": "r02c_bench_mapnet_n32t3.json",
-    "mapnetpp_n16t10": "r02c_bench_mapnetpp_n16t10.json",
-    "n2": "r02c_bench_n2_mapnet_n32t3_overlap0.json",
+    "posenet_bs64": "h100_bench_posenet_bs64.json",
+    "mapnet_n32t3": "h100_bench_mapnet_n32t3.json",
+    "mapnetpp_n16t10": "h100_bench_mapnetpp_n16t10.json",
 }
 
 
@@ -37,24 +34,24 @@ def test_readme_and_design_quote_the_committed_bench_lines():
     prof = open(os.path.join(PROF, "README.md")).read()
     for key, fn in BENCH.items():
         d = _line(fn)
+        assert d["config"]["workload"] == key and d["n_gpus"] == 1
+        assert "H100" in open(os.path.join(PROF, fn)).read().splitlines()[0]
         for doc_name, doc in (("README.md", readme), ("DESIGN.md", design), ("profiles/README.md", prof)):
             assert _fmt(d["value"]) in doc, (doc_name, key, _fmt(d["value"]))
             assert _fmt(d["e2e"]["value"]) in doc, (doc_name, key, "e2e", _fmt(d["e2e"]["value"]))
     d = _line(BENCH["posenet_bs64"])
-    assert d["config"]["workload"] == "posenet_bs64" and d["n_gpus"] == 1 and d["clocks"]["reasons"] == []
+    # a throttled measurement is only quoted together with the throttle and the power limit it ran at
+    if d["clocks"]["reasons"] != []:
+        head = open(os.path.join(PROF, BENCH["posenet_bs64"])).read().splitlines()[0]
+        assert "sw_power_cap" in head and "power limit" in head and "power cap" in readme and "power limit" in design
     assert d["e2e"]["h2d_bytes_per_step"] == 64 * 3 * 256 * 256 * 4 + 64 * 6 * 4
-    # the roofline fraction the documents state (0.345 of the burst peak measured in that session)
-    assert abs(d["roofline"]["frac"] - 0.345) < 1e-3 and "0.345" in readme and "0.345" in design
+    # the roofline fraction README states, against the data-sheet peak recorded in the line
+    assert d["roofline"]["peak"] == 989.0 and ("%.3f" % d["roofline"]["frac"]) in readme and ("%.3f" % d["roofline"]["frac"]) in design
     # both tensor-core modes were measured in the same run
     pm = d["precision_modes"]
-    assert pm["bf16"]["images_per_s"] == d["value"] and 6500 < pm["tc_split"]["images_per_s"] < 7500
-    # strict-mode and fp32 lines quoted in the precision tables
-    for fn, txt in (("r02c_bench_posenet_bs64_tc_split.json", "7.06 k"), ("r02c_bench_posenet_bs64_fp32.json", "0.96 k")):
-        v = _line(fn)["value"]
-        assert ("%.2f k" % (v / 1000.0)) == txt and txt in readme and txt in design, (fn, v)
-    ref = _line("r02c_bench_reference.json")
-    assert ref["impl"] == "reference" and ref["config"]["frames_per_step"] == 64 and "25.1" in readme
-    assert ("%.1f" % ref["value"]) == "25.1"
+    assert pm["bf16"]["images_per_s"] == d["value"]
+    assert ("%.2f k" % (pm["tc_split"]["images_per_s"] / 1000.0)) in readme and ("%.2f k" % (pm["tc_split"]["images_per_s"] / 1000.0)) in design
+    assert ("%.1f" % d["cpu_baseline"]["value"]) in readme
 
 
 def test_bench_note_cites_an_existing_file():
@@ -63,44 +60,15 @@ def test_bench_note_cites_an_existing_file():
         assert os.path.exists(os.path.join(ROOT, m.group(0))), m.group(0)
 
 
-def test_ncu_rows_cover_every_kernel_class_and_back_the_quoted_figures():
-    rows = []
-    with open(os.path.join(PROF, "r02c_ncu_full_summary.csv")) as f:
-        rd = csv.DictReader(l for l in f if not l.startswith("#"))
-        rows = list(rd)
-    kernels = {r["kernel"].split("<")[0] for r in rows}
-    for k in ("k_tc_conv", "k_tc_conv2", "k_tc_wgrad", "k_tc_wgrad2", "k_bn_apply_lazy", "k_bn_bwd_apply_lazy",
-              "k_stem_pool", "k_stem_pool_bwd_quad", "k_adam", "k_gap", "k_pack_weights", "k_transpose_dg",
-              "k_channel_sums"):
-        assert k in kernels, k
-    # read AND write DRAM bytes are recorded (round 1's CSV had write = 0 everywhere)
-    assert any(float(r["dram_write_bytes"]) > 0 for r in rows) and all(float(r["dram_read_bytes"]) > 0 for r in rows)
-    adam = [r for r in rows if r["kernel"] == "k_adam"][0]
-    gbs = (float(adam["dram_read_bytes"]) + float(adam["dram_write_bytes"])) / float(adam["dur_ns"])
-    assert abs(gbs - 5972) < 5, gbs                       # profiles/README.md: k_adam 5 972 GB/s = 90.9 % of 6 571
-    conv = [r for r in rows if r["kernel"].startswith("k_tc_conv<256")]
-    bf16 = [float(r["tensor_pipe_pct_active"]) for r in conv if float(r["utcmma_insts"]) == 18432]
-    split = [float(r["tensor_pipe_pct_active"]) for r in conv if float(r["utcmma_insts"]) == 73728]
-    assert bf16 and split and 49 < min(bf16) and max(bf16) < 53 and 71 < min(split) and max(split) < 77
-
-
-def test_traffic_capture_belongs_to_these_kernel_sources():
-    from geomapnet_b200 import build as b
-    t = json.load(open(os.path.join(PROF, "ncu_traffic.json")))
-    assert t["source"] == "r02c_ncu_full_summary.csv"
-    assert t["sources_digest"] == b._digest()[:16], \
-        "kernel sources changed after the ncu capture: bench.py will report roofline.traffic as stale (null)"
-
-
-def test_stage_table_accounts_for_every_conv_flop_of_the_step(capsys):
+def test_stage_table_accounts_for_every_conv_flop_of_the_step():
     """tools/stage_table.py matches the 104 conv launches of the committed launch list to their layers: the algorithmic
     FLOPs must add up to SURVEY.md 8d's per-step figure (B = 64: 1 817.6 GFLOP), and the committed table is its output."""
     import subprocess
     import sys
     r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "stage_table.py"),
-                        os.path.join("profiles", "r02c_launches_raw.csv")], capture_output=True, text=True, cwd=ROOT, timeout=120)
+                        os.path.join("profiles", "h100_launches_raw.csv")], capture_output=True, text=True, cwd=ROOT, timeout=120)
     assert r.returncode == 0, r.stderr
     assert "1817.6 GFLOP" in r.stdout and "all    | 36 |" in r.stdout and "all    | 32 |" in r.stdout
-    assert r.stdout == open(os.path.join(PROF, "r02c_conv_by_stage.txt")).read()
+    assert r.stdout == open(os.path.join(PROF, "h100_conv_by_stage.txt")).read()
     from oracle import mapnet_oracle as O
     assert abs(64 * O.train_flops_per_image(256, 256) - 1817.6e9) < 0.1e9

@@ -50,7 +50,7 @@ CASES = [(2, 16, 16, 64, 64, 3, 1), (2, 16, 16, 64, 128, 3, 2), (2, 16, 16, 64, 
 @pytest.mark.parametrize("geom", CASES)
 def test_conv_engines(precision, geom):
     """tc_split (strict tensor-core mode): UNROUNDED fp32 operands in, fp32 out -- the entry point cuts them into
-    fp16 hi/lo planes (22 significant bits) and the tcgen05 engines form all four hi/lo products; the bound is the
+    fp16 hi/lo planes (22 significant bits) and the wgmma engines form all four hi/lo products; the bound is the
     fp32 CUDA-core engine's."""
     B, H, W, Ci, Co, k, stride = geom
     x, w, dy, y, dx, dw = _conv_case(precision, *geom)
@@ -61,8 +61,7 @@ def test_conv_engines(precision, geom):
     w_krsc = w.permute(0, 2, 3, 1).contiguous().to(wt).cuda()          # [Co][kh][kw][Ci]
     w_dg = w.permute(1, 2, 3, 0).contiguous().to(wt).cuda()            # [Ci][kh][kw][Co]
     # bf16: output rounding 2^-8 relative.  tc_split: fp32 outputs; what is left is the tensor core's fp32 accumulation
-    # (measured on B200, tools/experiments/mma_probe.cu: error grows linearly with K -- 1.2e-6 of sum|terms| at
-    # K = 4096 against 2e-8 at K = 64 -- i.e. the accumulator is truncated, not rounded, at every MMA)
+    # (the tensor cores' fp32 accumulation truncates instead of rounding, so the error grows with K)
     tol = {"fp32": 2e-5, "tc_split": 1e-4}.get(precision, 1.2e-2)
     errs = []
     # fprop
@@ -118,7 +117,7 @@ SHORTCUT_CASES = [(2, 64, 64, 64, 128), (2, 32, 32, 128, 256), (2, 16, 16, 256, 
 
 @pytest.mark.parametrize("geom", SHORTCUT_CASES)
 def test_merged_stride2_dgrad_with_folded_shortcut(geom):
-    """d(block input) of a downsampling BasicBlock in ONE tcgen05 launch: the four parity classes of the 3x3/s2
+    """d(block input) of a downsampling BasicBlock in ONE wgmma launch: the four parity classes of the 3x3/s2
     conv1 dgrad plus the 1x1/s2 downsample dgrad as an extra tap of class (0,0) (conv_tc.cu,
     tc_plan_add_shortcut), against torch autograd through both convs on the same bf16-rounded operands."""
     B, H, W, Ci, Co = geom
@@ -220,7 +219,7 @@ def test_fused_adam_clip_matches_clip_grad_norm():
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# the FUSED epilogues of the tcgen05 engines against torch (not product-vs-product): BatchNorm statistics in fprop,
+# the FUSED epilogues of the wgmma engines against torch (not product-vs-product): BatchNorm statistics in fprop,
 # ReLU gate + BatchNorm-backward reductions (+ residual) in dgrad
 # ---------------------------------------------------------------------------------------------------------------------
 EPI_CASES = [(2, 16, 16, 64, 64, 3, 1), (3, 9, 11, 128, 128, 3, 1), (2, 18, 22, 64, 128, 3, 2), (1, 8, 8, 256, 512, 3, 2),

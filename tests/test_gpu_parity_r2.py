@@ -154,11 +154,11 @@ def _vs_emulated(emulate, precision, name):
 @pytest.mark.parametrize("name", ["posenet_b8_256", "posenet_b64_256", "mapnet_n32t3_256", "online_n16t10_256"])
 def test_step_bf16_matches_bf16_emulating_oracle(name):
     """Identical rounding points on both sides (bf16 operands, bf16-stored activations and gradients, fp32
-    accumulation / BN / loss).  Measured on B200 (round 2): the product sits at loss 5e-4 .. 7e-3, pose 2.7e-2 .. 3.4e-2
-    of the emulating oracle -- only ~2x closer than to the fp32 reference (pose 4e-2 .. 7e-2).  Rounding at the same
+    accumulation / BN / loss).  The product sits only ~2x closer to the emulating oracle than to the fp32 reference.
+    Rounding at the same
     POINTS does not make two bf16 implementations agree: a different fp32 summation order moves individual bf16
     roundings / ReLU masks, and 36 conv+BN layers at random initialisation amplify that to the percent level.  The
-    independent CUDA-core bf16 engine differs from the tcgen05 one by the same amount
+    independent CUDA-core bf16 engine differs from the wgmma one by the same amount
     (test_tensor_core_path_matches_cuda_core_path_on_bf16: pose 2.9e-2).  So these bounds (~2x measured) document the
     bf16 noise floor; kernel CORRECTNESS is carried by the per-conv / per-epilogue unit tests (bit-level operands
     against torch) and by the strict tensor-core mode, which meets 1e-4.  The tail of the backward pass (head, last

@@ -1,6 +1,6 @@
 """GPU run of the input-pipeline kernels (geomapnet_b200/csrc/preprocess.cu, SURVEY.md section 8 row f2) against Pillow /
 torchvision, bit for bit: Resize(256) -> [ColorJitter] -> ToTensor -> Normalize (scripts/train.py:119-128) and the
-MF tuple gather (dataset_loaders/composite.py:60-97).  First ran on a B200 in round 2 (4 passed); no longer opt-in."""
+MF tuple gather (dataset_loaders/composite.py:60-97)."""
 import numpy as np
 import pytest
 import torch

@@ -26,9 +26,8 @@ TOL_TC_SPLIT = dict(TOL_FP32, grad_head=3e-1)
 # bf16 tensor-core path vs the fp32 reference at the BASELINE sizes: plain bf16 operands
 # (8-bit mantissa) and bf16-stored activations through 36 conv+BN layers cannot meet
 # 1e-4; an fp32-graph emulation of the same rounding points (oracle emulate="bf16")
-# deviates from fp32 by the same amount (pred ~7e-2 max-abs relative).  Measured on
-# B200 (gpurun_out/parity_*_bf16.json): loss 2e-3..5e-3, pred 4e-2..7e-2, grad norms
-# <= 0.27.  The 1e-4 bar is met by precision="fp32" (tests above).
+# deviates from fp32 by the same amount (pred ~7e-2 max-abs relative).  The 1e-4 bar is
+# met by precision="fp32" (tests above).
 TOL_BF16 = dict(loss=2e-2, pred=1.5e-1, grad=4e-1, grad_head=6.0, post=3e-3, sgrad=1e-1)
 
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
@@ -76,7 +75,7 @@ def test_step_fp32_strict_full_size(name):
 
 @pytest.mark.parametrize("name", TINY)
 def test_step_tc_split_strict(name):
-    """The north-star bar ON the tensor cores: precision="tc_split" (tcgen05, fp16 hi/lo operand planes, 4 MMAs per
+    """The north-star bar ON the tensor cores: precision="tc_split" (wgmma, fp16 hi/lo operand planes, 4 MMAs per
     product, fp32 accumulate / storage) against the reference goldens at the fp32 tolerances."""
     _run(name, "tc_split", TOL_TC_SPLIT)
 
@@ -103,7 +102,7 @@ def test_step_bf16_tensor_core_tiny_shapes(name):
 
 @pytest.mark.parametrize("name", ["posenet_b8_256", "posenet_ragged", "posenet_7scenes_b4"])
 def test_tensor_core_path_matches_cuda_core_path_on_bf16(name):
-    """Same bf16 storage / operands, two independent engines: tcgen05 (precision bf16) vs
+    """Same bf16 storage / operands, two independent engines: wgmma (precision bf16) vs
     CUDA-core fp32 FMA (precision bf16_simt).  Only accumulation order differs."""
     from oracle import weights
     g, cfg = load_golden(name)
@@ -125,9 +124,8 @@ def test_tensor_core_path_matches_cuda_core_path_on_bf16(name):
            "feature_extractor.layer1.0.conv1.weight", "feature_extractor.conv1.weight")}
     print("tc-vs-simt", name, el, ep, eg)
     # same operands, only the fp32 accumulation order differs; what is left are bf16 rounding
-    # ties / ReLU mask flips (see test_fp32_error_is_at_reference_noise_floor).  Measured on B200
-    # for posenet_b8_256 (space-to-depth stem): loss 5.9e-3, pose 2.9e-2 -- the value moves with
-    # the engines' summation order, the bound is ~2x the measured.
+    # ties / ReLU mask flips (see test_fp32_error_is_at_reference_noise_floor); the value moves
+    # with the engines' summation order.
     assert el < (1e-2 if tight else 5e-2), (el, ep, eg)
     assert ep < (5e-2 if tight else 3e-1), (el, ep, eg)
     # early-layer gradients of this randomly initialised 34-layer BN network are chaotic in
@@ -265,7 +263,7 @@ def test_fp32_error_is_at_reference_noise_floor(name):
     crit = make_product_criterion(cfg["kind"])
     model.train()
     loss, pred, grads, sgrads = product_step(model, net, crit, x, targ, do_step=False)
-    # Per-tensor picture (tools/diag_grads.py on B200): the tail of the backward pass (head,
+    # Per-tensor picture (tools/diag_grads.py): the tail of the backward pass (head,
     # layer4.2) agrees to ~1e-5; further back the error moves in discrete jumps of ~2e-3 --
     # individual ReLU masks of activations within fp32 rounding of zero flip between any two
     # fp32 implementations -- and the reference's own fp32 run shows the same jumps against

@@ -1,7 +1,6 @@
-"""The CPU oracle (oracle/mapnet_oracle.py) pinned against outputs of the REFERENCE:
- * everywhere: the committed goldens in tests/golden/ (made by oracle/make_goldens.py
-   from /root/reference's own modules);
- * in the build container: the reference modules executed live through oracle.ref_loader."""
+"""The CPU oracle (oracle/mapnet_oracle.py) pinned against outputs of the REFERENCE: the committed goldens in
+tests/golden/, made by oracle/make_goldens.py from the reference's own modules (live_reference.npz holds what the
+reference modules computed on the configs below, gradients as fixed-stride samples plus full norms)."""
 import ast
 import os
 
@@ -10,7 +9,7 @@ import pytest
 import torch
 
 from oracle import mapnet_oracle as O
-from oracle import ref_loader, weights
+from oracle import weights
 
 SV = dict(sax=0.0, saq=-3.0, srx=0.0, srq=-3.0)
 
@@ -28,6 +27,9 @@ def test_oracle_step_matches_reference_golden(golden_dir, name):
     x, targ = weights.make_inputs(cfg, int(g["seed"]))
     if "x" in g.files:
         assert np.array_equal(x.numpy(), g["x"]), "input generator drifted"
+    if "x_head" in g.files:
+        assert np.array_equal(x.numpy().reshape(-1)[:g["x_head"].size], g["x_head"]), "input generator drifted"
+    assert abs(float(x.double().sum()) - float(g["x_checksum"])) < 1e-6 * max(1.0, abs(float(g["x_checksum"])))
     assert np.array_equal(targ.numpy(), g["targ"])
     r = O.train_step(cfg["kind"], st, x, targ, SV, lr=cfg.get("lr", 1e-4), weight_decay=cfg.get("wd", 5e-4),
                      max_grad_norm=cfg.get("clip", 0.0), filter_nans=cfg["kind"].startswith("online"))
@@ -79,65 +81,63 @@ def test_flop_model():
     assert abs(O.train_flops_per_image(256, 256) - 28.400e9) < 0.01e9
 
 
-@pytest.mark.skipif(not ref_loader.available(), reason="reference tree only exists in the build container")
+def _live(golden_dir):
+    return np.load(os.path.join(golden_dir, "live_reference.npz"))
+
+
+def _check_grad_samples(L, prefix, grads):
+    """oracle gradients vs the reference's: full norms and the stored fixed-stride samples"""
+    for i, k in enumerate(L[prefix + "grad_names"]):
+        v = grads[str(k)].detach().double().flatten()
+        ref_norm = float(L[prefix + "grad_norm"][i])
+        assert abs(float(v.norm()) - ref_norm) <= 1e-5 * ref_norm + 1e-12, k
+        sample = v[::int(L[prefix + "grad_stride"][i])].numpy()
+        assert float(np.linalg.norm(sample - L[prefix + "grad_%d" % i])) <= 1e-5 * ref_norm + 1e-12, k
+
+
 @pytest.mark.parametrize("kind,cfg", [("posenet", dict(kind="posenet", N=2, H=64, W=64)),
                                       ("online", dict(kind="online", N=2, T=4, H=64, W=64))])
-def test_oracle_matches_live_reference(kind, cfg):
-    ns = ref_loader.load()
+def test_oracle_matches_live_reference(golden_dir, kind, cfg):
+    L = _live(golden_dir)
     st = weights.make_state(3)
     x, targ = weights.make_inputs(cfg, 3)
-    model = ref_loader.build_reference_model(st, "posenet" if kind == "posenet" else "mapnet")
-    model.train()
-    if kind == "posenet":
-        crit = ns.PoseNetCriterion(sax=0.0, saq=-3.0, learn_beta=True)
-    else:
-        crit = ns.MapNetOnlineCriterion(sax=0.0, saq=-3.0, srx=0.0, srq=-3.0, learn_beta=True, learn_gamma=True)
-    loss, out, grads, cg = ref_loader.reference_step(model, crit, x, targ)
     r = O.train_step(kind, st, x, targ, SV)
+    loss = float(L["step_%s_loss" % kind])
+    out = torch.from_numpy(L["step_%s_out" % kind])
     assert abs(float(r["loss"]) - loss) <= 1e-6 * abs(loss)
     assert float((out - r["pred"].view_as(out)).abs().max()) <= 1e-6
-    for k, v in grads.items():
-        k2 = k.replace("mapnet.", "", 1)
-        assert float((v - r["grads"][k2]).norm()) <= 1e-5 * float(v.norm()) + 1e-12, k
+    _check_grad_samples(L, "step_%s_" % kind, r["grads"])
 
 
-@pytest.mark.skipif(not ref_loader.available(), reason="reference tree only exists in the build container")
-def test_oracle_nan_filter_matches_live_reference_hook():
+def test_oracle_nan_filter_matches_live_reference_hook(golden_dir):
     """models/posenet.py:28-34,50-51 with a NaN-producing gradient: degenerate state (fc_wpqr = 0 -> every predicted
     rotation is the identity -> qlog's backward gives NaN, the case the hook exists for) through the reference
     MapNet + MapNetOnlineCriterion with filter_nans=True, against the oracle.  The hook zeroes NaNs of the Linear's
     bias / input / weight gradients: whole weight rows and whole samples drop out, not single entries."""
-    ns = ref_loader.load()
+    L = _live(golden_dir)
     st = weights.make_state(3)
     st["fc_wpqr.weight"] = torch.zeros_like(st["fc_wpqr.weight"])
     st["fc_wpqr.bias"] = torch.zeros_like(st["fc_wpqr.bias"])
     cfg = dict(kind="online", N=2, T=4, H=64, W=64)
     x, targ = weights.make_inputs(cfg, 3)
-    model = ref_loader.build_reference_model(st, "mapnet", filter_nans=True)
-    model.train()
-    crit = ns.MapNetOnlineCriterion(sax=0.0, saq=-3.0, srx=0.0, srq=-3.0, learn_beta=True, learn_gamma=True)
-    import warnings
-    with warnings.catch_warnings():
-        warnings.simplefilter("ignore")
-        loss, out, grads, cg = ref_loader.reference_step(model, crit, x, targ, do_step=False)
     r = O.train_step("online", st, x, targ, SV, filter_nans=True, do_step=False)
     # the unfiltered gradient really is NaN in the rotation half
     r_nofilter = O.train_step("online", st, x, targ, SV, filter_nans=False, do_step=False)
     assert bool(torch.isnan(r_nofilter["grads"]["fc_wpqr.weight"]).any())
-    n_zero_rows = 0
-    for k, v in grads.items():
-        k2 = k.replace("mapnet.", "", 1)
-        assert bool(torch.isfinite(v).all()) and bool(torch.isfinite(r["grads"][k2]).all()), k
-        assert float((v - r["grads"][k2]).norm()) <= 1e-5 * float(v.norm()) + 1e-12, k
-    for j in range(3):
-        n_zero_rows += int(bool((grads["mapnet.fc_wpqr.weight"][j] == 0).all()))
+    assert bool(L["nanfilter_all_finite"].all())
+    for k in L["nanfilter_grad_names"]:
+        assert bool(torch.isfinite(r["grads"][str(k)]).all()), k
+    _check_grad_samples(L, "nanfilter_", r["grads"])
+    ref_w = torch.from_numpy(L["nanfilter_fc_wpqr_weight"])
+    assert float((ref_w - r["grads"]["fc_wpqr.weight"]).norm()) <= 1e-5 * float(ref_w.norm()) + 1e-12
+    n_zero_rows = sum(int(bool((ref_w[j] == 0).all())) for j in range(3))
     assert n_zero_rows >= 1, "the degenerate input was meant to wipe at least one fc_wpqr row"
 
 
-def test_baseline_config0_plumbing_single_frame():
+def test_baseline_config0_plumbing_single_frame(golden_dir):
     """BASELINE.json configs[0] / SURVEY.md section 8d "Config 1 (plumbing)": PoseNet ResNet-34 on ONE synthetic 256x256 frame,
-    PoseNetCriterion(sax=0, saq=-3), seed 7, on the CPU: a [1,6] output and a finite loss -- through the oracle everywhere,
-    and against the reference modules executed live where the reference tree exists."""
+    PoseNetCriterion(sax=0, saq=-3), seed 7, on the CPU: a [1,6] output and a finite loss -- through the oracle, and
+    against what the reference modules computed (tests/golden/live_reference.npz)."""
     st = weights.make_state(7)
     g = torch.Generator().manual_seed(7)
     x = torch.randn(1, 3, 256, 256, generator=g)
@@ -149,12 +149,8 @@ def test_baseline_config0_plumbing_single_frame():
     want = float((r["pred"][:, :3] - targ[:, :3]).abs().mean() + 0.0
                  + np.exp(3.0) * (r["pred"][:, 3:] - targ[:, 3:]).abs().mean() - 3.0)
     assert abs(float(r["loss"]) - want) <= 1e-5 * abs(want)
-    if ref_loader.available():
-        ns = ref_loader.load()
-        model = ref_loader.build_reference_model(st, "posenet")
-        model.train()
-        crit = ns.PoseNetCriterion(sax=0.0, saq=-3.0, learn_beta=True)
-        loss, out, _, _ = ref_loader.reference_step(model, crit, x, targ, do_step=False)
-        assert tuple(out.shape) == (1, 6)
-        assert abs(loss - float(r["loss"])) <= 1e-6 * abs(loss)
-        assert float((out - r["pred"]).abs().max()) <= 1e-6
+    L = _live(golden_dir)
+    loss, out = float(L["config0_loss"]), torch.from_numpy(L["config0_out"])
+    assert tuple(out.shape) == (1, 6)
+    assert abs(loss - float(r["loss"])) <= 1e-6 * abs(loss)
+    assert float((out - r["pred"]).abs().max()) <= 1e-6

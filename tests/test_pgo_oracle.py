@@ -1,11 +1,9 @@
-"""The CPU restatement of the reference's pose-graph optimisation (oracle/pgo_oracle.py) pinned against
- * the committed goldens tests/golden/pgo.npz (made by oracle/make_goldens.py from the reference's own PoseGraph /
-   PoseGraphFC classes), everywhere;
- * the reference classes executed live from /root/reference/common/pose_utils.py:306-804, in the build container."""
+"""The CPU restatement of the reference's pose-graph optimisation (oracle/pgo_oracle.py) pinned against the committed
+goldens tests/golden/pgo.npz and live_reference.npz, made by oracle/make_goldens.py from the reference's own
+PoseGraph / PoseGraphFC classes and numpy helpers (common/pose_utils.py:306-804)."""
 import os
 
 import numpy as np
-import pytest
 
 from oracle import pgo_oracle as P
 
@@ -45,23 +43,13 @@ def test_reference_step_is_not_the_gauss_newton_step(golden_dir):
         assert np.abs(exact - ref[0]).max() < 5e-2       # ... although both iterations settle near the same poses
 
 
-@pytest.mark.skipif(not P.available(), reason="reference tree only exists in the build container")
-def test_pgo_oracle_matches_live_reference_classes():
-    ns = P.load_reference()
-    rng = np.random.default_rng(11)
-    for N, fc in [(3, False), (6, False), (5, True)]:
-        t = rng.normal(size=(N, 3)).cumsum(0) * 0.3
-        v = rng.normal(size=(N, 3)) * 0.4
-        q = np.stack([np.concatenate(([np.cos(np.linalg.norm(a))], np.sinc(np.linalg.norm(a) / np.pi) * a)) for a in v])
-        gt = np.hstack((t, q))
-        pred = gt + rng.normal(size=gt.shape) * 0.05
-        E = P.edges(N, fc)
-        vos = np.stack([np.concatenate((P.rotate_vector(gt[j, :3] - gt[i, :3], P.qinverse(gt[i, 3:])),
-                                        P.qmult(P.qinverse(gt[i, 3:]), gt[j, 3:]))) for i, j in E])
-        ref = ns["optimize_poses"](pred_poses=pred.copy(), vos=vos.copy(), fc_vos=fc, sax=1.5, saq=0.3, srx=0.7, srq=0.1)
+def test_pgo_oracle_matches_live_reference_classes(golden_dir):
+    L = np.load(os.path.join(golden_dir, "live_reference.npz"))
+    for ci in range(3):
+        pred, vos, fc = L["pgo%d_pred" % ci], L["pgo%d_vos" % ci], bool(L["pgo%d_fc" % ci])
         got = P.optimize_poses(pred, vos, fc, sax=1.5, saq=0.3, srx=0.7, srq=0.1)
-        assert np.abs(ref - got).max() <= 1e-12
+        assert np.abs(L["pgo%d_out" % ci] - got).max() <= 1e-12
     # the numpy helpers one by one
     for name in ("dpq_q", "dpsq_q", "dpsq_p", "dqstq_t", "m_rot"):
-        x = rng.normal(size=(4, 1))
-        assert np.abs(ns[name](x) - getattr(P, name)(x)).max() <= 1e-15, name
+        x = L["pgohelper_%s_in" % name]
+        assert np.abs(L["pgohelper_%s_out" % name] - getattr(P, name)(x)).max() <= 1e-15, name

@@ -146,40 +146,24 @@ def test_color_jitter_sampler_draws_what_torchvision_draws(hp):
     assert r0[0] == 1.0 and r0[2] == 1.0 and r0[3] == 0.0 and 0.8 <= r0[1] <= 1.2
 
 
-def _reference_get_indices():
-    """MF.get_indices / __len__ executed from the reference's own source text (dataset_loaders/composite.py:60-75,
-    105-109) with the Python-2 integer divisions spelled `//` (the module itself imports py2-only dataset code)."""
-    path = "/root/reference/dataset_loaders/composite.py"
-    if not os.path.exists(path):
-        pytest.skip("reference tree only exists in the build container")
-    src = open(path).read().split("\n")
-    start = next(i for i, l in enumerate(src) if l.strip().startswith("def get_indices"))
-    end = next(i for i in range(start + 1, len(src)) if src[i].strip().startswith("def "))
-    body = "\n".join(l[2:] for l in src[start:end])
-    body = body.replace("len(offsets) / 2", "len(offsets) // 2").replace("self.steps/2", "self.steps//2").replace("np.int)", "int)")
-    ns = {"np": np}
-    exec(body, ns)
-    return ns["get_indices"]
-
-
-def test_tuple_indices_match_reference_mf():
-    from types import SimpleNamespace
+def test_tuple_indices_match_reference_mf(golden_dir):
+    """tuples.mf_indices against MF.get_indices / __len__ of the reference (dataset_loaders/composite.py:60-75,
+    105-109), as stored in tests/golden/live_reference.npz by oracle/make_goldens.py."""
     from geomapnet_b200.data import tuples
-    get_indices = _reference_get_indices()
-    for steps, skip, L in [(3, 10, 1000), (5, 10, 47), (2, 1, 5), (4, 3, 30), (3, 10, 12)]:
-        for nodup in (False, True):
-            me = SimpleNamespace(variable_skip=False, skip=skip, steps=steps, no_duplicates=nodup, dset=range(L))
-            n = tuples.mf_len(L, steps, skip, nodup)
-            assert n == (L - (steps - 1) * skip if nodup else L)
-            for index in list(range(0, min(n, 40))) + [max(n - 1, 0)]:
-                ref = get_indices(me, index)
-                got = tuples.mf_indices(index, L, steps, skip, nodup)
-                assert np.array_equal(ref, got), (steps, skip, L, nodup, index)
+    L = np.load(os.path.join(golden_dir, "live_reference.npz"))
+    cases = L["mf_cases"]
+    seen = set()
+    for row in cases:
+        steps, skip, length, nodup, index = (int(v) for v in row[:5])
+        n = tuples.mf_len(length, steps, skip, bool(nodup))
+        assert n == (length - (steps - 1) * skip if nodup else length)
+        got = tuples.mf_indices(index, length, steps, skip, bool(nodup))
+        assert np.array_equal(row[5:5 + steps], got), (steps, skip, length, nodup, index)
+        seen.add((steps, skip, length, nodup))
+    assert len(seen) == 10
     # variable_skip consumes np.random exactly as the reference does
-    me = SimpleNamespace(variable_skip=True, skip=7, steps=5, no_duplicates=False, dset=range(500))
-    np.random.seed(3); ref = get_indices(me, 250)
     np.random.seed(3); got = tuples.mf_indices(250, 500, 5, 7, variable_skip=True)
-    assert np.array_equal(ref, got)
+    assert np.array_equal(L["mf_variable_skip"], got)
     # MFOnline: train tuple | validation tuple (no_duplicates), both modulo their dataset length
     tr, va = tuples.mfonline_indices(123, 100, 60, 5, 10)
     assert np.array_equal(tr, tuples.mf_indices(123 % 100, 100, 5, 10)) and \

@@ -1,11 +1,11 @@
 """Host logic of the tensor-core conv engines, checked WITHOUT a GPU.
 
-`tc_plan_create` (geomapnet_b200/csrc/conv_tc.cu) turns a convolution into tiles, output-parity classes, filter
-taps (spatial offset, activation view, K index of the weight slice) and, for the halo engine, shifts in a padded
-linear pixel space.  That arithmetic is pure host code; the kernels only walk it.  Here the plan is exported as JSON
+`tc_plan_create` (geomapnet_b200/csrc/conv_tc.cu) turns a convolution into tiles, output-parity classes and filter
+taps (spatial offset, activation view, K index of the weight slice).  That arithmetic is pure host code; the kernels
+only walk it.  Here the plan is exported as JSON
 (`mapnet_test_plan_describe`) and REPLAYED on the CPU in float64 exactly as the kernels consume it -- TMA semantics:
 out-of-bounds rows read as zero, stride-2 convs read parity views -- and compared with torch's conv2d and its autograd
-(the third-party arithmetic the reference calls, /root/reference/models/posenet.py:66).  Shapes are fuzzed: odd
+(the third-party arithmetic the reference calls, reference models/posenet.py:66).  Shapes are fuzzed: odd
 sizes, both strides, 1x1 and 3x3, the downsample shortcut folded into the stride-2 dgrad."""
 import ctypes
 import os
@@ -100,29 +100,6 @@ def replay_launches(plan, views, wmats, out_shape):
     return out
 
 
-def replay_halo(plan, src, Wm):
-    """halo-resident 3x3 / stride-1 engine: nine shifts in the padded linear pixel space q = h*P + w + 1"""
-    H = plan["halo_params"]
-    B, Hh, Ww, P, Cs = H["Nimg"], H["H"], H["W"], H["P"], H["Cs"]
-    assert P == Ww + 2 and H["tiles_per_img"] * 128 >= Hh * P and H["n_tiles_m"] == B * H["tiles_per_img"]
-    for t in range(H["tiles_per_img"]):        # the patch box of R rows holds every row a tile's taps touch
-        q0 = 128 * t
-        h_lo = (q0 - P - 1) // P
-        h_hi = (min(q0 + 127, Hh * P - 1) + P + 1) // P
-        assert h_hi - h_lo + 1 <= H["R"] or h_hi >= Hh + 1, (t, h_lo, h_hi, H["R"])
-    padded = torch.zeros(B, (Hh + 4) * P + 2 * P, Cs, dtype=torch.float64)     # zero halo all around
-    base = 2 * P
-    for h in range(Hh):
-        padded[:, base + h * P + 1: base + h * P + 1 + Ww, :] = src[:, h, :, :]
-    out = torch.zeros(B, Hh, Ww, Wm.shape[0], dtype=torch.float64)
-    for t in range(9):
-        dq, kidx = H["dq"][t], H["kidx"][t]
-        for h in range(Hh):
-            q = base + h * P + 1 + dq
-            out[:, h, :, :] += padded[:, q:q + Ww, :] @ Wm[:, kidx * Cs:(kidx + 1) * Cs].T
-    return out
-
-
 GEOMS = [(2, 16, 16, 64, 64, 3, 1), (2, 16, 16, 64, 128, 3, 2), (2, 16, 16, 64, 128, 1, 2), (3, 9, 11, 128, 128, 3, 1),
          (2, 18, 22, 64, 128, 3, 2), (1, 8, 8, 128, 256, 3, 2), (1, 12, 10, 128, 64, 1, 1), (3, 17, 13, 64, 128, 3, 2),
          (2, 7, 5, 128, 128, 3, 2), (1, 33, 9, 64, 64, 3, 1), (2, 6, 40, 64, 64, 3, 1), (1, 11, 11, 64, 128, 1, 2)]
@@ -133,12 +110,9 @@ def test_fprop_plan_replays_to_conv2d(lib, geom):
     c = make_case(geom, 3)
     plan = describe(lib, 0, geom)
     B, H, W, Ci, Co, k, s = geom
-    if plan["halo"]:
-        got = replay_halo(plan, c["x"], w_krsc(c["w"]))
-    else:
-        maps = plan["launches"][0]["maps"]
-        views = [parity_view(c["x"], s, a, b) for a, b in maps] + [None] * 4
-        got = replay_launches(plan, views, [w_krsc(c["w"])], tuple(c["y"].shape))
+    maps = plan["launches"][0]["maps"]
+    views = [parity_view(c["x"], s, a, b) for a, b in maps] + [None] * 4
+    got = replay_launches(plan, views, [w_krsc(c["w"])], tuple(c["y"].shape))
     assert float((got - c["y"]).abs().max()) < 1e-9 * max(1.0, float(c["y"].abs().max()))
 
 
@@ -146,14 +120,11 @@ def test_fprop_plan_replays_to_conv2d(lib, geom):
 def test_dgrad_plan_replays_to_autograd(lib, geom):
     c = make_case(geom, 4)
     plan = describe(lib, 1, geom)
-    if plan["halo"]:
-        got = replay_halo(plan, c["dy"], w_dg(c["w"]))
-    else:
-        if geom[6] == 2:
-            assert len(plan["launches"]) == 1 and len(plan["launches"][0]["classes"]) == 4     # one launch, four parity classes
-            taps = sorted(len(cl["taps"]) for cl in plan["launches"][0]["classes"])
-            assert taps == ([1, 2, 2, 4] if geom[5] == 3 else [0, 0, 0, 1])
-        got = replay_launches(plan, [c["dy"], None, None, None], [w_dg(c["w"])], tuple(c["dx"].shape))
+    if geom[6] == 2:
+        assert len(plan["launches"]) == 1 and len(plan["launches"][0]["classes"]) == 4     # one launch, four parity classes
+        taps = sorted(len(cl["taps"]) for cl in plan["launches"][0]["classes"])
+        assert taps == ([1, 2, 2, 4] if geom[5] == 3 else [0, 0, 0, 1])
+    got = replay_launches(plan, [c["dy"], None, None, None], [w_dg(c["w"])], tuple(c["dx"].shape))
     assert float((got - c["dx"]).abs().max()) < 1e-9 * max(1.0, float(c["dx"].abs().max()))
 
 
@@ -171,7 +142,7 @@ def test_dgrad_plan_with_folded_shortcut(lib, geom):
     ((y1 * dy1).sum() + (y2 * dy2).sum()).backward()
     nhwc = lambda t: t.detach().permute(0, 2, 3, 1).contiguous()
     plan = describe(lib, 1, geom, shortcut=1)
-    assert plan["shortcut"] == 1 and not plan["halo"]
+    assert plan["shortcut"] == 1
     last = plan["launches"][0]["classes"][-1]
     assert (last["oa"], last["ob"]) == (0, 0) and last["taps"][-1] == [0, 0, 5, 0]      # map 1 | second weight matrix
     got = replay_launches(plan, [nhwc(dy1), nhwc(dy2), None, None], [w_dg(w1), w_dg(w2)], (B, H, W, Ci))
@@ -190,7 +161,7 @@ def test_wgrad_plan_replays_to_autograd(lib, geom):
     assert P["tiles_w"] * P["TW"] >= Wo and P["tiles_h"] * P["TH"] >= Ho and P["tiles_n"] * P["TN"] >= B
     assert P["splits"] * P["tiles_per_split"] >= P["n_pix_tiles"] and (P["splits"] - 1) * P["tiles_per_split"] < P["n_pix_tiles"]
     assert P["n_chunks"] == k * k * (Ci // 64) and len(P["chunks"]) == P["n_chunks"]
-    assert P["n_mtiles"] * (4 if plan["two_cta"] else 2) >= P["n_chunks"] and P["n_ntiles"] * P["BN"] == Co
+    assert P["n_mtiles"] * 2 >= P["n_chunks"] and P["n_ntiles"] * P["BN"] == Co
     views = [parity_view(c["x"], s, a, b) for a, b in P["maps"]]
     got = torch.full((Co, k * k, Ci), float("nan"), dtype=torch.float64)
     for dh, dw, mp, c0, tap in P["chunks"]:
@@ -211,21 +182,11 @@ def test_resnet34_layer_plans_at_benchmark_size(lib):
         for kind in (0, 1):
             p = describe(lib, kind, (64, H, H, Ci, Co, k, s), shortcut=1 if (kind == 1 and s == 2) else 0)
             n_out = Co if kind == 0 else Ci
-            if p["halo"]:
-                hp = p["halo_params"]
-                assert hp["smem"] <= 227 * 1024 and hp["NP"] >= 2
-                items = hp["n_tiles_m"] * hp["n_tiles_n"]
-            else:
-                L = p["launches"][0]
-                items = cdiv(L["n_tiles_m"], p["CL"]) * L["n_tiles_n"] * len(L["classes"])
-                assert n_out % p["BN"] == 0 and len(p["launches"]) == 1
-            rows.append((name, "fprop" if kind == 0 else "dgrad", "halo" if p["halo"] else ("pair" if p["two_cta"] else "1cta"),
-                         p["BN"], items))
+            L = p["launches"][0]
+            items = cdiv(L["n_tiles_m"], p["CL"]) * L["n_tiles_n"] * len(L["classes"])
+            assert n_out % p["BN"] == 0 and p["BN"] in (64, 128) and len(p["launches"]) == 1
+            rows.append((name, "fprop" if kind == 0 else "dgrad", p["BN"], items))
     table = {(r[0], r[1]): r[2:] for r in rows}
-    # round 2: layer1 runs on the per-tap engine with two CTAs per SM (BN = 64; profiles/r02b_conv_microbench.txt); the
-    # halo-resident engine (stationary weights, Cin = 64) is selected with MAPNET_TC_HALO=1
-    want = "halo" if os.environ.get("MAPNET_TC_HALO") == "1" else "1cta"
-    assert table[("layer1", "fprop")][0] == want and table[("layer1", "dgrad")][0] == want
-    assert table[("layer1", "fprop")][1] == 64
+    assert table[("layer1", "fprop")][0] == 64
     for r in rows:
-        assert r[4] >= 32, r          # enough work items to occupy a good part of the 148 SMs
+        assert r[3] >= 32, r          # enough work items to occupy a good part of the 132 SMs

@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 conv engines per ResNet-34 layer shape (GPU box).
+"""Micro-benchmark of the wgmma conv engines per ResNet-34 layer shape (GPU box).
 usage: python tools/bench_conv.py [B]   (env MAPNET_TC_* select the engine variant)"""
 import ctypes, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,4 +1,4 @@
-"""Throughput of the GPU input pipeline (SURVEY.md 8f, row f2) on one B200: Resize(256) -> [ColorJitter] -> ToTensor ->
+"""Throughput of the GPU input pipeline (SURVEY.md 8f, row f2) on one GPU: Resize(256) -> [ColorJitter] -> ToTensor ->
 Normalize over 64 frames of 480x640 (the 7-Scenes frame size), with and without the tuple gather and the jitter.
 HBM-bound byte work: algorithmic bytes = uint8 frames in + fp32 tensor out.  usage: python tools/bench_preprocess.py [out.json]"""
 import json, os, sys

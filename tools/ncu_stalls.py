@@ -6,7 +6,7 @@ reports themselves exceed gpurun's return limit).
 
 writes profiles/<tag>_ncu_stalls.txt: for every captured launch the share of each stall reason over all sampled
 instructions, and the `top` hottest SASS instructions with their own dominant reason -- the two things one reads
-off the source page to decide what a tcgen05 / TMA kernel is waiting for (stall_long_sb = global / TMEM loads in
+off the source page to decide what a wgmma / TMA kernel is waiting for (stall_long_sb = global loads in
 flight, stall_barrier / stall_membar = mbarrier and fence waits, stall_no_inst = instruction fetch, ...).
 """
 import csv

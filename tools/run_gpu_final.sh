@@ -1,5 +1,5 @@
 #!/bin/bash
-# Round-end evidence on one B200: ncu rows per kernel class + launch list (tools/run_ncu_classes.sh), then the bench
+# Round-end evidence on one GPU: ncu rows per kernel class + launch list (tools/run_ncu_classes.sh), then the bench
 # lines the profiles/ directory quotes.  Outputs -> gpurun_out/
 TAG=${1:-r02c}
 mkdir -p gpurun_out

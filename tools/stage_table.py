@@ -1,14 +1,15 @@
-"""Per-stage view of the conv launches of ONE training step, from the committed ncu launch list.
+"""Per-stage view of the conv launches of ONE training step, from a committed launch list.
 
-    python tools/stage_table.py profiles/r02c_launches_raw.csv [peak_tflops] > profiles/r02c_conv_by_stage.txt
+    python tools/stage_table.py profiles/h100_launches_raw.csv [peak_tflops] > profiles/h100_conv_by_stage.txt
 
-The launch list (tools/launch_shares.py: `ncu --metrics gpu__time_duration.sum --clock-control none`, one eager step of
-posenet_bs64) is in launch order, which is the trunk's schedule (geomapnet_b200/csrc/net.cu): forward = stem, then per
+The launch list (tools/profile_launches.py, torch.profiler's CUDA trace of one eager step of posenet_bs64; or
+tools/launch_shares.py from an ncu capture) is in launch order, which is the trunk's schedule (geomapnet_b200/csrc/net.cu): forward = stem, then per
 BasicBlock conv1, conv2[, downsample]; backward = blocks in reverse, per block dgrad(conv2) then dgrad(conv1) (a
 downsampling block's conv1 dgrad carries the 1x1 shortcut dgrad in the same launch), wgrad(conv2), wgrad(conv1)
 [, wgrad(downsample)], the stem's wgrad last.  Every conv launch is matched to its layer by position and its ALGORITHMIC
-FLOPs (B = 64, 256x256) are divided by its duration.  Durations under ncu are serialised and cold-cache: compare stages
-with each other and against bench.py's event-bracketed per-class numbers, not as absolute step time."""
+FLOPs (B = 64, 256x256) are divided by its duration.  Durations of an eager, traced step: compare stages with each other
+and against bench.py's event-bracketed per-class numbers, not as absolute step time.  Default peaks: the H100 SXM data
+sheet (989 dense bf16 TFLOP/s, 3350 GB/s HBM3), bounds that are not reached."""
 import csv
 import sys
 
@@ -33,7 +34,7 @@ def layers():
 
 def main():
     path = sys.argv[1]
-    peak = float(sys.argv[2]) if len(sys.argv) > 2 else 1653.4      # burst bf16 TFLOP/s measured in the capture's session
+    peak = float(sys.argv[2]) if len(sys.argv) > 2 else 989.0       # H100 SXM data sheet, dense bf16 TFLOP/s
     rows = list(csv.reader(open(path)))[1:]
     L = [(r[1], float(r[2]) / 1e3) for r in rows]                   # (kernel, us)
     stem, blocks = layers()
@@ -51,7 +52,7 @@ def main():
     w_order.append(("stem", stem))
     assert len(fw) == len(f_order) == 36 and len(dg) == len(d_order) == 32 and len(wg) == len(w_order) == 36, \
         (len(fw), len(dg), len(wg))
-    print("# %s: conv launches of one eager posenet_bs64 step by ResNet stage; peak = %.1f TFLOP/s (burst)" % (path, peak))
+    print("# %s: conv launches of one eager posenet_bs64 step by ResNet stage; peak = %.1f TFLOP/s" % (path, peak))
     grand_us = grand_fl = 0.0
     for name, lst, order in (("fprop", fw, f_order), ("dgrad", dg, d_order), ("wgrad", wg, w_order)):
         agg = {}
@@ -74,7 +75,7 @@ def main():
     elementwise(L, split)
 
 
-def elementwise(L, split, hbm=6571.2):
+def elementwise(L, split, hbm=3350.0):
     """BatchNorm apply kernels by stage, against the HBM roofline in ALGORITHMIC bytes (bf16 tensors): forward
     k_bn_apply_lazy<.., RES> reads y [+ the residual or the downsample conv's output] and writes z: 4 / 6 / 6 bytes per
     element for RES = 0 / 1 / 2; backward k_bn_bwd_apply*<.., DS, ..> reads the (already ReLU-gated) gradient and y and
