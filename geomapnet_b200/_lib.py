@@ -58,6 +58,13 @@ def lib():
     L.mapnet_adam_step_dev.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float, c_float, c_float,
                                        c_float, c_float, c_void_p, c_float, c_void_p, c_float, c_void_p]
     L.mapnet_adam_step_dev.restype = c_int
+    L.mapnet_sgd_step_dev.argtypes = [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, ctypes.c_double,
+                                      c_float, c_int, c_void_p, c_float, c_void_p, c_float, c_void_p]
+    L.mapnet_sgd_step_dev.restype = c_int
+    L.mapnet_rmsprop_step_dev.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                          ctypes.c_double, c_float, c_float, c_float, c_void_p, c_float, c_void_p,
+                                          c_float, c_void_p]
+    L.mapnet_rmsprop_step_dev.restype = c_int
     L.mapnet_test_conv.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                    c_void_p, c_void_p, c_void_p, c_void_p]
     L.mapnet_test_stem.argtypes = [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
@@ -107,7 +114,8 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_adam_step_dev", "mapnet_bench_conv", "mapnet_test_stem",
             "mapnet_test_dgrad_shortcut", "mapnet_test_plan_describe", "mapnet_preprocess_create",
             "mapnet_preprocess_output_size", "mapnet_preprocess_run", "mapnet_preprocess_destroy",
-            "mapnet_backward_part", "mapnet_grad_part_range", "mapnet_preprocess_run_ex", "mapnet_test_conv_epilogue", "mapnet_pose_post", "mapnet_pgo_optimize"]
+            "mapnet_backward_part", "mapnet_grad_part_range", "mapnet_preprocess_run_ex", "mapnet_test_conv_epilogue", "mapnet_pose_post", "mapnet_pgo_optimize",
+            "mapnet_sgd_step_dev", "mapnet_rmsprop_step_dev"]
 
 
 def check(rc, what):

@@ -17,7 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(CSRC, "libmapnet_b200.so")
 OBJ = os.path.join(CSRC, "_obj")
 SOURCES = ["api.cu", "net.cu", "bn.cu", "conv_simt.cu", "conv_tc.cu", "layout.cu", "head.cu", "loss.cu", "adam.cu",
-           "preprocess.cu", "pgo.cu"]
+           "optim.cu", "preprocess.cu", "pgo.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]

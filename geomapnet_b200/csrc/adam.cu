@@ -59,6 +59,12 @@ int launch_sqnorm(const float* g, long long n, float* partials, float* out_sq, c
 __global__ void k_inc_i32(int* c) {
   pdl_prologue(); *c += 1; }
 
+int launch_inc_i32(int* c, cudaStream_t st) {
+  MN_LAUNCH(k_inc_i32, 1, 1, 0, st, c);
+  MN_LAUNCH_CHECK();
+  return 0;
+}
+
 __global__ void __launch_bounds__(256)
 k_adam(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
        long long n, float lr, float b1, float b2, float eps, float wd, float bc1, float bc2_sqrt,
@@ -71,14 +77,7 @@ k_adam(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m
     bc1 = (float)(1.0 - pow((double)b1, t));
     bc2_sqrt = sqrtf((float)(1.0 - pow((double)b2, t)));
   }
-  float coef = gscale;
-  if (sqnorm != nullptr) {
-    // clip_grad_norm_: coef = max_norm / (total_norm + 1e-6), clamped to 1
-    const float total = sqrtf(sqnorm[0]) * gscale;
-    float c = max_norm / (total + 1e-6f);
-    if (c > 1.0f) c = 1.0f;
-    coef *= c;
-  }
+  const float coef = grad_coef(gscale, sqnorm, max_norm);
   const float step = lr / bc1;
   if (!vec) {      // some buffer is not 16-byte aligned (free-standing parameters): scalar grid-stride loop
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -125,10 +124,7 @@ int launch_adam(float* p, const float* g, float* m, float* v, long long n, float
   long long grid = ((n >> 2) + 255) / 256;
   if (grid > kNumSMs * 8LL) grid = kNumSMs * 8LL;
   if (grid < 1) grid = 1;
-  if (step_dev != nullptr) {
-    MN_LAUNCH(k_inc_i32, 1, 1, 0, st, step_dev);
-    MN_LAUNCH_CHECK();
-  }
+  if (step_dev != nullptr) MN_TRY(launch_inc_i32(step_dev, st));
   const int vec = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
                     reinterpret_cast<uintptr_t>(v)) & 15) == 0;
   MN_LAUNCH(k_adam, (int)grid, 256, 0, st, p, g, m, v, n, lr, beta1, beta2, eps, wd, bc1, sqrtf(bc2), gscale, sqnorm_or_null, max_norm, step_dev, vec);

@@ -124,6 +124,29 @@ int mapnet_adam_step_dev(float* p, const float* g, float* exp_avg, float* exp_av
                      sqnorm, max_norm, step_counter, (cudaStream_t)stream);
 }
 
+int mapnet_sgd_step_dev(float* p, const float* g, float* momentum_buf, int64_t n, const float* lr_dev, float momentum,
+                        double dampening, float weight_decay, int nesterov, int32_t* step_counter, float grad_scale,
+                        const float* sqnorm, float max_norm, void* stream) {
+  MN_CHECK(p && g && lr_dev && n > 0, "sgd_step_dev: bad argument");
+  MN_CHECK((momentum_buf != nullptr) == (momentum != 0.f), "sgd_step_dev: momentum_buf must be given exactly when "
+           "momentum != 0 (momentum %g)", (double)momentum);
+  MN_CHECK(momentum_buf == nullptr || step_counter != nullptr, "sgd_step_dev: momentum needs the step counter");
+  MN_CHECK(!nesterov || (momentum > 0.f && dampening == 0.0), "sgd_step_dev: nesterov needs momentum > 0 and "
+           "zero dampening");
+  return launch_sgd(p, g, momentum_buf, n, lr_dev, momentum, dampening, weight_decay, nesterov, step_counter,
+                    grad_scale, sqnorm, max_norm, (cudaStream_t)stream);
+}
+
+int mapnet_rmsprop_step_dev(float* p, const float* g, float* square_avg, float* grad_avg, float* momentum_buf,
+                            int64_t n, const float* lr_dev, double alpha, float eps, float weight_decay, float momentum,
+                            int32_t* step_counter, float grad_scale, const float* sqnorm, float max_norm, void* stream) {
+  MN_CHECK(p && g && square_avg && lr_dev && n > 0, "rmsprop_step_dev: bad argument");
+  MN_CHECK((momentum_buf != nullptr) == (momentum > 0.f), "rmsprop_step_dev: momentum_buf must be given exactly when "
+           "momentum > 0 (momentum %g)", (double)momentum);
+  return launch_rmsprop(p, g, square_avg, grad_avg, momentum_buf, n, lr_dev, alpha, eps, weight_decay, momentum,
+                        step_counter, grad_scale, sqnorm, max_norm, (cudaStream_t)stream);
+}
+
 unsigned long long mapnet_launch_count(void) { return g_launch_count; }
 
 int mapnet_profile(mapnet_trunk_t* h, int enable) {

@@ -166,5 +166,31 @@ int launch_sqnorm(const float* g, long long n, float* partials, float* out_sq, c
 int launch_adam(float* p, const float* g, float* m, float* v, long long n, float lr, float beta1, float beta2,
                 float eps, float wd, float bc1, float bc2, float gscale, const float* sqnorm_or_null,
                 float max_norm, int* step_dev, cudaStream_t st);
+int launch_inc_i32(int* c, cudaStream_t st);    // *c += 1 on the device (optimizer step counters)
+
+// Factor every optimizer kernel applies to the raw gradient: gscale (1/world after a sum-allreduce), times
+// clip_grad_norm_'s coefficient max_norm / (total_norm + 1e-6) clamped to 1 when sqnorm (the squared norm of the
+// unscaled gradient, launch_sqnorm) is given.
+__device__ __forceinline__ float grad_coef(float gscale, const float* __restrict__ sqnorm, float max_norm) {
+  float coef = gscale;
+  if (sqnorm != nullptr) {
+    const float total = sqrtf(sqnorm[0]) * gscale;
+    float c = max_norm / (total + 1e-6f);
+    if (c > 1.0f) c = 1.0f;
+    coef *= c;
+  }
+  return coef;
+}
+
+// ---- optim.cu ------------------------------------------------------------------
+// SGD / RMSprop on flat buffers; lr_dev is a device float (CUDA-graph capturable rate).  NULL state buffers select
+// the variant: no momentum buffer <=> momentum 0, grad_avg <=> centered RMSprop.  step_dev (SGD with momentum:
+// required) is incremented first; SGD's step 1 initialises the momentum buffer with the update direction.
+int launch_sgd(float* p, const float* g, float* buf, long long n, const float* lr_dev, float momentum,
+               double dampening, float wd, int nesterov, int* step_dev, float gscale, const float* sqnorm_or_null,
+               float max_norm, cudaStream_t st);
+int launch_rmsprop(float* p, const float* g, float* square_avg, float* grad_avg, float* buf, long long n,
+                   const float* lr_dev, double alpha, float eps, float wd, float momentum, int* step_dev, float gscale,
+                   const float* sqnorm_or_null, float max_norm, cudaStream_t st);
 
 }  // namespace mapnet

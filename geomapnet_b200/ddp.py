@@ -72,6 +72,9 @@ class FlatDataParallel(object):
         scale = dp.allreduce_grads()                  # joins the side stream (+ the scalars); returns 1/world
         optimizer.learner.step(grad_scale=scale)
 
+    The step(grad_scale=...) call works with all three of the package's learners (Optimizer 'adam', 'sgd' and
+    'rmsprop': FusedAdam, FusedSGD, FusedRMSprop), which fold the 1/world scale into their fused update.
+
     overlap=False (default): one allreduce of the whole buffer inside allreduce_grads(); overlap=True: three slices
     reduced from the backward-part hook on a side stream (see the module docstring for what was measured).
     """

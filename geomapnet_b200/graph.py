@@ -2,7 +2,7 @@
 
 The step is ~200 short kernel launches; replaying it as two CUDA graphs removes the
 host launch cost and most of the inter-kernel gaps.  Graph 1 =
-forward + criterion + zero_grad + backward, graph 2 = [clip +] Adam.  Data parallel: the
+forward + criterion + zero_grad + backward, graph 2 = [clip +] the optimizer step (Adam, SGD or RMSprop).  Data parallel: the
 whole-buffer allreduce of FlatDataParallel sits between the two graphs (default).  With
 FlatDataParallel(overlap=True) the three slice allreduces issued from the backward-part hook
 are captured INSIDE graph 1, on a side stream that forks from and joins the capturing stream,
@@ -19,7 +19,9 @@ cudaErrorStreamCaptureImplicit (torch: "delete all references to the autograd gr
 
 Everything captured is the same product code that runs eagerly (the reference-facing
 modules and the C ABI underneath); counters that change per step (Adam bias
-correction, dropout offset) live in device memory so replays stay correct.
+correction, SGD's first step, dropout offset) live in device memory so replays stay correct,
+and so does the SGD / RMSprop learning rate: a schedule (Optimizer.adjust_lr / mult_lr) changes
+param_groups on the host, and each call writes a changed rate to the device before graph 2 replays.
 """
 import torch
 
@@ -82,25 +84,23 @@ class GraphedTrainStep(object):
             cd = self.criterion.state_dict()
             for k, v in snap["crit"].items():
                 cd[k].copy_(v)
+            # every tensor of the optimizer state (Adam moments, SGD / RMSprop momentum buffers, square_avg,
+            # grad_avg, step): the snapshot's value, or zero for a slot the warm-up created
             for p, st in self.learner.state.items():
-                old = snap["opt"].get(p)
-                for k in ("exp_avg", "exp_avg_sq"):
-                    if k in st:
-                        if old is not None and k in old:
-                            st[k].copy_(old[k])
+                old = snap["opt"].get(p) or {}
+                for k, v in st.items():
+                    if torch.is_tensor(v):
+                        if torch.is_tensor(old.get(k)):
+                            v.copy_(old[k])
                         else:
-                            st[k].zero_()
+                            v.zero_()
             if hasattr(self.learner, "_runs"):
+                # the fused learners' device step counters and their host mirrors
                 for key, runs in self.learner._runs.values():
                     for r in runs:
-                        p0 = r["params"][0]
-                        old = snap["opt"].get(p0)
-                        step0 = int(float(old["step"])) if (old is not None and "step" in old) else 0
-                        r["step_host"] = step0
+                        step0 = self.learner._host_step(snap["opt"].get(r["params"][0]) or {})
+                        self.learner._set_host_step(r, step0)
                         r["step_dev"].fill_(step0)
-                        t = torch.tensor(float(step0))
-                        for p in r["params"]:
-                            self.learner.state[p]["step"] = t
         torch.cuda.synchronize()
 
     def _fwd_bwd(self):
@@ -127,6 +127,8 @@ class GraphedTrainStep(object):
         self.g1.replay()
         if self.dp is not None:
             self.dp.allreduce_grads(slices_in_graph=getattr(self.dp, "overlap", False))
+        if hasattr(self.learner, "sync_lr"):
+            self.learner.sync_lr()        # the captured SGD / RMSprop launches read the rate from device memory
         self.g2.replay()
         if hasattr(self.learner, "advance_host_step"):
             self.learner.advance_host_step(1)

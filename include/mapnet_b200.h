@@ -13,6 +13,7 @@
  *   common/criterion.py:42-52,76-109,137-184          mapnet_loss_fwd_bwd
  *   common/pose_utils.py:234-260 calc_vos*            mapnet_loss_fwd_bwd (folded in)
  *   common/optimizer.py:21-23 + train.py:357-359      mapnet_adam_step (+ mapnet_sqnorm)
+ *   common/optimizer.py:16-27 (sgd, rmsprop)          mapnet_sgd_step_dev / mapnet_rmsprop_step_dev
  *   models/posenet.py:37-63  parameter layout         mapnet_param_count / mapnet_param_info
  *
  * Conventions: every pointer is a DEVICE pointer unless named host_*; all
@@ -116,6 +117,19 @@ int mapnet_adam_step(float* p, const float* g, float* exp_avg, float* exp_avg_sq
 int mapnet_adam_step_dev(float* p, const float* g, float* exp_avg, float* exp_avg_sq, int64_t n, float lr,
                          float beta1, float beta2, float eps, float weight_decay, int32_t* step_counter,
                          float grad_scale, const float* sqnorm, float max_norm, void* stream);
+
+/* torch.optim.SGD / torch.optim.RMSprop semantics (L2 weight decay, maximize=False) on flat buffers, CUDA-graph
+ * capturable: the learning rate is read from the device float *lr_dev at run time (a schedule writes it between
+ * replays), and *step_counter (device int32, may be NULL unless an SGD momentum buffer is given) is incremented
+ * first -- SGD's step 1 sets momentum_buf = d instead of momentum*buf + (1-dampening)*d.  grad_scale, sqnorm and
+ * max_norm as for mapnet_adam_step.  State buffers a configuration does not use are NULL: momentum_buf exactly when
+ * momentum == 0, grad_avg unless RMSprop is centered.  (Added in ABI version 2, backward compatible.) */
+int mapnet_sgd_step_dev(float* p, const float* g, float* momentum_buf, int64_t n, const float* lr_dev, float momentum,
+                        double dampening, float weight_decay, int nesterov, int32_t* step_counter, float grad_scale,
+                        const float* sqnorm, float max_norm, void* stream);
+int mapnet_rmsprop_step_dev(float* p, const float* g, float* square_avg, float* grad_avg, float* momentum_buf,
+                            int64_t n, const float* lr_dev, double alpha, float eps, float weight_decay, float momentum,
+                            int32_t* step_counter, float grad_scale, const float* sqnorm, float max_norm, void* stream);
 
 /* ---- GPU-side input pipeline (SURVEY.md section 8 row f2; geomapnet_b200/csrc/preprocess.cu).
  * Replaces the per-image CPU transform stack of /root/reference/scripts/train.py:119-128 (and eval.py:97-101):
