@@ -99,6 +99,16 @@ def lib():
     L.mapnet_bench_conv.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_int, POINTER(c_float)]
     L.mapnet_bench_conv.restype = c_int
+    L.mapnet_test_conv_affine.argtypes = [c_int] * 8 + [c_void_p] * 5 + [c_int, c_void_p, c_void_p]
+    L.mapnet_test_conv_affine.restype = c_int
+    L.mapnet_infer_create.argtypes = [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int]
+    L.mapnet_infer_load.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p]
+    L.mapnet_infer_forward.argtypes = [c_void_p, c_void_p, c_int, c_float, c_uint64, c_uint64, c_void_p, c_void_p]
+    L.mapnet_infer_arena_bytes.argtypes = [c_int, c_int, c_int, c_int]
+    L.mapnet_infer_arena_bytes.restype = c_int64
+    L.mapnet_infer_destroy.argtypes = [c_void_p]
+    for name in ("mapnet_infer_create", "mapnet_infer_load", "mapnet_infer_forward", "mapnet_infer_destroy"):
+        getattr(L, name).restype = c_int
     for name in ("mapnet_trunk_create", "mapnet_trunk_destroy", "mapnet_param_count", "mapnet_param_info",
                  "mapnet_forward", "mapnet_backward", "mapnet_loss_fwd_bwd", "mapnet_sqnorm",
                  "mapnet_adam_step", "mapnet_test_conv"):
@@ -115,7 +125,9 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_test_dgrad_shortcut", "mapnet_test_plan_describe", "mapnet_preprocess_create",
             "mapnet_preprocess_output_size", "mapnet_preprocess_run", "mapnet_preprocess_destroy",
             "mapnet_backward_part", "mapnet_grad_part_range", "mapnet_preprocess_run_ex", "mapnet_test_conv_epilogue", "mapnet_pose_post", "mapnet_pgo_optimize",
-            "mapnet_sgd_step_dev", "mapnet_rmsprop_step_dev"]
+            "mapnet_sgd_step_dev", "mapnet_rmsprop_step_dev", "mapnet_test_conv_affine", "mapnet_infer_create",
+            "mapnet_infer_load", "mapnet_infer_forward", "mapnet_infer_arena_bytes", "mapnet_infer_destroy"]
+UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 
 
 def check(rc, what):
@@ -169,6 +181,35 @@ class Trunk(object):
     def close(self):
         if self.h:
             lib().mapnet_trunk_destroy(self.h)
+            self.h = c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class Infer(object):
+    """Owns one mapnet_infer_t handle (the eval-mode inference engine of one (max_B, H, W))."""
+
+    def __init__(self, max_B, H, W, feat_dim, precision):
+        self.h = c_void_p()
+        self.max_B, self.H, self.W, self.feat_dim, self.precision = max_B, H, W, feat_dim, precision
+        check(lib().mapnet_infer_create(ctypes.byref(self.h), max_B, H, W, feat_dim, PREC[precision]),
+              "mapnet_infer_create")
+
+    def load(self, params_flat, bufs_flat):
+        check(lib().mapnet_infer_load(self.h, params_flat.data_ptr(), bufs_flat.data_ptr(), stream_ptr()),
+              "mapnet_infer_load")
+
+    def forward(self, x, pred, droprate, seed, step=UINT64_MAX):
+        check(lib().mapnet_infer_forward(self.h, x.data_ptr(), x.shape[0], float(droprate), int(seed), int(step),
+                                         pred.data_ptr(), stream_ptr()), "mapnet_infer_forward")
+
+    def close(self):
+        if self.h:
+            lib().mapnet_infer_destroy(self.h)
             self.h = c_void_p()
 
     def __del__(self):

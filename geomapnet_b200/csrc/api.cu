@@ -5,10 +5,12 @@
 
 #include "../../include/mapnet_b200.h"
 #include "net.h"
+#include "infer.h"
 
 using namespace mapnet;
 
 struct mapnet_trunk { Net net; };
+struct mapnet_infer { InferNet net; };
 
 extern "C" {
 
@@ -338,6 +340,119 @@ int mapnet_test_stem(int B, int H, int W, const float* x_nchw, const float* w_oi
   if (pw) tc_plan_destroy(pw);
   cudaFree(S); cudaFree(wk); cudaFree(dwk); cudaFree(d_wd);
   return r;
+}
+
+// One wgmma fprop launch with the inference epilogue (conv_tc.cu, EPI_AFFINE): out = relu?(conv * scale + shift
+// [+ residual]).  flags: bit 0 ReLU, bit 1 (strict mode) residual in hi/lo plane form, bit 2 (strict mode) output in
+// hi/lo plane form.  k == 7: the stem as the engine runs it (in0 = fp32 NCHW image, wmat = fp32 [Co][3][7][7]).
+// Otherwise bf16 mode: in0 / residual / out bf16 NHWC, wmat bf16 [Co][k][k][Ci]; strict mode: fp32 NHWC in0 / residual
+// and fp32 [Co][k][k][Ci] wmat, cut into fp16 hi/lo planes here (the engine's operands are stored in that form).
+int mapnet_test_conv_affine(int precision, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* in0,
+                            const void* wmat, const float* scale, const float* shift, const void* residual, int flags,
+                            void* out, void* stream) {
+  MN_CHECK(precision == PREC_BF16_TC || precision == PREC_TC_SPLIT, "test_conv_affine: precision %d is not supported "
+           "(bf16 = %d or tc_split = %d)", precision, PREC_BF16_TC, PREC_TC_SPLIT);
+  MN_CHECK(in0 && wmat && scale && shift && out && B >= 1, "test_conv_affine: bad argument");
+  MN_CHECK(k != 7 || (Ci == 3 && Co == 64 && stride == 2 && residual == nullptr), "test_conv_affine: the stem is 7x7/s2, 3 -> 64, no residual");
+  MN_TRY(require_device());
+  const bool sp = precision == PREC_TC_SPLIT;
+  EpiAffine a;
+  a.scale = scale; a.shift = shift; a.relu = flags & 1; a.res_split = (flags >> 1) & 1; a.out_split = (flags >> 2) & 1;
+  MN_CHECK(tc_affine_supported(sp, residual != nullptr, a), "test_conv_affine: epilogue variant not built (flags %d, "
+           "residual %d)", flags, residual != nullptr);
+  cudaStream_t st = (cudaStream_t)stream;
+  ConvGeom g; WeightDesc wd; memset(&wd, 0, sizeof(wd));
+  if (k == 7) {
+    stem_s2d_geometry(Hi, Wi, 64, &g, &wd, sp ? 4 : 2);
+    MN_CHECK(tc_overlapped_view_supported(), "test_conv_affine: the driver rejects overlapped tensor maps");
+  } else {
+    g.Hi = Hi; g.Wi = Wi; g.Ci = Ci; g.Co = Co; g.KH = g.KW = k; g.stride = stride; g.pad = (k - 1) / 2;
+    g.Ho = (Hi + 2 * g.pad - k) / stride + 1; g.Wo = (Wi + 2 * g.pad - k) / stride + 1;
+  }
+  g.B = B;
+  if (sp) { g.split = 1; g.fmt_z = 0; g.fmt_g = 0; }
+  const long long n_out = (long long)B * g.Ho * g.Wo * Co;
+  void *x = nullptr, *w = nullptr, *r = nullptr, *f32 = nullptr; WeightDesc* d_wd = nullptr;
+  TcConvPlan* plan = nullptr;
+  auto body = [&]() -> int {
+    const void* xin = in0; const void* win = wmat; const void* rin = residual;
+    if (k == 7) {
+      const int Wsp = stem_s2d_wsp(g.Wo);
+      MN_CUDA(cudaMalloc(&x, (size_t)B * g.Hi * Wsp * 16 * (sp ? 4 : 2)));
+      MN_CUDA(cudaMalloc(&w, (size_t)64 * 256 * (sp ? 8 : 2)));
+      MN_CUDA(cudaMalloc((void**)&d_wd, sizeof(WeightDesc)));
+      MN_CUDA(cudaMemcpyAsync(d_wd, &wd, sizeof(wd), cudaMemcpyHostToDevice, st));
+      if (sp) {
+        MN_CUDA(cudaMalloc(&f32, (size_t)64 * 256 * 4));
+        MN_TRY(launch_stem_s2d<hsplit>((const float*)in0, (hsplit*)x, B, Hi, Wi, g.Hi, Wsp, st));
+        MN_TRY(launch_pack_weights_split(d_wd, 1, (const float*)wmat, (float*)f32, nullptr, w, nullptr, 64 * 256, 0, 0, st));
+      } else {
+        MN_TRY(launch_stem_s2d<bf16>((const float*)in0, (bf16*)x, B, Hi, Wi, g.Hi, Wsp, st));
+        MN_TRY(launch_pack_weights<bf16>(d_wd, 1, (const float*)wmat, (bf16*)w, nullptr, 64 * 256, 0, st));
+      }
+      xin = x; win = w;
+    } else if (sp) {
+      const long long n_in = (long long)B * Hi * Wi * Ci;
+      MN_CUDA(cudaMalloc(&x, (size_t)n_in * 4));
+      MN_TRY(launch_split_tensor((const float*)in0, x, n_in, 0, st));
+      MN_CUDA(cudaMalloc(&w, (size_t)Co * k * k * Ci * 8));
+      MN_TRY(launch_split_weight_matrix((const float*)wmat, w, Co, k * k, Ci, 0, st));
+      if (residual != nullptr && a.res_split) {
+        MN_CUDA(cudaMalloc(&r, (size_t)n_out * 4));
+        MN_TRY(launch_split_tensor((const float*)residual, r, n_out, 0, st));
+        rin = r;
+      }
+      xin = x; win = w;
+    }
+    MN_TRY(tc_plan_create(&plan, g, 0, (const bf16*)win));
+    MN_TRY(tc_plan_set_cluster(plan, 1));
+    MN_TRY(tc_conv_run(plan, (const bf16*)xin, nullptr, (const bf16*)rin, out, st, nullptr, nullptr, nullptr, &a));
+    MN_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  };
+  const int rc = body();
+  if (plan) tc_plan_destroy(plan);
+  cudaFree(x); cudaFree(w); cudaFree(r); cudaFree(f32); cudaFree(d_wd);
+  return rc;
+}
+
+// ---- eval-mode inference engine (infer.cu) ----
+int64_t mapnet_infer_arena_bytes(int max_B, int H, int W, int precision) {
+  return InferNet::arena_bytes(max_B, H, W, precision);
+}
+
+int mapnet_infer_create(mapnet_infer_t** out, int max_B, int H, int W, int feat_dim, int precision) {
+  MN_CHECK(out != nullptr, "infer_create: null out pointer");
+  *out = nullptr;
+  // argument errors first: nothing is allocated or launched for a call that cannot succeed
+  MN_CHECK(precision == PREC_BF16_TC || precision == PREC_TC_SPLIT, "infer_create: precision %d is not supported "
+           "(bf16 = %d or tc_split = %d)", precision, PREC_BF16_TC, PREC_TC_SPLIT);
+  MN_CHECK(max_B >= 1 && H >= 32 && W >= 32, "infer_create: need max_B >= 1 and H, W >= 32 (got %d, %d, %d)", max_B, H, W);
+  MN_CHECK(feat_dim >= 8 && feat_dim % 4 == 0, "infer_create: feat_dim must be a multiple of 4");
+  MN_TRY(require_device());
+  mapnet_infer* h = new mapnet_infer();
+  int r = h->net.init(max_B, H, W, feat_dim, precision);
+  if (r != 0) { h->net.destroy(); delete h; return r; }
+  *out = h;
+  return 0;
+}
+
+int mapnet_infer_load(mapnet_infer_t* h, const float* params_flat, const float* bufs_flat, void* stream) {
+  MN_CHECK(h != nullptr, "infer_load: null handle");
+  return h->net.load(params_flat, bufs_flat, (cudaStream_t)stream);
+}
+
+int mapnet_infer_forward(mapnet_infer_t* h, const float* x, int B, float droprate, uint64_t seed, uint64_t step,
+                         float* pred, void* stream) {
+  MN_CHECK(h != nullptr, "infer_forward: null handle");
+  return h->net.forward(x, B, droprate, seed, step, pred, (cudaStream_t)stream);
+}
+
+int mapnet_infer_destroy(mapnet_infer_t* h) {
+  if (h == nullptr) return 0;
+  h->net.destroy();
+  delete h;
+  return 0;
 }
 
 // micro-benchmark of one wgmma conv launch configuration (plan built once, CUDA-event timing)

@@ -564,7 +564,7 @@ k_stem_pool(const T* __restrict__ y, const float* __restrict__ scale, const floa
     uint2 packed;
     packed.x = (uint32_t)bi[0] | ((uint32_t)bi[1] << 8) | ((uint32_t)bi[2] << 16) | ((uint32_t)bi[3] << 24);
     packed.y = (uint32_t)bi[4] | ((uint32_t)bi[5] << 8) | ((uint32_t)bi[6] << 16) | ((uint32_t)bi[7] << 24);
-    *reinterpret_cast<uint2*>(amax + (size_t)i * 8) = packed;
+    if (amax != nullptr) *reinterpret_cast<uint2*>(amax + (size_t)i * 8) = packed;
   }
 }
 

@@ -226,6 +226,11 @@ enum : int {
   EPI_ZMASK = 8,    // gate = zmask > 0
   EPI_YD = 16,      // third sum over the downsample-branch BN input
   EPI_OUT32 = 32,   // strict mode: fp32 output and residual (combines with EPI_RES / EPI_STATS only)
+  // eval-mode inference (fprop, never with EPI_STATS / EPI_BWD): f = acc*s[c] + t[c] (+ residual) (ReLU), one rounding
+  EPI_AFFINE = 64,
+  EPI_RELU = 128,   // with EPI_AFFINE
+  EPI_HOUT = 256,   // with EPI_OUT32: store fp16 hi/lo planes (common.cuh: hsplit) instead of fp32
+  EPI_HRES = 512,   // with EPI_OUT32 | EPI_RES: the residual is in hi/lo plane form
 };
 
 struct EpiRegs { uint4 r[4], y[4], z[4], d[4]; };
@@ -339,9 +344,9 @@ __device__ __forceinline__ void epi_chunk(const float* __restrict__ scr, const E
     lo[i] = src[0]; hi[i] = src[1];
   }
   float msc[8], msh[8];
-  if ((F & EPI_BWD) && !(F & EPI_ZMASK)) {
-    const float4* a = reinterpret_cast<const float4*>(E.mscale + col0 + 8 * p);
-    const float4* b = reinterpret_cast<const float4*>(E.mshift + col0 + 8 * p);
+  if (((F & EPI_BWD) && !(F & EPI_ZMASK)) || (F & EPI_AFFINE)) {
+    const float4* a = reinterpret_cast<const float4*>(((F & EPI_AFFINE) ? E.ascale : E.mscale) + col0 + 8 * p);
+    const float4* b = reinterpret_cast<const float4*>(((F & EPI_AFFINE) ? E.ashift : E.mshift) + col0 + 8 * p);
     const float4 a0 = __ldg(a), a1 = __ldg(a + 1), b0 = __ldg(b), b1 = __ldg(b + 1);
     msc[0] = a0.x; msc[1] = a0.y; msc[2] = a0.z; msc[3] = a0.w; msc[4] = a1.x; msc[5] = a1.y; msc[6] = a1.z; msc[7] = a1.w;
     msh[0] = b0.x; msh[1] = b0.y; msh[2] = b0.z; msh[3] = b0.w; msh[4] = b1.x; msh[5] = b1.y; msh[6] = b1.z; msh[7] = b1.w;
@@ -359,7 +364,19 @@ __device__ __forceinline__ void epi_chunk(const float* __restrict__ scr, const E
 #pragma unroll
       for (int k = 0; k < 8; ++k) f[k] *= osc;
     }
-    if ((F & EPI_RES) && (F & EPI_OUT32)) {
+    if (F & EPI_AFFINE) {        // the same expression as k_bn_apply's, on the fp32 accumulator
+#pragma unroll
+      for (int k = 0; k < 8; ++k) f[k] = f[k] * msc[k] + msh[k];
+    }
+    if ((F & EPI_RES) && (F & EPI_HRES)) {       // hi planes in the r slot, lo planes in the y slot (Vec8<hsplit>::load)
+      const __half2* h = reinterpret_cast<const __half2*>(&G.r[i]);
+      const __half2* l = reinterpret_cast<const __half2*>(&G.y[i]);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float2 fh = __half22float2(h[k]), fl = __half22float2(l[k]);
+        f[2 * k] += fh.x + fl.x; f[2 * k + 1] += fh.y + fl.y;
+      }
+    } else if ((F & EPI_RES) && (F & EPI_OUT32)) {
       const float4 r0 = *reinterpret_cast<const float4*>(&G.r[i]), r1 = *reinterpret_cast<const float4*>(&G.y[i]);
       f[0] += r0.x; f[1] += r0.y; f[2] += r0.z; f[3] += r0.w; f[4] += r1.x; f[5] += r1.y; f[6] += r1.z; f[7] += r1.w;
     } else if (F & EPI_RES) {
@@ -380,8 +397,22 @@ __device__ __forceinline__ void epi_chunk(const float* __restrict__ scr, const E
         for (int k = 0; k < 8; ++k) f[k] = (yv[k] * msc[k] + msh[k] > 0.f) ? f[k] : 0.f;
       }
     }
+    if (F & EPI_RELU) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) f[k] = fmaxf(f[k], 0.f);
+    }
     uint4 o;
-    if (F & EPI_OUT32) {
+    if (F & EPI_HOUT) {          // 8 hi then 8 lo fp16 values: the operand form the next conv reads
+      if (rstore[i]) {
+        uint4 a, b;
+        __half* h = reinterpret_cast<__half*>(&a);
+        __half* l = reinterpret_cast<__half*>(&b);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) split_f16(f[k], h[k], l[k]);
+        uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<float*>(out) + rowoff[i] + coff + 8 * p);
+        op[0] = a; op[1] = b;
+      }
+    } else if (F & EPI_OUT32) {
       if (rstore[i]) {
         float* op = reinterpret_cast<float*>(out) + rowoff[i] + coff + 8 * p;
         *reinterpret_cast<float4*>(op) = make_float4(f[0], f[1], f[2], f[3]);
@@ -445,13 +476,30 @@ __device__ __forceinline__ void epi_tile(const float* __restrict__ rows, float (
 }
 
 // launch-uniform dispatch over the variants the network uses
-template <int BN>
+template <int BN, bool AFF>
 __device__ __forceinline__ void epi_tile_dispatch(const int mode, const float* __restrict__ rows,
                                                   float (*stw)[BN / 32][32], const long long (&rowoff)[4],
                                                   const bool (&rvalid)[4], const bool do_store, const int tn,
                                                   const bf16* residual, bf16* out, const EpiBwd& E, const int lane,
                                                   const int half) {
 #define MN_EPI_CASE(Fv) case (Fv): epi_tile<(Fv), BN>(rows, stw, rowoff, rvalid, do_store, tn, residual, out, E, lane, half); break;
+  if constexpr (AFF) {
+    // eval-mode inference, its own kernel instantiations (k_tc_conv<BN, CL, true>) so that the training kernels keep
+    // their register allocation: stem / conv1 (ReLU), downsample (no ReLU), conv2 (+ block input or downsample
+    // output, ReLU)
+    switch (mode) {
+      MN_EPI_CASE(EPI_AFFINE | EPI_RELU)
+      MN_EPI_CASE(EPI_AFFINE)
+      MN_EPI_CASE(EPI_AFFINE | EPI_RES | EPI_RELU)
+      MN_EPI_CASE(EPI_OUT32 | EPI_AFFINE | EPI_RELU)
+      MN_EPI_CASE(EPI_OUT32 | EPI_AFFINE | EPI_RELU | EPI_HOUT)
+      MN_EPI_CASE(EPI_OUT32 | EPI_AFFINE)
+      MN_EPI_CASE(EPI_OUT32 | EPI_AFFINE | EPI_RES | EPI_RELU | EPI_HOUT)
+      MN_EPI_CASE(EPI_OUT32 | EPI_AFFINE | EPI_RES | EPI_HRES | EPI_RELU | EPI_HOUT)
+      default: __trap();
+    }
+    return;
+  }
   switch (mode) {
     MN_EPI_CASE(0)
     MN_EPI_CASE(EPI_RES)
@@ -470,10 +518,34 @@ __device__ __forceinline__ void epi_tile_dispatch(const int mode, const float* _
 #undef MN_EPI_CASE
 }
 
+// the affine epilogue bits of a launch (host and device): what tc_affine_supported checks and epi_mode_of dispatches on
+__host__ __device__ __forceinline__ int affine_mode(const bool split, const bool residual, const int relu, const int res_split,
+                                                   const int out_split) {
+  int m = EPI_AFFINE | (residual ? EPI_RES : 0) | (relu ? EPI_RELU : 0);
+  if (split) m |= EPI_OUT32 | (out_split ? EPI_HOUT : 0) | ((residual && res_split) ? EPI_HRES : 0);
+  return m;
+}
+
+bool tc_affine_supported(bool split, bool residual, const EpiAffine& a) {
+  if (a.scale == nullptr || a.shift == nullptr) return false;
+  if (!split && (a.res_split || a.out_split)) return false;
+  static const int built[] = {
+      EPI_AFFINE | EPI_RELU, EPI_AFFINE, EPI_AFFINE | EPI_RES | EPI_RELU, EPI_OUT32 | EPI_AFFINE | EPI_RELU,
+      EPI_OUT32 | EPI_AFFINE | EPI_RELU | EPI_HOUT, EPI_OUT32 | EPI_AFFINE,
+      EPI_OUT32 | EPI_AFFINE | EPI_RES | EPI_RELU | EPI_HOUT,
+      EPI_OUT32 | EPI_AFFINE | EPI_RES | EPI_HRES | EPI_RELU | EPI_HOUT};
+  const int m = affine_mode(split, residual, a.relu, a.res_split, a.out_split);
+  for (int b : built) if (b == m) return true;
+  return false;
+}
+
+template <bool AFF>
 __device__ __forceinline__ int epi_mode_of(const bf16* residual, const double* stats, const EpiBwd& E, const int out32) {
   int m = (residual != nullptr) ? EPI_RES : 0;
   if (out32) m |= EPI_OUT32;
-  if (E.y != nullptr) {
+  if (AFF) {
+    m |= EPI_AFFINE | E.aflags;
+  } else if (E.y != nullptr) {
     m |= EPI_BWD;
     if (E.zmask != nullptr) m |= EPI_ZMASK;
     if (E.yd != nullptr) m |= EPI_YD;
@@ -599,7 +671,8 @@ __device__ __forceinline__ void mma_tile(float (&d)[BN / 2], const int kblocks, 
 // CL = thread-block cluster size along M: the CL CTAs of a cluster work on CL consecutive
 // M tiles of the same N tile and share the weight tile -- each loads 1/CL of it and TMA-
 // multicasts it to all (cuts the B traffic from L2 by CL).
-template <int BN, int CL>
+// AFF: the eval-mode inference epilogues (EPI_AFFINE) instead of the training ones.
+template <int BN, int CL, bool AFF>
 __global__ void __launch_bounds__(kConvThreads, 1)
 k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
           const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapA3,
@@ -684,7 +757,7 @@ k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
     const int half = wq & 1;                // which of the quarter's chunk subsets
     const bool arriver = (threadIdx.x & 127) == 0;
     float* stg = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)) + STAGES * STAGE_BYTES);
-    const int epi_mode = epi_mode_of(residual, stats, E, P.out32);
+    const int epi_mode = epi_mode_of<AFF>(residual, stats, E, P.out32);
     constexpr uint64_t DESC_BASE = make_smem_desc_base(16, 1024);
     int stage = 0; uint32_t phase = 0;
     // running column sums of this warp, [statistic][chunk][lane] (lane <-> column epi_stat_col(lane)); kept in
@@ -733,7 +806,7 @@ k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
       wg_bar(wg);                             // the previous tile's staged rows have been read
       acc_to_stage<BN>(d, stg + wg * 64 * RS, wq, lane);
       wg_bar(wg);
-      epi_tile_dispatch<BN>(epi_mode, stg + q * 32 * RS, stw, rowoff, rvalid, P.debug != 4, tn, residual, out, E, lane,
+      epi_tile_dispatch<BN, AFF>(epi_mode, stg + q * 32 * RS, stw, rowoff, rvalid, P.debug != 4, tn, residual, out, E, lane,
                             half);
     }
     if (stats != nullptr && st_tn >= 0) flush_stats(st_tn);
@@ -927,7 +1000,8 @@ struct TcConvPlan {
   // cached pointers the maps were encoded for
   const void *c_in0, *c_in1;
   bool smem_attr_set;
-  const float* out_scale;               // strict mode dgrad / wgrad: device scalar applied to the accumulators, or null
+  bool smem_attr_aff;                   // ... for the inference (EPI_AFFINE) instantiation of the fprop kernel
+  const float* out_scale;              // strict mode dgrad / wgrad: device scalar applied to the accumulators, or null
   float* ws;                            // wgrad with split-K: per-split dW slices (allocated at the first run)
 };
 
@@ -1005,7 +1079,7 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
   MN_CHECK(g.in_pix_stride == 0 || (g.stride == 1 && kind != 1), "tc conv: strided input views only for stride-1 fprop / wgrad");
   TcConvPlan* p = new TcConvPlan();
   p->g = g; p->kind = kind; p->wmat = wmat; p->wmat2 = nullptr; p->shortcut_flops_k = 0;
-  p->c_in0 = p->c_in1 = nullptr; p->smem_attr_set = false; p->out_scale = nullptr; p->ws = nullptr;
+  p->c_in0 = p->c_in1 = nullptr; p->smem_attr_set = false; p->smem_attr_aff = false; p->out_scale = nullptr; p->ws = nullptr;
   p->CL = pick_cl();
   const int s = g.stride, pad = g.pad, KK = g.KH * g.KW;
   // strict mode: the engines see 2*C 16-bit channels per pixel and every filter tap twice (hi / lo weight planes)
@@ -1165,6 +1239,12 @@ void tc_plan_destroy(TcConvPlan* p) {
   delete p;
 }
 void tc_plan_set_out_scale(TcConvPlan* p, const float* inv_scale) { if (p != nullptr) p->out_scale = inv_scale; }
+int tc_plan_set_cluster(TcConvPlan* p, int cl) {
+  MN_CHECK(p != nullptr && p->kind == 0 && (cl == 1 || cl == 2 || cl == 4), "tc_plan_set_cluster: bad argument");
+  p->CL = cl;
+  p->c_in0 = p->c_in1 = nullptr;        // the weight maps' box depends on CL: encode again at the next run
+  return 0;
+}
 
 // Fold the dgrad of the block's 1x1 / stride-2 downsample conv into the (merged) dgrad of its 3x3 / stride-2 conv1:
 // both produce d(block input), the shortcut only reaches the pixel class (0, 0), where it is one more filter tap
@@ -1263,8 +1343,15 @@ static int encode_view(CUtensorMap* m, const bf16* base, int N, int Hd, int Wd, 
 }
 
 int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* residual, void* out, cudaStream_t st,
-                double* stats, const EpiBwd* bwd, const EpiFin* fin) {
+                double* stats, const EpiBwd* bwd, const EpiFin* fin, const EpiAffine* aff) {
   MN_CHECK(p != nullptr, "tc_conv_run: null plan");
+  if (aff != nullptr) {
+    MN_CHECK(p->kind == 0 && stats == nullptr && bwd == nullptr && (fin == nullptr || fin->mode == 0),
+             "tc_conv_run: the affine (inference) epilogue is an fprop epilogue without statistics");
+    MN_CHECK(tc_affine_supported(p->g.split != 0, residual != nullptr, *aff),
+             "tc_conv_run: affine epilogue variant not built (split %d residual %d relu %d res_split %d out_split %d)",
+             p->g.split, residual != nullptr, aff->relu, aff->res_split, aff->out_split);
+  }
   EpiFin F; memset(&F, 0, sizeof(F));
   if (fin != nullptr && fin->mode != 0) {
     MN_CHECK(stats != nullptr && fin->counter != nullptr && p->kind != 2, "tc_conv_run: fused finalize needs statistics accumulators");
@@ -1282,6 +1369,11 @@ int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* res
   }
   MN_CHECK(!p->g.split || bwd == nullptr, "tc_conv_run: the fused BatchNorm-backward epilogue is a bf16-mode feature");
   E.oscale = p->out_scale;
+  if (aff != nullptr) {
+    E.ascale = aff->scale; E.ashift = aff->shift;
+    E.aflags = affine_mode(p->g.split != 0, residual != nullptr, aff->relu, aff->res_split, aff->out_split) &
+               (EPI_RELU | EPI_HOUT | EPI_HRES);
+  }
   const ConvGeom& g = p->g;
   const int SP = g.split ? 2 : 1;
   const int nsm = kNumSMs;
@@ -1309,13 +1401,18 @@ int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* res
     }
     const size_t smem = conv_smem_bytes(p->BN);
     void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, ConvParams, const bf16*, bf16*, double*, EpiBwd, EpiFin) = nullptr;
-#define PICK(BNv, CLv) if (p->BN == BNv && p->CL == CLv) kern = k_tc_conv<BNv, CLv>;
-    PICK(64, 1) PICK(128, 1) PICK(64, 2) PICK(128, 2) PICK(64, 4) PICK(128, 4)
+#define PICK(BNv, CLv) if (p->BN == BNv && p->CL == CLv) kern = k_tc_conv<BNv, CLv, false>;
+    if (aff != nullptr) {       // inference plans run unclustered (tc_plan_set_cluster)
+      if (p->CL == 1) kern = (p->BN == 64) ? k_tc_conv<64, 1, true> : k_tc_conv<128, 1, true>;
+    } else {
+      PICK(64, 1) PICK(128, 1) PICK(64, 2) PICK(128, 2) PICK(64, 4) PICK(128, 4)
+    }
 #undef PICK
-    MN_CHECK(kern != nullptr, "tc conv: no kernel for BN=%d CL=%d", p->BN, p->CL);
-    if (!p->smem_attr_set) {
+    MN_CHECK(kern != nullptr, "tc conv: no %s kernel for BN=%d CL=%d", aff ? "inference" : "training", p->BN, p->CL);
+    if (!p->smem_attr_set || p->smem_attr_aff != (aff != nullptr)) {
       MN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
       p->smem_attr_set = true;
+      p->smem_attr_aff = (aff != nullptr);
     }
     F.expected = 0;
     for (auto& L : p->launches) {     // the sums of a stride-2 dgrad come from all its parity classes / launches

@@ -38,6 +38,7 @@ int launch_bn_apply(const T* y, const float* scale, const float* shift, int res_
                     const float* scale2, const float* shift2, TZ* z, long long M, int C, int relu, cudaStream_t st,
                     const BnLazy* lazy = nullptr, const BnLazy* lazy2 = nullptr);
 // lazy (/ lazy2 for the downsample BN): the kernel finalizes the batch statistics itself (bn_fin.cuh, BnLazy)
+// amax == nullptr: the argmax positions are not stored (eval-mode inference: no backward follows)
 template <typename T, typename TZ>
 int launch_stem_pool(const T* y, const float* scale, const float* shift, TZ* z, uint8_t* amax, int B, int H,
                      int W, int Ho, int Wo, int C, cudaStream_t st, const BnLazy* lazy = nullptr);
@@ -73,6 +74,8 @@ int tc_plan_launches(const TcConvPlan* p);
 // dgrad / wgrad plans: multiply the accumulators by the device scalar *inv_scale before they are added to the residual /
 // the wgrad buffer (strict mode: the gradient operand planes carry a per-step power-of-two scale)
 void tc_plan_set_out_scale(TcConvPlan* p, const float* inv_scale);
+// fprop plans: thread-block cluster size (default MAPNET_TC_CLUSTER or 1); the inference epilogues are built for 1 only
+int tc_plan_set_cluster(TcConvPlan* p, int cl);
 int tc_plan_describe(const TcConvPlan* p, char* buf, int cap);      // JSON, host-only (CPU tests of the plan arithmetic)
 // fprop: in0 = x, out = y (bf16);  dgrad: in0 = dy [, in1 = the folded shortcut's dy], out = dx (bf16);
 // wgrad: in0 = x, in1 = dy, out = fp32 dW (accumulated)
@@ -88,12 +91,30 @@ struct EpiBwd {
   const float* mscale;  // gate recomputed from y when zmask is null
   const float* mshift;
   const float* oscale;  // strict mode (fp32 output): device scalar multiplied into the accumulators, or null (set by the plan)
+  // eval-mode inference (fprop only, set from EpiAffine by tc_conv_run): f = acc * ascale[c] + ashift[c] in fp32 before
+  // the residual; aflags = the conv_tc.cu epilogue bits for ReLU and the hi/lo plane output / residual formats
+  const float* ascale;
+  const float* ashift;
+  int aflags;
 };
+// Inference epilogue of an fprop launch (a frozen BatchNorm folded in as a per-channel affine map):
+//   out = relu?( acc * scale[c] + shift[c] [+ residual] ), rounded once, at the store.
+// bf16 mode: residual and output bf16.  Strict mode (split plans): out_split = 1 stores the fp16 hi/lo plane form
+// (common.cuh: hsplit) the next conv reads as its operand, 0 stores fp32; res_split = 1 reads the residual in that plane
+// form (a block input), 0 as fp32 (a downsample branch's output).  Only the combinations the eval-mode ResNet schedule
+// uses are built (tc_affine_supported).
+struct EpiAffine {
+  const float* scale;
+  const float* shift;
+  int relu, res_split, out_split;
+};
+bool tc_affine_supported(bool split, bool residual, const EpiAffine& a);
 // fin != nullptr (with stats): the last CTA to flush its sums also finalizes them (bn_fin.cuh) -- forward:
 // mean / invstd / scale / shift / running statistics; backward: d gamma, d beta, dy coefficients
 struct EpiFin;
 int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* residual, void* out, cudaStream_t st,
-                double* stats = nullptr, const EpiBwd* bwd = nullptr, const EpiFin* fin = nullptr);
+                double* stats = nullptr, const EpiBwd* bwd = nullptr, const EpiFin* fin = nullptr,
+                const EpiAffine* aff = nullptr);
 // finalize of the dgrad-fused reductions: d gamma, d beta and the dy = A*g + B*y + C coefficients
 int launch_bn_bwd_finalize_accum(long long M, int C, const float* gamma, const float* mean, const float* invstd,
                                  float* dgamma, float* dbeta, float* coef, const float* gamma2, const float* mean2,

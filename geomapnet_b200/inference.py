@@ -19,13 +19,118 @@ import torch
 from . import _lib
 from .common.pgo import optimize_pose_windows
 
-__all__ = ["predict", "post", "pgo", "pose_errors", "evaluate_tuples"]
+__all__ = ["Predictor", "predict", "post", "pgo", "pose_errors", "evaluate_tuples"]
+
+
+class Predictor(object):
+    """Frozen eval-mode predictor of a PoseNet or MapNet: a snapshot of its weights and BatchNorm running statistics,
+    run by the inference engine (csrc/infer.cu) with BatchNorm, residual and ReLU fused into the conv epilogues.
+
+        pr = Predictor(model, max_batch=64)
+        poses = pr(x)       # [L,3,H,W] -> [L,6];  [L,T,3,H,W] -> [L,T,6];  max_batch frames per engine call
+        pr.refresh()        # take a new snapshot of the model's current parameters / running statistics
+        pr.close()
+
+    Training the model afterwards does not change the predictor's output until ``refresh()``.  Precision, droprate and
+    seed follow the model ('bf16' or 'tc_split' only).  Every distinct (B, H, W) is captured into a CUDA graph on its first
+    call and replayed after that.  With droprate > 0 the masks follow the engine's own step counter (as the model's
+    dropout, the reference's F.dropout is active at eval)."""
+
+    def __init__(self, model, max_batch=64):
+        net = model.mapnet if hasattr(model, "mapnet") else model
+        if net.precision not in ("bf16", "tc_split"):
+            raise ValueError("Predictor supports the precisions 'bf16' and 'tc_split' (the model uses %r)" % net.precision)
+        if int(max_batch) < 1:
+            raise ValueError("max_batch must be >= 1")
+        self.model, self.net, self.max_batch = model, net, int(max_batch)
+        self.precision, self.droprate, self.seed = net.precision, float(net.droprate), net._seed
+        self.device = torch.device("cuda", torch.cuda.current_device())
+        self._engines = {}      # (H, W) -> _lib.Infer
+        self._graphs = {}       # (B, H, W) -> (CUDAGraph, static input, static output)
+        self._params = self._bufs = None
+        self.refresh()
+
+    def refresh(self):
+        """Snapshot the model's current parameters and running statistics into every engine of this predictor."""
+        net = self.net
+        if not net._is_flat(self.device):
+            net._reflatten(self.device)
+        with torch.no_grad():
+            self._params = net._flat.detach().clone()
+            self._bufs = net._bufs.detach().clone()
+        with torch.cuda.device(self.device):
+            for eng in self._engines.values():
+                eng.load(self._params, self._bufs)      # in place: the captured graphs read the engines' own buffers
+        torch.cuda.current_stream(self.device).synchronize()
+
+    def _engine(self, H, W):
+        eng = self._engines.get((H, W))
+        if eng is None:
+            with torch.cuda.device(self.device):
+                eng = _lib.Infer(self.max_batch, H, W, self.net.feat_dim, self.precision)
+                eng.load(self._params, self._bufs)
+            self._engines[(H, W)] = eng
+        return eng
+
+    def _run(self, xb):
+        """pred [B,6] for frames xb [B,3,H,W] (B <= max_batch): graph replay, captured on the first call of a shape."""
+        B, _, H, W = xb.shape
+        key = (B, H, W)
+        g = self._graphs.get(key)
+        if g is None:
+            eng = self._engine(H, W)
+            xs = torch.empty((B, 3, H, W), dtype=torch.float32, device=self.device)
+            ps = torch.empty((B, 6), dtype=torch.float32, device=self.device)
+            xs.copy_(xb)
+            cur = torch.cuda.current_stream(self.device)
+            side = torch.cuda.Stream(self.device)
+            side.wait_stream(cur)
+            with torch.cuda.stream(side):        # eager run first: tile plans, tensor maps, kernel attributes
+                eng.forward(xs, ps, self.droprate, self.seed)
+            cur.wait_stream(side)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                eng.forward(xs, ps, self.droprate, self.seed)
+            g = self._graphs[key] = (graph, xs, ps)
+        graph, xs, ps = g
+        xs.copy_(xb)
+        graph.replay()
+        return ps.clone()
+
+    @torch.no_grad()
+    def __call__(self, x):
+        if not x.is_cuda:
+            raise RuntimeError("geomapnet_b200.inference.Predictor has no CPU path: input must be a CUDA tensor "
+                               "(got %s)" % x.device)
+        if x.dim() not in (4, 5) or x.shape[-3] != 3:
+            raise ValueError("expected input [L,3,H,W] or [L,T,3,H,W], got %s" % (tuple(x.shape),))
+        if x.shape[0] < 1 or (x.dim() == 5 and x.shape[1] < 1):
+            raise ValueError("empty batch")
+        if self._params is None:
+            raise RuntimeError("Predictor is closed")
+        frames = x.reshape(-1, *x.shape[-3:])
+        if frames.dtype != torch.float32:
+            frames = frames.float()
+        with torch.cuda.device(self.device):
+            outs = [self._run(frames[i:i + self.max_batch]) for i in range(0, frames.shape[0], self.max_batch)]
+        out = torch.cat(outs, 0)
+        return out.view(*x.shape[:-3], 6)
+
+    def close(self):
+        self._graphs.clear()
+        for eng in self._engines.values():
+            eng.close()
+        self._engines.clear()
+        self._params = self._bufs = None
 
 
 @torch.no_grad()
 def predict(model, x, batch=64):
     """model(x) in eval mode, `batch` leading entries at a time.  x: [L,3,H,W] (PoseNet) or [L,T,3,H,W] (MapNet), on the
-    GPU or pinned host memory.  Returns float32 [L,6] / [L,T,6] on the device."""
+    GPU or pinned host memory.  Returns float32 [L,6] / [L,T,6] on the device.  `model` may be a Predictor, which runs
+    its snapshot in chunks of its own max_batch frames."""
+    if isinstance(model, Predictor):
+        return model(x if x.is_cuda else x.cuda(non_blocking=True))
     was_training = model.training
     model.eval()
     outs = []

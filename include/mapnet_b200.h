@@ -166,6 +166,24 @@ int mapnet_pose_post(const float* pred6, double* out7, int64_t n, const double* 
 int mapnet_pgo_optimize(const double* poses, const double* vos, double* out, int n_windows, int N, int fc_vos,
                         double sax, double saq, double srx, double srq, int n_iters, int flags, int* status_dev, void* stream);
 
+/* ---- eval-mode inference engine (csrc/infer.cu): a frozen snapshot of a PoseNet / MapNet trunk for
+ * scripts/eval.py-style prediction.  mapnet_infer_load copies the weights (packed fprop operands only), the eval-mode
+ * BatchNorm scale / shift (computed from the running statistics exactly as mapnet_forward(training = 0) does) and the
+ * head out of params_flat / bufs_flat; the engine never reads those buffers again.  mapnet_infer_forward then runs the
+ * eval forward with every BatchNorm, residual add and ReLU fused into its conv's epilogue: one launch per conv plus the
+ * stem operand, the pool and the head.  Dropout follows mapnet_forward (the reference's F.dropout is active at eval when
+ * droprate > 0): the same mask for the same (seed, step); step == UINT64_MAX takes the engine's device step counter
+ * (graph-capturable).  Precisions: MAPNET_PREC_BF16 and MAPNET_PREC_TC_SPLIT only.  Argument errors (precision, B >
+ * max_B, a forward before a load) return non-zero before anything is allocated or launched.
+ * mapnet_infer_arena_bytes: host-only, the activation bytes a handle of these shapes allocates (< 0 on bad arguments). */
+typedef struct mapnet_infer mapnet_infer_t;
+int mapnet_infer_create(mapnet_infer_t** out, int max_B, int H, int W, int feat_dim, int precision);
+int mapnet_infer_load(mapnet_infer_t* h, const float* params_flat, const float* bufs_flat, void* stream);
+int mapnet_infer_forward(mapnet_infer_t* h, const float* x, int B, float droprate, uint64_t seed, uint64_t step,
+                         float* pred, void* stream);
+int64_t mapnet_infer_arena_bytes(int max_B, int H, int W, int precision);
+int mapnet_infer_destroy(mapnet_infer_t* h);
+
 /* ---- measurement support (bench.py): number of kernels this library has launched so
  * far in this process, and per-class conv timing with CUDA events on the launching
  * stream (class 0 fprop, 1 dgrad, 2 wgrad; algorithmic FLOPs of each launch summed). */
@@ -196,6 +214,15 @@ int mapnet_test_dgrad_shortcut(int B, int Hi, int Wi, int Ci, int Co, const void
 int mapnet_test_conv_epilogue(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* in0,
                               const void* wmat, const void* residual, const void* y, const void* zmask, const void* yd,
                               const float* mscale, const float* mshift, void* out, double* host_sums, void* stream);
+
+/* one wgmma fprop launch with the inference epilogue: out = relu?(conv(in0, wmat) * scale[c] + shift[c] [+ residual]),
+ * rounded once at the store.  flags: bit 0 ReLU; strict mode only: bit 1 the residual is stored as hi/lo planes (a block
+ * input), bit 2 the output is (the next conv's operand).  k == 7 runs the stem as the engine does (in0 = fp32 NCHW
+ * image, wmat = fp32 [64][3][7][7]).  Otherwise bf16 mode takes bf16 NHWC tensors and a bf16 [Co][k][k][Ci] matrix,
+ * strict mode fp32 ones (cut into planes inside).  Only the variants the eval-mode schedule uses are built. */
+int mapnet_test_conv_affine(int precision, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* in0,
+                            const void* wmat, const float* scale, const float* shift, const void* residual, int flags,
+                            void* out, void* stream);
 
 /* the tensor-core stem (7x7/s2/p3, 3 -> 64) alone, as the trunk runs it: space-to-depth image, packed weights,
  * fprop into y_out (bf16 NHWC [B,Hc,Wc,64]) and, when dy / dw_oihw are given, the weight gradient in the
