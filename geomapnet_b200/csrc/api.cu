@@ -183,7 +183,7 @@ int mapnet_test_conv(int precision, int kind, int B, int Hi, int Wi, int Ci, int
   if (precision == PREC_TC_SPLIT) {
     // strict tensor-core mode: fp32 NHWC tensors and fp32 K-major weight matrices in (as for PREC_FP32), fp32 out;
     // the operands are cut into fp16 hi / lo planes here (the training step's element-wise kernels write that form)
-    g.split = 1; g.fmt_z = 0; g.fmt_g = 0;
+    g.split = 1;
     const long long n_in = (long long)B * Hi * Wi * Ci, n_out = (long long)B * g.Ho * g.Wo * Co;
     const int KK = k * k;
     void *s0 = nullptr, *s1 = nullptr, *sw = nullptr;
@@ -191,14 +191,14 @@ int mapnet_test_conv(int precision, int kind, int B, int Hi, int Wi, int Ci, int
     auto body = [&]() -> int {
       const long long n0 = (kind == 1) ? n_out : n_in;
       MN_CUDA(cudaMalloc(&s0, (size_t)n0 * 4));
-      MN_TRY(launch_split_tensor((const float*)in0, s0, n0, 0, st));
+      MN_TRY(launch_split_tensor((const float*)in0, s0, n0, st));
       if (kind == 2) {
         MN_CUDA(cudaMalloc(&s1, (size_t)n_out * 4));
-        MN_TRY(launch_split_tensor((const float*)in1, s1, n_out, 0, st));
+        MN_TRY(launch_split_tensor((const float*)in1, s1, n_out, st));
       } else {
         MN_CUDA(cudaMalloc(&sw, (size_t)Co * KK * Ci * 8));
-        if (kind == 0) MN_TRY(launch_split_weight_matrix((const float*)wmat, sw, Co, KK, Ci, 0, st));
-        else MN_TRY(launch_split_weight_matrix((const float*)wmat, sw, Ci, KK, Co, 0, st));
+        if (kind == 0) MN_TRY(launch_split_weight_matrix((const float*)wmat, sw, Co, KK, Ci, st));
+        else MN_TRY(launch_split_weight_matrix((const float*)wmat, sw, Ci, KK, Co, st));
       }
       MN_TRY(tc_plan_create(&plan, g, kind, (const bf16*)sw));
       MN_TRY(tc_conv_run(plan, (const bf16*)s0, (const bf16*)s1, nullptr, out, st));
@@ -370,7 +370,7 @@ int mapnet_test_conv_affine(int precision, int B, int Hi, int Wi, int Ci, int Co
     g.Ho = (Hi + 2 * g.pad - k) / stride + 1; g.Wo = (Wi + 2 * g.pad - k) / stride + 1;
   }
   g.B = B;
-  if (sp) { g.split = 1; g.fmt_z = 0; g.fmt_g = 0; }
+  if (sp) g.split = 1;
   const long long n_out = (long long)B * g.Ho * g.Wo * Co;
   void *x = nullptr, *w = nullptr, *r = nullptr, *f32 = nullptr; WeightDesc* d_wd = nullptr;
   TcConvPlan* plan = nullptr;
@@ -385,7 +385,7 @@ int mapnet_test_conv_affine(int precision, int B, int Hi, int Wi, int Ci, int Co
       if (sp) {
         MN_CUDA(cudaMalloc(&f32, (size_t)64 * 256 * 4));
         MN_TRY(launch_stem_s2d<hsplit>((const float*)in0, (hsplit*)x, B, Hi, Wi, g.Hi, Wsp, st));
-        MN_TRY(launch_pack_weights_split(d_wd, 1, (const float*)wmat, (float*)f32, nullptr, w, nullptr, 64 * 256, 0, 0, st));
+        MN_TRY(launch_pack_weights_split(d_wd, 1, (const float*)wmat, (float*)f32, nullptr, w, nullptr, 64 * 256, st));
       } else {
         MN_TRY(launch_stem_s2d<bf16>((const float*)in0, (bf16*)x, B, Hi, Wi, g.Hi, Wsp, st));
         MN_TRY(launch_pack_weights<bf16>(d_wd, 1, (const float*)wmat, (bf16*)w, nullptr, 64 * 256, 0, st));
@@ -394,19 +394,18 @@ int mapnet_test_conv_affine(int precision, int B, int Hi, int Wi, int Ci, int Co
     } else if (sp) {
       const long long n_in = (long long)B * Hi * Wi * Ci;
       MN_CUDA(cudaMalloc(&x, (size_t)n_in * 4));
-      MN_TRY(launch_split_tensor((const float*)in0, x, n_in, 0, st));
+      MN_TRY(launch_split_tensor((const float*)in0, x, n_in, st));
       MN_CUDA(cudaMalloc(&w, (size_t)Co * k * k * Ci * 8));
-      MN_TRY(launch_split_weight_matrix((const float*)wmat, w, Co, k * k, Ci, 0, st));
+      MN_TRY(launch_split_weight_matrix((const float*)wmat, w, Co, k * k, Ci, st));
       if (residual != nullptr && a.res_split) {
         MN_CUDA(cudaMalloc(&r, (size_t)n_out * 4));
-        MN_TRY(launch_split_tensor((const float*)residual, r, n_out, 0, st));
+        MN_TRY(launch_split_tensor((const float*)residual, r, n_out, st));
         rin = r;
       }
       xin = x; win = w;
     }
     MN_TRY(tc_plan_create(&plan, g, 0, (const bf16*)win));
-    MN_TRY(tc_plan_set_cluster(plan, 1));
-    MN_TRY(tc_conv_run(plan, (const bf16*)xin, nullptr, (const bf16*)rin, out, st, nullptr, nullptr, nullptr, &a));
+    MN_TRY(tc_conv_run(plan, (const bf16*)xin, nullptr, (const bf16*)rin, out, st, nullptr, nullptr, &a));
     MN_CUDA(cudaStreamSynchronize(st));
     return 0;
   };

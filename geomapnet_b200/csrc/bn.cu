@@ -147,44 +147,8 @@ static int launch_sums(int mode, const T* a, const TZ* zmask, const T* y, const 
   return 0;
 }
 
-// finalize for statistics accumulated by the wgmma conv epilogue (conv_tc.cu): sum the
-// replicas, produce mean / invstd / scale / shift, update the running stats, reset the replicas
-// block = 32 channels x 32 replicas: coalesced replica loads, shared-memory reduction over replicas
-__global__ void __launch_bounds__(1024)
-k_bn_finalize_accum(long long M, int C, BnFin f, double* __restrict__ accum) {
-  pdl_prologue();
-  __shared__ double s0s[32][33], s1s[32][33];
-  const int cl = threadIdx.x, r = threadIdx.y;
-  const int c = blockIdx.x * 32 + cl;
-  double v0 = 0.0, v1 = 0.0;
-  if (c < C && r < kReplicas) {
-    double* a = accum + (size_t)r * kAccStride;
-    v0 = a[c]; v1 = a[C + c];
-    a[c] = 0.0; a[C + c] = 0.0;
-  }
-  s0s[r][cl] = v0; s1s[r][cl] = v1;
-  __syncthreads();
-  if (r != 0 || c >= C) return;
-  double s0 = 0.0, s1 = 0.0;
-#pragma unroll
-  for (int k = 0; k < 32; ++k) { s0 += s0s[k][cl]; s1 += s1s[k][cl]; }
-  bn_fin_forward(c, s0, s1, M, f);
-}
-
-int launch_bn_finalize_accum(long long M, int C, const float* gamma, const float* beta, float* run_mean,
-                             float* run_var, float* mean_out, float* invstd_out, float* scale, float* shift,
-                             double* accum, cudaStream_t st) {
-  MN_CHECK(C <= 512, "bn_finalize_accum: C=%d", C);
-  BnFin f; memset(&f, 0, sizeof(f));
-  f.gamma = gamma; f.beta = beta; f.run_mean = run_mean; f.run_var = run_var; f.mean = mean_out;
-  f.invstd = invstd_out; f.scale = scale; f.shift = shift; f.training = 1;
-  MN_LAUNCH(k_bn_finalize_accum, cdiv(C, 32), dim3(32, 32), 0, st, M, C, f, accum);
-  MN_LAUNCH_CHECK();
-  return 0;
-}
-
-// finalize for the backward reductions accumulated by the dgrad epilogue (conv_tc.cu, EpiBwd):
-// same arithmetic as MODE 1 / 2 of k_channel_sums
+// finalize for backward reductions accumulated in bn_accum by another kernel (the stem's pool backward in the
+// CUDA-core modes): same arithmetic as MODE 1 / 2 of k_channel_sums
 __global__ void __launch_bounds__(1024)
 k_bn_bwd_finalize_accum(long long M, int C, BnFin f, double* __restrict__ accum, int nacc) {
   pdl_prologue();

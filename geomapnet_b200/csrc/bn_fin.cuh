@@ -1,5 +1,5 @@
-// BatchNorm finalize arithmetic shared by bn.cu (separate finalize kernels, k_channel_sums) and
-// conv_tc.cu (finalize fused into the LAST CTA of the conv that accumulated the sums).
+// BatchNorm finalize arithmetic of bn.cu: the separate finalize kernel, k_channel_sums and the lazy finalize of the
+// consuming element-wise kernels.
 // Reference semantics: torch.nn.BatchNorm2d training forward / backward as run by
 // /root/reference/models/posenet.py:66 (momentum 0.1, eps 1e-5, unbiased running variance).
 #pragma once
@@ -29,15 +29,6 @@ struct BnLazy {
   int nrep;
   long long M;               // pixels per channel
   double invM, unbias;       // 1 / M and M / (M - 1) from the host: no fp64 division on the consumers' critical path
-  BnFin f;
-};
-
-// what a conv kernel needs to finalize the sums it accumulated (conv_tc.cu)
-struct EpiFin {
-  int mode;                  // 0 none, 1 forward statistics, 2 backward reductions, 3 backward + downsample BN
-  unsigned int expected;     // CTAs (over all launches feeding the accumulators) that flush before the finalize
-  unsigned int* counter;     // zero on entry, reset by the finalizing CTA
-  long long M;               // pixels per channel
   BnFin f;
 };
 

@@ -27,7 +27,6 @@
 #include <vector>
 
 #include "kernels.h"
-#include "bn_fin.cuh"
 #include "tc_ptx.cuh"
 
 namespace mapnet {
@@ -128,18 +127,17 @@ struct ConvParams {
   int debug;     // micro-benchmark only: 1 = skip the MMAs, 2 = skip the TMA loads (results are garbage)
   int fmt_a, fmt_b;        // wgmma operand element formats (equal): 0 = fp16, 1 = bf16
   int out32;               // strict mode: output (and residual) are fp32 tensors
-  int epi_prefetch;        // epilogue warps pull the NEXT tile's residual / y / zmask / yd rows into L2 (env MAPNET_TC_EPI_PREFETCH)
 };
 
-// work item -> (class, N tile, first M tile of the group): classes are laid out one after the other
-// (heaviest first), inside a class the N tile varies fastest
-struct TileCoord { int cls, tn, group; };
+// work item -> (class, N tile, M tile): classes are laid out one after the other (heaviest first), inside a class the
+// N tile varies fastest
+struct TileCoord { int cls, tn, tm; };
 __device__ __forceinline__ TileCoord decode_tile(const int tile, const int per_class, const int n_tiles_n) {
   TileCoord t;
   t.cls = tile / per_class;
   const int r = tile - t.cls * per_class;
-  t.group = r / n_tiles_n;
-  t.tn = r - t.group * n_tiles_n;
+  t.tm = r / n_tiles_n;
+  t.tn = r - t.tm * n_tiles_n;
   return t;
 }
 
@@ -171,8 +169,7 @@ __device__ __forceinline__ WgradChunk wgrad_chunk(const WgradParams& P, int c) {
   return ch;
 }
 
-// BN statistic accumulators: kStatReplicas x [2][<=512] doubles (same buffer bn.cu uses)
-static const int kStatReplicas = 32;
+// BN statistic accumulators: replicas of [3][<=512] doubles (Net::kSlotStride)
 static const int kStatStride = 3 * 512;
 
 // x[32] per lane -> lane L ends with sum over the warp's lanes of x[L] (in x[0])
@@ -278,42 +275,6 @@ __device__ __forceinline__ void epi_issue_loads(EpiRegs& G, const long long (&ro
     if (F & EPI_BWD) G.y[i] = __ldg(reinterpret_cast<const uint4*>(E.y + off));
     if (F & EPI_ZMASK) G.z[i] = __ldg(reinterpret_cast<const uint4*>(E.zmask + off));
     if (F & EPI_YD) G.d[i] = __ldg(reinterpret_cast<const uint4*>(E.yd + off));
-  }
-}
-
-// EXPERIMENT (env MAPNET_TC_EPI_PREFETCH=1, default off: no gain measured).  The fused dgrad epilogues read up to four
-// more tensors per output element (skip-path gradient, conv output y, ReLU mask z, downsample-branch y), one 32-column
-// chunk at a time per warp.  Hypothesis: ~0.8 us of DRAM latency per chunk with only 4 warps of loads in flight.  While a
-// tile's accumulator is still being produced, each epilogue warp asks L2 for the rows of the tile it will process NEXT:
-// one prefetch per 128-byte line, lane p = lane & 3 takes line p of each of its 4 rows.
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" :: "l"(p)); }
-
-template <int BN>
-__device__ __forceinline__ void epi_prefetch_next(const ConvParams& P, const int tile, const int per_class, const int cl,
-                                                  const int crank, const int q, const int lane, const bf16* residual,
-                                                  const EpiBwd& E) {
-  const int p = lane & 3;
-  if (p * 64 >= BN) return;
-  const TileCoord tc = decode_tile(tile, per_class, P.n_tiles_n);
-  const ClassDesc cd = P.cls[tc.cls];
-  int tm = tc.group * cl + crank;
-  const int tw = tm % P.tiles_w; tm /= P.tiles_w;
-  const int th = tm % P.tiles_h;
-  const int tb = tm / P.tiles_h;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int m = q * 32 + 8 * i + (lane >> 2);
-    const int lw = m % P.TW;
-    const int lh = (m / P.TW) % P.TH;
-    const int ln = m / (P.TW * P.TH);
-    const int jw = tw * P.TW + lw, jh = th * P.TH + lh, n = tb * P.TN + ln;
-    if (!((jw < cd.Ws) && (jh < cd.Hs) && (n < P.Nimg))) continue;
-    const long long pix = ((long long)n * P.Hout + (jh * P.os + cd.oa)) * P.Wout + (jw * P.os + cd.ob);
-    const long long off = pix * P.Cout + tc.tn * BN + p * 64;
-    if (residual != nullptr) prefetch_l2(residual + off);
-    if (E.y != nullptr) prefetch_l2(E.y + off);
-    if (E.zmask != nullptr) prefetch_l2(E.zmask + off);
-    if (E.yd != nullptr) prefetch_l2(E.yd + off);
   }
 }
 
@@ -484,7 +445,7 @@ __device__ __forceinline__ void epi_tile_dispatch(const int mode, const float* _
                                                   const int half) {
 #define MN_EPI_CASE(Fv) case (Fv): epi_tile<(Fv), BN>(rows, stw, rowoff, rvalid, do_store, tn, residual, out, E, lane, half); break;
   if constexpr (AFF) {
-    // eval-mode inference, its own kernel instantiations (k_tc_conv<BN, CL, true>) so that the training kernels keep
+    // eval-mode inference, its own kernel instantiations (k_tc_conv<BN, true>) so that the training kernels keep
     // their register allocation: stem / conv1 (ReLU), downsample (no ReLU), conv2 (+ block input or downsample
     // output, ReLU)
     switch (mode) {
@@ -555,7 +516,7 @@ __device__ __forceinline__ int epi_mode_of(const bf16* residual, const double* s
   return m;
 }
 
-// ---- statistics flush + fused BatchNorm finalize (epilogue warps only: kEpiThreads threads, named barrier 1) ----
+// ---- statistics flush (epilogue warps only: kEpiThreads threads, named barrier 1) ----
 static constexpr int kConvReplicas = 8;        // accumulator replicas the conv engines spread their flushes over
 
 __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, %0;" ::"n"(kEpiThreads) : "memory"); }
@@ -578,59 +539,27 @@ __device__ __forceinline__ void epi_flush(float (*all)[3][BN / 32][32], double* 
   epi_bar();                                    // zeroed before any warp accumulates the next N tile
 }
 
-// The LAST CTA (over all launches that feed the accumulators) to finish its flushes turns the sums into the
-// BatchNorm quantities the next kernel needs -- no separate finalize launch.
-__device__ __forceinline__ void epi_finalize(const EpiFin& Fin, double* __restrict__ stats, const int C,
-                                             const int etid, unsigned int* s_flag) {
-  __threadfence();                              // this thread's atomics are ordered before the counter
-  epi_bar();
-  if (etid == 0) *s_flag = (atomicAdd(Fin.counter, 1u) == Fin.expected - 1u) ? 1u : 0u;
-  epi_bar();
-  if (*s_flag == 0u) return;
-  __threadfence();
-  const int nacc = (Fin.mode == 3) ? 3 : 2;
-#pragma unroll 1
-  for (int c = etid; c < C; c += kEpiThreads) {
-    double s[3] = {0.0, 0.0, 0.0};
-#pragma unroll
-    for (int r = 0; r < kConvReplicas; ++r) {
-      double* a = stats + (size_t)r * kStatStride;
-#pragma unroll
-      for (int j = 0; j < 3; ++j)
-        if (j < nacc) { s[j] += __ldcg(a + (size_t)j * C + c); a[(size_t)j * C + c] = 0.0; }
-    }
-    if (Fin.mode == 1) bn_fin_forward(c, s[0], s[1], Fin.M, Fin.f);
-    else bn_fin_backward(c, C, s[0], s[1], s[2], Fin.M, Fin.f, nacc == 3);
-  }
-  if (etid == 0) *Fin.counter = 0u;
-}
-
 // as many stages as fit in 227 KB next to the accumulator staging rows: the engines are bound by bytes in flight
 static constexpr int conv_stages(int BN) { return BN <= 64 ? 7 : 4; }
 static constexpr size_t conv_smem_bytes(int BN) {
   return (size_t)conv_stages(BN) * (128 * 128 + BN * 128) + (size_t)128 * (BN + 4) * 4 + 1024;
 }
-static constexpr int wgrad_stages(int BN) { return BN <= 64 ? 9 : 6; }
+// wgrad runs two CTAs per SM, each with half the stages that would fit for one: the store epilogue of one CTA overlaps
+// the other CTA's MMAs instead of idling the tensor cores (measured: 587 -> 781 TF/s on layer3/4 wgrad)
+static constexpr int wgrad_stages(int BN) { return (BN <= 64 ? 9 : 6) / 2; }
 
 // named barrier of one consumer warpgroup (barrier 0 is __syncthreads, 1 is epi_bar)
 __device__ __forceinline__ void wg_bar(const int wg) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); }
 
-// release a pipeline stage: one thread per consumer warpgroup arrives on the stage's empty barrier in every CTA of
-// the cluster (each CTA's producer multicasts its slice of the weight tile into all of them)
-template <int CL>
+// release a pipeline stage: one thread per consumer warpgroup arrives on the stage's empty barrier
 __device__ __forceinline__ void release_stage(const uint32_t empty_bar, const bool arriver) {
-  if (!arriver) return;
-  if (CL == 1) mbar_arrive(empty_bar);
-  else {
-#pragma unroll
-    for (int r = 0; r < CL; ++r) mbar_arrive_cluster(mapa(empty_bar, (uint32_t)r));
-  }
+  if (arriver) mbar_arrive(empty_bar);
 }
 
 // Mainloop of one tile for one consumer warpgroup: kblocks k-blocks of 64, each four wgmma K=16 steps.  A stage is
 // handed back as soon as the wgmma group that read it has retired (one group stays in flight behind the next).
 // a_off / a_step: this warpgroup's A rows inside a stage and the byte step per K=16; b_step likewise for B.
-template <int BN, int CL, int FMT, int TA, int TB>
+template <int BN, int FMT, int TA, int TB>
 __device__ __forceinline__ void mma_tile(float (&d)[BN / 2], const int kblocks, int& stage, uint32_t& phase,
                                          const int STAGES, const uint32_t stage_bytes, const uint32_t smem_base,
                                          const uint32_t a_off, const uint32_t a_step, const uint32_t b_off,
@@ -652,13 +581,13 @@ __device__ __forceinline__ void mma_tile(float (&d)[BN / 2], const int kblocks, 
       wgmma_wait<1>();
       wgmma_fence_acc(d);
     }
-    if (prev >= 0) release_stage<CL>(empty0 + 8 * prev, arriver);
+    if (prev >= 0) release_stage(empty0 + 8 * prev, arriver);
     prev = stage;
     if (++stage == STAGES) { stage = 0; phase ^= 1; }
   }
   wgmma_wait<0>();
   wgmma_fence_acc(d);
-  if (prev >= 0) release_stage<CL>(empty0 + 8 * prev, arriver);
+  if (prev >= 0) release_stage(empty0 + 8 * prev, arriver);
   if (kblocks == 0 || skip_mma) {         // no filter tap reaches this output class (or MMAs skipped): D = 0
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
@@ -668,17 +597,14 @@ __device__ __forceinline__ void mma_tile(float (&d)[BN / 2], const int kblocks, 
 // ---------------------------------------------------------------------------------
 // fprop / dgrad kernel
 // ---------------------------------------------------------------------------------
-// CL = thread-block cluster size along M: the CL CTAs of a cluster work on CL consecutive
-// M tiles of the same N tile and share the weight tile -- each loads 1/CL of it and TMA-
-// multicasts it to all (cuts the B traffic from L2 by CL).
 // AFF: the eval-mode inference epilogues (EPI_AFFINE) instead of the training ones.
-template <int BN, int CL, bool AFF>
+template <int BN, bool AFF = false>
 __global__ void __launch_bounds__(kConvThreads, 1)
 k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
           const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapA3,
           const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapB2,
           const __grid_constant__ ConvParams P, const bf16* __restrict__ residual,
-          bf16* __restrict__ out, double* __restrict__ stats, const EpiBwd E, const EpiFin Fin) {
+          bf16* __restrict__ out, double* __restrict__ stats, const EpiBwd E) {
   constexpr int STAGES = conv_stages(BN);
   constexpr uint32_t A_BYTES = 128 * 128;        // 128 pixels x 64 ch bf16
   constexpr uint32_t B_BYTES = BN * 128;
@@ -693,25 +619,19 @@ k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform for the compiler
   const int lane = threadIdx.x & 31;
 
-  const uint32_t crank = (CL > 1) ? cluster_ctarank() : 0u;
-  constexpr uint16_t CMASK = (uint16_t)((1u << CL) - 1u);
   if (warp == kProducerWarp && lane == 0) {
     prefetch_tmap(&mapA0); prefetch_tmap(&mapB);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(full0 + 8 * i, 1); mbar_init(empty0 + 8 * i, 2 * CL); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(full0 + 8 * i, 1); mbar_init(empty0 + 8 * i, 2); }
     fence_mbar_init();
   }
   __syncthreads();
-  if (CL > 1) cluster_sync();          // peers' barriers are initialised before any multicast
   pdl_prologue();      // nothing above touches global memory: setup overlaps the previous kernel's tail
 
-  // work items: (group of CL consecutive M tiles, N tile); every CTA of a cluster walks the
-  // same sequence, CTA r takes M tile group*CL + r (possibly past the end: a dummy tile whose
-  // loads are zero-filled by TMA and whose epilogue stores nothing)
-  const int n_groups = (P.n_tiles_m + CL - 1) / CL;
-  const int per_class = n_groups * P.n_tiles_n;
+  // work items: (M tile, N tile) per class; the persistent CTAs take them round-robin
+  const int per_class = P.n_tiles_m * P.n_tiles_n;
   const int total_tiles = per_class * P.n_classes;
-  const int first_tile = blockIdx.x / CL;
-  const int tile_step = gridDim.x / CL;
+  const int first_tile = blockIdx.x;
+  const int tile_step = gridDim.x;
 
   if (warp == kProducerWarp) {
     // ===================== TMA producer =====================
@@ -721,7 +641,7 @@ k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
         const TileCoord tc = decode_tile(tile, per_class, P.n_tiles_n);
         const ClassDesc cd = P.cls[tc.cls];
         const int tn = tc.tn;
-        int tm = tc.group * CL + (int)crank;
+        int tm = tc.tm;
         const int tw = tm % P.tiles_w; tm /= P.tiles_w;
         const int th = tm % P.tiles_h;
         const int tb = tm / P.tiles_h;
@@ -737,13 +657,7 @@ k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
             if (P.debug == 2) { mbar_arrive(full0 + 8 * stage); if (++stage == STAGES) { stage = 0; phase ^= 1; } continue; }
             mbar_expect_tx(full0 + 8 * stage, STAGE_BYTES);
             tma_load_4d(sa, mA, full0 + 8 * stage, cb * 64, jw0 + tap.dw, jh0 + tap.dh, n0);
-            if (CL == 1) {
-              tma_load_2d(sa + A_BYTES, mB, full0 + 8 * stage, tap.kidx * P.Cs + cb * 64, tn * BN);
-            } else {
-              constexpr int BROWS = BN / CL;      // this CTA's slice of the weight tile
-              tma_load_2d_mc(sa + A_BYTES + crank * (BROWS * 128), mB, full0 + 8 * stage,
-                             tap.kidx * P.Cs + cb * 64, tn * BN + (int)crank * BROWS, CMASK);
-            }
+            tma_load_2d(sa + A_BYTES, mB, full0 + 8 * stage, tap.kidx * P.Cs + cb * 64, tn * BN);
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
         }
@@ -777,13 +691,14 @@ k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
       const int tn = tc.tn;
       float d[BN / 2];
       if (P.fmt_a)
-        mma_tile<BN, CL, 1, 0, 0>(d, kblocks, stage, phase, STAGES, STAGE_BYTES, smem_base, wg * 64 * 128, 32, A_BYTES, 32,
-                                  DESC_BASE, DESC_BASE, full0, empty0, arriver, P.debug == 1);
+        mma_tile<BN, 1, 0, 0>(d, kblocks, stage, phase, STAGES, STAGE_BYTES, smem_base, wg * 64 * 128, 32, A_BYTES, 32,
+                              DESC_BASE, DESC_BASE, full0, empty0, arriver, P.debug == 1);
       else
-        mma_tile<BN, CL, 0, 0, 0>(d, kblocks, stage, phase, STAGES, STAGE_BYTES, smem_base, wg * 64 * 128, 32, A_BYTES, 32,
-                                  DESC_BASE, DESC_BASE, full0, empty0, arriver, P.debug == 1);
-      if (stats != nullptr && tn != st_tn) { if (st_tn >= 0) flush_stats(st_tn); st_tn = tn; }
-      int tm = tc.group * CL + (int)crank;
+        mma_tile<BN, 0, 0, 0>(d, kblocks, stage, phase, STAGES, STAGE_BYTES, smem_base, wg * 64 * 128, 32, A_BYTES, 32,
+                              DESC_BASE, DESC_BASE, full0, empty0, arriver, P.debug == 1);
+      // inference launches carry no statistics (tc_conv_run checks it): no flush is compiled into those kernels
+      if (!AFF && stats != nullptr && tn != st_tn) { if (st_tn >= 0) flush_stats(st_tn); st_tn = tn; }
+      int tm = tc.tm;
       const int tw = tm % P.tiles_w; tm /= P.tiles_w;
       const int th = tm % P.tiles_h;
       const int tb = tm / P.tiles_h;
@@ -800,25 +715,14 @@ k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
         const long long pix = ((long long)n * P.Hout + (jh * P.os + cd.oa)) * P.Wout + (jw * P.os + cd.ob);
         rowoff[i] = (rvalid[i] ? pix * P.Cout : 0) + tn * BN;     // outside rows: clamped, loads stay in bounds
       }
-      if (P.epi_prefetch && tile + tile_step < total_tiles)
-        epi_prefetch_next<BN>(P, tile + tile_step, per_class, CL, (int)crank, q, lane, residual, E);
-      if (P.debug == 3) continue;            // micro-benchmark: no epilogue work at all
+      if (P.debug == 3) continue;           // micro-benchmark: no epilogue work at all
       wg_bar(wg);                             // the previous tile's staged rows have been read
       acc_to_stage<BN>(d, stg + wg * 64 * RS, wq, lane);
       wg_bar(wg);
       epi_tile_dispatch<BN, AFF>(epi_mode, stg + q * 32 * RS, stw, rowoff, rvalid, P.debug != 4, tn, residual, out, E, lane,
                             half);
     }
-    if (stats != nullptr && st_tn >= 0) flush_stats(st_tn);
-    if (Fin.mode != 0) {
-      __shared__ unsigned int s_fin_flag;
-      epi_finalize(Fin, stats, P.Cout, etid, &s_fin_flag);
-    }
-  }
-  // ---- teardown ----
-  if (CL > 1) {
-    __syncthreads();
-    cluster_sync();                    // no CTA exits while a peer may still multicast into it or arrive on it
+    if (!AFF && stats != nullptr && st_tn >= 0) flush_stats(st_tn);
   }
 }
 
@@ -869,15 +773,14 @@ __device__ __forceinline__ void wgrad_store(const WgradParams& P, float* __restr
 // ---------------------------------------------------------------------------------
 // wgrad kernel: one CTA per (M-tile of 2 X chunks, N-tile of BN couts, K split); consumer warpgroup j owns chunk j
 // ---------------------------------------------------------------------------------
-// OCC = CTAs per SM: with 2, each CTA gets half the stages and the fp32-atomic epilogue of one CTA
-// overlaps the other CTA's MMAs instead of idling the tensor cores
-template <int BN, int OCC>
-__global__ void __launch_bounds__(kConvThreads, OCC)
+// two CTAs per SM (wgrad_stages)
+template <int BN>
+__global__ void __launch_bounds__(kConvThreads, 2)
 k_tc_wgrad(const __grid_constant__ CUtensorMap mapX0, const __grid_constant__ CUtensorMap mapX1,
            const __grid_constant__ CUtensorMap mapX2, const __grid_constant__ CUtensorMap mapX3,
            const __grid_constant__ CUtensorMap mapDY, const __grid_constant__ WgradParams P,
            float* __restrict__ dw) {
-  constexpr int STAGES = wgrad_stages(BN) / OCC;
+  constexpr int STAGES = wgrad_stages(BN);
   constexpr uint32_t CHUNK_BYTES = 64 * 128;     // 64 pixels x 64 ch bf16
   constexpr uint32_t A_BYTES = 2 * CHUNK_BYTES;
   constexpr uint32_t B_BYTES = (BN / 64) * CHUNK_BYTES;
@@ -941,11 +844,11 @@ k_tc_wgrad(const __grid_constant__ CUtensorMap mapX0, const __grid_constant__ CU
     float d[BN / 2];
     const bool arriver = (threadIdx.x & 127) == 0;
     if (P.fmt_a)
-      mma_tile<BN, 1, 1, 1, 1>(d, ksteps, stage, phase, STAGES, STAGE_BYTES, smem_base, wg * CHUNK_BYTES, 2048, A_BYTES,
-                               2048, DESC_BASE, DESC_BASE, full0, empty0, arriver, false);
+      mma_tile<BN, 1, 1, 1>(d, ksteps, stage, phase, STAGES, STAGE_BYTES, smem_base, wg * CHUNK_BYTES, 2048, A_BYTES,
+                            2048, DESC_BASE, DESC_BASE, full0, empty0, arriver, false);
     else
-      mma_tile<BN, 1, 0, 1, 1>(d, ksteps, stage, phase, STAGES, STAGE_BYTES, smem_base, wg * CHUNK_BYTES, 2048, A_BYTES,
-                               2048, DESC_BASE, DESC_BASE, full0, empty0, arriver, false);
+      mma_tile<BN, 0, 1, 1>(d, ksteps, stage, phase, STAGES, STAGE_BYTES, smem_base, wg * CHUNK_BYTES, 2048, A_BYTES,
+                            2048, DESC_BASE, DESC_BASE, full0, empty0, arriver, false);
     float* dst = (P.partial != nullptr) ? P.partial + (long long)split * P.part_stride : dw;
     if (ksteps > 0 && wg < n_valid_chunks && P.debug != 3)
       wgrad_store<BN>(P, dst, d, wgrad_chunk(P, c_lo + wg), nt * BN, warp & 3, lane);
@@ -990,8 +893,8 @@ struct TcConvPlan {
   int kind;
   const bf16* wmat;
   const bf16* wmat2;                    // dgrad weight matrix [Ci][Co2] of a folded 1x1/stride-2 shortcut conv, or null
-  int BN, CL;
-  std::vector<ConvLaunch> launches;     // fprop: 1; dgrad: 1 (stride 1) or 4 (stride 2)
+  int BN;
+  std::vector<ConvLaunch> launches;    // fprop: 1; dgrad: 1 (stride 1) or 4 (stride 2)
   // wgrad
   WgradParams WP;
   CUtensorMap mapX[4], mapDY;
@@ -1013,12 +916,6 @@ static void pick_box(int Wd, int Hd, int pixels, int* TW, int* TH, int* TN) {
   int tn = pixels / (tw * th);
   if (tn < 1) tn = 1;
   *TW = tw; *TH = th; *TN = tn;
-}
-
-static int pick_cl() {
-  static int cl = -1;
-  if (cl < 0) { const char* e = getenv("MAPNET_TC_CLUSTER"); cl = e ? atoi(e) : 1; if (cl != 1 && cl != 2 && cl != 4) cl = 1; }
-  return cl;
 }
 
 // N tile by a small cost model: wider tiles re-use the A operand more, but must still leave enough work items to
@@ -1080,7 +977,6 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
   TcConvPlan* p = new TcConvPlan();
   p->g = g; p->kind = kind; p->wmat = wmat; p->wmat2 = nullptr; p->shortcut_flops_k = 0;
   p->c_in0 = p->c_in1 = nullptr; p->smem_attr_set = false; p->smem_attr_aff = false; p->out_scale = nullptr; p->ws = nullptr;
-  p->CL = pick_cl();
   const int s = g.stride, pad = g.pad, KK = g.KH * g.KW;
   // strict mode: the engines see 2*C 16-bit channels per pixel and every filter tap twice (hi / lo weight planes)
   const int SP = g.split ? 2 : 1;
@@ -1091,7 +987,7 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
     ConvLaunch L; memset(&L, 0, sizeof(L));
     ConvParams& P = L.P;
     { const char* e = getenv("MAPNET_TC_DEBUG"); P.debug = e ? atoi(e) : 0; }
-    P.fmt_a = P.fmt_b = g.split ? g.fmt_z : 1; P.out32 = g.split;
+    P.fmt_a = P.fmt_b = g.split ? 0 : 1; P.out32 = g.split;
     P.Nimg = g.B;
     P.n_classes = 1;
     P.cls[0].Hs = g.Ho; P.cls[0].Ws = g.Wo; P.cls[0].oa = 0; P.cls[0].ob = 0; P.cls[0].tap0 = 0; P.cls[0].num_taps = SP * KK;
@@ -1151,7 +1047,7 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
       ConvLaunch L; memset(&L, 0, sizeof(L));
       ConvParams& P = L.P;
       { const char* e = getenv("MAPNET_TC_DEBUG"); P.debug = e ? atoi(e) : 0; }
-      P.fmt_a = P.fmt_b = g.split ? g.fmt_g : 1; P.out32 = g.split;
+      P.fmt_a = P.fmt_b = g.split ? 0 : 1; P.out32 = g.split;
       P.Nimg = g.B;
       pick_box(Ws0, Hs0, 128, &P.TW, &P.TH, &P.TN);
       P.tiles_w = cdiv(Ws0, P.TW); P.tiles_h = cdiv(Hs0, P.TH); P.tiles_n = cdiv(g.B, P.TN);
@@ -1178,7 +1074,7 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
       for (int i = 0; i < ncls; ++i) {
         ConvLaunch L; memset(&L, 0, sizeof(L));
         ConvParams& P = L.P;
-        P.fmt_a = P.fmt_b = g.split ? g.fmt_g : 1; P.out32 = g.split;
+        P.fmt_a = P.fmt_b = g.split ? 0 : 1; P.out32 = g.split;
         P.Nimg = g.B;
         P.n_classes = 1;
         ClassDesc& c = P.cls[0];
@@ -1200,8 +1096,7 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
     { const char* e = getenv("MAPNET_TC_DEBUG"); P.debug = e ? atoi(e) : 0; }
     const int CoS = SP * g.Co, CiS = SP * g.Ci;      // GEMM N / M extents in 16-bit operand elements
     p->BN = (CoS % 128 == 0) ? 128 : 64;      // 64 x BN fp32 accumulator per consumer warpgroup in registers
-    P.split = g.split; P.fmt_a = g.split ? g.fmt_z : 1; P.fmt_b = g.split ? g.fmt_g : 1;
-    MN_CHECK(P.fmt_a == P.fmt_b, "tc wgrad: wgmma needs both operands in the same 16-bit format");
+    P.split = g.split; P.fmt_a = P.fmt_b = g.split ? 0 : 1;
     P.BN = p->BN; P.Nimg = g.B; P.Ho = g.Ho; P.Wo = g.Wo; P.Ci = g.Ci; P.Co = g.Co; P.KK = KK;
     pick_box(g.Wo, g.Ho, 64, &P.TW, &P.TH, &P.TN);
     P.tiles_w = cdiv(g.Wo, P.TW); P.tiles_h = cdiv(g.Ho, P.TH); P.tiles_n = cdiv(g.B, P.TN);
@@ -1239,12 +1134,6 @@ void tc_plan_destroy(TcConvPlan* p) {
   delete p;
 }
 void tc_plan_set_out_scale(TcConvPlan* p, const float* inv_scale) { if (p != nullptr) p->out_scale = inv_scale; }
-int tc_plan_set_cluster(TcConvPlan* p, int cl) {
-  MN_CHECK(p != nullptr && p->kind == 0 && (cl == 1 || cl == 2 || cl == 4), "tc_plan_set_cluster: bad argument");
-  p->CL = cl;
-  p->c_in0 = p->c_in1 = nullptr;        // the weight maps' box depends on CL: encode again at the next run
-  return 0;
-}
 
 // Fold the dgrad of the block's 1x1 / stride-2 downsample conv into the (merged) dgrad of its 3x3 / stride-2 conv1:
 // both produce d(block input), the shortcut only reaches the pixel class (0, 0), where it is one more filter tap
@@ -1280,7 +1169,7 @@ int tc_plan_describe(const TcConvPlan* p, char* buf, int cap) {
     va_end(ap);
     if (w < 0 || w >= cap - n) ovf = true; else n += w;
   };
-  put("{\"kind\":%d,\"BN\":%d,\"CL\":%d,\"shortcut\":%d", p->kind, p->BN, p->CL, p->wmat2 != nullptr ? 1 : 0);
+  put("{\"kind\":%d,\"BN\":%d,\"shortcut\":%d", p->kind, p->BN, p->wmat2 != nullptr ? 1 : 0);
   if (p->kind == 2) {
     const WgradParams& P = p->WP;
     put(",\"wgrad\":{\"TW\":%d,\"TH\":%d,\"TN\":%d,\"tiles_w\":%d,\"tiles_h\":%d,\"tiles_n\":%d,\"n_pix_tiles\":%d,"
@@ -1343,20 +1232,14 @@ static int encode_view(CUtensorMap* m, const bf16* base, int N, int Hd, int Wd, 
 }
 
 int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* residual, void* out, cudaStream_t st,
-                double* stats, const EpiBwd* bwd, const EpiFin* fin, const EpiAffine* aff) {
+                double* stats, const EpiBwd* bwd, const EpiAffine* aff) {
   MN_CHECK(p != nullptr, "tc_conv_run: null plan");
   if (aff != nullptr) {
-    MN_CHECK(p->kind == 0 && stats == nullptr && bwd == nullptr && (fin == nullptr || fin->mode == 0),
+    MN_CHECK(p->kind == 0 && stats == nullptr && bwd == nullptr,
              "tc_conv_run: the affine (inference) epilogue is an fprop epilogue without statistics");
     MN_CHECK(tc_affine_supported(p->g.split != 0, residual != nullptr, *aff),
              "tc_conv_run: affine epilogue variant not built (split %d residual %d relu %d res_split %d out_split %d)",
              p->g.split, residual != nullptr, aff->relu, aff->res_split, aff->out_split);
-  }
-  EpiFin F; memset(&F, 0, sizeof(F));
-  if (fin != nullptr && fin->mode != 0) {
-    MN_CHECK(stats != nullptr && fin->counter != nullptr && p->kind != 2, "tc_conv_run: fused finalize needs statistics accumulators");
-    MN_CHECK((fin->mode == 1) == (bwd == nullptr), "tc_conv_run: finalize mode %d does not match the statistics kind", fin->mode);
-    F = *fin;
   }
   EpiBwd E; memset(&E, 0, sizeof(E));
   if (bwd != nullptr) {
@@ -1384,13 +1267,13 @@ int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* res
         if (p->kind == 0) {
           for (int i = 0; i < L.n_maps; ++i)
             MN_TRY(encode_view(&L.mapA[i], in0, g.B, g.Hi, g.Wi, SP * g.Ci, g.stride, L.pa[i], L.pb[i], L.P.TW, L.P.TH, L.P.TN, &g));
-          MN_TRY(encode_w_map(&L.mapB, p->wmat, SP * g.KH * g.KW * SP * g.Ci, g.Co, p->BN / p->CL));
+          MN_TRY(encode_w_map(&L.mapB, p->wmat, SP * g.KH * g.KW * SP * g.Ci, g.Co, p->BN));
         } else {
           MN_TRY(encode_view(&L.mapA[0], in0, g.B, g.Ho, g.Wo, SP * g.Co, 1, 0, 0, L.P.TW, L.P.TH, L.P.TN));
-          MN_TRY(encode_w_map(&L.mapB, p->wmat, SP * g.KH * g.KW * SP * g.Co, g.Ci, p->BN / p->CL));
+          MN_TRY(encode_w_map(&L.mapB, p->wmat, SP * g.KH * g.KW * SP * g.Co, g.Ci, p->BN));
           if (p->wmat2 != nullptr) {
             MN_TRY(encode_view(&L.mapA[1], in1, g.B, g.Ho, g.Wo, g.Co, 1, 0, 0, L.P.TW, L.P.TH, L.P.TN));
-            MN_TRY(encode_w_map(&L.mapB2, p->wmat2, g.Co, g.Ci, p->BN / p->CL));
+            MN_TRY(encode_w_map(&L.mapB2, p->wmat2, g.Co, g.Ci, p->BN));
             L.n_maps = 2;
           }
         }
@@ -1400,46 +1283,19 @@ int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* res
       p->c_in0 = in0; p->c_in1 = in1;
     }
     const size_t smem = conv_smem_bytes(p->BN);
-    void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, ConvParams, const bf16*, bf16*, double*, EpiBwd, EpiFin) = nullptr;
-#define PICK(BNv, CLv) if (p->BN == BNv && p->CL == CLv) kern = k_tc_conv<BNv, CLv, false>;
-    if (aff != nullptr) {       // inference plans run unclustered (tc_plan_set_cluster)
-      if (p->CL == 1) kern = (p->BN == 64) ? k_tc_conv<64, 1, true> : k_tc_conv<128, 1, true>;
-    } else {
-      PICK(64, 1) PICK(128, 1) PICK(64, 2) PICK(128, 2) PICK(64, 4) PICK(128, 4)
-    }
-#undef PICK
-    MN_CHECK(kern != nullptr, "tc conv: no %s kernel for BN=%d CL=%d", aff ? "inference" : "training", p->BN, p->CL);
+    void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, ConvParams, const bf16*, bf16*, double*, EpiBwd) =
+        (aff != nullptr) ? ((p->BN == 64) ? k_tc_conv<64, true> : k_tc_conv<128, true>)
+                         : ((p->BN == 64) ? k_tc_conv<64> : k_tc_conv<128>);
     if (!p->smem_attr_set || p->smem_attr_aff != (aff != nullptr)) {
       MN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
       p->smem_attr_set = true;
       p->smem_attr_aff = (aff != nullptr);
     }
-    F.expected = 0;
-    for (auto& L : p->launches) {     // the sums of a stride-2 dgrad come from all its parity classes / launches
-      const int groups = cdiv(L.P.n_tiles_m, p->CL) * L.P.n_tiles_n * L.P.n_classes;
-      const int max_clusters = (p->CL == 4) ? 32 : nsm / p->CL;
-      F.expected += (unsigned int)((groups < max_clusters ? groups : max_clusters) * p->CL);
-    }
-    static int epi_pf = -1;
-    // opt-in experiment: the fused dgrad epilogues read extra operands that are mostly L2 hits right behind their
-    // producers
-    if (epi_pf < 0) { const char* e = getenv("MAPNET_TC_EPI_PREFETCH"); epi_pf = e ? atoi(e) : 0; }
     for (auto& L : p->launches) {
-      const int groups = cdiv(L.P.n_tiles_m, p->CL) * L.P.n_tiles_n * L.P.n_classes;
-      const int max_clusters = (p->CL == 4) ? 32 : nsm / p->CL;
-      const int nclusters = groups < max_clusters ? groups : max_clusters;
-      // bf16 epilogues that read extra tensors (the fused dgrad variants): next-tile L2 prefetch
-      L.P.epi_prefetch = (epi_pf && !L.P.out32 && (residual != nullptr || E.y != nullptr)) ? 1 : 0;
-      cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof(cfg));
-      cfg.gridDim = dim3(nclusters * p->CL); cfg.blockDim = dim3(kConvThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-      cudaLaunchAttribute attr[2];
-      attr[0].id = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = p->CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-      attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[1].val.programmaticStreamSerializationAllowed = 1;
-      cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 2 : 1;
-      MN_CUDA(cudaLaunchKernelEx(&cfg, kern, L.mapA[0], L.mapA[1], L.mapA[2], L.mapA[3], L.mapB, L.mapB2, L.P, residual, (bf16*)out, stats, E, F));
-      ++g_launch_count;
+      const int items = L.P.n_tiles_m * L.P.n_tiles_n * L.P.n_classes;     // persistent CTAs: at most one per SM
+      MN_LAUNCH(kern, items < nsm ? items : nsm, kConvThreads, smem, st, L.mapA[0], L.mapA[1], L.mapA[2], L.mapA[3], L.mapB,
+                L.mapB2, L.P, residual, (bf16*)out, stats, E);
+      MN_LAUNCH_CHECK();
     }
     return 0;
   }
@@ -1453,13 +1309,9 @@ int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* res
     MN_TRY(encode_view(&p->mapDY, in1, g.B, g.Ho, g.Wo, SP * g.Co, 1, 0, 0, P.TW, P.TH, P.TN));
     p->c_in0 = in0; p->c_in1 = in1;
   }
-  static int occ = -1;
-  if (occ < 0) { const char* e = getenv("MAPNET_TC_WGRAD_OCC"); occ = (e && atoi(e) == 1) ? 1 : 2; }   // measured: 2 CTAs/SM = 587 -> 781 TF/s on layer3/4 wgrad
-  const int stages = wgrad_stages(p->BN) / occ;
-  const size_t smem = (size_t)stages * (2 * 8192 + (p->BN / 64) * 8192) + 1024;
+  const size_t smem = (size_t)wgrad_stages(p->BN) * (2 * 8192 + (p->BN / 64) * 8192) + 1024;
   void (*k1)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, WgradParams, float*) =
-      (occ == 2) ? ((p->BN == 64) ? k_tc_wgrad<64, 2> : k_tc_wgrad<128, 2>)
-                 : ((p->BN == 64) ? k_tc_wgrad<64, 1> : k_tc_wgrad<128, 1>);
+      (p->BN == 64) ? k_tc_wgrad<64> : k_tc_wgrad<128>;
   if (!p->smem_attr_set) {
     MN_TRY(set_smem(k1, smem));
     p->smem_attr_set = true;

@@ -126,8 +126,7 @@ int InferNet::load(const float* params, const float* bufs, cudaStream_t st) {
   } else {
     float* f32 = nullptr;       // the fp32 K-major matrices the hi / lo planes are cut from (load time only)
     MN_CUDA(cudaMallocAsync((void**)&f32, (size_t)spec.wk_total * 4, st));
-    const int r = launch_pack_weights_split(d_wdescs, nconv, params, f32, nullptr, wk, nullptr, spec.max_w_elems,
-                                            spec.split_fmt_z, spec.split_fmt_g, st);
+    const int r = launch_pack_weights_split(d_wdescs, nconv, params, f32, nullptr, wk, nullptr, spec.max_w_elems, st);
     MN_CUDA(cudaFreeAsync(f32, st));
     MN_TRY(r);
   }
@@ -150,10 +149,9 @@ int InferNet::ensure_plans(int B) {
   const bool sp = precision == PREC_TC_SPLIT;
   for (size_t i = 0; i < spec.convs.size(); ++i) {
     ConvGeom g = spec.convs[i].g; g.B = B;
-    if (sp) { g.split = 1; g.fmt_z = spec.split_fmt_z; g.fmt_g = spec.split_fmt_g; }
+    if (sp) g.split = 1;
     const bf16* w = (const bf16*)wk + (sp ? 4 : 1) * spec.convs[i].wd.k_off;
     MN_TRY(tc_plan_create(&plans[i], g, 0, w));
-    MN_TRY(tc_plan_set_cluster(plans[i], 1));
   }
   plan_B = B;
   return 0;
@@ -164,7 +162,7 @@ int InferNet::conv(int ci, const void* in, const void* residual, void* out, int 
   const int bi = spec.convs[ci].bn;
   EpiAffine a;
   a.scale = bn_scale[bi]; a.shift = bn_shift[bi]; a.relu = relu; a.res_split = res_split; a.out_split = out_split;
-  return tc_conv_run(plans[ci], (const bf16*)in, nullptr, (const bf16*)residual, out, st, nullptr, nullptr, nullptr, &a);
+  return tc_conv_run(plans[ci], (const bf16*)in, nullptr, (const bf16*)residual, out, st, nullptr, nullptr, &a);
 }
 
 template <typename P>

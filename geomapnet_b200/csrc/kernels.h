@@ -14,8 +14,8 @@ struct ConvGeom {
   long long in_pix_stride = 0, in_row_stride = 0, in_img_stride = 0;
   // tensor-core path, strict mode: activations / gradients are split 16-bit operand planes (common.cuh: hsplit,
   // 2*C 16-bit "channels" per pixel), the weight matrices hold hi and lo planes as 2*KH*KW taps (layout.cu),
-  // outputs are fp32.  fmt_z / fmt_g: element format of the forward / backward operands (0 = fp16, 1 = bf16).
-  int split = 0, fmt_z = 1, fmt_g = 1;
+  // outputs are fp32.  The planes are fp16.
+  int split = 0;
   __host__ __device__ long long M_out() const { return (long long)B * Ho * Wo; }
   __host__ __device__ long long M_in() const { return (long long)B * Hi * Wi; }
   __host__ __device__ int Kdim() const { return KH * KW * Ci; }
@@ -74,8 +74,6 @@ int tc_plan_launches(const TcConvPlan* p);
 // dgrad / wgrad plans: multiply the accumulators by the device scalar *inv_scale before they are added to the residual /
 // the wgrad buffer (strict mode: the gradient operand planes carry a per-step power-of-two scale)
 void tc_plan_set_out_scale(TcConvPlan* p, const float* inv_scale);
-// fprop plans: thread-block cluster size (default MAPNET_TC_CLUSTER or 1); the inference epilogues are built for 1 only
-int tc_plan_set_cluster(TcConvPlan* p, int cl);
 int tc_plan_describe(const TcConvPlan* p, char* buf, int cap);      // JSON, host-only (CPU tests of the plan arithmetic)
 // fprop: in0 = x, out = y (bf16);  dgrad: in0 = dy [, in1 = the folded shortcut's dy], out = dx (bf16);
 // wgrad: in0 = x, in1 = dy, out = fp32 dW (accumulated)
@@ -109,20 +107,14 @@ struct EpiAffine {
   int relu, res_split, out_split;
 };
 bool tc_affine_supported(bool split, bool residual, const EpiAffine& a);
-// fin != nullptr (with stats): the last CTA to flush its sums also finalizes them (bn_fin.cuh) -- forward:
-// mean / invstd / scale / shift / running statistics; backward: d gamma, d beta, dy coefficients
-struct EpiFin;
 int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* residual, void* out, cudaStream_t st,
-                double* stats = nullptr, const EpiBwd* bwd = nullptr, const EpiFin* fin = nullptr,
-                const EpiAffine* aff = nullptr);
-// finalize of the dgrad-fused reductions: d gamma, d beta and the dy = A*g + B*y + C coefficients
+                double* stats = nullptr, const EpiBwd* bwd = nullptr, const EpiAffine* aff = nullptr);
+// finalize of backward reductions accumulated in `accum` (the stem's pool backward in the CUDA-core modes): d gamma,
+// d beta and the dy = A*g + B*y + C coefficients
 int launch_bn_bwd_finalize_accum(long long M, int C, const float* gamma, const float* mean, const float* invstd,
                                  float* dgamma, float* dbeta, float* coef, const float* gamma2, const float* mean2,
                                  const float* invstd2, float* dgamma2, float* dbeta2, float* coef2, double* accum,
                                  cudaStream_t st);
-int launch_bn_finalize_accum(long long M, int C, const float* gamma, const float* beta, float* run_mean,
-                             float* run_var, float* mean_out, float* invstd_out, float* scale, float* shift,
-                             double* accum, cudaStream_t st);
 
 // true when the driver accepts a tiled tensor map whose second dimension's stride is smaller than the
 // first dimension's extent (overlapping windows) -- what the space-to-depth stem view needs
@@ -139,11 +131,11 @@ struct WeightDesc {   // one conv's weight in the flat parameter buffer and in t
 template <typename TW>
 int launch_pack_weights(const WeightDesc* d_descs, int nconv, const float* params, TW* w_krsc, TW* w_dg,
                         int max_elems, int round_bf16, cudaStream_t st);
-// strict tensor-core mode: hi / lo operand planes of the weights (layout.cu); fmt 0 = fp16, 1 = bf16
+// strict tensor-core mode: fp16 hi / lo operand planes of the weights (layout.cu)
 int launch_pack_weights_split(const WeightDesc* d_descs, int nconv, const float* params, float* w_krsc_f32, float* w_dg_f32,
-                              void* w_krsc2, void* w_dg2, int max_elems, int fmt_f, int fmt_g, cudaStream_t st);
-int launch_split_tensor(const float* in, void* out, long long n, int fmt, cudaStream_t st);
-int launch_split_weight_matrix(const float* w, void* out, long long rows, int KK, int C, int fmt, cudaStream_t st);
+                              void* w_krsc2, void* w_dg2, int max_elems, cudaStream_t st);
+int launch_split_tensor(const float* in, void* out, long long n, cudaStream_t st);
+int launch_split_weight_matrix(const float* w, void* out, long long rows, int KK, int C, cudaStream_t st);
 int launch_unpack_wgrads(const WeightDesc* d_descs, int nconv, const float* dw_krsc, float* grads,
                          int max_elems, cudaStream_t st);
 // space-to-depth image of the stem input: S[b][bh][bw][16] bf16, channel (pr*2+pc)*3+c of block (bh,bw)

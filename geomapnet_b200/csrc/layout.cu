@@ -124,13 +124,12 @@ template int launch_pack_weights<bf16>(const WeightDesc*, int, const float*, bf1
 //   tap  KK + t   holds lo(w) in both,
 // so an activation row [xh xl] (the same 8-interleaved K order) against the two taps gives
 // xh*wh + xl*wh + xh*wl + xl*wl = (xh + xl) * (wh + wl): every hi/lo cross product, fp32-accumulated by the tensor cores.
-//   w_krsc2[co][2*KK][2*Ci]   (fprop; element format fmt_f: 0 fp16, 1 bf16)
-//   w_dg2  [ci][2*KK][2*Co]   (dgrad; element format fmt_g)
+//   w_krsc2[co][2*KK][2*Ci]   (fprop, fp16 planes)
+//   w_dg2  [ci][2*KK][2*Co]   (dgrad, fp16 planes)
 // The stem's patch-matrix row (im2col_k, or 256 for the space-to-depth stem) is treated as ONE tap of that many channels.
 // Element offsets into the packed buffers are 4 x the bf16 ones (WeightDesc::k_off * 4).
 // ---------------------------------------------------------------------------------
-__device__ __forceinline__ void split16(float v, int fmt, uint16_t& hi, uint16_t& lo) {
-  (void)fmt;                 // only fp16 planes are built (0); the parameter documents the operand format
+__device__ __forceinline__ void split16(float v, uint16_t& hi, uint16_t& lo) {
   __half h, l; split_f16(v, h, l);
   hi = __half_as_ushort(h); lo = __half_as_ushort(l);
 }
@@ -141,7 +140,7 @@ __device__ __forceinline__ int split_k(int c, int p) { return ((c >> 3) << 4) + 
 // fprop / wgrad, rows = Ci, C = Co for dgrad); one thread converts 8 channels: coalesced 32-byte loads and stores
 __global__ void __launch_bounds__(256)
 k_split_weight_rows(const WeightDesc* __restrict__ descs, const float* __restrict__ w_krsc, const float* __restrict__ w_dg,
-                    uint16_t* __restrict__ w_krsc2, uint16_t* __restrict__ w_dg2, int fmt_f, int fmt_g) {
+                    uint16_t* __restrict__ w_krsc2, uint16_t* __restrict__ w_dg2) {
   pdl_prologue();
   const WeightDesc d = descs[blockIdx.y];
   const bool dg = blockIdx.z != 0;
@@ -151,7 +150,6 @@ k_split_weight_rows(const WeightDesc* __restrict__ descs, const float* __restric
   const int rows = dg ? d.Ci : d.Co;
   const float* src = (dg ? w_dg : w_krsc) + d.k_off;
   uint16_t* dst = (dg ? w_dg2 : w_krsc2) + 4 * d.k_off;
-  const int fmt = dg ? fmt_g : fmt_f;
   const int cv = C >> 3;
   const long long nvec = (long long)rows * KK * cv;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += (long long)gridDim.x * blockDim.x) {
@@ -164,7 +162,7 @@ k_split_weight_rows(const WeightDesc* __restrict__ descs, const float* __restric
     uint16_t* h = reinterpret_cast<uint16_t*>(&H);
     uint16_t* l = reinterpret_cast<uint16_t*>(&L);
 #pragma unroll
-    for (int k = 0; k < 8; ++k) split16(v.v[k], fmt, h[k], l[k]);
+    for (int k = 0; k < 8; ++k) split16(v.v[k], h[k], l[k]);
     uint4* o0 = reinterpret_cast<uint4*>(dst + ((r * 2 * KK + t) * 2 * C + c8 * 16));
     uint4* o1 = reinterpret_cast<uint4*>(dst + ((r * 2 * KK + KK + t) * 2 * C + c8 * 16));
     o0[0] = H; o0[1] = H; o1[0] = L; o1[1] = L;
@@ -173,18 +171,18 @@ k_split_weight_rows(const WeightDesc* __restrict__ descs, const float* __restric
 
 // w_krsc_f32 / w_dg_f32: scratch for the fp32 K-major matrices (wk_total floats each)
 int launch_pack_weights_split(const WeightDesc* d_descs, int nconv, const float* params, float* w_krsc_f32, float* w_dg_f32,
-                              void* w_krsc2, void* w_dg2, int max_elems, int fmt_f, int fmt_g, cudaStream_t st) {
+                              void* w_krsc2, void* w_dg2, int max_elems, cudaStream_t st) {
   MN_TRY(launch_pack_weights<float>(d_descs, nconv, params, w_krsc_f32, w_dg2 != nullptr ? w_dg_f32 : nullptr, max_elems, 0, st));
   dim3 grid(64, nconv, w_dg2 != nullptr ? 2 : 1);
   MN_LAUNCH(k_split_weight_rows, grid, 256, 0, st, d_descs, (const float*)w_krsc_f32, (const float*)w_dg_f32,
-            (uint16_t*)w_krsc2, (uint16_t*)w_dg2, fmt_f, fmt_g);
+            (uint16_t*)w_krsc2, (uint16_t*)w_dg2);
   MN_LAUNCH_CHECK();
   return 0;
 }
 
 // one fp32 K-major matrix [rows][KK][C] -> [rows][2*KK][2*C] hi / lo planes (test entry points)
 __global__ void __launch_bounds__(256)
-k_split_weight_matrix(const float* __restrict__ src, uint16_t* __restrict__ dst, long long rows, int KK, int C, int fmt) {
+k_split_weight_matrix(const float* __restrict__ src, uint16_t* __restrict__ dst, long long rows, int KK, int C) {
   pdl_prologue();
   const int cv = C >> 3;
   const long long nvec = rows * KK * cv;
@@ -198,15 +196,15 @@ k_split_weight_matrix(const float* __restrict__ src, uint16_t* __restrict__ dst,
     uint16_t* h = reinterpret_cast<uint16_t*>(&H);
     uint16_t* l = reinterpret_cast<uint16_t*>(&L);
 #pragma unroll
-    for (int k = 0; k < 8; ++k) split16(v.v[k], fmt, h[k], l[k]);
+    for (int k = 0; k < 8; ++k) split16(v.v[k], h[k], l[k]);
     uint4* o0 = reinterpret_cast<uint4*>(dst + ((r * 2 * KK + t) * 2 * C + c8 * 16));
     uint4* o1 = reinterpret_cast<uint4*>(dst + ((r * 2 * KK + KK + t) * 2 * C + c8 * 16));
     o0[0] = H; o0[1] = H; o1[0] = L; o1[1] = L;
   }
 }
-int launch_split_weight_matrix(const float* w, void* out, long long rows, int KK, int C, int fmt, cudaStream_t st) {
+int launch_split_weight_matrix(const float* w, void* out, long long rows, int KK, int C, cudaStream_t st) {
   MN_CHECK(C % 8 == 0, "split_weight_matrix: C must be a multiple of 8");
-  MN_LAUNCH(k_split_weight_matrix, 256, 256, 0, st, w, (uint16_t*)out, rows, KK, C, fmt);
+  MN_LAUNCH(k_split_weight_matrix, 256, 256, 0, st, w, (uint16_t*)out, rows, KK, C);
   MN_LAUNCH_CHECK();
   return 0;
 }
@@ -224,11 +222,10 @@ __global__ void __launch_bounds__(256) k_split_tensor(const float* __restrict__ 
     o.store(out + i * 8);
   }
 }
-int launch_split_tensor(const float* in, void* out, long long n, int fmt, cudaStream_t st) {
+int launch_split_tensor(const float* in, void* out, long long n, cudaStream_t st) {
   MN_CHECK(n % 8 == 0, "split_tensor: element count must be a multiple of 8");
   const long long nvec = n / 8;
   long long grid = (nvec + 255) / 256; if (grid > kNumSMs * 8) grid = kNumSMs * 8; if (grid < 1) grid = 1;
-  MN_CHECK(fmt == 0, "split_tensor: only fp16 planes are built");
   MN_LAUNCH(k_split_tensor<hsplit>, (int)grid, 256, 0, st, in, (hsplit*)out, nvec);
   MN_LAUNCH_CHECK();
   return 0;

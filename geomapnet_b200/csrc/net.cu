@@ -144,27 +144,15 @@ int Net::init(int max_B_, int H_, int W_, int feat_dim_, int precision_) {
   max_B = max_B_; H = H_; W = W_; feat_dim = feat_dim_; precision = precision_;
   MN_CHECK(max_B >= 0 && H >= 32 && W >= 32, "create: need max_B>=0 and H,W>=32 (got %d,%d,%d)", max_B, H, W);
   MN_CHECK(precision >= 0 && precision <= 3, "create: bad precision %d", precision);
-  // strict tensor-core mode: forward AND backward conv operands are fp16 hi/lo planes.  (bf16 planes for the gradients
-  // would need no scaling, but wgrad multiplies activations by gradients and wgmma takes A and B in ONE element
-  // format: fp16 x bf16 does not exist.)
-  split_fmt_z = 0; split_fmt_g = 0;
   MN_CHECK(feat_dim >= 8 && feat_dim % 4 == 0, "create: feat_dim must be a multiple of 4");
   last_B = 0; last_training = 0; last_has_mask = 0; tc_B = 0; profile_on = 0; prof_pool_used = 0;
   bwd_pre = false; bwd_next_part = 0;
-  side = nullptr; wgrad_async = 0; ring_pos = 0; cur_grads = nullptr; dw_stem_elems = 0;
+  side = nullptr; ring_pos = 0; cur_grads = nullptr; dw_stem_elems = 0;
   for (int i = 0; i < 4; ++i) { ring[i] = nullptr; ring_ready[i] = ring_done[i] = nullptr; ring_pending[i] = false; }
-  { const char* e = getenv("MAPNET_TC_FUSE_STATS"); fuse_stats = tc() && (e ? atoi(e) != 0 : 1); }
-  { const char* e = getenv("MAPNET_STEM_S2D");
-    stem_s2d = tc() && (e ? atoi(e) != 0 : 1) && (max_B == 0 || tc_overlapped_view_supported()); }
+  stem_s2d = tc() && (max_B == 0 || tc_overlapped_view_supported());
   Hc = conv_out(H, 7, 2, 3); Wc = conv_out(W, 7, 2, 3);        // (build_table sets them again)
-  { const char* e = getenv("MAPNET_STEM_FUSE"); stem_fuse = (e ? atoi(e) != 0 : 1) && (Hc % 2 == 0) && (Wc % 2 == 0); }
-  // finalizing inside the conv's last CTA costs every CTA a fence + counter round trip and the last one a serial tail;
-  // the separate (PDL-overlapped) finalize launches are the default
-  { const char* e = getenv("MAPNET_TC_FUSE_FIN"); fuse_fin = (precision == PREC_BF16_TC) && (e ? atoi(e) != 0 : 0); }
+  stem_fuse = (Hc % 2 == 0) && (Wc % 2 == 0);
   { const char* e = getenv("MAPNET_TC_FUSE_BWD"); fuse_bwd = (precision == PREC_BF16_TC) && (e ? atoi(e) != 0 : 1); }
-  // with the lazy finalize the consuming element-wise kernels do the BatchNorm finalize work in their prologue instead
-  // of 68 separate finalize launches per step
-  { const char* e = getenv("MAPNET_BN_LAZY_FIN"); lazy_fin = (fuse_stats && !fuse_fin && (e ? atoi(e) != 0 : 1)) ? 1 : 0; }
   stats_target = nullptr; bn_slots = nullptr; bn_slots_bytes = 0;
   { const char* e = getenv("MAPNET_TC_DS_FOLD"); ds_fold = (precision == PREC_BF16_TC) && (e ? atoi(e) != 0 : 1); }
   build_table();
@@ -179,7 +167,6 @@ int Net::init(int max_B_, int H_, int W_, int feat_dim_, int precision_) {
   for (int i = 0; i < 7; ++i) MN_TRY(alloc(&scratch[i], (size_t)scratch_elems * es));
   ring[0] = scratch[1]; ring[1] = scratch[2]; ring[2] = scratch[5]; ring[3] = scratch[6];
   ring_pos = 0;
-  { const char* e = getenv("MAPNET_WGRAD_ASYNC"); wgrad_async = e ? (atoi(e) != 0) : 1; }
   {
     int lo = 0, hi = 0;
     MN_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));       // lo = numerically greatest = lowest priority
@@ -321,15 +308,13 @@ template <typename P> struct SimtConv {
 };
 
 template <typename P>
-int Net::conv_fprop(int ci, const typename P::Z* x, const typename P::A* residual, typename P::A* y, int B, cudaStream_t st,
-                    bool with_stats, const EpiFin* fin) {
+int Net::conv_fprop(int ci, const typename P::Z* x, const typename P::A* residual, typename P::A* y, int B, cudaStream_t st) {
   ConvGeom g = convs[ci].g; g.B = B;
   cudaEvent_t e0 = nullptr;
   MN_TRY(prof_begin(st, &e0));
   int r;
   if (tc())
-    r = tc_conv_run(tc_fprop[ci], (const bf16*)x, nullptr, (const bf16*)residual, y, st, (with_stats && fuse_stats) ? (stats_target ? stats_target : bn_accum) : nullptr,
-                    nullptr, (with_stats && fuse_stats) ? fin : nullptr);
+    r = tc_conv_run(tc_fprop[ci], (const bf16*)x, nullptr, (const bf16*)residual, y, st, stats_target);
   else if constexpr (SimtConv<P>::ok)
     r = launch_conv_simt_fprop<typename P::A>(g, x, (const float*)w_krsc + convs[ci].wd.k_off, residual, y, st);
   else { set_last_error("conv_fprop: no CUDA-core engine for split operands"); r = 2; }
@@ -338,7 +323,7 @@ int Net::conv_fprop(int ci, const typename P::Z* x, const typename P::A* residua
 }
 template <typename P>
 int Net::conv_dgrad(int ci, const typename P::G* dy, const typename P::A* residual, typename P::A* dx, int B, cudaStream_t st,
-                    const EpiBwd* bwd, const EpiFin* fin, const typename P::G* dy_shortcut, int ci_shortcut) {
+                    const EpiBwd* bwd, const typename P::G* dy_shortcut, int ci_shortcut) {
   ConvGeom g = convs[ci].g; g.B = B;
   cudaEvent_t e0 = nullptr;
   MN_TRY(prof_begin(st, &e0));
@@ -346,8 +331,7 @@ int Net::conv_dgrad(int ci, const typename P::G* dy, const typename P::A* residu
   double flops = conv_flops(g, B, false);
   if (tc()) {
     // dy_shortcut: the block's downsample-conv dgrad rides in the same launch (tc_plan_add_shortcut)
-    r = tc_conv_run(tc_dgrad[ci], (const bf16*)dy, (const bf16*)dy_shortcut, (const bf16*)residual, dx, st, bwd ? (stats_target ? stats_target : bn_accum) : nullptr, bwd,
-                    bwd ? fin : nullptr);
+    r = tc_conv_run(tc_dgrad[ci], (const bf16*)dy, (const bf16*)dy_shortcut, (const bf16*)residual, dx, st, bwd ? stats_target : nullptr, bwd);
     if (dy_shortcut != nullptr) { ConvGeom gs = convs[ci_shortcut].g; gs.B = B; flops += conv_flops(gs, B, false); }
   } else if constexpr (SimtConv<P>::ok) {
     MN_CHECK(dy_shortcut == nullptr, "conv_dgrad: folded shortcut is a tensor-core path feature");
@@ -376,7 +360,7 @@ template <typename P>
 int Net::conv_wgrad(int ci, const typename P::Z* x, const typename P::G* dy, int B, cudaStream_t st) {
   ConvGeom g = convs[ci].g; g.B = B;
   const int slot = ring_slot(dy);
-  if (wgrad_async && !profile_on && slot >= 0) {
+  if (!profile_on && slot >= 0) {
     // fork: the side stream picks the gradient up where the compute stream has just finished writing it
     MN_CUDA(cudaEventRecord(ring_ready[slot], st));
     MN_CUDA(cudaStreamWaitEvent(side, ring_ready[slot], 0));
@@ -409,13 +393,13 @@ int Net::ensure_tc_plans(int B) {
   for (size_t i = 0; i < convs.size(); ++i) {
     ConvGeom g = convs[i].g; g.B = B;
     const bool sp = precision == PREC_TC_SPLIT;
-    if (sp) { g.split = 1; g.fmt_z = split_fmt_z; g.fmt_g = split_fmt_g; }
+    if (sp) g.split = 1;
     const bf16* wk = (const bf16*)w_krsc + (sp ? 4 : 1) * convs[i].wd.k_off;     // split planes: 4 x the 16-bit elements
     const bf16* wd = (const bf16*)w_dg + (sp ? 4 : 1) * convs[i].wd.k_off;
     MN_TRY(tc_plan_create(&tc_fprop[i], g, 0, wk));
     if (i > 0) MN_TRY(tc_plan_create(&tc_dgrad[i], g, 1, wd));
     MN_TRY(tc_plan_create(&tc_wgrad[i], g, 2, nullptr));
-    if (sp && split_fmt_g == 0) {       // fp16 gradient planes carry the step's power-of-two scale: divide it out
+    if (sp) {       // fp16 gradient planes carry the step's power-of-two scale: divide it out
       if (i > 0) tc_plan_set_out_scale(tc_dgrad[i], gscale + 1);
       tc_plan_set_out_scale(tc_wgrad[i], gscale + 1);
     }
@@ -437,10 +421,6 @@ int Net::bn_forward(int bi, const typename P::A* y, long long M, const float* pa
                     cudaStream_t st) {
   typedef typename P::A T;
   BNL& b = bns[bi];
-  if (fuse_stats && training && fuse_fin) return 0;   // the conv's last CTA finalized the statistics
-  if (fuse_stats && training)   // sums were accumulated by the conv epilogue
-    return launch_bn_finalize_accum(M, b.C, params + b.g_off, params + b.b_off, bufs + b.rm_off, bufs + b.rv_off,
-                                    b.mean, b.invstd, b.scale, b.shift, bn_accum, st);
   return launch_bn_stats<T>(y, M, b.C, params + b.g_off, params + b.b_off, bufs + b.rm_off, bufs + b.rv_off,
                             b.mean, b.invstd, b.scale, b.shift, training, bn_accum, bn_counter, st);
 }
@@ -470,31 +450,6 @@ BnLazy Net::lazy_backward(int bi, int bi_ds, long long M, const float* params, f
   return L;
 }
 
-// finalize descriptors for the conv kernels (conv_tc.cu: the last CTA finalizes the sums it helped accumulate)
-EpiFin Net::fin_forward(int bi, long long M, const float* params, float* bufs) {
-  EpiFin F; memset(&F, 0, sizeof(F));
-  if (!(fuse_fin && fuse_stats)) return F;
-  BNL& b = bns[bi];
-  F.mode = 1; F.counter = bn_counter; F.M = M;
-  F.f.gamma = params + b.g_off; F.f.beta = params + b.b_off; F.f.run_mean = bufs + b.rm_off; F.f.run_var = bufs + b.rv_off;
-  F.f.mean = b.mean; F.f.invstd = b.invstd; F.f.scale = b.scale; F.f.shift = b.shift; F.f.training = 1;
-  return F;
-}
-EpiFin Net::fin_backward(int bi, int bi_ds, long long M, const float* params, float* grads) {
-  EpiFin F; memset(&F, 0, sizeof(F));
-  if (!(fuse_fin && fuse_bwd)) return F;
-  BNL& b = bns[bi];
-  F.mode = (bi_ds >= 0) ? 3 : 2; F.counter = bn_counter; F.M = M;
-  F.f.gamma = params + b.g_off; F.f.mean = b.mean; F.f.invstd = b.invstd;
-  F.f.dgamma = grads + b.g_off; F.f.dbeta = grads + b.b_off; F.f.coef = b.coef;
-  if (bi_ds >= 0) {
-    BNL& d = bns[bi_ds];
-    F.f.gamma2 = params + d.g_off; F.f.mean2 = d.mean; F.f.invstd2 = d.invstd;
-    F.f.dgamma2 = grads + d.g_off; F.f.dbeta2 = grads + d.b_off; F.f.coef2 = d.coef;
-  }
-  return F;
-}
-
 // ---- forward -------------------------------------------------------------------
 template <typename P>
 int Net::forward_t(const float* x, const float* params, float* bufs, int B, int training, float droprate,
@@ -506,8 +461,7 @@ int Net::forward_t(const float* x, const float* params, float* bufs, int B, int 
   if (precision == PREC_BF16_TC)
     MN_TRY(launch_pack_weights<bf16>(d_wdescs, (int)convs.size(), params, (bf16*)w_krsc, (bf16*)w_dg, max_w_elems, 0, st));
   else if (precision == PREC_TC_SPLIT)
-    MN_TRY(launch_pack_weights_split(d_wdescs, (int)convs.size(), params, w_krsc_f32, w_dg_f32, w_krsc, w_dg, max_w_elems,
-                                     split_fmt_z, split_fmt_g, st));
+    MN_TRY(launch_pack_weights_split(d_wdescs, (int)convs.size(), params, w_krsc_f32, w_dg_f32, w_krsc, w_dg, max_w_elems, st));
   else
     MN_TRY(launch_pack_weights<float>(d_wdescs, (int)convs.size(), params, (float*)w_krsc, (float*)w_dg, max_w_elems,
                                       precision == PREC_BF16_SIMT, st));
@@ -519,13 +473,10 @@ int Net::forward_t(const float* x, const float* params, float* bufs, int B, int 
   else MN_TRY(launch_stem_im2col<TZ>(x, (TZ*)A0, B, H, W, Hc, Wc, kStemK, st));
   // lazy finalize: the conv epilogues accumulate into per-BatchNorm slots (zeroed here, once per step, for both passes)
   // and the consuming element-wise kernels finalize them -- no finalize launches
-  const bool lazy = lazy_fin && training;
+  const bool lazy = tc() && training;
   if (lazy) MN_CUDA(cudaMemsetAsync(bn_slots, 0, bn_slots_bytes, st));
-  {
-    const EpiFin f0 = fin_forward(convs[0].bn, (long long)B * Hc * Wc, params, bufs);
-    stats_target = lazy ? fwd_slot(convs[0].bn) : nullptr;
-    MN_TRY(conv_fprop<P>(0, (const TZ*)A0, nullptr, (T*)y0, B, st, training != 0, &f0));
-  }
+  stats_target = lazy ? fwd_slot(convs[0].bn) : nullptr;
+  MN_TRY(conv_fprop<P>(0, (const TZ*)A0, nullptr, (T*)y0, B, st));
   if (!lazy) MN_TRY(bn_forward<P>(convs[0].bn, (const T*)y0, (long long)B * Hc * Wc, params, bufs, training, st));
   {
     BNL& b = bns[convs[0].bn];
@@ -537,24 +488,21 @@ int Net::forward_t(const float* x, const float* params, float* bufs, int B, int 
     const long long Mo = (long long)B * bl.Ho * bl.Wo;
     BNL& b1 = bns[convs[bl.conv1].bn];
     BNL& b2 = bns[convs[bl.conv2].bn];
-    const EpiFin f1 = fin_forward(convs[bl.conv1].bn, Mo, params, bufs);
-    const EpiFin f2 = fin_forward(convs[bl.conv2].bn, Mo, params, bufs);
     const BnLazy l1 = lazy_forward(convs[bl.conv1].bn, Mo, params, bufs);
     const BnLazy l2 = lazy_forward(convs[bl.conv2].bn, Mo, params, bufs);
     stats_target = lazy ? fwd_slot(convs[bl.conv1].bn) : nullptr;
-    MN_TRY(conv_fprop<P>(bl.conv1, zin, nullptr, (T*)bl.y1, B, st, training != 0, &f1));
+    MN_TRY(conv_fprop<P>(bl.conv1, zin, nullptr, (T*)bl.y1, B, st));
     if (!lazy) MN_TRY(bn_forward<P>(convs[bl.conv1].bn, (const T*)bl.y1, Mo, params, bufs, training, st));
     MN_TRY((launch_bn_apply<T, TZ>((const T*)bl.y1, b1.scale, b1.shift, 0, nullptr, nullptr, nullptr, (TZ*)bl.h, Mo, bl.Cout, 1, st,
                                    lazy ? &l1 : nullptr)));
     stats_target = lazy ? fwd_slot(convs[bl.conv2].bn) : nullptr;
-    MN_TRY(conv_fprop<P>(bl.conv2, (const TZ*)bl.h, nullptr, (T*)bl.y2, B, st, training != 0, &f2));
+    MN_TRY(conv_fprop<P>(bl.conv2, (const TZ*)bl.h, nullptr, (T*)bl.y2, B, st));
     if (!lazy) MN_TRY(bn_forward<P>(convs[bl.conv2].bn, (const T*)bl.y2, Mo, params, bufs, training, st));
     if (bl.convd >= 0) {
       BNL& bd = bns[convs[bl.convd].bn];
-      const EpiFin fd = fin_forward(convs[bl.convd].bn, Mo, params, bufs);
       const BnLazy ld = lazy_forward(convs[bl.convd].bn, Mo, params, bufs);
       stats_target = lazy ? fwd_slot(convs[bl.convd].bn) : nullptr;
-      MN_TRY(conv_fprop<P>(bl.convd, zin, nullptr, (T*)bl.yd, B, st, training != 0, &fd));
+      MN_TRY(conv_fprop<P>(bl.convd, zin, nullptr, (T*)bl.yd, B, st));
       if (!lazy) MN_TRY(bn_forward<P>(convs[bl.convd].bn, (const T*)bl.yd, Mo, params, bufs, training, st));
       MN_TRY((launch_bn_apply<T, TZ>((const T*)bl.y2, b2.scale, b2.shift, 2, bl.yd, bd.scale, bd.shift, (TZ*)bl.out, Mo, bl.Cout, 1, st,
                                      lazy ? &l2 : nullptr, lazy ? &ld : nullptr)));
@@ -628,7 +576,7 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
   float* dpredh = dpredf + (size_t)max_B * 6;         // second filtered copy (gradient into the trunk)
   // strict mode: the backward conv operands are fp16 planes; ONE power-of-two scale per step (from max|d pred|)
   // places every gradient tensor inside fp16's window, the consuming conv epilogues divide it out again
-  const float* gs = (precision == PREC_TC_SPLIT && split_fmt_g == 0) ? gscale : nullptr;
+  const float* gs = (precision == PREC_TC_SPLIT) ? gscale : nullptr;
   if (do_head) {
   MN_TRY(launch_dpred_filter(dpred, dpredf, dpredh, B, filter_nans, st));
   if (gs != nullptr) MN_TRY(launch_grad_scale(dpredh, B * 6, gscale, st));
@@ -648,8 +596,8 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
 
   // ---- residual blocks, last to first ----
   // fuse_bwd (wgmma path): the dgrad that PRODUCES a BatchNorm's incoming gradient gates it with that
-  // BN's ReLU and accumulates its backward reductions in the epilogue (conv_tc.cu, EpiBwd), so only a tiny
-  // finalize and the apply pass remain.  `pre` = S0 arrives gated with the BN2 sums of this block pending.
+  // BN's ReLU and accumulates its backward reductions in the epilogue (conv_tc.cu, EpiBwd), so only the apply pass
+  // remains, and it finalizes the sums itself (BnLazy).  `pre` = S0 arrives gated with the BN2 sums of this block pending.
   bool pre = bwd_pre;
   int conv_lo = (int)convs.size(), conv_hi = -1;       // convs whose weight gradients this call completes
   for (int bi = (int)blocks.size() - 1; bi >= 0; --bi) {
@@ -671,12 +619,8 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
       BNL& bd = bns[convs[bl.convd].bn];
       if (pre) {
         const BnLazy lz = lazy_backward(convs[bl.conv2].bn, convs[bl.convd].bn, Mo, params, grads);
-        if (!fuse_fin && !lazy_fin)
-          MN_TRY(launch_bn_bwd_finalize_accum(Mo, C, params + b2.g_off, b2.mean, b2.invstd, grads + b2.g_off, grads + b2.b_off, b2.coef,
-                                              params + bd.g_off, bd.mean, bd.invstd, grads + bd.g_off, grads + bd.b_off, bd.coef,
-                                              bn_accum, st));
         MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S0, nullptr, (const T*)bl.y2, b2.coef, S1, (const T*)bl.yd, bd.coef, S2, nullptr, Mo, C, st, nullptr, nullptr, gs,
-                                               lazy_fin ? &lz : nullptr)));
+                                               &lz)));
       } else {
         MN_TRY((launch_bn_bwd_reduce<T, TZ>(S0, (const TZ*)bl.out, (const T*)bl.y2, (const T*)bl.yd, Mo, C,
                                        params + b2.g_off, b2.mean, b2.invstd, grads + b2.g_off, grads + b2.b_off, b2.coef,
@@ -686,11 +630,8 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
       }
     } else if (pre) {
       const BnLazy lz = lazy_backward(convs[bl.conv2].bn, -1, Mo, params, grads);
-      if (!fuse_fin && !lazy_fin)
-        MN_TRY(launch_bn_bwd_finalize_accum(Mo, C, params + b2.g_off, b2.mean, b2.invstd, grads + b2.g_off, grads + b2.b_off, b2.coef,
-                                            nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, bn_accum, st));
       MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S0, nullptr, (const T*)bl.y2, b2.coef, S1, nullptr, nullptr, nullptr, nullptr, Mo, C, st, nullptr, nullptr, gs,
-                                             lazy_fin ? &lz : nullptr)));
+                                             &lz)));
       gres = S0;              // already gated; conv1's dgrad adds it in place
     } else {
       MN_TRY((launch_bn_bwd_reduce<T, TZ>(S0, (const TZ*)bl.out, (const T*)bl.y2, nullptr, Mo, C,
@@ -707,16 +648,12 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
     if (fuse_bwd) {
       EpiBwd e1; memset(&e1, 0, sizeof(e1));
       e1.y = (const bf16*)bl.y1; e1.mscale = b1.scale; e1.mshift = b1.shift;
-      const EpiFin fb1 = fin_backward(convs[bl.conv1].bn, -1, Mo, params, grads);
       const BnLazy lz1 = lazy_backward(convs[bl.conv1].bn, -1, Mo, params, grads);
-      stats_target = lazy_fin ? bwd_slot(convs[bl.conv1].bn) : nullptr;
-      MN_TRY(conv_dgrad<P>(bl.conv2, dy2, nullptr, S4, B, st, &e1, &fb1));
+      stats_target = bwd_slot(convs[bl.conv1].bn);
+      MN_TRY(conv_dgrad<P>(bl.conv2, dy2, nullptr, S4, B, st, &e1));
       stats_target = nullptr;
-      if (!fuse_fin && !lazy_fin)
-        MN_TRY(launch_bn_bwd_finalize_accum(Mo, C, params + b1.g_off, b1.mean, b1.invstd, grads + b1.g_off, grads + b1.b_off, b1.coef,
-                                            nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, bn_accum, st));
       MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S4, nullptr, (const T*)bl.y1, b1.coef, S1, nullptr, nullptr, nullptr, nullptr, Mo, C, st, nullptr, nullptr, gs,
-                                             lazy_fin ? &lz1 : nullptr)));
+                                             &lz1)));
     } else {
       MN_TRY(conv_dgrad<P>(bl.conv2, dy2, nullptr, S4, B, st));
       MN_TRY((launch_bn_bwd_reduce<T, TZ>(S4, nullptr, (const T*)bl.y1, nullptr, Mo, C,
@@ -730,24 +667,22 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
     // and carries that block's BN2 (+ downsample BN) reductions
     const bool next_pre = fuse_bwd && bi > 0;
     EpiBwd e2; memset(&e2, 0, sizeof(e2));
-    EpiFin fb2; memset(&fb2, 0, sizeof(fb2));
     if (next_pre) {
       BlockL& pb = blocks[bi - 1];
       e2.y = (const bf16*)pb.y2; e2.zmask = (const bf16*)pb.out;
       e2.yd = (pb.convd >= 0) ? (const bf16*)pb.yd : nullptr;
-      fb2 = fin_backward(convs[pb.conv2].bn, (pb.convd >= 0) ? convs[pb.convd].bn : -1, (long long)B * pb.Ho * pb.Wo, params, grads);
-      stats_target = lazy_fin ? bwd_slot(convs[pb.conv2].bn) : nullptr;      // consumed at the top of the next iteration
+      stats_target = bwd_slot(convs[pb.conv2].bn);      // consumed at the top of the next iteration
     }
     MN_TRY(conv_wgrad<P>(bl.conv1, zin, S1, B, st));
     if (ds && bl.ds_fold) {
       MN_TRY(conv_wgrad<P>(bl.convd, zin, S2, B, st));
-      MN_TRY(conv_dgrad<P>(bl.conv1, S1, nullptr, S0, B, st, next_pre ? &e2 : nullptr, &fb2, S2, bl.convd));
+      MN_TRY(conv_dgrad<P>(bl.conv1, S1, nullptr, S0, B, st, next_pre ? &e2 : nullptr, S2, bl.convd));
     } else if (ds) {
       MN_TRY(conv_wgrad<P>(bl.convd, zin, S2, B, st));
       MN_TRY(conv_dgrad<P>(bl.convd, S2, nullptr, S0, B, st));
-      MN_TRY(conv_dgrad<P>(bl.conv1, S1, S0, S0, B, st, next_pre ? &e2 : nullptr, &fb2));
+      MN_TRY(conv_dgrad<P>(bl.conv1, S1, S0, S0, B, st, next_pre ? &e2 : nullptr));
     } else {
-      MN_TRY(conv_dgrad<P>(bl.conv1, S1, gres, S0, B, st, next_pre ? &e2 : nullptr, &fb2));
+      MN_TRY(conv_dgrad<P>(bl.conv1, S1, gres, S0, B, st, next_pre ? &e2 : nullptr));
     }
     stats_target = nullptr;
     pre = next_pre;
@@ -762,8 +697,8 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
     if (stem_fuse) {
       // the pool/ReLU backward accumulates the stem BN's (sum g, sum g*y) while it has g and y in registers
       MN_TRY(launch_stem_pool_bwd<T>(S0, amax0, (const T*)y0, b0.scale, b0.shift, S4, B, Hc, Wc, Hp, Wp, 64, st,
-                                     lazy_fin ? bwd_slot(convs[0].bn) : bn_accum));
-      if (!lazy_fin)
+                                     tc() ? bwd_slot(convs[0].bn) : bn_accum));
+      if (!tc())
         MN_TRY(launch_bn_bwd_finalize_accum(M0, 64, params + b0.g_off, b0.mean, b0.invstd, grads + b0.g_off, grads + b0.b_off, b0.coef,
                                             nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, bn_accum, st));
     } else {
@@ -774,7 +709,7 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
     }
     const BnLazy lz0 = lazy_backward(convs[0].bn, -1, M0, params, grads);
     MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S4, (const TZ*)nullptr, (const T*)y0, b0.coef, S2, nullptr, nullptr, nullptr, nullptr, M0, 64, st, nullptr, nullptr, gs,
-                                           (lazy_fin && stem_fuse) ? &lz0 : nullptr)));
+                                           (tc() && stem_fuse) ? &lz0 : nullptr)));
     MN_TRY(conv_wgrad<P>(0, (const TZ*)A0, S2, B, st));
   }
   MN_TRY(wgrad_join(st));       // every asynchronous wgrad of this part has landed in grads_flat (the stem's in dw_krsc)

@@ -65,7 +65,8 @@ struct Net {
   // they fill the SM time the chain leaves idle (latency-bound finalize / head / loss kernels, kernel tails) instead of
   // sitting in it.  The gradients they read (d conv output) rotate through a ring of four buffers; a slot is rewritten
   // only after the wgrad that read it has finished (event), and every part of the backward pass ends with a join.
-  cudaStream_t side; int wgrad_async;
+  // While profiling, the wgrads run on the compute stream inside their timing brackets.
+  cudaStream_t side;
   void* ring[4]; cudaEvent_t ring_ready[4], ring_done[4]; bool ring_pending[4]; int ring_pos;
   void* ring_next(cudaStream_t st);
   int ring_slot(const void* p) const;
@@ -76,15 +77,14 @@ struct Net {
   // where conv ci's wgrad engine accumulates: grads_flat at the parameter's offset (KRSC order), the stem in dw_krsc
   float* wgrad_out(int ci) { return ci == 0 ? dw_krsc : cur_grads + convs[ci].wd.p_off; }
   float *w_krsc_f32, *w_dg_f32;  // strict mode: fp32 K-major matrices the hi / lo weight planes are cut from
-  int split_fmt_z, split_fmt_g;  // strict mode: element format of the forward / backward operand planes (0 fp16, 1 bf16)
   float* gscale;                 // strict mode, device: {S, 1/S} -- this step's power-of-two gradient scale
   double* bn_accum; unsigned int* bn_counter;
-  // lazy BatchNorm finalize (bn_fin.cuh, BnLazy): one accumulator slot per BatchNorm and direction, zeroed once per step.
-  // Slots 0..35 forward statistics, 36..71 backward reductions (8 replicas x [3][512] doubles each, what the conv
-  // epilogues spread their flushes over), slot 72 (32 replicas) the stem's backward sums from the pool-backward kernel.
+  // Tensor-core training: the conv epilogues accumulate the BatchNorm sums and the consuming element-wise kernels
+  // finalize them (lazy finalize, bn_fin.cuh: BnLazy).  One accumulator slot per BatchNorm and direction, zeroed once
+  // per step.  Slots 0..35 forward statistics, 36..71 backward reductions (8 replicas x [3][512] doubles each, what the
+  // conv epilogues spread their flushes over), slot 72 (32 replicas) the stem's backward sums from the pool-backward kernel.
   double* bn_slots; size_t bn_slots_bytes;
-  int lazy_fin;                  // consumers finalize the sums themselves (env MAPNET_BN_LAZY_FIN, tensor-core modes)
-  double* stats_target;          // where the next conv_fprop / conv_dgrad with fused sums accumulates (nullptr: bn_accum)
+  double* stats_target;          // where the next conv_fprop / conv_dgrad with fused sums accumulates (nullptr: no sums)
   static constexpr int kSlotReplicas = 8, kStemBwdReplicas = 32, kSlotStride = 3 * 512;
   double* fwd_slot(int bn) { return bn_slots + (size_t)bn * kSlotReplicas * kSlotStride; }
   double* bwd_slot(int bn) { return bn_slots + (size_t)(bn == convs[0].bn ? 72 : 36 + bn) * kSlotReplicas * kSlotStride; }
@@ -105,11 +105,9 @@ struct Net {
   // optional per-conv-launch timing (bench.py roofline): CUDA events around every conv call
   struct ProfRec { cudaEvent_t e0, e1; int cls; double flops; };
   int profile_on;
-  int stem_s2d;                  // stem conv on an overlapped view of the space-to-depth image (env MAPNET_STEM_S2D)
-  int stem_fuse;                 // stem BN backward reductions inside the pool backward (env MAPNET_STEM_FUSE)
-  int fuse_fin;                  // BN finalize inside the last CTA of the accumulating conv (env MAPNET_TC_FUSE_FIN)
+  int stem_s2d;                  // stem conv on an overlapped view of the space-to-depth image (tensor-core modes)
+  int stem_fuse;                 // stem BN backward reductions inside the pool backward (even stem output sizes)
   int fuse_bwd;                  // BN backward reductions accumulated in the dgrad epilogue (env MAPNET_TC_FUSE_BWD)
-  int fuse_stats;                // BN statistics accumulated in the wgmma conv epilogue (env MAPNET_TC_FUSE_STATS)
   int ds_fold;                   // fold each 1x1/s2 downsample dgrad into its block's conv1 dgrad (env MAPNET_TC_DS_FOLD)
   std::vector<ProfRec> prof;
   std::vector<cudaEvent_t> prof_pool; size_t prof_pool_used;
@@ -142,12 +140,10 @@ struct Net {
   template <typename P> int backward_t(const float* dpred, const float* params, float* grads, int filter_nans,
                                        int part, cudaStream_t st);
   template <typename P> int conv_fprop(int ci, const typename P::Z* x, const typename P::A* residual, typename P::A* y, int B,
-                                       cudaStream_t st, bool with_stats = false, const EpiFin* fin = nullptr);
+                                       cudaStream_t st);
   template <typename P> int conv_dgrad(int ci, const typename P::G* dy, const typename P::A* residual, typename P::A* dx, int B,
-                                       cudaStream_t st, const EpiBwd* bwd = nullptr, const EpiFin* fin = nullptr,
+                                       cudaStream_t st, const EpiBwd* bwd = nullptr,
                                        const typename P::G* dy_shortcut = nullptr, int ci_shortcut = -1);
-  EpiFin fin_forward(int bi, long long M, const float* params, float* bufs);
-  EpiFin fin_backward(int bi, int bi_ds, long long M, const float* params, float* grads);
   template <typename P> int conv_wgrad(int ci, const typename P::Z* x, const typename P::G* dy, int B, cudaStream_t st);
   template <typename P> int bn_forward(int bi, const typename P::A* y, long long M, const float* params, float* bufs,
                                        int training, cudaStream_t st);

@@ -51,19 +51,21 @@ def test_library_targets_sm_90a_only(sass):
     assert set(per_arch) == {"sm_90a"} and per_arch["sm_90a"] > 50, per_arch
 
 
-def test_conv_engines_use_wgmma_tma_and_mbarriers(sass):
+def test_six_conv_engines_use_wgmma_tma_and_mbarriers(sass):
     k = _kernel_bodies(sass)
     conv = {n: b for n, b in k.items() if "k_tc_conv" in n or "k_tc_wgrad" in n}
-    assert len(conv) >= 10, sorted(conv)[:5]
+    # training fprop / dgrad, inference fprop (eval-mode epilogues) and wgrad, each with N tiles of 64 and 128
+    # (mangled: k_tc_conv<BN, AFF> = k_tc_convILi<BN>ELb<AFF>E..., k_tc_wgrad<BN> = k_tc_wgradILi<BN>EE...)
+    names = {re.search(r"k_tc_(conv|wgrad)ILi\d+E(Lb[01]E)?", n).group(0) for n in conv}
+    expected = {"k_tc_convILi%dELb%dE" % (bn, aff) for bn in (64, 128) for aff in (0, 1)} | \
+               {"k_tc_wgradILi%dE" % bn for bn in (64, 128)}
+    assert len(conv) == 6 and names == expected, sorted(conv)
     for n, b in conv.items():
         assert "HGMMA" in b, "no wgmma in %s" % n                        # warpgroup MMA, accumulator in registers
         assert "UTMALDG" in b, "no TMA tensor load in %s" % n          # cp.async.bulk.tensor
         assert "SYNCS.ARRIVE.TRANS64" in b, "no mbarrier transaction arrive in %s" % n
         assert "WARPGROUP.DEPBAR" in b, "no wgmma.wait_group in %s" % n
         assert not re.search(r"\bHMMA\.", b), "legacy tensor-core instruction in %s" % n
-    # the clustered fprop / dgrad engines multicast the weight tile to every CTA of the cluster
-    clustered = [b for n, b in conv.items() if re.search(r"k_tc_conv\w*ILi\d+ELi[24]E", n)]
-    assert clustered and all("UTMALDG.2D.MULTICAST" in b for b in clustered)
     # im2col happens in the load: the fprop / dgrad / wgrad engines read activations through 4-D tensor maps
     assert all("UTMALDG.4D" in b for n, b in conv.items())
     # wgrad writes every dW element with plain stores (one writer per element; split-K partials are added up in a fixed

@@ -1,5 +1,5 @@
 """Micro-benchmark of the wgmma conv engines per ResNet-34 layer shape (GPU box).
-usage: python tools/bench_conv.py [B]   (env MAPNET_TC_* select the engine variant)"""
+usage: python tools/bench_conv.py [B]   (env MAPNET_TC_BN=64|128 forces the N tile, MAPNET_TC_DEBUG skips parts of the work)"""
 import ctypes, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
