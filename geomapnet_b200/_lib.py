@@ -82,7 +82,15 @@ def lib():
     for name in ("mapnet_preprocess_create", "mapnet_preprocess_output_size", "mapnet_preprocess_run",
                  "mapnet_preprocess_run_ex", "mapnet_preprocess_destroy"):
         getattr(L, name).restype = c_int
-    L.mapnet_pose_post.argtypes = [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
+    L.mapnet_frame_cache_create.argtypes = [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int]
+    L.mapnet_frame_cache_ingest.argtypes = [c_void_p, c_void_p, c_int, c_int, c_void_p]
+    L.mapnet_frame_cache_assemble.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int,
+                                              POINTER(c_float), POINTER(c_float), c_void_p, c_void_p, c_void_p]
+    L.mapnet_frame_cache_destroy.argtypes = [c_void_p]
+    for name in ("mapnet_frame_cache_create", "mapnet_frame_cache_ingest", "mapnet_frame_cache_assemble",
+                 "mapnet_frame_cache_destroy"):
+        getattr(L, name).restype = c_int
+    L.mapnet_pose_post.argtypes =[c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
     L.mapnet_pose_post.restype = c_int
     L.mapnet_pgo_optimize.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, ctypes.c_double, ctypes.c_double,
                                       ctypes.c_double, ctypes.c_double, c_int, c_int, c_void_p, c_void_p]
@@ -126,7 +134,9 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_preprocess_output_size", "mapnet_preprocess_run", "mapnet_preprocess_destroy",
             "mapnet_backward_part", "mapnet_grad_part_range", "mapnet_preprocess_run_ex", "mapnet_test_conv_epilogue", "mapnet_pose_post", "mapnet_pgo_optimize",
             "mapnet_sgd_step_dev", "mapnet_rmsprop_step_dev", "mapnet_test_conv_affine", "mapnet_infer_create",
-            "mapnet_infer_load", "mapnet_infer_forward", "mapnet_infer_arena_bytes", "mapnet_infer_destroy"]
+            "mapnet_infer_load", "mapnet_infer_forward", "mapnet_infer_arena_bytes", "mapnet_infer_destroy",
+            "mapnet_frame_cache_create", "mapnet_frame_cache_ingest", "mapnet_frame_cache_assemble",
+            "mapnet_frame_cache_destroy"]
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 
 

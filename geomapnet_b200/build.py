@@ -17,10 +17,12 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(CSRC, "libmapnet_b200.so")
 OBJ = os.path.join(CSRC, "_obj")
 SOURCES = ["api.cu", "net.cu", "infer.cu", "bn.cu", "conv_simt.cu", "conv_tc.cu", "layout.cu", "head.cu", "loss.cu", "adam.cu",
-           "optim.cu", "preprocess.cu", "pgo.cu"]
+           "optim.cu", "preprocess.cu", "loader.cu", "pgo.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
+# per-source flags: loader.cu computes float32 pose targets that follow the reference's roundings (see its header)
+SOURCE_FLAGS = {"loader.cu": ["-fmad=false"]}
 
 
 def _digest():
@@ -31,12 +33,13 @@ def _digest():
                 with open(os.path.join(root, f), "rb") as fh:
                     h.update(f.encode()); h.update(fh.read())
     h.update(" ".join(FLAGS).encode())
+    h.update(repr(sorted(SOURCE_FLAGS.items())).encode())
     return h.hexdigest()
 
 
 def _compile(src):
     obj = os.path.join(OBJ, src.replace(".cu", ".o"))
-    cmd = [NVCC] + FLAGS + ["-c", os.path.join(CSRC, src), "-o", obj]
+    cmd = [NVCC] + FLAGS + SOURCE_FLAGS.get(src, []) + ["-c", os.path.join(CSRC, src), "-o", obj]
     r = subprocess.run(cmd, capture_output=True, text=True)
     with open(obj + ".log", "w") as f:
         f.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)

@@ -3,6 +3,8 @@
 #include "common.cuh"
 #include "bn_fin.cuh"
 
+struct mapnet_preprocess;
+
 namespace mapnet {
 
 // Geometry of one convolution (NHWC activations, weights [Co][KH][KW][Ci] "KRSC").
@@ -205,5 +207,11 @@ int launch_sgd(float* p, const float* g, float* buf, long long n, const float* l
 int launch_rmsprop(float* p, const float* g, float* square_avg, float* grad_avg, float* buf, long long n,
                    const float* lr_dev, double alpha, float eps, float wd, float momentum, int* step_dev, float gscale,
                    const float* sqnorm_or_null, float max_norm, cudaStream_t st);
+
+// input pipeline internals shared by preprocess.cu and the frame cache (loader.cu)
+struct JitterParams;
+int preprocess_resize_u8(struct ::mapnet_preprocess* h, const uint8_t* img, int n, uint8_t* out_u8, cudaStream_t st);
+int launch_jitter_luma_sum(const uint8_t* u8, const int* frame_index, const JitterParams* jp, unsigned int* sums,
+                           long long npix, int n, int gx, cudaStream_t st);
 
 }  // namespace mapnet

@@ -228,10 +228,12 @@ int Net::init(int max_B_, int H_, int W_, int feat_dim_, int precision_) {
 }
 
 void Net::destroy() {
-  for (auto* p : tc_fprop) tc_plan_destroy(p);
-  for (auto* p : tc_dgrad) tc_plan_destroy(p);
-  for (auto* p : tc_wgrad) tc_plan_destroy(p);
+  for (auto& kv : tc_sets)
+    for (auto* v : {&kv.second.fprop, &kv.second.dgrad, &kv.second.wgrad})
+      for (auto* p : *v) tc_plan_destroy(p);
+  tc_sets.clear();
   tc_fprop.clear(); tc_dgrad.clear(); tc_wgrad.clear();
+  tc_B = 0;
   for (void* p : allocs) cudaFree(p);
   allocs.clear();
   if (side != nullptr) {
@@ -384,12 +386,31 @@ int Net::conv_wgrad(int ci, const typename P::Z* x, const typename P::G* dy, int
 
 int Net::ensure_tc_plans(int B) {
   if (!tc() || tc_B == B) return 0;
-  for (auto* p : tc_fprop) tc_plan_destroy(p);
-  for (auto* p : tc_dgrad) tc_plan_destroy(p);
-  for (auto* p : tc_wgrad) tc_plan_destroy(p);
+  auto it = tc_sets.find(B);
+  if (it != tc_sets.end()) {
+    const TcPlanSet& s = it->second;
+    tc_fprop = s.fprop; tc_dgrad = s.dgrad; tc_wgrad = s.wgrad;
+    for (size_t k = 0; k < blocks.size(); ++k) blocks[k].ds_fold = s.ds_fold[k];
+    tc_B = B;
+    return 0;
+  }
+  tc_B = 0;
   tc_fprop.assign(convs.size(), nullptr);
   tc_dgrad.assign(convs.size(), nullptr);
   tc_wgrad.assign(convs.size(), nullptr);
+  const int r = build_tc_plans(B);
+  if (r != 0) {       // free what was built; the next call at this B starts over
+    for (auto* v : {&tc_fprop, &tc_dgrad, &tc_wgrad}) { for (auto* p : *v) tc_plan_destroy(p); v->clear(); }
+    return r;
+  }
+  TcPlanSet& s = tc_sets[B];
+  s.fprop = tc_fprop; s.dgrad = tc_dgrad; s.wgrad = tc_wgrad;
+  for (auto& bl : blocks) s.ds_fold.push_back(bl.ds_fold);
+  tc_B = B;
+  return 0;
+}
+
+int Net::build_tc_plans(int B) {
   for (size_t i = 0; i < convs.size(); ++i) {
     ConvGeom g = convs[i].g; g.B = B;
     const bool sp = precision == PREC_TC_SPLIT;
@@ -412,7 +433,6 @@ int Net::ensure_tc_plans(int B) {
     MN_TRY(tc_plan_add_shortcut(tc_dgrad[bl.conv1], (const bf16*)w_dg + convs[bl.convd].wd.k_off));
     bl.ds_fold = 1;
   }
-  tc_B = B;
   return 0;
 }
 

@@ -1,6 +1,7 @@
 // Host-side plan of the PoseNet(ResNet-34) training step: parameter table,
 // layer geometry, activation arena, forward / backward schedules.
 #pragma once
+#include <map>
 #include <string>
 #include <vector>
 
@@ -95,7 +96,12 @@ struct Net {
   float *sq_partials, *sq_out;
   unsigned long long* drop_ctr;  // device-side dropout step counter (graph capture)
 
-  // tensor-core plans (precision == PREC_BF16_TC), rebuilt when B changes
+  // tensor-core plans: one set per batch size, kept until destroy().  A CUDA graph captured at one B has its plans'
+  // split-K workspaces and tensor maps baked in, so a call at another B must not free them (an epoch's last, partial
+  // batch; a validation batch on the same trunk).  tc_fprop / tc_dgrad / tc_wgrad and the blocks' ds_fold are the
+  // set of the current B (tc_B).
+  struct TcPlanSet { std::vector<TcConvPlan*> fprop, dgrad, wgrad; std::vector<int> ds_fold; };
+  std::map<int, TcPlanSet> tc_sets;
   std::vector<TcConvPlan*> tc_fprop, tc_dgrad, tc_wgrad;
   int tc_B;
 
@@ -148,6 +154,7 @@ struct Net {
   template <typename P> int bn_forward(int bi, const typename P::A* y, long long M, const float* params, float* bufs,
                                        int training, cudaStream_t st);
   int ensure_tc_plans(int B);
+  int build_tc_plans(int B);     // fills tc_fprop / tc_dgrad / tc_wgrad (nullptr-initialised) and ds_fold for B
 };
 
 }  // namespace mapnet

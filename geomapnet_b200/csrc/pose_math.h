@@ -179,6 +179,32 @@ PM_HD void calc_vo_logq_bwd(Pose6 p0, Pose6 p1, Pose6 go, Pose6* g0, Pose6* g1) 
   g1->t = g_t1; g1->l = qexp_bwd(p1.l, g_q1);
 }
 
+// ---- calc_vo_logq_safe (:276-288): the VO targets of MFOnline's validation half ----------------
+// qexp_t_safe / qlog_t_safe run numpy's qexp / qlog (:307-327) on float32 rows, so every operation is float32:
+// qexp = (cos n, sinc(n / pi) q) with np.sinc(x) = sin(pi x) / (pi x); qlog has no clamp, as the reference.
+PM_HD Q4 qexp_safe(V3 l) {
+  const float n = sqrtf(l.x * l.x + l.y * l.y + l.z * l.z);
+  const float pi = 3.14159265358979323846f;
+  const float x = n / pi;
+  const float y = pi * (x == 0.0f ? 1.0e-20f : x);
+  Q4 q;
+  q.s = cosf(n);
+  q.v = mul(l, sinf(y) / y);
+  return q;
+}
+PM_HD V3 qlog_safe(Q4 q) {
+  if (q.v.x == 0.0f && q.v.y == 0.0f && q.v.z == 0.0f) return v3(0.0f, 0.0f, 0.0f);
+  return divs(mul(q.v, acosf(q.s)), norm3(q.v));
+}
+PM_HD Pose6 calc_vo_logq_safe(Pose6 p0, Pose6 p1) {
+  Q4 q0 = qexp_safe(p0.l), q1 = qexp_safe(p1.l);
+  Q4 q0i; q0i.s = q0.s; q0i.v = neg(q0.v);                // qinv
+  Pose6 o;
+  o.t = rotate(sub(p1.t, p0.t), q0i);
+  o.l = qlog_safe(qmult(q0i, q1));
+  return o;
+}
+
 PM_HD float sgnf(float d) { return (d > 0.0f) ? 1.0f : ((d < 0.0f) ? -1.0f : 0.0f); }
 
 }  // namespace posemath

@@ -79,10 +79,11 @@ k_pre_resize_v_norm(const uint8_t* __restrict__ tmp, float* __restrict__ out, ui
   }
 }
 
-// ColorJitter, pass A: per image, the luma sum of the image in its state just before the contrast adjustment
+// ColorJitter, pass A: per image, the luma sum of the image in its state just before the contrast adjustment.
+// frame_index: nullptr (image n is image n of u8) or the frame cache's gather (image n is frame frame_index[n])
 __global__ void __launch_bounds__(256)
-k_jitter_luma_sum(const uint8_t* __restrict__ u8, const JitterParams* __restrict__ jp, unsigned int* __restrict__ sums,
-                  long long npix /* per image */) {
+k_jitter_luma_sum(const uint8_t* __restrict__ u8, const int* __restrict__ frame_index, const JitterParams* __restrict__ jp,
+                  unsigned int* __restrict__ sums, long long npix /* per image */) {
   pdl_prologue();
   const int n = blockIdx.y;
   const JitterParams P = jp[n];
@@ -90,7 +91,7 @@ k_jitter_luma_sum(const uint8_t* __restrict__ u8, const JitterParams* __restrict
   while (npre < 4 && P.order[npre] != JIT_CONTRAST) ++npre;
   const uint8_t shift = jit_hue_shift(P.factor[JIT_HUE]);
   unsigned int acc = 0;
-  const uint8_t* base = u8 + (long long)n * npix * 3;
+  const uint8_t* base = u8 + (long long)(frame_index != nullptr ? frame_index[n] : n) * npix * 3;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < npix; i += (long long)gridDim.x * blockDim.x) {
     uint8_t px[3] = {base[3 * i], base[3 * i + 1], base[3 * i + 2]};
     for (int k = 0; k < npre; ++k) jit_apply(P.order[k], P.factor[P.order[k]], 0, shift, px);
@@ -140,6 +141,32 @@ using namespace mapnet;
 struct mapnet_preprocess {
   PreprocessPlan p;
 };
+
+namespace mapnet {
+// ---- used by the frame cache (loader.cu) --------------------------------------------------------------------------
+// Resize n frames (n <= the plan's max_images) into uint8 [n][Hout][Wout][3] at out_u8.
+int preprocess_resize_u8(mapnet_preprocess_t* h, const uint8_t* img, int n, uint8_t* out_u8, cudaStream_t st) {
+  PreprocessPlan& p = h->p;
+  MN_CHECK(n >= 1 && n <= p.max_images, "preprocess_resize_u8: %d images outside [1, max_images=%d]", n, p.max_images);
+  const long long t1 = (long long)n * p.Hin * p.Wout, t2 = (long long)n * p.Hout * p.Wout;
+  const int g1 = (int)((t1 + 255) / 256 < (long long)kNumSMs * 16 ? (t1 + 255) / 256 : (long long)kNumSMs * 16);
+  const int g2 = (int)((t2 + 255) / 256 < (long long)kNumSMs * 16 ? (t2 + 255) / 256 : (long long)kNumSMs * 16);
+  MN_LAUNCH(k_pre_resize_h, g1, 256, 0, st, img, (const int*)nullptr, p.d_tmp, p.d_bh, p.d_kh, p.ksh, (long long)n * p.Hin,
+            p.Hin, p.Win, p.Wout);
+  MN_LAUNCH_CHECK();
+  MN_LAUNCH(k_pre_resize_v_norm, g2, 256, 0, st, p.d_tmp, (float*)nullptr, out_u8, p.d_bv, p.d_kv, p.ksv, n, p.Hin, p.Hout,
+            p.Wout, 0.f, 0.f, 0.f, 1.f, 1.f, 1.f);
+  MN_LAUNCH_CHECK();
+  return 0;
+}
+int launch_jitter_luma_sum(const uint8_t* u8, const int* frame_index, const JitterParams* jp, unsigned int* sums,
+                           long long npix, int n, int gx, cudaStream_t st) {
+  MN_LAUNCH(k_jitter_luma_sum, dim3(gx, n), 256, 0, st, u8, frame_index, jp, sums, npix);
+  MN_LAUNCH_CHECK();
+  return 0;
+}
+}  // namespace mapnet
+
 
 extern "C" {
 
@@ -213,7 +240,8 @@ int mapnet_preprocess_run_ex(mapnet_preprocess_t* h, const void* img_nhwc_u8, in
   MN_LAUNCH_CHECK();
   MN_CUDA(cudaMemsetAsync(p.d_sums, 0, (size_t)n * sizeof(unsigned int), st));
   int gx = (int)((npix + 255) / 256); if (gx > 64) gx = 64;
-  MN_LAUNCH(k_jitter_luma_sum, dim3(gx, n), 256, 0, st, (const uint8_t*)p.d_u8, (const JitterParams*)jitter_dev, p.d_sums, npix);
+  MN_LAUNCH(k_jitter_luma_sum, dim3(gx, n), 256, 0, st, (const uint8_t*)p.d_u8, (const int*)nullptr,
+            (const JitterParams*)jitter_dev, p.d_sums, npix);
   MN_LAUNCH_CHECK();
   MN_LAUNCH(k_jitter_norm, dim3(gx, n), 256, 0, st, (const uint8_t*)p.d_u8, (const JitterParams*)jitter_dev,
             (const unsigned int*)p.d_sums, out_nchw, (uint8_t*)out_u8_or_null, p.Hout, p.Wout, mean3[0], mean3[1], mean3[2],

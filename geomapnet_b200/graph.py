@@ -124,7 +124,14 @@ class GraphedTrainStep(object):
     def __call__(self, x, targ):
         self.x.copy_(x, non_blocking=True)
         self.t.copy_(targ, non_blocking=True)
+        return self.replay()
+
+    def replay(self, inputs_read=None):
+        """One step on what self.x / self.t hold.  inputs_read: a torch.cuda.Event recorded once the step no longer
+        reads them (after graph 1), so the next batch can be written there while the optimizer runs."""
         self.g1.replay()
+        if inputs_read is not None:
+            inputs_read.record()
         if self.dp is not None:
             self.dp.allreduce_grads(slices_in_graph=getattr(self.dp, "overlap", False))
         if hasattr(self.learner, "sync_lr"):
@@ -133,3 +140,52 @@ class GraphedTrainStep(object):
         if hasattr(self.learner, "advance_host_step"):
             self.learner.advance_host_step(1)
         return self.loss
+
+
+def train_epoch(loader, model, criterion, optimizer, max_grad_norm=0.0, steps=None):
+    """One epoch of a geomapnet_b200.data.DeviceLoader through CUDA graphs, last partial batch included
+    (common/train.py:276-300 with step_feedfwd).  One GraphedTrainStep per distinct batch size, built before the
+    first step and full size first, so that the trunk's arena never grows under a captured graph.  Each batch is
+    assembled on a side stream straight into the static input of the step that takes it, while the previous step's
+    optimizer graph runs.  steps: a dict {batch size: GraphedTrainStep} kept by the caller to reuse the captures in
+    later epochs (filled on first use).  Returns the per-step losses as floats (one device sync, at the end)."""
+    ds = loader.dataset
+    dev = ds.device
+    steps = {} if steps is None else steps
+    sizes = [loader.batch_size]
+    last = len(ds) % loader.batch_size
+    if last:
+        sizes.append(last)
+    cur = torch.cuda.current_stream(dev)
+    side = torch.cuda.Stream(dev)
+    for n in sizes:
+        if n not in steps:
+            xs, ts = ds.batch_shapes(n)
+            x0, t0 = torch.empty(xs, device=dev), torch.empty(ts, device=dev)
+            ds.assemble(ds.example(n), x0, t0)
+            steps[n] = GraphedTrainStep(model, criterion, optimizer, x0, t0, max_grad_norm=max_grad_norm)
+    read = {n: torch.cuda.Event() for n in steps}
+    ready = torch.cuda.Event()
+    losses = []
+
+    def launch(batch):
+        st = steps[batch[3]]
+        side.wait_event(read[batch[3]])                   # the previous step of this size has read its inputs
+        with torch.cuda.stream(side):
+            ds.assemble(batch, st.x, st.t)
+        ready.record(side)
+        return st
+
+    it = loader.batches()
+    b = next(it, None)
+    if b is None:
+        return losses
+    st = launch(b)
+    while st is not None:
+        cur.wait_event(ready)
+        n = st.x.shape[0]
+        st.replay(inputs_read=read[n])
+        losses.append(st.loss.clone())
+        b = next(it, None)
+        st = launch(b) if b is not None else None
+    return [float(v) for v in torch.stack(losses).cpu()]

@@ -152,6 +152,28 @@ int mapnet_preprocess_run_ex(mapnet_preprocess_t* h, const void* img_nhwc_u8, in
                              void* out_u8_or_null, void* stream);
 int mapnet_preprocess_destroy(mapnet_preprocess_t* h);
 
+/* ---- device-resident training set (geomapnet_b200/csrc/loader.cu; Python: geomapnet_b200.data.DeviceDataset).
+ * Resize(size) is deterministic and comes before ColorJitter in the reference's transform stack, so its uint8 output is
+ * computed once per frame and kept: a cache of n_frames frames [Hout][Wout][3] in device memory.
+ * ingest: frames_nhwc_u8 (DEVICE memory, n <= chunk frames [Hin][Win][3]) are resized into cache slots [first, first + n).
+ *   Chunks of one cache are ingested on one stream.
+ * assemble: one training batch of n images, one kernel launch (two with ColorJitter: contrast needs the luma sum first):
+ *   image i is cache frame frame_index[i], [ColorJitter record i applied,] ToTensor + Normalize -> out_nchw float32
+ *   [n][3][Hout][Wout] (DEVICE memory, e.g. the static input of a captured training step).  The same launch writes n_targ
+ *   target rows of 6 floats into targ_out (DEVICE): row k is poses_dev row targ_rows[2k] when targ_rows[2k+1] == -1,
+ *   otherwise calc_vo_logq_safe(poses row targ_rows[2k], poses row targ_rows[2k+1]) (common/pose_utils.py:276-288; the
+ *   VO targets of MFOnline).  poses_dev: [n_poses][6] float32 in DEVICE memory.
+ *   frame_index, jitter (NULL, or n records as for mapnet_preprocess_run_ex) and targ_rows are HOST arrays, checked and
+ *   copied before the call returns; mean3 / std3 are HOST pointers to 3 floats.  Nothing is launched when a check fails. */
+typedef struct mapnet_frame_cache mapnet_frame_cache_t;
+int mapnet_frame_cache_create(mapnet_frame_cache_t** out, int n_frames, int Hin, int Win, int size, int chunk,
+                              int max_images, int max_targ);
+int mapnet_frame_cache_ingest(mapnet_frame_cache_t* h, const void* frames_nhwc_u8, int first, int n, void* stream);
+int mapnet_frame_cache_assemble(mapnet_frame_cache_t* h, int n, const int32_t* frame_index, const void* jitter,
+                                const float* poses_dev, int n_poses, const int32_t* targ_rows, int n_targ,
+                                const float* mean3, const float* std3, float* out_nchw, float* targ_out, void* stream);
+int mapnet_frame_cache_destroy(mapnet_frame_cache_t* h);
+
 /* ---- batched inference post-processing + pose-graph optimisation (SURVEY.md section 8 row f3; csrc/pgo.cu).
  * mapnet_pose_post: scripts/eval.py:163-181 for n poses at once -- pred6 = (t, log q) float32 -> out7 = (t * pose_s +
  * pose_m, qexp(log q)) float64; pose_m3 / pose_s3 are HOST pointers (pose_stats.txt) or NULL (keep the translations).
