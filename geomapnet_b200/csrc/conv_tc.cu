@@ -569,6 +569,10 @@ __device__ __forceinline__ void mma_tile(float (&d)[BN / 2], const int kblocks, 
   int prev = -1;
   for (int kb = 0; kb < kblocks; ++kb) {
     mbar_wait(full0 + 8 * stage, phase);
+    // One thread releases the stage for its whole warpgroup, which is only safe while every warp has passed the wait
+    // above.  The wgmma instructions (.sync.aligned) keep the four warps together; without them a warp could fall a
+    // whole ring behind, miss a phase of the full barrier and wait forever.
+    if (skip_mma) wg_bar(threadIdx.x >> 7);
     if (!skip_mma) {
       const uint32_t sa = smem_base + stage * stage_bytes + a_off;
       const uint32_t sb = smem_base + stage * stage_bytes + b_off;
@@ -744,17 +748,38 @@ __device__ __forceinline__ void wgrad_store(const WgradParams& P, float* __restr
   const bool store = P.partial != nullptr;
   auto put = [&](float* p, const float v) { if (store) *p = v; else *p += v; };
   if (!P.split) {
+    // Adding into dw reads it first.  The compiler cannot tell that the addresses differ, so one `+=` at a time makes
+    // every load wait for the previous store: BN / 2 dependent DRAM round trips per thread (measured on H100: more than
+    // half of a layer4 wgrad).  Groups of 16 loads are issued together before their adds and stores instead.
+    constexpr int JG = 4;                      // j values per group: 4 x 2 x 2 values
+    // element (co = col0 + c + k, row r) is at p0 + k * cstride
+    float* p0 = dw + ((long long)(col0 + c) * P.KK + ch.tap) * P.Ci + ch.c0 + r;
+    const int cstride = P.KK * P.Ci;
+    const int kend = P.Co - col0 - c;          // k < kend: inside the tensor
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j)
+    for (int j0 = 0; j0 < BN / 8; j0 += JG) {
+      float old[JG][2][2];
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int co = col0 + 8 * j + c + e;
-        if (co < P.Co) {
-          float* p = dw + ((long long)co * P.KK + ch.tap) * P.Ci + ch.c0 + r;
-          put(p, d[4 * j + e]);
-          put(p + 8, d[4 * j + 2 + e]);
+      for (int j = 0; j < JG; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int k = 8 * (j0 + j) + e;
+          const bool ld = !store && k < kend;
+          old[j][e][0] = ld ? p0[k * cstride] : 0.f;
+          old[j][e][1] = ld ? p0[k * cstride + 8] : 0.f;
         }
-      }
+#pragma unroll
+      for (int j = 0; j < JG; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int k = 8 * (j0 + j) + e;
+          if (k < kend) {
+            const float v0 = d[4 * (j0 + j) + e], v1 = d[4 * (j0 + j) + 2 + e];
+            p0[k * cstride] = store ? v0 : old[j][e][0] + v0;
+            p0[k * cstride + 8] = store ? v1 : old[j][e][1] + v1;
+          }
+        }
+    }
     return;
   }
   const float osc = (P.oscale != nullptr) ? __ldg(P.oscale) : 1.f;
@@ -922,7 +947,9 @@ static void pick_box(int Wd, int Hd, int pixels, int* TW, int* TH, int* TN) {
 // occupy the SMs.  A k-block costs max(bytes staged / ingest rate, MMA issue time) plus a fixed cost per work item
 // (prologue, epilogue).  The constants -- ~55 B per cycle of TMA ingest, 580 / 600 cycles of issue per k-block, ~2000
 // cycles per work item -- are carried over from a fit to an earlier tensor-memory engine on another GPU and have NOT
-// been measured for these wgmma engines on H100: treat the model as a ranking heuristic between BN = 64 and 128.
+// been measured for these wgmma engines on H100: treat the model as a ranking heuristic between BN = 64 and 128.  On
+// H100 the engines stage 20-47 B per cycle per SM and keep 79-93 % of their time with the loads skipped
+// (profiles/h100_conv_bound.md): ingest and MMA issue plus epilogue are nearly balanced, neither alone bounds a launch.
 // BN is 64 or 128 because a consumer warpgroup holds its 64 x BN fp32 accumulator in registers.  MAPNET_TC_BN=64|128
 // forces the choice (where Cout allows it).
 static int forced_bn() {
