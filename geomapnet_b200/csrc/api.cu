@@ -271,7 +271,7 @@ int mapnet_test_conv_epilogue(int kind, int B, int Hi, int Wi, int Ci, int Co, i
   g.Ho = (Hi + 2 * g.pad - k) / stride + 1; g.Wo = (Wi + 2 * g.pad - k) / stride + 1;
   cudaStream_t st = (cudaStream_t)stream;
   const int C = (kind == 0) ? Co : Ci;
-  const size_t acc_doubles = 32 * 3 * 512;
+  const size_t acc_doubles = (size_t)kBnAccReplicas * kBnAccStride;
   double* acc = nullptr;
   TcConvPlan* plan = nullptr;
   std::vector<double> h(acc_doubles);
@@ -294,7 +294,7 @@ int mapnet_test_conv_epilogue(int kind, int B, int Hi, int Wi, int Ci, int Co, i
     for (int j = 0; j < 3; ++j)
       for (int c = 0; c < C; ++c) {
         double s = 0.0;
-        for (int rep = 0; rep < 32; ++rep) s += h[(size_t)rep * 3 * 512 + (size_t)j * C + c];
+        for (int rep = 0; rep < kBnAccReplicas; ++rep) s += h[(size_t)rep * kBnAccStride + (size_t)j * C + c];
         host_sums[(size_t)j * C + c] = s;
       }
   if (plan) tc_plan_destroy(plan);
@@ -475,8 +475,8 @@ int mapnet_bench_conv(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, in
   EpiBwd E; memset(&E, 0, sizeof(E));
   const bf16* res = nullptr;
   if (epi && kind != 2) {
-    if (cudaMalloc((void**)&stats, 32 * 3 * 512 * sizeof(double)) != cudaSuccess) { set_last_error("bench_conv: cudaMalloc"); tc_plan_destroy(plan); return 1; }
-    cudaMemset(stats, 0, 32 * 3 * 512 * sizeof(double));
+    if (cudaMalloc((void**)&stats, kBnAccReplicas * kBnAccStride * sizeof(double)) != cudaSuccess) { set_last_error("bench_conv: cudaMalloc"); tc_plan_destroy(plan); return 1; }
+    cudaMemset(stats, 0, kBnAccReplicas * kBnAccStride * sizeof(double));
     if (kind == 1) { E.y = (const bf16*)out; E.zmask = (const bf16*)out; res = (const bf16*)out; }   // shaped like the output
   }
   cudaEvent_t iso;

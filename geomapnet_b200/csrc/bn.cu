@@ -2,20 +2,18 @@
 // and backward, on NHWC activations.  HBM-bound: 128-bit vectorised accesses,
 // fp32 math, per-thread channel-vector accumulators; block partials are combined with
 // fp64 atomics and the LAST block to arrive finalizes (no separate finalize launch).
+// One apply kernel per direction: it takes its per-channel parameters either from accumulated sums (finalized in its
+// prologue) or from memory (bn_fin.cuh, BnDesc).
 //
 // Replaces the library calls behind torchvision BasicBlock / ResNet.forward
 // (cuDNN BN fwd-training/bwd, THCUNN threshold, TH add, SpatialDilatedMaxPooling;
 // SURVEY.md section 2c) that /root/reference/models/posenet.py:66 runs.
-#include <stdlib.h>
-
 #include "kernels.h"
 #include "bn_fin.cuh"
 
 namespace mapnet {
 
 static const int kEwThreads = 256;
-static const int kReplicas = 32;        // accumulator replicas (must match Net's allocation)
-static const int kAccStride = 3 * 512;  // doubles per replica
 
 // ---------------------------------------------------------------------------
 // per-channel sums over pixels, finalize fused into the LAST block to arrive:
@@ -23,9 +21,8 @@ static const int kAccStride = 3 * 512;  // doubles per replica
 //   MODE 1: (sum g, sum g*y)            -> d gamma, d beta, dy = A*g + B*y + C coefficients
 //   MODE 2: (sum g, sum g*y, sum g*yd)  -> the same for the main AND the downsample BN
 //   g = dout * [z > 0]
-// Block partials are combined with fp64 atomics into kReplicas x [3][C] accumulators
-// (block b -> replica b % kReplicas: same-address atomics serialise at ~30 ns each, the
-// replicas keep that chain short); the finalizing block sums the replicas and resets them.
+// Block partials are combined with fp64 atomics into the replicated accumulators of bn_fin.cuh (same-address atomics
+// serialise at ~30 ns each); the finalizing block sums the replicas and resets them.
 // ---------------------------------------------------------------------------
 // 8 consecutive per-channel floats (32-byte aligned: channel offsets are multiples of 8) as two
 // 128-bit loads; scalar loads here cost 8 L1 wavefronts per warp instruction once C >= 256
@@ -83,7 +80,7 @@ k_channel_sums(const T* __restrict__ a, const TZ* __restrict__ zmask, const T* _
   }
   // replicas actually used by this launch: small grids need few (the finalizing block walks them all)
   int nrep = (int)gridDim.x / 16;
-  nrep = nrep < 4 ? 4 : (nrep > kReplicas ? kReplicas : nrep);
+  nrep = nrep < 4 ? 4 : (nrep > kBnAccReplicas ? kBnAccReplicas : nrep);
   // reduce across ty through shared memory (rows_par <= 32)
   extern __shared__ float sm[];               // [rows_par][NACC][C]
 #pragma unroll
@@ -94,7 +91,7 @@ k_channel_sums(const T* __restrict__ a, const TZ* __restrict__ zmask, const T* _
   for (int idx = threadIdx.x; idx < NACC * C; idx += kEwThreads) {
     float s = 0.f;
     for (int t = 0; t < rows_par; ++t) s += sm[(size_t)t * NACC * C + idx];
-    atomicAdd(accum + (size_t)(blockIdx.x % nrep) * kAccStride + idx, (double)s);
+    atomicAdd(accum + (size_t)(blockIdx.x % nrep) * kBnAccStride + idx, (double)s);
   }
   // ---- last block finalizes ----
   __shared__ unsigned int s_last;
@@ -106,14 +103,14 @@ k_channel_sums(const T* __restrict__ a, const TZ* __restrict__ zmask, const T* _
   __threadfence();
   // sum the replicas into shared memory (reuse the reduction buffer: NACC*C doubles <= 12 KB... held as
   // doubles in a separate static array to keep precision)
-  __shared__ double s_tot[3 * 512];
+  __shared__ double s_tot[kBnAccStride];
   for (int idx = threadIdx.x; idx < NACC * C; idx += kEwThreads) {
     double t = 0.0;
 #pragma unroll 8
-    for (int r = 0; r < nrep; ++r) t += __ldcg(accum + (size_t)r * kAccStride + idx);
+    for (int r = 0; r < nrep; ++r) t += __ldcg(accum + (size_t)r * kBnAccStride + idx);
     s_tot[idx] = t;
 #pragma unroll 8
-    for (int r = 0; r < nrep; ++r) accum[(size_t)r * kAccStride + idx] = 0.0;
+    for (int r = 0; r < nrep; ++r) accum[(size_t)r * kBnAccStride + idx] = 0.0;
   }
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += kEwThreads) {
@@ -156,8 +153,8 @@ k_bn_bwd_finalize_accum(long long M, int C, BnFin f, double* __restrict__ accum,
   const int cl = threadIdx.x, r = threadIdx.y;
   const int c = blockIdx.x * 32 + cl;
   double v0 = 0.0, v1 = 0.0, v2 = 0.0;
-  if (c < C && r < kReplicas) {
-    double* a = accum + (size_t)r * kAccStride;
+  if (c < C && r < kBnAccReplicas) {
+    double* a = accum + (size_t)r * kBnAccStride;
     v0 = a[c]; v1 = a[C + c];
     a[c] = 0.0; a[C + c] = 0.0;
     if (nacc == 3) { v2 = a[2 * C + c]; a[2 * C + c] = 0.0; }
@@ -171,124 +168,62 @@ k_bn_bwd_finalize_accum(long long M, int C, BnFin f, double* __restrict__ accum,
   bn_fin_backward(c, C, s0, s1, s1d, M, f, nacc == 3);
 }
 
-int launch_bn_bwd_finalize_accum(long long M, int C, const float* gamma, const float* mean, const float* invstd,
-                                 float* dgamma, float* dbeta, float* coef, const float* gamma2, const float* mean2,
-                                 const float* invstd2, float* dgamma2, float* dbeta2, float* coef2, double* accum,
-                                 cudaStream_t st) {
+int launch_bn_bwd_finalize_accum(long long M, int C, const BnFin& f, double* accum, cudaStream_t st) {
   MN_CHECK(C <= 512, "bn_bwd_finalize_accum: C=%d", C);
-  BnFin f; memset(&f, 0, sizeof(f));
-  f.gamma = gamma; f.mean = const_cast<float*>(mean); f.invstd = const_cast<float*>(invstd);
-  f.dgamma = dgamma; f.dbeta = dbeta; f.coef = coef;
-  f.gamma2 = gamma2; f.mean2 = mean2; f.invstd2 = invstd2; f.dgamma2 = dgamma2; f.dbeta2 = dbeta2; f.coef2 = coef2;
-  MN_LAUNCH(k_bn_bwd_finalize_accum, cdiv(C, 32), dim3(32, 32), 0, st, M, C, f, accum, gamma2 != nullptr ? 3 : 2);
+  MN_LAUNCH(k_bn_bwd_finalize_accum, cdiv(C, 32), dim3(32, 32), 0, st, M, C, f, accum, f.gamma2 != nullptr ? 3 : 2);
   MN_LAUNCH_CHECK();
   return 0;
 }
 
 // eval-mode scale/shift from the running statistics (no batch statistics)
-__global__ void k_bn_eval_scale(int C, const float* __restrict__ gamma, const float* __restrict__ beta,
-                                const float* __restrict__ run_mean, const float* __restrict__ run_var,
-                                float* __restrict__ mean_out, float* __restrict__ invstd_out,
-                                float* __restrict__ scale, float* __restrict__ shift) {
+__global__ void k_bn_eval_scale(int C, const BnFin f) {
   pdl_prologue();
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const float mean = run_mean[c];
-  const float invstd = 1.0f / sqrtf(run_var[c] + 1e-5f);
-  mean_out[c] = mean; invstd_out[c] = invstd;
-  const float sc = gamma[c] * invstd;
-  scale[c] = sc; shift[c] = beta[c] - mean * sc;
+  const float mean = f.run_mean[c];
+  const float invstd = 1.0f / sqrtf(f.run_var[c] + 1e-5f);
+  f.mean[c] = mean; f.invstd[c] = invstd;
+  const float sc = f.gamma[c] * invstd;
+  f.scale[c] = sc; f.shift[c] = f.beta[c] - mean * sc;
+}
+
+int launch_bn_eval_scale(int C, const BnFin& f, cudaStream_t st) {
+  MN_LAUNCH(k_bn_eval_scale, cdiv(C, 128), 128, 0, st, C, f);
+  MN_LAUNCH_CHECK();
+  return 0;
 }
 
 template <typename T>
-int launch_bn_stats(const T* y, long long M, int C, const float* gamma, const float* beta, float* run_mean,
-                    float* run_var, float* mean_out, float* invstd_out, float* scale, float* shift, int training,
-                    double* accum, unsigned int* counter, cudaStream_t st) {
-  if (!training) {
-    MN_LAUNCH(k_bn_eval_scale, cdiv(C, 128), 128, 0, st, C, gamma, beta, run_mean, run_var, mean_out, invstd_out, scale, shift);
-    MN_LAUNCH_CHECK();
-    return 0;
-  }
-  BnFin f; memset(&f, 0, sizeof(f));
-  f.gamma = gamma; f.beta = beta; f.run_mean = run_mean; f.run_var = run_var; f.mean = mean_out;
-  f.invstd = invstd_out; f.scale = scale; f.shift = shift; f.training = 1;
+int launch_bn_stats(const T* y, long long M, int C, const BnFin& f, double* accum, unsigned int* counter, cudaStream_t st) {
   return launch_sums<T, T>(0, y, nullptr, nullptr, nullptr, M, C, accum, counter, f, st);
 }
-template int launch_bn_stats<float>(const float*, long long, int, const float*, const float*, float*, float*, float*, float*, float*, float*, int, double*, unsigned int*, cudaStream_t);
-template int launch_bn_stats<bf16>(const bf16*, long long, int, const float*, const float*, float*, float*, float*, float*, float*, float*, int, double*, unsigned int*, cudaStream_t);
+template int launch_bn_stats<float>(const float*, long long, int, const BnFin&, double*, unsigned int*, cudaStream_t);
+template int launch_bn_stats<bf16>(const bf16*, long long, int, const BnFin&, double*, unsigned int*, cudaStream_t);
 
 template <typename T, typename TZ>
-int launch_bn_bwd_reduce(const T* dout, const TZ* zmask, const T* y, const T* yd, long long M, int C,
-                         const float* gamma, const float* mean, const float* invstd, float* dgamma, float* dbeta,
-                         float* coef, const float* gamma2, const float* mean2, const float* invstd2,
-                         float* dgamma2, float* dbeta2, float* coef2, double* accum, unsigned int* counter,
-                         cudaStream_t st, const float* mscale, const float* mshift) {
-  BnFin f; memset(&f, 0, sizeof(f));
-  f.mscale = mscale; f.mshift = mshift;
-  f.gamma = gamma; f.mean = const_cast<float*>(mean); f.invstd = const_cast<float*>(invstd);
-  f.dgamma = dgamma; f.dbeta = dbeta; f.coef = coef;
-  f.gamma2 = gamma2; f.mean2 = mean2; f.invstd2 = invstd2; f.dgamma2 = dgamma2; f.dbeta2 = dbeta2; f.coef2 = coef2;
+int launch_bn_bwd_reduce(const T* dout, const TZ* zmask, const T* y, const T* yd, long long M, int C, const BnFin& f,
+                         double* accum, unsigned int* counter, cudaStream_t st) {
   return launch_sums<T, TZ>(yd != nullptr ? 2 : 1, dout, zmask, y, yd, M, C, accum, counter, f, st);
 }
-#define MN_INST_BWD_REDUCE(TA, TZ) template int launch_bn_bwd_reduce<TA, TZ>(const TA*, const TZ*, const TA*, const TA*, long long, int, const float*, const float*, const float*, float*, float*, float*, const float*, const float*, const float*, float*, float*, float*, double*, unsigned int*, cudaStream_t, const float*, const float*);
+#define MN_INST_BWD_REDUCE(TA, TZ) template int launch_bn_bwd_reduce<TA, TZ>(const TA*, const TZ*, const TA*, const TA*, long long, int, const BnFin&, double*, unsigned int*, cudaStream_t);
 MN_INST_BWD_REDUCE(float, float)
 MN_INST_BWD_REDUCE(bf16, bf16)
 MN_INST_BWD_REDUCE(float, hsplit)
 
 // ---------------------------------------------------------------------------
-// forward apply:  z = relu?( scale*y + shift  [+ zres | + scale2*y2 + shift2] )
-// ---------------------------------------------------------------------------
-// y (and the downsample branch's conv output) are conv outputs (T); the identity residual and the result are
-// forward conv operands (TZ)
-template <typename T, typename TZ, int RES>  // RES 0 none, 1 identity tensor, 2 second BN (downsample branch)
-__global__ void __launch_bounds__(kEwThreads)
-k_bn_apply(const T* __restrict__ y, const float* __restrict__ scale, const float* __restrict__ shift,
-           const void* __restrict__ res, const float* __restrict__ scale2, const float* __restrict__ shift2,
-           TZ* __restrict__ z, long long nvec, int C, int relu) {
-  pdl_prologue();
-  const int cv = C >> 3;
-  const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  // the grid stride (gridDim*256) is a multiple of cv, so this thread always sees the same 8 channels
-  const int c0 = (int)(i0 % cv) * 8;
-  float sc[8], sh[8], sc2[8], sh2[8];
-  ld8(scale + c0, sc); ld8(shift + c0, sh);
-  if (RES == 2) { ld8(scale2 + c0, sc2); ld8(shift2 + c0, sh2); }
-#pragma unroll 4
-  for (long long i = i0; i < nvec; i += (long long)gridDim.x * blockDim.x) {
-    Vec8<T> v; v.load(y + i * 8);
-    float o[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) o[k] = v.v[k] * sc[k] + sh[k];
-    if (RES == 1) {
-      Vec8<TZ> r; r.load(reinterpret_cast<const TZ*>(res) + i * 8);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) o[k] += r.v[k];
-    } else if (RES == 2) {
-      Vec8<T> r; r.load(reinterpret_cast<const T*>(res) + i * 8);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) o[k] += r.v[k] * sc2[k] + sh2[k];
-    }
-    Vec8<TZ> w;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) w.v[k] = relu ? fmaxf(o[k], 0.f) : o[k];
-    w.store(z + i * 8);
-  }
-}
-
-
-// ---------------------------------------------------------------------------
-// Lazy finalize (bn_fin.cuh, BnLazy): the consuming kernel turns the accumulated sums into its per-channel parameters.
-// Blocks are laid out (x: pixel groups, y: 64-channel slices) so that a block only needs the sums of 64 channels:
-// thread t sums replicas (t >> 6), (t >> 6) + 4, ... of channel cbase + (t & 63) -- coalesced 512-byte rows of doubles --
-// the four partial sums meet in shared memory.  Thread t < 64 then owns channel cbase + t.
+// Apply kernels.  Blocks are laid out (x: pixel groups, y: 64-channel slices) so that a block only needs the
+// parameters of 64 channels; its prologue puts them in shared memory, read from memory or finalized from the sums
+// (bn_fin.cuh, BnDesc).  Lazy finalize: thread t sums replicas (t >> 6), (t >> 6) + 4, ... of channel cbase + (t & 63)
+// -- coalesced 512-byte rows of doubles -- the four partial sums meet in shared memory.  Thread t < 64 then owns
+// channel cbase + t.
 // ---------------------------------------------------------------------------
 template <int NACC>
-__device__ __forceinline__ void lazy_sums(const BnLazy& L, const int C, const int cbase, double (*part)[3][64],
+__device__ __forceinline__ void lazy_sums(const BnDesc& L, const int C, const int cbase, double (*part)[3][64],
                                           double (&s)[3]) {
   const int c = threadIdx.x & 63, rg = threadIdx.x >> 6;
   double t[3] = {0.0, 0.0, 0.0};
   for (int r = rg; r < L.nrep; r += 4) {
-    const double* a = L.accum + (size_t)r * kAccStride + cbase + c;
+    const double* a = L.accum + (size_t)r * kBnAccStride + cbase + c;
 #pragma unroll
     for (int j = 0; j < NACC; ++j) t[j] += __ldcg(a + (size_t)j * C);
   }
@@ -301,9 +236,8 @@ __device__ __forceinline__ void lazy_sums(const BnLazy& L, const int C, const in
 }
 
 // forward: (scale, shift) of the block's 64 channels into shared memory -- from the sums (lazy) or from memory
-__device__ __forceinline__ void lazy_forward_params(const BnLazy& L, const float* __restrict__ scale,
-                                                    const float* __restrict__ shift, const int C, const int cbase,
-                                                    double (*part)[3][64], float (*out)[64]) {
+__device__ __forceinline__ void lazy_forward_params(const BnDesc& L, const int C, const int cbase, double (*part)[3][64],
+                                                    float (*out)[64]) {
   if (L.accum != nullptr) {
     // gamma / beta are fetched before the sums so that the two memory latencies overlap
     float ga = 0.f, be = 0.f;
@@ -331,132 +265,116 @@ __device__ __forceinline__ void lazy_forward_params(const BnLazy& L, const float
       }
     }
   } else if (threadIdx.x < 64) {
-    out[0][threadIdx.x] = __ldg(scale + cbase + threadIdx.x);
-    out[1][threadIdx.x] = __ldg(shift + cbase + threadIdx.x);
+    out[0][threadIdx.x] = __ldg(L.f.scale + cbase + threadIdx.x);
+    out[1][threadIdx.x] = __ldg(L.f.shift + cbase + threadIdx.x);
   }
 }
 
+// at most 8 blocks of 256 threads per SM (full occupancy): with 4 loads in flight per thread they cover the HBM
+// latency-bandwidth product, and fewer, fatter threads amortise the per-block parameter prologue over more pixels
 static int slice_grid_x(long long M, int C) {
-  static int per_sm = 0;
-  if (per_sm == 0) { const char* e = getenv("MAPNET_EW_BLOCKS_PER_SM"); per_sm = e ? atoi(e) : 8; if (per_sm < 1 || per_sm > 8) per_sm = 8; }
   const long long slices = C >> 6;
   long long gx = (M + 31) / 32;
-  long long cap = ((long long)kNumSMs * per_sm) / slices;
+  long long cap = ((long long)kNumSMs * 8) / slices;
   if (cap < 1) cap = 1;
   if (gx > cap) gx = cap;
   return (int)(gx < 1 ? 1 : gx);
 }
 
-// k_bn_apply with the lazy finalize: block (x, y) walks pixels x*32 + (t >> 3), ... of channel slice y; thread t owns the
-// 8 channels cbase + 8 * (t & 7) (one 128-byte line of bf16 per pixel and slice)
+// The apply kernels request the first pixel's operands BEFORE their prologue (sums -> fp64 math -> shared memory), so
+// that the DRAM latency overlaps it: those operands are held raw (Raw8) and converted at first use.  The per-pixel body
+// takes each operand from there (PRE) or loads it (every later pixel).
+template <bool PRE, typename V, typename R, typename P>
+__device__ __forceinline__ void fetch8(V& v, const R& pre, const P* __restrict__ p) { if (PRE) pre.get(v); else v.load(p); }
+
+// ---------------------------------------------------------------------------
+// forward apply:  z = relu?( scale*y + shift  [+ zres | + scale2*y2 + shift2] )
+// ---------------------------------------------------------------------------
+// y (and the downsample branch's conv output) are conv outputs (T); the identity residual and the result are
+// forward conv operands (TZ).  RES 0 none, 1 identity tensor, 2 second BN (downsample branch).
+template <typename T, typename TZ, int RES>
+struct ApplyIn {
+  Raw8<T> y, y2; Raw8<TZ> r;
+  __device__ __forceinline__ void load(const T* __restrict__ py, const void* __restrict__ res, const long long off) {
+    y.load(py + off);
+    if (RES == 1) r.load(reinterpret_cast<const TZ*>(res) + off);
+    if (RES == 2) y2.load(reinterpret_cast<const T*>(res) + off);
+  }
+};
+
+// one pixel's 8 channels; p = {scale, shift, scale2, shift2}
+template <typename T, typename TZ, int RES, bool PRE>
+__device__ __forceinline__ void bn_apply_pixel(const ApplyIn<T, TZ, RES>& pre, const T* __restrict__ y,
+                                               const void* __restrict__ res, const float (&p)[4][8], const bool relu,
+                                               TZ* __restrict__ z, const long long off) {
+  Vec8<T> v; fetch8<PRE>(v, pre.y, y + off);
+  float o[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) o[k] = v.v[k] * p[0][k] + p[1][k];
+  if (RES == 1) {
+    Vec8<TZ> r; fetch8<PRE>(r, pre.r, reinterpret_cast<const TZ*>(res) + off);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) o[k] += r.v[k];
+  } else if (RES == 2) {
+    Vec8<T> r; fetch8<PRE>(r, pre.y2, reinterpret_cast<const T*>(res) + off);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) o[k] += r.v[k] * p[2][k] + p[3][k];
+  }
+  Vec8<TZ> w;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) w.v[k] = relu ? fmaxf(o[k], 0.f) : o[k];
+  w.store(z + off);
+}
+
+// block (x, y) walks pixels x*32 + (t >> 3), ... of channel slice y; thread t owns the 8 channels cbase + 8 * (t & 7)
+// (one 128-byte line of bf16 per pixel and slice)
 template <typename T, typename TZ, int RES>
 __global__ void __launch_bounds__(kEwThreads)
-k_bn_apply_lazy(const T* __restrict__ y, const void* __restrict__ res, TZ* __restrict__ z, long long M, int C, int relu,
-                const BnLazy L1, const BnLazy L2) {
+k_bn_apply(const T* __restrict__ y, const void* __restrict__ res, TZ* __restrict__ z, long long M, int C, int relu,
+           const BnDesc L1, const BnDesc L2) {
   pdl_prologue();
   __shared__ double part[4][3][64];
-  __shared__ float par[2][2][64];
+  __shared__ float par[4][64];
   const int cbase = blockIdx.y * 64;
   const int cl = (threadIdx.x & 7) * 8;
-  // the first pixel's operands are requested BEFORE the finalize chain (sums -> fp64 math -> shared memory): their
-  // DRAM latency overlaps it
   const long long p0 = (long long)blockIdx.x * 32 + (threadIdx.x >> 3);
   const long long pstep = (long long)gridDim.x * 32;
-  Raw8<T> v0raw, r0traw; Raw8<TZ> r0zraw;
-  if (p0 < M) {
-    const long long off = p0 * C + cbase + cl;
-    v0raw.load(y + off);
-    if (RES == 1) r0zraw.load(reinterpret_cast<const TZ*>(res) + off);
-    if (RES == 2) r0traw.load(reinterpret_cast<const T*>(res) + off);
-  }
-  lazy_forward_params(L1, L1.f.scale, L1.f.shift, C, cbase, part, par[0]);
-  if (RES == 2) lazy_forward_params(L2, L2.f.scale, L2.f.shift, C, cbase, part, par[1]);
+  ApplyIn<T, TZ, RES> in0;
+  if (p0 < M) in0.load(y, res, p0 * C + cbase + cl);
+  lazy_forward_params(L1, C, cbase, part, par);
+  if (RES == 2) lazy_forward_params(L2, C, cbase, part, par + 2);
   __syncthreads();
-  float sc[8], sh[8], sc2[8], sh2[8];
+  float p[4][8];
 #pragma unroll
-  for (int k = 0; k < 8; ++k) { sc[k] = par[0][0][cl + k]; sh[k] = par[0][1][cl + k]; }
-  if (RES == 2) {
+  for (int j = 0; j < (RES == 2 ? 4 : 2); ++j)
 #pragma unroll
-    for (int k = 0; k < 8; ++k) { sc2[k] = par[1][0][cl + k]; sh2[k] = par[1][1][cl + k]; }
-  }
-  if (p0 < M) {
-    const long long off = p0 * C + cbase + cl;
-    Vec8<T> v0, r0t; Vec8<TZ> r0z;
-    v0raw.get(v0);
-    if (RES == 1) r0zraw.get(r0z);
-    if (RES == 2) r0traw.get(r0t);
-    float o[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) o[k] = v0.v[k] * sc[k] + sh[k];
-    if (RES == 1) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) o[k] += r0z.v[k];
-    } else if (RES == 2) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) o[k] += r0t.v[k] * sc2[k] + sh2[k];
-    }
-    Vec8<TZ> w;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) w.v[k] = relu ? fmaxf(o[k], 0.f) : o[k];
-    w.store(z + off);
-  }
+    for (int k = 0; k < 8; ++k) p[j][k] = par[j][cl + k];
+  const bool rl = relu != 0;
+  if (p0 < M) bn_apply_pixel<T, TZ, RES, true>(in0, y, res, p, rl, z, p0 * C + cbase + cl);
 #pragma unroll 4
-  for (long long p = p0 + pstep; p < M; p += pstep) {
-    const long long off = p * C + cbase + cl;
-    Vec8<T> v; v.load(y + off);
-    float o[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) o[k] = v.v[k] * sc[k] + sh[k];
-    if (RES == 1) {
-      Vec8<TZ> r; r.load(reinterpret_cast<const TZ*>(res) + off);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) o[k] += r.v[k];
-    } else if (RES == 2) {
-      Vec8<T> r; r.load(reinterpret_cast<const T*>(res) + off);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) o[k] += r.v[k] * sc2[k] + sh2[k];
-    }
-    Vec8<TZ> w;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) w.v[k] = relu ? fmaxf(o[k], 0.f) : o[k];
-    w.store(z + off);
-  }
+  for (long long px = p0 + pstep; px < M; px += pstep)
+    bn_apply_pixel<T, TZ, RES, false>(in0, y, res, p, rl, z, px * C + cbase + cl);
 }
 
 static int ew_grid(long long n) {
   long long g = (n + kEwThreads - 1) / kEwThreads;
-  // few fat threads: the per-thread channel-parameter prologue is amortised over several vectors and
-  // 132*8 blocks x 256 threads (full occupancy) x 4 loads in flight cover the HBM latency-bandwidth product.
-  static int per_sm = 0;
-  if (per_sm == 0) { const char* e = getenv("MAPNET_EW_BLOCKS_PER_SM"); per_sm = e ? atoi(e) : 8; if (per_sm < 1 || per_sm > 8) per_sm = 8; }
-  const long long cap = (long long)kNumSMs * per_sm;
+  const long long cap = (long long)kNumSMs * 8;       // as slice_grid_x
   return (int)(g < cap ? (g < 1 ? 1 : g) : cap);
 }
 
 template <typename T, typename TZ>
-int launch_bn_apply(const T* y, const float* scale, const float* shift, int res_mode, const void* res,
-                    const float* scale2, const float* shift2, TZ* z, long long M, int C, int relu,
-                    cudaStream_t st, const BnLazy* lazy, const BnLazy* lazy2) {
-  if (lazy != nullptr) {
-    MN_CHECK(C % 64 == 0 && C <= 512, "bn_apply (lazy finalize): C=%d", C);
-    MN_CHECK(res_mode != 2 || lazy2 != nullptr, "bn_apply (lazy finalize): the downsample BN needs its descriptor too");
-    BnLazy none; memset(&none, 0, sizeof(none));
-    const dim3 grid(slice_grid_x(M, C), C >> 6);
-    if (res_mode == 0) MN_LAUNCH((k_bn_apply_lazy<T, TZ, 0>), grid, kEwThreads, 0, st, y, nullptr, z, M, C, relu, *lazy, none);
-    else if (res_mode == 1) MN_LAUNCH((k_bn_apply_lazy<T, TZ, 1>), grid, kEwThreads, 0, st, y, res, z, M, C, relu, *lazy, none);
-    else MN_LAUNCH((k_bn_apply_lazy<T, TZ, 2>), grid, kEwThreads, 0, st, y, res, z, M, C, relu, *lazy, *lazy2);
-    MN_LAUNCH_CHECK();
-    return 0;
-  }
-  const long long nvec = M * (C >> 3);
-  const int grid = ew_grid(nvec);
-  if (res_mode == 0) MN_LAUNCH((k_bn_apply<T, TZ, 0>), grid, kEwThreads, 0, st, y, scale, shift, nullptr, nullptr, nullptr, z, nvec, C, relu);
-  else if (res_mode == 1) MN_LAUNCH((k_bn_apply<T, TZ, 1>), grid, kEwThreads, 0, st, y, scale, shift, res, nullptr, nullptr, z, nvec, C, relu);
-  else MN_LAUNCH((k_bn_apply<T, TZ, 2>), grid, kEwThreads, 0, st, y, scale, shift, res, scale2, shift2, z, nvec, C, relu);
+int launch_bn_apply(const T* y, int res_mode, const void* res, TZ* z, long long M, int C, int relu, const BnDesc& bn,
+                    const BnDesc* bn_ds, cudaStream_t st) {
+  MN_CHECK(C % 64 == 0 && C <= 512, "bn_apply: C=%d", C);
+  MN_CHECK(res_mode != 2 || bn_ds != nullptr, "bn_apply: the downsample BN needs its descriptor too");
+  const dim3 grid(slice_grid_x(M, C), C >> 6);
+  if (res_mode == 0) MN_LAUNCH((k_bn_apply<T, TZ, 0>), grid, kEwThreads, 0, st, y, nullptr, z, M, C, relu, bn, bn);
+  else if (res_mode == 1) MN_LAUNCH((k_bn_apply<T, TZ, 1>), grid, kEwThreads, 0, st, y, res, z, M, C, relu, bn, bn);
+  else MN_LAUNCH((k_bn_apply<T, TZ, 2>), grid, kEwThreads, 0, st, y, res, z, M, C, relu, bn, *bn_ds);
   MN_LAUNCH_CHECK();
   return 0;
 }
-#define MN_INST_BN_APPLY(TA, TZ) template int launch_bn_apply<TA, TZ>(const TA*, const float*, const float*, int, const void*, const float*, const float*, TZ*, long long, int, int, cudaStream_t, const BnLazy*, const BnLazy*);
+#define MN_INST_BN_APPLY(TA, TZ) template int launch_bn_apply<TA, TZ>(const TA*, int, const void*, TZ*, long long, int, int, const BnDesc&, const BnDesc*, cudaStream_t);
 MN_INST_BN_APPLY(float, float)
 MN_INST_BN_APPLY(bf16, bf16)
 MN_INST_BN_APPLY(float, hsplit)
@@ -467,14 +385,14 @@ MN_INST_BN_APPLY(float, hsplit)
 // ---------------------------------------------------------------------------
 template <typename T, typename TZ>
 __global__ void __launch_bounds__(kEwThreads)
-k_stem_pool(const T* __restrict__ y, const float* __restrict__ scale, const float* __restrict__ shift,
-            TZ* __restrict__ z, uint8_t* __restrict__ amax, int B, int H, int W, int Ho, int Wo, int C, const BnLazy L) {
+k_stem_pool(const T* __restrict__ y, TZ* __restrict__ z, uint8_t* __restrict__ amax, int B, int H, int W, int Ho, int Wo,
+            int C, const BnDesc L) {
   pdl_prologue();
   // lazy finalize of the stem BatchNorm (C == 64: one channel slice, every block derives all 64 scale / shift pairs)
   __shared__ double part[4][3][64];
   __shared__ float par[2][64];
   if (L.accum != nullptr) {
-    lazy_forward_params(L, scale, shift, C, 0, part, par);
+    lazy_forward_params(L, C, 0, part, par);
     __syncthreads();
   }
   const int cv = C >> 3;
@@ -494,7 +412,7 @@ k_stem_pool(const T* __restrict__ y, const float* __restrict__ scale, const floa
     if (L.accum != nullptr) {
 #pragma unroll
       for (int k = 0; k < 8; ++k) { sc[k] = par[0][c0 + k]; sh[k] = par[1][c0 + k]; }
-    } else { ld8(scale + c0, sc); ld8(shift + c0, sh); }
+    } else { ld8(L.f.scale + c0, sc); ld8(L.f.shift + c0, sh); }
     // all nine window loads are issued unconditionally (border taps read a clamped, valid pixel and are masked out
     // below): with the loads under the border branches the compiler kept them serial and the kernel ran at 23 % of the
     // DRAM rate (ncu r02a: 89 us for 165 MB)
@@ -533,18 +451,16 @@ k_stem_pool(const T* __restrict__ y, const float* __restrict__ scale, const floa
 }
 
 template <typename T, typename TZ>
-int launch_stem_pool(const T* y, const float* scale, const float* shift, TZ* z, uint8_t* amax, int B, int H,
-                     int W, int Ho, int Wo, int C, cudaStream_t st, const BnLazy* lazy) {
+int launch_stem_pool(const T* y, TZ* z, uint8_t* amax, int B, int H, int W, int Ho, int Wo, int C, const BnDesc& bn,
+                     cudaStream_t st) {
   const long long nvec = (long long)B * Ho * Wo * (C >> 3);
   MN_CHECK(nvec < 2147483647LL, "stem_pool: tensor too large for 32-bit indexing");
-  MN_CHECK(lazy == nullptr || C == 64, "stem_pool (lazy finalize): C=%d", C);
-  BnLazy L; memset(&L, 0, sizeof(L));
-  if (lazy != nullptr) L = *lazy;
-  MN_LAUNCH((k_stem_pool<T, TZ>), ew_grid(nvec), kEwThreads, 0, st, y, scale, shift, z, amax, B, H, W, Ho, Wo, C, L);
+  MN_CHECK(bn.accum == nullptr || C == 64, "stem_pool (lazy finalize): C=%d", C);
+  MN_LAUNCH((k_stem_pool<T, TZ>), ew_grid(nvec), kEwThreads, 0, st, y, z, amax, B, H, W, Ho, Wo, C, bn);
   MN_LAUNCH_CHECK();
   return 0;
 }
-#define MN_INST_STEM_POOL(TA, TZ) template int launch_stem_pool<TA, TZ>(const TA*, const float*, const float*, TZ*, uint8_t*, int, int, int, int, int, int, cudaStream_t, const BnLazy*);
+#define MN_INST_STEM_POOL(TA, TZ) template int launch_stem_pool<TA, TZ>(const TA*, TZ*, uint8_t*, int, int, int, int, int, int, const BnDesc&, cudaStream_t);
 MN_INST_STEM_POOL(float, float)
 MN_INST_STEM_POOL(bf16, bf16)
 MN_INST_STEM_POOL(float, hsplit)
@@ -689,11 +605,11 @@ k_stem_pool_bwd_quad(const T* __restrict__ dz, const uint8_t* __restrict__ amax,
   for (int k = 0; k < 8; ++k) { sm[(ty * 2 + 0) * C + tx * 8 + k] = s0[k]; sm[(ty * 2 + 1) * C + tx * 8 + k] = s1[k]; }
   __syncthreads();
   int nrep = (int)gridDim.x / 16;
-  nrep = nrep < 4 ? 4 : (nrep > kReplicas ? kReplicas : nrep);
+  nrep = nrep < 4 ? 4 : (nrep > kBnAccReplicas ? kBnAccReplicas : nrep);
   for (int idx = threadIdx.x; idx < 2 * C; idx += kEwThreads) {
     float t = 0.f;
     for (int r = 0; r < rows; ++r) t += sm[r * 2 * C + idx];
-    atomicAdd(accum + (size_t)(blockIdx.x % nrep) * kAccStride + idx, (double)t);
+    atomicAdd(accum + (size_t)(blockIdx.x % nrep) * kBnAccStride + idx, (double)t);
   }
 }
 
@@ -717,202 +633,132 @@ int launch_stem_pool_bwd(const T* dz, const uint8_t* amax, const T* y, const flo
 template int launch_stem_pool_bwd<float>(const float*, const uint8_t*, const float*, const float*, const float*, float*, int, int, int, int, int, int, cudaStream_t, double*);
 template int launch_stem_pool_bwd<bf16>(const bf16*, const uint8_t*, const bf16*, const float*, const float*, bf16*, int, int, int, int, int, int, cudaStream_t, double*);
 
+// ---------------------------------------------------------------------------
 // backward apply: dy = A*g + B*y + C  [, dyd = Ad*g + Bd*yd + Cd] [, gout = g]
-// dout / y / yd / gout: fp32-math tensors (T); zmask: a forward conv operand (TZ); dy / dyd: backward conv operands (TG)
-template <typename T, typename TZ, typename TG, int DS, int GOUT>
-__global__ void __launch_bounds__(kEwThreads)
-k_bn_bwd_apply(const T* __restrict__ dout, const TZ* __restrict__ zmask, const T* __restrict__ y,
-               const float* __restrict__ coef, TG* __restrict__ dy, const T* __restrict__ yd,
-               const float* __restrict__ coefd, TG* __restrict__ dyd, T* __restrict__ gout, long long nvec,
-               int C, const float* __restrict__ mscale, const float* __restrict__ mshift,
-               const float* __restrict__ gscale) {
-  pdl_prologue();
-  const int cv = C >> 3;
-  const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const int c0 = (int)(i0 % cv) * 8;          // loop invariant (grid stride is a multiple of cv)
-  float cA[8], cB[8], cC[8], dA[8], dB[8], dC[8], msc[8], msh[8];
-  const bool ymask = (zmask == nullptr) && (mscale != nullptr);
-  if (ymask) { ld8(mscale + c0, msc); ld8(mshift + c0, msh); }
-  ld8(coef + c0, cA); ld8(coef + C + c0, cB); ld8(coef + 2 * C + c0, cC);
-  if (DS) { ld8(coefd + c0, dA); ld8(coefd + C + c0, dB); ld8(coefd + 2 * C + c0, dC); }
-  if (gscale != nullptr) {                     // the stored conv operands carry the step's power-of-two scale
-    const float S = __ldg(gscale);
-#pragma unroll
-    for (int k = 0; k < 8; ++k) { cA[k] *= S; cB[k] *= S; cC[k] *= S; if (DS) { dA[k] *= S; dB[k] *= S; dC[k] *= S; } }
+// ---------------------------------------------------------------------------
+// dout / y / yd / gout: fp32-math tensors (T); zmask: a forward conv operand (TZ); dy / dyd: backward conv operands (TG).
+template <typename T, typename TZ, int DS>
+struct BwdApplyIn {
+  Raw8<T> g, y, yd; Raw8<TZ> z;
+  __device__ __forceinline__ void load(const T* __restrict__ dout, const TZ* __restrict__ zmask, const T* __restrict__ py,
+                                       const T* __restrict__ pyd, const long long off) {
+    g.load(dout + off); y.load(py + off);
+    if (zmask != nullptr) z.load(zmask + off);
+    if (DS) yd.load(pyd + off);
   }
-#pragma unroll 4
-  for (long long i = i0; i < nvec; i += (long long)gridDim.x * blockDim.x) {
-    Vec8<T> g, yy; g.load(dout + i * 8); yy.load(y + i * 8);
-    if (zmask != nullptr) {
-      Vec8<TZ> z; z.load(zmask + i * 8);
+};
+
+// one pixel's 8 channels; g is gated by the ReLU: zmask > 0 or mscale*y + mshift > 0 (ygate);
+// p = {A, B, C, Ad, Bd, Cd, mscale, mshift}
+template <typename T, typename TZ, typename TG, int DS, int GOUT, bool PRE>
+__device__ __forceinline__ void bn_bwd_apply_pixel(const BwdApplyIn<T, TZ, DS>& pre, const T* __restrict__ dout,
+                                                   const TZ* __restrict__ zmask, const T* __restrict__ y,
+                                                   const T* __restrict__ yd, const float (&p)[8][8], const bool ygate,
+                                                   TG* __restrict__ dy, TG* __restrict__ dyd, T* __restrict__ gout,
+                                                   const long long off) {
+  Vec8<T> g, yy;
+  fetch8<PRE>(g, pre.g, dout + off); fetch8<PRE>(yy, pre.y, y + off);
+  if (zmask != nullptr) {
+    Vec8<TZ> z; fetch8<PRE>(z, pre.z, zmask + off);
 #pragma unroll
-      for (int k = 0; k < 8; ++k) g.v[k] = (z.v[k] > 0.f) ? g.v[k] : 0.f;
-    } else if (ymask) {
+    for (int k = 0; k < 8; ++k) g.v[k] = (z.v[k] > 0.f) ? g.v[k] : 0.f;
+  } else if (ygate) {
 #pragma unroll
-      for (int k = 0; k < 8; ++k) g.v[k] = (yy.v[k] * msc[k] + msh[k] > 0.f) ? g.v[k] : 0.f;
-    }
-    Vec8<TG> o;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) o.v[k] = cA[k] * g.v[k] + cB[k] * yy.v[k] + cC[k];
-    o.store(dy + i * 8);
-    if (DS) {
-      Vec8<T> y2; y2.load(yd + i * 8);
-      Vec8<TG> o2;
-#pragma unroll
-      for (int k = 0; k < 8; ++k) o2.v[k] = dA[k] * g.v[k] + dB[k] * y2.v[k] + dC[k];
-      o2.store(dyd + i * 8);
-    }
-    if (GOUT) g.store(gout + i * 8);
+    for (int k = 0; k < 8; ++k) g.v[k] = (yy.v[k] * p[6][k] + p[7][k] > 0.f) ? g.v[k] : 0.f;
   }
+  Vec8<TG> o;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) o.v[k] = p[0][k] * g.v[k] + p[1][k] * yy.v[k] + p[2][k];
+  o.store(dy + off);
+  if (DS) {
+    Vec8<T> y2; fetch8<PRE>(y2, pre.yd, yd + off);
+    Vec8<TG> o2;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) o2.v[k] = p[3][k] * g.v[k] + p[4][k] * y2.v[k] + p[5][k];
+    o2.store(dyd + off);
+  }
+  if (GOUT) g.store(gout + off);
 }
 
-// k_bn_bwd_apply with the lazy finalize (same block layout as k_bn_apply_lazy): the block derives A, B, C (and the
-// downsample BatchNorm's) for its 64 channels from the sums the producing dgrad / pool-backward kernel accumulated;
-// blockIdx.x == 0 writes d gamma / d beta (and the coefficients, for the record)
+// Same block layout as k_bn_apply.  With sums (L.accum != nullptr) the block derives A, B, C (and the downsample
+// BatchNorm's) for its 64 channels from the sums the producing dgrad / pool-backward kernel accumulated, and
+// blockIdx.x == 0 writes d gamma / d beta (and the coefficients, for the record); without, it reads the coefficients.
+// gscale != nullptr (strict mode): the coefficients are multiplied by the step's power-of-two scale *gscale in fp32.
 template <typename T, typename TZ, typename TG, int DS, int GOUT>
 __global__ void __launch_bounds__(kEwThreads)
-k_bn_bwd_apply_lazy(const T* __restrict__ dout, const TZ* __restrict__ zmask, const T* __restrict__ y,
-                    TG* __restrict__ dy, const T* __restrict__ yd, TG* __restrict__ dyd, T* __restrict__ gout,
-                    long long M, int C, const float* __restrict__ mscale, const float* __restrict__ mshift,
-                    const float* __restrict__ gscale, const BnLazy L) {
+k_bn_bwd_apply(const T* __restrict__ dout, const TZ* __restrict__ zmask, const T* __restrict__ y, TG* __restrict__ dy,
+               const T* __restrict__ yd, TG* __restrict__ dyd, T* __restrict__ gout, long long M, int C,
+               const float* __restrict__ gscale, const BnDesc L) {
   pdl_prologue();
   __shared__ double part[4][3][64];
   __shared__ float par[8][64];            // A, B, C, Ad, Bd, Cd, mscale, mshift
   const int cbase = blockIdx.y * 64;
   const int cl = (threadIdx.x & 7) * 8;
-  // the first pixel's operands are requested before the finalize chain: their DRAM latency overlaps it
   const long long p0 = (long long)blockIdx.x * 32 + (threadIdx.x >> 3);
   const long long pstep = (long long)gridDim.x * 32;
-  Raw8<T> g0raw, y0raw, yd0raw; Raw8<TZ> z0raw;
-  if (p0 < M) {
-    const long long off = p0 * C + cbase + cl;
-    g0raw.load(dout + off); y0raw.load(y + off);
-    if (zmask != nullptr) z0raw.load(zmask + off);
-    if (DS) yd0raw.load(yd + off);
-  }
+  BwdApplyIn<T, TZ, DS> in0;
+  if (p0 < M) in0.load(dout, zmask, y, yd, p0 * C + cbase + cl);
   {
+    const int t = threadIdx.x, c = cbase + t;
     // per-channel inputs of the finalize are fetched before the sums so that the memory latencies overlap
     float pmu = 0.f, pis = 0.f, pga = 0.f, pmu2 = 0.f, pis2 = 0.f, pga2 = 0.f, S = 1.f;
-    if (threadIdx.x < 64) {
-      const int c = cbase + threadIdx.x;
-      pmu = __ldg(L.f.mean + c); pis = __ldg(L.f.invstd + c); pga = __ldg(L.f.gamma + c);
-      if (DS) { pmu2 = __ldg(L.f.mean2 + c); pis2 = __ldg(L.f.invstd2 + c); pga2 = __ldg(L.f.gamma2 + c); }
-      if (gscale != nullptr) S = __ldg(gscale);                      // strict mode: the step's power-of-two scale
+    if (t < 64) {
+      if (gscale != nullptr) S = __ldg(gscale);
+      if (L.accum != nullptr) {
+        pmu = __ldg(L.f.mean + c); pis = __ldg(L.f.invstd + c); pga = __ldg(L.f.gamma + c);
+        if (DS) { pmu2 = __ldg(L.f.mean2 + c); pis2 = __ldg(L.f.invstd2 + c); pga2 = __ldg(L.f.gamma2 + c); }
+      } else {
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+          par[j][t] = __ldg(L.f.coef + j * C + c) * S;
+          if (DS) par[3 + j][t] = __ldg(L.f.coef2 + j * C + c) * S;
+        }
+      }
+      if (L.f.mscale != nullptr) { par[6][t] = __ldg(L.f.mscale + c); par[7][t] = __ldg(L.f.mshift + c); }
     }
-    double s[3];
-    lazy_sums<DS ? 3 : 2>(L, C, cbase, part, s);
-    if (threadIdx.x < 64) {
-      const int c = cbase + threadIdx.x;
-      const double invM = L.invM;
-      {   // the arithmetic of bn_fin_backward
-        const double mu = (double)pmu, is = (double)pis;
-        const double s2 = is * (s[1] - mu * s[0]);
-        const double A = (double)pga * is;
-        const double Bc = -A * is * s2 * invM;
-        const double Cc = -A * s[0] * invM - Bc * mu;
-        par[0][threadIdx.x] = (float)A * S; par[1][threadIdx.x] = (float)Bc * S; par[2][threadIdx.x] = (float)Cc * S;
+    if (L.accum != nullptr) {
+      double s[3];
+      lazy_sums<DS ? 3 : 2>(L, C, cbase, part, s);
+      if (t < 64) {
+        const BnBwdCoef k = bn_bwd_coef(pmu, pis, pga, s[0], s[1], L.invM);
+        par[0][t] = (float)k.A * S; par[1][t] = (float)k.B * S; par[2][t] = (float)k.C * S;
+        if (DS) {
+          const BnBwdCoef kd = bn_bwd_coef(pmu2, pis2, pga2, s[0], s[2], L.invM);
+          par[3][t] = (float)kd.A * S; par[4][t] = (float)kd.B * S; par[5][t] = (float)kd.C * S;
+        }
+        if (blockIdx.x == 0) bn_fin_backward(c, C, s[0], s[1], s[2], L.M, L.f, DS != 0);
       }
-      if (DS) {
-        const double mu = (double)pmu2, is = (double)pis2;
-        const double s2 = is * (s[2] - mu * s[0]);
-        const double A = (double)pga2 * is;
-        const double Bc = -A * is * s2 * invM;
-        const double Cc = -A * s[0] * invM - Bc * mu;
-        par[3][threadIdx.x] = (float)A * S; par[4][threadIdx.x] = (float)Bc * S; par[5][threadIdx.x] = (float)Cc * S;
-      }
-      if (mscale != nullptr) { par[6][threadIdx.x] = __ldg(mscale + c); par[7][threadIdx.x] = __ldg(mshift + c); }
-      if (blockIdx.x == 0) bn_fin_backward(c, C, s[0], s[1], s[2], L.M, L.f, DS != 0);
     }
   }
   __syncthreads();
-  float cA[8], cB[8], cC[8], dA[8], dB[8], dC[8], msc[8], msh[8];
-  const bool ymask = (zmask == nullptr) && (mscale != nullptr);
+  const bool ygate = zmask == nullptr && L.f.mscale != nullptr;
+  float p[8][8];
 #pragma unroll
-  for (int k = 0; k < 8; ++k) { cA[k] = par[0][cl + k]; cB[k] = par[1][cl + k]; cC[k] = par[2][cl + k]; }
-  if (DS) {
+  for (int j = 0; j < 8; ++j)
+    if (j < 3 || (DS && j < 6) || (j >= 6 && ygate))
 #pragma unroll
-    for (int k = 0; k < 8; ++k) { dA[k] = par[3][cl + k]; dB[k] = par[4][cl + k]; dC[k] = par[5][cl + k]; }
-  }
-  if (ymask) {
-#pragma unroll
-    for (int k = 0; k < 8; ++k) { msc[k] = par[6][cl + k]; msh[k] = par[7][cl + k]; }
-  }
-  if (p0 < M) {
-    const long long off = p0 * C + cbase + cl;
-    Vec8<T> g, yy; g0raw.get(g); y0raw.get(yy);
-    if (zmask != nullptr) {
-      Vec8<TZ> z; z0raw.get(z);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) g.v[k] = (z.v[k] > 0.f) ? g.v[k] : 0.f;
-    } else if (ymask) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) g.v[k] = (yy.v[k] * msc[k] + msh[k] > 0.f) ? g.v[k] : 0.f;
-    }
-    Vec8<TG> o;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) o.v[k] = cA[k] * g.v[k] + cB[k] * yy.v[k] + cC[k];
-    o.store(dy + off);
-    if (DS) {
-      Vec8<T> y2; yd0raw.get(y2);
-      Vec8<TG> o2;
-#pragma unroll
-      for (int k = 0; k < 8; ++k) o2.v[k] = dA[k] * g.v[k] + dB[k] * y2.v[k] + dC[k];
-      o2.store(dyd + off);
-    }
-    if (GOUT) g.store(gout + off);
-  }
+      for (int k = 0; k < 8; ++k) p[j][k] = par[j][cl + k];
+  if (p0 < M)
+    bn_bwd_apply_pixel<T, TZ, TG, DS, GOUT, true>(in0, dout, zmask, y, yd, p, ygate, dy, dyd, gout, p0 * C + cbase + cl);
 #pragma unroll 4
-  for (long long p = p0 + pstep; p < M; p += pstep) {
-    const long long off = p * C + cbase + cl;
-    Vec8<T> g, yy; g.load(dout + off); yy.load(y + off);
-    if (zmask != nullptr) {
-      Vec8<TZ> z; z.load(zmask + off);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) g.v[k] = (z.v[k] > 0.f) ? g.v[k] : 0.f;
-    } else if (ymask) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) g.v[k] = (yy.v[k] * msc[k] + msh[k] > 0.f) ? g.v[k] : 0.f;
-    }
-    Vec8<TG> o;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) o.v[k] = cA[k] * g.v[k] + cB[k] * yy.v[k] + cC[k];
-    o.store(dy + off);
-    if (DS) {
-      Vec8<T> y2; y2.load(yd + off);
-      Vec8<TG> o2;
-#pragma unroll
-      for (int k = 0; k < 8; ++k) o2.v[k] = dA[k] * g.v[k] + dB[k] * y2.v[k] + dC[k];
-      o2.store(dyd + off);
-    }
-    if (GOUT) g.store(gout + off);
-  }
+  for (long long px = p0 + pstep; px < M; px += pstep)
+    bn_bwd_apply_pixel<T, TZ, TG, DS, GOUT, false>(in0, dout, zmask, y, yd, p, ygate, dy, dyd, gout, px * C + cbase + cl);
 }
 
 template <typename T, typename TZ, typename TG>
-int launch_bn_bwd_apply(const T* dout, const TZ* zmask, const T* y, const float* coef, TG* dy, const T* yd,
-                        const float* coefd, TG* dyd, T* gout, long long M, int C, cudaStream_t st,
-                        const float* mscale, const float* mshift, const float* gscale, const BnLazy* lazy) {
+int launch_bn_bwd_apply(const T* dout, const TZ* zmask, const T* y, TG* dy, const T* yd, TG* dyd, T* gout, long long M,
+                        int C, const BnDesc& bn, const float* gscale, cudaStream_t st) {
+  MN_CHECK(C % 64 == 0 && C <= 512, "bn_bwd_apply: C=%d", C);
   const bool ds = (yd != nullptr), go = (gout != nullptr);
-  if (lazy != nullptr) {
-    MN_CHECK(C % 64 == 0 && C <= 512, "bn_bwd_apply (lazy finalize): C=%d", C);
-    const dim3 g2(slice_grid_x(M, C), C >> 6);
-    if (ds && !go) MN_LAUNCH((k_bn_bwd_apply_lazy<T, TZ, TG, 1, 0>), g2, kEwThreads, 0, st, dout, zmask, y, dy, yd, dyd, gout, M, C, mscale, mshift, gscale, *lazy);
-    else if (!ds && go) MN_LAUNCH((k_bn_bwd_apply_lazy<T, TZ, TG, 0, 1>), g2, kEwThreads, 0, st, dout, zmask, y, dy, yd, dyd, gout, M, C, mscale, mshift, gscale, *lazy);
-    else if (!ds && !go) MN_LAUNCH((k_bn_bwd_apply_lazy<T, TZ, TG, 0, 0>), g2, kEwThreads, 0, st, dout, zmask, y, dy, yd, dyd, gout, M, C, mscale, mshift, gscale, *lazy);
-    else MN_LAUNCH((k_bn_bwd_apply_lazy<T, TZ, TG, 1, 1>), g2, kEwThreads, 0, st, dout, zmask, y, dy, yd, dyd, gout, M, C, mscale, mshift, gscale, *lazy);
-    MN_LAUNCH_CHECK();
-    return 0;
-  }
-  const long long nvec = M * (C >> 3);
-  const int grid = ew_grid(nvec);
-  if (ds && !go) MN_LAUNCH((k_bn_bwd_apply<T, TZ, TG, 1, 0>), grid, kEwThreads, 0, st, dout, zmask, y, coef, dy, yd, coefd, dyd, gout, nvec, C, mscale, mshift, gscale);
-  else if (!ds && go) MN_LAUNCH((k_bn_bwd_apply<T, TZ, TG, 0, 1>), grid, kEwThreads, 0, st, dout, zmask, y, coef, dy, yd, coefd, dyd, gout, nvec, C, mscale, mshift, gscale);
-  else if (!ds && !go) MN_LAUNCH((k_bn_bwd_apply<T, TZ, TG, 0, 0>), grid, kEwThreads, 0, st, dout, zmask, y, coef, dy, yd, coefd, dyd, gout, nvec, C, mscale, mshift, gscale);
-  else MN_LAUNCH((k_bn_bwd_apply<T, TZ, TG, 1, 1>), grid, kEwThreads, 0, st, dout, zmask, y, coef, dy, yd, coefd, dyd, gout, nvec, C, mscale, mshift, gscale);
+  const dim3 grid(slice_grid_x(M, C), C >> 6);
+  if (ds && !go) MN_LAUNCH((k_bn_bwd_apply<T, TZ, TG, 1, 0>), grid, kEwThreads, 0, st, dout, zmask, y, dy, yd, dyd, gout, M, C, gscale, bn);
+  else if (!ds && go) MN_LAUNCH((k_bn_bwd_apply<T, TZ, TG, 0, 1>), grid, kEwThreads, 0, st, dout, zmask, y, dy, yd, dyd, gout, M, C, gscale, bn);
+  else if (!ds && !go) MN_LAUNCH((k_bn_bwd_apply<T, TZ, TG, 0, 0>), grid, kEwThreads, 0, st, dout, zmask, y, dy, yd, dyd, gout, M, C, gscale, bn);
+  else MN_LAUNCH((k_bn_bwd_apply<T, TZ, TG, 1, 1>), grid, kEwThreads, 0, st, dout, zmask, y, dy, yd, dyd, gout, M, C, gscale, bn);
   MN_LAUNCH_CHECK();
   return 0;
 }
-#define MN_INST_BWD_APPLY(TA, TZ, TG) template int launch_bn_bwd_apply<TA, TZ, TG>(const TA*, const TZ*, const TA*, const float*, TG*, const TA*, const float*, TG*, TA*, long long, int, cudaStream_t, const float*, const float*, const float*, const BnLazy*);
+#define MN_INST_BWD_APPLY(TA, TZ, TG) template int launch_bn_bwd_apply<TA, TZ, TG>(const TA*, const TZ*, const TA*, TG*, const TA*, TG*, TA*, long long, int, const BnDesc&, const float*, cudaStream_t);
 MN_INST_BWD_APPLY(float, float, float)
 MN_INST_BWD_APPLY(bf16, bf16, bf16)
 MN_INST_BWD_APPLY(float, hsplit, hsplit)

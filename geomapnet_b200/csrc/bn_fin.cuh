@@ -1,5 +1,5 @@
-// BatchNorm finalize arithmetic of bn.cu: the separate finalize kernel, k_channel_sums and the lazy finalize of the
-// consuming element-wise kernels.
+// BatchNorm finalize arithmetic of bn.cu (k_channel_sums, k_bn_bwd_finalize_accum and the prologues of the apply kernels)
+// and the descriptor through which the training step hands one BatchNorm to bn.cu.
 // Reference semantics: torch.nn.BatchNorm2d training forward / backward as run by
 // /root/reference/models/posenet.py:66 (momentum 0.1, eps 1e-5, unbiased running variance).
 #pragma once
@@ -7,25 +7,32 @@
 
 namespace mapnet {
 
+// Layout of the BatchNorm sum accumulators: replicas of [3][C] doubles (C <= 512), kBnAccStride doubles apart.  Block b of
+// a reducing kernel adds into replica b % nrep: same-address fp64 atomics serialise, the replicas keep that chain short.
+// k_channel_sums and the stem's pool backward use up to kBnAccReplicas replicas.
+constexpr int kBnAccReplicas = 32;
+constexpr int kBnAccStride = 3 * 512;
+
 struct BnFin {
   // forward: batch statistics -> mean / invstd / scale / shift, running statistics
   const float *gamma, *beta;
   float *run_mean, *run_var, *mean, *invstd, *scale, *shift;
-  int training;
   // backward: main BN then downsample BN
   const float *mscale, *mshift;      // optional: ReLU mask recomputed as (mscale*y + mshift > 0) instead of reading z
   const float *gamma2, *mean2, *invstd2;
   float *dgamma, *dbeta, *coef, *dgamma2, *dbeta2, *coef2;
 };
 
-// Finalize performed by the CONSUMING element-wise kernel (bn.cu, k_bn_apply_lazy / k_bn_bwd_apply_lazy / k_stem_pool):
-// every block sums the replicas of its own 64-channel slice and derives scale / shift (forward) or the dy = A*g + B*y + C
-// coefficients (backward) in its prologue; the blocks with blockIdx.x == 0 also write the per-channel results other
-// kernels read later (mean, invstd, scale, shift, running statistics; d gamma, d beta).  This removes the 68 tiny
-// finalize launches of a training step from the critical path (measured: 0.27 ms of a 3.9 ms step).  The accumulators
-// are per-BatchNorm slots zeroed once per step (nobody resets them between producer and consumers).
-struct BnLazy {
-  const double* accum;       // [nrep][3 * 512] replicas; nullptr: not lazy (parameters are read from memory)
+// One BatchNorm as seen by one launch of bn.cu.  With accum != nullptr the CONSUMING element-wise kernel
+// (k_bn_apply / k_bn_bwd_apply / k_stem_pool) finalizes the sums itself (lazy finalize): every block sums the replicas of
+// its own 64-channel slice and derives scale / shift (forward) or the dy = A*g + B*y + C coefficients (backward) in its
+// prologue; the blocks with blockIdx.x == 0 also write the per-channel results other kernels read later (mean, invstd,
+// scale, shift, running statistics; d gamma, d beta).  This removes the 68 tiny finalize launches of a training step from
+// the critical path (measured: 0.27 ms of a 3.9 ms step).  The accumulators are per-BatchNorm slots zeroed once per step
+// (nobody resets them between producer and consumers).  With accum == nullptr the kernels read scale / shift (forward)
+// or coef (backward) from memory, where an earlier finalize left them.
+struct BnDesc {
+  const double* accum;       // [nrep][kBnAccStride] replicas, or nullptr
   int nrep;
   long long M;               // pixels per channel
   double invM, unbias;       // 1 / M and M / (M - 1) from the host: no fp64 division on the consumers' critical path
@@ -52,29 +59,35 @@ __device__ __forceinline__ void bn_fin_forward(const int c, const double s0, con
   f.shift[c] = f.beta[c] - mean * sc;
 }
 
+// backward of one BatchNorm channel from s0 = sum g, s1 = sum g*y:  s2 = sum g * xhat (= d gamma) and the
+// dy = A*g + B*y + C coefficients
+struct BnBwdCoef { double s2, A, B, C; };
+__device__ __forceinline__ BnBwdCoef bn_bwd_coef(const float mean, const float invstd, const float gamma, const double s0,
+                                                 const double s1, const double invM) {
+  const double mu = (double)mean, is = (double)invstd;
+  BnBwdCoef k;
+  k.s2 = is * (s1 - mu * s0);
+  k.A = (double)gamma * is;
+  k.B = -k.A * is * k.s2 * invM;
+  k.C = -k.A * s0 * invM - k.B * mu;
+  return k;
+}
+
 // s0 = sum g, s1 = sum g*y [, s1d = sum g*yd]:  d gamma, d beta and dy = A*g + B*y + C coefficients
 __device__ __forceinline__ void bn_fin_backward(const int c, const int C, const double s0, const double s1,
                                                 const double s1d, const long long M, const BnFin& f, const bool ds) {
   const double invM = 1.0 / (double)M;
   {
-    const double mu = (double)f.mean[c], is = (double)f.invstd[c];
-    const double s2 = is * (s1 - mu * s0);          // sum g * xhat
-    f.dgamma[c] = (float)s2;
+    const BnBwdCoef k = bn_bwd_coef(f.mean[c], f.invstd[c], f.gamma[c], s0, s1, invM);
+    f.dgamma[c] = (float)k.s2;
     f.dbeta[c] = (float)s0;
-    const double A = (double)f.gamma[c] * is;
-    const double Bc = -A * is * s2 * invM;
-    const double Cc = -A * s0 * invM - Bc * mu;
-    f.coef[c] = (float)A; f.coef[C + c] = (float)Bc; f.coef[2 * C + c] = (float)Cc;
+    f.coef[c] = (float)k.A; f.coef[C + c] = (float)k.B; f.coef[2 * C + c] = (float)k.C;
   }
   if (ds) {
-    const double mu = (double)f.mean2[c], is = (double)f.invstd2[c];
-    const double s2 = is * (s1d - mu * s0);
-    f.dgamma2[c] = (float)s2;
+    const BnBwdCoef k = bn_bwd_coef(f.mean2[c], f.invstd2[c], f.gamma2[c], s0, s1d, invM);
+    f.dgamma2[c] = (float)k.s2;
     f.dbeta2[c] = (float)s0;
-    const double A = (double)f.gamma2[c] * is;
-    const double Bc = -A * is * s2 * invM;
-    const double Cc = -A * s0 * invM - Bc * mu;
-    f.coef2[c] = (float)A; f.coef2[C + c] = (float)Bc; f.coef2[2 * C + c] = (float)Cc;
+    f.coef2[c] = (float)k.A; f.coef2[C + c] = (float)k.B; f.coef2[2 * C + c] = (float)k.C;
   }
 }
 #endif

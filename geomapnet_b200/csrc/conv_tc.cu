@@ -169,9 +169,6 @@ __device__ __forceinline__ WgradChunk wgrad_chunk(const WgradParams& P, int c) {
   return ch;
 }
 
-// BN statistic accumulators: replicas of [3][<=512] doubles (Net::kSlotStride)
-static const int kStatStride = 3 * 512;
-
 // x[32] per lane -> lane L ends with sum over the warp's lanes of x[L] (in x[0])
 __device__ __forceinline__ void warp_transpose_reduce(float (&x)[32], int lane) {
 #pragma unroll
@@ -527,7 +524,7 @@ template <int BN>
 __device__ __forceinline__ void epi_flush(float (*all)[3][BN / 32][32], double* __restrict__ stats, const int Cout,
                                           const int tn, const bool third, const int etid) {
   epi_bar();                                    // every warp's sums for this N tile are in shared memory
-  double* acc = stats + (size_t)(blockIdx.x % kConvReplicas) * kStatStride;
+  double* acc = stats + (size_t)(blockIdx.x % kConvReplicas) * kBnAccStride;   // bn_fin.cuh layout
   const int nstat = third ? 3 : 2;
 #pragma unroll 1
   for (int e = etid; e < nstat * BN; e += kEpiThreads) {

@@ -132,10 +132,12 @@ int InferNet::load(const float* params, const float* bufs, cudaStream_t st) {
   }
   for (size_t i = 0; i < spec.bns.size(); ++i) {
     const BNL& b = spec.bns[i];
-    // training = 0: k_bn_eval_scale, the arithmetic of the live eval forward (running statistics are only read)
-    MN_TRY(launch_bn_stats<float>(nullptr, 0, b.C, params + b.g_off, params + b.b_off, const_cast<float*>(bufs + b.rm_off),
-                                  const_cast<float*>(bufs + b.rv_off), eval_scratch, eval_scratch + 512, bn_scale[i],
-                                  bn_shift[i], 0, nullptr, nullptr, st));
+    // the arithmetic of the live eval forward (running statistics are only read)
+    BnFin f; memset(&f, 0, sizeof(f));
+    f.gamma = params + b.g_off; f.beta = params + b.b_off;
+    f.run_mean = const_cast<float*>(bufs + b.rm_off); f.run_var = const_cast<float*>(bufs + b.rv_off);
+    f.mean = eval_scratch; f.invstd = eval_scratch + 512; f.scale = bn_scale[i]; f.shift = bn_shift[i];
+    MN_TRY(launch_bn_eval_scale(b.C, f, st));
   }
   MN_CUDA(cudaMemcpyAsync(head, params + spec.fc_w, (size_t)(spec.wpqr_b + 3 - spec.fc_w) * 4, cudaMemcpyDeviceToDevice, st));
   loaded = true;
@@ -177,7 +179,9 @@ int InferNet::forward_t(const float* x, int B, float droprate, unsigned long lon
   if (n.stem_s2d) MN_TRY(launch_stem_s2d<TZ>(x, (TZ*)A0, B, H, W, n.convs[0].g.Hi, stem_s2d_wsp(n.Wc), st));
   else MN_TRY(launch_stem_im2col<TZ>(x, (TZ*)A0, B, H, W, n.Hc, n.Wc, n.convs[0].g.Ci, st));
   MN_TRY(conv(0, A0, nullptr, y0, 1, 0, 0, st));
-  MN_TRY((launch_stem_pool<T, TZ>((const T*)y0, ident, ident + 64, (TZ*)act[0], nullptr, B, n.Hc, n.Wc, n.Hp, n.Wp, 64, st)));
+  BnDesc id; memset(&id, 0, sizeof(id));        // the stem's BatchNorm and ReLU are in the conv epilogue: identity map
+  id.f.scale = ident; id.f.shift = ident + 64;
+  MN_TRY((launch_stem_pool<T, TZ>((const T*)y0, (TZ*)act[0], nullptr, B, n.Hc, n.Wc, n.Hp, n.Wp, 64, id, st)));
   // blocks: (input, h, output) rotate through the three arena tensors
   int xi = 0;
   for (const BlockL& bl : n.blocks) {

@@ -24,36 +24,31 @@ struct ConvGeom {
 };
 
 // ---- bn.cu -------------------------------------------------------------------
+// accum / counter: the replicated accumulators of bn_fin.cuh and the counter that elects the finalizing block
 template <typename T>
-int launch_bn_stats(const T* y, long long M, int C, const float* gamma, const float* beta, float* run_mean,
-                    float* run_var, float* mean_out, float* invstd_out, float* scale, float* shift, int training,
-                    double* accum, unsigned int* counter, cudaStream_t st);
+int launch_bn_stats(const T* y, long long M, int C, const BnFin& f, double* accum, unsigned int* counter, cudaStream_t st);
+// eval mode: mean / invstd / scale / shift from the running statistics
+int launch_bn_eval_scale(int C, const BnFin& f, cudaStream_t st);
+// f.mscale != nullptr (and zmask == nullptr): the ReLU mask is recomputed from y
 template <typename T, typename TZ>
-int launch_bn_bwd_reduce(const T* dout, const TZ* zmask, const T* y, const T* yd, long long M, int C,
-                         const float* gamma, const float* mean, const float* invstd, float* dgamma, float* dbeta,
-                         float* coef, const float* gamma2, const float* mean2, const float* invstd2,
-                         float* dgamma2, float* dbeta2, float* coef2, double* accum, unsigned int* counter,
-                         cudaStream_t st, const float* mscale = nullptr, const float* mshift = nullptr);
-// res: res_mode 1 -> const TZ* (identity branch), 2 -> const T* (downsample branch conv output)
+int launch_bn_bwd_reduce(const T* dout, const TZ* zmask, const T* y, const T* yd, long long M, int C, const BnFin& f,
+                         double* accum, unsigned int* counter, cudaStream_t st);
+// res: res_mode 1 -> const TZ* (identity branch), 2 -> const T* (downsample branch conv output, BatchNorm bn_ds)
 template <typename T, typename TZ>
-int launch_bn_apply(const T* y, const float* scale, const float* shift, int res_mode, const void* res,
-                    const float* scale2, const float* shift2, TZ* z, long long M, int C, int relu, cudaStream_t st,
-                    const BnLazy* lazy = nullptr, const BnLazy* lazy2 = nullptr);
-// lazy (/ lazy2 for the downsample BN): the kernel finalizes the batch statistics itself (bn_fin.cuh, BnLazy)
+int launch_bn_apply(const T* y, int res_mode, const void* res, TZ* z, long long M, int C, int relu, const BnDesc& bn,
+                    const BnDesc* bn_ds, cudaStream_t st);
 // amax == nullptr: the argmax positions are not stored (eval-mode inference: no backward follows)
 template <typename T, typename TZ>
-int launch_stem_pool(const T* y, const float* scale, const float* shift, TZ* z, uint8_t* amax, int B, int H,
-                     int W, int Ho, int Wo, int C, cudaStream_t st, const BnLazy* lazy = nullptr);
+int launch_stem_pool(const T* y, TZ* z, uint8_t* amax, int B, int H, int W, int Ho, int Wo, int C, const BnDesc& bn,
+                     cudaStream_t st);
 template <typename T>
 int launch_stem_pool_bwd(const T* dz, const uint8_t* amax, const T* y, const float* scale, const float* shift,
                          T* g, int B, int H, int W, int Ho, int Wo, int C, cudaStream_t st, double* accum = nullptr);
+// yd != nullptr: dyd of the downsample BatchNorm too (the second BatchNorm of bn.f);  gscale != nullptr (strict mode):
+// dy / dyd are stored multiplied by the device scalar gscale[0] (a power of two)
 template <typename T, typename TZ, typename TG>
-int launch_bn_bwd_apply(const T* dout, const TZ* zmask, const T* y, const float* coef, TG* dy, const T* yd,
-                        const float* coefd, TG* dyd, T* gout, long long M, int C, cudaStream_t st,
-                        const float* mscale = nullptr, const float* mshift = nullptr, const float* gscale = nullptr,
-                        const BnLazy* lazy = nullptr);
-// gscale != nullptr (strict mode): dy / dyd are stored multiplied by the device scalar gscale[0] (a power of two)
-// lazy: coef / coefd are not read; the kernel derives them from the backward sums (3 per channel when yd != nullptr)
+int launch_bn_bwd_apply(const T* dout, const TZ* zmask, const T* y, TG* dy, const T* yd, TG* dyd, T* gout, long long M,
+                        int C, const BnDesc& bn, const float* gscale, cudaStream_t st);
 
 // ---- conv_simt.cu: fp32 CUDA-core implicit GEMM (strict-parity path) -----------
 template <typename T>
@@ -113,10 +108,7 @@ int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* res
                 double* stats = nullptr, const EpiBwd* bwd = nullptr, const EpiAffine* aff = nullptr);
 // finalize of backward reductions accumulated in `accum` (the stem's pool backward in the CUDA-core modes): d gamma,
 // d beta and the dy = A*g + B*y + C coefficients
-int launch_bn_bwd_finalize_accum(long long M, int C, const float* gamma, const float* mean, const float* invstd,
-                                 float* dgamma, float* dbeta, float* coef, const float* gamma2, const float* mean2,
-                                 const float* invstd2, float* dgamma2, float* dbeta2, float* coef2, double* accum,
-                                 cudaStream_t st);
+int launch_bn_bwd_finalize_accum(long long M, int C, const BnFin& f, double* accum, cudaStream_t st);
 
 // true when the driver accepts a tiled tensor map whose second dimension's stride is smaller than the
 // first dimension's extent (overlapping windows) -- what the space-to-depth stem view needs

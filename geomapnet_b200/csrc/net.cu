@@ -196,9 +196,9 @@ int Net::init(int max_B_, int H_, int W_, int feat_dim_, int precision_) {
   for (auto& c : convs) wd.push_back(c.wd);
   MN_TRY(alloc((void**)&d_wdescs, wd.size() * sizeof(WeightDesc)));
   MN_CUDA(cudaMemcpy(d_wdescs, wd.data(), wd.size() * sizeof(WeightDesc), cudaMemcpyHostToDevice));
-  MN_TRY(alloc((void**)&bn_accum, 32 * 3 * 512 * sizeof(double) + 64));      // kReplicas x [3][512] (bn.cu)
-  MN_CUDA(cudaMemset(bn_accum, 0, 32 * 3 * 512 * sizeof(double) + 64));
-  bn_counter = (unsigned int*)(bn_accum + 32 * 3 * 512);
+  MN_TRY(alloc((void**)&bn_accum, kBnAccReplicas * kBnAccStride * sizeof(double) + 64));
+  MN_CUDA(cudaMemset(bn_accum, 0, kBnAccReplicas * kBnAccStride * sizeof(double) + 64));
+  bn_counter = (unsigned int*)(bn_accum + kBnAccReplicas * kBnAccStride);
   MN_CHECK(bns.size() <= 36, "trunk: %d BatchNorm layers (36 accumulator slots)", (int)bns.size());
   bn_slots_bytes = (size_t)(72 * kSlotReplicas + kStemBwdReplicas) * kSlotStride * sizeof(double);
   MN_TRY(alloc((void**)&bn_slots, bn_slots_bytes));
@@ -440,25 +440,26 @@ template <typename P>
 int Net::bn_forward(int bi, const typename P::A* y, long long M, const float* params, float* bufs, int training,
                     cudaStream_t st) {
   typedef typename P::A T;
-  BNL& b = bns[bi];
-  return launch_bn_stats<T>(y, M, b.C, params + b.g_off, params + b.b_off, bufs + b.rm_off, bufs + b.rv_off,
-                            b.mean, b.invstd, b.scale, b.shift, training, bn_accum, bn_counter, st);
+  const BnFin f = lazy_forward(bi, M, params, bufs, false).f;
+  if (!training) return launch_bn_eval_scale(bns[bi].C, f, st);
+  return launch_bn_stats<T>(y, M, bns[bi].C, f, bn_accum, bn_counter, st);
 }
 
-// finalize descriptors for the consuming element-wise kernels (bn.cu, lazy finalize)
-BnLazy Net::lazy_forward(int bi, long long M, const float* params, float* bufs) {
-  BnLazy L; memset(&L, 0, sizeof(L));
+BnDesc Net::lazy_forward(int bi, long long M, const float* params, float* bufs, bool sums) {
+  BnDesc L; memset(&L, 0, sizeof(L));
   BNL& b = bns[bi];
-  L.accum = fwd_slot(bi); L.nrep = kSlotReplicas; L.M = M;
+  if (sums) { L.accum = fwd_slot(bi); L.nrep = kSlotReplicas; }
+  L.M = M;
   L.invM = 1.0 / (double)M; L.unbias = (M > 1) ? (double)M / (double)(M - 1) : 1.0;
   L.f.gamma = params + b.g_off; L.f.beta = params + b.b_off; L.f.run_mean = bufs + b.rm_off; L.f.run_var = bufs + b.rv_off;
-  L.f.mean = b.mean; L.f.invstd = b.invstd; L.f.scale = b.scale; L.f.shift = b.shift; L.f.training = 1;
+  L.f.mean = b.mean; L.f.invstd = b.invstd; L.f.scale = b.scale; L.f.shift = b.shift;
   return L;
 }
-BnLazy Net::lazy_backward(int bi, int bi_ds, long long M, const float* params, float* grads) {
-  BnLazy L; memset(&L, 0, sizeof(L));
+BnDesc Net::lazy_backward(int bi, int bi_ds, long long M, const float* params, float* grads, bool sums) {
+  BnDesc L; memset(&L, 0, sizeof(L));
   BNL& b = bns[bi];
-  L.accum = bwd_slot(bi); L.nrep = (bi == convs[0].bn) ? kStemBwdReplicas : kSlotReplicas; L.M = M;
+  if (sums) { L.accum = bwd_slot(bi); L.nrep = (bi == convs[0].bn) ? kStemBwdReplicas : kSlotReplicas; }
+  L.M = M;
   L.invM = 1.0 / (double)M; L.unbias = 1.0;
   L.f.gamma = params + b.g_off; L.f.mean = b.mean; L.f.invstd = b.invstd;
   L.f.dgamma = grads + b.g_off; L.f.dbeta = grads + b.b_off; L.f.coef = b.coef;
@@ -498,37 +499,28 @@ int Net::forward_t(const float* x, const float* params, float* bufs, int B, int 
   stats_target = lazy ? fwd_slot(convs[0].bn) : nullptr;
   MN_TRY(conv_fprop<P>(0, (const TZ*)A0, nullptr, (T*)y0, B, st));
   if (!lazy) MN_TRY(bn_forward<P>(convs[0].bn, (const T*)y0, (long long)B * Hc * Wc, params, bufs, training, st));
-  {
-    BNL& b = bns[convs[0].bn];
-    const BnLazy l0 = lazy_forward(convs[0].bn, (long long)B * Hc * Wc, params, bufs);
-    MN_TRY((launch_stem_pool<T, TZ>((const T*)y0, b.scale, b.shift, (TZ*)z0, amax0, B, Hc, Wc, Hp, Wp, 64, st, lazy ? &l0 : nullptr)));
-  }
+  MN_TRY((launch_stem_pool<T, TZ>((const T*)y0, (TZ*)z0, amax0, B, Hc, Wc, Hp, Wp, 64,
+                                  lazy_forward(convs[0].bn, (long long)B * Hc * Wc, params, bufs, lazy), st)));
   const TZ* zin = (const TZ*)z0;
   for (auto& bl : blocks) {
     const long long Mo = (long long)B * bl.Ho * bl.Wo;
-    BNL& b1 = bns[convs[bl.conv1].bn];
-    BNL& b2 = bns[convs[bl.conv2].bn];
-    const BnLazy l1 = lazy_forward(convs[bl.conv1].bn, Mo, params, bufs);
-    const BnLazy l2 = lazy_forward(convs[bl.conv2].bn, Mo, params, bufs);
+    const BnDesc l1 = lazy_forward(convs[bl.conv1].bn, Mo, params, bufs, lazy);
+    const BnDesc l2 = lazy_forward(convs[bl.conv2].bn, Mo, params, bufs, lazy);
     stats_target = lazy ? fwd_slot(convs[bl.conv1].bn) : nullptr;
     MN_TRY(conv_fprop<P>(bl.conv1, zin, nullptr, (T*)bl.y1, B, st));
     if (!lazy) MN_TRY(bn_forward<P>(convs[bl.conv1].bn, (const T*)bl.y1, Mo, params, bufs, training, st));
-    MN_TRY((launch_bn_apply<T, TZ>((const T*)bl.y1, b1.scale, b1.shift, 0, nullptr, nullptr, nullptr, (TZ*)bl.h, Mo, bl.Cout, 1, st,
-                                   lazy ? &l1 : nullptr)));
+    MN_TRY((launch_bn_apply<T, TZ>((const T*)bl.y1, 0, nullptr, (TZ*)bl.h, Mo, bl.Cout, 1, l1, nullptr, st)));
     stats_target = lazy ? fwd_slot(convs[bl.conv2].bn) : nullptr;
     MN_TRY(conv_fprop<P>(bl.conv2, (const TZ*)bl.h, nullptr, (T*)bl.y2, B, st));
     if (!lazy) MN_TRY(bn_forward<P>(convs[bl.conv2].bn, (const T*)bl.y2, Mo, params, bufs, training, st));
     if (bl.convd >= 0) {
-      BNL& bd = bns[convs[bl.convd].bn];
-      const BnLazy ld = lazy_forward(convs[bl.convd].bn, Mo, params, bufs);
+      const BnDesc ld = lazy_forward(convs[bl.convd].bn, Mo, params, bufs, lazy);
       stats_target = lazy ? fwd_slot(convs[bl.convd].bn) : nullptr;
       MN_TRY(conv_fprop<P>(bl.convd, zin, nullptr, (T*)bl.yd, B, st));
       if (!lazy) MN_TRY(bn_forward<P>(convs[bl.convd].bn, (const T*)bl.yd, Mo, params, bufs, training, st));
-      MN_TRY((launch_bn_apply<T, TZ>((const T*)bl.y2, b2.scale, b2.shift, 2, bl.yd, bd.scale, bd.shift, (TZ*)bl.out, Mo, bl.Cout, 1, st,
-                                     lazy ? &l2 : nullptr, lazy ? &ld : nullptr)));
+      MN_TRY((launch_bn_apply<T, TZ>((const T*)bl.y2, 2, bl.yd, (TZ*)bl.out, Mo, bl.Cout, 1, l2, &ld, st)));
     } else {
-      MN_TRY((launch_bn_apply<T, TZ>((const T*)bl.y2, b2.scale, b2.shift, 1, zin, nullptr, nullptr, (TZ*)bl.out, Mo, bl.Cout, 1, st,
-                                     lazy ? &l2 : nullptr)));
+      MN_TRY((launch_bn_apply<T, TZ>((const T*)bl.y2, 1, zin, (TZ*)bl.out, Mo, bl.Cout, 1, l2, nullptr, st)));
     }
     zin = (const TZ*)bl.out;
   }
@@ -617,7 +609,7 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
   // ---- residual blocks, last to first ----
   // fuse_bwd (wgmma path): the dgrad that PRODUCES a BatchNorm's incoming gradient gates it with that
   // BN's ReLU and accumulates its backward reductions in the epilogue (conv_tc.cu, EpiBwd), so only the apply pass
-  // remains, and it finalizes the sums itself (BnLazy).  `pre` = S0 arrives gated with the BN2 sums of this block pending.
+  // remains, and it finalizes the sums itself (BnDesc).  `pre` = S0 arrives gated with the BN2 sums of this block pending.
   bool pre = bwd_pre;
   int conv_lo = (int)convs.size(), conv_hi = -1;       // convs whose weight gradients this call completes
   for (int bi = (int)blocks.size() - 1; bi >= 0; --bi) {
@@ -629,35 +621,21 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
     const long long Mo = (long long)B * bl.Ho * bl.Wo;
     const int C = bl.Cout;
     BNL& b1 = bns[convs[bl.conv1].bn];
-    BNL& b2 = bns[convs[bl.conv2].bn];
     const bool ds = bl.convd >= 0;
     const T* gres = S3;       // gated d out, the gradient of the identity branch
-    // out = relu(bn2(y2) + idt): g = dout*[out>0]; BN2 (and downsample BN) backward
+    // out = relu(bn2(y2) + idt): g = dout*[out>0]; BN2 (and downsample BN) backward.  With `pre`, S0 is already gated
+    // and its sums are in the BN2 slot.
     S1 = (TG*)ring_next(st);
     if (ds) S2 = (TG*)ring_next(st);
-    if (ds) {
-      BNL& bd = bns[convs[bl.convd].bn];
-      if (pre) {
-        const BnLazy lz = lazy_backward(convs[bl.conv2].bn, convs[bl.convd].bn, Mo, params, grads);
-        MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S0, nullptr, (const T*)bl.y2, b2.coef, S1, (const T*)bl.yd, bd.coef, S2, nullptr, Mo, C, st, nullptr, nullptr, gs,
-                                               &lz)));
-      } else {
-        MN_TRY((launch_bn_bwd_reduce<T, TZ>(S0, (const TZ*)bl.out, (const T*)bl.y2, (const T*)bl.yd, Mo, C,
-                                       params + b2.g_off, b2.mean, b2.invstd, grads + b2.g_off, grads + b2.b_off, b2.coef,
-                                       params + bd.g_off, bd.mean, bd.invstd, grads + bd.g_off, grads + bd.b_off, bd.coef,
-                                       bn_accum, bn_counter, st)));
-        MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S0, (const TZ*)bl.out, (const T*)bl.y2, b2.coef, S1, (const T*)bl.yd, bd.coef, S2, nullptr, Mo, C, st, nullptr, nullptr, gs)));
-      }
-    } else if (pre) {
-      const BnLazy lz = lazy_backward(convs[bl.conv2].bn, -1, Mo, params, grads);
-      MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S0, nullptr, (const T*)bl.y2, b2.coef, S1, nullptr, nullptr, nullptr, nullptr, Mo, C, st, nullptr, nullptr, gs,
-                                             &lz)));
-      gres = S0;              // already gated; conv1's dgrad adds it in place
-    } else {
-      MN_TRY((launch_bn_bwd_reduce<T, TZ>(S0, (const TZ*)bl.out, (const T*)bl.y2, nullptr, Mo, C,
-                                     params + b2.g_off, b2.mean, b2.invstd, grads + b2.g_off, grads + b2.b_off, b2.coef,
-                                     nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, bn_accum, bn_counter, st)));
-      MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S0, (const TZ*)bl.out, (const T*)bl.y2, b2.coef, S1, nullptr, nullptr, nullptr, S3, Mo, C, st, nullptr, nullptr, gs)));
+    {
+      const BnDesc d2 = lazy_backward(convs[bl.conv2].bn, ds ? convs[bl.convd].bn : -1, Mo, params, grads, pre);
+      const TZ* zmask = pre ? nullptr : (const TZ*)bl.out;
+      const T* yd = ds ? (const T*)bl.yd : nullptr;
+      if (!pre) MN_TRY((launch_bn_bwd_reduce<T, TZ>(S0, zmask, (const T*)bl.y2, yd, Mo, C, d2.f, bn_accum, bn_counter, st)));
+      // identity branch: the gated gradient is written to S3, unless S0 already holds it (conv1's dgrad adds it in place)
+      T* gout = (ds || pre) ? nullptr : S3;
+      MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S0, zmask, (const T*)bl.y2, S1, yd, ds ? S2 : nullptr, gout, Mo, C, d2, gs, st)));
+      if (!ds && pre) gres = S0;
     }
     // conv2
     MN_TRY(conv_wgrad<P>(bl.conv2, (const TZ*)bl.h, S1, B, st));
@@ -668,20 +646,17 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
     if (fuse_bwd) {
       EpiBwd e1; memset(&e1, 0, sizeof(e1));
       e1.y = (const bf16*)bl.y1; e1.mscale = b1.scale; e1.mshift = b1.shift;
-      const BnLazy lz1 = lazy_backward(convs[bl.conv1].bn, -1, Mo, params, grads);
       stats_target = bwd_slot(convs[bl.conv1].bn);
       MN_TRY(conv_dgrad<P>(bl.conv2, dy2, nullptr, S4, B, st, &e1));
       stats_target = nullptr;
-      MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S4, nullptr, (const T*)bl.y1, b1.coef, S1, nullptr, nullptr, nullptr, nullptr, Mo, C, st, nullptr, nullptr, gs,
-                                             &lz1)));
+      MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S4, nullptr, (const T*)bl.y1, S1, nullptr, nullptr, nullptr, Mo, C,
+                                             lazy_backward(convs[bl.conv1].bn, -1, Mo, params, grads, true), gs, st)));
     } else {
       MN_TRY(conv_dgrad<P>(bl.conv2, dy2, nullptr, S4, B, st));
-      MN_TRY((launch_bn_bwd_reduce<T, TZ>(S4, nullptr, (const T*)bl.y1, nullptr, Mo, C,
-                                     params + b1.g_off, b1.mean, b1.invstd, grads + b1.g_off, grads + b1.b_off, b1.coef,
-                                     nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, bn_accum, bn_counter, st,
-                                     b1.scale, b1.shift)));
-      MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S4, nullptr, (const T*)bl.y1, b1.coef, S1, nullptr, nullptr, nullptr, nullptr, Mo, C, st,
-                                    b1.scale, b1.shift, gs)));
+      BnDesc d1 = lazy_backward(convs[bl.conv1].bn, -1, Mo, params, grads, false);
+      d1.f.mscale = b1.scale; d1.f.mshift = b1.shift;
+      MN_TRY((launch_bn_bwd_reduce<T, TZ>(S4, nullptr, (const T*)bl.y1, nullptr, Mo, C, d1.f, bn_accum, bn_counter, st)));
+      MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S4, nullptr, (const T*)bl.y1, S1, nullptr, nullptr, nullptr, Mo, C, d1, gs, st)));
     }
     // conv1 (+ downsample conv): d zin; with fuse_bwd it is gated by the previous block's output ReLU
     // and carries that block's BN2 (+ downsample BN) reductions
@@ -714,22 +689,17 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
     S2 = (TG*)ring_next(st);
     BNL& b0 = bns[convs[0].bn];
     const long long M0 = (long long)B * Hc * Wc;
+    const BnDesc d0 = lazy_backward(convs[0].bn, -1, M0, params, grads, tc() && stem_fuse);
     if (stem_fuse) {
       // the pool/ReLU backward accumulates the stem BN's (sum g, sum g*y) while it has g and y in registers
       MN_TRY(launch_stem_pool_bwd<T>(S0, amax0, (const T*)y0, b0.scale, b0.shift, S4, B, Hc, Wc, Hp, Wp, 64, st,
                                      tc() ? bwd_slot(convs[0].bn) : bn_accum));
-      if (!tc())
-        MN_TRY(launch_bn_bwd_finalize_accum(M0, 64, params + b0.g_off, b0.mean, b0.invstd, grads + b0.g_off, grads + b0.b_off, b0.coef,
-                                            nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, bn_accum, st));
+      if (!tc()) MN_TRY(launch_bn_bwd_finalize_accum(M0, 64, d0.f, bn_accum, st));
     } else {
       MN_TRY(launch_stem_pool_bwd<T>(S0, amax0, (const T*)y0, b0.scale, b0.shift, S4, B, Hc, Wc, Hp, Wp, 64, st));
-      MN_TRY((launch_bn_bwd_reduce<T, TZ>(S4, (const TZ*)nullptr, (const T*)y0, nullptr, M0, 64,
-                                     params + b0.g_off, b0.mean, b0.invstd, grads + b0.g_off, grads + b0.b_off, b0.coef,
-                                     nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, bn_accum, bn_counter, st)));
+      MN_TRY((launch_bn_bwd_reduce<T, TZ>(S4, (const TZ*)nullptr, (const T*)y0, nullptr, M0, 64, d0.f, bn_accum, bn_counter, st)));
     }
-    const BnLazy lz0 = lazy_backward(convs[0].bn, -1, M0, params, grads);
-    MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S4, (const TZ*)nullptr, (const T*)y0, b0.coef, S2, nullptr, nullptr, nullptr, nullptr, M0, 64, st, nullptr, nullptr, gs,
-                                           (tc() && stem_fuse) ? &lz0 : nullptr)));
+    MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S4, (const TZ*)nullptr, (const T*)y0, S2, nullptr, nullptr, nullptr, M0, 64, d0, gs, st)));
     MN_TRY(conv_wgrad<P>(0, (const TZ*)A0, S2, B, st));
   }
   MN_TRY(wgrad_join(st));       // every asynchronous wgrad of this part has landed in grads_flat (the stem's in dw_krsc)

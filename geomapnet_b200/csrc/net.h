@@ -81,16 +81,18 @@ struct Net {
   float* gscale;                 // strict mode, device: {S, 1/S} -- this step's power-of-two gradient scale
   double* bn_accum; unsigned int* bn_counter;
   // Tensor-core training: the conv epilogues accumulate the BatchNorm sums and the consuming element-wise kernels
-  // finalize them (lazy finalize, bn_fin.cuh: BnLazy).  One accumulator slot per BatchNorm and direction, zeroed once
+  // finalize them (lazy finalize, bn_fin.cuh: BnDesc).  One accumulator slot per BatchNorm and direction, zeroed once
   // per step.  Slots 0..35 forward statistics, 36..71 backward reductions (8 replicas x [3][512] doubles each, what the
   // conv epilogues spread their flushes over), slot 72 (32 replicas) the stem's backward sums from the pool-backward kernel.
   double* bn_slots; size_t bn_slots_bytes;
   double* stats_target;          // where the next conv_fprop / conv_dgrad with fused sums accumulates (nullptr: no sums)
-  static constexpr int kSlotReplicas = 8, kStemBwdReplicas = 32, kSlotStride = 3 * 512;
+  static constexpr int kSlotReplicas = 8, kStemBwdReplicas = kBnAccReplicas, kSlotStride = kBnAccStride;
   double* fwd_slot(int bn) { return bn_slots + (size_t)bn * kSlotReplicas * kSlotStride; }
   double* bwd_slot(int bn) { return bn_slots + (size_t)(bn == convs[0].bn ? 72 : 36 + bn) * kSlotReplicas * kSlotStride; }
-  BnLazy lazy_forward(int bi, long long M, const float* params, float* bufs);
-  BnLazy lazy_backward(int bi, int bi_ds, long long M, const float* params, float* grads);
+  // BatchNorm bi (bi_ds: the downsample BatchNorm applied with it, or -1) as bn.cu sees it; sums: the consuming kernel
+  // finalizes the sums in the BatchNorm's slot, otherwise it reads what an earlier finalize stored
+  BnDesc lazy_forward(int bi, long long M, const float* params, float* bufs, bool sums);
+  BnDesc lazy_backward(int bi, int bi_ds, long long M, const float* params, float* grads, bool sums);
   float *feat, *fcpre, *hdrop, *mask, *dh, *dfeat, *dpredf;
   float* bn_small;               // backing store of the BN small arrays
   float *sq_partials, *sq_out;

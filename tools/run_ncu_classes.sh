@@ -21,7 +21,7 @@ run() {   # name regex skip count [extra bench args]
 # ---- conv engines, bf16 mode (what the bench line runs): the 4th step (3 warm-up steps precede it) ----
 # (ncu matches the regex against the function's base name: no return type, namespace or template arguments)
 # per step: k_tc_conv 38 launches (13 forward: stem + layer1 two-CTA-per-SM <64,1,2>, layer4 <256,1,1>; then the dgrads),
-# k_tc_conv2 30, k_tc_wgrad 7, k_tc_wgrad2 29, k_bn_apply_lazy 32, k_bn_bwd_apply_lazy 33
+# k_tc_conv2 30, k_tc_wgrad 7, k_tc_wgrad2 29, k_bn_apply 32, k_bn_bwd_apply 33
 run conv1cta      '^k_tc_conv$'   114 10
 run conv1cta_bwd  '^k_tc_conv$'   127 6
 run conv1cta_l1bw '^k_tc_conv$'   145 5

@@ -77,13 +77,13 @@ def main():
 
 def elementwise(L, split, hbm=3350.0):
     """BatchNorm apply kernels by stage, against the HBM roofline in ALGORITHMIC bytes (bf16 tensors): forward
-    k_bn_apply_lazy<.., RES> reads y [+ the residual or the downsample conv's output] and writes z: 4 / 6 / 6 bytes per
+    k_bn_apply<.., RES> reads y [+ the residual or the downsample conv's output] and writes z: 4 / 6 / 6 bytes per
     element for RES = 0 / 1 / 2; backward k_bn_bwd_apply*<.., DS, ..> reads the (already ReLU-gated) gradient and y and
     writes dy: 6 bytes per element, 10 with the downsample BN's second input / output (DS = 1), +2 with a second gradient output (GO = 1).  Two launches per
     BasicBlock in each direction (+ the head-side one and the stem's in the backward)."""
     per_stage = [("layer1", 3, B * 64 * 64 * 64), ("layer2", 4, B * 32 * 32 * 128), ("layer3", 6, B * 16 * 16 * 256),
                  ("layer4", 3, B * 8 * 8 * 512)]
-    fw = [x for x in L[:split] if x[0].startswith("k_bn_apply_lazy")]
+    fw = [x for x in L[:split] if x[0].startswith("k_bn_apply")]
     bw = [x for x in L[split:] if x[0].startswith("k_bn_bwd_apply")]
     f_order = [(st, el) for st, nb, el in per_stage for _ in range(2 * nb)]
     b_order = [(st, el) for st, nb, el in reversed(per_stage) for _ in range(2 * nb)] + [("stem", B * 128 * 128 * 64)]
