@@ -12,6 +12,9 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libmapnet_b200.so")
 
 PREC = {"fp32": 0, "bf16": 1, "bf16_simt": 2, "tc_split": 3}
+# precisions of the inference engine (mapnet_infer_*): fp8 exists there only, training stays in PREC
+INFER_PREC = {"bf16": 1, "tc_split": 3, "fp8": 4}
+N_F8_TENSORS = 33      # e4m3 activation tensors of the fp8 engine at ResNet-34: the pool output, 16 x (h, block output)
 LOSS_MODE = {"posenet": 0, "mapnet": 1, "online": 2, "online_gps": 3}
 
 _lib = None
@@ -115,7 +118,12 @@ def lib():
     L.mapnet_infer_arena_bytes.argtypes = [c_int, c_int, c_int, c_int]
     L.mapnet_infer_arena_bytes.restype = c_int64
     L.mapnet_infer_destroy.argtypes = [c_void_p]
-    for name in ("mapnet_infer_create", "mapnet_infer_load", "mapnet_infer_forward", "mapnet_infer_destroy"):
+    L.mapnet_infer_calibrate.argtypes = [c_void_p, c_void_p, c_int, c_void_p]
+    L.mapnet_infer_act_scales.argtypes = [c_void_p, POINTER(c_float), c_int]
+    L.mapnet_test_conv_fp8.argtypes = [c_int] * 7 + [c_void_p] * 7 + [c_int, c_void_p, c_void_p, c_void_p]
+    L.mapnet_test_conv_fp8.restype = c_int
+    for name in ("mapnet_infer_create", "mapnet_infer_load", "mapnet_infer_forward", "mapnet_infer_destroy",
+                 "mapnet_infer_calibrate", "mapnet_infer_act_scales"):
         getattr(L, name).restype = c_int
     for name in ("mapnet_trunk_create", "mapnet_trunk_destroy", "mapnet_param_count", "mapnet_param_info",
                  "mapnet_forward", "mapnet_backward", "mapnet_loss_fwd_bwd", "mapnet_sqnorm",
@@ -136,7 +144,7 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_sgd_step_dev", "mapnet_rmsprop_step_dev", "mapnet_test_conv_affine", "mapnet_infer_create",
             "mapnet_infer_load", "mapnet_infer_forward", "mapnet_infer_arena_bytes", "mapnet_infer_destroy",
             "mapnet_frame_cache_create", "mapnet_frame_cache_ingest", "mapnet_frame_cache_assemble",
-            "mapnet_frame_cache_destroy"]
+            "mapnet_frame_cache_destroy", "mapnet_infer_calibrate", "mapnet_infer_act_scales", "mapnet_test_conv_fp8"]
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 
 
@@ -206,12 +214,24 @@ class Infer(object):
     def __init__(self, max_B, H, W, feat_dim, precision):
         self.h = c_void_p()
         self.max_B, self.H, self.W, self.feat_dim, self.precision = max_B, H, W, feat_dim, precision
-        check(lib().mapnet_infer_create(ctypes.byref(self.h), max_B, H, W, feat_dim, PREC[precision]),
-              "mapnet_infer_create")
+        check(lib().mapnet_infer_create(ctypes.byref(self.h), max_B, H, W, feat_dim,
+                                        INFER_PREC.get(precision, PREC.get(precision, -1))), "mapnet_infer_create")
 
     def load(self, params_flat, bufs_flat):
         check(lib().mapnet_infer_load(self.h, params_flat.data_ptr(), bufs_flat.data_ptr(), stream_ptr()),
               "mapnet_infer_load")
+
+    def calibrate(self, x):
+        """fp8 engines: activation scales from frames x [B,3,H,W] (float32, contiguous, on the device)"""
+        check(lib().mapnet_infer_calibrate(self.h, x.data_ptr(), x.shape[0], stream_ptr()), "mapnet_infer_calibrate")
+
+    def act_scales(self):
+        """fp8 engines: the activation scales in schedule order (pool output, then each block's h and output)"""
+        import torch
+        torch.cuda.current_stream().synchronize()      # the scales of a calibration queued on this stream
+        buf = (c_float * N_F8_TENSORS)()
+        check(lib().mapnet_infer_act_scales(self.h, buf, N_F8_TENSORS), "mapnet_infer_act_scales")
+        return list(buf)
 
     def forward(self, x, pred, droprate, seed, step=UINT64_MAX):
         check(lib().mapnet_infer_forward(self.h, x.data_ptr(), x.shape[0], float(droprate), int(seed), int(step),

@@ -415,6 +415,31 @@ int mapnet_test_conv_affine(int precision, int B, int Hi, int Wi, int Ci, int Co
   return rc;
 }
 
+// One k_f8_conv launch (conv_tc.cu): in0 e4m3 NHWC [B,Hi,Wi,Ci], wmat e4m3 [Co][k][k][Ci], scale / shift fp32 [Co] (the
+// folded table), residual e4m3 (flags bit 1, scaled by *res_scale) or bf16, out e4m3 (flags bit 2, stored as f * *out_inv)
+// or bf16; flags bit 0 ReLU, bit 3 calibration pass: max |f| into *amax (out untouched).
+int mapnet_test_conv_fp8(int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* in0, const void* wmat,
+                         const float* scale, const float* shift, const void* residual, const float* res_scale,
+                         const float* out_inv, int flags, void* out, unsigned int* amax, void* stream) {
+  MN_CHECK(in0 && wmat && scale && shift && B >= 1 && (out || (flags & 8)), "test_conv_fp8: bad argument");
+  MN_CHECK(k == 1 || k == 3, "test_conv_fp8: k must be 1 or 3");
+  MN_CHECK(!(flags & 8) || amax != nullptr, "test_conv_fp8: the calibration pass needs amax");
+  MN_TRY(require_device());
+  cudaStream_t st = (cudaStream_t)stream;
+  ConvGeom g;
+  g.B = B; g.Hi = Hi; g.Wi = Wi; g.Ci = Ci; g.Co = Co; g.KH = g.KW = k; g.stride = stride; g.pad = (k - 1) / 2;
+  g.Ho = (Hi + 2 * g.pad - k) / stride + 1; g.Wo = (Wi + 2 * g.pad - k) / stride + 1;
+  EpiF8 e; memset(&e, 0, sizeof(e));
+  e.scale = scale; e.shift = shift; e.relu = flags & 1; e.res_f8 = (flags >> 1) & 1; e.out_f8 = (flags >> 2) & 1;
+  e.res_scale = res_scale; e.out_inv = out_inv; e.amax = (flags & 8) ? amax : nullptr;
+  TcConvPlan* plan = nullptr;
+  int rc = tc_plan_create_f8(&plan, g, (const uint8_t*)wmat);
+  if (rc == 0) rc = tc_conv_run_f8(plan, (const uint8_t*)in0, residual, out, e, st);
+  if (rc == 0 && cudaStreamSynchronize(st) != cudaSuccess) { set_last_error("test_conv_fp8: %s", cudaGetErrorString(cudaGetLastError())); rc = 1; }
+  if (plan) tc_plan_destroy(plan);
+  return rc;
+}
+
 // ---- eval-mode inference engine (infer.cu) ----
 int64_t mapnet_infer_arena_bytes(int max_B, int H, int W, int precision) {
   return InferNet::arena_bytes(max_B, H, W, precision);
@@ -424,8 +449,8 @@ int mapnet_infer_create(mapnet_infer_t** out, int max_B, int H, int W, int feat_
   MN_CHECK(out != nullptr, "infer_create: null out pointer");
   *out = nullptr;
   // argument errors first: nothing is allocated or launched for a call that cannot succeed
-  MN_CHECK(precision == PREC_BF16_TC || precision == PREC_TC_SPLIT, "infer_create: precision %d is not supported "
-           "(bf16 = %d or tc_split = %d)", precision, PREC_BF16_TC, PREC_TC_SPLIT);
+  MN_CHECK(precision == PREC_BF16_TC || precision == PREC_TC_SPLIT || precision == PREC_FP8, "infer_create: precision %d "
+           "is not supported (bf16 = %d, tc_split = %d or fp8 = %d)", precision, PREC_BF16_TC, PREC_TC_SPLIT, PREC_FP8);
   MN_CHECK(max_B >= 1 && H >= 32 && W >= 32, "infer_create: need max_B >= 1 and H, W >= 32 (got %d, %d, %d)", max_B, H, W);
   MN_CHECK(feat_dim >= 8 && feat_dim % 4 == 0, "infer_create: feat_dim must be a multiple of 4");
   MN_TRY(require_device());
@@ -445,6 +470,17 @@ int mapnet_infer_forward(mapnet_infer_t* h, const float* x, int B, float droprat
                          float* pred, void* stream) {
   MN_CHECK(h != nullptr, "infer_forward: null handle");
   return h->net.forward(x, B, droprate, seed, step, pred, (cudaStream_t)stream);
+}
+
+int mapnet_infer_calibrate(mapnet_infer_t* h, const float* x, int B, void* stream) {
+  MN_CHECK(h != nullptr, "infer_calibrate: null handle");
+  return h->net.calibrate(x, B, (cudaStream_t)stream);
+}
+
+int mapnet_infer_act_scales(mapnet_infer_t* h, float* host_out, int cap) {
+  MN_CHECK(h != nullptr, "infer_act_scales: null handle");
+  const int r = h->net.act_scales(host_out, cap, nullptr);
+  return r < 0 ? r : 0;
 }
 
 int mapnet_infer_destroy(mapnet_infer_t* h) {

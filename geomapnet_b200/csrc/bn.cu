@@ -464,6 +464,7 @@ int launch_stem_pool(const T* y, TZ* z, uint8_t* amax, int B, int H, int W, int 
 MN_INST_STEM_POOL(float, float)
 MN_INST_STEM_POOL(bf16, bf16)
 MN_INST_STEM_POOL(float, hsplit)
+MN_INST_STEM_POOL(bf16, e4m3)     // fp8 inference: the scale table holds 1 / s (layer1's input scale), the store saturates
 
 // stem backward through max-pool and ReLU:  g0[b,ih,iw,c] = [a0>0] * sum_{windows whose argmax is (ih,iw)} dz
 template <typename T>

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -163,6 +164,49 @@ template <> struct Vec8<hsplit> {
     *(reinterpret_cast<uint4*>(p) + 1) = b;
   }
 };
+// ---- e4m3 activations (fp8 inference) -------------------------------------------------------
+// One byte per element; the tensor's power-of-two scale lives elsewhere (infer.cu), so Vec8 moves the scaled values:
+// load dequantizes without the scale, store rounds to nearest even and saturates to +-448 (cvt.rn.satfinite).
+struct e4m3 { uint8_t raw; };
+
+__device__ __forceinline__ uint16_t f8x2_pack(float a, float b) {
+  return (uint16_t)__nv_cvt_float2_to_fp8x2(make_float2(a, b), __NV_SATFINITE, __NV_E4M3);
+}
+__device__ __forceinline__ float2 f8x2_unpack(uint16_t v) {
+  const __half2 h = __half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)v, __NV_E4M3));
+  return __half22float2(h);
+}
+__device__ __forceinline__ uint2 f8x8_pack(const float (&v)[8]) {
+  uint2 r;
+  r.x = (uint32_t)f8x2_pack(v[0], v[1]) | ((uint32_t)f8x2_pack(v[2], v[3]) << 16);
+  r.y = (uint32_t)f8x2_pack(v[4], v[5]) | ((uint32_t)f8x2_pack(v[6], v[7]) << 16);
+  return r;
+}
+__device__ __forceinline__ void f8x8_unpack(const uint2 r, float (&v)[8]) {
+  float2 t;
+  t = f8x2_unpack((uint16_t)(r.x & 0xffffu)); v[0] = t.x; v[1] = t.y;
+  t = f8x2_unpack((uint16_t)(r.x >> 16)); v[2] = t.x; v[3] = t.y;
+  t = f8x2_unpack((uint16_t)(r.y & 0xffffu)); v[4] = t.x; v[5] = t.y;
+  t = f8x2_unpack((uint16_t)(r.y >> 16)); v[6] = t.x; v[7] = t.y;
+}
+// The scale of an e4m3 tensor or weight row with max |x| = amax: the smallest power of two s with 448 * s >= amax, i.e.
+// 2^ceil(log2(amax / 448)), taken from the exponent so that no rounded division or logarithm is involved (amax =
+// m * 2^k, m in [0.5, 1), 448 = 0.875 * 2^9).  amax 0 gives 1; s stays >= 2^-126 so 1 / s is finite.
+__host__ __device__ inline float f8_pow2_scale(float amax) {
+  if (!(amax > 0.f)) return 1.f;
+  if (amax > 3.4028234663852886e38f) return ldexpf(1.f, 120);
+  int k;
+  const float m = frexpf(amax, &k);
+  int e = (m <= 0.875f) ? k - 9 : k - 8;
+  if (e < -126) e = -126;
+  return ldexpf(1.f, e);
+}
+template <> struct Vec8<e4m3> {
+  float v[8];
+  __device__ __forceinline__ void load(const e4m3* p) { f8x8_unpack(*reinterpret_cast<const uint2*>(p), v); }
+  __device__ __forceinline__ void store(e4m3* p) const { *reinterpret_cast<uint2*>(p) = f8x8_pack(v); }
+};
+
 // The same 8 elements held RAW: issue the loads early (software pipelining across a prologue or a barrier -- a warp
 // issues in order, so an early load whose conversion follows at once would stall right there), convert at first use.
 template <typename T> struct Raw8;
@@ -209,6 +253,11 @@ struct TypesSplitHH { typedef float A; typedef hsplit Z; typedef hsplit G; };
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
 __device__ __forceinline__ double warp_sum_d(double v) {

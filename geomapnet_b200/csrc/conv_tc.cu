@@ -48,31 +48,37 @@ static PFN_cuTensorMapEncodeTiled_v12000 get_encode_fn() {
   return fn;
 }
 
-// 4-D NHWC view: dims {C, W, H, N} with byte strides; box {64, bw, bh, bn}; 128B swizzle; OOB -> 0
+// 4-D NHWC view: dims {C, W, H, N} with byte strides; box {box0, bw, bh, bn}; OOB -> 0.  bf16 tiles are 64 channels
+// in 128B-swizzled rows; e4m3 tiles (UINT8) are 128- or 64-channel rows with the matching swizzle.
 static int encode_act_map(CUtensorMap* m, const void* base, int C, int Wd, int Hd, int Nd, long long sw_bytes,
-                          long long sh_bytes, long long sn_bytes, int bw, int bh, int bn) {
+                          long long sh_bytes, long long sn_bytes, int bw, int bh, int bn,
+                          CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, int box0 = 64,
+                          CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
   auto fn = get_encode_fn();
   MN_CHECK(fn != nullptr, "cuTensorMapEncodeTiled entry point not available");
   cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)Wd, (cuuint64_t)Hd, (cuuint64_t)Nd};
   cuuint64_t strides[3] = {(cuuint64_t)sw_bytes, (cuuint64_t)sh_bytes, (cuuint64_t)sn_bytes};
-  cuuint32_t box[4] = {64u, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bn};
+  cuuint32_t box[4] = {(cuuint32_t)box0, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bn};
   cuuint32_t es[4] = {1u, 1u, 1u, 1u};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+  CUresult r = fn(m, dt, 4, const_cast<void*>(base), dims, strides, box, es,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   MN_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(act %dx%dx%dx%d box %d,%d,%d) failed: %d", C, Wd, Hd, Nd, bw, bh, bn, (int)r);
   return 0;
 }
-// 2-D weight matrix [rows][K] (K contiguous): box {64, brows}
-static int encode_w_map(CUtensorMap* m, const void* base, int K, int rows, int brows) {
+// 2-D weight matrix [rows][K] (K contiguous): box {box0, brows} (bf16: 64 elements; e4m3: 128 or 64 bytes)
+static int encode_w_map(CUtensorMap* m, const void* base, int K, int rows, int brows,
+                        CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, int box0 = 64,
+                        CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
   auto fn = get_encode_fn();
   MN_CHECK(fn != nullptr, "cuTensorMapEncodeTiled entry point not available");
+  const int elt = (dt == CU_TENSOR_MAP_DATA_TYPE_UINT8) ? 1 : 2;
   cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)K * 2};
-  cuuint32_t box[2] = {64u, (cuuint32_t)brows};
+  cuuint64_t strides[1] = {(cuuint64_t)K * elt};
+  cuuint32_t box[2] = {(cuuint32_t)box0, (cuuint32_t)brows};
   cuuint32_t es[2] = {1u, 1u};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+  CUresult r = fn(m, dt, 2, const_cast<void*>(base), dims, strides, box, es,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   MN_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(weights K=%d rows=%d) failed: %d", K, rows, (int)r);
   return 0;
@@ -225,6 +231,17 @@ enum : int {
   EPI_RELU = 128,   // with EPI_AFFINE
   EPI_HOUT = 256,   // with EPI_OUT32: store fp16 hi/lo planes (common.cuh: hsplit) instead of fp32
   EPI_HRES = 512,   // with EPI_OUT32 | EPI_RES: the residual is in hi/lo plane form
+  // fp8 inference (k_f8_conv only, with EPI_AFFINE: the scale table is bn_scale * s_in * s_w, see EpiF8)
+  EPI_F8OUT = 1024, // store e4m3(f / s_out) (satfinite) instead of bf16
+  EPI_F8RES = 2048, // with EPI_RES: the residual is e4m3, dequantized as r * s_res
+  EPI_AMAX = 4096,  // calibration: record max |f| over the tensor's rows, store nothing
+};
+
+// The fp8 engine's epilogue operands: EpiBwd's affine fields plus the device scalars of the e4m3 tensors involved
+struct EpiF8Dev : EpiBwd {
+  const float* res_scale;   // s_res (EPI_F8RES)
+  const float* out_inv;     // 1 / s_out (EPI_F8OUT)
+  unsigned int* amax;       // EPI_AMAX: max |f| as the bit pattern of a non-negative float (atomicMax)
 };
 
 struct EpiRegs { uint4 r[4], y[4], z[4], d[4]; };
@@ -268,6 +285,9 @@ __device__ __forceinline__ void epi_issue_loads(EpiRegs& G, const long long (&ro
       const float* rp = reinterpret_cast<const float*>(residual) + off;
       G.r[i] = *reinterpret_cast<const uint4*>(rp);
       G.y[i] = *reinterpret_cast<const uint4*>(rp + 4);
+    } else if ((F & EPI_RES) && (F & EPI_F8RES)) {   // 8 e4m3 values in the low half of the r slot
+      const uint2 v = *reinterpret_cast<const uint2*>(reinterpret_cast<const uint8_t*>(residual) + off);
+      G.r[i].x = v.x; G.r[i].y = v.y;
     } else if (F & EPI_RES) G.r[i] = *reinterpret_cast<const uint4*>(residual + off);   // may alias `out`: plain load
     if (F & EPI_BWD) G.y[i] = __ldg(reinterpret_cast<const uint4*>(E.y + off));
     if (F & EPI_ZMASK) G.z[i] = __ldg(reinterpret_cast<const uint4*>(E.zmask + off));
@@ -288,11 +308,12 @@ __device__ __forceinline__ void acc_to_stage(const float (&d)[BN / 2], float* __
   }
 }
 
-// one 32-column chunk of a warp's 32 staged rows (row stride RS floats)
-template <int F, int RS>
+// one 32-column chunk of a warp's 32 staged rows (row stride RS floats).  EP: EpiBwd, or EpiF8Dev for the fp8 engine's
+// flags (EPI_F8OUT / EPI_F8RES / EPI_AMAX; with EPI_AMAX s0 is the running max |f| of the rows inside the tensor)
+template <int F, int RS, typename EP>
 __device__ __forceinline__ void epi_chunk(const float* __restrict__ scr, const EpiRegs& G,
                                           const long long (&rowoff)[4], const bool (&rstore)[4], const float (&rw)[4],
-                                          const int coff, const int col0, bf16* out, const EpiBwd& E, const int lane,
+                                          const int coff, const int col0, bf16* out, const EP& E, const int lane,
                                           float& s0, float& s1, float& s2) {
   const int p = lane & 3, rr = lane >> 2;
   float4 lo[4], hi[4];
@@ -314,6 +335,9 @@ __device__ __forceinline__ void epi_chunk(const float* __restrict__ scr, const E
   for (int k = 0; k < 8; ++k) { c0[k] = 0.f; c1[k] = 0.f; c2[k] = 0.f; }
   float osc = 1.f;
   if (F & EPI_OUT32) { if (E.oscale != nullptr) osc = __ldg(E.oscale); }
+  float rsc = 1.f, oinv = 1.f;
+  if constexpr ((F & EPI_F8RES) != 0) rsc = __ldg(E.res_scale);
+  if constexpr ((F & EPI_F8OUT) != 0) oinv = __ldg(E.out_inv);
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     float f[8] = {lo[i].x, lo[i].y, lo[i].z, lo[i].w, hi[i].x, hi[i].y, hi[i].z, hi[i].w};
@@ -334,6 +358,11 @@ __device__ __forceinline__ void epi_chunk(const float* __restrict__ scr, const E
         const float2 fh = __half22float2(h[k]), fl = __half22float2(l[k]);
         f[2 * k] += fh.x + fl.x; f[2 * k + 1] += fh.y + fl.y;
       }
+    } else if ((F & EPI_RES) && (F & EPI_F8RES)) {      // r * s_res is exact (s_res a power of two)
+      float r[8];
+      f8x8_unpack(make_uint2(G.r[i].x, G.r[i].y), r);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) f[k] += r[k] * rsc;
     } else if ((F & EPI_RES) && (F & EPI_OUT32)) {
       const float4 r0 = *reinterpret_cast<const float4*>(&G.r[i]), r1 = *reinterpret_cast<const float4*>(&G.y[i]);
       f[0] += r0.x; f[1] += r0.y; f[2] += r0.z; f[3] += r0.w; f[4] += r1.x; f[5] += r1.y; f[6] += r1.z; f[7] += r1.w;
@@ -358,6 +387,18 @@ __device__ __forceinline__ void epi_chunk(const float* __restrict__ scr, const E
     if (F & EPI_RELU) {
 #pragma unroll
       for (int k = 0; k < 8; ++k) f[k] = fmaxf(f[k], 0.f);
+    }
+    if constexpr ((F & EPI_AMAX) != 0) {           // calibration pass: the values the storing pass would quantize
+#pragma unroll
+      for (int k = 0; k < 8; ++k) s0 = fmaxf(s0, rw[i] != 0.f ? fabsf(f[k]) : 0.f);
+      continue;
+    } else if constexpr ((F & EPI_F8OUT) != 0) {   // f / s_out is exact; one rounding, at the e4m3 cast
+      float q[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) q[k] = f[k] * oinv;
+      const uint2 pk = f8x8_pack(q);
+      if (rstore[i]) *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(out) + rowoff[i] + coff + 8 * p) = pk;
+      continue;
     }
     uint4 o;
     if (F & EPI_HOUT) {          // 8 hi then 8 lo fp16 values: the operand form the next conv reads
@@ -416,10 +457,10 @@ __device__ __forceinline__ void epi_chunk(const float* __restrict__ scr, const E
 }
 
 // One accumulator tile (this warp's 32 staged rows x BN columns): walk the warp's 32-column chunks.
-template <int F, int BN>
+template <int F, int BN, typename EP>
 __device__ __forceinline__ void epi_tile(const float* __restrict__ rows, float (*stw)[BN / 32][32],
                                          const long long (&rowoff)[4], const bool (&rvalid)[4], const bool do_store,
-                                         const int tn, const bf16* residual, bf16* out, const EpiBwd& E, const int lane,
+                                         const int tn, const bf16* residual, bf16* out, const EP& E, const int lane,
                                          const int half) {
   bool rstore[4]; float rw[4];
 #pragma unroll
@@ -553,10 +594,11 @@ __device__ __forceinline__ void release_stage(const uint32_t empty_bar, const bo
   if (arriver) mbar_arrive(empty_bar);
 }
 
-// Mainloop of one tile for one consumer warpgroup: kblocks k-blocks of 64, each four wgmma K=16 steps.  A stage is
-// handed back as soon as the wgmma group that read it has retired (one group stays in flight behind the next).
-// a_off / a_step: this warpgroup's A rows inside a stage and the byte step per K=16; b_step likewise for B.
-template <int BN, int FMT, int TA, int TB>
+// Mainloop of one tile for one consumer warpgroup: kblocks k-blocks, each KSTEPS wgmma instructions (bf16: 64 channels
+// as four K=16 steps; e4m3: 128 or 64 channels as four or two K=32 steps -- 32 bytes of a row per step either way).  A
+// stage is handed back as soon as the wgmma group that read it has retired (one group stays in flight behind the next).
+// a_off / a_step: this warpgroup's A rows inside a stage and the byte step per instruction; b_step likewise for B.
+template <int BN, int FMT, int TA, int TB, int KSTEPS = 4>
 __device__ __forceinline__ void mma_tile(float (&d)[BN / 2], const int kblocks, int& stage, uint32_t& phase,
                                          const int STAGES, const uint32_t stage_bytes, const uint32_t smem_base,
                                          const uint32_t a_off, const uint32_t a_step, const uint32_t b_off,
@@ -575,7 +617,7 @@ __device__ __forceinline__ void mma_tile(float (&d)[BN / 2], const int kblocks, 
       const uint32_t sb = smem_base + stage * stage_bytes + b_off;
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
+      for (int k = 0; k < KSTEPS; ++k)
         wgmma_k16<TA, TB>(WgmmaTag<BN, FMT>(), d, smem_desc(adesc, sa + k * a_step), smem_desc(bdesc, sb + k * b_step),
                           (kb > 0 || k > 0) ? 1u : 0u);
       wgmma_commit();
@@ -598,6 +640,63 @@ __device__ __forceinline__ void mma_tile(float (&d)[BN / 2], const int kblocks, 
 // ---------------------------------------------------------------------------------
 // fprop / dgrad kernel
 // ---------------------------------------------------------------------------------
+// TMA producer of the fprop / dgrad engines (one elected lane): every (work item, filter tap, channel block) of this
+// CTA into the stage ring.  KB: channels per block of the activation tensor (bf16: 64; e4m3: 128 or 64 = one 128- or
+// 64-byte row), which is also the K extent of the weight box.
+template <int STAGES, uint32_t A_BYTES, uint32_t STAGE_BYTES, int BN, int KB>
+__device__ __forceinline__ void conv_producer(const ConvParams& P, const CUtensorMap* mapA0, const CUtensorMap* mapA1,
+                                              const CUtensorMap* mapA2, const CUtensorMap* mapA3, const CUtensorMap* mapB,
+                                              const CUtensorMap* mapB2, const uint32_t smem_base, const uint32_t full0,
+                                              const uint32_t empty0, const int first_tile, const int total_tiles,
+                                              const int tile_step, const int per_class) {
+  int stage = 0; uint32_t phase = 0;
+  for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
+    const TileCoord tc = decode_tile(tile, per_class, P.n_tiles_n);
+    const ClassDesc cd = P.cls[tc.cls];
+    const int tn = tc.tn;
+    int tm = tc.tm;
+    const int tw = tm % P.tiles_w; tm /= P.tiles_w;
+    const int th = tm % P.tiles_h;
+    const int tb = tm / P.tiles_h;
+    const int jw0 = tw * P.TW, jh0 = th * P.TH, n0 = tb * P.TN;
+    for (int t = cd.tap0; t < cd.tap0 + cd.num_taps; ++t) {
+      const TapDesc tap = P.taps[t];
+      const int am = tap.map & 3;
+      const CUtensorMap* mA = (am == 0) ? mapA0 : (am == 1) ? mapA1 : (am == 2) ? mapA2 : mapA3;
+      const CUtensorMap* mB = (tap.map & 4) ? mapB2 : mapB;
+      for (int cb = 0; cb < P.cblocks; ++cb) {
+        mbar_wait(empty0 + 8 * stage, phase ^ 1);
+        const uint32_t sa = smem_base + stage * STAGE_BYTES;
+        if (P.debug == 2) { mbar_arrive(full0 + 8 * stage); if (++stage == STAGES) { stage = 0; phase ^= 1; } continue; }
+        mbar_expect_tx(full0 + 8 * stage, STAGE_BYTES);
+        tma_load_4d(sa, mA, full0 + 8 * stage, cb * KB, jw0 + tap.dw, jh0 + tap.dh, n0);
+        tma_load_2d(sa + A_BYTES, mB, full0 + 8 * stage, tap.kidx * P.Cs + cb * KB, tn * BN);
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+    }
+  }
+}
+
+// the 4 output rows this lane owns in the coalesced epilogue layout (tile row q*32 + 8i + (lane>>2)) of M tile tm:
+// element offsets of (row, column col0), and whether the row lies inside the tensor
+__device__ __forceinline__ void tile_rows(const ConvParams& P, const ClassDesc& cd, int tm, const int q, const int lane,
+                                          const int col0, long long (&rowoff)[4], bool (&rvalid)[4]) {
+  const int tw = tm % P.tiles_w; tm /= P.tiles_w;
+  const int th = tm % P.tiles_h;
+  const int tb = tm / P.tiles_h;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int m = q * 32 + 8 * i + (lane >> 2);
+    const int lw = m % P.TW;
+    const int lh = (m / P.TW) % P.TH;
+    const int ln = m / (P.TW * P.TH);
+    const int jw = tw * P.TW + lw, jh = th * P.TH + lh, n = tb * P.TN + ln;
+    rvalid[i] = (jw < cd.Ws) && (jh < cd.Hs) && (n < P.Nimg);
+    const long long pix = ((long long)n * P.Hout + (jh * P.os + cd.oa)) * P.Wout + (jw * P.os + cd.ob);
+    rowoff[i] = (rvalid[i] ? pix * P.Cout : 0) + col0;     // outside rows: clamped, loads stay in bounds
+  }
+}
+
 // AFF: the eval-mode inference epilogues (EPI_AFFINE) instead of the training ones.
 template <int BN, bool AFF = false>
 __global__ void __launch_bounds__(kConvThreads, 1)
@@ -636,34 +735,9 @@ k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
 
   if (warp == kProducerWarp) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
-      int stage = 0; uint32_t phase = 0;
-      for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
-        const TileCoord tc = decode_tile(tile, per_class, P.n_tiles_n);
-        const ClassDesc cd = P.cls[tc.cls];
-        const int tn = tc.tn;
-        int tm = tc.tm;
-        const int tw = tm % P.tiles_w; tm /= P.tiles_w;
-        const int th = tm % P.tiles_h;
-        const int tb = tm / P.tiles_h;
-        const int jw0 = tw * P.TW, jh0 = th * P.TH, n0 = tb * P.TN;
-        for (int t = cd.tap0; t < cd.tap0 + cd.num_taps; ++t) {
-          const TapDesc tap = P.taps[t];
-          const int am = tap.map & 3;
-          const CUtensorMap* mA = (am == 0) ? &mapA0 : (am == 1) ? &mapA1 : (am == 2) ? &mapA2 : &mapA3;
-          const CUtensorMap* mB = (tap.map & 4) ? &mapB2 : &mapB;
-          for (int cb = 0; cb < P.cblocks; ++cb) {
-            mbar_wait(empty0 + 8 * stage, phase ^ 1);
-            const uint32_t sa = smem_base + stage * STAGE_BYTES;
-            if (P.debug == 2) { mbar_arrive(full0 + 8 * stage); if (++stage == STAGES) { stage = 0; phase ^= 1; } continue; }
-            mbar_expect_tx(full0 + 8 * stage, STAGE_BYTES);
-            tma_load_4d(sa, mA, full0 + 8 * stage, cb * 64, jw0 + tap.dw, jh0 + tap.dh, n0);
-            tma_load_2d(sa + A_BYTES, mB, full0 + 8 * stage, tap.kidx * P.Cs + cb * 64, tn * BN);
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
+    if (elect_one())
+      conv_producer<STAGES, A_BYTES, STAGE_BYTES, BN, 64>(P, &mapA0, &mapA1, &mapA2, &mapA3, &mapB, &mapB2, smem_base, full0,
+                                                         empty0, first_tile, total_tiles, tile_step, per_class);
   } else {
     // ===================== consumer warpgroups: MMAs, then the epilogue of their own 64 rows =====================
     const int wg = warp >> 2;               // accumulator rows 64*wg .. 64*wg + 63 of the tile
@@ -699,23 +773,8 @@ k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
                               DESC_BASE, DESC_BASE, full0, empty0, arriver, P.debug == 1);
       // inference launches carry no statistics (tc_conv_run checks it): no flush is compiled into those kernels
       if (!AFF && stats != nullptr && tn != st_tn) { if (st_tn >= 0) flush_stats(st_tn); st_tn = tn; }
-      int tm = tc.tm;
-      const int tw = tm % P.tiles_w; tm /= P.tiles_w;
-      const int th = tm % P.tiles_h;
-      const int tb = tm / P.tiles_h;
-      // the 4 rows this lane owns in the coalesced layout: tile row q*32 + 8i + (lane>>2)
       long long rowoff[4]; bool rvalid[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int m = q * 32 + 8 * i + (lane >> 2);
-        const int lw = m % P.TW;
-        const int lh = (m / P.TW) % P.TH;
-        const int ln = m / (P.TW * P.TH);
-        const int jw = tw * P.TW + lw, jh = th * P.TH + lh, n = tb * P.TN + ln;
-        rvalid[i] = (jw < cd.Ws) && (jh < cd.Hs) && (n < P.Nimg);
-        const long long pix = ((long long)n * P.Hout + (jh * P.os + cd.oa)) * P.Wout + (jw * P.os + cd.ob);
-        rowoff[i] = (rvalid[i] ? pix * P.Cout : 0) + tn * BN;     // outside rows: clamped, loads stay in bounds
-      }
+      tile_rows(P, cd, tc.tm, q, lane, tn * BN, rowoff, rvalid);
       if (P.debug == 3) continue;           // micro-benchmark: no epilogue work at all
       wg_bar(wg);                             // the previous tile's staged rows have been read
       acc_to_stage<BN>(d, stg + wg * 64 * RS, wq, lane);
@@ -724,6 +783,103 @@ k_tc_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
                             half);
     }
     if (!AFF && stats != nullptr && st_tn >= 0) flush_stats(st_tn);
+  }
+}
+
+// ---------------------------------------------------------------------------------
+// fp8 inference fprop: e4m3 operands, fp32 accumulation, the affine epilogue on a folded table
+// ---------------------------------------------------------------------------------
+// The pipeline of k_tc_conv (producer warp, mbarrier ring, persistent tiles, coalesced epilogue) with e4m3 tiles.  A
+// k-block is one row of KB bytes = KB channels per pixel: KB = 128 keeps bf16's stage layout, 128B swizzle and 32-byte
+// instruction step (four m64nBNk32 per stage); KB = 64 (the Cin = 64 convs) uses 64B-swizzled rows, two instructions
+// per stage and twice the stages in the same shared memory.
+static constexpr int f8_stages(int BN, int KB) { return KB == 128 ? conv_stages(BN) : 2 * conv_stages(BN); }
+static constexpr size_t f8_smem_bytes(int BN, int KB) {
+  return (size_t)f8_stages(BN, KB) * (128 * KB + BN * KB) + (size_t)128 * (BN + 4) * 4 + 1024;
+}
+
+// launch-uniform dispatch over the variants the fp8 schedule uses (EpiF8::mode)
+template <int BN>
+__device__ __forceinline__ void f8_epi_dispatch(const int mode, const float* __restrict__ rows, float (*stw)[BN / 32][32],
+                                                const long long (&rowoff)[4], const bool (&rvalid)[4], const int tn,
+                                                const void* residual, void* out, const EpiF8Dev& E, const int lane,
+                                                const int half) {
+#define MN_F8_CASE(Fv) case (Fv): epi_tile<(Fv), BN>(rows, stw, rowoff, rvalid, true, tn, (const bf16*)residual, (bf16*)out, E, lane, half); break;
+  switch (mode) {
+    MN_F8_CASE(EPI_AFFINE | EPI_RELU | EPI_F8OUT)                         // conv1
+    MN_F8_CASE(EPI_AFFINE)                                                // downsample: bf16 out
+    MN_F8_CASE(EPI_AFFINE | EPI_RES | EPI_RELU | EPI_F8OUT)               // conv2 after a downsample (bf16 residual)
+    MN_F8_CASE(EPI_AFFINE | EPI_RES | EPI_F8RES | EPI_RELU | EPI_F8OUT)   // conv2, identity (e4m3 residual)
+    MN_F8_CASE(EPI_AFFINE | EPI_RELU | EPI_AMAX)                          // calibration of the three above
+    MN_F8_CASE(EPI_AFFINE | EPI_RES | EPI_RELU | EPI_AMAX)
+    MN_F8_CASE(EPI_AFFINE | EPI_RES | EPI_F8RES | EPI_RELU | EPI_AMAX)
+    default: __trap();
+  }
+#undef MN_F8_CASE
+}
+
+template <int BN, int KB>
+__global__ void __launch_bounds__(kConvThreads, 1)
+k_f8_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
+          const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapA3,
+          const __grid_constant__ CUtensorMap mapB, const __grid_constant__ ConvParams P, const void* __restrict__ residual,
+          void* __restrict__ out, const EpiF8Dev E) {
+  static_assert(KB == 128 || KB == 64, "e4m3 k-blocks are 128- or 64-byte rows");
+  constexpr int STAGES = f8_stages(BN, KB);
+  constexpr uint32_t A_BYTES = 128 * KB;         // 128 pixels x KB channels
+  constexpr uint32_t B_BYTES = BN * KB;
+  constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
+  constexpr int RS = BN + 4;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = __shfl_sync(0xffffffffu, (smem_u32(smem_raw) + 1023u) & ~1023u, 0);
+  __shared__ __align__(8) uint64_t bars[2 * STAGES];
+  const uint32_t full0 = __shfl_sync(0xffffffffu, smem_u32(&bars[0]), 0), empty0 = smem_u32(&bars[STAGES]);
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  if (warp == kProducerWarp && lane == 0) {
+    prefetch_tmap(&mapA0); prefetch_tmap(&mapB);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(full0 + 8 * i, 1); mbar_init(empty0 + 8 * i, 2); }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_prologue();
+  const int per_class = P.n_tiles_m * P.n_tiles_n;
+  const int total_tiles = per_class * P.n_classes;
+  if (warp == kProducerWarp) {
+    if (elect_one())
+      conv_producer<STAGES, A_BYTES, STAGE_BYTES, BN, KB>(P, &mapA0, &mapA1, &mapA2, &mapA3, &mapB, &mapB, smem_base, full0,
+                                                         empty0, blockIdx.x, total_tiles, gridDim.x, per_class);
+    return;
+  }
+  const int wg = warp >> 2, wq = warp & 3;
+  const int q = 2 * wg + (wq >> 1), half = wq & 1;
+  const bool arriver = (threadIdx.x & 127) == 0;
+  float* stg = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)) + STAGES * STAGE_BYTES);
+  constexpr uint64_t DESC_BASE = KB == 128 ? make_smem_desc_base(16, 1024) : make_smem_desc_base_sw64(16, 512);
+  // EPI_AMAX: per-warp running max |f| of each (chunk, lane), as the training kernels keep their column sums
+  __shared__ float epi_amax[4][3][BN / 32][32];
+  float (*stw)[BN / 32][32] = epi_amax[q];
+  for (int i = half; i < BN / 32; i += kEpiSplit) stw[0][i][lane] = 0.f;
+  int stage = 0; uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const TileCoord tc = decode_tile(tile, per_class, P.n_tiles_n);
+    const ClassDesc cd = P.cls[tc.cls];
+    float d[BN / 2];
+    mma_tile<BN, 2, 0, 0, KB / 32>(d, cd.num_taps * P.cblocks, stage, phase, STAGES, STAGE_BYTES, smem_base, wg * 64 * KB,
+                                   32, A_BYTES, 32, DESC_BASE, DESC_BASE, full0, empty0, arriver, false);
+    long long rowoff[4]; bool rvalid[4];
+    tile_rows(P, cd, tc.tm, q, lane, tc.tn * BN, rowoff, rvalid);
+    wg_bar(wg);
+    acc_to_stage<BN>(d, stg + wg * 64 * RS, wq, lane);
+    wg_bar(wg);
+    f8_epi_dispatch<BN>(E.aflags, stg + q * 32 * RS, stw, rowoff, rvalid, tc.tn, residual, out, E, lane, half);
+  }
+  if (E.aflags & EPI_AMAX) {        // the bit patterns of non-negative floats order as the floats do
+    float m = 0.f;
+    for (int i = half; i < BN / 32; i += kEpiSplit) m = fmaxf(m, stw[0][i][lane]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if (lane == 0) atomicMax(E.amax, __float_as_uint(m));
   }
 }
 
@@ -928,6 +1084,7 @@ struct TcConvPlan {
   bool smem_attr_aff;                   // ... for the inference (EPI_AFFINE) instantiation of the fprop kernel
   const float* out_scale;              // strict mode dgrad / wgrad: device scalar applied to the accumulators, or null
   float* ws;                            // wgrad with split-K: per-split dW slices (allocated at the first run)
+  int f8_kb;                            // fp8 fprop plan (tc_plan_create_f8): bytes per k-block row, 128 or 64; else 0
 };
 
 static void pick_box(int Wd, int Hd, int pixels, int* TW, int* TH, int* TN) {
@@ -1001,6 +1158,7 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
   TcConvPlan* p = new TcConvPlan();
   p->g = g; p->kind = kind; p->wmat = wmat; p->wmat2 = nullptr; p->shortcut_flops_k = 0;
   p->c_in0 = p->c_in1 = nullptr; p->smem_attr_set = false; p->smem_attr_aff = false; p->out_scale = nullptr; p->ws = nullptr;
+  p->f8_kb = 0;
   const int s = g.stride, pad = g.pad, KK = g.KH * g.KW;
   // strict mode: the engines see 2*C 16-bit channels per pixel and every filter tap twice (hi / lo weight planes)
   const int SP = g.split ? 2 : 1;
@@ -1253,6 +1411,80 @@ static int encode_view(CUtensorMap* m, const bf16* base, int N, int Hd, int Wd, 
   const int Hq = cdiv(Hd - a, 2), Wq = cdiv(Wd - b, 2);
   const bf16* vb = base + ((long long)a * Wd + b) * C;
   return encode_act_map(m, vb, C, Wq > 0 ? Wq : 1, Hq > 0 ? Hq : 1, N, (long long)C * 4, rowb * 2, imgb, bw, bh, bn);
+}
+
+// fp8 fprop plan: the bf16 fprop plan's tiles and taps with e4m3 k-blocks (128 channels, or 64 when Ci = 64)
+int tc_plan_create_f8(TcConvPlan** out, const ConvGeom& g, const uint8_t* wmat) {
+  *out = nullptr;
+  MN_CHECK(!g.split && g.in_pix_stride == 0 && g.KH == g.KW && (g.KH == 1 || g.KH == 3),
+           "tc fp8 conv: dense 1x1 / 3x3 convs only");
+  MN_CHECK(g.Ci % 64 == 0 && (g.Ci == 64 || g.Ci % 128 == 0), "tc fp8 conv: Ci must be 64 or a multiple of 128 (got %d)", g.Ci);
+  MN_TRY(tc_plan_create(out, g, 0, (const bf16*)wmat));
+  TcConvPlan* p = *out;
+  ConvParams& P = p->launches[0].P;
+  p->f8_kb = (g.Ci % 128 == 0) ? 128 : 64;
+  P.cblocks = g.Ci / p->f8_kb;
+  P.Cs = g.Ci;
+  P.fmt_a = P.fmt_b = 2;
+  p->BN = choose_bn(g.Co, g.M_out(), g.KH * g.KW * P.cblocks);
+  P.n_tiles_n = g.Co / p->BN;
+  return 0;
+}
+
+int tc_conv_run_f8(TcConvPlan* p, const uint8_t* in, const void* residual, void* out, const EpiF8& e, cudaStream_t st) {
+  MN_CHECK(p != nullptr && p->f8_kb != 0, "tc_conv_run_f8: not an fp8 plan");
+  MN_CHECK(e.scale != nullptr && e.shift != nullptr, "tc_conv_run_f8: null scale / shift table");
+  const bool res = residual != nullptr;
+  int mode = EPI_AFFINE | (res ? EPI_RES : 0) | (e.relu ? EPI_RELU : 0) | ((res && e.res_f8) ? EPI_F8RES : 0);
+  mode |= e.amax != nullptr ? EPI_AMAX : (e.out_f8 ? EPI_F8OUT : 0);
+  static const int built[] = {
+      EPI_AFFINE | EPI_RELU | EPI_F8OUT, EPI_AFFINE, EPI_AFFINE | EPI_RES | EPI_RELU | EPI_F8OUT,
+      EPI_AFFINE | EPI_RES | EPI_F8RES | EPI_RELU | EPI_F8OUT, EPI_AFFINE | EPI_RELU | EPI_AMAX,
+      EPI_AFFINE | EPI_RES | EPI_RELU | EPI_AMAX, EPI_AFFINE | EPI_RES | EPI_F8RES | EPI_RELU | EPI_AMAX};
+  bool ok = false;
+  for (int b : built) ok = ok || b == mode;
+  MN_CHECK(ok, "tc_conv_run_f8: epilogue variant not built (residual %d relu %d res_f8 %d out_f8 %d amax %d)", res, e.relu,
+           e.res_f8, e.out_f8, e.amax != nullptr);
+  MN_CHECK(!(mode & EPI_F8RES) || e.res_scale != nullptr, "tc_conv_run_f8: an e4m3 residual needs its scale");
+  MN_CHECK(!(mode & EPI_F8OUT) || e.out_inv != nullptr, "tc_conv_run_f8: an e4m3 output needs 1 / its scale");
+  MN_CHECK(out != nullptr || (mode & EPI_AMAX), "tc_conv_run_f8: null output");
+  const ConvGeom& g = p->g;
+  ConvLaunch& L = p->launches[0];
+  const int kb = p->f8_kb;
+  const CUtensorMapSwizzle swz = kb == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+  if (p->c_in0 != in) {
+    const long long rowb = (long long)g.Wi * g.Ci, imgb = (long long)g.Hi * rowb;
+    for (int i = 0; i < L.n_maps; ++i) {
+      if (g.stride == 1) {
+        MN_TRY(encode_act_map(&L.mapA[i], in, g.Ci, g.Wi, g.Hi, g.B, g.Ci, rowb, imgb, L.P.TW, L.P.TH, L.P.TN,
+                              CU_TENSOR_MAP_DATA_TYPE_UINT8, kb, swz));
+      } else {       // stride-2 parity view (a, b), as encode_view builds it for bf16
+        const int a = L.pa[i], b = L.pb[i];
+        const int Hq = cdiv(g.Hi - a, 2), Wq = cdiv(g.Wi - b, 2);
+        MN_TRY(encode_act_map(&L.mapA[i], in + ((long long)a * g.Wi + b) * g.Ci, g.Ci, Wq > 0 ? Wq : 1, Hq > 0 ? Hq : 1,
+                              g.B, 2LL * g.Ci, 2 * rowb, imgb, L.P.TW, L.P.TH, L.P.TN, CU_TENSOR_MAP_DATA_TYPE_UINT8, kb, swz));
+      }
+    }
+    for (int i = L.n_maps; i < 4; ++i) L.mapA[i] = L.mapA[0];
+    MN_TRY(encode_w_map(&L.mapB, p->wmat, g.KH * g.KW * g.Ci, g.Co, p->BN, CU_TENSOR_MAP_DATA_TYPE_UINT8, kb, swz));
+    p->c_in0 = in;
+  }
+  EpiF8Dev E; memset(&E, 0, sizeof(E));
+  E.ascale = e.scale; E.ashift = e.shift; E.aflags = mode;
+  E.res_scale = e.res_scale; E.out_inv = e.out_inv; E.amax = e.amax;
+  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, ConvParams, const void*, void*, EpiF8Dev) =
+      (kb == 128) ? ((p->BN == 64) ? k_f8_conv<64, 128> : k_f8_conv<128, 128>)
+                  : ((p->BN == 64) ? k_f8_conv<64, 64> : k_f8_conv<128, 64>);
+  const size_t smem = (kb == 128) ? f8_smem_bytes(p->BN, 128) : f8_smem_bytes(p->BN, 64);
+  if (!p->smem_attr_set) {
+    MN_TRY(set_smem(kern, smem));
+    p->smem_attr_set = true;
+  }
+  const int items = L.P.n_tiles_m * L.P.n_tiles_n;
+  MN_LAUNCH(kern, items < kNumSMs ? items : kNumSMs, kConvThreads, smem, st, L.mapA[0], L.mapA[1], L.mapA[2], L.mapA[3],
+            L.mapB, L.P, residual, out, E);
+  MN_LAUNCH_CHECK();
+  return 0;
 }
 
 int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* residual, void* out, cudaStream_t st,

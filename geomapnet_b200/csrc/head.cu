@@ -13,7 +13,8 @@ namespace mapnet {
 // loads across cv), the npg partial sums meet in shared memory.  (The first version -- one thread per (image, 8 channels),
 // 32 blocks in all -- took 20 us for 4 MB: ncu r02a, 2.5 % of DRAM peak.)
 template <typename T>
-__global__ void __launch_bounds__(256) k_gap(const T* __restrict__ z, float* __restrict__ feat, int B, int HW, int C) {
+__global__ void __launch_bounds__(256) k_gap(const T* __restrict__ z, float* __restrict__ feat, int B, int HW, int C,
+                                             const float* __restrict__ scale) {
   pdl_prologue();
   extern __shared__ float sm[];          // [npg][C]
   const int cv = C >> 3, npg = blockDim.x / cv;
@@ -34,23 +35,25 @@ __global__ void __launch_bounds__(256) k_gap(const T* __restrict__ z, float* __r
   }
   __syncthreads();
   const float inv = 1.0f / (float)HW;
+  const float sc = (scale != nullptr) ? __ldg(scale) : 1.f;     // e4m3 input: the tensor's scale (a power of two)
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float s = 0.f;
     for (int g = 0; g < npg; ++g) s += sm[g * C + c];
-    feat[(long long)b * C + c] = s * inv;
+    feat[(long long)b * C + c] = s * inv * sc;
   }
 }
 template <typename T>
-int launch_gap(const T* z, float* feat, int B, int HW, int C, cudaStream_t st) {
+int launch_gap(const T* z, float* feat, int B, int HW, int C, cudaStream_t st, const float* scale) {
   MN_CHECK(C % 8 == 0 && (C >> 3) <= 256, "gap: unsupported channel count %d", C);
   const int npg = 256 / (C >> 3);
-  MN_LAUNCH(k_gap<T>, B, 256, (size_t)npg * C * sizeof(float), st, z, feat, B, HW, C);
+  MN_LAUNCH(k_gap<T>, B, 256, (size_t)npg * C * sizeof(float), st, z, feat, B, HW, C, scale);
   MN_LAUNCH_CHECK();
   return 0;
 }
-template int launch_gap<float>(const float*, float*, int, int, int, cudaStream_t);
-template int launch_gap<bf16>(const bf16*, float*, int, int, int, cudaStream_t);
-template int launch_gap<hsplit>(const hsplit*, float*, int, int, int, cudaStream_t);
+template int launch_gap<float>(const float*, float*, int, int, int, cudaStream_t, const float*);
+template int launch_gap<bf16>(const bf16*, float*, int, int, int, cudaStream_t, const float*);
+template int launch_gap<hsplit>(const hsplit*, float*, int, int, int, cudaStream_t, const float*);
+template int launch_gap<e4m3>(const e4m3*, float*, int, int, int, cudaStream_t, const float*);
 
 template <typename T>
 __global__ void k_gap_bwd(const float* __restrict__ dfeat, T* __restrict__ dz, int B, int HW, int C) {

@@ -9,7 +9,17 @@
 // The schedule shares Net's parameter table and layer geometry (a spec-only Net, max_B = 0) and owns its resources:
 // the packed fprop operands, a per-channel scale / shift table computed by the same k_bn_eval_scale the live eval
 // forward runs, an fp32 copy of the head and an activation arena that holds only the live set of one block.
+//
+// fp8 (PREC_FP8): the stem conv stays on the bf16 engine; the pool output and every block's h and output are e4m3, each
+// with one power-of-two scale, and every other conv runs k_f8_conv on e4m3 weights with a power-of-two scale per output
+// channel.  Its epilogue applies S[c] = bn_scale[c] * s_in * s_w[c] (exact: powers of two), adds the residual (e4m3 *
+// s_res, or the bf16 downsample output), applies the ReLU and stores e4m3(f / s_out).  The activation scales come from
+// calibration over the engine's own schedule (calibrate): each tensor's scale is taken from the values its epilogue
+// would quantize with every earlier tensor already quantized, so a CPU emulation with the same scales reproduces the
+// engine's rounding points.
 #include "infer.h"
+
+#include <math.h>
 
 #include <string.h>
 
@@ -24,9 +34,39 @@ int InferNet::alloc(void** p, size_t bytes) {
   return 0;
 }
 
-int InferNet::sizes(const Net& n, Sizes* s) {
+// ---- fp8 calibration kernels (one launch each per tensor, at calibration time only) ----
+// max |y| of a bf16 tensor into *amax (bit pattern): the stem output, whose max is the pool output's (every stem pixel
+// lies in some pooling window, and max pooling keeps the largest value)
+__global__ void k_f8_amax_bf16(const bf16* __restrict__ y, long long n8, unsigned int* __restrict__ amax) {
+  pdl_prologue();
+  float m = 0.f;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
+    Vec8<bf16> v; v.load(y + 8 * i);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) m = fmaxf(m, fabsf(v.v[k]));
+  }
+  m = warp_max(m);
+  if ((threadIdx.x & 31) == 0) atomicMax(amax, __float_as_uint(m));
+}
+// tensor t's scale from its amax: slots[n + t] = s, slots[2n + t] = 1 / s; fill[0..nfill) = 1 / s (the pool's map)
+__global__ void k_f8_set_scale(float* __restrict__ slots, int n, int t, float* __restrict__ fill, int nfill) {
+  pdl_prologue();
+  const float s = f8_pow2_scale(__uint_as_float(reinterpret_cast<const unsigned int*>(slots)[t]));
+  if (threadIdx.x == 0) { slots[n + t] = s; slots[2 * n + t] = 1.f / s; }
+  for (int i = threadIdx.x; i < nfill; i += blockDim.x) fill[i] = 1.f / s;
+}
+// the epilogue table of one conv: S[c] = bn_scale[c] * s_in * s_w[c] (two power-of-two factors: exact)
+__global__ void k_f8_fold(const float* __restrict__ bn_scale, const float* __restrict__ s_w, const float* __restrict__ s_in,
+                          float* __restrict__ S, int C) {
+  pdl_prologue();
+  for (int c = threadIdx.x; c < C; c += blockDim.x) S[c] = bn_scale[c] * __ldg(s_in) * s_w[c];
+}
+
+int InferNet::sizes(const Net& n, int precision, Sizes* s) {
+  const bool f8 = precision == PREC_FP8;
   const long long ez = (n.precision == PREC_TC_SPLIT) ? 4 : 2;       // operand element (bf16 / hi+lo fp16 planes)
   const long long ea = (n.precision == PREC_TC_SPLIT) ? 4 : 2;       // conv output element (bf16 / fp32)
+  const long long eb = f8 ? 1 : ez;                                   // block tensors (fp8: e4m3)
   const ConvGeom& g0 = n.convs[0].g;
   s->a0 = n.stem_s2d ? (long long)g0.Hi * stem_s2d_wsp(n.Wc) * 16 * ez : (long long)n.Hc * n.Wc * g0.Ci * ez;
   s->y0 = (long long)n.Hc * n.Wc * 64 * ea;
@@ -36,41 +76,45 @@ int InferNet::sizes(const Net& n, Sizes* s) {
     if (e > act) act = e;
     if (b.convd >= 0 && e > ds) ds = e;
   }
-  s->act = act * ez;
+  s->act = act * eb;
   s->ds = ds * ea;
   s->head = (512 + 3LL * n.feat_dim) * 4;     // feat, fc output (pre-ReLU and dropped), dropout mask
   return 0;
 }
 
 long long InferNet::arena_bytes(int max_B, int H, int W, int precision) {
-  if (precision != PREC_BF16_TC && precision != PREC_TC_SPLIT) {
-    set_last_error("infer: precision %d is not supported (bf16 = %d or tc_split = %d)", precision, PREC_BF16_TC,
-                   PREC_TC_SPLIT);
+  if (precision != PREC_BF16_TC && precision != PREC_TC_SPLIT && precision != PREC_FP8) {
+    set_last_error("infer: precision %d is not supported (bf16 = %d, tc_split = %d or fp8 = %d)", precision, PREC_BF16_TC,
+                   PREC_TC_SPLIT, PREC_FP8);
     return -2;
   }
   if (max_B < 1 || H < 32 || W < 32) { set_last_error("infer: need max_B >= 1 and H, W >= 32 (got %d, %d, %d)", max_B, H, W); return -2; }
   Net n = Net();
-  if (n.init(0, H, W, 2048, precision) != 0) return -2;
+  if (n.init(0, H, W, 2048, precision == PREC_FP8 ? PREC_BF16_TC : precision) != 0) return -2;
   Sizes s;
-  sizes(n, &s);
+  sizes(n, precision, &s);
+  const long long slots = precision == PREC_FP8 ? f8_slot_bytes(n) : 0;
   n.destroy();
-  return (long long)max_B * (s.a0 + s.y0 + 3 * s.act + s.ds + s.head);
+  return (long long)max_B * (s.a0 + s.y0 + 3 * s.act + s.ds + s.head) + slots;
 }
 
 int InferNet::init(int max_B_, int H_, int W_, int feat_dim_, int precision_) {
   max_B = max_B_; H = H_; W = W_; feat_dim = feat_dim_; precision = precision_;
-  loaded = false; plan_B = 0;
+  loaded = false; calibrated = false; plan_B = 0;
   wk = nullptr; d_wdescs = nullptr; affine = head = ident = eval_scratch = nullptr;
+  wk8 = nullptr; s_w = f8_table = pool_map = f8_slots = nullptr; n_f8 = 0;
   A0 = y0 = ds = nullptr; act[0] = act[1] = act[2] = nullptr;
   feat = fcpre = hdrop = mask = nullptr; drop_ctr = nullptr;
-  MN_CHECK(precision == PREC_BF16_TC || precision == PREC_TC_SPLIT,
-           "infer_create: precision %d is not supported (bf16 = %d or tc_split = %d)", precision, PREC_BF16_TC, PREC_TC_SPLIT);
+  const bool f8 = precision == PREC_FP8;
+  MN_CHECK(precision == PREC_BF16_TC || precision == PREC_TC_SPLIT || f8,
+           "infer_create: precision %d is not supported (bf16 = %d, tc_split = %d or fp8 = %d)", precision, PREC_BF16_TC,
+           PREC_TC_SPLIT, PREC_FP8);
   MN_CHECK(max_B >= 1 && H >= 32 && W >= 32, "infer_create: need max_B >= 1 and H, W >= 32 (got %d, %d, %d)", max_B, H, W);
-  MN_TRY(spec.init(0, H, W, feat_dim, precision));
+  MN_TRY(spec.init(0, H, W, feat_dim, f8 ? PREC_BF16_TC : precision));     // fp8: the stem's operands are bf16
   MN_CHECK(!spec.stem_s2d || tc_overlapped_view_supported(),
            "infer_create: the driver rejects the overlapped tensor map of the space-to-depth stem");
   Sizes s;
-  sizes(spec, &s);
+  sizes(spec, precision, &s);
   const long long Bm = max_B;
   MN_TRY(alloc(&A0, (size_t)(Bm * s.a0)));
   MN_TRY(alloc(&y0, (size_t)(Bm * s.y0)));
@@ -81,7 +125,20 @@ int InferNet::init(int max_B_, int H_, int W_, int feat_dim_, int precision_) {
   MN_TRY(alloc((void**)&hdrop, (size_t)Bm * feat_dim * 4));
   MN_TRY(alloc((void**)&mask, (size_t)Bm * feat_dim * 4));
   // snapshot storage
-  MN_TRY(alloc(&wk, (size_t)spec.wk_total * (precision == PREC_TC_SPLIT ? 8 : 2)));
+  if (f8) {
+    const int nconv = (int)spec.convs.size();
+    MN_CHECK(spec.convs[0].wd.k_off == 0, "infer_create: the stem's packed weights must come first");
+    MN_TRY(alloc(&wk, (size_t)spec.convs[1].wd.k_off * 2));            // the stem's bf16 operand only
+    MN_TRY(alloc((void**)&wk8, (size_t)spec.wk_total));
+    MN_TRY(alloc((void**)&s_w, (size_t)nconv * 512 * 4));
+    MN_TRY(alloc((void**)&f8_table, (size_t)nconv * 512 * 4));
+    n_f8 = f8_tensors(spec);
+    MN_TRY(alloc((void**)&pool_map, (size_t)f8_slot_bytes(spec)));
+    MN_CUDA(cudaMemset(pool_map, 0, (size_t)f8_slot_bytes(spec)));
+    f8_slots = pool_map + 128;
+  } else {
+    MN_TRY(alloc(&wk, (size_t)spec.wk_total * (precision == PREC_TC_SPLIT ? 8 : 2)));
+  }
   std::vector<WeightDesc> wd;
   for (auto& c : spec.convs) wd.push_back(c.wd);
   MN_TRY(alloc((void**)&d_wdescs, wd.size() * sizeof(WeightDesc)));
@@ -121,7 +178,11 @@ int InferNet::load(const float* params, const float* bufs, cudaStream_t st) {
              "infer_load: params_flat / bufs_flat must be device memory");
   }
   const int nconv = (int)spec.convs.size();
-  if (precision == PREC_BF16_TC) {
+  calibrated = false;          // fp8: the activation scales belong to the previous weights
+  if (precision == PREC_FP8) {
+    MN_TRY(launch_pack_weights<bf16>(d_wdescs, 1, params, (bf16*)wk, nullptr, spec.max_w_elems, 0, st));   // the stem
+    MN_TRY(launch_pack_weights_fp8(d_wdescs, nconv, params, wk8, s_w, st));
+  } else if (precision == PREC_BF16_TC) {
     MN_TRY(launch_pack_weights<bf16>(d_wdescs, nconv, params, (bf16*)wk, nullptr, spec.max_w_elems, 0, st));
   } else {
     float* f32 = nullptr;       // the fp32 K-major matrices the hi / lo planes are cut from (load time only)
@@ -152,6 +213,10 @@ int InferNet::ensure_plans(int B) {
   for (size_t i = 0; i < spec.convs.size(); ++i) {
     ConvGeom g = spec.convs[i].g; g.B = B;
     if (sp) g.split = 1;
+    if (precision == PREC_FP8 && i > 0) {
+      MN_TRY(tc_plan_create_f8(&plans[i], g, wk8 + spec.convs[i].wd.k_off));
+      continue;
+    }
     const bf16* w = (const bf16*)wk + (sp ? 4 : 1) * spec.convs[i].wd.k_off;
     MN_TRY(tc_plan_create(&plans[i], g, 0, w));
   }
@@ -197,9 +262,15 @@ int InferNet::forward_t(const float* x, int B, float droprate, unsigned long lon
     }
     xi = (xi + 2) % 3;
   }
-  // head: exactly the calls of Net::forward_t, on the snapshot's copy of the head parameters
-  const float* hp = head - n.fc_w;      // indexed with the flat-buffer offsets
   MN_TRY(launch_gap<TZ>((const TZ*)act[xi], feat, B, n.Hf * n.Wf, 512, st));
+  return run_head(B, droprate, seed, step, pred, st);
+}
+
+// head on feat: exactly the calls of Net::forward_t, on the snapshot's copy of the head parameters
+int InferNet::run_head(int B, float droprate, unsigned long long seed, unsigned long long step, float* pred,
+                       cudaStream_t st) {
+  const Net& n = spec;
+  const float* hp = head - n.fc_w;      // indexed with the flat-buffer offsets
   const float* mk = nullptr;
   if (droprate > 0.f) {
     const unsigned long long stride = (unsigned long long)max_B * feat_dim;
@@ -217,11 +288,104 @@ int InferNet::forward_t(const float* x, int B, float droprate, unsigned long lon
 int InferNet::forward(const float* x, int B, float droprate, unsigned long long seed, unsigned long long step, float* pred,
                       cudaStream_t st) {
   MN_CHECK(loaded, "infer_forward: no snapshot loaded (call mapnet_infer_load first)");
+  MN_CHECK(precision != PREC_FP8 || calibrated,
+           "infer_forward: the fp8 engine has no activation scales for this snapshot (call mapnet_infer_calibrate)");
   MN_CHECK(B >= 1 && B <= max_B, "infer_forward: batch %d outside [1, max_B=%d]", B, max_B);
   MN_CHECK(x != nullptr && pred != nullptr, "infer_forward: null pointer argument");
   MN_CHECK(droprate >= 0.f && droprate < 1.f, "infer_forward: droprate %f outside [0,1)", droprate);
+  if (precision == PREC_FP8) {
+    int last = 0;
+    MN_TRY(run_f8(x, B, false, &last, st));
+    MN_TRY(launch_gap<e4m3>((const e4m3*)act[last], feat, B, spec.Hf * spec.Wf, 512, st, f8_slots + 2 * n_f8 - 1));
+    return run_head(B, droprate, seed, step, pred, st);
+  }
   if (precision == PREC_TC_SPLIT) return forward_t<TypesSplitHH>(x, B, droprate, seed, step, pred, st);
   return forward_t<TypesBF16>(x, B, droprate, seed, step, pred, st);
+}
+
+// one fp8 conv: t_in / t_res / t_out index the e4m3 tensors' scales (t_res < 0: bf16 residual or none; t_out < 0: bf16
+// output).  Calibrating, the epilogue table is folded with the input's new scale, and an e4m3 output's scale is taken
+// from an amax pass of the same epilogue before the storing pass.
+int InferNet::conv_f8(int ci, const void* in, int t_in, const void* res, int t_res, void* out, int t_out, int relu,
+                      bool calib, cudaStream_t st) {
+  const int bi = spec.convs[ci].bn, C = spec.convs[ci].g.Co;
+  float* S = f8_table + (size_t)ci * 512;
+  float* scale = f8_slots + n_f8;
+  float* inv = f8_slots + 2 * n_f8;
+  EpiF8 e; memset(&e, 0, sizeof(e));
+  e.scale = S; e.shift = bn_shift[bi]; e.relu = relu;
+  e.res_f8 = t_res >= 0; e.res_scale = t_res >= 0 ? scale + t_res : nullptr;
+  e.out_f8 = t_out >= 0; e.out_inv = t_out >= 0 ? inv + t_out : nullptr;
+  if (calib) {
+    MN_LAUNCH(k_f8_fold, 1, 512, 0, st, bn_scale[bi], s_w + (size_t)ci * 512, scale + t_in, S, C);
+    MN_LAUNCH_CHECK();
+    if (t_out >= 0) {
+      EpiF8 a = e;
+      a.amax = reinterpret_cast<unsigned int*>(f8_slots) + t_out;
+      MN_TRY(tc_conv_run_f8(plans[ci], (const uint8_t*)in, res, nullptr, a, st));
+      MN_LAUNCH(k_f8_set_scale, 1, 32, 0, st, f8_slots, n_f8, t_out, (float*)nullptr, 0);
+      MN_LAUNCH_CHECK();
+    }
+  }
+  return tc_conv_run_f8(plans[ci], (const uint8_t*)in, res, out, e, st);
+}
+
+int InferNet::run_f8(const float* x, int B, bool calib, int* last, cudaStream_t st) {
+  const Net& n = spec;
+  MN_TRY(ensure_plans(B));
+  MN_TRY(launch_stem_s2d<bf16>(x, (bf16*)A0, B, H, W, n.convs[0].g.Hi, stem_s2d_wsp(n.Wc), st));
+  MN_TRY(conv(0, A0, nullptr, y0, 1, 0, 0, st));
+  if (calib) {
+    MN_CUDA(cudaMemsetAsync(f8_slots, 0, (size_t)n_f8 * 4, st));
+    const long long n8 = (long long)B * n.Hc * n.Wc * 64 / 8;
+    MN_LAUNCH(k_f8_amax_bf16, (int)(n8 / 256 + 1 < 4 * kNumSMs ? n8 / 256 + 1 : 4 * kNumSMs), 256, 0, st, (const bf16*)y0,
+              n8, reinterpret_cast<unsigned int*>(f8_slots));
+    MN_LAUNCH_CHECK();
+    MN_LAUNCH(k_f8_set_scale, 1, 64, 0, st, f8_slots, n_f8, 0, pool_map, 64);
+    MN_LAUNCH_CHECK();
+  }
+  BnDesc id; memset(&id, 0, sizeof(id));
+  id.f.scale = pool_map; id.f.shift = pool_map + 64;
+  MN_TRY((launch_stem_pool<bf16, e4m3>((const bf16*)y0, (e4m3*)act[0], nullptr, B, n.Hc, n.Wc, n.Hp, n.Wp, 64, id, st)));
+  int xi = 0, t_in = 0;
+  for (size_t b = 0; b < n.blocks.size(); ++b) {
+    const BlockL& bl = n.blocks[b];
+    void* xin = act[xi];
+    void* h = act[(xi + 1) % 3];
+    void* out = act[(xi + 2) % 3];
+    const int t_h = 1 + 2 * (int)b, t_out = 2 + 2 * (int)b;
+    MN_TRY(conv_f8(bl.conv1, xin, t_in, nullptr, -1, h, t_h, 1, calib, st));
+    if (bl.convd >= 0) {
+      MN_TRY(conv_f8(bl.convd, xin, t_in, nullptr, -1, ds, -1, 0, calib, st));
+      MN_TRY(conv_f8(bl.conv2, h, t_h, ds, -1, out, t_out, 1, calib, st));
+    } else {
+      MN_TRY(conv_f8(bl.conv2, h, t_h, xin, t_in, out, t_out, 1, calib, st));
+    }
+    xi = (xi + 2) % 3;
+    t_in = t_out;
+  }
+  *last = xi;
+  return 0;
+}
+
+int InferNet::calibrate(const float* x, int B, cudaStream_t st) {
+  MN_CHECK(precision == PREC_FP8, "infer_calibrate: only the fp8 engine has activation scales (precision %d)", precision);
+  MN_CHECK(loaded, "infer_calibrate: no snapshot loaded (call mapnet_infer_load first)");
+  MN_CHECK(B >= 1 && B <= max_B, "infer_calibrate: %d calibration frames outside [1, max_B=%d]", B, max_B);
+  MN_CHECK(x != nullptr, "infer_calibrate: null pointer argument");
+  int last = 0;
+  MN_TRY(run_f8(x, B, true, &last, st));
+  calibrated = true;
+  return 0;
+}
+
+int InferNet::act_scales(float* host, int cap, cudaStream_t st) {
+  MN_CHECK(precision == PREC_FP8, "infer_act_scales: only the fp8 engine has activation scales (precision %d)", precision);
+  MN_CHECK(calibrated, "infer_act_scales: not calibrated");
+  MN_CHECK(host != nullptr && cap >= n_f8, "infer_act_scales: need room for %d scales", n_f8);
+  MN_CUDA(cudaMemcpyAsync(host, f8_slots + n_f8, (size_t)n_f8 * 4, cudaMemcpyDeviceToHost, st));
+  MN_CUDA(cudaStreamSynchronize(st));
+  return n_f8;
 }
 
 }  // namespace mapnet

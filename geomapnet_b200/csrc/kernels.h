@@ -106,6 +106,23 @@ struct EpiAffine {
 bool tc_affine_supported(bool split, bool residual, const EpiAffine& a);
 int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* residual, void* out, cudaStream_t st,
                 double* stats = nullptr, const EpiBwd* bwd = nullptr, const EpiAffine* aff = nullptr);
+// ---- fp8 inference fprop (k_f8_conv): e4m3 NHWC input, e4m3 K-major weights [Co][KH][KW][Ci], fp32 accumulation.
+//   f = acc * scale[c] + shift[c]  (scale = bn_scale * s_in * s_w[c], folded by the caller: powers of two, exact)
+//   (+ residual: e4m3 r * *res_scale when res_f8, else bf16) (ReLU), then
+//   out_f8: store e4m3(f * *out_inv) (satfinite), else bf16(f);  amax != nullptr: atomicMax of max |f| (bit pattern of a
+//   non-negative float) and no store at all -- the calibration pass of the same conv.
+// The scalars are read from device memory, so captured graphs stay valid when calibration rewrites them.
+struct EpiF8 {
+  const float* scale;
+  const float* shift;
+  const float* res_scale;
+  const float* out_inv;
+  unsigned int* amax;
+  int relu, res_f8, out_f8;
+};
+// fprop plan over e4m3 operands (1x1 / 3x3, Ci = 64 or a multiple of 128); wmat = e4m3 [Co][KH][KW][Ci]
+int tc_plan_create_f8(TcConvPlan** out, const ConvGeom& g, const uint8_t* wmat);
+int tc_conv_run_f8(TcConvPlan* p, const uint8_t* in, const void* residual, void* out, const EpiF8& e, cudaStream_t st);
 // finalize of backward reductions accumulated in `accum` (the stem's pool backward in the CUDA-core modes): d gamma,
 // d beta and the dy = A*g + B*y + C coefficients
 int launch_bn_bwd_finalize_accum(long long M, int C, const BnFin& f, double* accum, cudaStream_t st);
@@ -129,6 +146,10 @@ int launch_pack_weights(const WeightDesc* d_descs, int nconv, const float* param
 int launch_pack_weights_split(const WeightDesc* d_descs, int nconv, const float* params, float* w_krsc_f32, float* w_dg_f32,
                               void* w_krsc2, void* w_dg2, int max_elems, cudaStream_t st);
 int launch_split_tensor(const float* in, void* out, long long n, cudaStream_t st);
+// fp8 inference: per output channel co of every conv, s_w = 2^ceil(log2(amax_co / 448)) (1 when amax_co = 0) into
+// s_w[i * 512 + co] and e4m3(w / s_w) into w8 + k_off (the descriptors' non-stem convs; K-major params only)
+int launch_pack_weights_fp8(const WeightDesc* d_descs, int nconv, const float* params, uint8_t* w8, float* s_w,
+                            cudaStream_t st);
 int launch_split_weight_matrix(const float* w, void* out, long long rows, int KK, int C, cudaStream_t st);
 int launch_unpack_wgrads(const WeightDesc* d_descs, int nconv, const float* dw_krsc, float* grads,
                          int max_elems, cudaStream_t st);
@@ -143,8 +164,9 @@ template <typename T>
 int launch_stem_im2col(const float* x_nchw, T* A, int B, int H, int W, int Ho, int Wo, int Kpad, cudaStream_t st);
 
 // ---- head.cu -------------------------------------------------------------------
+// scale (device scalar, may be null): multiplies the mean -- the power-of-two scale of an e4m3 tensor
 template <typename T>
-int launch_gap(const T* z, float* feat, int B, int HW, int C, cudaStream_t st);
+int launch_gap(const T* z, float* feat, int B, int HW, int C, cudaStream_t st, const float* scale = nullptr);
 template <typename T>
 int launch_gap_bwd(const float* dfeat, T* dz, int B, int HW, int C, cudaStream_t st);
 // dst[i] += part[i] + part[n + i] + ... + part[(splits - 1) * n + i], summed in that order (n % 4 == 0): the

@@ -114,6 +114,39 @@ int launch_pack_weights(const WeightDesc* d_descs, int nconv, const float* param
   }
   return 0;
 }
+// fp8 inference: one block per (output channel, conv).  The row's amax is an order-independent max, and
+// s_w = 2^ceil(log2(amax / 448)) is taken from the exponent (f8_pow2_scale), so the packed weights are exactly reproducible.
+__global__ void __launch_bounds__(256)
+k_pack_weights_fp8(const WeightDesc* __restrict__ descs, const float* __restrict__ params, uint8_t* __restrict__ w8,
+                   float* __restrict__ s_w) {
+  pdl_prologue();
+  const WeightDesc d = descs[blockIdx.y];
+  const int co = blockIdx.x;
+  if (d.im2col_k > 0 || co >= d.Co) return;         // the stem stays bf16
+  const int n = d.KH * d.KW * d.Ci;
+  const float* src = params + d.p_off + (long long)co * n;
+  float m = 0.f;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(src[i]));
+  __shared__ float red[8];
+  m = warp_max(m);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = red[0];
+  for (int w = 1; w < 8; ++w) m = fmaxf(m, red[w]);
+  const float s = f8_pow2_scale(m), inv = 1.f / s;
+  if (threadIdx.x == 0) s_w[blockIdx.y * 512 + co] = s;
+  uint8_t* dst = w8 + d.k_off + (long long)co * n;
+  for (int i = threadIdx.x; 2 * i < n; i += blockDim.x)
+    *reinterpret_cast<uint16_t*>(dst + 2 * i) = f8x2_pack(src[2 * i] * inv, src[2 * i + 1] * inv);
+}
+
+int launch_pack_weights_fp8(const WeightDesc* d_descs, int nconv, const float* params, uint8_t* w8, float* s_w,
+                            cudaStream_t st) {
+  MN_LAUNCH(k_pack_weights_fp8, dim3(512, nconv), 256, 0, st, d_descs, params, w8, s_w);
+  MN_LAUNCH_CHECK();
+  return 0;
+}
+
 template int launch_pack_weights<float>(const WeightDesc*, int, const float*, float*, float*, int, int, cudaStream_t);
 template int launch_pack_weights<bf16>(const WeightDesc*, int, const float*, bf16*, bf16*, int, int, cudaStream_t);
 

@@ -12,7 +12,8 @@ namespace mapnet {
 
 // PREC_TC_SPLIT: strict tensor-core mode -- fp32-stored conv outputs, conv operands as split fp16 hi/lo planes (22
 // significant bits), every product formed by 4 wgmma MMAs (hi*hi + hi*lo + lo*hi + lo*lo), fp32 accumulation
-enum Precision { PREC_FP32 = 0, PREC_BF16_TC = 1, PREC_BF16_SIMT = 2, PREC_TC_SPLIT = 3 };
+// PREC_FP8: the inference engine only (infer.cu): e4m3 conv operands, calibrated power-of-two scales
+enum Precision { PREC_FP32 = 0, PREC_BF16_TC = 1, PREC_BF16_SIMT = 2, PREC_TC_SPLIT = 3, PREC_FP8 = 4 };
 
 struct ParamEntry {
   std::string name;

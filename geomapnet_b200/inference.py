@@ -34,21 +34,45 @@ class Predictor(object):
     Training the model afterwards does not change the predictor's output until ``refresh()``.  Precision, droprate and
     seed follow the model ('bf16' or 'tc_split' only).  Every distinct (B, H, W) is captured into a CUDA graph on its first
     call and replayed after that.  With droprate > 0 the masks follow the engine's own step counter (as the model's
-    dropout, the reference's F.dropout is active at eval)."""
+    dropout, the reference's F.dropout is active at eval).
 
-    def __init__(self, model, max_batch=64):
+    ``precision='fp8'`` (for a 'bf16' or 'tc_split' model) runs every conv but the stem on e4m3 operands: the weights get
+    a power-of-two scale per output channel, every activation tensor one power-of-two scale taken from ``calibration``
+    frames ([L,3,H,W] or [L,T,3,H,W] on the GPU, L*T <= max_batch).  The engine is fixed to the calibration frames' (H, W);
+    ``refresh()`` re-packs the weights and re-calibrates on a device copy of the frames, in place.  ``act_scales`` lists
+    the scales (pool output, then each block's h and output)."""
+
+    def __init__(self, model, max_batch=64, precision=None, calibration=None):
         net = model.mapnet if hasattr(model, "mapnet") else model
         if net.precision not in ("bf16", "tc_split"):
             raise ValueError("Predictor supports the precisions 'bf16' and 'tc_split' (the model uses %r)" % net.precision)
         if int(max_batch) < 1:
             raise ValueError("max_batch must be >= 1")
+        if precision not in (None, "fp8"):
+            raise ValueError("Predictor precision must be None (the model's) or 'fp8', got %r" % (precision,))
         self.model, self.net, self.max_batch = model, net, int(max_batch)
-        self.precision, self.droprate, self.seed = net.precision, float(net.droprate), net._seed
+        self.precision, self.droprate, self.seed = precision or net.precision, float(net.droprate), net._seed
         self.device = torch.device("cuda", torch.cuda.current_device())
+        self._calib = None      # fp8: device copy of the calibration frames [N,3,H,W]
+        if self.precision == "fp8":
+            if calibration is None:
+                raise ValueError("precision='fp8' needs calibration frames ([L,3,H,W] or [L,T,3,H,W] on the GPU)")
+            c = calibration
+            if not c.is_cuda or c.dim() not in (4, 5) or c.shape[-3] != 3:
+                raise ValueError("calibration must be a CUDA tensor [L,3,H,W] or [L,T,3,H,W], got %s on %s"
+                                 % (tuple(c.shape), c.device))
+            frames = c.reshape(-1, *c.shape[-3:])
+            if not 1 <= frames.shape[0] <= self.max_batch:
+                raise ValueError("%d calibration frames: need 1 .. max_batch=%d" % (frames.shape[0], self.max_batch))
+            self._calib = frames.detach().to(self.device, torch.float32).contiguous().clone()
+        elif calibration is not None:
+            raise ValueError("calibration frames are only used with precision='fp8'")
         self._engines = {}      # (H, W) -> _lib.Infer
         self._graphs = {}       # (B, H, W) -> (CUDAGraph, static input, static output)
         self._params = self._bufs = None
         self.refresh()
+        if self._calib is not None:
+            self._engine(*self._calib.shape[-2:])
 
     def refresh(self):
         """Snapshot the model's current parameters and running statistics into every engine of this predictor."""
@@ -61,7 +85,16 @@ class Predictor(object):
         with torch.cuda.device(self.device):
             for eng in self._engines.values():
                 eng.load(self._params, self._bufs)      # in place: the captured graphs read the engines' own buffers
+                if self._calib is not None:
+                    eng.calibrate(self._calib)
         torch.cuda.current_stream(self.device).synchronize()
+
+    @property
+    def act_scales(self):
+        """fp8: the 33 activation scales of the current snapshot, in schedule order"""
+        if self._calib is None:
+            raise RuntimeError("act_scales: only an fp8 Predictor has activation scales")
+        return self._engine(*self._calib.shape[-2:]).act_scales()
 
     def _engine(self, H, W):
         eng = self._engines.get((H, W))
@@ -69,6 +102,8 @@ class Predictor(object):
             with torch.cuda.device(self.device):
                 eng = _lib.Infer(self.max_batch, H, W, self.net.feat_dim, self.precision)
                 eng.load(self._params, self._bufs)
+                if self._calib is not None:
+                    eng.calibrate(self._calib)
             self._engines[(H, W)] = eng
         return eng
 
@@ -108,6 +143,9 @@ class Predictor(object):
             raise ValueError("empty batch")
         if self._params is None:
             raise RuntimeError("Predictor is closed")
+        if self._calib is not None and tuple(x.shape[-2:]) != tuple(self._calib.shape[-2:]):
+            raise ValueError("this fp8 Predictor was calibrated at %dx%d, got frames of %dx%d"
+                             % (self._calib.shape[-2], self._calib.shape[-1], x.shape[-2], x.shape[-1]))
         frames = x.reshape(-1, *x.shape[-3:])
         if frames.dtype != torch.float32:
             frames = frames.float()
@@ -121,7 +159,7 @@ class Predictor(object):
         for eng in self._engines.values():
             eng.close()
         self._engines.clear()
-        self._params = self._bufs = None
+        self._params = self._bufs = self._calib = None
 
 
 @torch.no_grad()

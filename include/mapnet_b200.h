@@ -42,6 +42,7 @@ typedef struct mapnet_trunk mapnet_trunk_t;
 #define MAPNET_PREC_BF16_SIMT 2 /* bf16 storage + CUDA-core fp32 math: cross-check of mode 1         */
 #define MAPNET_PREC_TC_SPLIT 3  /* wgmma strict mode: fp32 conv outputs, conv operands as split fp16 hi/lo planes,\
                                    4 MMAs per product, fp32 accumulate -- meets the 1e-4 parity bar on tensor cores */
+#define MAPNET_PREC_FP8 4       /* inference engine only (mapnet_infer_*): e4m3 conv operands, calibrated scales */
 
 /* criterion modes (common/criterion.py) */
 #define MAPNET_LOSS_POSENET 0    /* PoseNetCriterion      pred [N,6],    targ [N,6]        */
@@ -197,7 +198,15 @@ int mapnet_pgo_optimize(const double* poses, const double* vos, double* out, int
  * droprate > 0): the same mask for the same (seed, step); step == UINT64_MAX takes the engine's device step counter
  * (graph-capturable).  Precisions: MAPNET_PREC_BF16 and MAPNET_PREC_TC_SPLIT only.  Argument errors (precision, B >
  * max_B, a forward before a load) return non-zero before anything is allocated or launched.
- * mapnet_infer_arena_bytes: host-only, the activation bytes a handle of these shapes allocates (< 0 on bad arguments). */
+ * MAPNET_PREC_FP8 (inference only): every conv but the stem runs on e4m3 operands -- weights with a power-of-two scale per
+ * output channel (taken at load), activations with one power-of-two scale per tensor (the pool output, every block's h
+ * and output: 33 at ResNet-34).  mapnet_infer_calibrate takes those scales from frames x [B,3,H,W] (B <= max_B),
+ * progressively over the engine's own schedule; it is required after every load and before the next forward (a forward
+ * without it fails before any launch) and rewrites the scales in place, so captured graphs stay valid.  It fails on
+ * bf16 / tc_split handles.  mapnet_infer_act_scales copies the activation scales in schedule order to host memory and
+ * returns 0 (cap: room in floats).
+ * mapnet_infer_arena_bytes: host-only, the activation bytes a handle of these shapes allocates (< 0 on bad arguments);
+ * fp8 adds the scale slots. */
 typedef struct mapnet_infer mapnet_infer_t;
 int mapnet_infer_create(mapnet_infer_t** out, int max_B, int H, int W, int feat_dim, int precision);
 int mapnet_infer_load(mapnet_infer_t* h, const float* params_flat, const float* bufs_flat, void* stream);
@@ -205,6 +214,8 @@ int mapnet_infer_forward(mapnet_infer_t* h, const float* x, int B, float droprat
                          float* pred, void* stream);
 int64_t mapnet_infer_arena_bytes(int max_B, int H, int W, int precision);
 int mapnet_infer_destroy(mapnet_infer_t* h);
+int mapnet_infer_calibrate(mapnet_infer_t* h, const float* x, int B, void* stream);
+int mapnet_infer_act_scales(mapnet_infer_t* h, float* host_out, int cap);
 
 /* ---- measurement support (bench.py): number of kernels this library has launched so
  * far in this process, and per-class conv timing with CUDA events on the launching
@@ -245,6 +256,14 @@ int mapnet_test_conv_epilogue(int kind, int B, int Hi, int Wi, int Ci, int Co, i
 int mapnet_test_conv_affine(int precision, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* in0,
                             const void* wmat, const float* scale, const float* shift, const void* residual, int flags,
                             void* out, void* stream);
+
+/* one fp8 fprop launch of the inference engine: f = conv(in0, wmat) * scale[c] + shift[c] (+ residual) (ReLU), in0 e4m3
+ * NHWC, wmat e4m3 [Co][k][k][Ci] (k = 1 or 3; Ci = 64 or a multiple of 128), scale / shift fp32 [Co].  flags: bit 0
+ * ReLU; bit 1 the residual is e4m3 (times *res_scale), else bf16; bit 2 out is e4m3 (f * *out_inv, saturating), else
+ * bf16; bit 3 the calibration pass: max |f| over the output into *amax (a float's bit pattern), nothing stored. */
+int mapnet_test_conv_fp8(int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* in0, const void* wmat,
+                         const float* scale, const float* shift, const void* residual, const float* res_scale,
+                         const float* out_inv, int flags, void* out, unsigned int* amax, void* stream);
 
 /* the tensor-core stem (7x7/s2/p3, 3 -> 64) alone, as the trunk runs it: space-to-depth image, packed weights,
  * fprop into y_out (bf16 NHWC [B,Hc,Wc,64]) and, when dy / dw_oihw are given, the weight gradient in the
