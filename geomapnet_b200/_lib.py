@@ -122,6 +122,13 @@ def lib():
     L.mapnet_infer_act_scales.argtypes = [c_void_p, POINTER(c_float), c_int]
     L.mapnet_test_conv_fp8.argtypes = [c_int] * 7 + [c_void_p] * 7 + [c_int, c_void_p, c_void_p, c_void_p]
     L.mapnet_test_conv_fp8.restype = c_int
+    L.mapnet_test_bn_forward.argtypes = [c_int] * 4 + [c_int64, c_int] + [c_void_p] * 5 + [c_int, c_void_p, c_void_p]
+    L.mapnet_test_bn_backward.argtypes = [c_int] * 3 + [c_int64, c_int] + [c_void_p] * 9 + [c_int, c_float, c_void_p,
+                                                                                              c_void_p]
+    L.mapnet_test_stem_pool.argtypes = [c_int] * 6 + [c_void_p] * 8 + [c_int, c_void_p, c_void_p]
+    L.mapnet_test_gap.argtypes = [c_int] * 4 + [c_void_p] * 5
+    for name in ("mapnet_test_bn_forward", "mapnet_test_bn_backward", "mapnet_test_stem_pool", "mapnet_test_gap"):
+        getattr(L, name).restype = c_int
     for name in ("mapnet_infer_create", "mapnet_infer_load", "mapnet_infer_forward", "mapnet_infer_destroy",
                  "mapnet_infer_calibrate", "mapnet_infer_act_scales"):
         getattr(L, name).restype = c_int
@@ -144,7 +151,8 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_sgd_step_dev", "mapnet_rmsprop_step_dev", "mapnet_test_conv_affine", "mapnet_infer_create",
             "mapnet_infer_load", "mapnet_infer_forward", "mapnet_infer_arena_bytes", "mapnet_infer_destroy",
             "mapnet_frame_cache_create", "mapnet_frame_cache_ingest", "mapnet_frame_cache_assemble",
-            "mapnet_frame_cache_destroy", "mapnet_infer_calibrate", "mapnet_infer_act_scales", "mapnet_test_conv_fp8"]
+            "mapnet_frame_cache_destroy", "mapnet_infer_calibrate", "mapnet_infer_act_scales", "mapnet_test_conv_fp8",
+            "mapnet_test_bn_forward", "mapnet_test_bn_backward", "mapnet_test_stem_pool", "mapnet_test_gap"]
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 
 

@@ -440,6 +440,271 @@ int mapnet_test_conv_fp8(int B, int Hi, int Wi, int Ci, int Co, int k, int strid
   return rc;
 }
 
+}  // extern "C"
+
+// ---- the element-wise kernels of bn.cu / head.cu one launch sequence at a time (tests/test_gpu_bn_pool.py) ----
+// Per-BatchNorm state: kTestBnRows rows of C floats (rows as in include/mapnet_b200.h), uploaded from host_params before
+// every pass and copied back into host_out after it.
+enum { TB_GAMMA, TB_BETA, TB_RMEAN, TB_RVAR, TB_MEAN, TB_INVSTD, TB_SCALE, TB_SHIFT, TB_MSCALE, TB_MSHIFT, TB_DGAMMA,
+       TB_DBETA, TB_COEF, kTestBnRows = TB_COEF + 3 };
+
+static bool test_prec_ok(int p) {
+  return p == PREC_FP32 || p == PREC_BF16_TC || p == PREC_BF16_SIMT || p == PREC_TC_SPLIT;
+}
+
+// the (A, Z, G) element types Net uses for a training precision
+template <typename Fn>
+static int with_test_types(int precision, Fn&& fn) {
+  if (precision == PREC_FP32) return fn(TypesF32());
+  if (precision == PREC_TC_SPLIT) return fn(TypesSplitHH());
+  return fn(TypesBF16());
+}
+
+struct TestBnState {
+  float* d = nullptr;          // [nbn][kTestBnRows][C]
+  double* accum = nullptr;     // [slot][kBnAccReplicas][kBnAccStride]
+  unsigned int* counter = nullptr;
+  float* gscale = nullptr;
+  int nbn = 0, C = 0;
+  float* row(int bn, int r) const { return d + ((size_t)bn * kTestBnRows + r) * C; }
+  double* acc(int slot) const { return accum + (size_t)slot * kBnAccReplicas * kBnAccStride; }
+  // nslots accumulator slots of kBnAccReplicas replicas (zeroed) and one counter
+  int alloc(int nbn_, int C_, int nslots, cudaStream_t st) {
+    nbn = nbn_; C = C_;
+    const size_t acc_bytes = (size_t)nslots * kBnAccReplicas * kBnAccStride * sizeof(double);
+    MN_CUDA(cudaMalloc((void**)&d, (size_t)nbn * kTestBnRows * C * sizeof(float)));
+    MN_CUDA(cudaMalloc((void**)&accum, acc_bytes));
+    MN_CUDA(cudaMalloc((void**)&counter, sizeof(unsigned int)));
+    MN_CUDA(cudaMalloc((void**)&gscale, sizeof(float)));
+    MN_CUDA(cudaMemsetAsync(accum, 0, acc_bytes, st));
+    MN_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int), st));
+    return 0;
+  }
+  void release() { cudaFree(d); cudaFree(accum); cudaFree(counter); cudaFree(gscale); }
+  int upload(const float* host_params, cudaStream_t st) {
+    MN_CUDA(cudaMemcpyAsync(d, host_params, (size_t)nbn * kTestBnRows * C * sizeof(float), cudaMemcpyHostToDevice, st));
+    return 0;
+  }
+  // host_sums [nrep][3][C] into the replica layout of bn_fin.cuh (replica r at kBnAccStride * r)
+  int upload_sums(int slot, const double* host_sums, int nrep, cudaStream_t st) {
+    MN_CUDA(cudaMemcpy2DAsync(acc(slot), kBnAccStride * sizeof(double), host_sums, 3 * (size_t)C * sizeof(double),
+                              3 * (size_t)C * sizeof(double), nrep, cudaMemcpyHostToDevice, st));
+    return 0;
+  }
+  int download(float* host_out, cudaStream_t st) {
+    MN_CUDA(cudaMemcpyAsync(host_out, d, (size_t)nbn * kTestBnRows * C * sizeof(float), cudaMemcpyDeviceToHost, st));
+    MN_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  }
+  BnFin fwd(int bn) const {
+    BnFin f; memset(&f, 0, sizeof(f));
+    f.gamma = row(bn, TB_GAMMA); f.beta = row(bn, TB_BETA); f.run_mean = row(bn, TB_RMEAN); f.run_var = row(bn, TB_RVAR);
+    f.mean = row(bn, TB_MEAN); f.invstd = row(bn, TB_INVSTD); f.scale = row(bn, TB_SCALE); f.shift = row(bn, TB_SHIFT);
+    return f;
+  }
+  // the backward of BatchNorm 0 [and of the downsample BatchNorm 1]; gate 2: the ReLU gate recomputed from y
+  BnFin bwd(bool ds, int gate) const {
+    BnFin f; memset(&f, 0, sizeof(f));
+    f.gamma = row(0, TB_GAMMA); f.mean = row(0, TB_MEAN); f.invstd = row(0, TB_INVSTD);
+    f.dgamma = row(0, TB_DGAMMA); f.dbeta = row(0, TB_DBETA); f.coef = row(0, TB_COEF);
+    if (gate == 2) { f.mscale = row(0, TB_MSCALE); f.mshift = row(0, TB_MSHIFT); }
+    if (ds) {
+      f.gamma2 = row(1, TB_GAMMA); f.mean2 = row(1, TB_MEAN); f.invstd2 = row(1, TB_INVSTD);
+      f.dgamma2 = row(1, TB_DGAMMA); f.dbeta2 = row(1, TB_DBETA); f.coef2 = row(1, TB_COEF);
+    }
+    return f;
+  }
+  BnDesc desc(const BnFin& f, long long M, bool sums, int bn, int nrep, bool forward) const {
+    BnDesc L; memset(&L, 0, sizeof(L));
+    if (sums) { L.accum = acc(bn); L.nrep = nrep; }
+    L.M = M; L.invM = 1.0 / (double)M;
+    L.unbias = (forward && M > 1) ? (double)M / (double)(M - 1) : 1.0;
+    L.f = f;
+    return L;
+  }
+};
+
+// forward per-channel parameters of BatchNorm bn as Net derives them: source 0 k_channel_sums over y (finalize by the
+// last block), 2 k_bn_eval_scale; sources 1 (lazy: the consumer finalizes) and 3 (scale / shift as given) launch nothing
+template <typename T>
+static int test_bn_forward_params(const TestBnState& s, int bn, int source, const T* y, long long M, cudaStream_t st) {
+  if (source == 0) return launch_bn_stats<T>(y, M, s.C, s.fwd(bn), s.acc(bn), s.counter, st);
+  if (source == 2) return launch_bn_eval_scale(s.C, s.fwd(bn), st);
+  return 0;
+}
+
+extern "C" {
+
+int mapnet_test_bn_forward(int precision, int res_mode, int relu, int source, int64_t M, int C, const void* y,
+                           const void* res, void* z, const float* host_params, const double* host_sums, int nrep,
+                           float* host_out, void* stream) {
+  MN_CHECK(test_prec_ok(precision), "test_bn_forward: precision %d is not a training precision", precision);
+  MN_CHECK(res_mode >= 0 && res_mode <= 2, "test_bn_forward: res_mode %d outside [0, 2]", res_mode);
+  MN_CHECK(source >= 0 && source <= 3, "test_bn_forward: source %d outside [0, 3]", source);
+  MN_CHECK(M >= 1 && C >= 64 && C <= 512 && C % 64 == 0, "test_bn_forward: need M >= 1 and C a multiple of 64 in "
+           "[64, 512] (got M %lld, C %d)", (long long)M, C);
+  MN_CHECK(y && z && host_params && host_out, "test_bn_forward: null argument");
+  MN_CHECK(res_mode == 0 || res != nullptr, "test_bn_forward: res_mode %d needs res (%s)", res_mode,
+           res_mode == 2 ? "the downsample branch's conv output, second BatchNorm" : "the identity branch");
+  MN_CHECK(source != 1 || (host_sums && nrep >= 1 && nrep <= kBnAccReplicas), "test_bn_forward: the lazy source needs "
+           "host_sums and 1 <= nrep <= %d (got %d)", kBnAccReplicas, nrep);
+  MN_TRY(require_device());
+  cudaStream_t st = (cudaStream_t)stream;
+  const int nbn = res_mode == 2 ? 2 : 1;
+  const int passes = source == 0 ? 2 : 1;     // source 0: the reduction twice on the same accumulators and counter
+  TestBnState s;
+  auto body = [&]() -> int {
+    MN_TRY(s.alloc(nbn, C, nbn, st));
+    for (int pass = 0; pass < passes; ++pass) {
+      MN_TRY(s.upload(host_params, st));
+      if (source == 1)
+        for (int bn = 0; bn < nbn; ++bn) MN_TRY(s.upload_sums(bn, host_sums + (size_t)bn * nrep * 3 * C, nrep, st));
+      MN_TRY(with_test_types(precision, [&](auto tp) -> int {
+        typedef typename decltype(tp)::A T;
+        typedef typename decltype(tp)::Z TZ;
+        MN_TRY(test_bn_forward_params<T>(s, 0, source, (const T*)y, M, st));
+        if (nbn == 2) MN_TRY(test_bn_forward_params<T>(s, 1, source, (const T*)res, M, st));
+        const BnDesc l1 = s.desc(s.fwd(0), M, source == 1, 0, nrep, true);
+        const BnDesc l2 = s.desc(s.fwd(nbn - 1), M, source == 1, nbn - 1, nrep, true);
+        return launch_bn_apply<T, TZ>((const T*)y, res_mode, res, (TZ*)z, M, C, relu, l1, nbn == 2 ? &l2 : nullptr, st);
+      }));
+      MN_TRY(s.download(host_out + (size_t)pass * nbn * kTestBnRows * C, st));
+    }
+    return 0;
+  };
+  const int r = body();
+  s.release();
+  return r;
+}
+
+int mapnet_test_bn_backward(int precision, int source, int gate, int64_t M, int C, const void* dout, const void* zmask,
+                            const void* y, const void* yd, void* dy, void* dyd, void* gout, const float* host_params,
+                            const double* host_sums, int nrep, float gscale, float* host_out, void* stream) {
+  MN_CHECK(test_prec_ok(precision), "test_bn_backward: precision %d is not a training precision", precision);
+  MN_CHECK(source == 0 || source == 1, "test_bn_backward: source %d is neither 0 (reduce) nor 1 (lazy)", source);
+  MN_CHECK(gate >= 0 && gate <= 2, "test_bn_backward: gate %d outside [0, 2]", gate);
+  MN_CHECK(M >= 1 && C >= 64 && C <= 512 && C % 64 == 0, "test_bn_backward: need M >= 1 and C a multiple of 64 in "
+           "[64, 512] (got M %lld, C %d)", (long long)M, C);
+  MN_CHECK(dout && y && dy && host_params && host_out, "test_bn_backward: null argument");
+  MN_CHECK((gate == 1) == (zmask != nullptr), "test_bn_backward: zmask is given exactly when gate == 1");
+  MN_CHECK((yd != nullptr) == (dyd != nullptr), "test_bn_backward: yd and dyd go together (downsample BatchNorm)");
+  MN_CHECK(source != 1 || (host_sums && nrep >= 1 && nrep <= kBnAccReplicas), "test_bn_backward: the lazy source needs "
+           "host_sums and 1 <= nrep <= %d (got %d)", kBnAccReplicas, nrep);
+  MN_CHECK(gscale >= 0.f, "test_bn_backward: gscale %g < 0", (double)gscale);
+  MN_TRY(require_device());
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool ds = yd != nullptr;
+  const int nbn = ds ? 2 : 1;
+  const int passes = source == 0 ? 2 : 1;
+  TestBnState s;
+  auto body = [&]() -> int {
+    MN_TRY(s.alloc(nbn, C, nbn, st));
+    MN_CUDA(cudaMemcpyAsync(s.gscale, &gscale, sizeof(float), cudaMemcpyHostToDevice, st));
+    for (int pass = 0; pass < passes; ++pass) {
+      MN_TRY(s.upload(host_params, st));
+      if (source == 1) MN_TRY(s.upload_sums(0, host_sums, nrep, st));
+      MN_TRY(with_test_types(precision, [&](auto tp) -> int {
+        typedef typename decltype(tp)::A T;
+        typedef typename decltype(tp)::Z TZ;
+        typedef typename decltype(tp)::G TG;
+        const BnFin f = s.bwd(ds, gate);
+        if (source == 0)
+          MN_TRY((launch_bn_bwd_reduce<T, TZ>((const T*)dout, (const TZ*)zmask, (const T*)y, (const T*)yd, M, C, f,
+                                              s.acc(0), s.counter, st)));
+        return launch_bn_bwd_apply<T, TZ, TG>((const T*)dout, (const TZ*)zmask, (const T*)y, (TG*)dy, (const T*)yd,
+                                              (TG*)dyd, (T*)gout, M, C, s.desc(f, M, source == 1, 0, nrep, false),
+                                              gscale > 0.f ? s.gscale : nullptr, st);
+      }));
+      MN_TRY(s.download(host_out + (size_t)pass * nbn * kTestBnRows * C, st));
+    }
+    return 0;
+  };
+  const int r = body();
+  s.release();
+  return r;
+}
+
+int mapnet_test_stem_pool(int precision, int source, int bsource, int B, int Hc, int Wc, const void* y, void* z,
+                          void* amax, const void* dz, void* g, void* dy, const float* host_params,
+                          const double* host_sums, int nrep, float* host_out, void* stream) {
+  const bool f8 = precision == PREC_FP8;
+  MN_CHECK(test_prec_ok(precision) || f8, "test_stem_pool: precision %d is neither a training precision nor fp8",
+           precision);
+  MN_CHECK(source >= 0 && source <= 3, "test_stem_pool: source %d outside [0, 3]", source);
+  MN_CHECK(B >= 1 && Hc >= 1 && Wc >= 1, "test_stem_pool: bad shape %dx%dx%d", B, Hc, Wc);
+  MN_CHECK(y && z && host_params && host_out, "test_stem_pool: null argument");
+  MN_CHECK(!f8 || (source == 3 && dz == nullptr), "test_stem_pool: fp8 is the inference pool (source 3, no backward)");
+  MN_CHECK(source != 1 || (host_sums && nrep >= 1 && nrep <= kBnAccReplicas), "test_stem_pool: the lazy source needs "
+           "host_sums and 1 <= nrep <= %d (got %d)", kBnAccReplicas, nrep);
+  const bool even = Hc % 2 == 0 && Wc % 2 == 0;
+  if (dz != nullptr) {
+    MN_CHECK(amax && g && dy && source != 3, "test_stem_pool: the backward needs amax, g, dy and batch statistics");
+    MN_CHECK(bsource == 0 || bsource == 1, "test_stem_pool: bsource %d is neither 0 nor 1 (lazy)", bsource);
+    MN_CHECK(bsource == 0 || even, "test_stem_pool: the lazy backward needs even Hc, Wc (got %dx%d)", Hc, Wc);
+  }
+  MN_TRY(require_device());
+  cudaStream_t st = (cudaStream_t)stream;
+  const int C = 64;
+  const int Ho = (Hc - 1) / 2 + 1, Wo = (Wc - 1) / 2 + 1;
+  const long long M = (long long)B * Hc * Wc;
+  TestBnState s;
+  auto body = [&]() -> int {
+    MN_TRY(s.alloc(1, C, 2, st));        // slot 0: the forward sums, slot 1: the backward's (as Net's two slots)
+    MN_TRY(s.upload(host_params, st));
+    if (source == 1) MN_TRY(s.upload_sums(0, host_sums, nrep, st));
+    const BnDesc lf = s.desc(s.fwd(0), M, source == 1, 0, nrep, true);
+    if (f8) {
+      MN_TRY((launch_stem_pool<bf16, e4m3>((const bf16*)y, (e4m3*)z, (uint8_t*)amax, B, Hc, Wc, Ho, Wo, C, lf, st)));
+      return s.download(host_out, st);
+    }
+    MN_TRY(with_test_types(precision, [&](auto tp) -> int {
+      typedef typename decltype(tp)::A T;
+      typedef typename decltype(tp)::Z TZ;
+      typedef typename decltype(tp)::G TG;
+      MN_TRY(test_bn_forward_params<T>(s, 0, source, (const T*)y, M, st));
+      MN_TRY((launch_stem_pool<T, TZ>((const T*)y, (TZ*)z, (uint8_t*)amax, B, Hc, Wc, Ho, Wo, C, lf, st)));
+      if (dz == nullptr) return 0;
+      // the stem's backward as Net runs it: even sizes accumulate the BatchNorm sums in the pool backward (finalized by
+      // k_bn_bwd_finalize_accum, or lazily by the apply kernel over kBnAccReplicas replicas), odd sizes reduce afterwards
+      const BnFin fb = s.bwd(false, 0);
+      if (even) {
+        MN_TRY(launch_stem_pool_bwd<T>((const T*)dz, (const uint8_t*)amax, (const T*)y, s.row(0, TB_SCALE),
+                                       s.row(0, TB_SHIFT), (T*)g, B, Hc, Wc, Ho, Wo, C, st, s.acc(1)));
+        if (bsource == 0) MN_TRY(launch_bn_bwd_finalize_accum(M, C, fb, s.acc(1), st));
+      } else {
+        MN_TRY(launch_stem_pool_bwd<T>((const T*)dz, (const uint8_t*)amax, (const T*)y, s.row(0, TB_SCALE),
+                                       s.row(0, TB_SHIFT), (T*)g, B, Hc, Wc, Ho, Wo, C, st));
+        MN_TRY((launch_bn_bwd_reduce<T, TZ>((const T*)g, (const TZ*)nullptr, (const T*)y, nullptr, M, C, fb, s.acc(1),
+                                            s.counter, st)));
+      }
+      return launch_bn_bwd_apply<T, TZ, TG>((const T*)g, (const TZ*)nullptr, (const T*)y, (TG*)dy, nullptr, nullptr,
+                                            nullptr, M, C, s.desc(fb, M, bsource == 1, 1, kBnAccReplicas, false),
+                                            nullptr, st);
+    }));
+    return s.download(host_out, st);
+  };
+  const int r = body();
+  s.release();
+  return r;
+}
+
+int mapnet_test_gap(int precision, int B, int HW, int C, const void* z, float* feat, const float* dfeat, void* dz,
+                    void* stream) {
+  MN_CHECK(test_prec_ok(precision), "test_gap: precision %d is not a training precision", precision);
+  MN_CHECK(B >= 1 && HW >= 1 && C >= 8 && C <= 2048 && C % 8 == 0, "test_gap: bad shape B %d HW %d C %d", B, HW, C);
+  MN_CHECK(z && feat && dfeat && dz, "test_gap: null argument");
+  MN_TRY(require_device());
+  cudaStream_t st = (cudaStream_t)stream;
+  MN_TRY(with_test_types(precision, [&](auto tp) -> int {
+    typedef typename decltype(tp)::A T;
+    typedef typename decltype(tp)::Z TZ;
+    MN_TRY(launch_gap<TZ>((const TZ*)z, feat, B, HW, C, st));
+    return launch_gap_bwd<T>(dfeat, (T*)dz, B, HW, C, st);
+  }));
+  MN_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
 // ---- eval-mode inference engine (infer.cu) ----
 int64_t mapnet_infer_arena_bytes(int max_B, int H, int W, int precision) {
   return InferNet::arena_bytes(max_B, H, W, precision);

@@ -265,6 +265,40 @@ int mapnet_test_conv_fp8(int B, int Hi, int Wi, int Ci, int Co, int k, int strid
                          const float* scale, const float* shift, const void* residual, const float* res_scale,
                          const float* out_inv, int flags, void* out, unsigned int* amax, void* stream);
 
+/* ---- the element-wise kernels of the training step (bn.cu, head.cu) one launch sequence at a time, as the trunk
+ * runs them, for the per-kernel tests (tests/test_gpu_bn_pool.py).  precision selects the storage types the trunk uses:
+ * fp32 -> fp32 everywhere; bf16 / bf16_simt -> bf16; tc_split -> conv outputs and gradients w.r.t. block outputs fp32,
+ * forward and backward conv operands (z, the identity residual, zmask, dy, dyd) fp16 hi/lo planes.  Tensors are NHWC
+ * device memory; every call allocates its own accumulators and counter, synchronizes and frees them again.
+ * BatchNorm state: host_params / host_out hold, per BatchNorm, 15 rows of C floats: gamma, beta, running_mean,
+ * running_var, mean, invstd, scale, shift, mscale, mshift (ReLU gate recomputed from y), dgamma, dbeta and the three
+ * dy = A*g + B*y + C coefficients.  host_params is uploaded before every pass, host_out receives the state after it.
+ * Lazy sums (source 1): host_sums [nrep][3][C] doubles per BatchNorm, copied into nrep accumulator replicas that the
+ * consuming kernel finalizes. */
+/* z = relu?(scale*y + shift [+ res | + scale2*res + shift2]); res_mode 0 none, 1 identity (z's type), 2 downsample
+ * branch (y's type, second BatchNorm).  source 0: batch statistics by the reducing kernel, run twice on the same
+ * accumulators and counter (host_out: 2 passes); 1: lazy sums; 2: eval-mode scale / shift from the running statistics;
+ * 3: scale / shift as given. */
+int mapnet_test_bn_forward(int precision, int res_mode, int relu, int source, int64_t M, int C, const void* y,
+                           const void* res, void* z, const float* host_params, const double* host_sums, int nrep,
+                           float* host_out, void* stream);
+/* dy = A*g + B*y + C [, dyd = Ad*g + Bd*yd + Cd] [, gout = g], g = dout gated by: gate 0 nothing, 1 zmask > 0, 2
+ * mscale*y + mshift > 0.  yd / dyd: the downsample BatchNorm (second state block).  source 0: sums by the reducing
+ * kernel, run twice (host_out: 2 passes); 1: lazy sums.  gscale > 0: dy / dyd are scaled by it (strict mode). */
+int mapnet_test_bn_backward(int precision, int source, int gate, int64_t M, int C, const void* dout, const void* zmask,
+                            const void* y, const void* yd, void* dy, void* dyd, void* gout, const float* host_params,
+                            const double* host_sums, int nrep, float gscale, float* host_out, void* stream);
+/* the stem's BatchNorm + ReLU + 3x3/s2/p1 max pool on y [B,Hc,Wc,64] -> z, argmax bytes -> amax (may be NULL), with
+ * source as for mapnet_test_bn_forward (once).  precision MAPNET_PREC_FP8: bf16 y, e4m3 z, source 3 only.  dz != NULL:
+ * then the backward from amax: g = pool / ReLU backward, the BatchNorm's sums (even Hc, Wc: fused into the pool backward,
+ * finalized by k_bn_bwd_finalize_accum when bsource is 0, lazily over 32 replicas when 1; odd: a reducing pass), dy. */
+int mapnet_test_stem_pool(int precision, int source, int bsource, int B, int Hc, int Wc, const void* y, void* z,
+                          void* amax, const void* dz, void* g, void* dy, const float* host_params,
+                          const double* host_sums, int nrep, float* host_out, void* stream);
+/* feat [B,C] = mean over HW pixels of z [B,HW,C] (z's type); dz [B,HW,C] = dfeat / HW (gradient type) */
+int mapnet_test_gap(int precision, int B, int HW, int C, const void* z, float* feat, const float* dfeat, void* dz,
+                    void* stream);
+
 /* the tensor-core stem (7x7/s2/p3, 3 -> 64) alone, as the trunk runs it: space-to-depth image, packed weights,
  * fprop into y_out (bf16 NHWC [B,Hc,Wc,64]) and, when dy / dw_oihw are given, the weight gradient in the
  * .grad layout [64,3,7,7].  Replaces torchvision ResNet.conv1 (/root/reference/models/posenet.py:66). */

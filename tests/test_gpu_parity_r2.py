@@ -8,7 +8,9 @@
    fixtures tests/golden/emu_bf16_*.npz).  Measured: only ~2x closer than to the fp32 reference -- two bf16
    implementations that round at the same points still differ at the percent level after 36 layers (summation order moves
    individual roundings and ReLU masks); the bounds document that noise floor, kernel correctness is carried by the
-   per-conv and per-epilogue unit tests (tests/test_gpu_kernels.py) and by the strict mode;
+   per-conv and per-epilogue unit tests (tests/test_gpu_kernels.py), the per-kernel float64 tests of the BatchNorm,
+   ReLU / residual, stem max-pool and global-average-pool kernels in every storage mode, bf16 included
+   (tests/test_gpu_bn_pool.py), and by the strict mode;
  * the strict tensor-core product against the f16x2-emulating oracle;
  * multi-step trajectories with gradient clipping and learnable criterion scalars (clip_grad_norm_ covers
    model.parameters() only: common/train.py:357-358).

@@ -109,3 +109,55 @@ def test_mf_tuple_lengths_and_clipping():
     assert tr.tolist() == [81, 83, 85, 87, 89] and va.tolist() == [(85 % 92) + k for k in (0, 2, 4, 6, 8)]
     idx = T.batch_frame_indices([0, 50], 100, 3, 10)
     assert idx.dtype == np.int32 and idx.tolist() == [0, 0, 10, 40, 50, 60]
+
+
+def _rc_and_message(fn, *args):
+    from geomapnet_b200 import _lib
+    rc = fn(*args)
+    msg = _lib.lib().mapnet_last_error()
+    return rc, (msg.decode() if msg else "")
+
+
+def test_element_wise_test_entry_points_fail_with_a_message(built):
+    """mapnet_test_bn_forward / _bn_backward / _stem_pool / _gap check their arguments before they touch the device:
+    on any host a bad call returns non-zero with a message (the pointers below are never dereferenced); on a host
+    without a device so does a well-formed call."""
+    from geomapnet_b200 import _lib
+    L = _lib.lib()
+    buf = np.zeros(64, dtype=np.float32)
+    h = buf.ctypes.data
+    fwd = lambda prec, res_mode, source, M, C, res, nrep=8: _rc_and_message(
+        L.mapnet_test_bn_forward, prec, res_mode, 1, source, M, C, h, res, h, h, h, nrep, h, None)
+    cases = [
+        (fwd(1, 0, 1, 64, 96, None), "multiple of 64"),                  # the apply kernels take 64-channel slices
+        (fwd(1, 2, 0, 64, 64, None), "res_mode 2 needs res"),           # the downsample branch is missing
+        (fwd(4, 0, 0, 64, 64, None), "not a training precision"),       # fp8 has no training element-wise path
+        (fwd(1, 3, 0, 64, 64, None), "res_mode 3"),
+        (fwd(1, 0, 1, 64, 64, None, nrep=33), "nrep"),                   # more replicas than a slot has
+        (_rc_and_message(L.mapnet_test_bn_backward, 1, 0, 1, 64, 64, h, None, h, None, h, None, None, h, None, 0, 0.0,
+                         h, None), "zmask is given exactly when gate == 1"),
+        (_rc_and_message(L.mapnet_test_bn_backward, 3, 2, 0, 64, 64, h, None, h, None, h, None, None, h, None, 0, 0.0,
+                         h, None), "neither 0 (reduce) nor 1 (lazy)"),
+        (_rc_and_message(L.mapnet_test_stem_pool, 1, 1, 1, 1, 7, 9, h, h, h, h, h, h, h, h, 8, h, None),
+         "lazy backward needs even Hc, Wc"),
+        (_rc_and_message(L.mapnet_test_stem_pool, 4, 0, 0, 1, 8, 8, h, h, h, None, None, None, h, None, 8, h, None),
+         "fp8 is the inference pool"),
+        (_rc_and_message(L.mapnet_test_gap, 7, 2, 4, 512, h, h, h, h, None), "not a training precision"),
+        (_rc_and_message(L.mapnet_test_gap, 1, 2, 4, 12, h, h, h, h, None), "bad shape"),
+    ]
+    for (rc, msg), want in cases:
+        assert rc != 0 and want in msg, (rc, msg, want)
+    if torch.cuda.is_available():       # the well-formed calls below would run (the pointers are host memory)
+        return
+    # without a CUDA device, well-formed calls fail with a message instead of crashing
+    buf = np.zeros(64 * 15 * 2, dtype=np.float32)
+    h = buf.ctypes.data
+    calls = [
+        (L.mapnet_test_bn_forward, 1, 0, 1, 0, 64, 64, h, None, h, h, None, 0, h, None),
+        (L.mapnet_test_bn_backward, 1, 0, 0, 64, 64, h, None, h, None, h, None, None, h, None, 0, 0.0, h, None),
+        (L.mapnet_test_stem_pool, 1, 0, 0, 1, 8, 8, h, h, h, None, None, None, h, None, 0, h, None),
+        (L.mapnet_test_gap, 1, 2, 4, 512, h, h, h, h, None),
+    ]
+    for fn, *args in calls:
+        rc, msg = _rc_and_message(fn, *args)
+        assert rc != 0 and "no CUDA device" in msg, (fn.__name__, rc, msg)
