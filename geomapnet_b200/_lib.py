@@ -53,6 +53,8 @@ def lib():
     L.mapnet_backward_part.restype = c_int
     L.mapnet_grad_part_range.argtypes = [c_void_p, c_int, POINTER(c_int64), POINTER(c_int64)]
     L.mapnet_grad_part_range.restype = c_int
+    L.mapnet_trunk_set_trainable.argtypes = [c_void_p, POINTER(ctypes.c_uint8), c_int]
+    L.mapnet_trunk_set_trainable.restype = c_int
     L.mapnet_loss_fwd_bwd.argtypes = [c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
                                       c_void_p, c_void_p, c_void_p]
     L.mapnet_sqnorm.argtypes = [c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
@@ -152,7 +154,8 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_infer_load", "mapnet_infer_forward", "mapnet_infer_arena_bytes", "mapnet_infer_destroy",
             "mapnet_frame_cache_create", "mapnet_frame_cache_ingest", "mapnet_frame_cache_assemble",
             "mapnet_frame_cache_destroy", "mapnet_infer_calibrate", "mapnet_infer_act_scales", "mapnet_test_conv_fp8",
-            "mapnet_test_bn_forward", "mapnet_test_bn_backward", "mapnet_test_stem_pool", "mapnet_test_gap"]
+            "mapnet_test_bn_forward", "mapnet_test_bn_backward", "mapnet_test_stem_pool", "mapnet_test_gap",
+            "mapnet_trunk_set_trainable"]
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 
 
@@ -173,8 +176,19 @@ class Trunk(object):
     def __init__(self, max_B, H, W, feat_dim, precision):
         self.h = c_void_p()
         self.max_B, self.H, self.W, self.feat_dim, self.precision = max_B, H, W, feat_dim, precision
+        self.trainable = None         # the mask last passed to mapnet_trunk_set_trainable
         check(lib().mapnet_trunk_create(ctypes.byref(self.h), max_B, H, W, feat_dim, PREC[precision]),
               "mapnet_trunk_create")
+
+    def set_trainable(self, mask):
+        """mask: one flag per trainable entry (kind 0) of the parameter table, in table order.  The handle is told only
+        when the mask differs from the one last passed."""
+        mask = tuple(bool(m) for m in mask)
+        if mask == self.trainable:
+            return
+        buf = (ctypes.c_uint8 * len(mask))(*mask)
+        check(lib().mapnet_trunk_set_trainable(self.h, buf, len(mask)), "mapnet_trunk_set_trainable")
+        self.trainable = mask
 
     def table(self):
         L = lib()

@@ -88,6 +88,11 @@ int mapnet_backward_part(mapnet_trunk_t* h, int part, const float* dpred, const 
   return h->net.backward(dpred, params_flat, grads_flat, filter_nans, part, (cudaStream_t)stream);
 }
 
+int mapnet_trunk_set_trainable(mapnet_trunk_t* h, const uint8_t* host_mask, int n) {
+  MN_CHECK(h != nullptr, "set_trainable: null handle");
+  return h->net.set_trainable(host_mask, n);
+}
+
 int mapnet_grad_part_range(mapnet_trunk_t* h, int part, int64_t* host_lo, int64_t* host_hi) {
   MN_CHECK(h != nullptr && host_lo && host_hi && part >= 0 && part <= 2, "grad_part_range: bad argument");
   long long lo = 0, hi = 0;

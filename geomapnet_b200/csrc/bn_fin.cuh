@@ -73,20 +73,21 @@ __device__ __forceinline__ BnBwdCoef bn_bwd_coef(const float mean, const float i
   return k;
 }
 
-// s0 = sum g, s1 = sum g*y [, s1d = sum g*yd]:  d gamma, d beta and dy = A*g + B*y + C coefficients
+// s0 = sum g, s1 = sum g*y [, s1d = sum g*yd]:  d gamma, d beta and dy = A*g + B*y + C coefficients.
+// A null dgamma / dbeta (a frozen parameter) is not written; the coefficients always are.
 __device__ __forceinline__ void bn_fin_backward(const int c, const int C, const double s0, const double s1,
                                                 const double s1d, const long long M, const BnFin& f, const bool ds) {
   const double invM = 1.0 / (double)M;
   {
     const BnBwdCoef k = bn_bwd_coef(f.mean[c], f.invstd[c], f.gamma[c], s0, s1, invM);
-    f.dgamma[c] = (float)k.s2;
-    f.dbeta[c] = (float)s0;
+    if (f.dgamma != nullptr) f.dgamma[c] = (float)k.s2;
+    if (f.dbeta != nullptr) f.dbeta[c] = (float)s0;
     f.coef[c] = (float)k.A; f.coef[C + c] = (float)k.B; f.coef[2 * C + c] = (float)k.C;
   }
   if (ds) {
     const BnBwdCoef k = bn_bwd_coef(f.mean2[c], f.invstd2[c], f.gamma2[c], s0, s1d, invM);
-    f.dgamma2[c] = (float)k.s2;
-    f.dbeta2[c] = (float)s0;
+    if (f.dgamma2 != nullptr) f.dgamma2[c] = (float)k.s2;
+    if (f.dbeta2 != nullptr) f.dbeta2[c] = (float)s0;
     f.coef2[c] = (float)k.A; f.coef2[C + c] = (float)k.B; f.coef2[2 * C + c] = (float)k.C;
   }
 }

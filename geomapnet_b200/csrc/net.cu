@@ -156,6 +156,11 @@ int Net::init(int max_B_, int H_, int W_, int feat_dim_, int precision_) {
   stats_target = nullptr; bn_slots = nullptr; bn_slots_bytes = 0;
   { const char* e = getenv("MAPNET_TC_DS_FOLD"); ds_fold = (precision == PREC_BF16_TC) && (e ? atoi(e) != 0 : 1); }
   build_table();
+  {
+    std::vector<uint8_t> all;
+    for (auto& e : table) if (e.kind == 0) all.push_back(1);
+    MN_TRY(set_trainable(all.data(), (int)all.size()));
+  }
   if (max_B == 0) return 0;      // spec-only handle: parameter table, no device memory
   const size_t es = elt();
   const long long Bm = max_B;
@@ -224,6 +229,27 @@ int Net::init(int max_B_, int H_, int W_, int feat_dim_, int precision_) {
   MN_TRY(alloc((void**)&gscale, 16));
   { const float one[2] = {1.f, 1.f}; MN_CUDA(cudaMemcpy(gscale, one, sizeof(one), cudaMemcpyHostToDevice)); }
   MN_CUDA(cudaMemset(drop_ctr, 0, 16));
+  return 0;
+}
+
+int Net::set_trainable(const uint8_t* host_mask, int n) {
+  int nk = 0;
+  for (auto& e : table) nk += (e.kind == 0);
+  MN_CHECK(host_mask != nullptr, "set_trainable: null mask");
+  MN_CHECK(n == nk, "set_trainable: mask has %d entries, the parameter table %d trainable ones", n, nk);
+  std::map<long long, bool> by_off;       // parameter offset -> needs a gradient
+  int k = 0;
+  for (auto& e : table) if (e.kind == 0) by_off[e.offset] = host_mask[k++] != 0;
+  for (auto& c : convs) c.train = by_off[c.wd.p_off];
+  for (auto& b : bns) { b.train_g = by_off[b.g_off]; b.train_b = by_off[b.b_off]; }
+  train_fc_w = by_off[fc_w]; train_fc_b = by_off[fc_b];
+  train_xyz_w = by_off[xyz_w]; train_xyz_b = by_off[xyz_b];
+  train_wpqr_w = by_off[wpqr_w]; train_wpqr_b = by_off[wpqr_b];
+  auto conv_trains = [&](int ci) { return ci >= 0 && (convs[ci].train || bns[convs[ci].bn].train_g || bns[convs[ci].bn].train_b); };
+  bwd_lo = (int)blocks.size();
+  for (int bi = (int)blocks.size() - 1; bi >= 0; --bi)
+    if (conv_trains(blocks[bi].conv1) || conv_trains(blocks[bi].conv2) || conv_trains(blocks[bi].convd)) bwd_lo = bi;
+  if (conv_trains(0)) bwd_lo = -1;
   return 0;
 }
 
@@ -462,11 +488,13 @@ BnDesc Net::lazy_backward(int bi, int bi_ds, long long M, const float* params, f
   L.M = M;
   L.invM = 1.0 / (double)M; L.unbias = 1.0;
   L.f.gamma = params + b.g_off; L.f.mean = b.mean; L.f.invstd = b.invstd;
-  L.f.dgamma = grads + b.g_off; L.f.dbeta = grads + b.b_off; L.f.coef = b.coef;
+  // a frozen gamma / beta gets no gradient: its grads_flat entries keep the zero of the pass's opening memset
+  L.f.dgamma = b.train_g ? grads + b.g_off : nullptr; L.f.dbeta = b.train_b ? grads + b.b_off : nullptr; L.f.coef = b.coef;
   if (bi_ds >= 0) {
     BNL& d = bns[bi_ds];
     L.f.gamma2 = params + d.g_off; L.f.mean2 = d.mean; L.f.invstd2 = d.invstd;
-    L.f.dgamma2 = grads + d.g_off; L.f.dbeta2 = grads + d.b_off; L.f.coef2 = d.coef;
+    L.f.dgamma2 = d.train_g ? grads + d.g_off : nullptr; L.f.dbeta2 = d.train_b ? grads + d.b_off : nullptr;
+    L.f.coef2 = d.coef;
   }
   return L;
 }
@@ -589,20 +617,24 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
   // strict mode: the backward conv operands are fp16 planes; ONE power-of-two scale per step (from max|d pred|)
   // places every gradient tensor inside fp16's window, the consuming conv epilogues divide it out again
   const float* gs = (precision == PREC_TC_SPLIT) ? gscale : nullptr;
+  const bool trunk = bwd_lo < (int)blocks.size();       // a conv or BatchNorm parameter needs a gradient
   if (do_head) {
   MN_TRY(launch_dpred_filter(dpred, dpredf, dpredh, B, filter_nans, st));
-  if (gs != nullptr) MN_TRY(launch_grad_scale(dpredh, B * 6, gscale, st));
+  if (gs != nullptr && trunk) MN_TRY(launch_grad_scale(dpredh, B * 6, gscale, st));
   // dW_xyz[c][j] = sum_b dpred[b][c] * hdrop[b][j]
-  MN_TRY(launch_small_gemm(0, dpredf, 1, 6, hdrop, 1, F, grads + xyz_w, F, 3, F, B, nullptr, nullptr, nullptr, st));
-  MN_TRY(launch_small_gemm(0, dpredf + 3, 1, 6, hdrop, 1, F, grads + wpqr_w, F, 3, F, B, nullptr, nullptr, nullptr, st));
-  MN_TRY(launch_colsum(dpredf, 6, B, 3, grads + xyz_b, st));
-  MN_TRY(launch_colsum(dpredf + 3, 6, B, 3, grads + wpqr_b, st));
-  MN_TRY(launch_head_dh(dpredh, params + xyz_w, params + wpqr_w, last_has_mask ? mask : nullptr, fcpre, dh, B, F, st));
+  if (train_xyz_w) MN_TRY(launch_small_gemm(0, dpredf, 1, 6, hdrop, 1, F, grads + xyz_w, F, 3, F, B, nullptr, nullptr, nullptr, st));
+  if (train_wpqr_w) MN_TRY(launch_small_gemm(0, dpredf + 3, 1, 6, hdrop, 1, F, grads + wpqr_w, F, 3, F, B, nullptr, nullptr, nullptr, st));
+  if (train_xyz_b) MN_TRY(launch_colsum(dpredf, 6, B, 3, grads + xyz_b, st));
+  if (train_wpqr_b) MN_TRY(launch_colsum(dpredf + 3, 6, B, 3, grads + wpqr_b, st));
+  if (train_fc_w || train_fc_b || trunk)
+    MN_TRY(launch_head_dh(dpredh, params + xyz_w, params + wpqr_w, last_has_mask ? mask : nullptr, fcpre, dh, B, F, st));
   // dW_fc[o][i] = sum_b dh[b][o] * feat[b][i];  db_fc = colsum(dh);  dfeat = dh @ W_fc
-  MN_TRY(launch_small_gemm(0, dh, 1, F, feat, 1, 512, grads + fc_w, 512, F, 512, B, nullptr, nullptr, nullptr, st));
-  MN_TRY(launch_colsum(dh, F, B, F, grads + fc_b, st));
-  MN_TRY(launch_small_gemm(0, dh, F, 1, params + fc_w, 1, 512, dfeat, 512, B, 512, F, nullptr, nullptr, nullptr, st));
-  MN_TRY(launch_gap_bwd<T>(dfeat, S0, B, Hf * Wf, 512, st));
+  if (train_fc_w) MN_TRY(launch_small_gemm(0, dh, 1, F, feat, 1, 512, grads + fc_w, 512, F, 512, B, nullptr, nullptr, nullptr, st));
+  if (train_fc_b) MN_TRY(launch_colsum(dh, F, B, F, grads + fc_b, st));
+  if (trunk) {
+    MN_TRY(launch_small_gemm(0, dh, F, 1, params + fc_w, 1, 512, dfeat, 512, B, 512, F, nullptr, nullptr, nullptr, st));
+    MN_TRY(launch_gap_bwd<T>(dfeat, S0, B, Hf * Wf, 512, st));
+  }
   bwd_pre = false;
   }
 
@@ -610,13 +642,14 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
   // fuse_bwd (wgmma path): the dgrad that PRODUCES a BatchNorm's incoming gradient gates it with that
   // BN's ReLU and accumulates its backward reductions in the epilogue (conv_tc.cu, EpiBwd), so only the apply pass
   // remains, and it finalizes the sums itself (BnDesc).  `pre` = S0 arrives gated with the BN2 sums of this block pending.
+  // Frozen parameters: the pass stops at the lowest block that trains (lo), and that block computes no gradient w.r.t.
+  // its input (conv1 and downsample dgrad) unless the stem trains.
   bool pre = bwd_pre;
-  int conv_lo = (int)convs.size(), conv_hi = -1;       // convs whose weight gradients this call completes
-  for (int bi = (int)blocks.size() - 1; bi >= 0; --bi) {
+  const int lo = bwd_lo > 0 ? bwd_lo : 0;
+  for (int bi = (int)blocks.size() - 1; bi >= lo; --bi) {
     if (part >= 0 && part_of_block(bi) != part) continue;
     BlockL& bl = blocks[bi];
-    conv_lo = bl.conv1 < conv_lo ? bl.conv1 : conv_lo;
-    { const int last = bl.convd >= 0 ? bl.convd : bl.conv2; conv_hi = last > conv_hi ? last : conv_hi; }
+    const bool dgrad_in = bi > bwd_lo;
     const TZ* zin = (bi == 0) ? (const TZ*)z0 : (const TZ*)blocks[bi - 1].out;
     const long long Mo = (long long)B * bl.Ho * bl.Wo;
     const int C = bl.Cout;
@@ -633,12 +666,12 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
       const T* yd = ds ? (const T*)bl.yd : nullptr;
       if (!pre) MN_TRY((launch_bn_bwd_reduce<T, TZ>(S0, zmask, (const T*)bl.y2, yd, Mo, C, d2.f, bn_accum, bn_counter, st)));
       // identity branch: the gated gradient is written to S3, unless S0 already holds it (conv1's dgrad adds it in place)
-      T* gout = (ds || pre) ? nullptr : S3;
+      T* gout = (ds || pre || !dgrad_in) ? nullptr : S3;
       MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S0, zmask, (const T*)bl.y2, S1, yd, ds ? S2 : nullptr, gout, Mo, C, d2, gs, st)));
       if (!ds && pre) gres = S0;
     }
     // conv2
-    MN_TRY(conv_wgrad<P>(bl.conv2, (const TZ*)bl.h, S1, B, st));
+    if (convs[bl.conv2].train) MN_TRY(conv_wgrad<P>(bl.conv2, (const TZ*)bl.h, S1, B, st));
     // h = relu(bn1(y1)) has no residual: its ReLU mask is recomputed from y1 (scale*y+shift > 0),
     // one tensor read less in both backward passes
     const TG* dy2 = S1;
@@ -660,7 +693,8 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
     }
     // conv1 (+ downsample conv): d zin; with fuse_bwd it is gated by the previous block's output ReLU
     // and carries that block's BN2 (+ downsample BN) reductions
-    const bool next_pre = fuse_bwd && bi > 0;
+    // (armed only when block bi - 1 runs: otherwise nothing would consume the sums)
+    const bool next_pre = fuse_bwd && bi > lo;
     EpiBwd e2; memset(&e2, 0, sizeof(e2));
     if (next_pre) {
       BlockL& pb = blocks[bi - 1];
@@ -668,15 +702,14 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
       e2.yd = (pb.convd >= 0) ? (const bf16*)pb.yd : nullptr;
       stats_target = bwd_slot(convs[pb.conv2].bn);      // consumed at the top of the next iteration
     }
-    MN_TRY(conv_wgrad<P>(bl.conv1, zin, S1, B, st));
-    if (ds && bl.ds_fold) {
-      MN_TRY(conv_wgrad<P>(bl.convd, zin, S2, B, st));
+    if (convs[bl.conv1].train) MN_TRY(conv_wgrad<P>(bl.conv1, zin, S1, B, st));
+    if (ds && convs[bl.convd].train) MN_TRY(conv_wgrad<P>(bl.convd, zin, S2, B, st));
+    if (dgrad_in && ds && bl.ds_fold) {
       MN_TRY(conv_dgrad<P>(bl.conv1, S1, nullptr, S0, B, st, next_pre ? &e2 : nullptr, S2, bl.convd));
-    } else if (ds) {
-      MN_TRY(conv_wgrad<P>(bl.convd, zin, S2, B, st));
+    } else if (dgrad_in && ds) {
       MN_TRY(conv_dgrad<P>(bl.convd, S2, nullptr, S0, B, st));
       MN_TRY(conv_dgrad<P>(bl.conv1, S1, S0, S0, B, st, next_pre ? &e2 : nullptr));
-    } else {
+    } else if (dgrad_in) {
       MN_TRY(conv_dgrad<P>(bl.conv1, S1, gres, S0, B, st, next_pre ? &e2 : nullptr));
     }
     stats_target = nullptr;
@@ -684,8 +717,8 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
   }
   bwd_pre = pre;
   // ---- stem: maxpool -> ReLU -> BN -> conv (no input gradient: nothing consumes it) ----
-  if (do_stem) {
-    conv_lo = 0; if (conv_hi < 0) conv_hi = 0;
+  const bool stem = do_stem && bwd_lo < 0, stem_w = stem && convs[0].train;
+  if (stem) {
     S2 = (TG*)ring_next(st);
     BNL& b0 = bns[convs[0].bn];
     const long long M0 = (long long)B * Hc * Wc;
@@ -700,11 +733,10 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
       MN_TRY((launch_bn_bwd_reduce<T, TZ>(S4, (const TZ*)nullptr, (const T*)y0, nullptr, M0, 64, d0.f, bn_accum, bn_counter, st)));
     }
     MN_TRY((launch_bn_bwd_apply<T, TZ, TG>(S4, (const TZ*)nullptr, (const T*)y0, S2, nullptr, nullptr, nullptr, M0, 64, d0, gs, st)));
-    MN_TRY(conv_wgrad<P>(0, (const TZ*)A0, S2, B, st));
+    if (stem_w) MN_TRY(conv_wgrad<P>(0, (const TZ*)A0, S2, B, st));
   }
   MN_TRY(wgrad_join(st));       // every asynchronous wgrad of this part has landed in grads_flat (the stem's in dw_krsc)
-  if (conv_hi >= conv_lo && conv_lo == 0)
-    MN_TRY(launch_unpack_wgrads(d_wdescs, 1, dw_krsc, grads, max_w_elems, st));
+  if (stem_w) MN_TRY(launch_unpack_wgrads(d_wdescs, 1, dw_krsc, grads, max_w_elems, st));
   return 0;
 }
 

@@ -30,12 +30,14 @@ struct ConvL {
   ConvGeom g;             // B filled per call; for the stem this is the 1x1 "GEMM" view over the im2col matrix
   WeightDesc wd;
   int bn;
+  bool train;             // the weight needs a gradient (mapnet_trunk_set_trainable)
 };
 
 struct BNL {
   int C;
   long long g_off, b_off, rm_off, rv_off;
   float *mean, *invstd, *scale, *shift, *coef;   // device, [C] each (coef [3C])
+  bool train_g, train_b;  // gamma / beta need a gradient
 };
 
 struct BlockL {
@@ -58,6 +60,12 @@ struct Net {
   int max_w_elems;
   // parameter offsets of the head
   long long fc_w, fc_b, xyz_w, xyz_b, wpqr_w, wpqr_b;
+  // Which parameters need a gradient (set_trainable; default all).  The backward pass skips the weight gradients of the
+  // others and every input gradient below the lowest layer that trains: bwd_lo is that layer's block, -1 for the stem,
+  // blocks.size() when no conv or BatchNorm parameter trains.
+  bool train_fc_w, train_fc_b, train_xyz_w, train_xyz_b, train_wpqr_w, train_wpqr_b;
+  int bwd_lo;
+  int set_trainable(const uint8_t* host_mask, int n);
 
   // device memory owned by the handle
   std::vector<void*> allocs;

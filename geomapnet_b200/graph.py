@@ -55,6 +55,8 @@ class GraphedTrainStep(object):
         torch.cuda.synchronize(dev)
         from . import _lib
         lc = _lib.lib().mapnet_launch_count()
+        # graph 1 holds the backward schedule of the parameters that train now (frozen ones get no gradient)
+        self.trainable = self.posenet.trainable_mask()
         self.g1 = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.g1):
             self.loss = self._fwd_bwd()
@@ -121,6 +123,12 @@ class GraphedTrainStep(object):
         if hasattr(self.learner, "advance_host_step"):
             self.learner.advance_host_step(-1)
 
+    def check_trainable(self):
+        if self.posenet.trainable_mask() != self.trainable:
+            raise RuntimeError("GraphedTrainStep: requires_grad of the model's parameters changed since the step was "
+                               "captured; the graph would replay the old backward schedule.  Build a new "
+                               "GraphedTrainStep for the new set of trainable parameters.")
+
     def __call__(self, x, targ):
         self.x.copy_(x, non_blocking=True)
         self.t.copy_(targ, non_blocking=True)
@@ -129,6 +137,7 @@ class GraphedTrainStep(object):
     def replay(self, inputs_read=None):
         """One step on what self.x / self.t hold.  inputs_read: a torch.cuda.Event recorded once the step no longer
         reads them (after graph 1), so the next batch can be written there while the optimizer runs."""
+        self.check_trainable()
         self.g1.replay()
         if inputs_read is not None:
             inputs_read.record()
@@ -164,6 +173,8 @@ def train_epoch(loader, model, criterion, optimizer, max_grad_norm=0.0, steps=No
             x0, t0 = torch.empty(xs, device=dev), torch.empty(ts, device=dev)
             ds.assemble(ds.example(n), x0, t0)
             steps[n] = GraphedTrainStep(model, criterion, optimizer, x0, t0, max_grad_norm=max_grad_norm)
+    for st in steps.values():      # captures kept from an earlier epoch: before any batch is assembled
+        st.check_trainable()
     read = {n: torch.cuda.Event() for n in steps}
     ready = torch.cuda.Event()
     losses = []

@@ -55,7 +55,9 @@ class _TrunkFn(torch.autograd.Function):
         if ctx.fwd_id != net._fwd_id:
             raise RuntimeError("geomapnet_b200: backward() must follow the forward() it belongs to "
                                "(activations of one step are kept in a static arena)")
-        grads = net._run_backward(dpred)
+        # needs_input_grad: each parameter's requires_grad at forward time.  Frozen parameters get no gradient, and the
+        # trunk skips their weight gradients and every input gradient below the lowest layer that trains.
+        grads = net._run_backward(dpred, ctx.needs_input_grad[2:])
         return (None, None) + tuple(grads)
 
 
@@ -271,13 +273,18 @@ class PoseNet(nn.Module):
         self._last_shape = (dev, B, H, W)
         return pred
 
-    def _run_backward(self, dpred):
+    def trainable_mask(self):
+        """One flag per parameter, in parameter-table order (= self.parameters()): its requires_grad."""
+        return tuple(bool(p.requires_grad) for p in self._param_list)
+
+    def _run_backward(self, dpred, needs):
         dev, B, H, W = self._last_shape
         trunk = self._trunks[(dev.index, H, W)]
         dpred = dpred.contiguous().float()
+        trunk.set_trainable(needs)
         # two flat gradient buffers: never write into the one p.grad currently aliases
         sel = self._gsel
-        g0 = self._param_list[0].grad
+        g0 = next((p.grad for p, n in zip(self._param_list, needs) if n), None)
         for cand in (sel, 1 - sel):
             buf = self._gflat[cand]
             if buf is None or buf.device != dev:
@@ -309,7 +316,7 @@ class PoseNet(nn.Module):
         for name, kind, shape, off in self._table:
             if kind == 0:
                 n = self._by_name[name][5]
-                out.append(self._pview(gbuf, name, off, n, shape))
+                out.append(self._pview(gbuf, name, off, n, shape) if needs[len(out)] else None)
         return out
 
     # ------------------------------------------------------- flat-buffer API

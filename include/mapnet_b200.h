@@ -98,6 +98,15 @@ int mapnet_backward_part(mapnet_trunk_t* h, int part, const float* dpred, const 
                          int filter_nans, void* stream);
 int mapnet_grad_part_range(mapnet_trunk_t* h, int part, int64_t* host_lo, int64_t* host_hi);
 
+/* Which trainable entries (kind 0 of the parameter table, in table order) need a gradient. n must equal the number
+ * of kind-0 entries. Applies to every later mapnet_backward / mapnet_backward_part on this handle, until set again.
+ * Default: all 1 (the full backward pass). Host-only, no launch: a CUDA graph captures the schedule of the mask in force.
+ * The pass then skips the weight gradient of every frozen conv and head layer, and every input gradient below the
+ * lowest layer that trains (torch's requires_grad_(False) semantics). The grads_flat entries of frozen parameters are 0.
+ * A frozen BatchNorm still passes its input gradient through; its running statistics follow the forward as before.
+ * (Added in ABI version 2, backward compatible.) */
+int mapnet_trunk_set_trainable(mapnet_trunk_t* h, const uint8_t* host_mask, int n);
+
 /* ---- fused criterion forward+backward.  s4 = device (sax,saq,srx,srq).
  * Outputs: loss[1], dpred (same shape as pred), ds4[4] = d loss / d s4. */
 int mapnet_loss_fwd_bwd(int mode, const float* pred, const float* targ, int N, int T_pred, int T_targ,
