@@ -72,6 +72,8 @@ def lib():
     L.mapnet_rmsprop_step_dev.restype = c_int
     L.mapnet_test_conv.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                    c_void_p, c_void_p, c_void_p, c_void_p]
+    L.mapnet_test_conv_ex.argtypes = [c_int] * 9 + [c_void_p] * 4 + [c_float, c_void_p, c_void_p]
+    L.mapnet_test_conv_ex.restype = c_int
     L.mapnet_test_stem.argtypes = [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     L.mapnet_test_stem.restype = c_int
     L.mapnet_test_dgrad_shortcut.argtypes = [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -155,7 +157,7 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_frame_cache_create", "mapnet_frame_cache_ingest", "mapnet_frame_cache_assemble",
             "mapnet_frame_cache_destroy", "mapnet_infer_calibrate", "mapnet_infer_act_scales", "mapnet_test_conv_fp8",
             "mapnet_test_bn_forward", "mapnet_test_bn_backward", "mapnet_test_stem_pool", "mapnet_test_gap",
-            "mapnet_trunk_set_trainable"]
+            "mapnet_trunk_set_trainable", "mapnet_test_conv_ex"]
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 
 

@@ -185,15 +185,43 @@ int mapnet_test_conv(int precision, int kind, int B, int Hi, int Wi, int Ci, int
     if (kind == 1) return launch_conv_simt_dgrad<bf16>(g, (const bf16*)in0, (const float*)wmat, nullptr, (bf16*)out, st);
     return launch_conv_simt_wgrad<bf16>(g, (const bf16*)in0, (const bf16*)in1, (float*)out, st);
   }
-  if (precision == PREC_TC_SPLIT) {
-    // strict tensor-core mode: fp32 NHWC tensors and fp32 K-major weight matrices in (as for PREC_FP32), fp32 out;
-    // the operands are cut into fp16 hi / lo planes here (the training step's element-wise kernels write that form)
-    g.split = 1;
-    const long long n_in = (long long)B * Hi * Wi * Ci, n_out = (long long)B * g.Ho * g.Wo * Co;
-    const int KK = k * k;
-    void *s0 = nullptr, *s1 = nullptr, *sw = nullptr;
-    TcConvPlan* plan = nullptr;
-    auto body = [&]() -> int {
+  MN_CHECK(precision == PREC_BF16_TC || precision == PREC_TC_SPLIT, "test_conv: bad precision");
+  return mapnet_test_conv_ex(precision, kind, B, Hi, Wi, Ci, Co, k, stride, in0, in1, wmat, nullptr, 0.f, out, stream);
+}
+
+// The tensor-core engines of mapnet_test_conv, plus the two strict-mode features the trunk's backward uses:
+// a dgrad residual (strict mode: fp32; it may be `out` itself, as in conv_dgrad(conv1, S1, S0, S0)) and the gradient
+// out-scale (tc_plan_set_out_scale), a device scalar multiplied into the accumulators before they are stored.
+int mapnet_test_conv_ex(int precision, int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride,
+                        const void* in0, const void* in1, const void* wmat, const void* residual, float out_scale,
+                        void* out, void* stream) {
+  MN_CHECK(precision == PREC_BF16_TC || precision == PREC_TC_SPLIT, "test_conv_ex: precision %d is not a tensor-core "
+           "training precision (bf16 = %d or tc_split = %d)", precision, PREC_BF16_TC, PREC_TC_SPLIT);
+  MN_CHECK(kind >= 0 && kind <= 2, "test_conv_ex: kind %d outside [0, 2]", kind);
+  MN_CHECK(B >= 1 && Hi >= 1 && Wi >= 1 && (k == 1 || k == 3) && (stride == 1 || stride == 2) && Ci % 64 == 0 &&
+           Co % 64 == 0 && Ci > 0 && Co > 0, "test_conv_ex: bad shape (B %d, %dx%d, Ci %d, Co %d, k %d, stride %d)", B, Hi,
+           Wi, Ci, Co, k, stride);
+  MN_CHECK(in0 && out && (kind == 2 ? in1 != nullptr : wmat != nullptr), "test_conv_ex: null argument");
+  MN_CHECK(residual == nullptr || kind == 1, "test_conv_ex: a residual is a dgrad feature");
+  MN_CHECK(out_scale == 0.f || (precision == PREC_TC_SPLIT && kind >= 1 && isfinite(out_scale) && out_scale > 0.f),
+           "test_conv_ex: out_scale %g: a positive gradient scale of a strict-mode dgrad / wgrad, or 0", out_scale);
+  MN_TRY(require_device());
+  ConvGeom g;
+  g.B = B; g.Hi = Hi; g.Wi = Wi; g.Ci = Ci; g.Co = Co; g.KH = g.KW = k; g.stride = stride; g.pad = (k - 1) / 2;
+  g.Ho = (Hi + 2 * g.pad - k) / stride + 1; g.Wo = (Wi + 2 * g.pad - k) / stride + 1;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long n_in = (long long)B * Hi * Wi * Ci, n_out = (long long)B * g.Ho * g.Wo * Co;
+  const int KK = k * k;
+  void *s0 = nullptr, *s1 = nullptr, *sw = nullptr;
+  float* d_scale = nullptr;
+  TcConvPlan* plan = nullptr;
+  auto body = [&]() -> int {
+    const void *x0 = in0, *x1 = in1, *w = wmat;
+    if (precision == PREC_TC_SPLIT) {
+      // strict tensor-core mode: fp32 NHWC tensors and fp32 K-major weight matrices in (as for PREC_FP32), fp32 out
+      // (and residual); the operands are cut into fp16 hi / lo planes here (the training step's element-wise kernels
+      // write that form)
+      g.split = 1;
       const long long n0 = (kind == 1) ? n_out : n_in;
       MN_CUDA(cudaMalloc(&s0, (size_t)n0 * 4));
       MN_TRY(launch_split_tensor((const float*)in0, s0, n0, st));
@@ -205,36 +233,37 @@ int mapnet_test_conv(int precision, int kind, int B, int Hi, int Wi, int Ci, int
         if (kind == 0) MN_TRY(launch_split_weight_matrix((const float*)wmat, sw, Co, KK, Ci, st));
         else MN_TRY(launch_split_weight_matrix((const float*)wmat, sw, Ci, KK, Co, st));
       }
-      MN_TRY(tc_plan_create(&plan, g, kind, (const bf16*)sw));
-      MN_TRY(tc_conv_run(plan, (const bf16*)s0, (const bf16*)s1, nullptr, out, st));
-      MN_CUDA(cudaStreamSynchronize(st));
-      return 0;
-    };
-    const int r = body();
-    if (plan) tc_plan_destroy(plan);
-    cudaFree(s0); cudaFree(s1); cudaFree(sw);
-    return r;
-  }
-  MN_CHECK(precision == PREC_BF16_TC, "test_conv: bad precision");
-  TcConvPlan* plan = nullptr;
-  MN_TRY(tc_plan_create(&plan, g, kind, (const bf16*)wmat));
-  int r = tc_conv_run(plan, (const bf16*)in0, (const bf16*)in1, nullptr, out, st);
-  if (r == 0) { cudaError_t e = cudaStreamSynchronize(st); if (e != cudaSuccess) { set_last_error("test_conv: %s", cudaGetErrorString(e)); r = 1; } }
-  tc_plan_destroy(plan);
+      x0 = s0; x1 = s1; w = sw;
+    }
+    MN_TRY(tc_plan_create(&plan, g, kind, (const bf16*)w));
+    if (out_scale != 0.f) {
+      MN_CUDA(cudaMalloc((void**)&d_scale, sizeof(float)));
+      MN_CUDA(cudaMemcpyAsync(d_scale, &out_scale, sizeof(float), cudaMemcpyHostToDevice, st));
+      tc_plan_set_out_scale(plan, d_scale);
+    }
+    MN_TRY(tc_conv_run(plan, (const bf16*)x0, (const bf16*)x1, (const bf16*)residual, out, st));
+    MN_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  };
+  const int r = body();
+  if (plan) tc_plan_destroy(plan);
+  cudaFree(s0); cudaFree(s1); cudaFree(sw); cudaFree(d_scale);
   return r;
 }
 
-// JSON description of the plan the tensor-core engines would use for this conv (no device needed)
-int mapnet_test_plan_describe(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, int with_shortcut,
+// JSON description of the plan the tensor-core engines would use for this conv (no device needed).  flags: bit 0 folds
+// the downsample shortcut into a stride-2 dgrad; bit 1 describes the strict-mode (split-operand) plan instead of bf16's
+int mapnet_test_plan_describe(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, int flags,
                               char* buf, int cap) {
   ConvGeom g;
   g.B = B; g.Hi = Hi; g.Wi = Wi; g.Ci = Ci; g.Co = Co; g.KH = g.KW = k; g.stride = stride; g.pad = (k - 1) / 2;
   g.Ho = (Hi + 2 * g.pad - k) / stride + 1; g.Wo = (Wi + 2 * g.pad - k) / stride + 1;
+  if (flags & 2) g.split = 1;
   TcConvPlan* plan = nullptr;
   static const bf16 dummy[8] = {};
   MN_TRY(tc_plan_create(&plan, g, kind, dummy));
   int r = 0;
-  if (with_shortcut) r = tc_plan_add_shortcut(plan, dummy);
+  if (flags & 1) r = tc_plan_add_shortcut(plan, dummy);
   if (r == 0) r = tc_plan_describe(plan, buf, cap);
   tc_plan_destroy(plan);
   return r;

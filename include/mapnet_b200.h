@@ -236,10 +236,18 @@ int mapnet_profile_read(mapnet_trunk_t* h, double* host_ms3, double* host_flops3
 /* ---- unit entry points used by the parity tests (tests/test_gpu_kernels.py) */
 int mapnet_test_conv(int precision, int kind /*0 fprop 1 dgrad 2 wgrad*/, int B, int Hi, int Wi, int Ci, int Co,
                      int k, int stride, const void* in0, const void* in1, const void* wmat, void* out, void* stream);
+/* mapnet_test_conv's tensor-core engines (precision bf16 or tc_split) plus, for dgrad, a residual added before the
+ * store (out's type and shape; it may be `out` itself, as in the trunk's strict-mode downsampling blocks), and for
+ * strict-mode dgrad / wgrad a gradient out-scale multiplied into the accumulators before they are stored (uploaded to
+ * a device scalar; 0 = none).  Arguments are checked before the device is touched. */
+int mapnet_test_conv_ex(int precision, int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride,
+                        const void* in0, const void* in1, const void* wmat, const void* residual, float out_scale,
+                        void* out, void* stream);
 
 /* host-only: the tile / parity-class / filter-tap plan of the tensor-core engines for one conv, as JSON
- * (tests/test_tc_plan.py replays it on the CPU against torch's convolutions; kind 0 fprop, 1 dgrad, 2 wgrad) */
-int mapnet_test_plan_describe(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, int with_shortcut,
+ * (tests/test_tc_plan.py replays it on the CPU against torch's convolutions; kind 0 fprop, 1 dgrad, 2 wgrad).
+ * flags: bit 0 folds the downsample shortcut into a 3x3/s2 dgrad; bit 1 describes the strict-mode (tc_split) plan. */
+int mapnet_test_plan_describe(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, int flags,
                               char* buf, int cap);
 
 /* the tensor-core dgrad of a downsampling BasicBlock's two input-side convs in ONE launch, as the trunk runs it:

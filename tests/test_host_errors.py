@@ -161,3 +161,34 @@ def test_element_wise_test_entry_points_fail_with_a_message(built):
     for fn, *args in calls:
         rc, msg = _rc_and_message(fn, *args)
         assert rc != 0 and "no CUDA device" in msg, (fn.__name__, rc, msg)
+
+
+def test_conv_ex_test_entry_point_fails_with_a_message(built):
+    """mapnet_test_conv_ex checks its arguments before it touches the device (the pointers below are never
+    dereferenced); on a host without a device a well-formed call fails with a message too."""
+    from geomapnet_b200 import _lib
+    L = _lib.lib()
+    buf = np.zeros(64, dtype=np.float32)
+    h = buf.ctypes.data
+    ex = lambda prec, kind, Ci, k, stride, in1, wmat, res, scale: _rc_and_message(
+        L.mapnet_test_conv_ex, prec, kind, 2, 8, 8, Ci, 64, k, stride, h, in1, wmat, res, scale, h, None)
+    cases = [
+        (ex(0, 0, 64, 3, 1, None, h, None, 0.0), "not a tensor-core training precision"),   # fp32 is mapnet_test_conv's
+        (ex(1, 3, 64, 3, 1, None, h, None, 0.0), "kind 3"),
+        (ex(1, 0, 96, 3, 1, None, h, None, 0.0), "bad shape"),                               # 64-channel k-blocks
+        (ex(1, 0, 64, 5, 1, None, h, None, 0.0), "bad shape"),
+        (ex(1, 2, 64, 3, 1, None, None, None, 0.0), "null argument"),                        # wgrad needs dy
+        (ex(1, 0, 64, 3, 1, None, None, None, 0.0), "null argument"),                        # fprop needs weights
+        (ex(1, 0, 64, 3, 1, None, h, h, 0.0), "a residual is a dgrad feature"),
+        (ex(1, 1, 64, 3, 1, None, h, None, 0.5), "out_scale"),                               # bf16 has no gradient scale
+        (ex(3, 0, 64, 3, 1, None, h, None, 0.5), "out_scale"),                               # nor does strict fprop
+        (ex(3, 1, 64, 3, 1, None, h, None, -0.5), "out_scale"),
+        (ex(3, 2, 64, 3, 1, h, None, None, float("inf")), "out_scale"),
+    ]
+    for (rc, msg), want in cases:
+        assert rc != 0 and want in msg, (rc, msg, want)
+    if torch.cuda.is_available():
+        return
+    for prec, kind, in1, wmat, res, scale in ((1, 0, None, h, None, 0.0), (3, 1, None, h, h, 0.25), (3, 2, h, None, None, 0.25)):
+        rc, msg = ex(prec, kind, 64, 3, 2, in1, wmat, res, scale)
+        assert rc != 0 and "no CUDA device" in msg, (prec, kind, rc, msg)
