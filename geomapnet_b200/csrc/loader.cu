@@ -11,6 +11,7 @@
 #include "preprocess_core.h"
 #include "jitter_core.h"
 #include "pose_math.h"
+#include "pose_post.cuh"
 
 #include "../../include/mapnet_b200.h"
 
@@ -67,6 +68,39 @@ k_loader_assemble(const uint8_t* __restrict__ frames, const int* __restrict__ fr
     for (int k = 0; k < 4; ++k) jit_apply(P.order[k], P.factor[P.order[k]], gray_mean, shift, px);
 #pragma unroll
     for (int c = 0; c < 3; ++c) dst[c * npix + i] = pre_normalize(px[c], mean[c], stdev[c]);
+  }
+}
+
+// ---- evaluation windows (inference.evaluate_sequence): per-frame predictions -> the [L,T] windows scripts/eval.py
+// post-processes.  Rows 0 .. n_win*T-1: pred7 / targ7 of window slot r; rows n_win*T .. +n_vo-1: VO k.  Translations
+// stay normalised (PGO works on them), the quaternions are post_qexp of the float32 log q, as mapnet_pose_post.
+__device__ __forceinline__ posemath::Pose6 ld_pose6(const float* p) {
+  posemath::Pose6 o;
+  o.t = posemath::v3(p[0], p[1], p[2]); o.l = posemath::v3(p[3], p[4], p[5]);
+  return o;
+}
+__device__ __forceinline__ void st_pose7(const float* p6, double* o7) {
+  o7[0] = (double)p6[0]; o7[1] = (double)p6[1]; o7[2] = (double)p6[2];
+  post_qexp(p6[3], p6[4], p6[5], o7 + 3);
+}
+
+__global__ void __launch_bounds__(128)
+k_eval_windows(const float* __restrict__ pred6, const float* __restrict__ poses, const float* __restrict__ vo_poses,
+               const int* __restrict__ frame, const int* __restrict__ slot, int n_rows, const TargRow* __restrict__ vo_rows,
+               int n_vo, double* __restrict__ pred7, double* __restrict__ targ7, double* __restrict__ vos7) {
+  pdl_prologue();
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < n_rows) {
+    st_pose7(pred6 + 6LL * slot[r], pred7 + 7LL * r);
+    st_pose7(poses + 6LL * frame[r], targ7 + 7LL * r);
+  } else if (r < n_rows + n_vo) {
+    const int k = r - n_rows;
+    const TargRow p = vo_rows[k];
+    // calc_vos_safe / calc_vos_safe_fc (common/pose_utils.py:276-304) on the VO library's float32 poses, as the
+    // MFOnline targets of k_loader_assemble
+    const posemath::Pose6 v = posemath::calc_vo_logq_safe(ld_pose6(vo_poses + 6LL * p.a), ld_pose6(vo_poses + 6LL * p.b));
+    const float v6[6] = {v.t.x, v.t.y, v.t.z, v.l.x, v.l.y, v.l.z};
+    st_pose7(v6, vos7 + 7LL * k);
   }
 }
 
@@ -195,6 +229,38 @@ int mapnet_frame_cache_assemble(mapnet_frame_cache_t* h, int n, const int32_t* f
             (const TargRow*)(ds + h->off_rows), n_targ, targ_out);
   MN_LAUNCH_CHECK();
   MN_CUDA(cudaEventRecord(h->done[s], st));
+  return 0;
+}
+
+int mapnet_eval_windows(const float* pred6, int n_pred, const float* poses, const float* vo_poses, int n_poses,
+                        const int32_t* frame, const int32_t* slot, int n_rows, const int32_t* vo_rows, int n_vo,
+                        double* pred7, double* targ7, double* vos7, void* stream) {
+  MN_CHECK(pred6 != nullptr && poses != nullptr && frame != nullptr && slot != nullptr && pred7 != nullptr &&
+           targ7 != nullptr, "eval_windows: null argument");
+  MN_CHECK(n_rows >= 1 && n_pred >= 1 && n_poses >= 1 && n_vo >= 0, "eval_windows: bad count");
+  MN_CHECK(n_vo == 0 || (vo_poses != nullptr && vo_rows != nullptr && vos7 != nullptr),
+           "eval_windows: %d VO rows need vo_poses, vo_rows and vos7", n_vo);
+  MN_CHECK((long long)n_rows + n_vo < (1LL << 31), "eval_windows: %d + %d rows", n_rows, n_vo);
+  for (int r = 0; r < n_rows; ++r)
+    MN_CHECK(frame[r] >= 0 && frame[r] < n_poses && slot[r] >= 0 && slot[r] < n_pred,
+             "eval_windows: row %d = (frame %d, slot %d) outside the %d poses / %d predictions", r, frame[r], slot[r],
+             n_poses, n_pred);
+  for (int k = 0; k < 2 * n_vo; ++k)
+    MN_CHECK(vo_rows[k] >= 0 && vo_rows[k] < n_poses, "eval_windows: VO row %d = (%d, %d) outside the %d poses", k / 2,
+             vo_rows[k & ~1], vo_rows[k | 1], n_poses);
+  MN_CHECK(device_memory(pred6) && device_memory(poses) && device_memory(pred7) && device_memory(targ7) &&
+           (n_vo == 0 || (device_memory(vo_poses) && device_memory(vos7))), "eval_windows: tensors must be device memory");
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t bytes = (2 * (size_t)n_rows + 2 * (size_t)n_vo) * sizeof(int32_t);
+  int32_t* d = nullptr;                // the index tables, stream-ordered: freed once the kernel has read them
+  MN_CUDA(cudaMallocAsync((void**)&d, bytes, st));
+  MN_CUDA(cudaMemcpyAsync(d, frame, (size_t)n_rows * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  MN_CUDA(cudaMemcpyAsync(d + n_rows, slot, (size_t)n_rows * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (n_vo > 0) MN_CUDA(cudaMemcpyAsync(d + 2 * n_rows, vo_rows, 2 * (size_t)n_vo * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  MN_LAUNCH(k_eval_windows, (int)cdiv((long long)n_rows + n_vo, 128), 128, 0, st, pred6, poses, vo_poses, (const int*)d,
+            (const int*)(d + n_rows), n_rows, (const TargRow*)(d + 2 * n_rows), n_vo, pred7, targ7, vos7);
+  MN_LAUNCH_CHECK();
+  MN_CUDA(cudaFreeAsync(d, st));
   return 0;
 }
 

@@ -25,6 +25,7 @@
 #include <math.h>
 
 #include "kernels.h"
+#include "pose_post.cuh"
 #include "../../include/mapnet_b200.h"
 
 namespace mapnet {
@@ -268,17 +269,12 @@ __global__ void k_pose_post(const float* __restrict__ p6, double* __restrict__ o
   pdl_prologue();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  // numpy on the float32 row (eval.py:166): n = linalg.norm(q); hstack((cos n, sinc(n / pi) * q)) -- float32 arithmetic
-  const float x = p6[6 * i + 3], y = p6[6 * i + 4], z = p6[6 * i + 5];
-  const float nn = sqrtf(x * x + y * y + z * z);
-  const float sc = (nn == 0.f) ? 1.f : (float)(sin((double)nn) / (double)nn);
   const double ms[3] = {m0, m1, m2}, ss[3] = {s0, s1, s2};
   for (int k = 0; k < 3; ++k) {
     const double t = (double)p6[6 * i + k];
     out7[7 * i + k] = unnormalize ? t * ss[k] + ms[k] : t;
   }
-  out7[7 * i + 3] = (double)(float)cos((double)nn);
-  out7[7 * i + 4] = (double)(sc * x); out7[7 * i + 5] = (double)(sc * y); out7[7 * i + 6] = (double)(sc * z);
+  post_qexp(p6[6 * i + 3], p6[6 * i + 4], p6[6 * i + 5], out7 + 7 * i + 3);
 }
 }  // namespace mapnet
 

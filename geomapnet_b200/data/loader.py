@@ -112,6 +112,31 @@ class ItemLayout(object):
         rows = np.ascontiguousarray(np.concatenate([it[2] for it in items]), dtype=np.int32)
         return fr, jit, rows, len(items)
 
+    def eval_tables(self, unique=True, vo_fc=False):
+        """The windows scripts/eval.py evaluates: one per item, in index order, as DataLoader(shuffle=False) draws them
+        (with variable_skip, np.random is consumed as in the reference's loop).  Returns host int32 tables:
+          windows [L,T]   the frame of every window slot (T = 1 for single frames);
+          frames [F]      the frames that go through the network, in that order;
+          slots [L,T]     the row of `frames` whose prediction fills each window slot;
+          vo_rows [L,E,2] the frame pairs of each window's VOs: consecutive slots (calc_vos_safe, E = T-1) or every
+                          pair i<j in row-major order (vo_fc: calc_vos_safe_fc, E = T(T-1)/2).
+        unique=True: every distinct frame once, in frame order.  unique=False: every window's frames in window order
+        (frames = windows.ravel()), what a network that draws dropout masks at eval needs to see."""
+        if self.online or self.jitter is not None:
+            raise ValueError("evaluation windows need a single-frame or MF layout without ColorJitter")
+        windows = np.stack([self.item(i)[0] for i in range(len(self))]).astype(np.int32)
+        L, T = windows.shape
+        if unique:
+            frames, inv = np.unique(windows, return_inverse=True)
+            slots = inv.reshape(L, T)
+        else:
+            frames, slots = windows.reshape(-1), np.arange(L * T).reshape(L, T)
+        pairs = [(i, j) for i in range(T) for j in range(i + 1, T)] if vo_fc else [(i, i + 1) for i in range(T - 1)]
+        pairs = np.asarray(pairs, dtype=np.int64).reshape(-1, 2)
+        vo_rows = windows[:, pairs] if len(pairs) else np.zeros((L, 0, 2), np.int32)
+        return dict(windows=windows, frames=np.ascontiguousarray(frames, dtype=np.int32),
+                    slots=np.ascontiguousarray(slots, dtype=np.int32), vo_rows=np.ascontiguousarray(vo_rows, dtype=np.int32))
+
     def example(self, n):
         """A batch record of items 0, 1, ... (n of them) that makes no random draw (fixed skips, no ColorJitter): an
         input for warm-up and capture that leaves the RNG streams where the reference's loop has them."""
@@ -126,13 +151,15 @@ class ItemLayout(object):
 class DeviceDataset(ItemLayout):
     def __init__(self, frames, mean, std, poses=None, color_jitter=0.0, steps=None, skip=1, variable_skip=False,
                  online=False, val_frames=None, val_poses=None, gps_mode=False, size=256, max_batch=64, chunk=64,
-                 device=None):
+                 device=None, vo_poses=None):
         """frames: uint8 [L,H,W,3] (RGB, numpy or torch) or a reference-style dataset (see _frames_and_poses); poses:
         [L,6] float32 targets.  mean / std: as handed to transforms.Normalize.  color_jitter: the ColorJitter of
         scripts/train.py:121-124 (brightness = contrast = saturation = color_jitter, hue = 0.5) when > 0.
         steps=None: single frames (posenet); steps=T: MF(steps, skip, variable_skip) tuples; online=True: MFOnline,
         with the validation sequence val_frames and its VO-library ("real") poses val_poses, gps_mode as the reference.
-        max_batch: the largest batch (in items) assemble() takes."""
+        max_batch: the largest batch (in items) assemble() takes.  vo_poses: [L,6] float32, the VO-library ("real")
+        pose of every frame, from which evaluation derives the windows' VOs as MF(real=True, include_vos=True) does
+        (dataset_loaders/composite.py:47-97; the poses stay the targets, as its gt_dset's)."""
         frames, poses = _frames_and_poses(frames, poses)
         if online:
             val_frames, val_poses = _frames_and_poses(val_frames, val_poses)
@@ -146,6 +173,11 @@ class DeviceDataset(ItemLayout):
             shapes.add(tuple(f.shape[1:3]))
         if len(shapes) != 1:
             raise ValueError("all frames must have one size, got %s" % sorted(shapes))
+        if vo_poses is not None:
+            if online:
+                raise ValueError("vo_poses are for evaluation windows; MFOnline takes its VO poses as val_poses")
+            if tuple(np.shape(vo_poses)) != (frames.shape[0], 6):
+                raise ValueError("expected vo_poses [%d,6], got %s" % (frames.shape[0], np.shape(vo_poses)))
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         if self.device.type != "cuda":
             raise RuntimeError("geomapnet_b200.data.DeviceDataset has no CPU path: device must be CUDA")
@@ -160,6 +192,8 @@ class DeviceDataset(ItemLayout):
             raise ValueError("std must be positive, got %s" % (self.std,))
         self.poses = torch.as_tensor(np.concatenate([np.asarray(p, dtype=np.float32) for _, p in seqs]),
                                      dtype=torch.float32).to(self.device).contiguous()
+        self.vo_poses = None if vo_poses is None else torch.as_tensor(
+            np.asarray(vo_poses, dtype=np.float32)).to(self.device).contiguous()
         # the cache: every frame resized once, in chunks (training sequence first, then the validation sequence)
         self.max_batch = int(max_batch)
         if self.max_batch < 1:
@@ -213,6 +247,21 @@ class DeviceDataset(ItemLayout):
                 self.poses.shape[0], rows.ctypes.data, rows.shape[0], self.mean.ctypes.data_as(fp),
                 self.std.ctypes.data_as(fp), x_out.data_ptr(), targ_out.data_ptr(), _lib.stream_ptr()),
                 "mapnet_frame_cache_assemble")
+
+
+    def assemble_frames(self, frames, x_out):
+        """Frames `frames` (host int32 [n], n <= max_batch * frames_per_item) of the cache into the float32 CUDA tensor
+        x_out [n,3,Ho,Wo] (ToTensor + Normalize, no ColorJitter), on the current stream: one launch."""
+        fr = np.ascontiguousarray(frames, dtype=np.int32)
+        n = fr.shape[0]
+        if not (torch.is_tensor(x_out) and x_out.is_cuda and x_out.dtype == torch.float32 and x_out.is_contiguous()
+                and tuple(x_out.shape) == (n, 3, self.Ho, self.Wo) and x_out.device == self.device):
+            raise ValueError("x_out must be a contiguous float32 tensor %s on %s" % ((n, 3, self.Ho, self.Wo), self.device))
+        fp = ctypes.POINTER(ctypes.c_float)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().mapnet_frame_cache_assemble(
+                self.h, n, fr.ctypes.data, None, None, 0, None, 0, self.mean.ctypes.data_as(fp),
+                self.std.ctypes.data_as(fp), x_out.data_ptr(), None, _lib.stream_ptr()), "mapnet_frame_cache_assemble")
 
 
 class _Items(torch.utils.data.Dataset):

@@ -5,7 +5,8 @@ Host-side mirror of /root/reference/scripts/eval.py:137-199.  The reference runs
 frame and keeps the middle prediction of each tuple.  Here: ``predict`` runs the eval-mode forward in batches of tuples
 through the same fprop engines as training (BatchNorm running statistics, no dropout at eval -- see note), ``post`` does
 qexp + un-normalisation for all poses in one launch, ``pgo`` optimises all windows in one launch (csrc/pgo.cu), and
-``pose_errors`` gives the translation / rotation errors eval.py prints (:193-199).
+``pose_errors`` gives the translation / rotation errors eval.py prints (:193-199).  ``evaluate_sequence`` runs the
+whole loop from a device-resident sequence (data.DeviceDataset), each distinct frame through the network once.
 
 Note on dropout: models/posenet.py:68-69 calls F.dropout without ``training=``, so the reference drops features at eval
 time too whenever droprate > 0; scripts/eval.py builds the model with the ini's dropout.  ``predict`` follows the
@@ -19,7 +20,7 @@ import torch
 from . import _lib
 from .common.pgo import optimize_pose_windows
 
-__all__ = ["Predictor", "predict", "post", "pgo", "pose_errors", "evaluate_tuples"]
+__all__ = ["Predictor", "predict", "post", "pgo", "pose_errors", "evaluate_tuples", "evaluate_sequence"]
 
 
 class Predictor(object):
@@ -107,16 +108,17 @@ class Predictor(object):
             self._engines[(H, W)] = eng
         return eng
 
-    def _run(self, xb):
-        """pred [B,6] for frames xb [B,3,H,W] (B <= max_batch): graph replay, captured on the first call of a shape."""
-        B, _, H, W = xb.shape
-        key = (B, H, W)
+    def _graph(self, B, H, W, xb=None, slot=0):
+        """(CUDA graph, static input [B,3,H,W], static output [B,6]) of one batch shape, captured on first use after an
+        eager run on xb (zeros when None).  slot > 0: a further graph of the same shape with its own input buffer."""
+        key = (B, H, W) if slot == 0 else (B, H, W, slot)
         g = self._graphs.get(key)
         if g is None:
             eng = self._engine(H, W)
-            xs = torch.empty((B, 3, H, W), dtype=torch.float32, device=self.device)
+            xs = torch.zeros((B, 3, H, W), dtype=torch.float32, device=self.device)
             ps = torch.empty((B, 6), dtype=torch.float32, device=self.device)
-            xs.copy_(xb)
+            if xb is not None:
+                xs.copy_(xb)
             cur = torch.cuda.current_stream(self.device)
             side = torch.cuda.Stream(self.device)
             side.wait_stream(cur)
@@ -127,7 +129,11 @@ class Predictor(object):
             with torch.cuda.graph(graph):
                 eng.forward(xs, ps, self.droprate, self.seed)
             g = self._graphs[key] = (graph, xs, ps)
-        graph, xs, ps = g
+        return g
+
+    def _run(self, xb):
+        """pred [B,6] for frames xb [B,3,H,W] (B <= max_batch): graph replay, captured on the first call of a shape."""
+        graph, xs, ps = self._graph(xb.shape[0], xb.shape[2], xb.shape[3], xb)
         xs.copy_(xb)
         graph.replay()
         return ps.clone()
@@ -231,3 +237,140 @@ def evaluate_tuples(model, x, targ6, vos7=None, pose_m=None, pose_s=None, batch=
     p_mid, t_mid = pred[:, mid], targ[:, mid]
     t_err, q_err = pose_errors(p_mid, t_mid)
     return dict(pred7=p_mid, targ7=t_mid, t_err=t_err, q_err=q_err)
+
+
+def _frame_runners(pr, net, sizes, n_slots, H, W, dev):
+    """{(frames, slot): (static input [n,3,H,W], run(), static output [n,6])}: Predictor graphs, or the live eval forward
+    of `net` on plain buffers when there is no Predictor."""
+    runners = {}
+    for n in sizes:
+        for s in range(n_slots):
+            if pr is not None:
+                graph, xs, ps = pr._graph(n, H, W, slot=s)
+                runners[(n, s)] = (xs, graph.replay, ps)
+            else:
+                xs = torch.empty((n, 3, H, W), dtype=torch.float32, device=dev)
+                ps = torch.empty((n, 6), dtype=torch.float32, device=dev)
+                runners[(n, s)] = (xs, (lambda xs=xs, ps=ps: ps.copy_(net(xs))), ps)
+    return runners
+
+
+@torch.no_grad()
+def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, **sigmas):
+    """The whole loop of scripts/eval.py:117-199 over a device-resident sequence: the windows of MF(steps, skip,
+    variable_skip, no_duplicates=False) -- or single frames when dataset.steps is None -- one per frame index, in index
+    order.  Returns what evaluate_tuples returns (pred7 [L,7], targ7 [L,7], t_err, q_err: the middle frame of each
+    window) and n_frames, the number of frames that went through the network.
+
+    model: a PoseNet / MapNet or a Predictor (any precision).  A live model whose precision a Predictor supports is
+    run by a temporary Predictor; any other runs its own eval forward.  dataset: a DeviceDataset without ColorJitter;
+    its poses are the targets.  With dataset.vo_poses, each window's VOs (calc_vos_safe of the VO-library poses, or
+    calc_vos_safe_fc when vo_fc) drive the pose-graph optimisation, with the covariances `sigmas` (sax, saq, srx, srq).
+
+    In eval mode BatchNorm uses running statistics, so a frame's pose does not depend on the rest of its window:
+    with droprate == 0 every distinct frame goes through the network once, in chunks of the Predictor's max_batch,
+    and the windows are rebuilt from the per-frame poses.  With droprate > 0 (the reference's dropout is active at
+    eval) each window's frames go through the network together, one window per forward, as in the reference's loop.
+    Chunk k+1 is assembled on a side stream while chunk k runs.  variable_skip draws from np.random as the
+    reference's DataLoader(shuffle=False) does."""
+    from .data.loader import DeviceDataset
+    ds = dataset
+    if not isinstance(ds, DeviceDataset):
+        raise TypeError("evaluate_sequence needs a geomapnet_b200.data.DeviceDataset, got %s" % type(ds).__name__)
+    if ds.jitter is not None:
+        raise ValueError("evaluate_sequence: the dataset applies ColorJitter; build it with color_jitter=0")
+    if ds.online:
+        raise ValueError("evaluate_sequence: MFOnline datasets are not evaluation sequences")
+    if not ds.h:
+        raise RuntimeError("evaluate_sequence: the dataset is closed")
+    pr = model if isinstance(model, Predictor) else None
+    net = pr.net if pr is not None else (model.mapnet if hasattr(model, "mapnet") else model)
+    dev = pr.device if pr is not None else next(net.parameters()).device
+    if dev != ds.device:
+        raise RuntimeError("geomapnet_b200.inference.evaluate_sequence has no CPU path: the model is on %s and the "
+                           "dataset on %s; both must be on one CUDA device" % (dev, ds.device))
+    if pr is not None and pr._params is None:
+        raise RuntimeError("Predictor is closed")
+    if pr is not None and pr._calib is not None and tuple(pr._calib.shape[-2:]) != (ds.Ho, ds.Wo):
+        raise ValueError("this fp8 Predictor was calibrated at %dx%d, the dataset's frames are %dx%d"
+                         % (pr._calib.shape[-2], pr._calib.shape[-1], ds.Ho, ds.Wo))
+    vo = ds.vo_poses is not None
+    T = 1 if ds.steps is None else ds.steps
+    if vo and T < 2:
+        raise ValueError("pose-graph optimisation needs windows of >= 2 frames (dataset.steps)")
+    if vo_fc and not vo:
+        raise ValueError("vo_fc: the dataset has no vo_poses")
+    droprate = pr.droprate if pr is not None else float(net.droprate)
+    cap = ds.max_batch * ds.frames_per_item                  # frames the dataset's cache assembles per call
+    own = pr is None and net.precision in ("bf16", "tc_split")
+    B = min(pr.max_batch if pr is not None else 64, cap)
+    if droprate > 0:
+        if B < T:
+            raise ValueError("droprate > 0 runs one window of %d frames per forward; max_batch allows %d" % (T, B))
+        B = T
+    tab = ds.eval_tables(unique=droprate == 0, vo_fc=vo_fc)
+    frames, L = tab["frames"], tab["windows"].shape[0]
+    F = frames.shape[0]
+    if own:
+        pr = Predictor(model, max_batch=min(64, cap))
+    was_training = net.training
+    net.eval()
+    try:
+        with torch.cuda.device(dev):
+            chunks = [(lo, min(lo + B, F)) for lo in range(0, F, B)]
+            # two input buffers per chunk size, so that the next chunk is assembled while this one runs; one when the
+            # forward draws dropout masks, which then follow the Predictor's own sequence of forwards
+            n_slots = 2 if droprate == 0 and len(chunks) > 1 else 1
+            runners = _frame_runners(pr, net, sorted({hi - lo for lo, hi in chunks}), n_slots, ds.Ho, ds.Wo, dev)
+            cur = torch.cuda.current_stream(dev)
+            side = torch.cuda.Stream(dev)
+            side.wait_stream(cur)
+            read = {k: torch.cuda.Event() for k in runners}
+            ready = torch.cuda.Event()
+            pred6 = torch.empty((F, 6), dtype=torch.float32, device=dev)
+
+            def launch(k):
+                lo, hi = chunks[k]
+                key = (hi - lo, k % n_slots)
+                side.wait_event(read[key])                   # the previous forward from this buffer has read it
+                with torch.cuda.stream(side):
+                    ds.assemble_frames(frames[lo:hi], runners[key][0])
+                ready.record(side)
+                return key
+
+            key = launch(0)
+            for k in range(len(chunks)):
+                cur.wait_event(ready)
+                _, run, out = runners[key]
+                run()
+                read[key].record(cur)
+                lo, hi = chunks[k]
+                pred6[lo:hi].copy_(out)
+                if k + 1 < len(chunks):
+                    key = launch(k + 1)
+            E = tab["vo_rows"].shape[1]
+            pred7 = torch.empty((L, T, 7), dtype=torch.float64, device=dev)
+            targ7 = torch.empty_like(pred7)
+            vos7 = torch.empty((L, E, 7), dtype=torch.float64, device=dev) if vo else None
+            _lib.check(_lib.lib().mapnet_eval_windows(
+                pred6.data_ptr(), F, ds.poses.data_ptr(), ds.vo_poses.data_ptr() if vo else None, ds.poses.shape[0],
+                tab["windows"].ctypes.data, tab["slots"].ctypes.data, L * T,
+                tab["vo_rows"].ctypes.data if vo else None, L * E if vo else 0, pred7.data_ptr(), targ7.data_ptr(),
+                vos7.data_ptr() if vo else None, _lib.stream_ptr()), "mapnet_eval_windows")
+            pred, targ = pred7, targ7
+            if vo:
+                pred = pgo(pred, vos7, fc_vos=vo_fc, **sigmas)
+            if pose_m is not None:       # eval.py:180-181, as evaluate_tuples
+                m = torch.as_tensor(np.asarray(pose_m, dtype=np.float64), device=dev)
+                s = torch.as_tensor(np.asarray(pose_s, dtype=np.float64), device=dev)
+                pred = torch.cat((pred[..., :3] * s + m, pred[..., 3:]), -1)
+                targ = torch.cat((targ[..., :3] * s + m, targ[..., 3:]), -1)
+            mid = T // 2
+            p_mid, t_mid = pred[:, mid], targ[:, mid]
+            t_err, q_err = pose_errors(p_mid, t_mid)
+    finally:
+        net.train(was_training)
+        if own:
+            torch.cuda.current_stream(dev).synchronize()     # the temporary engines are freed once their work is done
+            pr.close()
+    return dict(pred7=p_mid, targ7=t_mid, t_err=t_err, q_err=q_err, n_frames=F)

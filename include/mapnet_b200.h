@@ -184,6 +184,19 @@ int mapnet_frame_cache_assemble(mapnet_frame_cache_t* h, int n, const int32_t* f
                                 const float* mean3, const float* std3, float* out_nchw, float* targ_out, void* stream);
 int mapnet_frame_cache_destroy(mapnet_frame_cache_t* h);
 
+/* ---- evaluation windows (csrc/loader.cu; geomapnet_b200.inference.evaluate_sequence): scripts/eval.py:163-170 for a
+ * whole sequence whose frames went through the network once each.  For every window slot r < n_rows:
+ *   pred7[r] = (t, qexp(log q)) of pred6[slot[r]],  targ7[r] = the same of poses[frame[r]]
+ * and for every VO k < n_vo: vos7[k] = (t, qexp(log q)) of calc_vo_logq_safe(vo_poses[a], vo_poses[b]) with
+ * (a, b) = vo_rows[2k], vo_rows[2k+1] (common/pose_utils.py:276-304; the same float32 arithmetic as the MFOnline VO
+ * targets of mapnet_frame_cache_assemble).  qexp is mapnet_pose_post's, bit for bit; translations are not
+ * un-normalised.  pred6 [n_pred][6], poses / vo_poses [n_poses][6] (float32) and the float64 outputs are device memory;
+ * frame, slot and vo_rows are HOST int32 arrays, checked and copied before the call returns.  n_vo = 0: no VOs
+ * (vo_poses, vo_rows, vos7 may be NULL).  Nothing is launched when a check fails. */
+int mapnet_eval_windows(const float* pred6, int n_pred, const float* poses, const float* vo_poses, int n_poses,
+                        const int32_t* frame, const int32_t* slot, int n_rows, const int32_t* vo_rows, int n_vo,
+                        double* pred7, double* targ7, double* vos7, void* stream);
+
 /* ---- batched inference post-processing + pose-graph optimisation (SURVEY.md section 8 row f3; csrc/pgo.cu).
  * mapnet_pose_post: scripts/eval.py:163-181 for n poses at once -- pred6 = (t, log q) float32 -> out7 = (t * pose_s +
  * pose_m, qexp(log q)) float64; pose_m3 / pose_s3 are HOST pointers (pose_stats.txt) or NULL (keep the translations).
