@@ -100,6 +100,9 @@ def lib():
     L.mapnet_eval_windows.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int,
                                       c_void_p, c_void_p, c_void_p, c_void_p]
     L.mapnet_eval_windows.restype = c_int
+    L.mapnet_batch_losses.argtypes = [c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int,
+                                      c_void_p, c_void_p, c_void_p]
+    L.mapnet_batch_losses.restype = c_int
     L.mapnet_pose_post.argtypes =[c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
     L.mapnet_pose_post.restype = c_int
     L.mapnet_pgo_optimize.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, ctypes.c_double, ctypes.c_double,
@@ -160,7 +163,8 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_frame_cache_create", "mapnet_frame_cache_ingest", "mapnet_frame_cache_assemble",
             "mapnet_frame_cache_destroy", "mapnet_infer_calibrate", "mapnet_infer_act_scales", "mapnet_test_conv_fp8",
             "mapnet_test_bn_forward", "mapnet_test_bn_backward", "mapnet_test_stem_pool", "mapnet_test_gap",
-            "mapnet_trunk_set_trainable", "mapnet_test_conv_ex", "mapnet_eval_windows"]
+            "mapnet_trunk_set_trainable", "mapnet_test_conv_ex", "mapnet_eval_windows",
+            "mapnet_batch_losses"]
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 
 

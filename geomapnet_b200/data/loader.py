@@ -137,6 +137,31 @@ class ItemLayout(object):
         return dict(windows=windows, frames=np.ascontiguousarray(frames, dtype=np.int32),
                     slots=np.ascontiguousarray(slots, dtype=np.int32), vo_rows=np.ascontiguousarray(vo_rows, dtype=np.int32))
 
+    def val_tables(self, batch_size, shuffle=True, unique=True):
+        """One validation pass (common/train.py:214-250) as DataLoader(dataset, batch_size, shuffle, num_workers=0) draws
+        it: the batch records of host_batches, drawn in full (the global torch and numpy RNG streams advance as in the
+        reference's loop), and host int32 tables over the items of the pass in loader order:
+          batch_items [n_batches+1]  item offset of each batch (the last batch may be partial);
+          targ_rows [I,T]            the pose row of every window slot (T = 1 for single frames);
+          frames [F]                 the frames that go through the network, in that order;
+          pred_rows [I,T]            the row of `frames` whose prediction fills each window slot.
+        unique=True: every distinct frame of the pass once, in frame order.  unique=False: every item's frames in loader
+        order (pred_rows is the identity), what a forward that draws dropout masks or a jittered batch needs."""
+        if self.online:
+            raise ValueError("validation passes need a single-frame or MF layout (MFOnline never validates)")
+        batches = list(host_batches(self, batch_size, shuffle))
+        T = self.frames_per_item
+        items = np.cumsum([0] + [b[3] for b in batches]).astype(np.int32)
+        fr = np.concatenate([b[0] for b in batches]).astype(np.int32)
+        targ = np.concatenate([b[2][:, 0] for b in batches]).astype(np.int32).reshape(-1, T)
+        if unique:
+            frames, inv = np.unique(fr, return_inverse=True)
+        else:
+            frames, inv = fr, np.arange(fr.shape[0])
+        return dict(batches=batches, batch_items=items, targ_rows=np.ascontiguousarray(targ),
+                    frames=np.ascontiguousarray(frames, dtype=np.int32),
+                    pred_rows=np.ascontiguousarray(inv.reshape(-1, T), dtype=np.int32))
+
     def example(self, n):
         """A batch record of items 0, 1, ... (n of them) that makes no random draw (fixed skips, no ColorJitter): an
         input for warm-up and capture that leaves the RNG streams where the reference's loop has them."""

@@ -25,7 +25,7 @@ param_groups on the host, and each call writes a changed rate to the device befo
 """
 import torch
 
-__all__ = ["GraphedTrainStep"]
+__all__ = ["GraphedTrainStep", "train_val"]
 
 
 class GraphedTrainStep(object):
@@ -200,3 +200,37 @@ def train_epoch(loader, model, criterion, optimizer, max_grad_norm=0.0, steps=No
         b = next(it, None)
         st = launch(b) if b is not None else None
     return [float(v) for v in torch.stack(losses).cpu()]
+
+
+def train_val(model, train_loader, val_loader, train_criterion, val_criterion, optimizer, n_epochs, val_freq, snapshot,
+              logdir, max_grad_norm=0.0, start_epoch=0):
+    """Trainer.train_val (common/train.py:212-317) over DeviceLoaders, in the reference's order.  For each epoch from
+    start_epoch: validate (inference.validate) when epoch % val_freq == 0 or it is the last epoch, unless val_loader is
+    None (do_val = no); save a checkpoint (common.checkpoint.save_checkpoint, with train_criterion) when
+    epoch % snapshot == 0; optimizer.adjust_lr(epoch); one train_epoch.  Then a final checkpoint at n_epochs.
+
+    One Predictor of the model (bf16 / tc_split) serves every validation pass, refreshed before each; any other model
+    runs its own eval forward.  The train_epoch captures are kept across epochs.  Returns {"val": {epoch: avg loss},
+    "train": {epoch: [per-step losses]}} and prints nothing."""
+    from .common.checkpoint import save_checkpoint
+    from .inference import Predictor, validate
+    net = model.mapnet if hasattr(model, "mapnet") else model
+    pr = Predictor(model) if val_loader is not None and net.precision in ("bf16", "tc_split") else None
+    steps, out = {}, {"val": {}, "train": {}}
+    try:
+        for epoch in range(int(start_epoch), int(n_epochs)):
+            if val_loader is not None and (epoch % val_freq == 0 or epoch == n_epochs - 1):
+                if pr is not None:
+                    pr.refresh()
+                out["val"][epoch] = validate(pr if pr is not None else model, val_loader, val_criterion)[0]
+            if epoch % snapshot == 0:
+                save_checkpoint(logdir, epoch, model, optimizer, train_criterion)
+            optimizer.adjust_lr(epoch)
+            model.train()
+            out["train"][epoch] = train_epoch(train_loader, model, train_criterion, optimizer,
+                                              max_grad_norm=max_grad_norm, steps=steps)
+        save_checkpoint(logdir, int(n_epochs), model, optimizer, train_criterion)
+    finally:
+        if pr is not None:
+            pr.close()
+    return out

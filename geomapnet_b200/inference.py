@@ -6,7 +6,8 @@ frame and keeps the middle prediction of each tuple.  Here: ``predict`` runs the
 through the same fprop engines as training (BatchNorm running statistics, no dropout at eval -- see note), ``post`` does
 qexp + un-normalisation for all poses in one launch, ``pgo`` optimises all windows in one launch (csrc/pgo.cu), and
 ``pose_errors`` gives the translation / rotation errors eval.py prints (:193-199).  ``evaluate_sequence`` runs the
-whole loop from a device-resident sequence (data.DeviceDataset), each distinct frame through the network once.
+whole loop from a device-resident sequence (data.DeviceDataset), each distinct frame through the network once, and
+``validate`` the trainer's validation pass (common/train.py:214-250) over a data.DeviceLoader.
 
 Note on dropout: models/posenet.py:68-69 calls F.dropout without ``training=``, so the reference drops features at eval
 time too whenever droprate > 0; scripts/eval.py builds the model with the ini's dropout.  ``predict`` follows the
@@ -20,7 +21,7 @@ import torch
 from . import _lib
 from .common.pgo import optimize_pose_windows
 
-__all__ = ["Predictor", "predict", "post", "pgo", "pose_errors", "evaluate_tuples", "evaluate_sequence"]
+__all__ = ["Predictor", "predict", "post", "pgo", "pose_errors", "evaluate_tuples", "evaluate_sequence", "validate"]
 
 
 class Predictor(object):
@@ -108,9 +109,10 @@ class Predictor(object):
             self._engines[(H, W)] = eng
         return eng
 
-    def _graph(self, B, H, W, xb=None, slot=0):
+    def _graph(self, B, H, W, xb=None, slot=0, warm_droprate=None):
         """(CUDA graph, static input [B,3,H,W], static output [B,6]) of one batch shape, captured on first use after an
-        eager run on xb (zeros when None).  slot > 0: a further graph of the same shape with its own input buffer."""
+        eager run on xb (zeros when None).  slot > 0: a further graph of the same shape with its own input buffer.
+        warm_droprate: the droprate of that eager run (default the predictor's; 0 leaves the dropout counter alone)."""
         key = (B, H, W) if slot == 0 else (B, H, W, slot)
         g = self._graphs.get(key)
         if g is None:
@@ -123,7 +125,7 @@ class Predictor(object):
             side = torch.cuda.Stream(self.device)
             side.wait_stream(cur)
             with torch.cuda.stream(side):        # eager run first: tile plans, tensor maps, kernel attributes
-                eng.forward(xs, ps, self.droprate, self.seed)
+                eng.forward(xs, ps, self.droprate if warm_droprate is None else warm_droprate, self.seed)
             cur.wait_stream(side)
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
@@ -239,20 +241,123 @@ def evaluate_tuples(model, x, targ6, vos7=None, pose_m=None, pose_s=None, batch=
     return dict(pred7=p_mid, targ7=t_mid, t_err=t_err, q_err=q_err)
 
 
-def _frame_runners(pr, net, sizes, n_slots, H, W, dev):
-    """{(frames, slot): (static input [n,3,H,W], run(), static output [n,6])}: Predictor graphs, or the live eval forward
-    of `net` on plain buffers when there is no Predictor."""
+def _frame_runners(pr, net, keys, H, W, dev, quiet=()):
+    """{(frames, slot): (static input [n,3,H,W], run(), static output [n,6])} for keys [(n, slot)], created in that
+    order: Predictor graphs, or the live eval forward of `net` on plain buffers when there is no Predictor.  The graphs
+    of `quiet` keys are captured after an eager run without dropout, which leaves the engine's dropout counter alone."""
     runners = {}
-    for n in sizes:
-        for s in range(n_slots):
-            if pr is not None:
-                graph, xs, ps = pr._graph(n, H, W, slot=s)
-                runners[(n, s)] = (xs, graph.replay, ps)
-            else:
-                xs = torch.empty((n, 3, H, W), dtype=torch.float32, device=dev)
-                ps = torch.empty((n, 6), dtype=torch.float32, device=dev)
-                runners[(n, s)] = (xs, (lambda xs=xs, ps=ps: ps.copy_(net(xs))), ps)
+    for n, s in keys:
+        if pr is not None:
+            graph, xs, ps = pr._graph(n, H, W, slot=s, warm_droprate=0.0 if (n, s) in quiet else None)
+            runners[(n, s)] = (xs, graph.replay, ps)
+        else:
+            xs = torch.empty((n, 3, H, W), dtype=torch.float32, device=dev)
+            ps = torch.empty((n, 6), dtype=torch.float32, device=dev)
+            runners[(n, s)] = (xs, (lambda xs=xs, ps=ps: ps.copy_(net(xs))), ps)
     return runners
+
+
+def _model_for(model, ds, what):
+    """(Predictor or None, network, device) of a model or Predictor that runs over the DeviceDataset ds"""
+    pr = model if isinstance(model, Predictor) else None
+    net = pr.net if pr is not None else (model.mapnet if hasattr(model, "mapnet") else model)
+    dev = pr.device if pr is not None else next(net.parameters()).device
+    if dev != ds.device:
+        raise RuntimeError("geomapnet_b200.inference.%s has no CPU path: the model is on %s and the dataset on %s; both "
+                           "must be on one CUDA device" % (what, dev, ds.device))
+    if pr is not None and pr._params is None:
+        raise RuntimeError("Predictor is closed")
+    if pr is not None and pr._calib is not None and tuple(pr._calib.shape[-2:]) != (ds.Ho, ds.Wo):
+        raise ValueError("this fp8 Predictor was calibrated at %dx%d, the dataset's frames are %dx%d"
+                         % (pr._calib.shape[-2], pr._calib.shape[-1], ds.Ho, ds.Wo))
+    return pr, net, dev
+
+
+def _predict_frames(pr, net, ds, frames, B, n_slots, dev):
+    """pred [F,6] of the cache frames `frames` (host int32 [F]), B frames per forward, in order.  With two slots the
+    next chunk is assembled on a side stream while this one runs; with one the forwards follow each other."""
+    F = frames.shape[0]
+    chunks = [(lo, min(lo + B, F)) for lo in range(0, F, B)]
+    n_slots = n_slots if len(chunks) > 1 else 1
+    runners = _frame_runners(pr, net, [(n, s) for n in sorted({hi - lo for lo, hi in chunks}) for s in range(n_slots)],
+                             ds.Ho, ds.Wo, dev)
+    cur = torch.cuda.current_stream(dev)
+    side = torch.cuda.Stream(dev)
+    side.wait_stream(cur)
+    read = {k: torch.cuda.Event() for k in runners}
+    ready = torch.cuda.Event()
+    pred6 = torch.empty((F, 6), dtype=torch.float32, device=dev)
+
+    def launch(k):
+        lo, hi = chunks[k]
+        key = (hi - lo, k % n_slots)
+        side.wait_event(read[key])                   # the previous forward from this buffer has read it
+        with torch.cuda.stream(side):
+            ds.assemble_frames(frames[lo:hi], runners[key][0])
+        ready.record(side)
+        return key
+
+    key = launch(0)
+    for k in range(len(chunks)):
+        cur.wait_event(ready)
+        _, run, out = runners[key]
+        run()
+        read[key].record(cur)
+        lo, hi = chunks[k]
+        pred6[lo:hi].copy_(out)
+        if k + 1 < len(chunks):
+            key = launch(k + 1)
+    return pred6
+
+
+def _predict_batches(pr, net, ds, batches, droprate, dev):
+    """(pred [I*T,6], targ [I*T,6]) of a pass's batch records, in order: each batch is assembled, with its ColorJitter
+    records, straight into the input of its forward on a side stream (two slots) while the previous batch runs.
+
+    With dropout the masks follow the Predictor's own sequence of forwards, and that sequence is the one calling the
+    Predictor batch by batch makes: a batch size met for the first time costs one eager forward, before its first
+    replay.  The graphs of the second slot are captured without touching the dropout counter, and the eager forward
+    of a new size that is not the first batch's is run just before that size's first replay."""
+    T, H, W = ds.frames_per_item, ds.Ho, ds.Wo
+    sizes = [b[3] * T for b in batches]
+    n_slots = 2 if len(batches) > 1 else 1
+    keys = [(n, k % n_slots) for k, n in enumerate(sizes)]
+    order = list(dict.fromkeys([(n, 0) for n in sizes] + keys))      # each size's own graph first, as the Predictor
+    counted = pr is not None and droprate > 0
+    new = {n for n in sizes if (n, H, W) not in pr._graphs} if counted else set()
+    runners = _frame_runners(pr, net, order, H, W, dev, quiet=set(order[1:]) if counted else ())
+    pending = new - {sizes[0]}          # the eager forwards still to run, one per new size
+    I = sum(b[3] for b in batches)
+    pred = torch.empty((I * T, 6), dtype=torch.float32, device=dev)
+    targ = torch.empty((I * T, 6), dtype=torch.float32, device=dev)
+    cur = torch.cuda.current_stream(dev)
+    side = torch.cuda.Stream(dev)
+    side.wait_stream(cur)
+    read = {k: torch.cuda.Event() for k in runners}
+    ready = torch.cuda.Event()
+    rows = np.cumsum([0] + sizes)
+
+    def launch(k):
+        n = batches[k][3]
+        xs_shape, t_shape = ds.batch_shapes(n)
+        side.wait_event(read[keys[k]])
+        with torch.cuda.stream(side):
+            ds.assemble(batches[k], runners[keys[k]][0].view(xs_shape), targ[rows[k]:rows[k + 1]].view(t_shape))
+        ready.record(side)
+
+    launch(0)
+    for k in range(len(batches)):
+        cur.wait_event(ready)
+        xs, run, out = runners[keys[k]]
+        if sizes[k] in pending:
+            pending.discard(sizes[k])
+            pr._engine(H, W).forward(xs, out, pr.droprate, pr.seed)
+        run()
+        read[keys[k]].record(cur)
+        pred[rows[k]:rows[k + 1]].copy_(out)
+        if k + 1 < len(batches):
+            launch(k + 1)
+    return pred, targ
 
 
 @torch.no_grad()
@@ -283,17 +388,7 @@ def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, **s
         raise ValueError("evaluate_sequence: MFOnline datasets are not evaluation sequences")
     if not ds.h:
         raise RuntimeError("evaluate_sequence: the dataset is closed")
-    pr = model if isinstance(model, Predictor) else None
-    net = pr.net if pr is not None else (model.mapnet if hasattr(model, "mapnet") else model)
-    dev = pr.device if pr is not None else next(net.parameters()).device
-    if dev != ds.device:
-        raise RuntimeError("geomapnet_b200.inference.evaluate_sequence has no CPU path: the model is on %s and the "
-                           "dataset on %s; both must be on one CUDA device" % (dev, ds.device))
-    if pr is not None and pr._params is None:
-        raise RuntimeError("Predictor is closed")
-    if pr is not None and pr._calib is not None and tuple(pr._calib.shape[-2:]) != (ds.Ho, ds.Wo):
-        raise ValueError("this fp8 Predictor was calibrated at %dx%d, the dataset's frames are %dx%d"
-                         % (pr._calib.shape[-2], pr._calib.shape[-1], ds.Ho, ds.Wo))
+    pr, net, dev = _model_for(model, ds, "evaluate_sequence")
     vo = ds.vo_poses is not None
     T = 1 if ds.steps is None else ds.steps
     if vo and T < 2:
@@ -317,37 +412,9 @@ def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, **s
     net.eval()
     try:
         with torch.cuda.device(dev):
-            chunks = [(lo, min(lo + B, F)) for lo in range(0, F, B)]
-            # two input buffers per chunk size, so that the next chunk is assembled while this one runs; one when the
-            # forward draws dropout masks, which then follow the Predictor's own sequence of forwards
-            n_slots = 2 if droprate == 0 and len(chunks) > 1 else 1
-            runners = _frame_runners(pr, net, sorted({hi - lo for lo, hi in chunks}), n_slots, ds.Ho, ds.Wo, dev)
-            cur = torch.cuda.current_stream(dev)
-            side = torch.cuda.Stream(dev)
-            side.wait_stream(cur)
-            read = {k: torch.cuda.Event() for k in runners}
-            ready = torch.cuda.Event()
-            pred6 = torch.empty((F, 6), dtype=torch.float32, device=dev)
-
-            def launch(k):
-                lo, hi = chunks[k]
-                key = (hi - lo, k % n_slots)
-                side.wait_event(read[key])                   # the previous forward from this buffer has read it
-                with torch.cuda.stream(side):
-                    ds.assemble_frames(frames[lo:hi], runners[key][0])
-                ready.record(side)
-                return key
-
-            key = launch(0)
-            for k in range(len(chunks)):
-                cur.wait_event(ready)
-                _, run, out = runners[key]
-                run()
-                read[key].record(cur)
-                lo, hi = chunks[k]
-                pred6[lo:hi].copy_(out)
-                if k + 1 < len(chunks):
-                    key = launch(k + 1)
+            # two input buffers, so that the next chunk is assembled while this one runs; one when the forward draws
+            # dropout masks, which then follow the Predictor's own sequence of forwards
+            pred6 = _predict_frames(pr, net, ds, frames, B, 2 if droprate == 0 else 1, dev)
             E = tab["vo_rows"].shape[1]
             pred7 = torch.empty((L, T, 7), dtype=torch.float64, device=dev)
             targ7 = torch.empty_like(pred7)
@@ -374,3 +441,79 @@ def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, **s
             torch.cuda.current_stream(dev).synchronize()     # the temporary engines are freed once their work is done
             pr.close()
     return dict(pred7=p_mid, targ7=t_mid, t_err=t_err, q_err=q_err, n_frames=F)
+
+
+@torch.no_grad()
+def validate(model, loader, criterion):
+    """The validation pass of common/train.py:214-250 over a DeviceLoader: every batch of DataLoader(val_set,
+    batch_size, shuffle) through the eval-mode model and `criterion`.  Returns (avg, losses): the per-batch losses as
+    floats in batch order and their plain mean, the reference's AverageMeter.avg (the last, partial batch weighs as
+    much as any other).  The batch records are drawn with loader.batches(), so the torch and numpy RNG streams advance
+    as the reference's DataLoader advances them (sampler permutation, ColorJitter, variable_skip).
+
+    model: a PoseNet / MapNet or a Predictor, handled as evaluate_sequence handles it; the model's training flag is
+    left as it was.  loader: over a single-frame or MF DeviceDataset.  criterion: PoseNetCriterion for single frames,
+    MapNetCriterion for MF tuples; its sax, saq, srx, srq are read on the device (scripts/train.py default-constructs
+    the validation criterion, all four 0).
+
+    With droprate == 0 and no ColorJitter each distinct frame of the pass goes through the network once (a frame's
+    eval-mode pose does not depend on the other frames of its batch).  Otherwise each batch is assembled with its
+    jitter records straight into a forward input and run on its own, in batch order; dropout masks then follow the
+    Predictor's sequence of forwards as when it is called batch by batch.  All batch losses come from one
+    mapnet_batch_losses launch, bit for bit what the criterion returns per batch, and the pass synchronises with the
+    host once, at its end."""
+    from .common.criterion import MapNetCriterion, PoseNetCriterion
+    from .data.loader import DeviceLoader
+    if not isinstance(loader, DeviceLoader):
+        raise TypeError("validate needs a geomapnet_b200.data.DeviceLoader, got %s" % type(loader).__name__)
+    ds = loader.dataset
+    if ds.online:
+        raise ValueError("validate: MFOnline datasets are not validated (scripts/train.py builds no val_set for them)")
+    mode = "posenet" if isinstance(criterion, PoseNetCriterion) else ("mapnet" if isinstance(criterion, MapNetCriterion)
+                                                                     else None)
+    if mode is None or (mode == "posenet") != (ds.steps is None):
+        raise ValueError("validate: a %s does not fit the dataset's %s; use PoseNetCriterion for single frames and "
+                         "MapNetCriterion for MF tuples" % (type(criterion).__name__,
+                                                            "single frames" if ds.steps is None else "MF tuples"))
+    if not ds.h:
+        raise RuntimeError("validate: the dataset is closed")
+    pr, net, dev = _model_for(model, ds, "validate")
+    droprate = pr.droprate if pr is not None else float(net.droprate)
+    unique = droprate == 0 and ds.jitter is None
+    T = ds.frames_per_item
+    per_batch = loader.batch_size * T
+    if not unique and pr is not None and per_batch > pr.max_batch:
+        raise ValueError("with dropout or ColorJitter one batch of %d frames runs per forward; the Predictor's "
+                         "max_batch allows %d" % (per_batch, pr.max_batch))
+    cap = ds.max_batch * T                                   # frames the dataset's cache assembles per call
+    own = pr is None and net.precision in ("bf16", "tc_split")
+    tab = ds.val_tables(loader.batch_size, loader.shuffle, unique)
+    n_batches = len(tab["batches"])
+    if own:
+        pr = Predictor(model, max_batch=min(64, cap) if unique else max(64, per_batch))
+    was_training = net.training
+    net.eval()
+    try:
+        with torch.cuda.device(dev):
+            zero = torch.zeros(1, dtype=torch.float32, device=dev)
+            s4 = torch.cat([getattr(criterion, k).detach().float().to(dev).reshape(1) if hasattr(criterion, k) else zero
+                            for k in ("sax", "saq", "srx", "srq")])
+            if unique:
+                pred = _predict_frames(pr, net, ds, tab["frames"], min(pr.max_batch if pr is not None else 64, cap), 2,
+                                       dev)
+                targ, pred_rows, targ_rows = ds.poses, tab["pred_rows"], tab["targ_rows"]
+            else:
+                pred, targ = _predict_batches(pr, net, ds, tab["batches"], droprate, dev)
+                pred_rows = targ_rows = tab["pred_rows"]           # the identity: pred and targ are in loader order
+            out = torch.empty(n_batches, dtype=torch.float32, device=dev)
+            _lib.check(_lib.lib().mapnet_batch_losses(
+                _lib.LOSS_MODE[mode], pred.data_ptr(), pred.shape[0], targ.data_ptr(), targ.shape[0],
+                pred_rows.ctypes.data, targ_rows.ctypes.data, T, tab["batch_items"].ctypes.data, n_batches,
+                s4.data_ptr(), out.data_ptr(), _lib.stream_ptr()), "mapnet_batch_losses")
+            losses = out.cpu().tolist()                             # the pass's one host synchronisation
+    finally:
+        net.train(was_training)
+        if own:
+            torch.cuda.current_stream(dev).synchronize()     # the temporary engines are freed once their work is done
+            pr.close()
+    return sum(losses) / len(losses), losses

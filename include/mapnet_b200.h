@@ -112,6 +112,18 @@ int mapnet_trunk_set_trainable(mapnet_trunk_t* h, const uint8_t* host_mask, int 
 int mapnet_loss_fwd_bwd(int mode, const float* pred, const float* targ, int N, int T_pred, int T_targ,
                         const float* s4, float* loss, float* dpred, float* ds4, void* stream);
 
+/* ---- every batch loss of a validation pass in one launch (csrc/loss.cu; geomapnet_b200.inference.validate).
+ * Item i of the pass (loader order) is the window of rows pred_rows[i*T + t] of pred [n_pred][6] and targ_rows[i*T + t]
+ * of targ [n_targ][6], t < T; batch b holds items [batch_items[b], batch_items[b+1]).  losses[b] is bit for bit the
+ * loss mapnet_loss_fwd_bwd returns for batch b gathered into [N_b][T][6] (same per-pose core, thread mapping and
+ * reduction tree, one block per batch, no atomics).  mode: posenet (0, T = 1) or mapnet (1).  pred, targ, s4 (device
+ * sax, saq, srx, srq) and losses [n_batches] are device memory; pred_rows, targ_rows and batch_items [n_batches + 1]
+ * are HOST int32 arrays, checked (bounds, batch_items[0] = 0 and strictly increasing) and copied before the call
+ * returns.  Nothing is launched when a check fails. */
+int mapnet_batch_losses(int mode, const float* pred, int n_pred, const float* targ, int n_targ, const int32_t* pred_rows,
+                        const int32_t* targ_rows, int T, const int32_t* batch_items, int n_batches, const float* s4,
+                        float* losses, void* stream);
+
 /* ---- optimizer step on flat buffers (torch.optim.Adam semantics, L2 weight decay).
  * grad_scale multiplies the gradient first (1/world_size after a sum-allreduce).
  * sqnorm: device scalar holding the squared global grad norm (mapnet_sqnorm) to
