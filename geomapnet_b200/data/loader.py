@@ -17,6 +17,7 @@ and a per-image Pillow / torchvision transform stack (scripts/train.py:119-128).
   on the device, calc_vos_safe).  Results are bit-identical to Pillow + torchvision on the CPU
   (tests/test_gpu_loader.py).
 """
+import collections
 import ctypes
 
 import numpy as np
@@ -308,6 +309,35 @@ def host_batches(layout, batch_size, shuffle=True):
                                             num_workers=0, collate_fn=layout.collate))
 
 
+class SidePipeline(object):
+    """Buffers, named by hashable keys, filled on one side stream while the current stream consumes earlier fills.
+
+        pipe.fill(key, fn)          # fn() writes the key's buffer on the side stream
+        pipe.take(key)              # the current stream waits for that fill
+        pipe.read(key).record()     # the consumer is done with the buffer: the next fill of the key may start
+
+    Each key has its own "ready" event, so that a fill of one buffer made before another buffer is taken does not
+    delay the take.  Fills also come after everything the current stream had queued when the pipeline was made."""
+
+    def __init__(self, device):
+        self.side = torch.cuda.Stream(device)
+        self.side.wait_stream(torch.cuda.current_stream(device))
+        self._ready = collections.defaultdict(torch.cuda.Event)
+        self._read = collections.defaultdict(torch.cuda.Event)
+
+    def fill(self, key, fn):
+        self.side.wait_event(self._read[key])
+        with torch.cuda.stream(self.side):
+            fn()
+        self._ready[key].record(self.side)
+
+    def take(self, key):
+        torch.cuda.current_stream(self.side.device).wait_event(self._ready[key])
+
+    def read(self, key):
+        return self._read[key]
+
+
 class DeviceLoader(object):
     """DataLoader(dataset, batch_size, shuffle, num_workers=0) over a DeviceDataset: yields device (x, targ) batches,
     the last one partial.  The sampling is torch's own DataLoader over the host part of each item, so the global torch
@@ -332,32 +362,23 @@ class DeviceLoader(object):
         if self._bufs is None:
             xs, ts = ds.batch_shapes(self.batch_size)
             self._bufs = [(torch.empty(xs, device=dev), torch.empty(ts, device=dev)) for _ in range(2)]
-            self._side = torch.cuda.Stream(dev)
-            self._ready = [torch.cuda.Event() for _ in range(2)]
-            self._free = [torch.cuda.Event() for _ in range(2)]
+            self._pipe = SidePipeline(dev)
+        pipe = self._pipe
 
-        def launch(batch, slot):
+        def fill(batch, slot):
             x, t = self._bufs[slot]
-            n = batch[3]
-            self._side.wait_event(self._free[slot])           # the consumer of the slot's previous batch is done
-            with torch.cuda.stream(self._side):
-                ds.assemble(batch, x[:n], t[:n])
-            self._ready[slot].record(self._side)
-            return n
+            pipe.fill(slot, lambda: ds.assemble(batch, x[:batch[3]], t[:batch[3]]))
 
         it = self.batches()
-        first = next(it, None)
-        if first is None:
-            return
-        slot, n = 0, launch(first, 0)
-        while True:
+        batch, slot = next(it, None), 0
+        if batch is not None:
+            fill(batch, slot)
+        while batch is not None:
             nxt = next(it, None)
-            nn = launch(nxt, 1 - slot) if nxt is not None else 0
-            cur = torch.cuda.current_stream(dev)
-            cur.wait_event(self._ready[slot])
+            if nxt is not None:
+                fill(nxt, 1 - slot)
+            pipe.take(slot)
             x, t = self._bufs[slot]
-            yield x[:n], t[:n]
-            self._free[slot].record(torch.cuda.current_stream(dev))
-            if nxt is None:
-                return
-            slot, n = 1 - slot, nn
+            yield x[:batch[3]], t[:batch[3]]
+            pipe.read(slot).record(torch.cuda.current_stream(dev))
+            batch, slot = nxt, 1 - slot

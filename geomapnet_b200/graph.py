@@ -158,6 +158,7 @@ def train_epoch(loader, model, criterion, optimizer, max_grad_norm=0.0, steps=No
     assembled on a side stream straight into the static input of the step that takes it, while the previous step's
     optimizer graph runs.  steps: a dict {batch size: GraphedTrainStep} kept by the caller to reuse the captures in
     later epochs (filled on first use).  Returns the per-step losses as floats (one device sync, at the end)."""
+    from .data.loader import SidePipeline
     ds = loader.dataset
     dev = ds.device
     steps = {} if steps is None else steps
@@ -165,8 +166,6 @@ def train_epoch(loader, model, criterion, optimizer, max_grad_norm=0.0, steps=No
     last = len(ds) % loader.batch_size
     if last:
         sizes.append(last)
-    cur = torch.cuda.current_stream(dev)
-    side = torch.cuda.Stream(dev)
     for n in sizes:
         if n not in steps:
             xs, ts = ds.batch_shapes(n)
@@ -175,31 +174,24 @@ def train_epoch(loader, model, criterion, optimizer, max_grad_norm=0.0, steps=No
             steps[n] = GraphedTrainStep(model, criterion, optimizer, x0, t0, max_grad_norm=max_grad_norm)
     for st in steps.values():      # captures kept from an earlier epoch: before any batch is assembled
         st.check_trainable()
-    read = {n: torch.cuda.Event() for n in steps}
-    ready = torch.cuda.Event()
+    pipe = SidePipeline(dev)          # one buffer per batch size: the static inputs of its step
     losses = []
 
-    def launch(batch):
+    def fill(batch):
         st = steps[batch[3]]
-        side.wait_event(read[batch[3]])                   # the previous step of this size has read its inputs
-        with torch.cuda.stream(side):
-            ds.assemble(batch, st.x, st.t)
-        ready.record(side)
-        return st
+        pipe.fill(batch[3], lambda: ds.assemble(batch, st.x, st.t))
+        return batch[3]
 
     it = loader.batches()
     b = next(it, None)
-    if b is None:
-        return losses
-    st = launch(b)
-    while st is not None:
-        cur.wait_event(ready)
-        n = st.x.shape[0]
-        st.replay(inputs_read=read[n])
-        losses.append(st.loss.clone())
+    n = fill(b) if b is not None else None
+    while n is not None:
+        pipe.take(n)
+        steps[n].replay(inputs_read=pipe.read(n))
+        losses.append(steps[n].loss.clone())
         b = next(it, None)
-        st = launch(b) if b is not None else None
-    return [float(v) for v in torch.stack(losses).cpu()]
+        n = fill(b) if b is not None else None
+    return [float(v) for v in torch.stack(losses).cpu()] if losses else []
 
 
 def train_val(model, train_loader, val_loader, train_criterion, val_criterion, optimizer, n_epochs, val_freq, snapshot,

@@ -13,6 +13,7 @@ Note on dropout: models/posenet.py:68-69 calls F.dropout without ``training=``, 
 time too whenever droprate > 0; scripts/eval.py builds the model with the ini's dropout.  ``predict`` follows the
 module (geomapnet_b200.models.PoseNet keeps that behaviour); pass a model built with droprate=0 for deterministic poses.
 """
+import contextlib
 import ctypes
 
 import numpy as np
@@ -20,6 +21,7 @@ import torch
 
 from . import _lib
 from .common.pgo import optimize_pose_windows
+from .data.loader import SidePipeline
 
 __all__ = ["Predictor", "predict", "post", "pgo", "pose_errors", "evaluate_tuples", "evaluate_sequence", "validate"]
 
@@ -133,6 +135,14 @@ class Predictor(object):
             g = self._graphs[key] = (graph, xs, ps)
         return g
 
+    def _check_frames(self, H, W):
+        """raises unless the predictor is open and takes frames of H x W (an fp8 one only its calibration size)"""
+        if self._params is None:
+            raise RuntimeError("Predictor is closed")
+        if self._calib is not None and (H, W) != tuple(self._calib.shape[-2:]):
+            raise ValueError("this fp8 Predictor was calibrated at %dx%d, got frames of %dx%d"
+                             % (self._calib.shape[-2], self._calib.shape[-1], H, W))
+
     def _run(self, xb):
         """pred [B,6] for frames xb [B,3,H,W] (B <= max_batch): graph replay, captured on the first call of a shape."""
         graph, xs, ps = self._graph(xb.shape[0], xb.shape[2], xb.shape[3], xb)
@@ -149,11 +159,7 @@ class Predictor(object):
             raise ValueError("expected input [L,3,H,W] or [L,T,3,H,W], got %s" % (tuple(x.shape),))
         if x.shape[0] < 1 or (x.dim() == 5 and x.shape[1] < 1):
             raise ValueError("empty batch")
-        if self._params is None:
-            raise RuntimeError("Predictor is closed")
-        if self._calib is not None and tuple(x.shape[-2:]) != tuple(self._calib.shape[-2:]):
-            raise ValueError("this fp8 Predictor was calibrated at %dx%d, got frames of %dx%d"
-                             % (self._calib.shape[-2], self._calib.shape[-1], x.shape[-2], x.shape[-1]))
+        self._check_frames(x.shape[-2], x.shape[-1])
         frames = x.reshape(-1, *x.shape[-3:])
         if frames.dtype != torch.float32:
             frames = frames.float()
@@ -225,17 +231,22 @@ def evaluate_tuples(model, x, targ6, vos7=None, pose_m=None, pose_s=None, batch=
     """The whole loop of eval.py:147-199 for a MapNet: x [L,T,3,H,W], targ6 [L,T,6] (log-q targets), vos7 [L,T-1,7]
     or None (no PGO).  Keeps the middle prediction of every tuple.  Returns dict(pred7 [L,7], targ7 [L,7], t_err, q_err)."""
     out6 = predict(model, x, batch)                     # [L,T,6]
-    T = out6.shape[1]
     pred = post(out6)                                   # normalised translations, as PGO sees them (eval.py:172-178)
     targ = post(targ6.to(out6.device))
     if vos7 is not None:
         pred = pgo(pred, vos7.to(out6.device), **sigmas)
+    return _window_errors(pred, targ, pose_m, pose_s)
+
+
+def _window_errors(pred, targ, pose_m, pose_s):
+    """eval.py:180-199 on windows pred7, targ7 [L,T,7]: translations un-normalised with pose_m / pose_s (when given),
+    the middle pose of every window and its errors.  Returns dict(pred7 [L,7], targ7 [L,7], t_err, q_err)."""
     if pose_m is not None:
         m = torch.as_tensor(np.asarray(pose_m, dtype=np.float64), device=pred.device)
         s = torch.as_tensor(np.asarray(pose_s, dtype=np.float64), device=pred.device)
         pred = torch.cat((pred[..., :3] * s + m, pred[..., 3:]), -1)
         targ = torch.cat((targ[..., :3] * s + m, targ[..., 3:]), -1)
-    mid = T // 2                                        # eval.py:183-185 (py2 integer division)
+    mid = pred.shape[1] // 2                            # eval.py:183-185 (py2 integer division)
     p_mid, t_mid = pred[:, mid], targ[:, mid]
     t_err, q_err = pose_errors(p_mid, t_mid)
     return dict(pred7=p_mid, targ7=t_mid, t_err=t_err, q_err=q_err)
@@ -265,12 +276,29 @@ def _model_for(model, ds, what):
     if dev != ds.device:
         raise RuntimeError("geomapnet_b200.inference.%s has no CPU path: the model is on %s and the dataset on %s; both "
                            "must be on one CUDA device" % (what, dev, ds.device))
-    if pr is not None and pr._params is None:
-        raise RuntimeError("Predictor is closed")
-    if pr is not None and pr._calib is not None and tuple(pr._calib.shape[-2:]) != (ds.Ho, ds.Wo):
-        raise ValueError("this fp8 Predictor was calibrated at %dx%d, the dataset's frames are %dx%d"
-                         % (pr._calib.shape[-2], pr._calib.shape[-1], ds.Ho, ds.Wo))
+    if pr is not None:
+        pr._check_frames(ds.Ho, ds.Wo)
     return pr, net, dev
+
+
+@contextlib.contextmanager
+def _eval_pass(model, pr, net, dev, max_batch):
+    """The body of an evaluation pass on dev with the network in eval mode.  Yields the Predictor that runs it: pr, or
+    for a live bf16 / tc_split model a temporary one of max_batch frames, closed at the end; None for any other live
+    model, which runs its own eval forward.  The network's training flag is restored at the end."""
+    own = pr is None and net.precision in ("bf16", "tc_split")
+    if own:
+        pr = Predictor(model, max_batch=max_batch)
+    was_training = net.training
+    net.eval()
+    try:
+        with torch.cuda.device(dev):
+            yield pr
+    finally:
+        net.train(was_training)
+        if own:
+            torch.cuda.current_stream(dev).synchronize()     # the temporary engines are freed once their work is done
+            pr.close()
 
 
 def _predict_frames(pr, net, ds, frames, B, n_slots, dev):
@@ -279,34 +307,25 @@ def _predict_frames(pr, net, ds, frames, B, n_slots, dev):
     F = frames.shape[0]
     chunks = [(lo, min(lo + B, F)) for lo in range(0, F, B)]
     n_slots = n_slots if len(chunks) > 1 else 1
-    runners = _frame_runners(pr, net, [(n, s) for n in sorted({hi - lo for lo, hi in chunks}) for s in range(n_slots)],
+    keys = [(hi - lo, k % n_slots) for k, (lo, hi) in enumerate(chunks)]
+    runners = _frame_runners(pr, net, [(n, s) for n in sorted({n for n, _ in keys}) for s in range(n_slots)],
                              ds.Ho, ds.Wo, dev)
-    cur = torch.cuda.current_stream(dev)
-    side = torch.cuda.Stream(dev)
-    side.wait_stream(cur)
-    read = {k: torch.cuda.Event() for k in runners}
-    ready = torch.cuda.Event()
+    pipe = SidePipeline(dev)
     pred6 = torch.empty((F, 6), dtype=torch.float32, device=dev)
 
-    def launch(k):
+    def fill(k):
         lo, hi = chunks[k]
-        key = (hi - lo, k % n_slots)
-        side.wait_event(read[key])                   # the previous forward from this buffer has read it
-        with torch.cuda.stream(side):
-            ds.assemble_frames(frames[lo:hi], runners[key][0])
-        ready.record(side)
-        return key
+        pipe.fill(keys[k], lambda: ds.assemble_frames(frames[lo:hi], runners[keys[k]][0]))
 
-    key = launch(0)
-    for k in range(len(chunks)):
-        cur.wait_event(ready)
-        _, run, out = runners[key]
+    fill(0)
+    for k, (lo, hi) in enumerate(chunks):
+        _, run, out = runners[keys[k]]
+        pipe.take(keys[k])
         run()
-        read[key].record(cur)
-        lo, hi = chunks[k]
+        pipe.read(keys[k]).record(torch.cuda.current_stream(dev))
         pred6[lo:hi].copy_(out)
         if k + 1 < len(chunks):
-            key = launch(k + 1)
+            fill(k + 1)
     return pred6
 
 
@@ -330,33 +349,26 @@ def _predict_batches(pr, net, ds, batches, droprate, dev):
     I = sum(b[3] for b in batches)
     pred = torch.empty((I * T, 6), dtype=torch.float32, device=dev)
     targ = torch.empty((I * T, 6), dtype=torch.float32, device=dev)
-    cur = torch.cuda.current_stream(dev)
-    side = torch.cuda.Stream(dev)
-    side.wait_stream(cur)
-    read = {k: torch.cuda.Event() for k in runners}
-    ready = torch.cuda.Event()
+    pipe = SidePipeline(dev)
     rows = np.cumsum([0] + sizes)
 
-    def launch(k):
-        n = batches[k][3]
-        xs_shape, t_shape = ds.batch_shapes(n)
-        side.wait_event(read[keys[k]])
-        with torch.cuda.stream(side):
-            ds.assemble(batches[k], runners[keys[k]][0].view(xs_shape), targ[rows[k]:rows[k + 1]].view(t_shape))
-        ready.record(side)
+    def fill(k):
+        xs_shape, t_shape = ds.batch_shapes(batches[k][3])
+        pipe.fill(keys[k], lambda: ds.assemble(batches[k], runners[keys[k]][0].view(xs_shape),
+                                               targ[rows[k]:rows[k + 1]].view(t_shape)))
 
-    launch(0)
+    fill(0)
     for k in range(len(batches)):
-        cur.wait_event(ready)
         xs, run, out = runners[keys[k]]
+        pipe.take(keys[k])
         if sizes[k] in pending:
             pending.discard(sizes[k])
             pr._engine(H, W).forward(xs, out, pr.droprate, pr.seed)
         run()
-        read[keys[k]].record(cur)
+        pipe.read(keys[k]).record(torch.cuda.current_stream(dev))
         pred[rows[k]:rows[k + 1]].copy_(out)
         if k + 1 < len(batches):
-            launch(k + 1)
+            fill(k + 1)
     return pred, targ
 
 
@@ -397,7 +409,6 @@ def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, **s
         raise ValueError("vo_fc: the dataset has no vo_poses")
     droprate = pr.droprate if pr is not None else float(net.droprate)
     cap = ds.max_batch * ds.frames_per_item                  # frames the dataset's cache assembles per call
-    own = pr is None and net.precision in ("bf16", "tc_split")
     B = min(pr.max_batch if pr is not None else 64, cap)
     if droprate > 0:
         if B < T:
@@ -406,41 +417,21 @@ def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, **s
     tab = ds.eval_tables(unique=droprate == 0, vo_fc=vo_fc)
     frames, L = tab["frames"], tab["windows"].shape[0]
     F = frames.shape[0]
-    if own:
-        pr = Predictor(model, max_batch=min(64, cap))
-    was_training = net.training
-    net.eval()
-    try:
-        with torch.cuda.device(dev):
-            # two input buffers, so that the next chunk is assembled while this one runs; one when the forward draws
-            # dropout masks, which then follow the Predictor's own sequence of forwards
-            pred6 = _predict_frames(pr, net, ds, frames, B, 2 if droprate == 0 else 1, dev)
-            E = tab["vo_rows"].shape[1]
-            pred7 = torch.empty((L, T, 7), dtype=torch.float64, device=dev)
-            targ7 = torch.empty_like(pred7)
-            vos7 = torch.empty((L, E, 7), dtype=torch.float64, device=dev) if vo else None
-            _lib.check(_lib.lib().mapnet_eval_windows(
-                pred6.data_ptr(), F, ds.poses.data_ptr(), ds.vo_poses.data_ptr() if vo else None, ds.poses.shape[0],
-                tab["windows"].ctypes.data, tab["slots"].ctypes.data, L * T,
-                tab["vo_rows"].ctypes.data if vo else None, L * E if vo else 0, pred7.data_ptr(), targ7.data_ptr(),
-                vos7.data_ptr() if vo else None, _lib.stream_ptr()), "mapnet_eval_windows")
-            pred, targ = pred7, targ7
-            if vo:
-                pred = pgo(pred, vos7, fc_vos=vo_fc, **sigmas)
-            if pose_m is not None:       # eval.py:180-181, as evaluate_tuples
-                m = torch.as_tensor(np.asarray(pose_m, dtype=np.float64), device=dev)
-                s = torch.as_tensor(np.asarray(pose_s, dtype=np.float64), device=dev)
-                pred = torch.cat((pred[..., :3] * s + m, pred[..., 3:]), -1)
-                targ = torch.cat((targ[..., :3] * s + m, targ[..., 3:]), -1)
-            mid = T // 2
-            p_mid, t_mid = pred[:, mid], targ[:, mid]
-            t_err, q_err = pose_errors(p_mid, t_mid)
-    finally:
-        net.train(was_training)
-        if own:
-            torch.cuda.current_stream(dev).synchronize()     # the temporary engines are freed once their work is done
-            pr.close()
-    return dict(pred7=p_mid, targ7=t_mid, t_err=t_err, q_err=q_err, n_frames=F)
+    with _eval_pass(model, pr, net, dev, min(64, cap)) as pr:
+        # two input buffers, so that the next chunk is assembled while this one runs; one when the forward draws
+        # dropout masks, which then follow the Predictor's own sequence of forwards
+        pred6 = _predict_frames(pr, net, ds, frames, B, 2 if droprate == 0 else 1, dev)
+        E = tab["vo_rows"].shape[1]
+        pred7 = torch.empty((L, T, 7), dtype=torch.float64, device=dev)
+        targ7 = torch.empty_like(pred7)
+        vos7 = torch.empty((L, E, 7), dtype=torch.float64, device=dev) if vo else None
+        _lib.check(_lib.lib().mapnet_eval_windows(
+            pred6.data_ptr(), F, ds.poses.data_ptr(), ds.vo_poses.data_ptr() if vo else None, ds.poses.shape[0],
+            tab["windows"].ctypes.data, tab["slots"].ctypes.data, L * T,
+            tab["vo_rows"].ctypes.data if vo else None, L * E if vo else 0, pred7.data_ptr(), targ7.data_ptr(),
+            vos7.data_ptr() if vo else None, _lib.stream_ptr()), "mapnet_eval_windows")
+        out = _window_errors(pgo(pred7, vos7, fc_vos=vo_fc, **sigmas) if vo else pred7, targ7, pose_m, pose_s)
+    return dict(out, n_frames=F)
 
 
 @torch.no_grad()
@@ -486,34 +477,22 @@ def validate(model, loader, criterion):
         raise ValueError("with dropout or ColorJitter one batch of %d frames runs per forward; the Predictor's "
                          "max_batch allows %d" % (per_batch, pr.max_batch))
     cap = ds.max_batch * T                                   # frames the dataset's cache assembles per call
-    own = pr is None and net.precision in ("bf16", "tc_split")
     tab = ds.val_tables(loader.batch_size, loader.shuffle, unique)
     n_batches = len(tab["batches"])
-    if own:
-        pr = Predictor(model, max_batch=min(64, cap) if unique else max(64, per_batch))
-    was_training = net.training
-    net.eval()
-    try:
-        with torch.cuda.device(dev):
-            zero = torch.zeros(1, dtype=torch.float32, device=dev)
-            s4 = torch.cat([getattr(criterion, k).detach().float().to(dev).reshape(1) if hasattr(criterion, k) else zero
-                            for k in ("sax", "saq", "srx", "srq")])
-            if unique:
-                pred = _predict_frames(pr, net, ds, tab["frames"], min(pr.max_batch if pr is not None else 64, cap), 2,
-                                       dev)
-                targ, pred_rows, targ_rows = ds.poses, tab["pred_rows"], tab["targ_rows"]
-            else:
-                pred, targ = _predict_batches(pr, net, ds, tab["batches"], droprate, dev)
-                pred_rows = targ_rows = tab["pred_rows"]           # the identity: pred and targ are in loader order
-            out = torch.empty(n_batches, dtype=torch.float32, device=dev)
-            _lib.check(_lib.lib().mapnet_batch_losses(
-                _lib.LOSS_MODE[mode], pred.data_ptr(), pred.shape[0], targ.data_ptr(), targ.shape[0],
-                pred_rows.ctypes.data, targ_rows.ctypes.data, T, tab["batch_items"].ctypes.data, n_batches,
-                s4.data_ptr(), out.data_ptr(), _lib.stream_ptr()), "mapnet_batch_losses")
-            losses = out.cpu().tolist()                             # the pass's one host synchronisation
-    finally:
-        net.train(was_training)
-        if own:
-            torch.cuda.current_stream(dev).synchronize()     # the temporary engines are freed once their work is done
-            pr.close()
+    with _eval_pass(model, pr, net, dev, min(64, cap) if unique else max(64, per_batch)) as pr:
+        zero = torch.zeros(1, dtype=torch.float32, device=dev)
+        s4 = torch.cat([getattr(criterion, k).detach().float().to(dev).reshape(1) if hasattr(criterion, k) else zero
+                        for k in ("sax", "saq", "srx", "srq")])
+        if unique:
+            pred = _predict_frames(pr, net, ds, tab["frames"], min(pr.max_batch if pr is not None else 64, cap), 2, dev)
+            targ, pred_rows, targ_rows = ds.poses, tab["pred_rows"], tab["targ_rows"]
+        else:
+            pred, targ = _predict_batches(pr, net, ds, tab["batches"], droprate, dev)
+            pred_rows = targ_rows = tab["pred_rows"]           # the identity: pred and targ are in loader order
+        out = torch.empty(n_batches, dtype=torch.float32, device=dev)
+        _lib.check(_lib.lib().mapnet_batch_losses(
+            _lib.LOSS_MODE[mode], pred.data_ptr(), pred.shape[0], targ.data_ptr(), targ.shape[0],
+            pred_rows.ctypes.data, targ_rows.ctypes.data, T, tab["batch_items"].ctypes.data, n_batches,
+            s4.data_ptr(), out.data_ptr(), _lib.stream_ptr()), "mapnet_batch_losses")
+        losses = out.cpu().tolist()                             # the pass's one host synchronisation
     return sum(losses) / len(losses), losses
