@@ -130,6 +130,11 @@ def lib():
     L.mapnet_infer_destroy.argtypes = [c_void_p]
     L.mapnet_infer_calibrate.argtypes = [c_void_p, c_void_p, c_int, c_void_p]
     L.mapnet_infer_act_scales.argtypes = [c_void_p, POINTER(c_float), c_int]
+    L.mapnet_infer_forward_frames.argtypes = [c_void_p, c_void_p, c_void_p, c_int, POINTER(c_float), POINTER(c_float),
+                                              c_float, c_uint64, c_uint64, c_void_p, c_void_p]
+    L.mapnet_test_stem_operand.argtypes = [c_int, c_void_p, c_void_p, c_void_p, c_int, POINTER(c_float), POINTER(c_float),
+                                           c_void_p, c_void_p]
+    L.mapnet_test_stem_operand.restype = c_int
     L.mapnet_test_conv_fp8.argtypes = [c_int] * 7 + [c_void_p] * 7 + [c_int, c_void_p, c_void_p, c_void_p]
     L.mapnet_test_conv_fp8.restype = c_int
     L.mapnet_test_bn_forward.argtypes = [c_int] * 4 + [c_int64, c_int] + [c_void_p] * 5 + [c_int, c_void_p, c_void_p]
@@ -140,7 +145,7 @@ def lib():
     for name in ("mapnet_test_bn_forward", "mapnet_test_bn_backward", "mapnet_test_stem_pool", "mapnet_test_gap"):
         getattr(L, name).restype = c_int
     for name in ("mapnet_infer_create", "mapnet_infer_load", "mapnet_infer_forward", "mapnet_infer_destroy",
-                 "mapnet_infer_calibrate", "mapnet_infer_act_scales"):
+                 "mapnet_infer_calibrate", "mapnet_infer_act_scales", "mapnet_infer_forward_frames"):
         getattr(L, name).restype = c_int
     for name in ("mapnet_trunk_create", "mapnet_trunk_destroy", "mapnet_param_count", "mapnet_param_info",
                  "mapnet_forward", "mapnet_backward", "mapnet_loss_fwd_bwd", "mapnet_sqnorm",
@@ -164,7 +169,7 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_frame_cache_destroy", "mapnet_infer_calibrate", "mapnet_infer_act_scales", "mapnet_test_conv_fp8",
             "mapnet_test_bn_forward", "mapnet_test_bn_backward", "mapnet_test_stem_pool", "mapnet_test_gap",
             "mapnet_trunk_set_trainable", "mapnet_test_conv_ex", "mapnet_eval_windows",
-            "mapnet_batch_losses"]
+            "mapnet_batch_losses", "mapnet_infer_forward_frames", "mapnet_test_stem_operand"]
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 
 

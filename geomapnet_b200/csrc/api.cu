@@ -771,6 +771,37 @@ int mapnet_infer_forward(mapnet_infer_t* h, const float* x, int B, float droprat
   return h->net.forward(x, B, droprate, seed, step, pred, (cudaStream_t)stream);
 }
 
+int mapnet_infer_forward_frames(mapnet_infer_t* h, mapnet_preprocess_t* pre, const void* frames_nhwc_u8, int B,
+                                const float* mean3, const float* std3, float droprate, uint64_t seed, uint64_t step,
+                                float* pred, void* stream) {
+  MN_CHECK(h != nullptr, "infer_forward_frames: null handle");
+  return h->net.forward_frames(pre, (const uint8_t*)frames_nhwc_u8, B, mean3, std3, droprate, seed, step, pred,
+                               (cudaStream_t)stream);
+}
+
+// The stem operand of the inference engine from one of its two sources: uint8 frames through pre (the fused vertical
+// pass), or float32 images of pre's output size through k_stem_s2d (what mapnet_infer_forward writes).
+int mapnet_test_stem_operand(int precision, mapnet_preprocess_t* pre, const void* frames_nhwc_u8, const float* x_nchw,
+                             int B, const float* mean3, const float* std3, void* S, void* stream) {
+  MN_CHECK(precision == PREC_BF16_TC || precision == PREC_TC_SPLIT || precision == PREC_FP8,
+           "test_stem_operand: precision %d has no space-to-depth stem operand", precision);
+  MN_CHECK(pre != nullptr && S != nullptr && (frames_nhwc_u8 == nullptr) != (x_nchw == nullptr),
+           "test_stem_operand: need pre, S and exactly one of frames / x");
+  int H = 0, W = 0, max_images = 0;
+  MN_TRY(preprocess_geometry(pre, &H, &W, &max_images));
+  const int hc = (H - 1) / 2 + 1, Hs = hc + 3, Wsp = stem_s2d_wsp((W - 1) / 2 + 1);
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool sp = precision == PREC_TC_SPLIT;
+  if (frames_nhwc_u8 != nullptr) {
+    const uint8_t* f = (const uint8_t*)frames_nhwc_u8;
+    return sp ? preprocess_stem_s2d<hsplit>(pre, f, B, mean3, std3, (hsplit*)S, Hs, Wsp, st)
+              : preprocess_stem_s2d<bf16>(pre, f, B, mean3, std3, (bf16*)S, Hs, Wsp, st);
+  }
+  MN_CHECK(B >= 1, "test_stem_operand: batch %d", B);
+  return sp ? launch_stem_s2d<hsplit>(x_nchw, (hsplit*)S, B, H, W, Hs, Wsp, st)
+            : launch_stem_s2d<bf16>(x_nchw, (bf16*)S, B, H, W, Hs, Wsp, st);
+}
+
 int mapnet_infer_calibrate(mapnet_infer_t* h, const float* x, int B, void* stream) {
   MN_CHECK(h != nullptr, "infer_calibrate: null handle");
   return h->net.calibrate(x, B, (cudaStream_t)stream);

@@ -232,17 +232,38 @@ int InferNet::conv(int ci, const void* in, const void* residual, void* out, int 
   return tc_conv_run(plans[ci], (const bf16*)in, nullptr, (const bf16*)residual, out, st, nullptr, nullptr, &a);
 }
 
+// the stem operand A0 of frames x [B,3,H,W]: the space-to-depth image (or the im2col matrix), in the stem's operand type
+int InferNet::stem_operand(const float* x, int B, cudaStream_t st) {
+  const Net& n = spec;
+  if (precision == PREC_TC_SPLIT) {
+    if (n.stem_s2d) return launch_stem_s2d<hsplit>(x, (hsplit*)A0, B, H, W, n.convs[0].g.Hi, stem_s2d_wsp(n.Wc), st);
+    return launch_stem_im2col<hsplit>(x, (hsplit*)A0, B, H, W, n.Hc, n.Wc, n.convs[0].g.Ci, st);
+  }
+  if (n.stem_s2d) return launch_stem_s2d<bf16>(x, (bf16*)A0, B, H, W, n.convs[0].g.Hi, stem_s2d_wsp(n.Wc), st);
+  return launch_stem_im2col<bf16>(x, (bf16*)A0, B, H, W, n.Hc, n.Wc, n.convs[0].g.Ci, st);
+}
+
+// everything after the stem operand: stem conv .. head
+int InferNet::trunk(int B, float droprate, unsigned long long seed, unsigned long long step, float* pred, cudaStream_t st) {
+  if (precision == PREC_FP8) {
+    int last = 0;
+    MN_TRY(run_f8(B, false, &last, st));
+    MN_TRY(launch_gap<e4m3>((const e4m3*)act[last], feat, B, spec.Hf * spec.Wf, 512, st, f8_slots + 2 * n_f8 - 1));
+    return run_head(B, droprate, seed, step, pred, st);
+  }
+  if (precision == PREC_TC_SPLIT) return forward_t<TypesSplitHH>(B, droprate, seed, step, pred, st);
+  return forward_t<TypesBF16>(B, droprate, seed, step, pred, st);
+}
+
 template <typename P>
-int InferNet::forward_t(const float* x, int B, float droprate, unsigned long long seed, unsigned long long step,
-                        float* pred, cudaStream_t st) {
+int InferNet::forward_t(int B, float droprate, unsigned long long seed, unsigned long long step, float* pred,
+                        cudaStream_t st) {
   typedef typename P::A T;        // stem / downsample conv outputs (bf16, or fp32 in strict mode)
   typedef typename P::Z TZ;       // conv operands (bf16, or fp16 hi/lo planes)
   const int sp = (precision == PREC_TC_SPLIT) ? 1 : 0;
   const Net& n = spec;
   MN_TRY(ensure_plans(B));
-  // stem: operand image -> conv + BN + ReLU (epilogue) -> 3x3/s2 max pool
-  if (n.stem_s2d) MN_TRY(launch_stem_s2d<TZ>(x, (TZ*)A0, B, H, W, n.convs[0].g.Hi, stem_s2d_wsp(n.Wc), st));
-  else MN_TRY(launch_stem_im2col<TZ>(x, (TZ*)A0, B, H, W, n.Hc, n.Wc, n.convs[0].g.Ci, st));
+  // stem: operand image (A0, already written) -> conv + BN + ReLU (epilogue) -> 3x3/s2 max pool
   MN_TRY(conv(0, A0, nullptr, y0, 1, 0, 0, st));
   BnDesc id; memset(&id, 0, sizeof(id));        // the stem's BatchNorm and ReLU are in the conv epilogue: identity map
   id.f.scale = ident; id.f.shift = ident + 64;
@@ -293,14 +314,37 @@ int InferNet::forward(const float* x, int B, float droprate, unsigned long long 
   MN_CHECK(B >= 1 && B <= max_B, "infer_forward: batch %d outside [1, max_B=%d]", B, max_B);
   MN_CHECK(x != nullptr && pred != nullptr, "infer_forward: null pointer argument");
   MN_CHECK(droprate >= 0.f && droprate < 1.f, "infer_forward: droprate %f outside [0,1)", droprate);
-  if (precision == PREC_FP8) {
-    int last = 0;
-    MN_TRY(run_f8(x, B, false, &last, st));
-    MN_TRY(launch_gap<e4m3>((const e4m3*)act[last], feat, B, spec.Hf * spec.Wf, 512, st, f8_slots + 2 * n_f8 - 1));
-    return run_head(B, droprate, seed, step, pred, st);
-  }
-  if (precision == PREC_TC_SPLIT) return forward_t<TypesSplitHH>(x, B, droprate, seed, step, pred, st);
-  return forward_t<TypesBF16>(x, B, droprate, seed, step, pred, st);
+  MN_TRY(ensure_plans(B));
+  MN_TRY(stem_operand(x, B, st));
+  return trunk(B, droprate, seed, step, pred, st);
+}
+
+// Camera frames in: Resize + ToTensor + Normalize written by pre straight into the stem operand (two launches instead
+// of pre's two and the stem operand's one), then the forward from the stem conv on.  Every check comes before the first
+// launch.
+int InferNet::forward_frames(struct ::mapnet_preprocess* pre, const uint8_t* frames, int B, const float* mean3,
+                             const float* std3, float droprate, unsigned long long seed, unsigned long long step,
+                             float* pred, cudaStream_t st) {
+  MN_CHECK(loaded, "infer_forward_frames: no snapshot loaded (call mapnet_infer_load first)");
+  MN_CHECK(precision != PREC_FP8 || calibrated,
+           "infer_forward_frames: the fp8 engine has no activation scales for this snapshot (call mapnet_infer_calibrate)");
+  MN_CHECK(pre != nullptr && frames != nullptr && mean3 != nullptr && std3 != nullptr && pred != nullptr,
+           "infer_forward_frames: null pointer argument");
+  int Ho = 0, Wo = 0, max_images = 0;
+  MN_TRY(preprocess_geometry(pre, &Ho, &Wo, &max_images));
+  MN_CHECK(Ho == H && Wo == W, "infer_forward_frames: the preprocess plan resizes to %dx%d, the engine takes %dx%d", Ho,
+           Wo, H, W);
+  MN_CHECK(B >= 1 && B <= max_B && B <= max_images,
+           "infer_forward_frames: batch %d outside [1, min(max_B=%d, the plan's max_images=%d)]", B, max_B, max_images);
+  MN_CHECK(spec.stem_s2d, "infer_forward_frames: the engine's stem has no space-to-depth operand");
+  MN_CHECK(droprate >= 0.f && droprate < 1.f, "infer_forward_frames: droprate %f outside [0,1)", droprate);
+  for (int c = 0; c < 3; ++c)
+    MN_CHECK(std3[c] > 0.f, "infer_forward_frames: std[%d] = %f must be positive", c, std3[c]);
+  MN_TRY(ensure_plans(B));
+  const int Hs = spec.convs[0].g.Hi, Wsp = stem_s2d_wsp(spec.Wc);
+  if (precision == PREC_TC_SPLIT) MN_TRY(preprocess_stem_s2d<hsplit>(pre, frames, B, mean3, std3, (hsplit*)A0, Hs, Wsp, st));
+  else MN_TRY(preprocess_stem_s2d<bf16>(pre, frames, B, mean3, std3, (bf16*)A0, Hs, Wsp, st));
+  return trunk(B, droprate, seed, step, pred, st);
 }
 
 // one fp8 conv: t_in / t_res / t_out index the e4m3 tensors' scales (t_res < 0: bf16 residual or none; t_out < 0: bf16
@@ -330,10 +374,9 @@ int InferNet::conv_f8(int ci, const void* in, int t_in, const void* res, int t_r
   return tc_conv_run_f8(plans[ci], (const uint8_t*)in, res, out, e, st);
 }
 
-int InferNet::run_f8(const float* x, int B, bool calib, int* last, cudaStream_t st) {
+int InferNet::run_f8(int B, bool calib, int* last, cudaStream_t st) {
   const Net& n = spec;
   MN_TRY(ensure_plans(B));
-  MN_TRY(launch_stem_s2d<bf16>(x, (bf16*)A0, B, H, W, n.convs[0].g.Hi, stem_s2d_wsp(n.Wc), st));
   MN_TRY(conv(0, A0, nullptr, y0, 1, 0, 0, st));
   if (calib) {
     MN_CUDA(cudaMemsetAsync(f8_slots, 0, (size_t)n_f8 * 4, st));
@@ -374,7 +417,9 @@ int InferNet::calibrate(const float* x, int B, cudaStream_t st) {
   MN_CHECK(B >= 1 && B <= max_B, "infer_calibrate: %d calibration frames outside [1, max_B=%d]", B, max_B);
   MN_CHECK(x != nullptr, "infer_calibrate: null pointer argument");
   int last = 0;
-  MN_TRY(run_f8(x, B, true, &last, st));
+  MN_TRY(ensure_plans(B));
+  MN_TRY(stem_operand(x, B, st));
+  MN_TRY(run_f8(B, true, &last, st));
   calibrated = true;
   return 0;
 }

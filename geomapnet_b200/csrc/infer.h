@@ -44,6 +44,9 @@ struct InferNet {
   int load(const float* params, const float* bufs, cudaStream_t st);
   int forward(const float* x, int B, float droprate, unsigned long long seed, unsigned long long step, float* pred,
               cudaStream_t st);
+  // the same forward on uint8 camera frames [B][Hin][Win][3] that pre resizes to (H, W) (mapnet_infer_forward_frames)
+  int forward_frames(struct ::mapnet_preprocess* pre, const uint8_t* frames, int B, const float* mean3, const float* std3,
+                     float droprate, unsigned long long seed, unsigned long long step, float* pred, cudaStream_t st);
   // fp8: the activation scales, progressively over the engine's own schedule on frames x [B,3,H,W] (B <= max_B)
   int calibrate(const float* x, int B, cudaStream_t st);
   int act_scales(float* host, int cap, cudaStream_t st);
@@ -58,14 +61,16 @@ struct InferNet {
   static long long f8_slot_bytes(const Net& spec) { return 4LL * (3 * f8_tensors(spec) + 128); }
   int alloc(void** p, size_t bytes);
   int ensure_plans(int B);
-  template <typename P> int forward_t(const float* x, int B, float droprate, unsigned long long seed,
-                                      unsigned long long step, float* pred, cudaStream_t st);
+  int stem_operand(const float* x, int B, cudaStream_t st);
+  int trunk(int B, float droprate, unsigned long long seed, unsigned long long step, float* pred, cudaStream_t st);
+  template <typename P> int forward_t(int B, float droprate, unsigned long long seed, unsigned long long step,
+                                      float* pred, cudaStream_t st);
   int conv(int ci, const void* in, const void* residual, void* out, int relu, int res_split, int out_split,
            cudaStream_t st);
-  // fp8 schedule (stem .. last block) on frames x; calib: take every tensor's scale first.  Returns the index of the
-  // last block's output in act[] through *last.
   int run_head(int B, float droprate, unsigned long long seed, unsigned long long step, float* pred, cudaStream_t st);
-  int run_f8(const float* x, int B, bool calib, int* last, cudaStream_t st);
+  // fp8 schedule (stem conv .. last block) on the stem operand A0; calib: take every tensor's scale first.  Returns the
+  // index of the last block's output in act[] through *last.
+  int run_f8(int B, bool calib, int* last, cudaStream_t st);
   int conv_f8(int ci, const void* in, int t_in, const void* res, int t_res, void* out, int t_out, int relu, bool calib,
               cudaStream_t st);
 };

@@ -227,5 +227,13 @@ struct JitterParams;
 int preprocess_resize_u8(struct ::mapnet_preprocess* h, const uint8_t* img, int n, uint8_t* out_u8, cudaStream_t st);
 int launch_jitter_luma_sum(const uint8_t* u8, const int* frame_index, const JitterParams* jp, unsigned int* sums,
                            long long npix, int n, int gx, cudaStream_t st);
+// a plan's output size (Resize's) and the most frames one call takes
+int preprocess_geometry(const struct ::mapnet_preprocess* h, int* Hout, int* Wout, int* max_images);
+// the inference engine's input from camera frames: n uint8 frames [Hin][Win][3] (device memory, n <= max_images) through
+// Resize + ToTensor + Normalize (mean3 / std3: host) straight into the space-to-depth stem operand S [n][Hs][Wsp][16]
+// (launch_stem_s2d's layout and values, bit for bit; Hs, Wsp of the plan's output size).  Two launches.
+template <typename TZ>
+int preprocess_stem_s2d(struct ::mapnet_preprocess* h, const uint8_t* img, int n, const float* mean3, const float* std3,
+                        TZ* S, int Hs, int Wsp, cudaStream_t st);
 
 }  // namespace mapnet

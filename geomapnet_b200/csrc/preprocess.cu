@@ -79,6 +79,53 @@ k_pre_resize_v_norm(const uint8_t* __restrict__ tmp, float* __restrict__ out, ui
   }
 }
 
+// Inference from camera frames: pass 2 (vertical resample + ToTensor + Normalize) written straight into the inference
+// engine's space-to-depth stem operand, the layout of k_stem_s2d (layout.cu): S[b][bh][bw][16], channel (pr*2+pc)*3+c
+// of block (bh, bw) is pixel (2*bh+pr-4, 2*bw+pc-4) of the resized image, zero outside it and in channels 12..15.  The
+// float32 image is never stored: each value is the pre_normalize result k_stem_s2d would have read, converted once by
+// the same Vec8 store, so S is bitwise what k_stem_s2d writes over k_pre_resize_v_norm's output.  One thread per 2x2
+// block: a warp reads 32 consecutive 6-byte pixel pairs of each intermediate row it needs and writes 32 consecutive
+// blocks (1 KB in bf16).
+template <typename TZ>
+__global__ void __launch_bounds__(256)
+k_pre_resize_v_s2d(const uint8_t* __restrict__ tmp, TZ* __restrict__ S, const int* __restrict__ bounds,
+                   const int* __restrict__ kk, int ksize, int nimg, int Hin, int Hout, int Wout, int Hs, int Wsp,
+                   float m0, float m1, float m2, float s0, float s1, float s2) {
+  pdl_prologue();
+  const long long total = (long long)nimg * Hs * Wsp;
+  const float mean[3] = {m0, m1, m2}, stdev[3] = {s0, s1, s2};
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int bw = (int)(i % Wsp);
+    const long long r = i / Wsp;
+    const int bh = (int)(r % Hs);
+    const long long n = r / Hs;
+    float v[16];
+#pragma unroll
+    for (int k = 0; k < 16; ++k) v[k] = 0.f;
+#pragma unroll
+    for (int pr = 0; pr < 2; ++pr) {
+      const int yy = 2 * bh + pr - 4;
+      if (yy < 0 || yy >= Hout) continue;
+      const int ymin = bounds[2 * yy], cnt = bounds[2 * yy + 1];
+      const int* k = kk + (long long)yy * ksize;
+#pragma unroll
+      for (int pc = 0; pc < 2; ++pc) {
+        const int xx = 2 * bw + pc - 4;
+        if (xx < 0 || xx >= Wout) continue;
+        const uint8_t* src = tmp + ((n * Hin + ymin) * Wout + xx) * 3;
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+          v[(pr * 2 + pc) * 3 + c] = pre_normalize(pre_resample(src + c, (long long)Wout * 3, cnt, k), mean[c], stdev[c]);
+      }
+    }
+    Vec8<TZ> o0, o1;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) { o0.v[k] = v[k]; o1.v[k] = v[8 + k]; }
+    o0.store(S + i * 16);
+    o1.store(S + i * 16 + 8);
+  }
+}
+
 // ColorJitter, pass A: per image, the luma sum of the image in its state just before the contrast adjustment.
 // frame_index: nullptr (image n is image n of u8) or the frame cache's gather (image n is frame frame_index[n])
 __global__ void __launch_bounds__(256)
@@ -165,6 +212,36 @@ int launch_jitter_luma_sum(const uint8_t* u8, const int* frame_index, const Jitt
   MN_LAUNCH_CHECK();
   return 0;
 }
+
+// ---- used by the inference engine (infer.cu) ----------------------------------------------------------------------
+int preprocess_geometry(const mapnet_preprocess_t* h, int* Hout, int* Wout, int* max_images) {
+  MN_CHECK(h != nullptr, "preprocess: null plan");
+  *Hout = h->p.Hout; *Wout = h->p.Wout; *max_images = h->p.max_images;
+  return 0;
+}
+template <typename TZ>
+int preprocess_stem_s2d(mapnet_preprocess_t* h, const uint8_t* img, int n, const float* mean3, const float* std3, TZ* S,
+                        int Hs, int Wsp, cudaStream_t st) {
+  MN_CHECK(h != nullptr && img != nullptr && mean3 != nullptr && std3 != nullptr && S != nullptr,
+           "preprocess_stem_s2d: null argument");
+  PreprocessPlan& p = h->p;
+  MN_CHECK(n >= 1 && n <= p.max_images, "preprocess_stem_s2d: %d images outside [1, max_images=%d]", n, p.max_images);
+  for (int c = 0; c < 3; ++c) MN_CHECK(std3[c] > 0.f, "preprocess_stem_s2d: std[%d] = %f must be positive", c, std3[c]);
+  const long long t1 = (long long)n * p.Hin * p.Wout, t2 = (long long)n * Hs * Wsp;
+  const int g1 = (int)((t1 + 255) / 256 < (long long)kNumSMs * 16 ? (t1 + 255) / 256 : (long long)kNumSMs * 16);
+  const int g2 = (int)((t2 + 255) / 256 < (long long)kNumSMs * 16 ? (t2 + 255) / 256 : (long long)kNumSMs * 16);
+  MN_LAUNCH(k_pre_resize_h, g1, 256, 0, st, img, (const int*)nullptr, p.d_tmp, p.d_bh, p.d_kh, p.ksh, (long long)n * p.Hin,
+            p.Hin, p.Win, p.Wout);
+  MN_LAUNCH_CHECK();
+  MN_LAUNCH(k_pre_resize_v_s2d<TZ>, g2, 256, 0, st, (const uint8_t*)p.d_tmp, S, (const int*)p.d_bv, (const int*)p.d_kv,
+            p.ksv, n, p.Hin, p.Hout, p.Wout, Hs, Wsp, mean3[0], mean3[1], mean3[2], std3[0], std3[1], std3[2]);
+  MN_LAUNCH_CHECK();
+  return 0;
+}
+template int preprocess_stem_s2d<bf16>(mapnet_preprocess_t*, const uint8_t*, int, const float*, const float*, bf16*, int,
+                                       int, cudaStream_t);
+template int preprocess_stem_s2d<hsplit>(mapnet_preprocess_t*, const uint8_t*, int, const float*, const float*, hsplit*,
+                                         int, int, cudaStream_t);
 }  // namespace mapnet
 
 

@@ -23,7 +23,7 @@ from . import _lib
 from .common.pgo import optimize_pose_windows
 from .data.loader import SidePipeline
 
-__all__ = ["Predictor", "predict", "post", "pgo", "pose_errors", "evaluate_tuples", "evaluate_sequence", "validate"]
+__all__ = ["Predictor", "Localizer", "predict", "post", "pgo", "pose_errors", "evaluate_tuples", "evaluate_sequence", "validate"]
 
 
 class Predictor(object):
@@ -211,6 +211,138 @@ def post(pred6, pose_m=None, pose_s=None):
     with torch.cuda.device(p.device):
         _lib.check(_lib.lib().mapnet_pose_post(p.data_ptr(), out.data_ptr(), n, m, s, _lib.stream_ptr()), "mapnet_pose_post")
     return out
+
+
+class Localizer(object):
+    """Camera frames in, metric poses out: Resize(size) + ToTensor + Normalize(mean, std), the Predictor's snapshot and
+    ``post`` in one CUDA graph per batch shape.
+
+        loc = Localizer(predictor, mean, std, pose_m=None, pose_s=None, size=256)
+        poses = loc(frames)     # uint8 [L,H,W,3] or [H,W,3] (RGB, as PIL decodes), a CUDA or host tensor or an ndarray
+                                # -> float64 [L,7] (or [7]) on the device: (t * pose_s + pose_m, qexp(log q))
+        loc.close()
+
+    ``loc(frames)`` is bit for bit ``post(predictor(ImagePipeline(mean, std, size)(frames.cuda())), pose_m, pose_s)``,
+    but the normalised image is written straight into the engine's stem operand (csrc/preprocess.cu,
+    k_pre_resize_v_s2d) instead of going through a float32 tensor, and the whole call replays one graph: the horizontal
+    resize, that fused pass, the engine from the stem conv on and the pose post-processing.  The snapshot, ``refresh()``,
+    precision (bf16, tc_split or fp8), ``max_batch`` and the dropout counter are the predictor's: the Localizer runs the
+    predictor's own engines, so with droprate > 0 the masks follow the same sequence of engine calls as calling the
+    predictor does.  An fp8 predictor takes only frames that resize to its calibration size.  Each distinct (B, H, W)
+    is captured after one eager run, as Predictor's graphs are; longer inputs run in chunks of max_batch frames.
+    mean / std are rounded to float32 as ImagePipeline rounds them; pose_m / pose_s (pose_stats.txt) may be left out
+    together, which keeps the normalised translations."""
+
+    def __init__(self, predictor, mean, std, pose_m=None, pose_s=None, size=256):
+        if not isinstance(predictor, Predictor):
+            raise TypeError("Localizer wraps a geomapnet_b200.inference.Predictor, got %s" % type(predictor).__name__)
+        self.mean = np.asarray(mean, dtype=np.float64).astype(np.float32).reshape(3).copy()
+        self.std = np.asarray(std, dtype=np.float64).astype(np.float32).reshape(3).copy()
+        if not (self.std > 0).all():
+            raise ValueError("std must be positive, got %s" % (self.std,))
+        if (pose_m is None) != (pose_s is None):
+            raise ValueError("pose_m and pose_s go together (pose_stats.txt rows 0 and 1), or neither is given")
+        self._m = self._s = None
+        if pose_m is not None:
+            self._m = (ctypes.c_double * 3)(*[float(v) for v in np.asarray(pose_m).reshape(3)])
+            self._s = (ctypes.c_double * 3)(*[float(v) for v in np.asarray(pose_s).reshape(3)])
+        self.predictor, self.size = predictor, int(size)
+        self._plans = {}        # (H_in, W_in) -> mapnet_preprocess_t of max_batch frames
+        self._graphs = {}       # (B, H_in, W_in) -> (CUDAGraph, static uint8 input, static float64 output, pred6)
+        self._warm = set()      # engine shapes (B, H', W') whose eager run has drawn a dropout mask
+        self._open = True
+
+    def _resized(self, H, W):
+        """the (H, W) the engine sees for frames of H x W: torchvision's Resize(size)"""
+        from .data.preprocess import resize_output_size
+        return resize_output_size(H, W, self.size)
+
+    def _plan(self, H, W):
+        h = self._plans.get((H, W))
+        if h is None:
+            h = ctypes.c_void_p()
+            _lib.check(_lib.lib().mapnet_preprocess_create(ctypes.byref(h), H, W, self.size, self.predictor.max_batch),
+                       "mapnet_preprocess_create")
+            self._plans[(H, W)] = h
+        return h
+
+    def _launch(self, eng, pre, xs, pred, out, droprate):
+        """the call's library launches on the current stream: frames xs -> pred [B,6] -> out [B,7]"""
+        pr, L, B = self.predictor, _lib.lib(), xs.shape[0]
+        fp = ctypes.POINTER(ctypes.c_float)
+        _lib.check(L.mapnet_infer_forward_frames(eng.h, pre, xs.data_ptr(), B, self.mean.ctypes.data_as(fp),
+                                                 self.std.ctypes.data_as(fp), droprate, int(pr.seed), _lib.UINT64_MAX,
+                                                 pred.data_ptr(), _lib.stream_ptr()), "mapnet_infer_forward_frames")
+        _lib.check(L.mapnet_pose_post(pred.data_ptr(), out.data_ptr(), B, self._m, self._s, _lib.stream_ptr()),
+                   "mapnet_pose_post")
+
+    def _graph(self, fb):
+        """(CUDA graph, static input, static output, static pred6) of frames shaped like fb.  The eager run before the
+        capture draws a dropout mask only where calling the predictor would run one: the first time this Localizer
+        or the predictor meets the engine shape (B, H', W'), so frame sizes that resize alike share one draw."""
+        B, H, W = fb.shape[:3]
+        g = self._graphs.get((B, H, W))
+        if g is None:
+            pr = self.predictor
+            Ho, Wo = self._resized(H, W)
+            eng, pre = pr._engine(Ho, Wo), self._plan(H, W)
+            new_shape = (B, Ho, Wo) not in pr._graphs and (B, Ho, Wo) not in self._warm
+            self._warm.add((B, Ho, Wo))
+            xs = torch.empty((B, H, W, 3), dtype=torch.uint8, device=pr.device)
+            pred = torch.empty((B, 6), dtype=torch.float32, device=pr.device)
+            out = torch.empty((B, 7), dtype=torch.float64, device=pr.device)
+            xs.copy_(fb)
+            cur = torch.cuda.current_stream(pr.device)
+            side = torch.cuda.Stream(pr.device)
+            side.wait_stream(cur)
+            with torch.cuda.stream(side):        # eager run first: tile plans, tensor maps, kernel attributes
+                self._launch(eng, pre, xs, pred, out, pr.droprate if new_shape else 0.0)
+            cur.wait_stream(side)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                self._launch(eng, pre, xs, pred, out, pr.droprate)
+            g = self._graphs[(B, H, W)] = (graph, xs, out, pred)
+        return g
+
+    def _run(self, fb):
+        graph, xs, out, _ = self._graph(fb)
+        xs.copy_(fb, non_blocking=True)
+        graph.replay()
+        return out.clone()
+
+    @torch.no_grad()
+    def __call__(self, frames):
+        if not self._open or self.predictor._params is None:
+            raise ValueError("Localizer is closed" if not self._open else "the Localizer's Predictor is closed")
+        if isinstance(frames, np.ndarray):
+            if frames.dtype != np.uint8:
+                raise ValueError("expected uint8 frames, got %s" % frames.dtype)
+            frames = torch.from_numpy(np.ascontiguousarray(frames))
+        if not torch.is_tensor(frames) or frames.dtype != torch.uint8:
+            raise ValueError("expected uint8 frames, got %s" % getattr(frames, "dtype", type(frames).__name__))
+        if frames.dim() not in (3, 4) or frames.shape[-1] != 3:
+            raise ValueError("expected RGB frames [L,H,W,3] or [H,W,3], got %s" % (tuple(frames.shape),))
+        single = frames.dim() == 3
+        x = frames.unsqueeze(0) if single else frames
+        if x.shape[0] < 1 or x.shape[1] < 1 or x.shape[2] < 1:
+            raise ValueError("empty batch: frames of shape %s" % (tuple(frames.shape),))
+        self.predictor._check_frames(*self._resized(x.shape[1], x.shape[2]))
+        x = x.contiguous()
+        mb = self.predictor.max_batch
+        with torch.cuda.device(self.predictor.device):
+            outs = [self._run(x[i:i + mb]) for i in range(0, x.shape[0], mb)]
+        out = outs[0] if len(outs) == 1 else torch.cat(outs, 0)
+        return out[0] if single else out
+
+    def close(self):
+        """Free the graphs and preprocess plans (the predictor stays open)."""
+        if self._graphs or self._plans:
+            torch.cuda.current_stream(self.predictor.device).synchronize()
+        self._graphs.clear()
+        for h in self._plans.values():
+            _lib.lib().mapnet_preprocess_destroy(h)
+        self._plans.clear()
+        self._open = False
 
 
 def pgo(pred7, vos7, sax=1.0, saq=1.0, srx=1.0, srq=1.0, fc_vos=False):

@@ -250,6 +250,16 @@ int64_t mapnet_infer_arena_bytes(int max_B, int H, int W, int precision);
 int mapnet_infer_destroy(mapnet_infer_t* h);
 int mapnet_infer_calibrate(mapnet_infer_t* h, const float* x, int B, void* stream);
 int mapnet_infer_act_scales(mapnet_infer_t* h, float* host_out, int cap);
+/* mapnet_infer_forward_frames: the same forward from camera frames -- frames_nhwc_u8 uint8 [B][Hin][Win][3] (RGB, device
+ * memory) through pre's Resize, then ToTensor + Normalize(mean3, std3) (HOST pointers to 3 floats, as for
+ * mapnet_preprocess_run), written straight into the engine's space-to-depth stem operand: two launches take the place of
+ * mapnet_preprocess_run's two and the forward's stem-operand launch, and the float32 image is never stored.  pred is
+ * bitwise what mapnet_preprocess_run followed by mapnet_infer_forward computes.  Refused before any launch: pre resizing
+ * to another size than the engine's (H, W), B above max_B or pre's max_images, an engine without a space-to-depth stem
+ * (every tensor-core engine has one), a forward before a load, an uncalibrated fp8 engine.  Graph-capturable. */
+int mapnet_infer_forward_frames(mapnet_infer_t* h, mapnet_preprocess_t* pre, const void* frames_nhwc_u8, int B,
+                                const float* mean3, const float* std3, float droprate, uint64_t seed, uint64_t step,
+                                float* pred, void* stream);
 
 /* ---- measurement support (bench.py): number of kernels this library has launched so
  * far in this process, and per-class conv timing with CUDA events on the launching
@@ -346,6 +356,14 @@ int mapnet_test_gap(int precision, int B, int HW, int C, const void* z, float* f
  * .grad layout [64,3,7,7].  Replaces torchvision ResNet.conv1 (/root/reference/models/posenet.py:66). */
 int mapnet_test_stem(int B, int H, int W, const float* x_nchw, const float* w_oihw, void* y_out, const void* dy,
                      float* dw_oihw, void* stream);
+
+/* the inference engine's stem operand alone, [B][Hs][Wsp][16] in the precision's operand type (bf16 for MAPNET_PREC_BF16
+ * and MAPNET_PREC_FP8, fp16 hi/lo planes for MAPNET_PREC_TC_SPLIT; Hs = Hc + 3, Wsp = (Wc + 6) / 4 * 4 for the stem
+ * conv's output Hc x Wc at pre's output size), from exactly one source: frames_nhwc_u8 (uint8, device) through pre as
+ * mapnet_infer_forward_frames writes it, or x_nchw (float32 [B,3,Hout,Wout], device) as mapnet_infer_forward writes it.
+ * mean3 / std3: host, frames only. */
+int mapnet_test_stem_operand(int precision, mapnet_preprocess_t* pre, const void* frames_nhwc_u8, const float* x_nchw,
+                             int B, const float* mean3, const float* std3, void* S, void* stream);
 
 /* micro-benchmark of one tensor-core conv configuration (tools/bench_conv.py): average ms per launch */
 int mapnet_bench_conv(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* in0,
