@@ -132,6 +132,15 @@ def lib():
     L.mapnet_infer_act_scales.argtypes = [c_void_p, POINTER(c_float), c_int]
     L.mapnet_infer_forward_frames.argtypes = [c_void_p, c_void_p, c_void_p, c_int, POINTER(c_float), POINTER(c_float),
                                               c_float, c_uint64, c_uint64, c_void_p, c_void_p]
+    L.mapnet_infer_sample.argtypes = [c_void_p, c_void_p, c_int, c_int, c_float, c_uint64, c_uint64, c_void_p, c_void_p,
+                                      c_void_p, c_void_p]
+    L.mapnet_infer_sample_frames.argtypes = [c_void_p, c_void_p, c_void_p, c_int, POINTER(c_float), POINTER(c_float), c_int,
+                                             c_float, c_uint64, c_uint64, c_void_p, c_void_p, c_void_p, c_void_p]
+    L.mapnet_sample_post.argtypes = [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_void_p, c_void_p]
+    L.mapnet_test_small_gemm_plan.argtypes = [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int)]
+    for name in ("mapnet_infer_sample", "mapnet_infer_sample_frames", "mapnet_sample_post", "mapnet_test_small_gemm_plan"):
+        getattr(L, name).restype = c_int
     L.mapnet_test_stem_operand.argtypes = [c_int, c_void_p, c_void_p, c_void_p, c_int, POINTER(c_float), POINTER(c_float),
                                            c_void_p, c_void_p]
     L.mapnet_test_stem_operand.restype = c_int
@@ -169,8 +178,10 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_frame_cache_destroy", "mapnet_infer_calibrate", "mapnet_infer_act_scales", "mapnet_test_conv_fp8",
             "mapnet_test_bn_forward", "mapnet_test_bn_backward", "mapnet_test_stem_pool", "mapnet_test_gap",
             "mapnet_trunk_set_trainable", "mapnet_test_conv_ex", "mapnet_eval_windows",
-            "mapnet_batch_losses", "mapnet_infer_forward_frames", "mapnet_test_stem_operand"]
+            "mapnet_batch_losses", "mapnet_infer_forward_frames", "mapnet_test_stem_operand", "mapnet_infer_sample",
+            "mapnet_infer_sample_frames", "mapnet_sample_post", "mapnet_test_small_gemm_plan"]
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
+MAX_SAMPLE_DRAWS = 1024      # mapnet_infer_sample: S in [2, MAX_SAMPLE_DRAWS] dropout draws per frame
 
 
 def check(rc, what):
@@ -272,6 +283,13 @@ class Infer(object):
     def forward(self, x, pred, droprate, seed, step=UINT64_MAX):
         check(lib().mapnet_infer_forward(self.h, x.data_ptr(), x.shape[0], float(droprate), int(seed), int(step),
                                          pred.data_ptr(), stream_ptr()), "mapnet_infer_forward")
+
+    def sample(self, x, S, droprate, seed, samples, mean, cov, step=UINT64_MAX):
+        """S Monte-Carlo dropout draws per frame of x [B,3,H,W] from one trunk forward: samples [B,S,6] float32 (or
+        None), mean [B,6] and cov [B,6,6] float64 (mapnet_infer_sample)"""
+        check(lib().mapnet_infer_sample(self.h, x.data_ptr(), x.shape[0], int(S), float(droprate), int(seed), int(step),
+                                        None if samples is None else samples.data_ptr(), mean.data_ptr(),
+                                        cov.data_ptr(), stream_ptr()), "mapnet_infer_sample")
 
     def close(self):
         if self.h:

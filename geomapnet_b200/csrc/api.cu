@@ -779,6 +779,28 @@ int mapnet_infer_forward_frames(mapnet_infer_t* h, mapnet_preprocess_t* pre, con
                                (cudaStream_t)stream);
 }
 
+int mapnet_infer_sample(mapnet_infer_t* h, const float* x, int B, int S, float droprate, uint64_t seed, uint64_t step,
+                        float* samples, double* mean, double* cov, void* stream) {
+  MN_CHECK(h != nullptr, "infer_sample: null handle");
+  return h->net.sample(x, B, S, droprate, seed, step, samples, mean, cov, (cudaStream_t)stream);
+}
+
+int mapnet_infer_sample_frames(mapnet_infer_t* h, mapnet_preprocess_t* pre, const void* frames_nhwc_u8, int B,
+                               const float* mean3, const float* std3, int S, float droprate, uint64_t seed,
+                               uint64_t step, float* samples, double* mean, double* cov, void* stream) {
+  MN_CHECK(h != nullptr, "infer_sample_frames: null handle");
+  return h->net.sample_frames(pre, (const uint8_t*)frames_nhwc_u8, B, mean3, std3, S, droprate, seed, step, samples,
+                              mean, cov, (cudaStream_t)stream);
+}
+
+// host-only: launch_small_gemm's split-K plan of one product
+int mapnet_test_small_gemm_plan(int epi, int M, int N, int K, int* splits, int* kchunk) {
+  MN_CHECK(epi >= 0 && epi <= 2 && M >= 1 && N >= 1 && K >= 1 && splits != nullptr && kchunk != nullptr,
+           "test_small_gemm_plan: bad argument");
+  *splits = small_gemm_split_plan(epi, M, N, K, kchunk);
+  return 0;
+}
+
 // The stem operand of the inference engine from one of its two sources: uint8 frames through pre (the fused vertical
 // pass), or float32 images of pre's output size through k_stem_s2d (what mapnet_infer_forward writes).
 int mapnet_test_stem_operand(int precision, mapnet_preprocess_t* pre, const void* frames_nhwc_u8, const float* x_nchw,

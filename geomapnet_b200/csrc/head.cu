@@ -221,19 +221,26 @@ __global__ void k_split_sum(const float* __restrict__ part, int splits, int M, i
   C[(i / N) * ldc + i % N] = s;
 }
 
+int small_gemm_split_plan(int epi, int M, int N, int K, int* kchunk) {
+  const int tiles = cdiv(N, 32) * cdiv(M, 32);
+  *kchunk = K;
+  if (epi == 0 && tiles < kNumSMs / 2 && K >= 256) {
+    int splits = kNumSMs / tiles;
+    if (splits > K / 64) splits = K / 64;
+    if (splits > 1) {
+      *kchunk = ((K + splits - 1) / splits + 63) / 64 * 64;
+      return cdiv(K, *kchunk);
+    }
+  }
+  return 1;
+}
+
 int launch_small_gemm(int epi, const float* A, long long sam, long long sak, const float* Bm, long long sbn,
                       long long sbk, float* C, int ldc, int M, int N, int K, const float* bias, float* aux,
                       const float* mask, cudaStream_t st) {
   dim3 grid(cdiv(N, 32), cdiv(M, 32), 1);
   int kchunk = K;
-  if (epi == 0 && (int)(grid.x * grid.y) < kNumSMs / 2 && K >= 256) {
-    int splits = kNumSMs / (int)(grid.x * grid.y);
-    if (splits > K / 64) splits = K / 64;
-    if (splits > 1) {
-      kchunk = ((K + splits - 1) / splits + 63) / 64 * 64;
-      grid.z = cdiv(K, kchunk);
-    }
-  }
+  grid.z = small_gemm_split_plan(epi, M, N, K, &kchunk);
   // split-K: the splits store their partial C in a stream-ordered workspace, k_split_sum adds them in a fixed order
   float* part = nullptr;
   if (grid.z > 1) MN_CUDA(cudaMallocAsync((void**)&part, (size_t)grid.z * M * N * sizeof(float), st));
@@ -314,6 +321,16 @@ int launch_dpred_filter(const float* in, float* out_w, float* out_h, int B, int 
 __global__ void k_inc_u64(unsigned long long* c) {
   pdl_prologue(); *c += 1ULL; }
 
+// the mask value of flat element e = offset + i: keep_scale = 1 / (1 - p) or 0 (k_dropout_mask and k_head_draws)
+__device__ __forceinline__ float dropout_mask_at(unsigned long long seed, unsigned long long e, float p, float keep_scale) {
+  unsigned long long z = seed + 0x9E3779B97F4A7C15ULL * (e + 1ULL);
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
+  z = z ^ (z >> 31);
+  const float u = (float)(z >> 40) * (1.0f / 16777216.0f);
+  return (u >= p) ? keep_scale : 0.f;
+}
+
 __global__ void k_dropout_mask(float* __restrict__ mask, long long n, float p, unsigned long long seed,
                                unsigned long long offset, const unsigned long long* __restrict__ ctr,
                                unsigned long long ctr_stride) {
@@ -321,14 +338,8 @@ __global__ void k_dropout_mask(float* __restrict__ mask, long long n, float p, u
   if (ctr != nullptr) offset = (*ctr) * ctr_stride;      // device-side step counter (graph replay)
   const float keep_scale = 1.0f / (1.0f - p);
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
-       i += (long long)gridDim.x * blockDim.x) {
-    unsigned long long z = seed + 0x9E3779B97F4A7C15ULL * (offset + (unsigned long long)i + 1ULL);
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-    z = z ^ (z >> 31);
-    const float u = (float)(z >> 40) * (1.0f / 16777216.0f);
-    mask[i] = (u >= p) ? keep_scale : 0.f;
-  }
+       i += (long long)gridDim.x * blockDim.x)
+    mask[i] = dropout_mask_at(seed, offset + (unsigned long long)i, p, keep_scale);
 }
 int launch_dropout_mask(float* mask, long long n, float p, unsigned long long seed, unsigned long long offset,
                         unsigned long long* ctr_dev, unsigned long long ctr_stride, cudaStream_t st) {
@@ -339,6 +350,133 @@ int launch_dropout_mask(float* mask, long long n, float p, unsigned long long se
     MN_LAUNCH(k_inc_u64, 1, 1, 0, st, ctr_dev);
     MN_LAUNCH_CHECK();
   }
+  return 0;
+}
+
+// ---- Monte-Carlo dropout: S head draws per frame from one fc pre-activation ----------------------------------------
+// Draw s of frame b is bit for bit the pose the (s+1)-th of S consecutive ordinary forwards of the same B frames
+// returns (run_head: dropout mask, fc with the ReLU x mask epilogue, two feat_dim -> 3 small_gemm products):
+//  - mask: draw s uses dropout step c + s, c the engine's step (*ctr when ctr != null, else the host's `step`), and
+//    element j of frame b the flat index (c + s) * max_B * F + b * F + j of k_dropout_mask -- same splitmix64, same
+//    keep scale 1 / (1 - p) -- computed on the fly: no [S,B,F] mask is stored.  h = fmaxf(fcpre, 0) * mask, as the fc
+//    epilogue forms it (fcpre does not depend on the mask, so one fc product serves every draw).
+//  - summation order: launch_small_gemm splits K by the plan small_gemm_split_plan(0, B, 3, F) gives for the forward's
+//    B rows (not B * S: a different plan would give different bits).  Split z is one fmaf chain from 0 over
+//    [z * kchunk, min((z + 1) * kchunk, F)) with the bias added to split 0 only, and k_split_sum adds the partials in
+//    split order from 0 (with one split the partial is the output).  Here thread (draw, z) runs split z's six chains
+//    and one thread per (draw, output) adds the partials in that order.
+// grid (B, cdiv(S, dpb)), dpb draws x splits threads per block (draw index fastest), head_sample_smem bytes of shared
+// memory (F + 6 * dpb * splits floats).  draws: [B][S][6].
+__global__ void __launch_bounds__(256)
+k_head_draws(const float* __restrict__ fcpre, int F, const float* __restrict__ wx, const float* __restrict__ bx,
+             const float* __restrict__ wq, const float* __restrict__ bq, int S, int dpb, int splits, int kchunk,
+             float p, unsigned long long seed, unsigned long long step, const unsigned long long* __restrict__ ctr,
+             unsigned long long stride, float* __restrict__ draws) {
+  pdl_prologue();
+  extern __shared__ float hs[];                 // [F] relu(fcpre[b]), then [dpb][6][splits] split partials
+  float* part = hs + F;
+  const int b = blockIdx.x;
+  for (int j = threadIdx.x; j < F; j += blockDim.x) hs[j] = fmaxf(fcpre[(long long)b * F + j], 0.f);
+  __syncthreads();
+  const unsigned long long c = (ctr != nullptr) ? *ctr : step;
+  const float keep_scale = 1.0f / (1.0f - p);
+  const int sl = threadIdx.x % dpb, z = threadIdx.x / dpb;
+  const int s = blockIdx.y * dpb + sl;
+  if (z < splits && s < S) {
+    const unsigned long long e0 = (c + (unsigned long long)s) * stride + (unsigned long long)b * F;
+    const int k0 = z * kchunk, k1 = (k0 + kchunk < F) ? k0 + kchunk : F;
+    float acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int k = k0; k < k1; ++k) {
+      const float h = hs[k] * dropout_mask_at(seed, e0 + (unsigned long long)k, p, keep_scale);
+#pragma unroll
+      for (int o = 0; o < 3; ++o) {
+        acc[o] = fmaf(h, __ldg(wx + (long long)o * F + k), acc[o]);
+        acc[3 + o] = fmaf(h, __ldg(wq + (long long)o * F + k), acc[3 + o]);
+      }
+    }
+    if (z == 0) {
+#pragma unroll
+      for (int o = 0; o < 3; ++o) { acc[o] += bx[o]; acc[3 + o] += bq[o]; }
+    }
+#pragma unroll
+    for (int o = 0; o < 6; ++o) part[(sl * 6 + o) * splits + z] = acc[o];
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < dpb * 6; t += blockDim.x) {
+    const int d = t / 6, o = t - d * 6, s2 = blockIdx.y * dpb + d;
+    if (s2 >= S) continue;
+    const float* pp = part + (d * 6 + o) * splits;
+    float v = pp[0];
+    if (splits > 1) {
+      v = 0.f;
+      for (int zz = 0; zz < splits; ++zz) v += pp[zz];
+    }
+    draws[((long long)b * S + s2) * 6 + o] = v;
+  }
+}
+
+// per frame, in float64 and a fixed order: mean = (sum of the draws in s order) / S, cov = the two-pass sample
+// covariance (deviations from mean, divisor S - 1).  One block per frame; the frame's S x 6 draws are staged in shared
+// memory (24 KB at the bound S = kMaxSampleDraws = 1024).  ctr != null: advanced by S once every draw is read.
+__global__ void __launch_bounds__(64)
+k_head_stats(const float* __restrict__ draws, int S, double* __restrict__ mean, double* __restrict__ cov,
+             unsigned long long* __restrict__ ctr) {
+  pdl_prologue();
+  extern __shared__ float xs[];                 // [S][6]
+  __shared__ double m[6];
+  const int b = blockIdx.x;
+  for (int i = threadIdx.x; i < S * 6; i += blockDim.x) xs[i] = draws[(long long)b * S * 6 + i];
+  __syncthreads();
+  if (threadIdx.x < 6) {
+    double a = 0.0;
+    for (int s = 0; s < S; ++s) a += (double)xs[s * 6 + threadIdx.x];
+    m[threadIdx.x] = a / (double)S;
+    mean[b * 6 + threadIdx.x] = m[threadIdx.x];
+  }
+  __syncthreads();
+  if (threadIdx.x < 21) {                       // the upper triangle (i <= j), row by row
+    int i = 0, r = threadIdx.x;
+    while (r >= 6 - i) { r -= 6 - i; ++i; }
+    const int j = i + r;
+    double a = 0.0;
+    for (int s = 0; s < S; ++s) a += ((double)xs[s * 6 + i] - m[i]) * ((double)xs[s * 6 + j] - m[j]);
+    a /= (double)(S - 1);
+    cov[(long long)b * 36 + i * 6 + j] = a;
+    cov[(long long)b * 36 + j * 6 + i] = a;
+  }
+  if (ctr != nullptr && b == 0 && threadIdx.x == 0) *ctr += (unsigned long long)S;
+}
+
+size_t head_sample_smem(int B, int F, int S) {
+  int kchunk = F;
+  const int splits = small_gemm_split_plan(0, B, 3, F, &kchunk);
+  int dpb = 128 / splits;
+  if (dpb < 1) dpb = 1;
+  if (dpb > S) dpb = S;
+  return ((size_t)F + 6 * (size_t)dpb * splits) * sizeof(float);
+}
+
+int launch_head_sample(const float* fcpre, int B, int F, const float* wx, const float* bx, const float* wq,
+                       const float* bq, int S, float p, unsigned long long seed, unsigned long long step,
+                       unsigned long long* ctr_dev, unsigned long long stride, float* samples, double* mean,
+                       double* cov, cudaStream_t st) {
+  MN_CHECK(S >= 2 && S <= kMaxSampleDraws, "head_sample: %d draws outside [2, %d]", S, kMaxSampleDraws);
+  int kchunk = F;
+  const int splits = small_gemm_split_plan(0, B, 3, F, &kchunk);
+  int dpb = 128 / splits;                       // about 128 threads a block: B = 1 still spreads over several SMs
+  if (dpb < 1) dpb = 1;
+  if (dpb > S) dpb = S;
+  const int threads = (dpb * splits + 31) / 32 * 32;
+  const size_t smem = head_sample_smem(B, F, S);
+  MN_CHECK(smem <= 48 * 1024 && threads <= 256, "head_sample: feat_dim %d needs %zu bytes of shared memory", F, smem);
+  float* draws = samples;
+  if (draws == nullptr) MN_CUDA(cudaMallocAsync((void**)&draws, (size_t)B * S * 6 * sizeof(float), st));
+  MN_LAUNCH(k_head_draws, dim3(B, cdiv(S, dpb)), threads, smem, st, fcpre, F, wx, bx, wq, bq, S, dpb, splits, kchunk, p,
+            seed, step, (const unsigned long long*)ctr_dev, stride, draws);
+  MN_LAUNCH_CHECK();
+  MN_LAUNCH(k_head_stats, B, 64, (size_t)S * 6 * sizeof(float), st, (const float*)draws, S, mean, cov, ctr_dev);
+  MN_LAUNCH_CHECK();
+  if (samples == nullptr) MN_CUDA(cudaFreeAsync(draws, st));
   return 0;
 }
 

@@ -245,19 +245,23 @@ int InferNet::stem_operand(const float* x, int B, cudaStream_t st) {
 
 // everything after the stem operand: stem conv .. head
 int InferNet::trunk(int B, float droprate, unsigned long long seed, unsigned long long step, float* pred, cudaStream_t st) {
+  MN_TRY(features(B, st));
+  return run_head(B, droprate, seed, step, pred, st);
+}
+
+// stem conv .. global average pool: feat [B,512]
+int InferNet::features(int B, cudaStream_t st) {
   if (precision == PREC_FP8) {
     int last = 0;
     MN_TRY(run_f8(B, false, &last, st));
-    MN_TRY(launch_gap<e4m3>((const e4m3*)act[last], feat, B, spec.Hf * spec.Wf, 512, st, f8_slots + 2 * n_f8 - 1));
-    return run_head(B, droprate, seed, step, pred, st);
+    return launch_gap<e4m3>((const e4m3*)act[last], feat, B, spec.Hf * spec.Wf, 512, st, f8_slots + 2 * n_f8 - 1);
   }
-  if (precision == PREC_TC_SPLIT) return forward_t<TypesSplitHH>(B, droprate, seed, step, pred, st);
-  return forward_t<TypesBF16>(B, droprate, seed, step, pred, st);
+  if (precision == PREC_TC_SPLIT) return forward_t<TypesSplitHH>(B, st);
+  return forward_t<TypesBF16>(B, st);
 }
 
 template <typename P>
-int InferNet::forward_t(int B, float droprate, unsigned long long seed, unsigned long long step, float* pred,
-                        cudaStream_t st) {
+int InferNet::forward_t(int B, cudaStream_t st) {
   typedef typename P::A T;        // stem / downsample conv outputs (bf16, or fp32 in strict mode)
   typedef typename P::Z TZ;       // conv operands (bf16, or fp16 hi/lo planes)
   const int sp = (precision == PREC_TC_SPLIT) ? 1 : 0;
@@ -283,8 +287,7 @@ int InferNet::forward_t(int B, float droprate, unsigned long long seed, unsigned
     }
     xi = (xi + 2) % 3;
   }
-  MN_TRY(launch_gap<TZ>((const TZ*)act[xi], feat, B, n.Hf * n.Wf, 512, st));
-  return run_head(B, droprate, seed, step, pred, st);
+  return launch_gap<TZ>((const TZ*)act[xi], feat, B, n.Hf * n.Wf, 512, st);
 }
 
 // head on feat: exactly the calls of Net::forward_t, on the snapshot's copy of the head parameters
@@ -306,6 +309,45 @@ int InferNet::run_head(int B, float droprate, unsigned long long seed, unsigned 
   return 0;
 }
 
+// S Monte-Carlo dropout draws of the head on feat: the fc product once, without a mask (fcpre is the same for every
+// draw), then launch_head_sample, which forms every draw's mask and products in run_head's order (head.cu)
+int InferNet::sample_head(int B, int S, float droprate, unsigned long long seed, unsigned long long step, float* samples,
+                          double* mean, double* cov, cudaStream_t st) {
+  const Net& n = spec;
+  const float* hp = head - n.fc_w;
+  MN_TRY(launch_small_gemm(1, feat, 512, 1, hp + n.fc_w, 512, 1, hdrop, feat_dim, B, feat_dim, 512, hp + n.fc_b, fcpre,
+                           nullptr, st));
+  const bool dev_ctr = (step == ~0ULL);
+  return launch_head_sample(fcpre, B, feat_dim, hp + n.xyz_w, hp + n.xyz_b, hp + n.wpqr_w, hp + n.wpqr_b, S, droprate,
+                            seed, dev_ctr ? 0ULL : step, dev_ctr ? drop_ctr : nullptr,
+                            (unsigned long long)max_B * feat_dim, samples, mean, cov, st);
+}
+
+// the checks shared by sample and sample_frames (before any launch)
+int InferNet::check_sample(const char* what, int S, float droprate, const double* mean, const double* cov) const {
+  MN_CHECK(S >= 2 && S <= kMaxSampleDraws, "%s: S = %d draws outside [2, %d]", what, S, kMaxSampleDraws);
+  MN_CHECK(droprate > 0.f && droprate < 1.f, "%s: droprate %f outside (0,1): without dropout every draw is the same pose",
+           what, droprate);
+  MN_CHECK(mean != nullptr && cov != nullptr, "%s: null pointer argument", what);
+  MN_CHECK(head_sample_smem(max_B, feat_dim, S) <= 48 * 1024, "%s: feat_dim %d is too large for the draw kernel", what,
+           feat_dim);
+  return 0;
+}
+
+int InferNet::sample(const float* x, int B, int S, float droprate, unsigned long long seed, unsigned long long step,
+                     float* samples, double* mean, double* cov, cudaStream_t st) {
+  MN_CHECK(loaded, "infer_sample: no snapshot loaded (call mapnet_infer_load first)");
+  MN_CHECK(precision != PREC_FP8 || calibrated,
+           "infer_sample: the fp8 engine has no activation scales for this snapshot (call mapnet_infer_calibrate)");
+  MN_CHECK(B >= 1 && B <= max_B, "infer_sample: batch %d outside [1, max_B=%d]", B, max_B);
+  MN_CHECK(x != nullptr, "infer_sample: null pointer argument");
+  MN_TRY(check_sample("infer_sample", S, droprate, mean, cov));
+  MN_TRY(ensure_plans(B));
+  MN_TRY(stem_operand(x, B, st));
+  MN_TRY(features(B, st));
+  return sample_head(B, S, droprate, seed, step, samples, mean, cov, st);
+}
+
 int InferNet::forward(const float* x, int B, float droprate, unsigned long long seed, unsigned long long step, float* pred,
                       cudaStream_t st) {
   MN_CHECK(loaded, "infer_forward: no snapshot loaded (call mapnet_infer_load first)");
@@ -325,26 +367,49 @@ int InferNet::forward(const float* x, int B, float droprate, unsigned long long 
 int InferNet::forward_frames(struct ::mapnet_preprocess* pre, const uint8_t* frames, int B, const float* mean3,
                              const float* std3, float droprate, unsigned long long seed, unsigned long long step,
                              float* pred, cudaStream_t st) {
-  MN_CHECK(loaded, "infer_forward_frames: no snapshot loaded (call mapnet_infer_load first)");
+  MN_CHECK(pred != nullptr, "infer_forward_frames: null pointer argument");
+  MN_TRY(check_frames("infer_forward_frames", pre, frames, B, mean3, std3));
+  MN_CHECK(droprate >= 0.f && droprate < 1.f, "infer_forward_frames: droprate %f outside [0,1)", droprate);
+  MN_TRY(frames_operand(pre, frames, B, mean3, std3, st));
+  return trunk(B, droprate, seed, step, pred, st);
+}
+
+// S Monte-Carlo dropout draws from camera frames: forward_frames' stem operand and trunk, then sample_head
+int InferNet::sample_frames(struct ::mapnet_preprocess* pre, const uint8_t* frames, int B, const float* mean3,
+                            const float* std3, int S, float droprate, unsigned long long seed, unsigned long long step,
+                            float* samples, double* mean, double* cov, cudaStream_t st) {
+  MN_TRY(check_frames("infer_sample_frames", pre, frames, B, mean3, std3));
+  MN_TRY(check_sample("infer_sample_frames", S, droprate, mean, cov));
+  MN_TRY(frames_operand(pre, frames, B, mean3, std3, st));
+  MN_TRY(features(B, st));
+  return sample_head(B, S, droprate, seed, step, samples, mean, cov, st);
+}
+
+// the checks of a call on camera frames through pre (host-only)
+int InferNet::check_frames(const char* what, struct ::mapnet_preprocess* pre, const uint8_t* frames, int B,
+                           const float* mean3, const float* std3) const {
+  MN_CHECK(loaded, "%s: no snapshot loaded (call mapnet_infer_load first)", what);
   MN_CHECK(precision != PREC_FP8 || calibrated,
-           "infer_forward_frames: the fp8 engine has no activation scales for this snapshot (call mapnet_infer_calibrate)");
-  MN_CHECK(pre != nullptr && frames != nullptr && mean3 != nullptr && std3 != nullptr && pred != nullptr,
-           "infer_forward_frames: null pointer argument");
+           "%s: the fp8 engine has no activation scales for this snapshot (call mapnet_infer_calibrate)", what);
+  MN_CHECK(pre != nullptr && frames != nullptr && mean3 != nullptr && std3 != nullptr, "%s: null pointer argument", what);
   int Ho = 0, Wo = 0, max_images = 0;
   MN_TRY(preprocess_geometry(pre, &Ho, &Wo, &max_images));
-  MN_CHECK(Ho == H && Wo == W, "infer_forward_frames: the preprocess plan resizes to %dx%d, the engine takes %dx%d", Ho,
-           Wo, H, W);
+  MN_CHECK(Ho == H && Wo == W, "%s: the preprocess plan resizes to %dx%d, the engine takes %dx%d", what, Ho, Wo, H, W);
   MN_CHECK(B >= 1 && B <= max_B && B <= max_images,
-           "infer_forward_frames: batch %d outside [1, min(max_B=%d, the plan's max_images=%d)]", B, max_B, max_images);
-  MN_CHECK(spec.stem_s2d, "infer_forward_frames: the engine's stem has no space-to-depth operand");
-  MN_CHECK(droprate >= 0.f && droprate < 1.f, "infer_forward_frames: droprate %f outside [0,1)", droprate);
+           "%s: batch %d outside [1, min(max_B=%d, the plan's max_images=%d)]", what, B, max_B, max_images);
+  MN_CHECK(spec.stem_s2d, "%s: the engine's stem has no space-to-depth operand", what);
   for (int c = 0; c < 3; ++c)
-    MN_CHECK(std3[c] > 0.f, "infer_forward_frames: std[%d] = %f must be positive", c, std3[c]);
+    MN_CHECK(std3[c] > 0.f, "%s: std[%d] = %f must be positive", what, c, std3[c]);
+  return 0;
+}
+
+// the stem operand written from camera frames by pre (after check_frames)
+int InferNet::frames_operand(struct ::mapnet_preprocess* pre, const uint8_t* frames, int B, const float* mean3,
+                             const float* std3, cudaStream_t st) {
   MN_TRY(ensure_plans(B));
   const int Hs = spec.convs[0].g.Hi, Wsp = stem_s2d_wsp(spec.Wc);
-  if (precision == PREC_TC_SPLIT) MN_TRY(preprocess_stem_s2d<hsplit>(pre, frames, B, mean3, std3, (hsplit*)A0, Hs, Wsp, st));
-  else MN_TRY(preprocess_stem_s2d<bf16>(pre, frames, B, mean3, std3, (bf16*)A0, Hs, Wsp, st));
-  return trunk(B, droprate, seed, step, pred, st);
+  if (precision == PREC_TC_SPLIT) return preprocess_stem_s2d<hsplit>(pre, frames, B, mean3, std3, (hsplit*)A0, Hs, Wsp, st);
+  return preprocess_stem_s2d<bf16>(pre, frames, B, mean3, std3, (bf16*)A0, Hs, Wsp, st);
 }
 
 // one fp8 conv: t_in / t_res / t_out index the e4m3 tensors' scales (t_res < 0: bf16 residual or none; t_out < 0: bf16

@@ -47,6 +47,13 @@ struct InferNet {
   // the same forward on uint8 camera frames [B][Hin][Win][3] that pre resizes to (H, W) (mapnet_infer_forward_frames)
   int forward_frames(struct ::mapnet_preprocess* pre, const uint8_t* frames, int B, const float* mean3, const float* std3,
                      float droprate, unsigned long long seed, unsigned long long step, float* pred, cudaStream_t st);
+  // S Monte-Carlo dropout draws of the head per frame, from one trunk forward (mapnet_infer_sample): samples [B,S,6]
+  // (may be null), mean [B,6] and cov [B,6,6] in float64
+  int sample(const float* x, int B, int S, float droprate, unsigned long long seed, unsigned long long step,
+             float* samples, double* mean, double* cov, cudaStream_t st);
+  int sample_frames(struct ::mapnet_preprocess* pre, const uint8_t* frames, int B, const float* mean3, const float* std3,
+                    int S, float droprate, unsigned long long seed, unsigned long long step, float* samples,
+                    double* mean, double* cov, cudaStream_t st);
   // fp8: the activation scales, progressively over the engine's own schedule on frames x [B,3,H,W] (B <= max_B)
   int calibrate(const float* x, int B, cudaStream_t st);
   int act_scales(float* host, int cap, cudaStream_t st);
@@ -62,12 +69,19 @@ struct InferNet {
   int alloc(void** p, size_t bytes);
   int ensure_plans(int B);
   int stem_operand(const float* x, int B, cudaStream_t st);
+  int check_frames(const char* what, struct ::mapnet_preprocess* pre, const uint8_t* frames, int B, const float* mean3,
+                   const float* std3) const;
+  int frames_operand(struct ::mapnet_preprocess* pre, const uint8_t* frames, int B, const float* mean3,
+                     const float* std3, cudaStream_t st);
+  int check_sample(const char* what, int S, float droprate, const double* mean, const double* cov) const;
   int trunk(int B, float droprate, unsigned long long seed, unsigned long long step, float* pred, cudaStream_t st);
-  template <typename P> int forward_t(int B, float droprate, unsigned long long seed, unsigned long long step,
-                                      float* pred, cudaStream_t st);
+  int features(int B, cudaStream_t st);           // stem conv .. global average pool: feat
+  template <typename P> int forward_t(int B, cudaStream_t st);
   int conv(int ci, const void* in, const void* residual, void* out, int relu, int res_split, int out_split,
            cudaStream_t st);
   int run_head(int B, float droprate, unsigned long long seed, unsigned long long step, float* pred, cudaStream_t st);
+  int sample_head(int B, int S, float droprate, unsigned long long seed, unsigned long long step, float* samples,
+                  double* mean, double* cov, cudaStream_t st);
   // fp8 schedule (stem conv .. last block) on the stem operand A0; calib: take every tensor's scale first.  Returns the
   // index of the last block's output in act[] through *last.
   int run_f8(int B, bool calib, int* last, cudaStream_t st);

@@ -175,6 +175,18 @@ int launch_split_reduce(const float* part, int splits, long long n, float* dst, 
 int launch_small_gemm(int epi, const float* A, long long sam, long long sak, const float* Bm, long long sbn,
                       long long sbk, float* C, int ldc, int M, int N, int K, const float* bias, float* aux,
                       const float* mask, cudaStream_t st);
+// host-only: the split-K plan launch_small_gemm runs for an [M,K] x [N,K]^T product -- the number of K splits (grid.z),
+// and through *kchunk the length of every split but the last (K when there is one split)
+int small_gemm_split_plan(int epi, int M, int N, int K, int* kchunk);
+// Monte-Carlo dropout head (k_head_draws + k_head_stats): S draws of the head for every frame of fcpre [B,F], bit for
+// bit the outputs of S consecutive run_head calls from dropout step c (ctr_dev != null: c = *ctr_dev, advanced by S;
+// else c = step); samples [B,S,6] (may be null), mean [B,6] and cov [B,6,6] in float64.  stride = max_B * F.
+constexpr int kMaxSampleDraws = 1024;
+size_t head_sample_smem(int B, int F, int S);     // shared memory of k_head_draws (host-only; <= 48 KB to launch)
+int launch_head_sample(const float* fcpre, int B, int F, const float* wx, const float* bx, const float* wq,
+                       const float* bq, int S, float p, unsigned long long seed, unsigned long long step,
+                       unsigned long long* ctr_dev, unsigned long long stride, float* samples, double* mean,
+                       double* cov, cudaStream_t st);
 int launch_colsum(const float* A, int lda, int M, int N, float* out, cudaStream_t st);
 // two NaN-filtered copies of d pred [B,6] (models/posenet.py:28-34 hook semantics, head.cu): out_w for the head's weight /
 // bias gradients, out_h for the gradient into the trunk; filter == 0: plain copies

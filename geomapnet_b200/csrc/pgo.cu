@@ -287,3 +287,52 @@ extern "C" int mapnet_pose_post(const float* pred6, double* out7, int64_t n, con
   MN_LAUNCH_CHECK();
   return 0;
 }
+
+// Monte-Carlo dropout poses in metric units (mapnet_sample_post), float64 throughout: with D = diag(pose_s, 1, 1, 1),
+// pose7 = (mean_t * pose_s + pose_m, qexp(mean_logq)), qexp(v) = (cos n, sin n / n * v) with n = |v| ((1, 0, 0, 0) at
+// n = 0), cov_metric = D cov D, t_std = sqrt(trace of cov_metric's translation block) and q_std_deg = 2 sqrt(trace of
+// the log q block) * 180 / pi (a log q perturbation dv turns the rotation by about 2 |dv|).
+namespace mapnet {
+__global__ void k_sample_post(const double* __restrict__ mean, const double* __restrict__ cov, long long n, double m0,
+                              double m1, double m2, double s0, double s1, double s2, double* __restrict__ pose7,
+                              double* __restrict__ cov_out, double* __restrict__ t_std, double* __restrict__ q_std_deg) {
+  pdl_prologue();
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double* mu = mean + 6 * i;
+  const double* C = cov + 36 * i;
+  const double ms[3] = {m0, m1, m2}, d[6] = {s0, s1, s2, 1.0, 1.0, 1.0};
+  if (pose7 != nullptr) {
+    double* o = pose7 + 7 * i;
+    for (int k = 0; k < 3; ++k) o[k] = mu[k] * d[k] + ms[k];
+    const double vx = mu[3], vy = mu[4], vz = mu[5];
+    const double nn = sqrt(vx * vx + vy * vy + vz * vz);
+    const double f = nn > 0.0 ? sin(nn) / nn : 0.0;
+    o[3] = nn > 0.0 ? cos(nn) : 1.0;
+    o[4] = f * vx; o[5] = f * vy; o[6] = f * vz;
+  }
+  if (cov_out != nullptr)
+    for (int r = 0; r < 6; ++r)
+      for (int c = 0; c < 6; ++c) cov_out[36 * i + 6 * r + c] = d[r] * C[6 * r + c] * d[c];
+  double tt = 0.0, tq = 0.0;
+  for (int k = 0; k < 3; ++k) {
+    tt += d[k] * C[7 * k] * d[k];
+    tq += C[7 * (k + 3)];
+  }
+  t_std[i] = sqrt(tt);
+  q_std_deg[i] = 2.0 * sqrt(tq) * (180.0 / 3.14159265358979323846);
+}
+}  // namespace mapnet
+
+extern "C" int mapnet_sample_post(const double* mean, const double* cov, int64_t n, const double* pose_m3,
+                                  const double* pose_s3, double* pose7, double* cov_metric, double* t_std,
+                                  double* q_std_deg, void* stream) {
+  MN_CHECK(mean && cov && t_std && q_std_deg && n >= 1, "sample_post: bad argument");
+  MN_CHECK((pose_m3 == nullptr) == (pose_s3 == nullptr), "sample_post: pose_m3 and pose_s3 go together");
+  const int un = pose_m3 != nullptr;
+  MN_LAUNCH(k_sample_post, cdiv(n, 128), 128, 0, (cudaStream_t)stream, mean, cov, (long long)n, un ? pose_m3[0] : 0.0,
+            un ? pose_m3[1] : 0.0, un ? pose_m3[2] : 0.0, un ? pose_s3[0] : 1.0, un ? pose_s3[1] : 1.0,
+            un ? pose_s3[2] : 1.0, pose7, cov_metric, t_std, q_std_deg);
+  MN_LAUNCH_CHECK();
+  return 0;
+}

@@ -33,6 +33,7 @@ class Predictor(object):
         pr = Predictor(model, max_batch=64)
         poses = pr(x)       # [L,3,H,W] -> [L,6];  [L,T,3,H,W] -> [L,T,6];  max_batch frames per engine call
         pr.refresh()        # take a new snapshot of the model's current parameters / running statistics
+        mc = pr.sample(x, 32)   # droprate > 0: mean [L,6] / cov [L,6,6] of 32 dropout draws per frame, one trunk forward
         pr.close()
 
     Training the model afterwards does not change the predictor's output until ``refresh()``.  Precision, droprate and
@@ -73,6 +74,7 @@ class Predictor(object):
             raise ValueError("calibration frames are only used with precision='fp8'")
         self._engines = {}      # (H, W) -> _lib.Infer
         self._graphs = {}       # (B, H, W) -> (CUDAGraph, static input, static output)
+        self._sample_graphs = {}    # (B, H, W, S) -> (CUDAGraph, static input, static outputs)
         self._params = self._bufs = None
         self.refresh()
         if self._calib is not None:
@@ -150,8 +152,8 @@ class Predictor(object):
         graph.replay()
         return ps.clone()
 
-    @torch.no_grad()
-    def __call__(self, x):
+    def _frames(self, x):
+        """float32 frames [N,3,H,W] of an input [L,3,H,W] or [L,T,3,H,W]; raises on anything this predictor cannot run"""
         if not x.is_cuda:
             raise RuntimeError("geomapnet_b200.inference.Predictor has no CPU path: input must be a CUDA tensor "
                                "(got %s)" % x.device)
@@ -161,19 +163,98 @@ class Predictor(object):
             raise ValueError("empty batch")
         self._check_frames(x.shape[-2], x.shape[-1])
         frames = x.reshape(-1, *x.shape[-3:])
-        if frames.dtype != torch.float32:
-            frames = frames.float()
+        return frames if frames.dtype == torch.float32 else frames.float()
+
+    @torch.no_grad()
+    def __call__(self, x):
+        frames = self._frames(x)
         with torch.cuda.device(self.device):
             outs = [self._run(frames[i:i + self.max_batch]) for i in range(0, frames.shape[0], self.max_batch)]
         out = torch.cat(outs, 0)
         return out.view(*x.shape[:-3], 6)
 
+    def _sample_graph(self, B, H, W, S):
+        """(CUDA graph, static input [B,3,H,W], static outputs) of S dropout draws per frame for one batch shape,
+        captured after an eager run at an explicit dropout step, which leaves the engine's dropout counter alone"""
+        key = (B, H, W, S)
+        g = self._sample_graphs.get(key)
+        if g is None:
+            eng, dev, L = self._engine(H, W), self.device, _lib.lib()
+            xs = torch.zeros((B, 3, H, W), dtype=torch.float32, device=dev)
+            o = _sample_outputs(B, S, dev)
+
+            def launch(step):
+                eng.sample(xs, S, self.droprate, self.seed, o["samples"], o["mean"], o["cov"], step)
+                _lib.check(L.mapnet_sample_post(o["mean"].data_ptr(), o["cov"].data_ptr(), B, None, None, None, None,
+                                                o["t_std"].data_ptr(), o["q_std_deg"].data_ptr(), _lib.stream_ptr()),
+                           "mapnet_sample_post")
+
+            cur = torch.cuda.current_stream(dev)
+            side = torch.cuda.Stream(dev)
+            side.wait_stream(cur)
+            with torch.cuda.stream(side):        # eager run first: tile plans, tensor maps, kernel attributes
+                launch(0)
+            cur.wait_stream(side)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                launch(_lib.UINT64_MAX)
+            g = self._sample_graphs[key] = (graph, xs, o)
+        return g
+
+    @torch.no_grad()
+    def sample(self, x, S, keep_samples=False):
+        """Monte-Carlo dropout: S dropout draws of every frame's pose from one trunk forward.  x as for ``__call__``
+        ([L,3,H,W] or [L,T,3,H,W] on the GPU).  Returns dict(mean [...,6] float64, cov [...,6,6] float64 (two-pass,
+        divisor S - 1), t_std [...] = sqrt(trace of the translation block) in the model's normalised units, q_std_deg
+        [...] = 2 sqrt(trace of the log q block) in degrees, and samples [...,S,6] float32 when keep_samples).
+
+        Only the head differs between draws, so the trunk and the fc product run once per frame and one kernel forms
+        the S masks and products (csrc/head.cu, k_head_draws).  Draw s is bit for bit what the (s+1)-th of S calls
+        ``self(x)`` returns on the same frames, and the dropout counter ends where those S calls leave it.  Inputs of
+        more than max_batch frames run in chunks of max_batch; each chunk takes S consecutive dropout steps, in chunk
+        order (as S calls on the first chunk, then S calls on the next).  One graph per (B, H, W, S), replayed once per
+        chunk.  2 <= S <= 1024; a model without dropout (droprate == 0) has nothing to sample and raises ValueError."""
+        S = _check_draws(S, self.droprate)
+        frames = self._frames(x)
+        n, H, W, mb = frames.shape[0], frames.shape[2], frames.shape[3], self.max_batch
+        out = _sample_outputs(n, S, self.device, keep_samples)
+        with torch.cuda.device(self.device):
+            for lo in range(0, n, mb):
+                fb = frames[lo:lo + mb]
+                graph, xs, o = self._sample_graph(fb.shape[0], H, W, S)
+                xs.copy_(fb)
+                graph.replay()
+                for k, v in out.items():
+                    v[lo:lo + fb.shape[0]].copy_(o[k])
+        lead = tuple(x.shape[:-3])
+        return {k: v.view(*(lead + tuple(v.shape[1:]))) for k, v in out.items()}
+
     def close(self):
         self._graphs.clear()
+        self._sample_graphs.clear()
         for eng in self._engines.values():
             eng.close()
         self._engines.clear()
         self._params = self._bufs = self._calib = None
+
+
+def _check_draws(S, droprate):
+    """S as an int in [2, MAX_SAMPLE_DRAWS]; raises when there is no dropout to sample"""
+    if isinstance(S, bool) or not isinstance(S, (int, np.integer)) or not 2 <= S <= _lib.MAX_SAMPLE_DRAWS:
+        raise ValueError("S must be an int in [2, %d], got %r" % (_lib.MAX_SAMPLE_DRAWS, S))
+    if not droprate > 0:
+        raise ValueError("sample: the model has no dropout (droprate == 0), so every draw is the same pose")
+    return int(S)
+
+
+def _sample_outputs(n, S, dev, keep_samples=True):
+    """the device outputs of n frames' S-draw Monte-Carlo statistics"""
+    f64 = dict(dtype=torch.float64, device=dev)
+    out = dict(mean=torch.empty((n, 6), **f64), cov=torch.empty((n, 6, 6), **f64), t_std=torch.empty(n, **f64),
+               q_std_deg=torch.empty(n, **f64))
+    if keep_samples:
+        out["samples"] = torch.empty((n, S, 6), dtype=torch.float32, device=dev)
+    return out
 
 
 @torch.no_grad()
@@ -220,6 +301,7 @@ class Localizer(object):
         loc = Localizer(predictor, mean, std, pose_m=None, pose_s=None, size=256)
         poses = loc(frames)     # uint8 [L,H,W,3] or [H,W,3] (RGB, as PIL decodes), a CUDA or host tensor or an ndarray
                                 # -> float64 [L,7] (or [7]) on the device: (t * pose_s + pose_m, qexp(log q))
+        mc = loc.sample(frames, 32)     # droprate > 0: metric mean pose7 [L,7] and cov [L,6,6] of 32 dropout draws
         loc.close()
 
     ``loc(frames)`` is bit for bit ``post(predictor(ImagePipeline(mean, std, size)(frames.cuda())), pose_m, pose_s)``,
@@ -250,6 +332,7 @@ class Localizer(object):
         self._plans = {}        # (H_in, W_in) -> mapnet_preprocess_t of max_batch frames
         self._graphs = {}       # (B, H_in, W_in) -> (CUDAGraph, static uint8 input, static float64 output, pred6)
         self._warm = set()      # engine shapes (B, H', W') whose eager run has drawn a dropout mask
+        self._sample_graphs = {}    # (B, H_in, W_in, S) -> (CUDAGraph, static uint8 input, static outputs)
         self._open = True
 
     def _resized(self, H, W):
@@ -310,8 +393,9 @@ class Localizer(object):
         graph.replay()
         return out.clone()
 
-    @torch.no_grad()
-    def __call__(self, frames):
+    def _frames(self, frames):
+        """(contiguous uint8 frames [L,H,W,3], whether a single [H,W,3] frame was given); raises on anything this
+        Localizer cannot run"""
         if not self._open or self.predictor._params is None:
             raise ValueError("Localizer is closed" if not self._open else "the Localizer's Predictor is closed")
         if isinstance(frames, np.ndarray):
@@ -327,18 +411,91 @@ class Localizer(object):
         if x.shape[0] < 1 or x.shape[1] < 1 or x.shape[2] < 1:
             raise ValueError("empty batch: frames of shape %s" % (tuple(frames.shape),))
         self.predictor._check_frames(*self._resized(x.shape[1], x.shape[2]))
-        x = x.contiguous()
+        return x.contiguous(), single
+
+    @torch.no_grad()
+    def __call__(self, frames):
+        x, single = self._frames(frames)
         mb = self.predictor.max_batch
         with torch.cuda.device(self.predictor.device):
             outs = [self._run(x[i:i + mb]) for i in range(0, x.shape[0], mb)]
         out = outs[0] if len(outs) == 1 else torch.cat(outs, 0)
         return out[0] if single else out
 
+    def _sample_launch(self, eng, pre, xs, o, S, step):
+        """the sample call's library launches on the current stream: frames xs -> S draws -> float64 metric post"""
+        pr, L, B = self.predictor, _lib.lib(), xs.shape[0]
+        fp = ctypes.POINTER(ctypes.c_float)
+        _lib.check(L.mapnet_infer_sample_frames(eng.h, pre, xs.data_ptr(), B, self.mean.ctypes.data_as(fp),
+                                                self.std.ctypes.data_as(fp), S, pr.droprate, int(pr.seed), step,
+                                                o["samples"].data_ptr(), o["mean"].data_ptr(), o["cov6"].data_ptr(),
+                                                _lib.stream_ptr()), "mapnet_infer_sample_frames")
+        _lib.check(L.mapnet_sample_post(o["mean"].data_ptr(), o["cov6"].data_ptr(), B, self._m, self._s,
+                                        o["pose7"].data_ptr(), o["cov"].data_ptr(), o["t_std"].data_ptr(),
+                                        o["q_std_deg"].data_ptr(), _lib.stream_ptr()), "mapnet_sample_post")
+
+    def _sample_graph(self, fb, S):
+        """(CUDA graph, static input, static outputs) of S draws per frame for frames shaped like fb, captured after an
+        eager run at an explicit dropout step (the dropout counter is left alone)"""
+        B, H, W = fb.shape[:3]
+        g = self._sample_graphs.get((B, H, W, S))
+        if g is None:
+            pr = self.predictor
+            eng, pre = pr._engine(*self._resized(H, W)), self._plan(H, W)
+            xs = torch.empty((B, H, W, 3), dtype=torch.uint8, device=pr.device)
+            xs.copy_(fb)
+            o = _sample_outputs(B, S, pr.device)
+            o["cov6"] = torch.empty_like(o["cov"])
+            o["pose7"] = torch.empty((B, 7), dtype=torch.float64, device=pr.device)
+            cur = torch.cuda.current_stream(pr.device)
+            side = torch.cuda.Stream(pr.device)
+            side.wait_stream(cur)
+            with torch.cuda.stream(side):        # eager run first: tile plans, tensor maps, kernel attributes
+                self._sample_launch(eng, pre, xs, o, S, 0)
+            cur.wait_stream(side)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                self._sample_launch(eng, pre, xs, o, S, _lib.UINT64_MAX)
+            g = self._sample_graphs[(B, H, W, S)] = (graph, xs, o)
+        return g
+
+    @torch.no_grad()
+    def sample(self, frames, S, keep_samples=False):
+        """Monte-Carlo dropout poses: S dropout draws of every frame's pose from one trunk forward, in metric units.
+        frames as for ``__call__``.  Returns dict(pose7 [L,7] float64 = (mean_t * pose_s + pose_m, qexp(mean log q)),
+        cov [L,6,6] float64 = D cov D with D = diag(pose_s, 1, 1, 1) (translation block in metres, log q block
+        unscaled), t_std [L] = sqrt(trace of the translation block), q_std_deg [L] = 2 sqrt(trace of the log q block)
+        in degrees, and samples [L,S,6] float32 -- the draws in the model's normalised units -- when keep_samples); a
+        single [H,W,3] frame drops the leading L.  Without pose_m / pose_s, D is the identity.
+
+        Draw s is bit for bit what the (s+1)-th of S calls ``self(frames)`` draws (Predictor.sample); the Localizer
+        shares the predictor's engines and dropout counter as ``__call__`` does, and longer inputs run in chunks of
+        max_batch frames, each taking S consecutive dropout steps.  Each chunk replays one graph: the resize, the fused
+        stem operand, the engine, the draws and the float64 post step.  2 <= S <= 1024; a model without dropout raises
+        ValueError."""
+        x, single = self._frames(frames)
+        pr = self.predictor
+        S = _check_draws(S, pr.droprate)
+        n, mb = x.shape[0], pr.max_batch
+        out = _sample_outputs(n, S, pr.device, keep_samples)
+        del out["mean"]                                 # the normalised mean: pose7 is what a caller of loc uses
+        out["pose7"] = torch.empty((n, 7), dtype=torch.float64, device=pr.device)
+        with torch.cuda.device(pr.device):
+            for lo in range(0, n, mb):
+                fb = x[lo:lo + mb]
+                graph, xs, o = self._sample_graph(fb, S)
+                xs.copy_(fb, non_blocking=True)
+                graph.replay()
+                for k, v in out.items():
+                    v[lo:lo + fb.shape[0]].copy_(o[k])
+        return {k: v[0] for k, v in out.items()} if single else out
+
     def close(self):
         """Free the graphs and preprocess plans (the predictor stays open)."""
         if self._graphs or self._plans:
             torch.cuda.current_stream(self.predictor.device).synchronize()
         self._graphs.clear()
+        self._sample_graphs.clear()
         for h in self._plans.values():
             _lib.lib().mapnet_preprocess_destroy(h)
         self._plans.clear()

@@ -261,6 +261,31 @@ int mapnet_infer_forward_frames(mapnet_infer_t* h, mapnet_preprocess_t* pre, con
                                 const float* mean3, const float* std3, float droprate, uint64_t seed, uint64_t step,
                                 float* pred, void* stream);
 
+/* mapnet_infer_sample: Monte-Carlo dropout -- S draws of the pose head per frame from ONE trunk forward of x
+ * [B,3,H,W].  The trunk output and the fc pre-activation are the same for every draw, so the trunk and the fc product
+ * run once and one kernel forms each draw's dropout mask on the fly and its two feat_dim -> 3 products.  Draw s is bit
+ * for bit the pred the (s+1)-th of S consecutive mapnet_infer_forward calls on the same B frames returns: it uses
+ * dropout step c + s, and the products keep the forward's split-K summation order for B rows.  step == UINT64_MAX
+ * takes c from the engine's device step counter and advances it by S (graph-capturable, as mapnet_infer_forward);
+ * otherwise c = step and the counter is not touched.  Outputs (device memory): samples [B][S][6] float32 (NULL: not
+ * stored), mean [B][6] (the draws summed in s order, / S) and cov [B][6][6] (two-pass, divisor S - 1), float64,
+ * deterministic.  Refused before any launch: S outside [2, 1024], droprate outside (0, 1), B outside [1, max_B], a
+ * call before a load, an uncalibrated fp8 engine.
+ * mapnet_infer_sample_frames: the same from camera frames through pre, with mapnet_infer_forward_frames' stem operand
+ * and checks.  Graph-capturable. */
+int mapnet_infer_sample(mapnet_infer_t* h, const float* x, int B, int S, float droprate, uint64_t seed, uint64_t step,
+                        float* samples, double* mean, double* cov, void* stream);
+int mapnet_infer_sample_frames(mapnet_infer_t* h, mapnet_preprocess_t* pre, const void* frames_nhwc_u8, int B,
+                               const float* mean3, const float* std3, int S, float droprate, uint64_t seed,
+                               uint64_t step, float* samples, double* mean, double* cov, void* stream);
+/* mapnet_sample_post: metric poses and spreads of n Monte-Carlo means / covariances (mapnet_infer_sample's mean
+ * [n][6], cov [n][6][6]), float64: with D = diag(pose_s, 1, 1, 1), pose7 = (mean_t * pose_s + pose_m, qexp(mean_logq))
+ * (qexp in float64: (cos |v|, sin |v| / |v| * v), (1, 0, 0, 0) at v = 0), cov_metric = D cov D, t_std = sqrt(trace of
+ * cov_metric's translation block), q_std_deg = 2 sqrt(trace of the log q block) * 180 / pi.  pose_m3 / pose_s3: HOST
+ * pointers or both NULL (D = I); pose7 / cov_metric may be NULL (not stored).  Device outputs, one launch. */
+int mapnet_sample_post(const double* mean, const double* cov, int64_t n, const double* pose_m3, const double* pose_s3,
+                       double* pose7, double* cov_metric, double* t_std, double* q_std_deg, void* stream);
+
 /* ---- measurement support (bench.py): number of kernels this library has launched so
  * far in this process, and per-class conv timing with CUDA events on the launching
  * stream (class 0 fprop, 1 dgrad, 2 wgrad; algorithmic FLOPs of each launch summed). */
@@ -364,6 +389,10 @@ int mapnet_test_stem(int B, int H, int W, const float* x_nchw, const float* w_oi
  * mean3 / std3: host, frames only. */
 int mapnet_test_stem_operand(int precision, mapnet_preprocess_t* pre, const void* frames_nhwc_u8, const float* x_nchw,
                              int B, const float* mean3, const float* std3, void* S, void* stream);
+
+/* host-only: the split-K plan of the head's small fp32 GEMM for an [M,K] x [N,K]^T product with epilogue epi -- the
+ * number of K splits and the length of each but the last (the plan mapnet_infer_sample reproduces for B rows) */
+int mapnet_test_small_gemm_plan(int epi, int M, int N, int K, int* splits, int* kchunk);
 
 /* micro-benchmark of one tensor-core conv configuration (tools/bench_conv.py): average ms per launch */
 int mapnet_bench_conv(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* in0,
