@@ -252,16 +252,29 @@ int mapnet_test_conv_ex(int precision, int kind, int B, int Hi, int Wi, int Ci, 
 }
 
 // JSON description of the plan the tensor-core engines would use for this conv (no device needed).  flags: bit 0 folds
-// the downsample shortcut into a stride-2 dgrad; bit 1 describes the strict-mode (split-operand) plan instead of bf16's
+// the downsample shortcut into a stride-2 dgrad; bit 1 describes the strict-mode (split-operand) plan instead of bf16's;
+// bit 2 describes the fp8 fprop plan (tc_plan_create_f8).  k == 7 (fprop): the stem as the engines run it, the 4x1 conv
+// on the space-to-depth image of an Hi x Wi frame (mapnet_test_conv_affine's k == 7)
 int mapnet_test_plan_describe(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, int flags,
                               char* buf, int cap) {
+  MN_CHECK(!(flags & 4) || (kind == 0 && !(flags & 3)),
+           "test_plan_describe: flag 4 (fp8) describes an fprop plan, without flags 1 or 2");
   ConvGeom g;
-  g.B = B; g.Hi = Hi; g.Wi = Wi; g.Ci = Ci; g.Co = Co; g.KH = g.KW = k; g.stride = stride; g.pad = (k - 1) / 2;
-  g.Ho = (Hi + 2 * g.pad - k) / stride + 1; g.Wo = (Wi + 2 * g.pad - k) / stride + 1;
+  if (k == 7) {
+    MN_CHECK(kind == 0 && Ci == 3 && Co == 64 && stride == 2 && !(flags & 5), "test_plan_describe: the stem is a 7x7/s2 "
+             "fprop, 3 -> 64");
+    WeightDesc wd;
+    stem_s2d_geometry(Hi, Wi, 64, &g, &wd, (flags & 2) ? 4 : 2);
+  } else {
+    g.Hi = Hi; g.Wi = Wi; g.Ci = Ci; g.Co = Co; g.KH = g.KW = k; g.stride = stride; g.pad = (k - 1) / 2;
+    g.Ho = (Hi + 2 * g.pad - k) / stride + 1; g.Wo = (Wi + 2 * g.pad - k) / stride + 1;
+  }
+  g.B = B;
   if (flags & 2) g.split = 1;
   TcConvPlan* plan = nullptr;
   static const bf16 dummy[8] = {};
-  MN_TRY(tc_plan_create(&plan, g, kind, dummy));
+  if (flags & 4) MN_TRY(tc_plan_create_f8(&plan, g, (const uint8_t*)dummy));
+  else MN_TRY(tc_plan_create(&plan, g, kind, dummy));
   int r = 0;
   if (flags & 1) r = tc_plan_add_shortcut(plan, dummy);
   if (r == 0) r = tc_plan_describe(plan, buf, cap);

@@ -1351,7 +1351,7 @@ int tc_plan_describe(const TcConvPlan* p, char* buf, int cap) {
     va_end(ap);
     if (w < 0 || w >= cap - n) ovf = true; else n += w;
   };
-  put("{\"kind\":%d,\"BN\":%d,\"shortcut\":%d", p->kind, p->BN, p->wmat2 != nullptr ? 1 : 0);
+  put("{\"kind\":%d,\"BN\":%d,\"shortcut\":%d,\"f8_kb\":%d", p->kind, p->BN, p->wmat2 != nullptr ? 1 : 0, p->f8_kb);
   if (p->kind == 2) {
     const WgradParams& P = p->WP;
     put(",\"wgrad\":{\"TW\":%d,\"TH\":%d,\"TN\":%d,\"tiles_w\":%d,\"tiles_h\":%d,\"tiles_n\":%d,\"n_pix_tiles\":%d,"

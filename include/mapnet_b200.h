@@ -306,7 +306,10 @@ int mapnet_test_conv_ex(int precision, int kind, int B, int Hi, int Wi, int Ci, 
 
 /* host-only: the tile / parity-class / filter-tap plan of the tensor-core engines for one conv, as JSON
  * (tests/test_tc_plan.py replays it on the CPU against torch's convolutions; kind 0 fprop, 1 dgrad, 2 wgrad).
- * flags: bit 0 folds the downsample shortcut into a 3x3/s2 dgrad; bit 1 describes the strict-mode (tc_split) plan. */
+ * flags: bit 0 folds the downsample shortcut into a 3x3/s2 dgrad; bit 1 describes the strict-mode (tc_split) plan;
+ * bit 2 describes the fp8 fprop plan of mapnet_test_conv_fp8 (kind 0, alone).  "f8_kb" is the fp8 plan's bytes per
+ * k-block row (128, or 64 when Ci = 64), 0 for every other plan.  k == 7 (kind 0, Ci 3, Co 64, stride 2) describes the
+ * stem as mapnet_test_conv_affine's k == 7 runs it: a 4x1 conv on the space-to-depth image of an Hi x Wi frame. */
 int mapnet_test_plan_describe(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, int flags,
                               char* buf, int cap);
 
