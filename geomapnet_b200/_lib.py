@@ -17,6 +17,10 @@ INFER_PREC = {"bf16": 1, "tc_split": 3, "fp8": 4}
 N_F8_TENSORS = 33      # e4m3 activation tensors of the fp8 engine at ResNet-34: the pool output, 16 x (h, block output)
 LOSS_MODE = {"posenet": 0, "mapnet": 1, "online": 2, "online_gps": 3}
 
+TRACK_API = ["mapnet_track_create", "mapnet_track_step", "mapnet_track_flush", "mapnet_track_reset", "mapnet_track_status",
+             "mapnet_track_destroy"]
+MAX_TRACK_STEPS = 16    # mapnet_track_create: windows of at most 16 frames (the PGO kernel's limit)
+
 _lib = None
 
 
@@ -141,6 +145,14 @@ def lib():
     L.mapnet_test_small_gemm_plan.argtypes = [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int)]
     for name in ("mapnet_infer_sample", "mapnet_infer_sample_frames", "mapnet_sample_post", "mapnet_test_small_gemm_plan"):
         getattr(L, name).restype = c_int
+    L.mapnet_track_create.argtypes = [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]
+    L.mapnet_track_step.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]
+    L.mapnet_track_flush.argtypes = [c_void_p, c_void_p, c_void_p]
+    L.mapnet_track_reset.argtypes = [c_void_p, c_void_p]
+    L.mapnet_track_status.argtypes = [c_void_p, POINTER(c_int64), POINTER(c_int), c_void_p]
+    L.mapnet_track_destroy.argtypes = [c_void_p]
+    for name in TRACK_API:
+        getattr(L, name).restype = c_int
     L.mapnet_test_stem_operand.argtypes = [c_int, c_void_p, c_void_p, c_void_p, c_int, POINTER(c_float), POINTER(c_float),
                                            c_void_p, c_void_p]
     L.mapnet_test_stem_operand.restype = c_int
@@ -179,7 +191,7 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_test_bn_forward", "mapnet_test_bn_backward", "mapnet_test_stem_pool", "mapnet_test_gap",
             "mapnet_trunk_set_trainable", "mapnet_test_conv_ex", "mapnet_eval_windows",
             "mapnet_batch_losses", "mapnet_infer_forward_frames", "mapnet_test_stem_operand", "mapnet_infer_sample",
-            "mapnet_infer_sample_frames", "mapnet_sample_post", "mapnet_test_small_gemm_plan"]
+            "mapnet_infer_sample_frames", "mapnet_sample_post", "mapnet_test_small_gemm_plan"] + TRACK_API
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 MAX_SAMPLE_DRAWS = 1024      # mapnet_infer_sample: S in [2, MAX_SAMPLE_DRAWS] dropout draws per frame
 

@@ -12,6 +12,7 @@
 #include "jitter_core.h"
 #include "pose_math.h"
 #include "pose_post.cuh"
+#include "track_core.h"
 
 #include "../../include/mapnet_b200.h"
 
@@ -102,6 +103,88 @@ k_eval_windows(const float* __restrict__ pred6, const float* __restrict__ poses,
     const float v6[6] = {v.t.x, v.t.y, v.t.z, v.l.x, v.l.y, v.l.z};
     st_pose7(v6, vos7 + 7LL * k);
   }
+}
+
+// ---- streaming pose-graph tracker (mapnet_track_*, inference.Tracker): eval.py's windows over frames as they arrive.
+// Device state of one sequence: `seen` frames so far; n_win: the windows the current call completes, written by
+// k_track_gather for k_pgo and k_track_emit; status: 1 once a window's normal matrix was not positive definite.
+struct TrackDev {
+  long long seen;
+  int n_win, status;
+};
+
+__device__ __forceinline__ const float* track_src(const float* fresh, const float* ring, long long f, long long seen,
+                                                  long long R) {
+  return f >= seen ? fresh + 6 * (f - seen) : ring + 6 * (f % R);
+}
+
+// One thread per row: the n new frames into the rings (pose7 of pred6, the VO-library pose as given), then slot
+// (w, k) of every completed window w < n_win (rows n .. n + max_win*T - 1), then VO (w, e) (the next max_win*E rows).
+// A slot's frame comes from this call's inputs when it is new, else from the ring: R = max_batch + (T-1)*skip frames
+// hold every older frame a window of this call reaches, none of them in a ring slot this call writes.  The values are
+// k_eval_windows': st_pose7 of the float32 pose, calc_vo_logq_safe of the float32 VO-library poses.
+__global__ void __launch_bounds__(128)
+k_track_gather(const float* __restrict__ pred6, const float* __restrict__ vo6, int n, int flush,
+               TrackDev* __restrict__ st, double* __restrict__ ring7, float* __restrict__ ring_vo, long long R, int T,
+               int skip, int fc, int max_win, double* __restrict__ win7, double* __restrict__ vos7) {
+  pdl_prologue();
+  const long long seen = st->seen, total = seen + n, lag = trackcore::lag(T, skip);
+  const long long first = trackcore::first_pending(seen, lag);
+  const int n_win = (int)((flush ? total : trackcore::first_pending(total, lag)) - first);
+  const int E = fc ? T * (T - 1) / 2 : T - 1;
+  long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r == 0) st->n_win = n_win;
+  if (r < n) {
+    const long long f = seen + r;
+    st_pose7(pred6 + 6 * r, ring7 + 7 * (f % R));
+#pragma unroll
+    for (int c = 0; c < 6; ++c) ring_vo[6 * (f % R) + c] = vo6[6 * r + c];
+    return;
+  }
+  r -= n;
+  if (r < (long long)max_win * T) {
+    const int w = (int)(r / T), k = (int)(r % T);
+    if (w >= n_win) return;
+    const long long f = trackcore::slot_frame(first + w, k, T, skip, total - 1);
+    if (f >= seen) st_pose7(pred6 + 6 * (f - seen), win7 + 7 * r);
+    else {
+#pragma unroll
+      for (int c = 0; c < 7; ++c) win7[7 * r + c] = ring7[7 * (f % R) + c];
+    }
+    return;
+  }
+  r -= (long long)max_win * T;
+  if (r < (long long)max_win * E) {
+    const int w = (int)(r / E), e = (int)(r % E);
+    if (w >= n_win) return;
+    int i, j;
+    trackcore::vo_pair(e, T, fc, &i, &j);
+    const long long fa = trackcore::slot_frame(first + w, i, T, skip, total - 1);
+    const long long fb = trackcore::slot_frame(first + w, j, T, skip, total - 1);
+    const posemath::Pose6 v = posemath::calc_vo_logq_safe(ld_pose6(track_src(vo6, ring_vo, fa, seen, R)),
+                                                          ld_pose6(track_src(vo6, ring_vo, fb, seen, R)));
+    const float v6[6] = {v.t.x, v.t.y, v.t.z, v.l.x, v.l.y, v.l.z};
+    st_pose7(v6, vos7 + 7 * r);
+  }
+}
+
+// One thread per completed window: its optimised middle slot, translations un-normalised as _window_errors does
+// (un = 0: kept), into out7 row w; thread 0 advances the frame counter by the call's n frames.
+__global__ void __launch_bounds__(128)
+k_track_emit(const double* __restrict__ opt7, TrackDev* __restrict__ st, int n, int T, int un, double m0,
+             double m1, double m2, double s0, double s1, double s2, double* __restrict__ out7) {
+  pdl_prologue();
+  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+  const int n_win = st->n_win;
+  if (w == 0) st->seen += n;
+  if (w >= n_win) return;
+  const double* p = opt7 + 7 * ((long long)w * T + T / 2);
+  double* o = out7 + 7LL * w;
+  const double ms[3] = {m0, m1, m2}, ss[3] = {s0, s1, s2};
+#pragma unroll
+  for (int k = 0; k < 3; ++k) o[k] = un ? trackcore::unnormalize(p[k], ss[k], ms[k]) : p[k];
+#pragma unroll
+  for (int k = 3; k < 7; ++k) o[k] = p[k];
 }
 
 }  // namespace mapnet
@@ -261,6 +344,113 @@ int mapnet_eval_windows(const float* pred6, int n_pred, const float* poses, cons
             (const int*)(d + n_rows), n_rows, (const TargRow*)(d + 2 * n_rows), n_vo, pred7, targ7, vos7);
   MN_LAUNCH_CHECK();
   MN_CUDA(cudaFreeAsync(d, st));
+  return 0;
+}
+
+}  // extern "C"
+
+struct mapnet_track {
+  int T, skip, fc, max_batch, E, max_win;   // max_win: the most windows one call completes, max(max_batch, lag)
+  long long R, lag;
+  double w4[4];                             // PGO weights 1/sqrt(sigma) of sax, saq, srx, srq
+  int un;
+  double m[3], s[3];
+  TrackDev* st;
+  double* ring7;                            // [R][7]: pose7 of the last R frames, normalised translations
+  float* ring_vo;                           // [R][6]: their VO-library poses
+  double *win7, *vos7, *opt7;               // [max_win][T][7], [max_win][E][7], [max_win][T][7]
+};
+
+// the three launches of one call: n new frames (a step) or none (flush), out7 [max_win][7]
+static int track_launch(mapnet_track_t* h, const float* pred6, const float* vo6, int n, int flush, double* out7,
+                        cudaStream_t st) {
+  const int nw = flush ? (int)(h->lag < h->max_win ? h->lag : h->max_win) : n;   // the grid's windows
+  const long long rows = n + (long long)nw * (h->T + h->E);
+  MN_LAUNCH(k_track_gather, cdiv(rows, 128), 128, 0, st, pred6, vo6, n, flush, h->st, h->ring7, h->ring_vo, h->R, h->T,
+            h->skip, h->fc, nw, h->win7, h->vos7);
+  MN_LAUNCH_CHECK();
+  MN_TRY(launch_pgo(h->win7, h->vos7, h->opt7, nw, h->T, h->fc, h->w4, 10, 0, &h->st->status, &h->st->n_win, st));
+  MN_LAUNCH(k_track_emit, cdiv(nw, 128), 128, 0, st, (const double*)h->opt7, h->st, n, h->T, h->un, h->m[0], h->m[1],
+            h->m[2], h->s[0], h->s[1], h->s[2], out7);
+  MN_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" {
+
+int mapnet_track_create(mapnet_track_t** out, int T, int skip, int fc_vos, int max_batch, const double* sigmas4,
+                        const double* pose_m3, const double* pose_s3) {
+  MN_CHECK(out != nullptr && sigmas4 != nullptr, "track_create: null argument");
+  *out = nullptr;
+  MN_CHECK(T >= 2 && T <= 16, "track_create: windows of %d frames outside [2, 16]", T);
+  MN_CHECK(skip >= 1 && max_batch >= 1, "track_create: skip = %d and max_batch = %d must be >= 1", skip, max_batch);
+  for (int k = 0; k < 4; ++k) MN_CHECK(sigmas4[k] > 0, "track_create: sigma %d = %g must be positive", k, sigmas4[k]);
+  MN_CHECK((pose_m3 == nullptr) == (pose_s3 == nullptr), "track_create: pose_m3 and pose_s3 go together");
+  const long long lag = trackcore::lag(T, skip), R = trackcore::ring_frames(max_batch, T, skip);
+  MN_CHECK(R < (1LL << 26), "track_create: a ring of %lld frames", R);
+  int ndev = 0;
+  MN_CHECK(cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0, "track_create: no CUDA device (this library has no CPU fallback)");
+  MN_TRY(pgo_prepare());
+  mapnet_track* h = new mapnet_track();
+  h->T = T; h->skip = skip; h->fc = fc_vos ? 1 : 0; h->max_batch = max_batch;
+  h->E = h->fc ? T * (T - 1) / 2 : T - 1;
+  h->lag = lag; h->R = R;
+  h->max_win = (int)(lag > max_batch ? lag : max_batch);
+  pgo_weights(sigmas4[0], sigmas4[1], sigmas4[2], sigmas4[3], h->w4);
+  h->un = pose_m3 != nullptr;
+  for (int k = 0; k < 3; ++k) { h->m[k] = h->un ? pose_m3[k] : 0.0; h->s[k] = h->un ? pose_s3[k] : 1.0; }
+  const size_t W = (size_t)h->max_win;
+  bool ok = cudaMalloc((void**)&h->st, sizeof(TrackDev)) == cudaSuccess &&
+            cudaMalloc((void**)&h->ring7, (size_t)R * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->ring_vo, (size_t)R * 6 * sizeof(float)) == cudaSuccess &&
+            cudaMalloc((void**)&h->win7, W * T * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->vos7, W * h->E * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->opt7, W * T * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMemset(h->st, 0, sizeof(TrackDev)) == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess;
+  if (!ok) {
+    cudaGetLastError();
+    set_last_error("track_create: device allocation of a ring of %lld frames and %d windows failed", R, h->max_win);
+    mapnet_track_destroy(h);
+    return 1;
+  }
+  *out = h;
+  return 0;
+}
+
+int mapnet_track_step(mapnet_track_t* h, const float* pred6, const float* vo6, int B, double* out7, void* stream) {
+  MN_CHECK(h != nullptr, "track_step: null handle");
+  MN_CHECK(pred6 != nullptr && vo6 != nullptr && out7 != nullptr, "track_step: null argument");
+  MN_CHECK(B >= 1 && B <= h->max_batch, "track_step: %d frames outside [1, max_batch=%d]", B, h->max_batch);
+  return track_launch(h, pred6, vo6, B, 0, out7, (cudaStream_t)stream);
+}
+
+int mapnet_track_flush(mapnet_track_t* h, double* out7, void* stream) {
+  MN_CHECK(h != nullptr, "track_flush: null handle");
+  MN_CHECK(out7 != nullptr, "track_flush: null argument");
+  if (h->lag == 0) return 0;                 // every window was complete when its last frame arrived
+  return track_launch(h, nullptr, nullptr, 0, 1, out7, (cudaStream_t)stream);
+}
+
+int mapnet_track_reset(mapnet_track_t* h, void* stream) {
+  MN_CHECK(h != nullptr, "track_reset: null handle");
+  MN_CUDA(cudaMemsetAsync(h->st, 0, sizeof(TrackDev), (cudaStream_t)stream));
+  return 0;
+}
+
+int mapnet_track_status(mapnet_track_t* h, int64_t* frames_seen, int* failed, void* stream) {
+  MN_CHECK(h != nullptr, "track_status: null handle");
+  TrackDev d;
+  MN_CUDA(cudaMemcpyAsync(&d, h->st, sizeof(TrackDev), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  MN_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+  if (frames_seen != nullptr) *frames_seen = d.seen;
+  if (failed != nullptr) *failed = d.status;
+  return 0;
+}
+
+int mapnet_track_destroy(mapnet_track_t* h) {
+  if (h == nullptr) return 0;
+  cudaFree(h->st); cudaFree(h->ring7); cudaFree(h->ring_vo); cudaFree(h->win7); cudaFree(h->vos7); cudaFree(h->opt7);
+  delete h;
   return 0;
 }
 

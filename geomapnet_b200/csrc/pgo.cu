@@ -79,9 +79,14 @@ __device__ __forceinline__ void dqstq_t(const Q4& q, double D[3][3]) {
 
 // One window per block.  Constraints are dealt to threads; each thread accumulates into the shared H / b with
 // double atomics (a few hundred constraints x <= 144 entries: contention is irrelevant next to the Cholesky).
+// n_win_dev (may be null): the device count of windows to optimise; the blocks beyond it exit, so a captured graph can
+// keep a fixed grid while the count changes from replay to replay.
 __global__ void __launch_bounds__(kPgoThreads)
 k_pgo(const double* __restrict__ poses, const double* __restrict__ vos, double* __restrict__ out, int N, int fc,
-      double w_ax, double w_aq, double w_rx, double w_rq, int n_iters, int exact, int* __restrict__ status) {
+      double w_ax, double w_aq, double w_rx, double w_rq, int n_iters, int exact, int* __restrict__ status,
+      const int* __restrict__ n_win_dev) {
+  pdl_prologue();
+  if (n_win_dev != nullptr && (int)blockIdx.x >= *n_win_dev) return;
   extern __shared__ double sm[];
   const int D = 6 * N;
   double* H = sm;                 // D x D
@@ -240,6 +245,27 @@ k_pgo(const double* __restrict__ poses, const double* __restrict__ vos, double* 
   if (threadIdx.x == 0 && s_fail && status != nullptr) atomicExch(status, 1);
 }
 
+int pgo_prepare() {
+  static bool attr = false;
+  if (!attr) { MN_CUDA(cudaFuncSetAttribute(k_pgo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(96 * 96 + 96 * 2 + 7 * 16) * 8)); attr = true; }
+  return 0;
+}
+
+int launch_pgo(const double* poses, const double* vos, double* out, int n_windows, int N, int fc, const double w4[4],
+               int n_iters, int exact, int* status, const int* n_win_dev, cudaStream_t st) {
+  MN_TRY(pgo_prepare());
+  const int D = 6 * N;
+  const size_t smem = (size_t)(D * D + D + 7 * N + D) * sizeof(double);
+  MN_LAUNCH(k_pgo, n_windows, kPgoThreads, smem, st, poses, vos, out, N, fc, w4[0], w4[1], w4[2], w4[3], n_iters, exact,
+            status, n_win_dev);
+  MN_LAUNCH_CHECK();
+  return 0;
+}
+
+void pgo_weights(double sax, double saq, double srx, double srq, double w4[4]) {
+  w4[0] = 1.0 / sqrt(sax); w4[1] = 1.0 / sqrt(saq); w4[2] = 1.0 / sqrt(srx); w4[3] = 1.0 / sqrt(srq);
+}
+
 }  // namespace mapnet
 
 using namespace mapnet;
@@ -252,14 +278,10 @@ extern "C" int mapnet_pgo_optimize(const double* poses, const double* vos, doubl
   MN_CHECK(sax > 0 && saq > 0 && srx > 0 && srq > 0 && n_iters >= 0, "pgo_optimize: covariances must be positive");
   int ndev = 0;
   MN_CHECK(cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0, "pgo_optimize: no CUDA device (this library has no CPU fallback)");
-  const int D = 6 * N;
-  const size_t smem = (size_t)(D * D + D + 7 * N + D) * sizeof(double);
-  static bool attr = false;
-  if (!attr) { MN_CUDA(cudaFuncSetAttribute(k_pgo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(96 * 96 + 96 * 2 + 7 * 16) * 8)); attr = true; }
-  MN_LAUNCH(k_pgo, n_windows, kPgoThreads, smem, (cudaStream_t)stream, poses, vos, out, N, fc_vos ? 1 : 0, 1.0 / sqrt(sax),
-            1.0 / sqrt(saq), 1.0 / sqrt(srx), 1.0 / sqrt(srq), n_iters, flags & 1, status_dev);
-  MN_LAUNCH_CHECK();
-  return 0;
+  double w4[4];
+  pgo_weights(sax, saq, srx, srq, w4);
+  return launch_pgo(poses, vos, out, n_windows, N, fc_vos ? 1 : 0, w4, n_iters, flags & 1, status_dev, nullptr,
+                    (cudaStream_t)stream);
 }
 
 // qexp + un-normalisation of a batch of 6-vectors (scripts/eval.py:163-181): out[i] = (t * pose_s + pose_m, qexp(logq))

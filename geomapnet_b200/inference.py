@@ -23,7 +23,7 @@ from . import _lib
 from .common.pgo import optimize_pose_windows
 from .data.loader import SidePipeline
 
-__all__ = ["Predictor", "Localizer", "predict", "post", "pgo", "pose_errors", "evaluate_tuples", "evaluate_sequence", "validate"]
+__all__ = ["Predictor", "Localizer", "Tracker", "predict", "post", "pgo", "pose_errors", "evaluate_tuples", "evaluate_sequence", "validate"]
 
 
 class Predictor(object):
@@ -349,41 +349,59 @@ class Localizer(object):
             self._plans[(H, W)] = h
         return h
 
+    def _forward(self, eng, pre, xs, pred, droprate):
+        """the engine's launches on the current stream: frames xs -> pred [B,6]"""
+        fp = ctypes.POINTER(ctypes.c_float)
+        _lib.check(_lib.lib().mapnet_infer_forward_frames(
+            eng.h, pre, xs.data_ptr(), xs.shape[0], self.mean.ctypes.data_as(fp), self.std.ctypes.data_as(fp),
+            droprate, int(self.predictor.seed), _lib.UINT64_MAX, pred.data_ptr(), _lib.stream_ptr()),
+            "mapnet_infer_forward_frames")
+
+    def _post(self, pred, out):
+        _lib.check(_lib.lib().mapnet_pose_post(pred.data_ptr(), out.data_ptr(), pred.shape[0], self._m, self._s,
+                                               _lib.stream_ptr()), "mapnet_pose_post")
+
     def _launch(self, eng, pre, xs, pred, out, droprate):
         """the call's library launches on the current stream: frames xs -> pred [B,6] -> out [B,7]"""
-        pr, L, B = self.predictor, _lib.lib(), xs.shape[0]
-        fp = ctypes.POINTER(ctypes.c_float)
-        _lib.check(L.mapnet_infer_forward_frames(eng.h, pre, xs.data_ptr(), B, self.mean.ctypes.data_as(fp),
-                                                 self.std.ctypes.data_as(fp), droprate, int(pr.seed), _lib.UINT64_MAX,
-                                                 pred.data_ptr(), _lib.stream_ptr()), "mapnet_infer_forward_frames")
-        _lib.check(L.mapnet_pose_post(pred.data_ptr(), out.data_ptr(), B, self._m, self._s, _lib.stream_ptr()),
-                   "mapnet_pose_post")
+        self._forward(eng, pre, xs, pred, droprate)
+        self._post(pred, out)
+
+    def _capture(self, fb, tail, eager_tail=True):
+        """(CUDA graph, static uint8 input, static pred6 [B,6]) of frames shaped like fb: the engine's forward, then
+        tail(pred6)'s launches.  Captured after an eager run of the forward (and of tail when eager_tail): tile plans,
+        tensor maps, kernel attributes.  That eager run draws a dropout mask only where calling the predictor would run
+        one: the first time this Localizer or the predictor meets the engine shape (B, H', W'), so frame sizes that
+        resize alike share one draw."""
+        B, H, W = fb.shape[:3]
+        pr = self.predictor
+        Ho, Wo = self._resized(H, W)
+        eng, pre = pr._engine(Ho, Wo), self._plan(H, W)
+        new_shape = (B, Ho, Wo) not in pr._graphs and (B, Ho, Wo) not in self._warm
+        self._warm.add((B, Ho, Wo))
+        xs = torch.empty((B, H, W, 3), dtype=torch.uint8, device=pr.device)
+        pred = torch.empty((B, 6), dtype=torch.float32, device=pr.device)
+        xs.copy_(fb)
+        cur = torch.cuda.current_stream(pr.device)
+        side = torch.cuda.Stream(pr.device)
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):
+            self._forward(eng, pre, xs, pred, pr.droprate if new_shape else 0.0)
+            if eager_tail:
+                tail(pred)
+        cur.wait_stream(side)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            self._forward(eng, pre, xs, pred, pr.droprate)
+            tail(pred)
+        return graph, xs, pred
 
     def _graph(self, fb):
-        """(CUDA graph, static input, static output, static pred6) of frames shaped like fb.  The eager run before the
-        capture draws a dropout mask only where calling the predictor would run one: the first time this Localizer
-        or the predictor meets the engine shape (B, H', W'), so frame sizes that resize alike share one draw."""
+        """(CUDA graph, static input, static output, static pred6) of frames shaped like fb (see _capture)"""
         B, H, W = fb.shape[:3]
         g = self._graphs.get((B, H, W))
         if g is None:
-            pr = self.predictor
-            Ho, Wo = self._resized(H, W)
-            eng, pre = pr._engine(Ho, Wo), self._plan(H, W)
-            new_shape = (B, Ho, Wo) not in pr._graphs and (B, Ho, Wo) not in self._warm
-            self._warm.add((B, Ho, Wo))
-            xs = torch.empty((B, H, W, 3), dtype=torch.uint8, device=pr.device)
-            pred = torch.empty((B, 6), dtype=torch.float32, device=pr.device)
-            out = torch.empty((B, 7), dtype=torch.float64, device=pr.device)
-            xs.copy_(fb)
-            cur = torch.cuda.current_stream(pr.device)
-            side = torch.cuda.Stream(pr.device)
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):        # eager run first: tile plans, tensor maps, kernel attributes
-                self._launch(eng, pre, xs, pred, out, pr.droprate if new_shape else 0.0)
-            cur.wait_stream(side)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                self._launch(eng, pre, xs, pred, out, pr.droprate)
+            out = torch.empty((B, 7), dtype=torch.float64, device=self.predictor.device)
+            graph, xs, pred = self._capture(fb, lambda pred: self._post(pred, out))
             g = self._graphs[(B, H, W)] = (graph, xs, out, pred)
         return g
 
@@ -499,6 +517,170 @@ class Localizer(object):
         for h in self._plans.values():
             _lib.lib().mapnet_preprocess_destroy(h)
         self._plans.clear()
+        self._open = False
+
+
+def _first_pending(seen, lag):
+    """the first frame whose window is not complete after `seen` frames (csrc/track_core.h, first_pending)"""
+    return max(seen - lag, 0)
+
+
+def _int_arg(v, name, lo, hi=None):
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < lo or (hi is not None and v > hi):
+        raise ValueError("%s must be an int in [%d, %s], got %r" % (name, lo, "inf" if hi is None else hi, v))
+    return int(v)
+
+
+class Tracker(object):
+    """MapNet+PGO on a camera stream: scripts/eval.py's pose-graph optimisation (--pose_graph) over frames as they
+    arrive, from a Localizer.
+
+        loc = Localizer(Predictor(model, max_batch=8), mean, std, pose_m, pose_s)
+        trk = Tracker(loc, steps=7, skip=10, vo_fc=True, sax=1, saq=1, srx=20, srq=20)    # pgo_inference_RobotCar.ini
+        first, pose7 = trk(frames, vo_poses)    # uint8 [B,H,W,3] or [H,W,3] as loc takes them; float32 [B,6] or [6]
+                                                # -> frames first .. first+n-1 whose windows completed: float64 [n,7]
+        first, pose7 = trk.flush()              # the last min(lag, seen) frames; starts a new sequence
+        trk.reset(); trk.lag; trk.close()
+
+    The window of frame i is eval.py's MF(steps, skip, real=True, include_vos=True): slot k holds frame
+    clip(i + (k - steps//2) * skip, 0, L-1); its VOs are calc_vos_safe of the VO-library poses of consecutive slots (or
+    calc_vos_safe_fc of every pair i<j when vo_fc); PGO runs on the normalised translations (10 iterations, the
+    reference's literal linear solve, covariances sax, saq, srx, srq) and the middle slot, un-normalised with the
+    Localizer's pose_m / pose_s (kept normalised without them), is frame i's pose.  Frame i's window is complete once
+    frame i + lag has arrived, lag = (steps - 1 - steps//2) * skip (30 frames at RobotCar's steps=7, skip=10; 450 at
+    7Scenes' skip=150): a fixed-lag smoother, faithful to eval.py, not a zero-lag filter.  flush() emits the last frames
+    with their windows clipped at the last frame seen, as eval.py clips them at the sequence's end.  vo_poses: the VO
+    library's per-frame poses in the dataset's normalisation ((t - pose_m) / pose_s, log q), as DeviceDataset(vo_poses=)
+    takes them; any real floating dtype, rounded to float32 as DeviceDataset rounds them.
+
+    With droprate == 0 the poses are bit for bit evaluate_sequence's on a DeviceDataset of the same frames, when the
+    Predictor runs the same chunks.  With droprate > 0 every frame goes through the network once and every window that
+    holds it reuses that draw, where eval.py draws each window's frames anew: the poses are what eval.py's windows of
+    exactly those per-frame draws give.  Engines, snapshot, refresh(), precision and dropout counter are the
+    Localizer's predictor's.  Each chunk of max_batch frames replays one CUDA graph, captured per (B, H, W) after an
+    eager forward as the Localizer captures: mapnet_infer_forward_frames, then three tracking launches (csrc/loader.cu:
+    gather the windows from device rings of recent poses, k_pgo, emit), with the frame counter in device memory; a
+    call never waits for the device.  The host counts frames too, so the frames a call emits follow from the call
+    sizes.  A window whose normal matrix is not positive definite (where scipy's cholesky raises) is reported by
+    flush(), which raises np.linalg.LinAlgError after resetting."""
+
+    def __init__(self, localizer, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0):
+        if not isinstance(localizer, Localizer):
+            raise TypeError("Tracker wraps a geomapnet_b200.inference.Localizer, got %s" % type(localizer).__name__)
+        self.steps = _int_arg(steps, "steps", 2, _lib.MAX_TRACK_STEPS)
+        self.skip = _int_arg(skip, "skip", 1)
+        self.sigmas = [float(v) for v in (sax, saq, srx, srq)]
+        if not all(v > 0 for v in self.sigmas):
+            raise ValueError("sax, saq, srx, srq must be positive, got %s" % (self.sigmas,))
+        self.loc, self.vo_fc = localizer, bool(vo_fc)
+        self.lag = (self.steps - 1 - self.steps // 2) * self.skip
+        self.seen = 0           # frames of the current sequence, mirrored on the device
+        self._graphs = {}       # (B, H, W) -> (CUDAGraph, static uint8 input, vo [B,6], out [B,7], pred6 [B,6])
+        self.h = ctypes.c_void_p()      # mapnet_track_t, created with the first call
+        self._open = True
+
+    def _check_open(self):
+        if not self._open:
+            raise ValueError("Tracker is closed")
+        if not self.loc._open or self.loc.predictor._params is None:
+            raise ValueError("the Tracker's Localizer is closed" if not self.loc._open else
+                             "the Tracker's Predictor is closed")
+
+    def _vo(self, vo_poses, n, single):
+        """vo_poses as a tensor [n,6] of a real floating dtype; raises on anything else"""
+        v = torch.from_numpy(np.ascontiguousarray(vo_poses)) if isinstance(vo_poses, np.ndarray) else vo_poses
+        if not torch.is_tensor(v) or v.dtype not in (torch.float16, torch.bfloat16, torch.float32, torch.float64):
+            raise ValueError("vo_poses must be a float tensor or array, got %s" % getattr(v, "dtype", type(v).__name__))
+        want = (6,) if single else (n, 6)
+        if tuple(v.shape) != want:
+            raise ValueError("vo_poses must be %s for %s, got %s" % (
+                list(want), "one [H,W,3] frame" if single else "%d frames" % n, tuple(v.shape)))
+        return v.reshape(n, 6)
+
+    def _handle(self):
+        if not self.h:
+            pr = self.loc.predictor
+            sig = (ctypes.c_double * 4)(*self.sigmas)
+            _lib.check(_lib.lib().mapnet_track_create(ctypes.byref(self.h), self.steps, self.skip, int(self.vo_fc),
+                                                      pr.max_batch, sig, self.loc._m, self.loc._s),
+                       "mapnet_track_create")
+        return self.h
+
+    def _graph(self, fb):
+        B, H, W = fb.shape[:3]
+        g = self._graphs.get((B, H, W))
+        if g is None:
+            dev, h = self.loc.predictor.device, self._handle()
+            vs = torch.zeros((B, 6), dtype=torch.float32, device=dev)
+            out = torch.empty((B, 7), dtype=torch.float64, device=dev)
+
+            def track(pred):
+                _lib.check(_lib.lib().mapnet_track_step(h, pred.data_ptr(), vs.data_ptr(), B, out.data_ptr(),
+                                                        _lib.stream_ptr()), "mapnet_track_step")
+
+            graph, xs, pred = self.loc._capture(fb, track, eager_tail=False)  # the eager run must not advance the stream
+            g = self._graphs[(B, H, W)] = (graph, xs, vs, out, pred)      # every buffer the graph reads stays alive
+        return g
+
+    @torch.no_grad()
+    def __call__(self, frames, vo_poses):
+        """-> (first, pose7 float64 [n,7] on the device): the frames first .. first+n-1 whose windows this call
+        completed, n = max(seen + B - lag, 0) - max(seen - lag, 0) for the B frames given"""
+        self._check_open()
+        x, single = self.loc._frames(frames)
+        vo = self._vo(vo_poses, x.shape[0], single)
+        pr = self.loc.predictor
+        mb, first = pr.max_batch, _first_pending(self.seen, self.lag)
+        outs = []
+        with torch.cuda.device(pr.device):
+            for lo in range(0, x.shape[0], mb):
+                fb = x[lo:lo + mb]
+                graph, xs, vs, out, _ = self._graph(fb)
+                xs.copy_(fb, non_blocking=True)
+                vs.copy_(vo[lo:lo + mb], non_blocking=True)
+                graph.replay()
+                n = _first_pending(self.seen + fb.shape[0], self.lag) - _first_pending(self.seen, self.lag)
+                self.seen += fb.shape[0]
+                outs.append(out[:n].clone())
+        return first, (outs[0] if len(outs) == 1 else torch.cat(outs, 0))
+
+    @torch.no_grad()
+    def flush(self):
+        """-> (first, pose7 [n,7]): the last n = min(lag, seen) frames, their windows clipped at the last frame seen.
+        Synchronises, starts a new sequence, and raises np.linalg.LinAlgError if a window of the sequence that ended
+        was not positive definite."""
+        self._check_open()
+        pr = self.loc.predictor
+        first = _first_pending(self.seen, self.lag)
+        n, failed = self.seen - first, ctypes.c_int(0)
+        with torch.cuda.device(pr.device):
+            out = torch.empty((max(self.lag, 1), 7), dtype=torch.float64, device=pr.device)
+            if self.h:
+                L = _lib.lib()
+                _lib.check(L.mapnet_track_flush(self.h, out.data_ptr(), _lib.stream_ptr()), "mapnet_track_flush")
+                _lib.check(L.mapnet_track_status(self.h, None, ctypes.byref(failed), _lib.stream_ptr()),
+                           "mapnet_track_status")
+        self.reset()
+        if failed.value:
+            raise np.linalg.LinAlgError("pose graph: the normal matrix of a window of the sequence is not positive "
+                                        "definite")
+        return first, out[:n]
+
+    def reset(self):
+        """Start a new sequence: the next frame is frame 0 (stream-ordered)."""
+        self._check_open()
+        if self.h:
+            with torch.cuda.device(self.loc.predictor.device):
+                _lib.check(_lib.lib().mapnet_track_reset(self.h, _lib.stream_ptr()), "mapnet_track_reset")
+        self.seen = 0
+
+    def close(self):
+        """Free the graphs and the device state (the Localizer and its predictor stay open)."""
+        if self.h:
+            torch.cuda.current_stream(self.loc.predictor.device).synchronize()
+            self._graphs.clear()
+            _lib.lib().mapnet_track_destroy(self.h)
+            self.h = ctypes.c_void_p()
         self._open = False
 
 

@@ -223,6 +223,38 @@ int mapnet_pose_post(const float* pred6, double* out7, int64_t n, const double* 
 int mapnet_pgo_optimize(const double* poses, const double* vos, double* out, int n_windows, int N, int fc_vos,
                         double sax, double saq, double srx, double srq, int n_iters, int flags, int* status_dev, void* stream);
 
+/* ---- streaming pose-graph tracker (csrc/loader.cu; geomapnet_b200.inference.Tracker): scripts/eval.py's MapNet+PGO
+ * loop over frames as they arrive.  The window of frame c is eval.py's MF(steps=T, skip) tuple: slot k holds frame
+ * clip(c + (k - T/2) * skip, 0, last), its VOs are calc_vos_safe of the VO-library poses of consecutive slots (or of
+ * every pair i < j in row-major order when fc_vos), PGO runs on the normalised translations with 10 iterations and the
+ * reference's literal linear solve (mapnet_pgo_optimize, flags 0), and the middle slot T/2 is kept.  Frame c is
+ * final once frame c + lag has arrived, lag = (T - 1 - T/2) * skip: a fixed-lag smoother, not a zero-lag filter.
+ *   mapnet_track_create: 2 <= T <= 16, skip >= 1, up to max_batch frames per step; sigmas4 = (sax, saq, srx, srq)
+ *     (HOST, positive); pose_m3 / pose_s3: HOST pointers (the emitted translations become t * pose_s + pose_m, a
+ *     float64 multiply and an add each rounded, as torch computes it) or both NULL.
+ *   mapnet_track_step: B new frames (1 <= B <= max_batch): pred6 [B][6] float32 (the engine's (t, log q)) and vo6
+ *     [B][6] float32 (the VO-library poses, normalised as the dataset's poses).  It writes out7 [n][7] float64 for the
+ *     n frames whose windows this call completes, first_pending(seen) .. first_pending(seen + B) - 1 with
+ *     first_pending(s) = max(s - lag, 0): n is a function of the call sizes alone, so the caller keeps count on the
+ *     host.  out7 has room for B rows.  Three launches (gather, k_pgo, emit), graph-capturable: the frame counter, the
+ *     rings of the last max_batch + (T-1)*skip poses and VO poses, and a status word live in device memory, and
+ *     nothing is read back.
+ *   mapnet_track_flush: the windows of the last min(lag, seen) frames, clipped at the last frame seen, into out7
+ *     (room for lag rows); the counter stays (mapnet_track_reset starts a new sequence).  Three launches (none when
+ *     lag = 0).
+ *   mapnet_track_reset: stream-ordered: the next step is frame 0 of a new sequence, the status word is cleared.
+ *   mapnet_track_status: synchronises the stream and returns the frames seen and the status (1: a window's normal
+ *     matrix was not positive definite, where scipy's cholesky raises).
+ * Pointers are device memory unless marked HOST.  Argument errors return non-zero before any launch. */
+typedef struct mapnet_track mapnet_track_t;
+int mapnet_track_create(mapnet_track_t** out, int T, int skip, int fc_vos, int max_batch, const double* sigmas4,
+                        const double* pose_m3, const double* pose_s3);
+int mapnet_track_step(mapnet_track_t* h, const float* pred6, const float* vo6, int B, double* out7, void* stream);
+int mapnet_track_flush(mapnet_track_t* h, double* out7, void* stream);
+int mapnet_track_reset(mapnet_track_t* h, void* stream);
+int mapnet_track_status(mapnet_track_t* h, int64_t* frames_seen, int* failed, void* stream);
+int mapnet_track_destroy(mapnet_track_t* h);
+
 /* ---- eval-mode inference engine (csrc/infer.cu): a frozen snapshot of a PoseNet / MapNet trunk for
  * scripts/eval.py-style prediction.  mapnet_infer_load copies the weights (packed fprop operands only), the eval-mode
  * BatchNorm scale / shift (computed from the running statistics exactly as mapnet_forward(training = 0) does) and the
