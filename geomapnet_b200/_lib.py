@@ -18,7 +18,7 @@ N_F8_TENSORS = 33      # e4m3 activation tensors of the fp8 engine at ResNet-34:
 LOSS_MODE = {"posenet": 0, "mapnet": 1, "online": 2, "online_gps": 3}
 
 TRACK_API = ["mapnet_track_create", "mapnet_track_step", "mapnet_track_flush", "mapnet_track_reset", "mapnet_track_status",
-             "mapnet_track_destroy"]
+             "mapnet_track_destroy", "mapnet_track_step_now"]
 MAX_TRACK_STEPS = 16    # mapnet_track_create: windows of at most 16 frames (the PGO kernel's limit)
 
 _lib = None
@@ -147,6 +147,7 @@ def lib():
         getattr(L, name).restype = c_int
     L.mapnet_track_create.argtypes = [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]
     L.mapnet_track_step.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]
+    L.mapnet_track_step_now.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]
     L.mapnet_track_flush.argtypes = [c_void_p, c_void_p, c_void_p]
     L.mapnet_track_reset.argtypes = [c_void_p, c_void_p]
     L.mapnet_track_status.argtypes = [c_void_p, POINTER(c_int64), POINTER(c_int), c_void_p]

@@ -122,18 +122,22 @@ __device__ __forceinline__ const float* track_src(const float* fresh, const floa
 // (w, k) of every completed window w < n_win (rows n .. n + max_win*T - 1), then VO (w, e) (the next max_win*E rows).
 // A slot's frame comes from this call's inputs when it is new, else from the ring: R = max_batch + (T-1)*skip frames
 // hold every older frame a window of this call reaches, none of them in a ring slot this call writes.  The values are
-// k_eval_windows': st_pose7 of the float32 pose, calc_vo_logq_safe of the float32 VO-library poses.
+// k_eval_windows': st_pose7 of the float32 pose, calc_vo_logq_safe of the float32 VO-library poses.  A zero-lag call
+// (now) gathers the n windows that end at its frames instead, from centre now_first(seen); st->n_win is the count of
+// completed windows either way.
 __global__ void __launch_bounds__(128)
-k_track_gather(const float* __restrict__ pred6, const float* __restrict__ vo6, int n, int flush,
+k_track_gather(const float* __restrict__ pred6, const float* __restrict__ vo6, int n, int flush, int now,
                TrackDev* __restrict__ st, double* __restrict__ ring7, float* __restrict__ ring_vo, long long R, int T,
                int skip, int fc, int max_win, double* __restrict__ win7, double* __restrict__ vos7) {
   pdl_prologue();
   const long long seen = st->seen, total = seen + n, lag = trackcore::lag(T, skip);
-  const long long first = trackcore::first_pending(seen, lag);
-  const int n_win = (int)((flush ? total : trackcore::first_pending(total, lag)) - first);
+  const long long pending = trackcore::first_pending(seen, lag);
+  const int n_done = (int)((flush ? total : trackcore::first_pending(total, lag)) - pending);
+  const long long first = now ? trackcore::now_first(seen, lag) : pending;
+  const int n_win = now ? n : n_done;
   const int E = fc ? T * (T - 1) / 2 : T - 1;
   long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r == 0) st->n_win = n_win;
+  if (r == 0) st->n_win = n_done;
   if (r < n) {
     const long long f = seen + r;
     st_pose7(pred6 + 6 * r, ring7 + 7 * (f % R));
@@ -168,23 +172,36 @@ k_track_gather(const float* __restrict__ pred6, const float* __restrict__ vo6, i
   }
 }
 
-// One thread per completed window: its optimised middle slot, translations un-normalised as _window_errors does
-// (un = 0: kept), into out7 row w; thread 0 advances the frame counter by the call's n frames.
-__global__ void __launch_bounds__(128)
-k_track_emit(const double* __restrict__ opt7, TrackDev* __restrict__ st, int n, int T, int un, double m0,
-             double m1, double m2, double s0, double s1, double s2, double* __restrict__ out7) {
-  pdl_prologue();
-  const int w = blockIdx.x * blockDim.x + threadIdx.x;
-  const int n_win = st->n_win;
-  if (w == 0) st->seen += n;
-  if (w >= n_win) return;
-  const double* p = opt7 + 7 * ((long long)w * T + T / 2);
-  double* o = out7 + 7LL * w;
-  const double ms[3] = {m0, m1, m2}, ss[3] = {s0, s1, s2};
+__device__ __forceinline__ void track_emit_pose(const double* p, int un, const double ms[3], const double ss[3],
+                                                double* o) {
 #pragma unroll
   for (int k = 0; k < 3; ++k) o[k] = un ? trackcore::unnormalize(p[k], ss[k], ms[k]) : p[k];
 #pragma unroll
   for (int k = 3; k < 7; ++k) o[k] = p[k];
+}
+
+// One thread per completed window: its optimised middle slot, translations un-normalised as _window_errors does
+// (un = 0: kept), into out7 row w; thread 0 advances the frame counter by the call's n frames.  With now7 (a zero-lag
+// call: n windows, the last n_win of them completed) thread w also writes window w's last slot into now7 row w, and the
+// completed window n - n_win + j feeds out7 row j.
+__global__ void __launch_bounds__(128)
+k_track_emit(const double* __restrict__ opt7, TrackDev* __restrict__ st, int n, int T, int un, double m0,
+             double m1, double m2, double s0, double s1, double s2, double* __restrict__ out7,
+             double* __restrict__ now7) {
+  pdl_prologue();
+  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+  const int n_win = st->n_win;
+  if (w == 0) st->seen += n;
+  const double ms[3] = {m0, m1, m2}, ss[3] = {s0, s1, s2};
+  const double* win = opt7 + 7LL * w * T;
+  if (now7 == nullptr) {
+    if (w < n_win) track_emit_pose(win + 7 * (T / 2), un, ms, ss, out7 + 7LL * w);
+    return;
+  }
+  if (w >= n) return;
+  track_emit_pose(win + 7 * (T - 1), un, ms, ss, now7 + 7LL * w);
+  const int lead = n - n_win;
+  if (w >= lead) track_emit_pose(win + 7 * (T / 2), un, ms, ss, out7 + 7LL * (w - lead));
 }
 
 }  // namespace mapnet
@@ -361,17 +378,19 @@ struct mapnet_track {
   double *win7, *vos7, *opt7;               // [max_win][T][7], [max_win][E][7], [max_win][T][7]
 };
 
-// the three launches of one call: n new frames (a step) or none (flush), out7 [max_win][7]
+// the three launches of one call: n new frames (a step) or none (flush), out7 [max_win][7]; with now7 [n][7] a
+// zero-lag step, which solves all n of its windows, so k_pgo needs no device count
 static int track_launch(mapnet_track_t* h, const float* pred6, const float* vo6, int n, int flush, double* out7,
-                        cudaStream_t st) {
+                        double* now7, cudaStream_t st) {
   const int nw = flush ? (int)(h->lag < h->max_win ? h->lag : h->max_win) : n;   // the grid's windows
   const long long rows = n + (long long)nw * (h->T + h->E);
-  MN_LAUNCH(k_track_gather, cdiv(rows, 128), 128, 0, st, pred6, vo6, n, flush, h->st, h->ring7, h->ring_vo, h->R, h->T,
-            h->skip, h->fc, nw, h->win7, h->vos7);
+  MN_LAUNCH(k_track_gather, cdiv(rows, 128), 128, 0, st, pred6, vo6, n, flush, now7 != nullptr ? 1 : 0, h->st, h->ring7,
+            h->ring_vo, h->R, h->T, h->skip, h->fc, nw, h->win7, h->vos7);
   MN_LAUNCH_CHECK();
-  MN_TRY(launch_pgo(h->win7, h->vos7, h->opt7, nw, h->T, h->fc, h->w4, 10, 0, &h->st->status, &h->st->n_win, st));
+  MN_TRY(launch_pgo(h->win7, h->vos7, h->opt7, nw, h->T, h->fc, h->w4, 10, 0, &h->st->status,
+                    now7 != nullptr ? nullptr : &h->st->n_win, st));
   MN_LAUNCH(k_track_emit, cdiv(nw, 128), 128, 0, st, (const double*)h->opt7, h->st, n, h->T, h->un, h->m[0], h->m[1],
-            h->m[2], h->s[0], h->s[1], h->s[2], out7);
+            h->m[2], h->s[0], h->s[1], h->s[2], out7, now7);
   MN_LAUNCH_CHECK();
   return 0;
 }
@@ -421,14 +440,22 @@ int mapnet_track_step(mapnet_track_t* h, const float* pred6, const float* vo6, i
   MN_CHECK(h != nullptr, "track_step: null handle");
   MN_CHECK(pred6 != nullptr && vo6 != nullptr && out7 != nullptr, "track_step: null argument");
   MN_CHECK(B >= 1 && B <= h->max_batch, "track_step: %d frames outside [1, max_batch=%d]", B, h->max_batch);
-  return track_launch(h, pred6, vo6, B, 0, out7, (cudaStream_t)stream);
+  return track_launch(h, pred6, vo6, B, 0, out7, nullptr, (cudaStream_t)stream);
+}
+
+int mapnet_track_step_now(mapnet_track_t* h, const float* pred6, const float* vo6, int B, double* out7, double* now7,
+                          void* stream) {
+  MN_CHECK(h != nullptr, "track_step_now: null handle");
+  MN_CHECK(pred6 != nullptr && vo6 != nullptr && out7 != nullptr && now7 != nullptr, "track_step_now: null argument");
+  MN_CHECK(B >= 1 && B <= h->max_batch, "track_step_now: %d frames outside [1, max_batch=%d]", B, h->max_batch);
+  return track_launch(h, pred6, vo6, B, 0, out7, now7, (cudaStream_t)stream);
 }
 
 int mapnet_track_flush(mapnet_track_t* h, double* out7, void* stream) {
   MN_CHECK(h != nullptr, "track_flush: null handle");
   MN_CHECK(out7 != nullptr, "track_flush: null argument");
   if (h->lag == 0) return 0;                 // every window was complete when its last frame arrived
-  return track_launch(h, nullptr, nullptr, 0, 1, out7, (cudaStream_t)stream);
+  return track_launch(h, nullptr, nullptr, 0, 1, out7, nullptr, (cudaStream_t)stream);
 }
 
 int mapnet_track_reset(mapnet_track_t* h, void* stream) {

@@ -113,9 +113,12 @@ class ItemLayout(object):
         rows = np.ascontiguousarray(np.concatenate([it[2] for it in items]), dtype=np.int32)
         return fr, jit, rows, len(items)
 
-    def eval_tables(self, unique=True, vo_fc=False):
+    def eval_tables(self, unique=True, vo_fc=False, zero_lag=False):
         """The windows scripts/eval.py evaluates: one per item, in index order, as DataLoader(shuffle=False) draws them
-        (with variable_skip, np.random is consumed as in the reference's loop).  Returns host int32 tables:
+        (with variable_skip, np.random is consumed as in the reference's loop).  zero_lag=True: item i's window is the
+        one that ends at frame i instead, MF.get_indices(i - lag) with lag = (steps - 1 - steps//2) * skip (slots below
+        0 clipped at 0), the causal windows whose last slot inference.Tracker.step emits; it needs fixed skips.
+        Returns host int32 tables:
           windows [L,T]   the frame of every window slot (T = 1 for single frames);
           frames [F]      the frames that go through the network, in that order;
           slots [L,T]     the row of `frames` whose prediction fills each window slot;
@@ -125,7 +128,14 @@ class ItemLayout(object):
         (frames = windows.ravel()), what a network that draws dropout masks at eval needs to see."""
         if self.online or self.jitter is not None:
             raise ValueError("evaluation windows need a single-frame or MF layout without ColorJitter")
-        windows = np.stack([self.item(i)[0] for i in range(len(self))]).astype(np.int32)
+        if zero_lag:
+            if self.steps is None or self.variable_skip:
+                raise ValueError("zero_lag windows need an MF layout (steps) with fixed skips (no variable_skip)")
+            lag = (self.steps - 1 - self.steps // 2) * self.skip
+            windows = np.stack([tuples.mf_indices(i - lag, self.L, self.steps, self.skip)
+                                for i in range(len(self))]).astype(np.int32)
+        else:
+            windows = np.stack([self.item(i)[0] for i in range(len(self))]).astype(np.int32)
         L, T = windows.shape
         if unique:
             frames, inv = np.unique(windows, return_inverse=True)

@@ -539,6 +539,7 @@ class Tracker(object):
         trk = Tracker(loc, steps=7, skip=10, vo_fc=True, sax=1, saq=1, srx=20, srq=20)    # pgo_inference_RobotCar.ini
         first, pose7 = trk(frames, vo_poses)    # uint8 [B,H,W,3] or [H,W,3] as loc takes them; float32 [B,6] or [6]
                                                 # -> frames first .. first+n-1 whose windows completed: float64 [n,7]
+        now7, first, pose7 = trk.step(frames, vo_poses)     # also each given frame's zero-lag pose: float64 [B,7]
         first, pose7 = trk.flush()              # the last min(lag, seen) frames; starts a new sequence
         trk.reset(); trk.lag; trk.close()
 
@@ -548,10 +549,16 @@ class Tracker(object):
     reference's literal linear solve, covariances sax, saq, srx, srq) and the middle slot, un-normalised with the
     Localizer's pose_m / pose_s (kept normalised without them), is frame i's pose.  Frame i's window is complete once
     frame i + lag has arrived, lag = (steps - 1 - steps//2) * skip (30 frames at RobotCar's steps=7, skip=10; 450 at
-    7Scenes' skip=150): a fixed-lag smoother, faithful to eval.py, not a zero-lag filter.  flush() emits the last frames
-    with their windows clipped at the last frame seen, as eval.py clips them at the sequence's end.  vo_poses: the VO
-    library's per-frame poses in the dataset's normalisation ((t - pose_m) / pose_s, log q), as DeviceDataset(vo_poses=)
-    takes them; any real floating dtype, rounded to float32 as DeviceDataset rounds them.
+    7Scenes' skip=150): a fixed-lag smoother, faithful to eval.py.  flush() emits the last frames with their windows
+    clipped at the last frame seen, as eval.py clips them at the sequence's end.  vo_poses: the VO library's per-frame
+    poses in the dataset's normalisation ((t - pose_m) / pose_s, log q), as DeviceDataset(vo_poses=) takes them; any
+    real floating dtype, rounded to float32 as DeviceDataset rounds them.
+
+    step() is the zero-lag output for live use: besides what the call emits, each frame f it brings gets the last slot
+    of the optimised window that ends at f -- frame (f - lag)'s window, slots below 0 clipped at 0 during the first lag
+    frames -- in the call that brings it.  That is the window a call solves anyway once f >= lag, so a step costs what
+    a call costs past the lag, and one window more per frame before it.  evaluate_sequence(..., zero_lag=True) is its
+    offline counterpart on a labelled sequence.  Calls and steps share the sequence, so they may be mixed.
 
     With droprate == 0 the poses are bit for bit evaluate_sequence's on a DeviceDataset of the same frames, when the
     Predictor runs the same chunks.  With droprate > 0 every frame goes through the network once and every window that
@@ -576,6 +583,7 @@ class Tracker(object):
         self.lag = (self.steps - 1 - self.steps // 2) * self.skip
         self.seen = 0           # frames of the current sequence, mirrored on the device
         self._graphs = {}       # (B, H, W) -> (CUDAGraph, static uint8 input, vo [B,6], out [B,7], pred6 [B,6])
+        self._now_graphs = {}   # the same for step(), with now7 [B,7] last
         self.h = ctypes.c_void_p()      # mapnet_track_t, created with the first call
         self._open = True
 
@@ -606,43 +614,69 @@ class Tracker(object):
                        "mapnet_track_create")
         return self.h
 
-    def _graph(self, fb):
+    def _graph(self, fb, now=False):
         B, H, W = fb.shape[:3]
-        g = self._graphs.get((B, H, W))
+        graphs = self._now_graphs if now else self._graphs
+        g = graphs.get((B, H, W))
         if g is None:
             dev, h = self.loc.predictor.device, self._handle()
             vs = torch.zeros((B, 6), dtype=torch.float32, device=dev)
             out = torch.empty((B, 7), dtype=torch.float64, device=dev)
+            now7 = torch.empty((B, 7), dtype=torch.float64, device=dev) if now else None
 
             def track(pred):
-                _lib.check(_lib.lib().mapnet_track_step(h, pred.data_ptr(), vs.data_ptr(), B, out.data_ptr(),
-                                                        _lib.stream_ptr()), "mapnet_track_step")
+                if now:
+                    _lib.check(_lib.lib().mapnet_track_step_now(h, pred.data_ptr(), vs.data_ptr(), B, out.data_ptr(),
+                                                                now7.data_ptr(), _lib.stream_ptr()),
+                               "mapnet_track_step_now")
+                else:
+                    _lib.check(_lib.lib().mapnet_track_step(h, pred.data_ptr(), vs.data_ptr(), B, out.data_ptr(),
+                                                            _lib.stream_ptr()), "mapnet_track_step")
 
             graph, xs, pred = self.loc._capture(fb, track, eager_tail=False)  # the eager run must not advance the stream
-            g = self._graphs[(B, H, W)] = (graph, xs, vs, out, pred)      # every buffer the graph reads stays alive
+            g = (graph, xs, vs, out, pred) + ((now7,) if now else ())     # every buffer the graph reads stays alive
+            graphs[(B, H, W)] = g
         return g
 
-    @torch.no_grad()
-    def __call__(self, frames, vo_poses):
-        """-> (first, pose7 float64 [n,7] on the device): the frames first .. first+n-1 whose windows this call
-        completed, n = max(seen + B - lag, 0) - max(seen - lag, 0) for the B frames given"""
+    def _run(self, frames, vo_poses, now):
+        """(first, pose7 [n,7], now7 [B,7] or None): the chunks of max_batch frames, one graph replay each"""
         self._check_open()
         x, single = self.loc._frames(frames)
         vo = self._vo(vo_poses, x.shape[0], single)
         pr = self.loc.predictor
         mb, first = pr.max_batch, _first_pending(self.seen, self.lag)
-        outs = []
+        outs, nows = [], []
         with torch.cuda.device(pr.device):
             for lo in range(0, x.shape[0], mb):
                 fb = x[lo:lo + mb]
-                graph, xs, vs, out, _ = self._graph(fb)
+                g = self._graph(fb, now)
+                graph, xs, vs, out = g[:4]
                 xs.copy_(fb, non_blocking=True)
                 vs.copy_(vo[lo:lo + mb], non_blocking=True)
                 graph.replay()
                 n = _first_pending(self.seen + fb.shape[0], self.lag) - _first_pending(self.seen, self.lag)
                 self.seen += fb.shape[0]
                 outs.append(out[:n].clone())
-        return first, (outs[0] if len(outs) == 1 else torch.cat(outs, 0))
+                if now:
+                    nows.append(g[5].clone())
+        cat = lambda ts: ts[0] if len(ts) == 1 else torch.cat(ts, 0)
+        return first, cat(outs), (cat(nows) if now else None)
+
+    @torch.no_grad()
+    def __call__(self, frames, vo_poses):
+        """-> (first, pose7 float64 [n,7] on the device): the frames first .. first+n-1 whose windows this call
+        completed, n = max(seen + B - lag, 0) - max(seen - lag, 0) for the B frames given"""
+        first, pose7, _ = self._run(frames, vo_poses, False)
+        return first, pose7
+
+    @torch.no_grad()
+    def step(self, frames, vo_poses):
+        """-> (now7 float64 [B,7] on the device, first, pose7 [n,7]): row b of now7 is the zero-lag pose of the b-th
+        frame given, f = seen + b: slot steps-1 of the optimised window that ends at f (frame (f - lag)'s window,
+        clipped at 0), un-normalised as pose7; (first, pose7) is what self(frames, vo_poses) returns.  Takes what
+        __call__ takes; each chunk replays a graph of its own, the same three tracking launches."""
+        first, pose7, now7 = self._run(frames, vo_poses, True)
+        return now7, first, pose7
 
     @torch.no_grad()
     def flush(self):
@@ -679,6 +713,7 @@ class Tracker(object):
         if self.h:
             torch.cuda.current_stream(self.loc.predictor.device).synchronize()
             self._graphs.clear()
+            self._now_graphs.clear()
             _lib.lib().mapnet_track_destroy(self.h)
             self.h = ctypes.c_void_p()
         self._open = False
@@ -709,15 +744,16 @@ def evaluate_tuples(model, x, targ6, vos7=None, pose_m=None, pose_s=None, batch=
     return _window_errors(pred, targ, pose_m, pose_s)
 
 
-def _window_errors(pred, targ, pose_m, pose_s):
+def _window_errors(pred, targ, pose_m, pose_s, last=False):
     """eval.py:180-199 on windows pred7, targ7 [L,T,7]: translations un-normalised with pose_m / pose_s (when given),
-    the middle pose of every window and its errors.  Returns dict(pred7 [L,7], targ7 [L,7], t_err, q_err)."""
+    the middle pose of every window (the last one when `last`: zero-lag windows) and its errors.  Returns
+    dict(pred7 [L,7], targ7 [L,7], t_err, q_err)."""
     if pose_m is not None:
         m = torch.as_tensor(np.asarray(pose_m, dtype=np.float64), device=pred.device)
         s = torch.as_tensor(np.asarray(pose_s, dtype=np.float64), device=pred.device)
         pred = torch.cat((pred[..., :3] * s + m, pred[..., 3:]), -1)
         targ = torch.cat((targ[..., :3] * s + m, targ[..., 3:]), -1)
-    mid = pred.shape[1] // 2                            # eval.py:183-185 (py2 integer division)
+    mid = pred.shape[1] - 1 if last else pred.shape[1] // 2     # eval.py:183-185 (py2 integer division)
     p_mid, t_mid = pred[:, mid], targ[:, mid]
     t_err, q_err = pose_errors(p_mid, t_mid)
     return dict(pred7=p_mid, targ7=t_mid, t_err=t_err, q_err=q_err)
@@ -844,11 +880,15 @@ def _predict_batches(pr, net, ds, batches, droprate, dev):
 
 
 @torch.no_grad()
-def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, **sigmas):
+def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, zero_lag=False, **sigmas):
     """The whole loop of scripts/eval.py:117-199 over a device-resident sequence: the windows of MF(steps, skip,
     variable_skip, no_duplicates=False) -- or single frames when dataset.steps is None -- one per frame index, in index
     order.  Returns what evaluate_tuples returns (pred7 [L,7], targ7 [L,7], t_err, q_err: the middle frame of each
     window) and n_frames, the number of frames that went through the network.
+
+    zero_lag=True evaluates the pose a live tracker has for each frame when it arrives (Tracker.step): item i's window
+    is the one that ends at frame i, MF.get_indices(i - lag) with lag = (steps - 1 - steps//2) * skip, and its last
+    slot is kept.  It needs dataset.steps and fixed skips (no variable_skip), else ValueError before any launch.
 
     model: a PoseNet / MapNet or a Predictor (any precision).  A live model whose precision a Predictor supports is
     run by a temporary Predictor; any other runs its own eval forward.  dataset: a DeviceDataset without ColorJitter;
@@ -871,6 +911,9 @@ def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, **s
         raise ValueError("evaluate_sequence: MFOnline datasets are not evaluation sequences")
     if not ds.h:
         raise RuntimeError("evaluate_sequence: the dataset is closed")
+    if zero_lag and (ds.steps is None or ds.variable_skip):
+        raise ValueError("evaluate_sequence: zero_lag needs a windowed dataset (steps) with fixed skips; got %s" %
+                         ("single frames" if ds.steps is None else "variable_skip"))
     pr, net, dev = _model_for(model, ds, "evaluate_sequence")
     vo = ds.vo_poses is not None
     T = 1 if ds.steps is None else ds.steps
@@ -885,7 +928,7 @@ def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, **s
         if B < T:
             raise ValueError("droprate > 0 runs one window of %d frames per forward; max_batch allows %d" % (T, B))
         B = T
-    tab = ds.eval_tables(unique=droprate == 0, vo_fc=vo_fc)
+    tab = ds.eval_tables(unique=droprate == 0, vo_fc=vo_fc, zero_lag=zero_lag)
     frames, L = tab["frames"], tab["windows"].shape[0]
     F = frames.shape[0]
     with _eval_pass(model, pr, net, dev, min(64, cap)) as pr:
@@ -901,7 +944,8 @@ def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, **s
             tab["windows"].ctypes.data, tab["slots"].ctypes.data, L * T,
             tab["vo_rows"].ctypes.data if vo else None, L * E if vo else 0, pred7.data_ptr(), targ7.data_ptr(),
             vos7.data_ptr() if vo else None, _lib.stream_ptr()), "mapnet_eval_windows")
-        out = _window_errors(pgo(pred7, vos7, fc_vos=vo_fc, **sigmas) if vo else pred7, targ7, pose_m, pose_s)
+        out = _window_errors(pgo(pred7, vos7, fc_vos=vo_fc, **sigmas) if vo else pred7, targ7, pose_m, pose_s,
+                             last=zero_lag)
     return dict(out, n_frames=F)
 
 

@@ -228,7 +228,8 @@ int mapnet_pgo_optimize(const double* poses, const double* vos, double* out, int
  * clip(c + (k - T/2) * skip, 0, last), its VOs are calc_vos_safe of the VO-library poses of consecutive slots (or of
  * every pair i < j in row-major order when fc_vos), PGO runs on the normalised translations with 10 iterations and the
  * reference's literal linear solve (mapnet_pgo_optimize, flags 0), and the middle slot T/2 is kept.  Frame c is
- * final once frame c + lag has arrived, lag = (T - 1 - T/2) * skip: a fixed-lag smoother, not a zero-lag filter.
+ * final once frame c + lag has arrived, lag = (T - 1 - T/2) * skip: a fixed-lag smoother.  Its last slot T-1 is the
+ * zero-lag estimate of frame c + lag, which mapnet_track_step_now emits as well.
  *   mapnet_track_create: 2 <= T <= 16, skip >= 1, up to max_batch frames per step; sigmas4 = (sax, saq, srx, srq)
  *     (HOST, positive); pose_m3 / pose_s3: HOST pointers (the emitted translations become t * pose_s + pose_m, a
  *     float64 multiply and an add each rounded, as torch computes it) or both NULL.
@@ -239,6 +240,11 @@ int mapnet_pgo_optimize(const double* poses, const double* vos, double* out, int
  *     host.  out7 has room for B rows.  Three launches (gather, k_pgo, emit), graph-capturable: the frame counter, the
  *     rings of the last max_batch + (T-1)*skip poses and VO poses, and a status word live in device memory, and
  *     nothing is read back.
+ *   mapnet_track_step_now: mapnet_track_step's out7 for the same frames, and the zero-lag poses: now7 [B][7] float64
+ *     row b is slot T-1 of the optimised window that ends at new frame f = seen + b, i.e. the window of frame f - lag
+ *     (slots clipped at 0 while f < lag), translated as out7.  Every call solves B windows; those of frames f >= lag
+ *     are the ones mapnet_track_step completes.  Same three launches, graph-capturable, nothing read back; the status
+ *     word also records these windows.  The two steps share the counter and rings, so a sequence may mix them.
  *   mapnet_track_flush: the windows of the last min(lag, seen) frames, clipped at the last frame seen, into out7
  *     (room for lag rows); the counter stays (mapnet_track_reset starts a new sequence).  Three launches (none when
  *     lag = 0).
@@ -250,6 +256,8 @@ typedef struct mapnet_track mapnet_track_t;
 int mapnet_track_create(mapnet_track_t** out, int T, int skip, int fc_vos, int max_batch, const double* sigmas4,
                         const double* pose_m3, const double* pose_s3);
 int mapnet_track_step(mapnet_track_t* h, const float* pred6, const float* vo6, int B, double* out7, void* stream);
+int mapnet_track_step_now(mapnet_track_t* h, const float* pred6, const float* vo6, int B, double* out7, double* now7,
+                          void* stream);
 int mapnet_track_flush(mapnet_track_t* h, double* out7, void* stream);
 int mapnet_track_reset(mapnet_track_t* h, void* stream);
 int mapnet_track_status(mapnet_track_t* h, int64_t* frames_seen, int* failed, void* stream);
