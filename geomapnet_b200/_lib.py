@@ -143,7 +143,11 @@ def lib():
     L.mapnet_sample_post.argtypes = [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                      c_void_p, c_void_p]
     L.mapnet_test_small_gemm_plan.argtypes = [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int)]
-    for name in ("mapnet_infer_sample", "mapnet_infer_sample_frames", "mapnet_sample_post", "mapnet_test_small_gemm_plan"):
+    L.mapnet_test_stem_ex.argtypes = [c_int] * 4 + [c_void_p] * 5 + [c_float, c_void_p, c_void_p]
+    L.mapnet_test_head.argtypes = [c_int, c_int, c_void_p, c_void_p, c_float, c_uint64, c_uint64, c_uint64] + \
+        [c_void_p] * 6 + [c_int] + [c_void_p] * 5
+    for name in ("mapnet_infer_sample", "mapnet_infer_sample_frames", "mapnet_sample_post", "mapnet_test_small_gemm_plan",
+                 "mapnet_test_stem_ex", "mapnet_test_head"):
         getattr(L, name).restype = c_int
     L.mapnet_track_create.argtypes = [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]
     L.mapnet_track_step.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]
@@ -192,7 +196,8 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_test_bn_forward", "mapnet_test_bn_backward", "mapnet_test_stem_pool", "mapnet_test_gap",
             "mapnet_trunk_set_trainable", "mapnet_test_conv_ex", "mapnet_eval_windows",
             "mapnet_batch_losses", "mapnet_infer_forward_frames", "mapnet_test_stem_operand", "mapnet_infer_sample",
-            "mapnet_infer_sample_frames", "mapnet_sample_post", "mapnet_test_small_gemm_plan"] + TRACK_API
+            "mapnet_infer_sample_frames", "mapnet_sample_post", "mapnet_test_small_gemm_plan", "mapnet_test_stem_ex",
+            "mapnet_test_head"] + TRACK_API
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 MAX_SAMPLE_DRAWS = 1024      # mapnet_infer_sample: S in [2, MAX_SAMPLE_DRAWS] dropout draws per frame
 

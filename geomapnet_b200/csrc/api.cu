@@ -254,15 +254,16 @@ int mapnet_test_conv_ex(int precision, int kind, int B, int Hi, int Wi, int Ci, 
 // JSON description of the plan the tensor-core engines would use for this conv (no device needed).  flags: bit 0 folds
 // the downsample shortcut into a stride-2 dgrad; bit 1 describes the strict-mode (split-operand) plan instead of bf16's;
 // bit 2 describes the fp8 fprop plan (tc_plan_create_f8).  k == 7 (fprop): the stem as the engines run it, the 4x1 conv
-// on the space-to-depth image of an Hi x Wi frame (mapnet_test_conv_affine's k == 7)
+// on the space-to-depth image of an Hi x Wi frame (mapnet_test_conv_affine's k == 7); kind 2 with k == 7: the stem's
+// wgrad over that image (mapnet_test_stem_ex)
 int mapnet_test_plan_describe(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, int flags,
                               char* buf, int cap) {
   MN_CHECK(!(flags & 4) || (kind == 0 && !(flags & 3)),
            "test_plan_describe: flag 4 (fp8) describes an fprop plan, without flags 1 or 2");
   ConvGeom g;
   if (k == 7) {
-    MN_CHECK(kind == 0 && Ci == 3 && Co == 64 && stride == 2 && !(flags & 5), "test_plan_describe: the stem is a 7x7/s2 "
-             "fprop, 3 -> 64");
+    MN_CHECK((kind == 0 || kind == 2) && Ci == 3 && Co == 64 && stride == 2 && !(flags & 5), "test_plan_describe: the "
+             "stem is a 7x7/s2 conv, 3 -> 64, with an fprop and a wgrad");
     WeightDesc wd;
     stem_s2d_geometry(Hi, Wi, 64, &g, &wd, (flags & 2) ? 4 : 2);
   } else {
@@ -349,43 +350,99 @@ int mapnet_test_conv_epilogue(int kind, int B, int Hi, int Wi, int Ci, int Co, i
   return r;
 }
 
-// the tensor-core stem alone: space-to-depth image -> packed weights -> fprop [-> wgrad -> .grad layout]
+// the tensor-core stem alone (bf16 mode, no statistics)
 int mapnet_test_stem(int B, int H, int W, const float* x_nchw, const float* w_oihw, void* y_out, const void* dy,
                      float* dw_oihw, void* stream) {
+  return mapnet_test_stem_ex(PREC_BF16_TC, B, H, W, x_nchw, w_oihw, y_out, dw_oihw ? dy : nullptr, dy ? dw_oihw : nullptr,
+                             0.f, nullptr, stream);
+}
+
+// The training step's stem (Net::forward_t / backward_t, tensor-core modes): space-to-depth image of the operand type,
+// the mode's weight pack, fprop with the BatchNorm-statistics epilogue (host_sums != null), and with dy the wgrad into
+// the [64][4][64] patch-matrix accumulator (zeroed first, as backward_t zeroes dw_krsc) re-laid out by k_unpack_wgrads.
+// Strict mode: y_out and dy are fp32 (dy cut into fp16 planes here, as the step's element-wise kernels write it) and
+// out_scale (0: none) is the wgrad's gradient out-scale.
+int mapnet_test_stem_ex(int precision, int B, int H, int W, const float* x_nchw, const float* w_oihw, void* y_out,
+                        const void* dy, float* dw_oihw, float out_scale, double* host_sums, void* stream) {
+  MN_CHECK(precision == PREC_BF16_TC || precision == PREC_TC_SPLIT, "test_stem_ex: precision %d is not a tensor-core "
+           "training precision (bf16 = %d or tc_split = %d)", precision, PREC_BF16_TC, PREC_TC_SPLIT);
+  MN_CHECK(B >= 1 && H >= 32 && W >= 32, "test_stem_ex: bad shape (B %d, %dx%d)", B, H, W);
+  MN_CHECK(x_nchw && w_oihw && y_out, "test_stem_ex: null argument");
+  MN_CHECK((dy == nullptr) == (dw_oihw == nullptr), "test_stem_ex: dy and dw_oihw go together");
+  MN_CHECK(out_scale == 0.f || (precision == PREC_TC_SPLIT && dy != nullptr && isfinite(out_scale) && out_scale > 0.f),
+           "test_stem_ex: out_scale %g: a positive gradient scale of the strict-mode wgrad, or 0", out_scale);
   MN_TRY(require_device());
-  MN_CHECK(B >= 1 && H >= 32 && W >= 32 && x_nchw && w_oihw && y_out, "test_stem: bad argument");
-  MN_CHECK(tc_overlapped_view_supported(), "test_stem: the driver rejects overlapped tensor maps");
+  MN_CHECK(tc_overlapped_view_supported(), "test_stem_ex: the driver rejects overlapped tensor maps");
   cudaStream_t st = (cudaStream_t)stream;
+  const bool sp = precision == PREC_TC_SPLIT;
+  const size_t ez = sp ? 4 : 2;                     // bytes per stored element (split: an fp16 hi / lo pair)
   ConvGeom g; WeightDesc wd; memset(&wd, 0, sizeof(wd));
-  stem_s2d_geometry(H, W, 64, &g, &wd);
+  stem_s2d_geometry(H, W, 64, &g, &wd, (int)ez);
   g.B = B; wd.p_off = 0; wd.k_off = 0;
+  if (sp) g.split = 1;
   const int Hs = g.Hi, Wsp = stem_s2d_wsp(g.Wo);
-  bf16 *S = nullptr, *wk = nullptr; float* dwk = nullptr; WeightDesc* d_wd = nullptr;
+  const long long n_y = (long long)B * g.Ho * g.Wo * 64;
+  const size_t acc_doubles = (size_t)kBnAccReplicas * kBnAccStride;
+  void *S = nullptr, *wk = nullptr, *dys = nullptr; float *dwk = nullptr, *f32 = nullptr, *d_scale = nullptr;
+  double* acc = nullptr; WeightDesc* d_wd = nullptr;
   TcConvPlan *pf = nullptr, *pw = nullptr;
-  int r = 0;
+  std::vector<double> h;
   auto body = [&]() -> int {
-    MN_CUDA(cudaMalloc(&S, (size_t)B * Hs * Wsp * 16 * sizeof(bf16)));
-    MN_CUDA(cudaMalloc(&wk, (size_t)64 * 256 * sizeof(bf16)));
+    MN_CUDA(cudaMalloc(&S, (size_t)B * Hs * Wsp * 16 * ez));
+    MN_CUDA(cudaMalloc(&wk, (size_t)64 * 256 * (sp ? 8 : 2)));
     MN_CUDA(cudaMalloc(&dwk, (size_t)64 * 256 * sizeof(float)));
     MN_CUDA(cudaMalloc(&d_wd, sizeof(WeightDesc)));
     MN_CUDA(cudaMemcpyAsync(d_wd, &wd, sizeof(wd), cudaMemcpyHostToDevice, st));
     MN_CUDA(cudaMemsetAsync(dwk, 0, (size_t)64 * 256 * sizeof(float), st));
-    MN_TRY(launch_stem_s2d<bf16>(x_nchw, S, B, H, W, Hs, Wsp, st));
-    MN_TRY(launch_pack_weights<bf16>(d_wd, 1, w_oihw, wk, nullptr, 64 * 256, 0, st));
-    MN_TRY(tc_plan_create(&pf, g, 0, wk));
-    MN_TRY(tc_conv_run(pf, S, nullptr, nullptr, y_out, st));
-    if (dy != nullptr && dw_oihw != nullptr) {
+    if (sp) {
+      MN_CUDA(cudaMalloc(&f32, (size_t)64 * 256 * sizeof(float)));
+      MN_TRY(launch_stem_s2d<hsplit>(x_nchw, (hsplit*)S, B, H, W, Hs, Wsp, st));
+      MN_TRY(launch_pack_weights_split(d_wd, 1, w_oihw, f32, nullptr, wk, nullptr, 64 * 256, st));
+    } else {
+      MN_TRY(launch_stem_s2d<bf16>(x_nchw, (bf16*)S, B, H, W, Hs, Wsp, st));
+      MN_TRY(launch_pack_weights<bf16>(d_wd, 1, w_oihw, (bf16*)wk, nullptr, 64 * 256, 0, st));
+    }
+    if (host_sums != nullptr) {
+      MN_CUDA(cudaMalloc((void**)&acc, acc_doubles * sizeof(double)));
+      MN_CUDA(cudaMemsetAsync(acc, 0, acc_doubles * sizeof(double), st));
+    }
+    MN_TRY(tc_plan_create(&pf, g, 0, (const bf16*)wk));
+    MN_TRY(tc_conv_run(pf, (const bf16*)S, nullptr, nullptr, y_out, st, acc));
+    if (dy != nullptr) {
+      const void* g_in = dy;
+      if (sp) {
+        MN_CUDA(cudaMalloc(&dys, (size_t)n_y * 4));
+        MN_TRY(launch_split_tensor((const float*)dy, dys, n_y, st));
+        g_in = dys;
+      }
       MN_TRY(tc_plan_create(&pw, g, 2, nullptr));
-      MN_TRY(tc_conv_run(pw, S, (const bf16*)dy, nullptr, dwk, st));
+      if (out_scale != 0.f) {
+        MN_CUDA(cudaMalloc((void**)&d_scale, sizeof(float)));
+        MN_CUDA(cudaMemcpyAsync(d_scale, &out_scale, sizeof(float), cudaMemcpyHostToDevice, st));
+        tc_plan_set_out_scale(pw, d_scale);
+      }
+      MN_TRY(tc_conv_run(pw, (const bf16*)S, (const bf16*)g_in, nullptr, dwk, st));
       MN_TRY(launch_unpack_wgrads(d_wd, 1, dwk, dw_oihw, 64 * 256, st));
+    }
+    if (acc != nullptr) {
+      h.resize(acc_doubles);
+      MN_CUDA(cudaMemcpyAsync(h.data(), acc, acc_doubles * sizeof(double), cudaMemcpyDeviceToHost, st));
     }
     MN_CUDA(cudaStreamSynchronize(st));
     return 0;
   };
-  r = body();
+  const int r = body();
+  if (r == 0 && host_sums != nullptr)
+    for (int j = 0; j < 2; ++j)
+      for (int c = 0; c < 64; ++c) {
+        double s = 0.0;
+        for (int rep = 0; rep < kBnAccReplicas; ++rep) s += h[(size_t)rep * kBnAccStride + (size_t)j * 64 + c];
+        host_sums[(size_t)j * 64 + c] = s;
+      }
   if (pf) tc_plan_destroy(pf);
   if (pw) tc_plan_destroy(pw);
-  cudaFree(S); cudaFree(wk); cudaFree(dwk); cudaFree(d_wd);
+  cudaFree(S); cudaFree(wk); cudaFree(dwk); cudaFree(dys); cudaFree(f32); cudaFree(d_scale); cudaFree(acc);
+  cudaFree(d_wd);
   return r;
 }
 
@@ -812,6 +869,45 @@ int mapnet_test_small_gemm_plan(int epi, int M, int N, int K, int* splits, int* 
            "test_small_gemm_plan: bad argument");
   *splits = small_gemm_split_plan(epi, M, N, K, kchunk);
   return 0;
+}
+
+// The pose head as the training step runs it (head_forward, then with dpred head_backward with every parameter
+// trained) on caller-owned fp32 device tensors.  params / grads: fc_w [F][512], fc_b [F], xyz_w [3][F], xyz_b [3],
+// wpqr_w [3][F], wpqr_b [3], packed in that order.
+int mapnet_test_head(int B, int F, const float* feat, const float* params, float droprate, uint64_t seed, uint64_t step,
+                     uint64_t stride, uint64_t* ctr, float* mask, float* fcpre, float* hdrop, float* pred,
+                     const float* dpred, int filter_nans, float* dh, float* dfeat, float* grads, float* scale2,
+                     void* stream) {
+  MN_CHECK(B >= 1 && F >= 8 && F % 4 == 0, "test_head: need B >= 1 and F a multiple of 4, >= 8 (got B %d, F %d)", B, F);
+  MN_CHECK(feat && params && fcpre && hdrop && pred, "test_head: null argument");
+  MN_CHECK(droprate >= 0.f && droprate < 1.f, "test_head: droprate %g outside [0, 1)", (double)droprate);
+  MN_CHECK(droprate == 0.f || (mask != nullptr && stride >= (uint64_t)B * F && (step != ~0ULL || ctr != nullptr)),
+           "test_head: dropout needs mask, stride >= B * F (got %llu) and, at step ~0, the device counter ctr",
+           (unsigned long long)stride);
+  MN_CHECK(dpred == nullptr || (dh && dfeat && grads), "test_head: the backward needs dh, dfeat and grads");
+  MN_CHECK(scale2 == nullptr || dpred != nullptr, "test_head: the gradient scale is a backward output");
+  MN_TRY(require_device());
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long F512 = (long long)F * 512;
+  const HeadParams hp{params, params + F512, params + F512 + F, params + F512 + 4 * F, params + F512 + 4 * F + 3,
+                      params + F512 + 7 * F + 3};
+  float* dpf = nullptr;
+  auto body = [&]() -> int {
+    MN_TRY(head_forward(hp, feat, B, F, droprate, seed, step, (unsigned long long*)ctr, stride, mask, fcpre, hdrop, pred,
+                        st));
+    if (dpred != nullptr) {
+      const HeadGrads hg{grads, grads + F512, grads + F512 + F, grads + F512 + 4 * F, grads + F512 + 4 * F + 3,
+                         grads + F512 + 7 * F + 3};
+      MN_CUDA(cudaMalloc((void**)&dpf, (size_t)B * 12 * sizeof(float)));
+      MN_TRY(head_backward(hp, hg, dpred, filter_nans, feat, droprate > 0.f ? mask : nullptr, fcpre, hdrop, B, F, dpf,
+                           dpf + (size_t)B * 6, scale2, dh, dfeat, st));
+    }
+    MN_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  };
+  const int r = body();
+  cudaFree(dpf);
+  return r;
 }
 
 // The stem operand of the inference engine from one of its two sources: uint8 frames through pre (the fused vertical

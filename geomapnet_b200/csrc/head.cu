@@ -99,7 +99,7 @@ __global__ void k_grad_scale(const float* __restrict__ g, int n, float* __restri
   if (threadIdx.x == 0) {
     for (int w = 1; w < (int)(blockDim.x >> 5); ++w) m = (red[w] > m || red[w] != red[w]) ? red[w] : m;
     float S = 1.f;
-    if (m > 0.f && m < 3.0e38f) {            // finite and non-zero (NaN fails both comparisons)
+    if (m > 0.f && isfinite(m)) {            // finite and non-zero (NaN fails the comparison)
       int e;
       frexpf(m, &e);                          // m = f * 2^e, f in [0.5, 1)  =>  m <= 2^e
       int k = 8 - e;
@@ -504,6 +504,42 @@ int launch_head_dh(const float* dpred, const float* wx, const float* wq, const f
   long long grid = ((long long)B * F + 255) / 256; if (grid > 592) grid = 592;
   MN_LAUNCH(k_head_dh, (int)grid, 256, 0, st, dpred, wx, wq, mask, fcpre, dh, B, F);
   MN_LAUNCH_CHECK();
+  return 0;
+}
+
+// ---- the head's forward and backward launch sequences (models/posenet.py:67-73, NaN filter :28-34) ----
+int head_forward(const HeadParams& hp, const float* feat, int B, int F, float droprate, unsigned long long seed,
+                 unsigned long long step, unsigned long long* ctr, unsigned long long stride, float* mask, float* fcpre,
+                 float* hdrop, float* pred, cudaStream_t st) {
+  const float* mk = nullptr;
+  if (droprate > 0.f) {
+    const bool dev_ctr = (step == ~0ULL);
+    MN_TRY(launch_dropout_mask(mask, (long long)B * F, droprate, seed, dev_ctr ? 0ULL : step * stride,
+                               dev_ctr ? ctr : nullptr, stride, st));
+    mk = mask;
+  }
+  // hdrop = relu(feat @ Wfc^T + b) * mask ; fcpre kept for the ReLU gate
+  MN_TRY(launch_small_gemm(1, feat, 512, 1, hp.fc_w, 512, 1, hdrop, F, B, F, 512, hp.fc_b, fcpre, mk, st));
+  MN_TRY(launch_small_gemm(0, hdrop, F, 1, hp.xyz_w, F, 1, pred, 6, B, 3, F, hp.xyz_b, nullptr, nullptr, st));
+  MN_TRY(launch_small_gemm(0, hdrop, F, 1, hp.wpqr_w, F, 1, pred + 3, 6, B, 3, F, hp.wpqr_b, nullptr, nullptr, st));
+  return 0;
+}
+
+int head_backward(const HeadParams& hp, const HeadGrads& hg, const float* dpred, int filter_nans, const float* feat,
+                  const float* mask, const float* fcpre, const float* hdrop, int B, int F, float* dpredw, float* dpredh,
+                  float* gscale, float* dh, float* dfeat, cudaStream_t st) {
+  MN_TRY(launch_dpred_filter(dpred, dpredw, dpredh, B, filter_nans, st));
+  if (gscale != nullptr) MN_TRY(launch_grad_scale(dpredh, B * 6, gscale, st));
+  // dW_xyz[c][j] = sum_b dpred[b][c] * hdrop[b][j]
+  if (hg.xyz_w) MN_TRY(launch_small_gemm(0, dpredw, 1, 6, hdrop, 1, F, hg.xyz_w, F, 3, F, B, nullptr, nullptr, nullptr, st));
+  if (hg.wpqr_w) MN_TRY(launch_small_gemm(0, dpredw + 3, 1, 6, hdrop, 1, F, hg.wpqr_w, F, 3, F, B, nullptr, nullptr, nullptr, st));
+  if (hg.xyz_b) MN_TRY(launch_colsum(dpredw, 6, B, 3, hg.xyz_b, st));
+  if (hg.wpqr_b) MN_TRY(launch_colsum(dpredw + 3, 6, B, 3, hg.wpqr_b, st));
+  if (hg.fc_w || hg.fc_b || dfeat) MN_TRY(launch_head_dh(dpredh, hp.xyz_w, hp.wpqr_w, mask, fcpre, dh, B, F, st));
+  // dW_fc[o][i] = sum_b dh[b][o] * feat[b][i];  db_fc = colsum(dh);  dfeat = dh @ W_fc
+  if (hg.fc_w) MN_TRY(launch_small_gemm(0, dh, 1, F, feat, 1, 512, hg.fc_w, 512, F, 512, B, nullptr, nullptr, nullptr, st));
+  if (hg.fc_b) MN_TRY(launch_colsum(dh, F, B, F, hg.fc_b, st));
+  if (dfeat) MN_TRY(launch_small_gemm(0, dh, F, 1, hp.fc_w, 1, 512, dfeat, 512, B, 512, F, nullptr, nullptr, nullptr, st));
   return 0;
 }
 }  // namespace mapnet

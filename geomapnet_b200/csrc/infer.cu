@@ -295,18 +295,8 @@ int InferNet::run_head(int B, float droprate, unsigned long long seed, unsigned 
                        cudaStream_t st) {
   const Net& n = spec;
   const float* hp = head - n.fc_w;      // indexed with the flat-buffer offsets
-  const float* mk = nullptr;
-  if (droprate > 0.f) {
-    const unsigned long long stride = (unsigned long long)max_B * feat_dim;
-    const bool dev_ctr = (step == ~0ULL);
-    MN_TRY(launch_dropout_mask(mask, (long long)B * feat_dim, droprate, seed, dev_ctr ? 0ULL : step * stride,
-                               dev_ctr ? drop_ctr : nullptr, stride, st));
-    mk = mask;
-  }
-  MN_TRY(launch_small_gemm(1, feat, 512, 1, hp + n.fc_w, 512, 1, hdrop, feat_dim, B, feat_dim, 512, hp + n.fc_b, fcpre, mk, st));
-  MN_TRY(launch_small_gemm(0, hdrop, feat_dim, 1, hp + n.xyz_w, feat_dim, 1, pred, 6, B, 3, feat_dim, hp + n.xyz_b, nullptr, nullptr, st));
-  MN_TRY(launch_small_gemm(0, hdrop, feat_dim, 1, hp + n.wpqr_w, feat_dim, 1, pred + 3, 6, B, 3, feat_dim, hp + n.wpqr_b, nullptr, nullptr, st));
-  return 0;
+  return head_forward(n.head_params(hp), feat, B, feat_dim, droprate, seed, step, drop_ctr,
+                      (unsigned long long)max_B * feat_dim, mask, fcpre, hdrop, pred, st);
 }
 
 // S Monte-Carlo dropout draws of the head on feat: the fc product once, without a mask (fcpre is the same for every

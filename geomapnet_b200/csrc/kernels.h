@@ -197,6 +197,22 @@ int launch_dropout_mask(float* mask, long long n, float p, unsigned long long se
                         unsigned long long* ctr_dev, unsigned long long ctr_stride, cudaStream_t st);
 int launch_head_dh(const float* dpred, const float* wx, const float* wq, const float* mask, const float* fcpre,
                    float* dh, int B, int F, cudaStream_t st);
+// The head's launch sequences, shared by the training step (Net::forward_t / backward_t), the inference engine's
+// run_head and mapnet_test_head.  Parameters fc [F][512] + [F], fc_xyz / fc_wpqr [3][F] + [3]; gradients in the same
+// shapes, a null gradient pointer is a frozen parameter (nothing computed for it).
+struct HeadParams { const float *fc_w, *fc_b, *xyz_w, *xyz_b, *wpqr_w, *wpqr_b; };
+struct HeadGrads { float *fc_w, *fc_b, *xyz_w, *xyz_b, *wpqr_w, *wpqr_b; };
+// droprate > 0: the dropout mask [B][F] from (seed, flat offset step * stride), or from the device counter *ctr when
+// step == ~0 (ctr advanced by one); hdrop = relu(fcpre) * mask, fcpre = feat @ fc_w^T + fc_b; pred [B][6]
+int head_forward(const HeadParams& hp, const float* feat, int B, int F, float droprate, unsigned long long seed,
+                 unsigned long long step, unsigned long long* ctr, unsigned long long stride, float* mask, float* fcpre,
+                 float* hdrop, float* pred, cudaStream_t st);
+// dpred [B][6] -> the two NaN-filtered copies dpredw / dpredh, gscale != null: this step's gradient scale of dpredh
+// (strict mode), the weight / bias gradients of hg, dh [B][F] (when fc trains or dfeat is wanted) and dfeat [B][512]
+// (dfeat != null: the trunk needs its gradient).  mask: the forward's dropout mask, or null.
+int head_backward(const HeadParams& hp, const HeadGrads& hg, const float* dpred, int filter_nans, const float* feat,
+                  const float* mask, const float* fcpre, const float* hdrop, int B, int F, float* dpredw, float* dpredh,
+                  float* gscale, float* dh, float* dfeat, cudaStream_t st);
 
 // ---- loss.cu -------------------------------------------------------------------
 int launch_loss(int mode, const float* pred, const float* targ, int N, int Tp, int Tt, const float* s4,

@@ -555,19 +555,9 @@ int Net::forward_t(const float* x, const float* params, float* bufs, int B, int 
   stats_target = nullptr;
   // head
   MN_TRY(launch_gap<TZ>(zin, feat, B, Hf * Wf, 512, st));
-  const float* mk = nullptr;
-  if (droprate > 0.f) {
-    const unsigned long long stride = (unsigned long long)max_B * feat_dim;
-    const bool dev_ctr = (step == ~0ULL);
-    MN_TRY(launch_dropout_mask(mask, (long long)B * feat_dim, droprate, seed, dev_ctr ? 0ULL : step * stride,
-                               dev_ctr ? drop_ctr : nullptr, stride, st));
-    mk = mask;
-  }
-  // hdrop = relu(feat @ Wfc^T + b) * mask ; fcpre kept for the ReLU gate
-  MN_TRY(launch_small_gemm(1, feat, 512, 1, params + fc_w, 512, 1, hdrop, feat_dim, B, feat_dim, 512, params + fc_b, fcpre, mk, st));
-  MN_TRY(launch_small_gemm(0, hdrop, feat_dim, 1, params + xyz_w, feat_dim, 1, pred, 6, B, 3, feat_dim, params + xyz_b, nullptr, nullptr, st));
-  MN_TRY(launch_small_gemm(0, hdrop, feat_dim, 1, params + wpqr_w, feat_dim, 1, pred + 3, 6, B, 3, feat_dim, params + wpqr_b, nullptr, nullptr, st));
-  last_B = B; last_training = training; last_has_mask = (mk != nullptr);
+  MN_TRY(head_forward(head_params(params), feat, B, feat_dim, droprate, seed, step, drop_ctr,
+                      (unsigned long long)max_B * feat_dim, mask, fcpre, hdrop, pred, st));
+  last_B = B; last_training = training; last_has_mask = droprate > 0.f;
   bwd_next_part = 0;
   return 0;
 }
@@ -619,23 +609,14 @@ int Net::backward_t(const float* dpred, const float* params, float* grads, int f
   const float* gs = (precision == PREC_TC_SPLIT) ? gscale : nullptr;
   const bool trunk = bwd_lo < (int)blocks.size();       // a conv or BatchNorm parameter needs a gradient
   if (do_head) {
-  MN_TRY(launch_dpred_filter(dpred, dpredf, dpredh, B, filter_nans, st));
-  if (gs != nullptr && trunk) MN_TRY(launch_grad_scale(dpredh, B * 6, gscale, st));
-  // dW_xyz[c][j] = sum_b dpred[b][c] * hdrop[b][j]
-  if (train_xyz_w) MN_TRY(launch_small_gemm(0, dpredf, 1, 6, hdrop, 1, F, grads + xyz_w, F, 3, F, B, nullptr, nullptr, nullptr, st));
-  if (train_wpqr_w) MN_TRY(launch_small_gemm(0, dpredf + 3, 1, 6, hdrop, 1, F, grads + wpqr_w, F, 3, F, B, nullptr, nullptr, nullptr, st));
-  if (train_xyz_b) MN_TRY(launch_colsum(dpredf, 6, B, 3, grads + xyz_b, st));
-  if (train_wpqr_b) MN_TRY(launch_colsum(dpredf + 3, 6, B, 3, grads + wpqr_b, st));
-  if (train_fc_w || train_fc_b || trunk)
-    MN_TRY(launch_head_dh(dpredh, params + xyz_w, params + wpqr_w, last_has_mask ? mask : nullptr, fcpre, dh, B, F, st));
-  // dW_fc[o][i] = sum_b dh[b][o] * feat[b][i];  db_fc = colsum(dh);  dfeat = dh @ W_fc
-  if (train_fc_w) MN_TRY(launch_small_gemm(0, dh, 1, F, feat, 1, 512, grads + fc_w, 512, F, 512, B, nullptr, nullptr, nullptr, st));
-  if (train_fc_b) MN_TRY(launch_colsum(dh, F, B, F, grads + fc_b, st));
-  if (trunk) {
-    MN_TRY(launch_small_gemm(0, dh, F, 1, params + fc_w, 1, 512, dfeat, 512, B, 512, F, nullptr, nullptr, nullptr, st));
-    MN_TRY(launch_gap_bwd<T>(dfeat, S0, B, Hf * Wf, 512, st));
-  }
-  bwd_pre = false;
+    HeadGrads hg;
+    hg.fc_w = train_fc_w ? grads + fc_w : nullptr; hg.fc_b = train_fc_b ? grads + fc_b : nullptr;
+    hg.xyz_w = train_xyz_w ? grads + xyz_w : nullptr; hg.xyz_b = train_xyz_b ? grads + xyz_b : nullptr;
+    hg.wpqr_w = train_wpqr_w ? grads + wpqr_w : nullptr; hg.wpqr_b = train_wpqr_b ? grads + wpqr_b : nullptr;
+    MN_TRY(head_backward(head_params(params), hg, dpred, filter_nans, feat, last_has_mask ? mask : nullptr, fcpre, hdrop,
+                         B, F, dpredf, dpredh, (trunk && gs != nullptr) ? gscale : nullptr, dh, trunk ? dfeat : nullptr, st));
+    if (trunk) MN_TRY(launch_gap_bwd<T>(dfeat, S0, B, Hf * Wf, 512, st));
+    bwd_pre = false;
   }
 
   // ---- residual blocks, last to first ----

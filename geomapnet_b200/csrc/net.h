@@ -60,6 +60,9 @@ struct Net {
   int max_w_elems;
   // parameter offsets of the head
   long long fc_w, fc_b, xyz_w, xyz_b, wpqr_w, wpqr_b;
+  HeadParams head_params(const float* params) const {
+    return HeadParams{params + fc_w, params + fc_b, params + xyz_w, params + xyz_b, params + wpqr_w, params + wpqr_b};
+  }
   // Which parameters need a gradient (set_trainable; default all).  The backward pass skips the weight gradients of the
   // others and every input gradient below the lowest layer that trains: bwd_lo is that layer's block, -1 for the stem,
   // blocks.size() when no conv or BatchNorm parameter trains.

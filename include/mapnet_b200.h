@@ -349,7 +349,8 @@ int mapnet_test_conv_ex(int precision, int kind, int B, int Hi, int Wi, int Ci, 
  * flags: bit 0 folds the downsample shortcut into a 3x3/s2 dgrad; bit 1 describes the strict-mode (tc_split) plan;
  * bit 2 describes the fp8 fprop plan of mapnet_test_conv_fp8 (kind 0, alone).  "f8_kb" is the fp8 plan's bytes per
  * k-block row (128, or 64 when Ci = 64), 0 for every other plan.  k == 7 (kind 0, Ci 3, Co 64, stride 2) describes the
- * stem as mapnet_test_conv_affine's k == 7 runs it: a 4x1 conv on the space-to-depth image of an Hi x Wi frame. */
+ * stem as mapnet_test_conv_affine's k == 7 runs it: a 4x1 conv on the space-to-depth image of an Hi x Wi frame; kind 2
+ * with k == 7 (flags 0 or 2) the stem's wgrad over that image, as mapnet_test_stem_ex runs it. */
 int mapnet_test_plan_describe(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, int flags,
                               char* buf, int cap);
 
@@ -436,6 +437,25 @@ int mapnet_test_stem_operand(int precision, mapnet_preprocess_t* pre, const void
 /* host-only: the split-K plan of the head's small fp32 GEMM for an [M,K] x [N,K]^T product with epilogue epi -- the
  * number of K splits and the length of each but the last (the plan mapnet_infer_sample reproduces for B rows) */
 int mapnet_test_small_gemm_plan(int epi, int M, int N, int K, int* splits, int* kchunk);
+/* the training step's stem (tensor-core modes: precision bf16 or tc_split) alone, as Net runs it: the space-to-depth
+ * image of x_nchw (fp32 [B,3,H,W]), the mode's pack of w_oihw (fp32 [64,3,7,7]), fprop into y_out ([B,Hc,Wc,64] NHWC;
+ * bf16, strict mode fp32) with, when host_sums != NULL, the BatchNorm-statistics epilogue: host_sums [2][64] doubles =
+ * (sum y, sum y^2) over the stored values.  dy != NULL (y_out's type and shape; strict mode cut into fp16 planes here):
+ * the wgrad, with out_scale (strict mode; 0 = none) as its gradient out-scale, re-laid out into dw_oihw [64,3,7,7].
+ * Arguments are checked before the device is touched.  mapnet_test_plan_describe(kind 0 / 2, k 7) gives its plans. */
+int mapnet_test_stem_ex(int precision, int B, int H, int W, const float* x_nchw, const float* w_oihw, void* y_out,
+                        const void* dy, float* dw_oihw, float out_scale, double* host_sums, void* stream);
+/* the pose head's forward and backward launch sequences, the ones the training step runs, on caller-owned fp32 device
+ * tensors: feat [B,512]; params (and grads) packed fc_w [F,512], fc_b [F], xyz_w [3,F], xyz_b [3], wpqr_w [3,F],
+ * wpqr_b [3].  Forward: droprate > 0 writes the dropout mask [B,F] of flat offset step * stride (step == UINT64_MAX: of
+ * the device counter *ctr, which is advanced by one); fcpre, hdrop [B,F] and pred [B,6].  dpred != NULL [B,6]: the
+ * backward with every parameter trained and the NaN filter when filter_nans: dh [B,F], dfeat [B,512], grads, and with
+ * scale2 != NULL the strict mode's gradient scale pair {S, 1/S} of the filtered dpred.  Arguments are checked before the
+ * device is touched. */
+int mapnet_test_head(int B, int F, const float* feat, const float* params, float droprate, uint64_t seed, uint64_t step,
+                     uint64_t stride, uint64_t* ctr, float* mask, float* fcpre, float* hdrop, float* pred,
+                     const float* dpred, int filter_nans, float* dh, float* dfeat, float* grads, float* scale2,
+                     void* stream);
 
 /* micro-benchmark of one tensor-core conv configuration (tools/bench_conv.py): average ms per launch */
 int mapnet_bench_conv(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* in0,
