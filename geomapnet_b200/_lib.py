@@ -20,6 +20,9 @@ LOSS_MODE = {"posenet": 0, "mapnet": 1, "online": 2, "online_gps": 3}
 TRACK_API = ["mapnet_track_create", "mapnet_track_step", "mapnet_track_flush", "mapnet_track_reset", "mapnet_track_status",
              "mapnet_track_destroy", "mapnet_track_step_now"]
 MAX_TRACK_STEPS = 16    # mapnet_track_create: windows of at most 16 frames (the PGO kernel's limit)
+TRACK_MULTI_API = ["mapnet_track_multi_create", "mapnet_track_multi_step", "mapnet_track_multi_flush",
+                   "mapnet_track_multi_reset", "mapnet_track_multi_status", "mapnet_track_multi_destroy"]
+MAX_TRACK_STREAMS = 65536   # mapnet_track_multi_create: MAPNET_TRACK_MAX_STREAMS
 
 _lib = None
 
@@ -158,6 +161,15 @@ def lib():
     L.mapnet_track_destroy.argtypes = [c_void_p]
     for name in TRACK_API:
         getattr(L, name).restype = c_int
+    L.mapnet_track_multi_create.argtypes = [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                            c_void_p]
+    L.mapnet_track_multi_step.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]
+    L.mapnet_track_multi_flush.argtypes = [c_void_p, c_int, c_void_p, c_void_p]
+    L.mapnet_track_multi_reset.argtypes = [c_void_p, c_int, c_void_p]
+    L.mapnet_track_multi_status.argtypes = [c_void_p, c_int, POINTER(c_int64), POINTER(c_int), c_void_p]
+    L.mapnet_track_multi_destroy.argtypes = [c_void_p]
+    for name in TRACK_MULTI_API:
+        getattr(L, name).restype = c_int
     L.mapnet_test_stem_operand.argtypes = [c_int, c_void_p, c_void_p, c_void_p, c_int, POINTER(c_float), POINTER(c_float),
                                            c_void_p, c_void_p]
     L.mapnet_test_stem_operand.restype = c_int
@@ -197,7 +209,7 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_trunk_set_trainable", "mapnet_test_conv_ex", "mapnet_eval_windows",
             "mapnet_batch_losses", "mapnet_infer_forward_frames", "mapnet_test_stem_operand", "mapnet_infer_sample",
             "mapnet_infer_sample_frames", "mapnet_sample_post", "mapnet_test_small_gemm_plan", "mapnet_test_stem_ex",
-            "mapnet_test_head"] + TRACK_API
+            "mapnet_test_head"] + TRACK_API + TRACK_MULTI_API
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 MAX_SAMPLE_DRAWS = 1024      # mapnet_infer_sample: S in [2, MAX_SAMPLE_DRAWS] dropout draws per frame
 

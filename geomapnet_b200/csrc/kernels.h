@@ -252,11 +252,12 @@ int launch_rmsprop(float* p, const float* g, float* square_avg, float* grad_avg,
 
 // ---- pgo.cu: pose-graph optimisation of n_windows windows of N poses (k_pgo) --------------------------------------
 // w4 = (1/sqrt(sax), 1/sqrt(saq), 1/sqrt(srx), 1/sqrt(srq)) from pgo_weights; n_win_dev (may be null): a device count
-// of windows, the blocks beyond it exit.  pgo_prepare sets k_pgo's shared-memory limit once (not graph-capturable).
+// of windows, the blocks beyond it exit; win_fail (may be null): per window 1 / 0, whether its normal matrix was not
+// positive definite.  pgo_prepare sets k_pgo's shared-memory limit once (not graph-capturable).
 int pgo_prepare();
 void pgo_weights(double sax, double saq, double srx, double srq, double w4[4]);
 int launch_pgo(const double* poses, const double* vos, double* out, int n_windows, int N, int fc, const double w4[4],
-               int n_iters, int exact, int* status, const int* n_win_dev, cudaStream_t st);
+               int n_iters, int exact, int* status, const int* n_win_dev, cudaStream_t st, int* win_fail = nullptr);
 
 // input pipeline internals shared by preprocess.cu and the frame cache (loader.cu)
 struct JitterParams;

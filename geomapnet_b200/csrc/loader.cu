@@ -204,6 +204,166 @@ k_track_emit(const double* __restrict__ opt7, TrackDev* __restrict__ st, int n, 
   if (w >= lead) track_emit_pose(win + 7 * (T / 2), un, ms, ss, out7 + 7LL * (w - lead));
 }
 
+// ---- multi-stream tracker (mapnet_track_multi_*, inference.MultiTracker): the same windows for n_streams independent
+// sequences, one set of launches per call.  Per stream: its frames so far and its status word; the rings are
+// [n_streams][R].  The host keeps count of every stream and builds one record per frame of a call, so the kernels
+// find every window without reading a counter: stream, rank among that stream's frames in the call, that stream's
+// frame count in the call, absolute frame index, the output row of the frame's completed window (-1: none yet), and
+// (a per-row field) the record whose completed window is output row b (-1 once the call's rows are done).
+struct MTrackDev {
+  long long seen;
+  int status, pad;
+};
+struct MTrackRec { int stream, rank, count, frame, row, win; };
+
+// one window of a multi-stream call: its stream, centre, the last frame its slots may reach and the stream's first
+// frame in this call (slots from there on come from the call's inputs)
+struct MWin {
+  int s;
+  long long c, last, f0;
+};
+
+// Window w of a call, false when the call has no window w.  A step's windows are the completed ones in output-row
+// order (rec[w].win), a zero-lag step's the one that ends at each record's frame (record w); a flush of stream
+// flush_s >= 0 solves that stream's pending windows, clipped at its last frame.
+__device__ __forceinline__ bool mtrack_window(const MTrackRec* rec, int B, int w, int now, int flush_s,
+                                              const MTrackDev* st, int n_streams, long long lag, MWin* o) {
+  if (flush_s >= 0) {
+    const long long seen = st[flush_s].seen, first = trackcore::first_pending(seen, lag);
+    if (w >= seen - first) return false;
+    o->s = flush_s; o->c = first + w; o->last = seen - 1; o->f0 = seen;
+    return true;
+  }
+  if (w >= B) return false;
+  const int b = now ? w : rec[w].win;
+  if (b < 0 || b >= B) return false;
+  const MTrackRec r = rec[b];
+  if (r.stream < 0 || r.stream >= n_streams) return false;
+  o->s = r.stream;
+  o->c = trackcore::now_first(r.frame, lag);       // frame (f - lag)'s window ends at f
+  o->f0 = (long long)r.frame - r.rank;
+  o->last = o->f0 + r.count - 1;
+  return true;
+}
+
+// input row of new frame f of window m's stream: the record of that stream at rank f - f0 (the call's only search)
+__device__ __forceinline__ int mtrack_input(const MTrackRec* rec, int B, const MWin& m, long long f) {
+  const int rank = (int)(f - m.f0);
+  for (int b = 0; b < B; ++b)
+    if (rec[b].stream == m.s && rec[b].rank == rank) return b;
+  return -1;
+}
+
+__device__ __forceinline__ posemath::Pose6 mtrack_vo(const float* vo6, const float* ring_vo, const MTrackRec* rec,
+                                                     int B, const MWin& m, long long f, long long R) {
+  if (f >= m.f0) {
+    const int b = mtrack_input(rec, B, m, f);
+    if (b >= 0) return ld_pose6(vo6 + 6LL * b);
+    const float nan = __int_as_float(0x7fc00000);   // an inconsistent record table: a visible NaN, no stray read
+    const float v6[6] = {nan, nan, nan, nan, nan, nan};
+    return ld_pose6(v6);
+  }
+  return ld_pose6(ring_vo + 6 * (m.s * R + f % R));
+}
+
+// k_track_gather for B frames of several streams (records rec) or a flush of stream flush_s: rows 0 .. B-1 write
+// the new frames into their streams' rings, then slot (w, k) of window w < max_win, then VO (w, e).  The values are
+// k_track_gather's (st_pose7, calc_vo_logq_safe), so each window is bit for bit the single-stream tracker's.  Thread
+// 0 writes the count of windows k_pgo and the emit read: the completed windows of a step (the records with a row), B
+// for a zero-lag step, the stream's pending windows for a flush.
+__global__ void __launch_bounds__(128)
+k_track_multi_gather(const float* __restrict__ pred6, const float* __restrict__ vo6, const MTrackRec* __restrict__ rec,
+                     int B, int now, int flush_s, const MTrackDev* __restrict__ st, int n_streams,
+                     int* __restrict__ n_win_dev, double* __restrict__ ring7, float* __restrict__ ring_vo, long long R,
+                     int T, int skip, int fc, int max_win, double* __restrict__ win7, double* __restrict__ vos7) {
+  pdl_prologue();
+  const long long lag = trackcore::lag(T, skip);
+  const int E = fc ? T * (T - 1) / 2 : T - 1;
+  long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r == 0) {
+    int n = 0;
+    if (flush_s >= 0) n = (int)(st[flush_s].seen - trackcore::first_pending(st[flush_s].seen, lag));
+    else if (now) n = B;
+    else while (n < B && rec[n].win >= 0) ++n;
+    *n_win_dev = n;
+  }
+  if (r < B) {
+    const MTrackRec q = rec[r];
+    if (q.stream < 0 || q.stream >= n_streams) return;
+    const long long k = q.stream * R + q.frame % R;
+    st_pose7(pred6 + 6 * r, ring7 + 7 * k);
+#pragma unroll
+    for (int c = 0; c < 6; ++c) ring_vo[6 * k + c] = vo6[6 * r + c];
+    return;
+  }
+  r -= B;
+  MWin m;
+  if (r < (long long)max_win * T) {
+    const int w = (int)(r / T), k = (int)(r % T);
+    if (!mtrack_window(rec, B, w, now, flush_s, st, n_streams, lag, &m)) return;
+    const long long f = trackcore::slot_frame(m.c, k, T, skip, m.last);
+    if (f >= m.f0) {
+      const int b = mtrack_input(rec, B, m, f);
+      const float nan = __int_as_float(0x7fc00000);
+      const float v6[6] = {nan, nan, nan, nan, nan, nan};
+      st_pose7(b >= 0 ? pred6 + 6LL * b : v6, win7 + 7 * r);
+    } else {
+      const double* src = ring7 + 7 * (m.s * R + f % R);
+#pragma unroll
+      for (int c = 0; c < 7; ++c) win7[7 * r + c] = src[c];
+    }
+    return;
+  }
+  r -= (long long)max_win * T;
+  if (r < (long long)max_win * E) {
+    const int w = (int)(r / E), e = (int)(r % E);
+    if (!mtrack_window(rec, B, w, now, flush_s, st, n_streams, lag, &m)) return;
+    int i, j;
+    trackcore::vo_pair(e, T, fc, &i, &j);
+    const long long fa = trackcore::slot_frame(m.c, i, T, skip, m.last);
+    const long long fb = trackcore::slot_frame(m.c, j, T, skip, m.last);
+    const posemath::Pose6 v = posemath::calc_vo_logq_safe(mtrack_vo(vo6, ring_vo, rec, B, m, fa, R),
+                                                          mtrack_vo(vo6, ring_vo, rec, B, m, fb, R));
+    const float v6[6] = {v.t.x, v.t.y, v.t.z, v.l.x, v.l.y, v.l.z};
+    st_pose7(v6, vos7 + 7 * r);
+  }
+}
+
+// k_track_emit for several streams: window w's middle slot into out7 row w (a zero-lag step: into row rec[w].row
+// when the window completed a frame, and its last slot into now7 row w); a window k_pgo marked failed sets its
+// stream's status; the last record of each stream in the call sets that stream's frame count.
+__global__ void __launch_bounds__(128)
+k_track_multi_emit(const double* __restrict__ opt7, const int* __restrict__ win_fail, const MTrackRec* __restrict__ rec,
+                   int B, int flush_s, MTrackDev* __restrict__ st, int n_streams, const int* __restrict__ n_win_dev,
+                   int T, int un, double m0, double m1, double m2, double s0, double s1, double s2,
+                   double* __restrict__ out7, double* __restrict__ now7) {
+  pdl_prologue();
+  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+  const double ms[3] = {m0, m1, m2}, ss[3] = {s0, s1, s2};
+  const double* win = opt7 + 7LL * w * T;
+  if (w < B) {
+    const MTrackRec q = rec[w];
+    const bool ok = q.stream >= 0 && q.stream < n_streams;
+    if (ok && q.rank == q.count - 1) st[q.stream].seen = (long long)q.frame + 1;
+    if (now7 != nullptr) {
+      if (!ok) return;
+      track_emit_pose(win + 7 * (T - 1), un, ms, ss, now7 + 7LL * w);
+      if (q.row >= 0) track_emit_pose(win + 7 * (T / 2), un, ms, ss, out7 + 7LL * q.row);
+      if (win_fail[w]) atomicExch(&st[q.stream].status, 1);
+      return;
+    }
+  }
+  if (now7 != nullptr || w >= *n_win_dev) return;
+  int s = flush_s;
+  if (s < 0) {
+    const int b = rec[w].win;
+    s = b >= 0 && b < B ? rec[b].stream : -1;
+    if (s < 0 || s >= n_streams) return;
+  }
+  track_emit_pose(win + 7 * (T / 2), un, ms, ss, out7 + 7LL * w);
+  if (win_fail[w]) atomicExch(&st[s].status, 1);
+}
+
 }  // namespace mapnet
 
 using namespace mapnet;
@@ -366,12 +526,39 @@ int mapnet_eval_windows(const float* pred6, int n_pred, const float* poses, cons
 
 }  // extern "C"
 
-struct mapnet_track {
+// what a tracker handle is created with: window geometry, PGO weights, pose statistics (single and multi-stream)
+struct TrackCfg {
   int T, skip, fc, max_batch, E, max_win;   // max_win: the most windows one call completes, max(max_batch, lag)
   long long R, lag;
   double w4[4];                             // PGO weights 1/sqrt(sigma) of sax, saq, srx, srq
   int un;
   double m[3], s[3];
+};
+
+// checks a tracker's arguments (messages prefixed with `who`) and fills c; nothing is allocated or launched
+static int track_config(TrackCfg* c, const char* who, int T, int skip, int fc_vos, int max_batch, const double* sigmas4,
+                        const double* pose_m3, const double* pose_s3) {
+  MN_CHECK(T >= 2 && T <= 16, "%s: windows of %d frames outside [2, 16]", who, T);
+  MN_CHECK(skip >= 1 && max_batch >= 1, "%s: skip = %d and max_batch = %d must be >= 1", who, skip, max_batch);
+  for (int k = 0; k < 4; ++k) MN_CHECK(sigmas4[k] > 0, "%s: sigma %d = %g must be positive", who, k, sigmas4[k]);
+  MN_CHECK((pose_m3 == nullptr) == (pose_s3 == nullptr), "%s: pose_m3 and pose_s3 go together", who);
+  const long long lag = trackcore::lag(T, skip), R = trackcore::ring_frames(max_batch, T, skip);
+  MN_CHECK(R < (1LL << 26), "%s: a ring of %lld frames", who, R);
+  int ndev = 0;
+  MN_CHECK(cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0, "%s: no CUDA device (this library has no CPU fallback)",
+           who);
+  MN_TRY(pgo_prepare());
+  c->T = T; c->skip = skip; c->fc = fc_vos ? 1 : 0; c->max_batch = max_batch;
+  c->E = c->fc ? T * (T - 1) / 2 : T - 1;
+  c->lag = lag; c->R = R;
+  c->max_win = (int)(lag > max_batch ? lag : max_batch);
+  pgo_weights(sigmas4[0], sigmas4[1], sigmas4[2], sigmas4[3], c->w4);
+  c->un = pose_m3 != nullptr;
+  for (int k = 0; k < 3; ++k) { c->m[k] = c->un ? pose_m3[k] : 0.0; c->s[k] = c->un ? pose_s3[k] : 1.0; }
+  return 0;
+}
+
+struct mapnet_track : TrackCfg {
   TrackDev* st;
   double* ring7;                            // [R][7]: pose7 of the last R frames, normalised translations
   float* ring_vo;                           // [R][6]: their VO-library poses
@@ -401,23 +588,11 @@ int mapnet_track_create(mapnet_track_t** out, int T, int skip, int fc_vos, int m
                         const double* pose_m3, const double* pose_s3) {
   MN_CHECK(out != nullptr && sigmas4 != nullptr, "track_create: null argument");
   *out = nullptr;
-  MN_CHECK(T >= 2 && T <= 16, "track_create: windows of %d frames outside [2, 16]", T);
-  MN_CHECK(skip >= 1 && max_batch >= 1, "track_create: skip = %d and max_batch = %d must be >= 1", skip, max_batch);
-  for (int k = 0; k < 4; ++k) MN_CHECK(sigmas4[k] > 0, "track_create: sigma %d = %g must be positive", k, sigmas4[k]);
-  MN_CHECK((pose_m3 == nullptr) == (pose_s3 == nullptr), "track_create: pose_m3 and pose_s3 go together");
-  const long long lag = trackcore::lag(T, skip), R = trackcore::ring_frames(max_batch, T, skip);
-  MN_CHECK(R < (1LL << 26), "track_create: a ring of %lld frames", R);
-  int ndev = 0;
-  MN_CHECK(cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0, "track_create: no CUDA device (this library has no CPU fallback)");
-  MN_TRY(pgo_prepare());
+  TrackCfg c;
+  MN_TRY(track_config(&c, "track_create", T, skip, fc_vos, max_batch, sigmas4, pose_m3, pose_s3));
+  const long long R = c.R;
   mapnet_track* h = new mapnet_track();
-  h->T = T; h->skip = skip; h->fc = fc_vos ? 1 : 0; h->max_batch = max_batch;
-  h->E = h->fc ? T * (T - 1) / 2 : T - 1;
-  h->lag = lag; h->R = R;
-  h->max_win = (int)(lag > max_batch ? lag : max_batch);
-  pgo_weights(sigmas4[0], sigmas4[1], sigmas4[2], sigmas4[3], h->w4);
-  h->un = pose_m3 != nullptr;
-  for (int k = 0; k < 3; ++k) { h->m[k] = h->un ? pose_m3[k] : 0.0; h->s[k] = h->un ? pose_s3[k] : 1.0; }
+  static_cast<TrackCfg&>(*h) = c;
   const size_t W = (size_t)h->max_win;
   bool ok = cudaMalloc((void**)&h->st, sizeof(TrackDev)) == cudaSuccess &&
             cudaMalloc((void**)&h->ring7, (size_t)R * 7 * sizeof(double)) == cudaSuccess &&
@@ -477,6 +652,120 @@ int mapnet_track_status(mapnet_track_t* h, int64_t* frames_seen, int* failed, vo
 int mapnet_track_destroy(mapnet_track_t* h) {
   if (h == nullptr) return 0;
   cudaFree(h->st); cudaFree(h->ring7); cudaFree(h->ring_vo); cudaFree(h->win7); cudaFree(h->vos7); cudaFree(h->opt7);
+  delete h;
+  return 0;
+}
+
+}  // extern "C"
+
+struct mapnet_track_multi : TrackCfg {
+  int n_streams;
+  MTrackDev* st;                            // [n_streams]
+  int* n_win;                               // the windows of the current call, written by the gather
+  int* win_fail;                            // [max_win]: k_pgo's per-window failure flags
+  double* ring7;                            // [n_streams][R][7]
+  float* ring_vo;                           // [n_streams][R][6]
+  double *win7, *vos7, *opt7;               // [max_win][T][7], [max_win][E][7], [max_win][T][7]
+};
+
+// the three launches of a multi-stream call: B frames with records rec (a step; with now7 a zero-lag step, which
+// solves all B of its windows) or a flush of stream flush_s (B = 0)
+static int track_multi_launch(mapnet_track_multi_t* h, const float* pred6, const float* vo6, const MTrackRec* rec,
+                              int B, int flush_s, double* out7, double* now7, cudaStream_t st) {
+  const int nw = flush_s >= 0 ? (int)(h->lag < h->max_win ? h->lag : h->max_win) : B;    // the grid's windows
+  const int now = now7 != nullptr ? 1 : 0;
+  const long long rows = B + (long long)nw * (h->T + h->E);
+  MN_LAUNCH(k_track_multi_gather, cdiv(rows, 128), 128, 0, st, pred6, vo6, rec, B, now, flush_s,
+            (const MTrackDev*)h->st, h->n_streams, h->n_win, h->ring7, h->ring_vo, h->R, h->T, h->skip, h->fc, nw,
+            h->win7, h->vos7);
+  MN_LAUNCH_CHECK();
+  MN_TRY(launch_pgo(h->win7, h->vos7, h->opt7, nw, h->T, h->fc, h->w4, 10, 0, nullptr, now ? nullptr : h->n_win, st,
+                    h->win_fail));
+  MN_LAUNCH(k_track_multi_emit, cdiv(nw > B ? nw : B, 128), 128, 0, st, (const double*)h->opt7,
+            (const int*)h->win_fail, rec, B, flush_s, h->st, h->n_streams, (const int*)h->n_win, h->T, h->un, h->m[0],
+            h->m[1], h->m[2], h->s[0], h->s[1], h->s[2], out7, now7);
+  MN_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" {
+
+int mapnet_track_multi_create(mapnet_track_multi_t** out, int n_streams, int T, int skip, int fc_vos, int max_batch,
+                              const double* sigmas4, const double* pose_m3, const double* pose_s3) {
+  MN_CHECK(out != nullptr && sigmas4 != nullptr, "track_multi_create: null argument");
+  *out = nullptr;
+  MN_CHECK(n_streams >= 1 && n_streams <= MAPNET_TRACK_MAX_STREAMS, "track_multi_create: %d streams outside [1, %d]",
+           n_streams, MAPNET_TRACK_MAX_STREAMS);
+  TrackCfg c;
+  MN_TRY(track_config(&c, "track_multi_create", T, skip, fc_vos, max_batch, sigmas4, pose_m3, pose_s3));
+  const size_t W = (size_t)c.max_win, ring = (size_t)n_streams * (size_t)c.R;
+  const size_t bytes = ring * (7 * sizeof(double) + 6 * sizeof(float)) + W * (2 * c.T + c.E) * 7 * sizeof(double) +
+                       (size_t)n_streams * sizeof(MTrackDev) + (W + 1) * sizeof(int);
+  MN_CHECK(ring < (1ull << 31), "track_multi_create: %d streams x rings of %lld frames = %zu frames (%.3f GB) exceed "
+           "2^31 ring frames", n_streams, c.R, ring, bytes / 1e9);
+  mapnet_track_multi* h = new mapnet_track_multi();
+  static_cast<TrackCfg&>(*h) = c;
+  h->n_streams = n_streams;
+  bool ok = cudaMalloc((void**)&h->st, (size_t)n_streams * sizeof(MTrackDev)) == cudaSuccess &&
+            cudaMalloc((void**)&h->n_win, (W + 1) * sizeof(int)) == cudaSuccess &&
+            cudaMalloc((void**)&h->ring7, ring * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->ring_vo, ring * 6 * sizeof(float)) == cudaSuccess &&
+            cudaMalloc((void**)&h->win7, W * c.T * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->vos7, W * c.E * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->opt7, W * c.T * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMemset(h->st, 0, (size_t)n_streams * sizeof(MTrackDev)) == cudaSuccess &&
+            cudaMemset(h->n_win, 0, (W + 1) * sizeof(int)) == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess;
+  if (!ok) {
+    cudaGetLastError();
+    set_last_error("track_multi_create: device allocation of %zu bytes (%d streams x rings of %lld frames, %d windows) "
+                   "failed", bytes, n_streams, c.R, c.max_win);
+    mapnet_track_multi_destroy(h);
+    return 1;
+  }
+  h->win_fail = h->n_win + 1;
+  *out = h;
+  return 0;
+}
+
+int mapnet_track_multi_step(mapnet_track_multi_t* h, const float* pred6, const float* vo6, const int32_t* rec, int B,
+                            double* out7, double* now7, void* stream) {
+  MN_CHECK(h != nullptr, "track_multi_step: null handle");
+  MN_CHECK(pred6 != nullptr && vo6 != nullptr && rec != nullptr && out7 != nullptr, "track_multi_step: null argument");
+  MN_CHECK(B >= 1 && B <= h->max_batch, "track_multi_step: %d frames outside [1, max_batch=%d]", B, h->max_batch);
+  return track_multi_launch(h, pred6, vo6, (const MTrackRec*)rec, B, -1, out7, now7, (cudaStream_t)stream);
+}
+
+int mapnet_track_multi_flush(mapnet_track_multi_t* h, int s, double* out7, void* stream) {
+  MN_CHECK(h != nullptr, "track_multi_flush: null handle");
+  MN_CHECK(out7 != nullptr, "track_multi_flush: null argument");
+  MN_CHECK(s >= 0 && s < h->n_streams, "track_multi_flush: stream %d outside [0, %d)", s, h->n_streams);
+  if (h->lag == 0) return 0;                 // every window was complete when its last frame arrived
+  return track_multi_launch(h, nullptr, nullptr, nullptr, 0, s, out7, nullptr, (cudaStream_t)stream);
+}
+
+int mapnet_track_multi_reset(mapnet_track_multi_t* h, int s, void* stream) {
+  MN_CHECK(h != nullptr, "track_multi_reset: null handle");
+  MN_CHECK(s >= -1 && s < h->n_streams, "track_multi_reset: stream %d outside [-1, %d)", s, h->n_streams);
+  const size_t n = s < 0 ? (size_t)h->n_streams : 1;
+  MN_CUDA(cudaMemsetAsync(h->st + (s < 0 ? 0 : s), 0, n * sizeof(MTrackDev), (cudaStream_t)stream));
+  return 0;
+}
+
+int mapnet_track_multi_status(mapnet_track_multi_t* h, int s, int64_t* frames_seen, int* failed, void* stream) {
+  MN_CHECK(h != nullptr, "track_multi_status: null handle");
+  MN_CHECK(s >= 0 && s < h->n_streams, "track_multi_status: stream %d outside [0, %d)", s, h->n_streams);
+  MTrackDev d;
+  MN_CUDA(cudaMemcpyAsync(&d, h->st + s, sizeof(MTrackDev), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  MN_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+  if (frames_seen != nullptr) *frames_seen = d.seen;
+  if (failed != nullptr) *failed = d.status;
+  return 0;
+}
+
+int mapnet_track_multi_destroy(mapnet_track_multi_t* h) {
+  if (h == nullptr) return 0;
+  cudaFree(h->st); cudaFree(h->n_win); cudaFree(h->ring7); cudaFree(h->ring_vo); cudaFree(h->win7); cudaFree(h->vos7);
+  cudaFree(h->opt7);
   delete h;
   return 0;
 }

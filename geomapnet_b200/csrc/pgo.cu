@@ -80,11 +80,12 @@ __device__ __forceinline__ void dqstq_t(const Q4& q, double D[3][3]) {
 // One window per block.  Constraints are dealt to threads; each thread accumulates into the shared H / b with
 // double atomics (a few hundred constraints x <= 144 entries: contention is irrelevant next to the Cholesky).
 // n_win_dev (may be null): the device count of windows to optimise; the blocks beyond it exit, so a captured graph can
-// keep a fixed grid while the count changes from replay to replay.
+// keep a fixed grid while the count changes from replay to replay.  win_fail (may be null): per window, 1 when its
+// normal matrix was not positive definite, else 0, so a caller can tell which windows failed.
 __global__ void __launch_bounds__(kPgoThreads)
 k_pgo(const double* __restrict__ poses, const double* __restrict__ vos, double* __restrict__ out, int N, int fc,
       double w_ax, double w_aq, double w_rx, double w_rq, int n_iters, int exact, int* __restrict__ status,
-      const int* __restrict__ n_win_dev) {
+      const int* __restrict__ n_win_dev, int* __restrict__ win_fail) {
   pdl_prologue();
   if (n_win_dev != nullptr && (int)blockIdx.x >= *n_win_dev) return;
   extern __shared__ double sm[];
@@ -243,6 +244,7 @@ k_pgo(const double* __restrict__ poses, const double* __restrict__ vos, double* 
   double* O = out + (size_t)W * N * 7;
   for (int i = threadIdx.x; i < 7 * N; i += blockDim.x) O[i] = z[i];
   if (threadIdx.x == 0 && s_fail && status != nullptr) atomicExch(status, 1);
+  if (threadIdx.x == 0 && win_fail != nullptr) win_fail[W] = s_fail;
 }
 
 int pgo_prepare() {
@@ -252,12 +254,12 @@ int pgo_prepare() {
 }
 
 int launch_pgo(const double* poses, const double* vos, double* out, int n_windows, int N, int fc, const double w4[4],
-               int n_iters, int exact, int* status, const int* n_win_dev, cudaStream_t st) {
+               int n_iters, int exact, int* status, const int* n_win_dev, cudaStream_t st, int* win_fail) {
   MN_TRY(pgo_prepare());
   const int D = 6 * N;
   const size_t smem = (size_t)(D * D + D + 7 * N + D) * sizeof(double);
   MN_LAUNCH(k_pgo, n_windows, kPgoThreads, smem, st, poses, vos, out, N, fc, w4[0], w4[1], w4[2], w4[3], n_iters, exact,
-            status, n_win_dev);
+            status, n_win_dev, win_fail);
   MN_LAUNCH_CHECK();
   return 0;
 }

@@ -23,7 +23,7 @@ from . import _lib
 from .common.pgo import optimize_pose_windows
 from .data.loader import SidePipeline
 
-__all__ = ["Predictor", "Localizer", "Tracker", "predict", "post", "pgo", "pose_errors", "evaluate_tuples", "evaluate_sequence", "validate"]
+__all__ = ["Predictor", "Localizer", "Tracker", "MultiTracker", "predict", "post", "pgo", "pose_errors", "evaluate_tuples", "evaluate_sequence", "validate"]
 
 
 class Predictor(object):
@@ -571,6 +571,8 @@ class Tracker(object):
     sizes.  A window whose normal matrix is not positive definite (where scipy's cholesky raises) is reported by
     flush(), which raises np.linalg.LinAlgError after resetting."""
 
+    _DESTROY = "mapnet_track_destroy"      # the C call that frees the handle
+
     def __init__(self, localizer, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0):
         if not isinstance(localizer, Localizer):
             raise TypeError("Tracker wraps a geomapnet_b200.inference.Localizer, got %s" % type(localizer).__name__)
@@ -588,11 +590,11 @@ class Tracker(object):
         self._open = True
 
     def _check_open(self):
+        name = type(self).__name__
         if not self._open:
-            raise ValueError("Tracker is closed")
+            raise ValueError("%s is closed" % name)
         if not self.loc._open or self.loc.predictor._params is None:
-            raise ValueError("the Tracker's Localizer is closed" if not self.loc._open else
-                             "the Tracker's Predictor is closed")
+            raise ValueError("the %s's %s is closed" % (name, "Localizer" if not self.loc._open else "Predictor"))
 
     def _vo(self, vo_poses, n, single):
         """vo_poses as a tensor [n,6] of a real floating dtype; raises on anything else"""
@@ -714,9 +716,196 @@ class Tracker(object):
             torch.cuda.current_stream(self.loc.predictor.device).synchronize()
             self._graphs.clear()
             self._now_graphs.clear()
-            _lib.lib().mapnet_track_destroy(self.h)
+            getattr(_lib.lib(), self._DESTROY)(self.h)
             self.h = ctypes.c_void_p()
         self._open = False
+
+
+def _stream_records(seen, streams, lag):
+    """The records of one chunk of a multi-stream call (mapnet_track_multi_step's rec): streams int64 [B], the stream
+    of each frame in call order; seen int64 [n_streams], each stream's frames before the chunk.  Returns (rec int32
+    [B,6], sid int64 [n], fid int64 [n]): a completed window per frame f >= lag of its stream, that of frame f - lag,
+    in call order.  Adding np.bincount(streams) to seen gives the counts after the chunk."""
+    B = streams.shape[0]
+    order = np.argsort(streams, kind="stable")
+    srt = streams[order]
+    rank = np.empty(B, np.int64)
+    rank[order] = np.arange(B) - np.searchsorted(srt, srt, side="left")
+    count = np.bincount(streams, minlength=seen.shape[0])[streams]
+    frame = seen[streams] + rank
+    if B and frame.max() >= 2 ** 31:
+        raise ValueError("a stream reached frame 2^31; flush or reset it")
+    done = np.flatnonzero(frame >= lag)
+    rec = np.full((B, 6), -1, dtype=np.int32)
+    rec[:, 0], rec[:, 1], rec[:, 2], rec[:, 3] = streams, rank, count, frame
+    rec[done, 4] = np.arange(done.shape[0])
+    rec[:done.shape[0], 5] = done
+    return rec, streams[done], frame[done] - lag
+
+
+def _stream_chunks(seen, streams, lag, max_batch):
+    """Yields (lo, rec, sid, fid) for each chunk of max_batch frames of a multi-stream call (_stream_records), and
+    advances seen (int64 [n_streams], in place) by the chunk's frames once the caller has run it."""
+    for lo in range(0, streams.shape[0], max_batch):
+        sb = streams[lo:lo + max_batch]
+        rec, sid, fid = _stream_records(seen, sb, lag)
+        yield (lo, rec, sid, fid)
+        seen += np.bincount(sb, minlength=seen.shape[0])
+
+
+class MultiTracker(Tracker):
+    """Tracker for n_streams independent camera streams that share one Localizer: the frames of any streams go through
+    the engine as one batch, and one set of tracking launches serves all of them.
+
+        mt = MultiTracker(loc, n_streams=64, steps=7, skip=10, vo_fc=True, sax=1, saq=1, srx=20, srq=20)
+        sid, fid, pose7 = mt(frames, vo_poses, streams)     # frames / vo_poses as Tracker takes them; streams: B ints
+        now7, sid, fid, pose7 = mt.step(frames, vo_poses, streams)
+        first, pose7 = mt.flush(s)          # stream s alone: its last min(lag, seen[s]) frames; starts a new sequence
+        mt.reset(); mt.reset(s); mt.seen; mt.lag; mt.close()
+
+    streams gives each frame's stream, an int in [0, n_streams): a list, an ndarray or a CPU integer tensor (an int for
+    one [H,W,3] frame).  A stream may appear several times in a call, its frames in call order; streams absent from a
+    call are untouched.  Each stream is tracked exactly as a Tracker of the same arguments tracks it: its poses are bit
+    for bit what a Tracker fed that stream's frames in order gives (with droprate > 0, from the same per-frame draws).
+    (sid, fid, pose7) are the windows the call completes, one row per given frame f >= lag of its stream, for frame
+    f - lag of stream sid, in call order; sid and fid are int64 CPU tensors the host knows without waiting for the
+    device, pose7 is float64 [n,7] on the device.  step's now7 [B,7] is each given frame's zero-lag pose
+    (Tracker.step), in the order given.  seen is each stream's frame count (int64 [n_streams]).
+
+    A call of more than max_batch frames runs in chunks of max_batch, in order, one graph replay each: the engine's
+    launches and three tracking launches (csrc/loader.cu, mapnet_track_multi_*), captured per (B, H, W) as Tracker
+    captures; the per-frame records (stream, rank, counts, frame index, output row) are built on the host from its own
+    counts and copied in with the frames.  All frames of a call share one H x W.  A window whose normal matrix is not
+    positive definite marks its own stream only: flush(s) raises np.linalg.LinAlgError for stream s after resetting
+    it."""
+
+    _DESTROY = "mapnet_track_multi_destroy"
+
+    def __init__(self, localizer, n_streams, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0):
+        super(MultiTracker, self).__init__(localizer, steps, skip, vo_fc, sax, saq, srx, srq)
+        self.n_streams = _int_arg(n_streams, "n_streams", 1, _lib.MAX_TRACK_STREAMS)
+        self.seen = np.zeros(self.n_streams, dtype=np.int64)    # frames of each stream's sequence, mirrored on the device
+
+    def _handle(self):
+        if not self.h:
+            pr = self.loc.predictor
+            sig = (ctypes.c_double * 4)(*self.sigmas)
+            _lib.check(_lib.lib().mapnet_track_multi_create(ctypes.byref(self.h), self.n_streams, self.steps, self.skip,
+                                                            int(self.vo_fc), pr.max_batch, sig, self.loc._m,
+                                                            self.loc._s), "mapnet_track_multi_create")
+        return self.h
+
+    def _stream_ids(self, streams, B, single):
+        """streams as int64 [B]; raises on anything that is not B ints in [0, n_streams)"""
+        if torch.is_tensor(streams):
+            if streams.device.type != "cpu":
+                raise ValueError("streams must be a list, an ndarray or a CPU integer tensor, got a tensor on %s"
+                                 % streams.device)
+            streams = streams.numpy()
+        ids = np.asarray(streams)
+        if ids.dtype.kind not in "iu":
+            raise ValueError("stream ids must be integers, got %s" % ids.dtype)
+        if ids.ndim == 0 and single:
+            ids = ids.reshape(1)
+        if ids.ndim != 1 or ids.shape[0] != B:
+            raise ValueError("streams must hold one id per frame: %d, got shape %s" % (B, tuple(ids.shape)))
+        if B and (ids.min() < 0 or ids.max() >= self.n_streams):
+            raise ValueError("stream ids must be in [0, %d), got %d .. %d" % (self.n_streams, ids.min(), ids.max()))
+        return ids.astype(np.int64)
+
+    def _graph(self, fb, now=False):
+        B, H, W = fb.shape[:3]
+        graphs = self._now_graphs if now else self._graphs
+        g = graphs.get((B, H, W))
+        if g is None:
+            dev, h = self.loc.predictor.device, self._handle()
+            vs = torch.zeros((B, 6), dtype=torch.float32, device=dev)
+            rs = torch.zeros((B, 6), dtype=torch.int32, device=dev)
+            out = torch.empty((B, 7), dtype=torch.float64, device=dev)
+            now7 = torch.empty((B, 7), dtype=torch.float64, device=dev) if now else None
+
+            def track(pred):
+                _lib.check(_lib.lib().mapnet_track_multi_step(h, pred.data_ptr(), vs.data_ptr(), rs.data_ptr(), B,
+                                                              out.data_ptr(), now7.data_ptr() if now else None,
+                                                              _lib.stream_ptr()), "mapnet_track_multi_step")
+
+            graph, xs, pred = self.loc._capture(fb, track, eager_tail=False)  # the eager run must not advance a stream
+            g = graphs[(B, H, W)] = (graph, xs, vs, rs, out, pred, now7)     # every buffer the graph reads stays alive
+        return g
+
+    def _run(self, frames, vo_poses, streams, now):
+        """(sid [n], fid [n], pose7 [n,7], now7 [B,7] or None): the chunks of max_batch frames, one graph replay each"""
+        self._check_open()
+        x, single = self.loc._frames(frames)
+        vo = self._vo(vo_poses, x.shape[0], single)
+        ids = self._stream_ids(streams, x.shape[0], single)
+        pr = self.loc.predictor
+        mb = pr.max_batch
+        sids, fids, outs, nows = [], [], [], []
+        with torch.cuda.device(pr.device):
+            for lo, rec, sid, fid in _stream_chunks(self.seen, ids, self.lag, mb):
+                fb = x[lo:lo + mb]
+                graph, xs, vs, rs, out, _, now7 = self._graph(fb, now)
+                xs.copy_(fb, non_blocking=True)
+                vs.copy_(vo[lo:lo + mb], non_blocking=True)
+                rs.copy_(torch.from_numpy(rec), non_blocking=True)
+                graph.replay()
+                sids.append(torch.from_numpy(sid))
+                fids.append(torch.from_numpy(fid))
+                outs.append(out[:sid.shape[0]].clone())
+                if now:
+                    nows.append(now7.clone())
+        cat = lambda ts: ts[0] if len(ts) == 1 else torch.cat(ts, 0)
+        return cat(sids), cat(fids), cat(outs), (cat(nows) if now else None)
+
+    @torch.no_grad()
+    def __call__(self, frames, vo_poses, streams):
+        """-> (sid int64 [n], fid int64 [n], pose7 float64 [n,7] on the device): the windows this call completes"""
+        sid, fid, pose7, _ = self._run(frames, vo_poses, streams, False)
+        return sid, fid, pose7
+
+    @torch.no_grad()
+    def step(self, frames, vo_poses, streams):
+        """-> (now7 float64 [B,7] on the device, sid, fid, pose7): row b of now7 is the zero-lag pose of the b-th frame
+        given, as Tracker.step defines it for that frame's stream; (sid, fid, pose7) is what __call__ returns"""
+        sid, fid, pose7, now7 = self._run(frames, vo_poses, streams, True)
+        return now7, sid, fid, pose7
+
+    @torch.no_grad()
+    def flush(self, s):
+        """-> (first, pose7 [n,7]): stream s's last n = min(lag, seen[s]) frames, their windows clipped at its last
+        frame.  Synchronises, starts a new sequence on stream s alone, and raises np.linalg.LinAlgError if a window of
+        stream s's sequence that ended was not positive definite."""
+        self._check_open()
+        s = _int_arg(s, "stream", 0, self.n_streams - 1)
+        pr = self.loc.predictor
+        first = _first_pending(int(self.seen[s]), self.lag)
+        n, failed = int(self.seen[s]) - first, ctypes.c_int(0)
+        with torch.cuda.device(pr.device):
+            out = torch.empty((max(self.lag, 1), 7), dtype=torch.float64, device=pr.device)
+            if self.h:
+                L = _lib.lib()
+                _lib.check(L.mapnet_track_multi_flush(self.h, s, out.data_ptr(), _lib.stream_ptr()),
+                           "mapnet_track_multi_flush")
+                _lib.check(L.mapnet_track_multi_status(self.h, s, None, ctypes.byref(failed), _lib.stream_ptr()),
+                           "mapnet_track_multi_status")
+        self.reset(s)
+        if failed.value:
+            raise np.linalg.LinAlgError("pose graph: the normal matrix of a window of stream %d's sequence is not "
+                                        "positive definite" % s)
+        return first, out[:n]
+
+    def reset(self, s=None):
+        """Start a new sequence on stream s, or on every stream when s is None (stream-ordered)."""
+        self._check_open()
+        s = -1 if s is None else _int_arg(s, "stream", 0, self.n_streams - 1)
+        if self.h:
+            with torch.cuda.device(self.loc.predictor.device):
+                _lib.check(_lib.lib().mapnet_track_multi_reset(self.h, s, _lib.stream_ptr()), "mapnet_track_multi_reset")
+        if s < 0:
+            self.seen[:] = 0
+        else:
+            self.seen[s] = 0
 
 
 def pgo(pred7, vos7, sax=1.0, saq=1.0, srx=1.0, srq=1.0, fc_vos=False):

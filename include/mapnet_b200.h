@@ -263,6 +263,43 @@ int mapnet_track_reset(mapnet_track_t* h, void* stream);
 int mapnet_track_status(mapnet_track_t* h, int64_t* frames_seen, int* failed, void* stream);
 int mapnet_track_destroy(mapnet_track_t* h);
 
+/* ---- multi-stream tracker (csrc/loader.cu; geomapnet_b200.inference.MultiTracker): n_streams independent sequences,
+ * each tracked exactly as a mapnet_track_t of the same arguments would track it, with one set of launches per call for
+ * all of them.  Stream s's poses are bit for bit those of a single-stream handle fed stream s's frames in order.
+ *   mapnet_track_multi_create: 1 <= n_streams <= MAPNET_TRACK_MAX_STREAMS plus mapnet_track_create's arguments, with
+ *     its checks.  Per stream a frame count, a status word and rings of R = max_batch + (T-1)*skip poses (float64
+ *     pose7) and VO poses (float32); the error of a failed allocation states its total bytes.
+ *   mapnet_track_multi_step: B frames of any streams (1 <= B <= max_batch, so a stream gets at most max_batch frames
+ *     per call): pred6 [B][6], vo6 [B][6] as mapnet_track_step takes them, and rec [B][6] int32, one record per frame
+ *     in call order, built by the caller from its own per-stream counts (inference._stream_records):
+ *       rec[b] = (stream, rank, count, frame, row, win): the frame's stream; its rank among that stream's frames in
+ *       this call (0, 1, ...); that stream's number of frames in this call; its absolute frame index in the stream
+ *       (seen + rank, < 2^31); the out7 row of the window this frame completes (frame - lag's, when frame >= lag) or
+ *       -1; and, per row b rather than per frame, the record whose completed window is out7 row b, or -1 for every
+ *       b >= the call's number of rows (rows are numbered in call order).
+ *     out7 [n][7] (room for B rows) gets each completed window's middle slot; with now7 (may be NULL) [B][7] also
+ *     gets, in row b, the zero-lag pose of frame b as mapnet_track_step_now defines it for that frame's stream.  Three
+ *     launches (gather, k_pgo, emit), graph-capturable, nothing read back: rec is device memory, so a captured graph
+ *     reads the records copied into it before each replay.  A record whose stream is outside [0, n_streams) is skipped.
+ *   mapnet_track_multi_flush: mapnet_track_flush of stream s alone (0 <= s < n_streams): its last min(lag, seen)
+ *     windows, clipped at its last frame, into out7 (room for lag rows).  Three launches (none when lag = 0).
+ *   mapnet_track_multi_reset: stream-ordered: stream s (or every stream when s = -1) starts a new sequence at frame 0
+ *     and its status word is cleared.
+ *   mapnet_track_multi_status: synchronises the stream and returns stream s's frames seen and status (1: a window of s
+ *     had a normal matrix that was not positive definite; k_pgo flags windows one by one, so other streams are not
+ *     marked).
+ * Pointers are device memory unless marked HOST.  Argument errors return non-zero before any launch. */
+#define MAPNET_TRACK_MAX_STREAMS 65536
+typedef struct mapnet_track_multi mapnet_track_multi_t;
+int mapnet_track_multi_create(mapnet_track_multi_t** out, int n_streams, int T, int skip, int fc_vos, int max_batch,
+                              const double* sigmas4, const double* pose_m3, const double* pose_s3);
+int mapnet_track_multi_step(mapnet_track_multi_t* h, const float* pred6, const float* vo6, const int32_t* rec, int B,
+                            double* out7, double* now7, void* stream);
+int mapnet_track_multi_flush(mapnet_track_multi_t* h, int s, double* out7, void* stream);
+int mapnet_track_multi_reset(mapnet_track_multi_t* h, int s, void* stream);
+int mapnet_track_multi_status(mapnet_track_multi_t* h, int s, int64_t* frames_seen, int* failed, void* stream);
+int mapnet_track_multi_destroy(mapnet_track_multi_t* h);
+
 /* ---- eval-mode inference engine (csrc/infer.cu): a frozen snapshot of a PoseNet / MapNet trunk for
  * scripts/eval.py-style prediction.  mapnet_infer_load copies the weights (packed fprop operands only), the eval-mode
  * BatchNorm scale / shift (computed from the running statistics exactly as mapnet_forward(training = 0) does) and the
