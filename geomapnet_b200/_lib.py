@@ -23,6 +23,10 @@ MAX_TRACK_STEPS = 16    # mapnet_track_create: windows of at most 16 frames (the
 TRACK_MULTI_API = ["mapnet_track_multi_create", "mapnet_track_multi_step", "mapnet_track_multi_flush",
                    "mapnet_track_multi_reset", "mapnet_track_multi_status", "mapnet_track_multi_destroy"]
 MAX_TRACK_STREAMS = 65536   # mapnet_track_multi_create: MAPNET_TRACK_MAX_STREAMS
+TRACK_SAMPLE_API = ["mapnet_track_sample_create", "mapnet_track_sample_step", "mapnet_track_sample_step_now",
+                    "mapnet_track_sample_flush", "mapnet_track_sample_reset", "mapnet_track_sample_status",
+                    "mapnet_track_sample_destroy"]
+TRACK_SAMPLE_ROW = 45       # mapnet_track_sample_step: pose7 [7], cov [36], t_std, q_std_deg per output row
 
 _lib = None
 
@@ -170,6 +174,22 @@ def lib():
     L.mapnet_track_multi_destroy.argtypes = [c_void_p]
     for name in TRACK_MULTI_API:
         getattr(L, name).restype = c_int
+    L.mapnet_pgo_optimize_cov.argtypes = [c_void_p] * 5 + [c_int, c_int, c_int, ctypes.c_double, ctypes.c_double, c_int,
+                                                           c_void_p, c_void_p]
+    L.mapnet_pgo_optimize_cov.restype = c_int
+    L.mapnet_track_sample_create.argtypes = [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]
+    L.mapnet_track_sample_step.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]
+    L.mapnet_track_sample_step_now.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
+                                               c_void_p]
+    L.mapnet_track_sample_flush.argtypes = [c_void_p, c_void_p, c_void_p]
+    L.mapnet_track_sample_reset.argtypes = [c_void_p, c_void_p]
+    L.mapnet_track_sample_status.argtypes = [c_void_p, POINTER(c_int64), POINTER(c_int), c_void_p]
+    L.mapnet_track_sample_destroy.argtypes = [c_void_p]
+    for name in TRACK_SAMPLE_API:
+        getattr(L, name).restype = c_int
+    L.mapnet_test_sample_factor.argtypes = [c_void_p, c_void_p, c_int64, ctypes.c_double, ctypes.c_double, c_void_p,
+                                            c_void_p, c_void_p]
+    L.mapnet_test_sample_factor.restype = c_int
     L.mapnet_test_stem_operand.argtypes = [c_int, c_void_p, c_void_p, c_void_p, c_int, POINTER(c_float), POINTER(c_float),
                                            c_void_p, c_void_p]
     L.mapnet_test_stem_operand.restype = c_int
@@ -209,7 +229,8 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_trunk_set_trainable", "mapnet_test_conv_ex", "mapnet_eval_windows",
             "mapnet_batch_losses", "mapnet_infer_forward_frames", "mapnet_test_stem_operand", "mapnet_infer_sample",
             "mapnet_infer_sample_frames", "mapnet_sample_post", "mapnet_test_small_gemm_plan", "mapnet_test_stem_ex",
-            "mapnet_test_head"] + TRACK_API + TRACK_MULTI_API
+            "mapnet_test_head", "mapnet_pgo_optimize_cov",
+            "mapnet_test_sample_factor"] + TRACK_API + TRACK_MULTI_API + TRACK_SAMPLE_API
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 MAX_SAMPLE_DRAWS = 1024      # mapnet_infer_sample: S in [2, MAX_SAMPLE_DRAWS] dropout draws per frame
 

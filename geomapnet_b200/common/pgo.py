@@ -12,7 +12,7 @@ import torch
 
 from .. import _lib
 
-__all__ = ["optimize_poses", "optimize_pose_windows", "vos_from_target_poses"]
+__all__ = ["optimize_poses", "optimize_pose_windows", "optimize_pose_windows_cov", "vos_from_target_poses"]
 
 
 def _qmult(a, b):
@@ -62,6 +62,39 @@ def optimize_pose_windows(pred_poses, vos, fc_vos=False, sax=1.0, saq=1.0, srx=1
     if int(status.item()) != 0:
         raise np.linalg.LinAlgError("pose graph: normal matrix of a window is not positive definite")
     return out
+
+
+def optimize_pose_windows_cov(pred_poses, abs_cov7, vos, fc_vos=False, srx=1.0, srq=1.0, n_iters=10):
+    """Covariance-weighted pose graph (csrc/pgo.cu, k_pgo_cov): pred_poses [W,N,7] (translation + quaternion wxyz),
+    abs_cov7 [W,N,7,7] the covariance S7 of each absolute pose, vos as for optimize_pose_windows.  Slot k's absolute
+    factor has residual C^-1 (z_k - p_k) with S7 = C C' (lower Cholesky factor); the relative factors (srx, srq), state
+    and manifold update are optimize_pose_windows'; every iteration takes the exact Gauss-Newton step.  Returns
+    (poses [W,N,7], cov [W,N,6,6]) float64 on the device: cov is each slot's posterior covariance, the 6 x 6 diagonal
+    block of the inverse normal matrix at the returned state, in (t, log q) coordinates.  Raises
+    np.linalg.LinAlgError if a window's normal matrix (or one of its S7) is not positive definite."""
+    device = pred_poses.device if torch.is_tensor(pred_poses) and pred_poses.is_cuda else torch.device("cuda")
+    p = torch.as_tensor(pred_poses, dtype=torch.float64).to(device).contiguous()
+    c = torch.as_tensor(abs_cov7, dtype=torch.float64).to(device).contiguous()
+    v = torch.as_tensor(vos, dtype=torch.float64).to(device).contiguous()
+    if p.dim() != 3 or p.shape[2] != 7:
+        raise ValueError("pred_poses must be [W,N,7], got %s" % (tuple(p.shape),))
+    W, N, _ = p.shape
+    E = N * (N - 1) // 2 if fc_vos else N - 1
+    if tuple(c.shape) != (W, N, 7, 7):
+        raise ValueError("abs_cov7 must be [%d,%d,7,7], got %s" % (W, N, tuple(c.shape)))
+    if tuple(v.shape) != (W, E, 7):
+        raise ValueError("vos must be [%d,%d,7], got %s" % (W, E, tuple(v.shape)))
+    out = torch.empty_like(p)
+    cov = torch.empty((W, N, 6, 6), dtype=torch.float64, device=device)
+    status = torch.zeros(1, dtype=torch.int32, device=device)
+    with torch.cuda.device(device):
+        _lib.check(_lib.lib().mapnet_pgo_optimize_cov(p.data_ptr(), c.data_ptr(), v.data_ptr(), out.data_ptr(),
+                                                      cov.data_ptr(), W, N, 1 if fc_vos else 0, float(srx), float(srq),
+                                                      int(n_iters), status.data_ptr(), _lib.stream_ptr()),
+                   "mapnet_pgo_optimize_cov")
+    if int(status.item()) != 0:
+        raise np.linalg.LinAlgError("pose graph: normal matrix of a window is not positive definite")
+    return out, cov
 
 
 def optimize_poses(pred_poses, vos=None, fc_vos=False, target_poses=None, sax=1, saq=1, srx=1, srq=1):

@@ -258,6 +258,13 @@ int pgo_prepare();
 void pgo_weights(double sax, double saq, double srx, double srq, double w4[4]);
 int launch_pgo(const double* poses, const double* vos, double* out, int n_windows, int N, int fc, const double w4[4],
                int n_iters, int exact, int* status, const int* n_win_dev, cudaStream_t st, int* win_fail = nullptr);
+// k_pgo_cov: sig7 [n_windows][N][7][7] covariances of the absolute factors, relative weights w_rx = 1/sqrt(srx) and
+// w_rq = 1/sqrt(srq), the exact Gauss-Newton step; out [n_windows][N][7] and the posterior cov [n_windows][N][6][6]
+// in (t, log q).  n_win_dev, win_fail, status as launch_pgo's.  pgo_cov_prepare sets its shared-memory limit once.
+int pgo_cov_prepare();
+int launch_pgo_cov(const double* poses, const double* sig7, const double* vos, double* out, double* cov, int n_windows,
+                   int N, int fc, double w_rx, double w_rq, int n_iters, int* status, const int* n_win_dev,
+                   int* win_fail, cudaStream_t st);
 
 // input pipeline internals shared by preprocess.cu and the frame cache (loader.cu)
 struct JitterParams;

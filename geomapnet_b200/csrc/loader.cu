@@ -204,6 +204,150 @@ k_track_emit(const double* __restrict__ opt7, TrackDev* __restrict__ st, int n, 
   if (w >= lead) track_emit_pose(win + 7 * (T / 2), un, ms, ss, out7 + 7LL * (w - lead));
 }
 
+// ---- Monte-Carlo tracker (mapnet_track_sample_*, inference.SampledTracker): mapnet_track_*'s windows, with each
+// frame's S-draw mean (t, log q) and covariance Sigma [6][6] (float64, mapnet_infer_sample_frames' outputs) in place of
+// its one draw.  A new frame's absolute pose p = (mean_t, qexp(mean_v)) (k_sample_post's qexp) and its factor covariance
+// S7 = A Sigma A' + diag(sax I3, saq I4), A = blockdiag(I3, E(mean_v)), are formed once, into rings of R frames; the
+// windows gather them, k_pgo_cov solves them, and the emit writes per window row pose7 [7], cov [36] = D cov D,
+// t_std, q_std_deg (k_sample_post's statistics), kTrackSampleRow doubles.
+static constexpr int kTrackSampleRow = 45;
+
+// E(v) = d qexp(v) / dv (4 x 3): row 0 -sinc(n) v', rows 1..3 sinc(n) I + g(n) v v', g = (n cos n - sin n) / n^3
+// (its series below n = 0.1, where the difference cancels), sinc(n) = sin n / n
+__device__ __forceinline__ void qexp_jac(const double v[3], double Ej[4][3]) {
+  const double n2 = v[0] * v[0] + v[1] * v[1] + v[2] * v[2], n = sqrt(n2);
+  const double sc = n > 0.0 ? sin(n) / n : 1.0;
+  const double g = n < 0.1 ? -1.0 / 3.0 + n2 * (1.0 / 30.0 + n2 * (-1.0 / 840.0 + n2 * (1.0 / 45360.0 -
+                                                                                      n2 / 3991680.0)))
+                           : (n * cos(n) - sin(n)) / (n2 * n);
+  for (int b = 0; b < 3; ++b) {
+    Ej[0][b] = -sc * v[b];
+    for (int a = 0; a < 3; ++a) Ej[1 + a][b] = (a == b ? sc : 0.0) + g * v[a] * v[b];
+  }
+}
+
+// one frame's absolute pose p7 and factor covariance S7 [7][7] from its draws' mean [6] and covariance [36]
+__device__ __forceinline__ void sample_factor(const double* mu, const double* C, double sax, double saq, double p7[7],
+                                              double S7[49]) {
+  p7[0] = mu[0]; p7[1] = mu[1]; p7[2] = mu[2];
+  sample_qexp(mu[3], mu[4], mu[5], p7 + 3);
+  double Ej[4][3];
+  qexp_jac(mu + 3, Ej);
+  double A[7][6] = {};
+  for (int a = 0; a < 3; ++a) A[a][a] = 1.0;
+  for (int a = 0; a < 4; ++a)
+    for (int b = 0; b < 3; ++b) A[3 + a][3 + b] = Ej[a][b];
+  for (int r = 0; r < 7; ++r)
+    for (int c = 0; c < 7; ++c) {
+      double v = 0.0;
+      for (int k = 0; k < 6; ++k) {
+        double ac = 0.0;
+        for (int l = 0; l < 6; ++l) ac += C[6 * k + l] * A[c][l];
+        v += A[r][k] * ac;
+      }
+      S7[7 * r + c] = v + (r == c ? (r < 3 ? sax : saq) : 0.0);
+    }
+}
+
+// mapnet_test_sample_factor: sample_factor of n frames, the tracker's own arithmetic, for tests that compose its windows
+__global__ void __launch_bounds__(128)
+k_test_sample_factor(const double* __restrict__ mean, const double* __restrict__ cov, long long n, double sax,
+                     double saq, double* __restrict__ p7, double* __restrict__ s7) {
+  pdl_prologue();
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) sample_factor(mean + 6 * i, cov + 36 * i, sax, saq, p7 + 7 * i, s7 + 49 * i);
+}
+
+// k_track_gather for the sampled tracker: rows 0 .. n-1 form the n new frames' p7 / S7 into the rings and into every
+// window slot of this call that holds them (each formed once); then slot (w, k) of window w < n_win for the frames
+// before this call, from the rings; then VO (w, e), as k_track_gather computes it.
+__global__ void __launch_bounds__(128)
+k_track_sample_gather(const double* __restrict__ mean, const double* __restrict__ cov, const float* __restrict__ vo6,
+                      int n, int flush, int now, TrackDev* __restrict__ st, double* __restrict__ ring7,
+                      double* __restrict__ ring49, float* __restrict__ ring_vo, long long R, int T, int skip, int fc,
+                      int max_win, double sax, double saq, double* __restrict__ win7, double* __restrict__ win49,
+                      double* __restrict__ vos7) {
+  pdl_prologue();
+  const long long seen = st->seen, total = seen + n, lag = trackcore::lag(T, skip);
+  const long long pending = trackcore::first_pending(seen, lag);
+  const int n_done = (int)((flush ? total : trackcore::first_pending(total, lag)) - pending);
+  const long long first = now ? trackcore::now_first(seen, lag) : pending;
+  const int n_win = now ? n : n_done;
+  const int E = fc ? T * (T - 1) / 2 : T - 1;
+  long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r == 0) st->n_win = n_done;
+  if (r < n) {
+    const long long f = seen + r, q = f % R;
+    double p7[7], S7[49];
+    sample_factor(mean + 6 * r, cov + 36 * r, sax, saq, p7, S7);
+    for (int c = 0; c < 7; ++c) ring7[7 * q + c] = p7[c];
+    for (int c = 0; c < 49; ++c) ring49[49 * q + c] = S7[c];
+#pragma unroll
+    for (int c = 0; c < 6; ++c) ring_vo[6 * q + c] = vo6[6 * r + c];
+    for (int w = 0; w < n_win; ++w)
+      for (int k = 0; k < T; ++k) {
+        if (trackcore::slot_frame(first + w, k, T, skip, total - 1) != f) continue;
+        const long long s = (long long)w * T + k;
+        for (int c = 0; c < 7; ++c) win7[7 * s + c] = p7[c];
+        for (int c = 0; c < 49; ++c) win49[49 * s + c] = S7[c];
+      }
+    return;
+  }
+  r -= n;
+  if (r < (long long)max_win * T) {
+    const int w = (int)(r / T), k = (int)(r % T);
+    if (w >= n_win) return;
+    const long long f = trackcore::slot_frame(first + w, k, T, skip, total - 1);
+    if (f >= seen) return;                 // a new frame: written by its own row
+    const long long q = f % R;
+    for (int c = 0; c < 7; ++c) win7[7 * r + c] = ring7[7 * q + c];
+    for (int c = 0; c < 49; ++c) win49[49 * r + c] = ring49[49 * q + c];
+    return;
+  }
+  r -= (long long)max_win * T;
+  if (r < (long long)max_win * E) {
+    const int w = (int)(r / E), e = (int)(r % E);
+    if (w >= n_win) return;
+    int i, j;
+    trackcore::vo_pair(e, T, fc, &i, &j);
+    const long long fa = trackcore::slot_frame(first + w, i, T, skip, total - 1);
+    const long long fb = trackcore::slot_frame(first + w, j, T, skip, total - 1);
+    const posemath::Pose6 v = posemath::calc_vo_logq_safe(ld_pose6(track_src(vo6, ring_vo, fa, seen, R)),
+                                                          ld_pose6(track_src(vo6, ring_vo, fb, seen, R)));
+    const float v6[6] = {v.t.x, v.t.y, v.t.z, v.l.x, v.l.y, v.l.z};
+    st_pose7(v6, vos7 + 7 * r);
+  }
+}
+
+__device__ __forceinline__ void track_sample_row(const double* p7, const double* C, int un, const double ms[3],
+                                                 const double ss[3], double* o) {
+  track_emit_pose(p7, un, ms, ss, o);
+  const double d[6] = {ss[0], ss[1], ss[2], 1.0, 1.0, 1.0};
+  sample_stats(C, d, o + 7, o + 43, o + 44);
+}
+
+// k_track_emit for the sampled tracker: window w's middle slot into out row w (a zero-lag call: its last slot into now
+// row w, and the completed window n - n_win + j into out row j); thread 0 advances the frame counter
+__global__ void __launch_bounds__(128)
+k_track_sample_emit(const double* __restrict__ opt7, const double* __restrict__ cov36, TrackDev* __restrict__ st, int n,
+                    int T, int un, double m0, double m1, double m2, double s0, double s1, double s2,
+                    double* __restrict__ out, double* __restrict__ now) {
+  pdl_prologue();
+  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+  const int n_win = st->n_win;
+  if (w == 0) st->seen += n;
+  const double ms[3] = {m0, m1, m2}, ss[3] = {s0, s1, s2};
+  const long long mid = (long long)w * T + T / 2, last = (long long)w * T + T - 1;
+  if (now == nullptr) {
+    if (w < n_win) track_sample_row(opt7 + 7 * mid, cov36 + 36 * mid, un, ms, ss, out + kTrackSampleRow * (long long)w);
+    return;
+  }
+  if (w >= n) return;
+  track_sample_row(opt7 + 7 * last, cov36 + 36 * last, un, ms, ss, now + kTrackSampleRow * (long long)w);
+  const int lead = n - n_win;
+  if (w >= lead) track_sample_row(opt7 + 7 * mid, cov36 + 36 * mid, un, ms, ss, out + kTrackSampleRow * (long long)(w - lead));
+}
+
 // ---- multi-stream tracker (mapnet_track_multi_*, inference.MultiTracker): the same windows for n_streams independent
 // sequences, one set of launches per call.  Per stream: its frames so far and its status word; the rings are
 // [n_streams][R].  The host keeps count of every stream and builds one record per frame of a call, so the kernels
@@ -652,6 +796,126 @@ int mapnet_track_status(mapnet_track_t* h, int64_t* frames_seen, int* failed, vo
 int mapnet_track_destroy(mapnet_track_t* h) {
   if (h == nullptr) return 0;
   cudaFree(h->st); cudaFree(h->ring7); cudaFree(h->ring_vo); cudaFree(h->win7); cudaFree(h->vos7); cudaFree(h->opt7);
+  delete h;
+  return 0;
+}
+
+}  // extern "C"
+
+struct mapnet_track_sample : TrackCfg {
+  TrackDev* st;
+  double sax, saq;                          // the floors of the absolute factors' covariances
+  double *ring7, *ring49;                   // [R][7], [R][7][7]: p and S7 of the last R frames
+  float* ring_vo;                           // [R][6]
+  double *win7, *win49, *vos7, *opt7, *cov36;   // [max_win][T][7], [.][T][49], [.][E][7], [.][T][7], [.][T][36]
+};
+
+// the three launches of a sampled call: n new frames (a step) or none (flush); out [max_win][45], now [n][45] or null
+static int track_sample_launch(mapnet_track_sample_t* h, const double* mean, const double* cov, const float* vo6, int n,
+                               int flush, double* out, double* now, cudaStream_t st) {
+  const int nw = flush ? (int)(h->lag < h->max_win ? h->lag : h->max_win) : n;
+  const long long rows = n + (long long)nw * (h->T + h->E);
+  MN_LAUNCH(k_track_sample_gather, cdiv(rows, 128), 128, 0, st, mean, cov, vo6, n, flush, now != nullptr ? 1 : 0, h->st,
+            h->ring7, h->ring49, h->ring_vo, h->R, h->T, h->skip, h->fc, nw, h->sax, h->saq, h->win7, h->win49,
+            h->vos7);
+  MN_LAUNCH_CHECK();
+  MN_TRY(launch_pgo_cov(h->win7, h->win49, h->vos7, h->opt7, h->cov36, nw, h->T, h->fc, h->w4[2], h->w4[3], 10,
+                        &h->st->status, now != nullptr ? nullptr : &h->st->n_win, nullptr, st));
+  MN_LAUNCH(k_track_sample_emit, cdiv(nw, 128), 128, 0, st, (const double*)h->opt7, (const double*)h->cov36, h->st, n,
+            h->T, h->un, h->m[0], h->m[1], h->m[2], h->s[0], h->s[1], h->s[2], out, now);
+  MN_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" {
+
+int mapnet_track_sample_create(mapnet_track_sample_t** out, int T, int skip, int fc_vos, int max_batch,
+                               const double* sigmas4, const double* pose_m3, const double* pose_s3) {
+  MN_CHECK(out != nullptr && sigmas4 != nullptr, "track_sample_create: null argument");
+  *out = nullptr;
+  TrackCfg c;
+  MN_TRY(track_config(&c, "track_sample_create", T, skip, fc_vos, max_batch, sigmas4, pose_m3, pose_s3));
+  MN_TRY(pgo_cov_prepare());
+  const size_t R = (size_t)c.R, W = (size_t)c.max_win, WT = W * T;
+  mapnet_track_sample* h = new mapnet_track_sample();
+  static_cast<TrackCfg&>(*h) = c;
+  h->sax = sigmas4[0]; h->saq = sigmas4[1];
+  bool ok = cudaMalloc((void**)&h->st, sizeof(TrackDev)) == cudaSuccess &&
+            cudaMalloc((void**)&h->ring7, R * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->ring49, R * 49 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->ring_vo, R * 6 * sizeof(float)) == cudaSuccess &&
+            cudaMalloc((void**)&h->win7, WT * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->win49, WT * 49 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->vos7, W * c.E * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->opt7, WT * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->cov36, WT * 36 * sizeof(double)) == cudaSuccess &&
+            cudaMemset(h->st, 0, sizeof(TrackDev)) == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess;
+  if (!ok) {
+    cudaGetLastError();
+    set_last_error("track_sample_create: device allocation of a ring of %lld frames and %d windows failed", c.R,
+                   c.max_win);
+    mapnet_track_sample_destroy(h);
+    return 1;
+  }
+  *out = h;
+  return 0;
+}
+
+int mapnet_track_sample_step(mapnet_track_sample_t* h, const double* mean6, const double* cov36, const float* vo6, int B,
+                             double* out, void* stream) {
+  MN_CHECK(h != nullptr, "track_sample_step: null handle");
+  MN_CHECK(mean6 != nullptr && cov36 != nullptr && vo6 != nullptr && out != nullptr, "track_sample_step: null argument");
+  MN_CHECK(B >= 1 && B <= h->max_batch, "track_sample_step: %d frames outside [1, max_batch=%d]", B, h->max_batch);
+  return track_sample_launch(h, mean6, cov36, vo6, B, 0, out, nullptr, (cudaStream_t)stream);
+}
+
+int mapnet_track_sample_step_now(mapnet_track_sample_t* h, const double* mean6, const double* cov36, const float* vo6,
+                                 int B, double* out, double* now, void* stream) {
+  MN_CHECK(h != nullptr, "track_sample_step_now: null handle");
+  MN_CHECK(mean6 != nullptr && cov36 != nullptr && vo6 != nullptr && out != nullptr && now != nullptr,
+           "track_sample_step_now: null argument");
+  MN_CHECK(B >= 1 && B <= h->max_batch, "track_sample_step_now: %d frames outside [1, max_batch=%d]", B, h->max_batch);
+  return track_sample_launch(h, mean6, cov36, vo6, B, 0, out, now, (cudaStream_t)stream);
+}
+
+int mapnet_track_sample_flush(mapnet_track_sample_t* h, double* out, void* stream) {
+  MN_CHECK(h != nullptr, "track_sample_flush: null handle");
+  MN_CHECK(out != nullptr, "track_sample_flush: null argument");
+  if (h->lag == 0) return 0;
+  return track_sample_launch(h, nullptr, nullptr, nullptr, 0, 1, out, nullptr, (cudaStream_t)stream);
+}
+
+int mapnet_track_sample_reset(mapnet_track_sample_t* h, void* stream) {
+  MN_CHECK(h != nullptr, "track_sample_reset: null handle");
+  MN_CUDA(cudaMemsetAsync(h->st, 0, sizeof(TrackDev), (cudaStream_t)stream));
+  return 0;
+}
+
+int mapnet_track_sample_status(mapnet_track_sample_t* h, int64_t* frames_seen, int* failed, void* stream) {
+  MN_CHECK(h != nullptr, "track_sample_status: null handle");
+  TrackDev d;
+  MN_CUDA(cudaMemcpyAsync(&d, h->st, sizeof(TrackDev), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  MN_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+  if (frames_seen != nullptr) *frames_seen = d.seen;
+  if (failed != nullptr) *failed = d.status;
+  return 0;
+}
+
+int mapnet_test_sample_factor(const double* mean6, const double* cov36, int64_t n, double sax, double saq, double* p7,
+                              double* s7, void* stream) {
+  MN_CHECK(mean6 != nullptr && cov36 != nullptr && p7 != nullptr && s7 != nullptr && n >= 1,
+           "test_sample_factor: bad argument");
+  MN_CHECK(sax > 0 && saq > 0, "test_sample_factor: sax = %g and saq = %g must be positive", sax, saq);
+  MN_LAUNCH(k_test_sample_factor, cdiv(n, 128), 128, 0, (cudaStream_t)stream, mean6, cov36, (long long)n, sax, saq, p7,
+            s7);
+  MN_LAUNCH_CHECK();
+  return 0;
+}
+
+int mapnet_track_sample_destroy(mapnet_track_sample_t* h) {
+  if (h == nullptr) return 0;
+  cudaFree(h->st); cudaFree(h->ring7); cudaFree(h->ring49); cudaFree(h->ring_vo); cudaFree(h->win7);
+  cudaFree(h->win49); cudaFree(h->vos7); cudaFree(h->opt7); cudaFree(h->cov36);
   delete h;
   return 0;
 }

@@ -26,6 +26,7 @@
 
 #include "kernels.h"
 #include "pose_post.cuh"
+#include "track_core.h"
 #include "../../include/mapnet_b200.h"
 
 namespace mapnet {
@@ -268,6 +269,381 @@ void pgo_weights(double sax, double saq, double srx, double srq, double w4[4]) {
   w4[0] = 1.0 / sqrt(sax); w4[1] = 1.0 / sqrt(saq); w4[2] = 1.0 / sqrt(srx); w4[3] = 1.0 / sqrt(srq);
 }
 
+// ---- covariance-weighted pose graph (mapnet_pgo_optimize_cov, inference.SampledTracker).  k_pgo's state, relative
+// factors and manifold update, with a full 7 x 7 covariance S7 = C C' per absolute factor (residual C^-1 (z - p),
+// Jacobian C^-1 blockdiag(I, m_rot(q))), the exact Gauss-Newton step, and the posterior covariance of every slot:
+// the 6 x 6 diagonal blocks of H^-1 at the returned state, mapped from (dt, x) to (t, log q).
+//
+// Deterministic: every factor first writes its Jacobian products into its own shared-memory record, then one thread
+// per H / b entry adds the records that touch it in a fixed order (no atomics).  The Cholesky and the inverse
+// R^-1 are right-looking over the block; the two triangular solves run in warp 0 with three rows per lane in
+// registers (D <= 96), so they need shuffles instead of block barriers.
+static constexpr int kUnaryRec = 42;      // per slot: JtJ [6][6], Jtr [6]
+static constexpr int kEdgeRec = 45;       // per edge: Tt [3][3], gt [3], Haa, Hbb, Hab [3][3], ga [3], gb [3]
+
+// index of the relative factor between slots i < j, -1 when there is none (the order of trackcore::vo_pair)
+__device__ __forceinline__ int pgo_edge(int i, int j, int N, int fc) {
+  if (!fc) return j == i + 1 ? i : -1;
+  return i * (N - 1) - i * (i - 1) / 2 + (j - i - 1);
+}
+
+// G(q) = d qlog(q * dq(x)) / dx at x = 0 = Jlog(q) m_rot(q), qlog(w, u) = atan2(|u|, w) u / |u|
+__device__ __forceinline__ void qlog_jac(const Q4& q, double G[3][3]) {
+  const double u[3] = {q.x, q.y, q.z};
+  const double s2 = u[0] * u[0] + u[1] * u[1] + u[2] * u[2], s = sqrt(s2), n2 = q.w * q.w + s2;
+  double f, c;                            // d qlog / du = f I + c u u',  d qlog / dw = -u / n2
+  const double t = s / q.w;
+  if (q.w > 0.0 && t < 1e-2) {            // series in t = |u| / w: atan(t) / t and (w / n2 - f) / s2
+    const double t2 = t * t;
+    f = (1.0 + t2 * (-1.0 / 3.0 + t2 * (1.0 / 5.0 + t2 * (-1.0 / 7.0 + t2 / 9.0)))) / q.w;
+    c = (-2.0 / 3.0 + t2 * (4.0 / 5.0 + t2 * (-6.0 / 7.0 + t2 * (8.0 / 9.0)))) / (q.w * q.w * q.w);
+  } else {
+    f = atan2(s, q.w) / s;
+    c = (q.w / n2 - f) / s2;
+  }
+  double J[3][4];
+  for (int a = 0; a < 3; ++a) {
+    J[a][0] = -u[a] / n2;
+    for (int b = 0; b < 3; ++b) J[a][1 + b] = (a == b ? f : 0.0) + c * u[a] * u[b];
+  }
+  double M[4][3];
+  m_rot(q, M);
+  for (int a = 0; a < 3; ++a)
+    for (int b = 0; b < 3; ++b) {
+      double v = 0.0;
+      for (int k = 0; k < 4; ++k) v += J[a][k] * M[k][b];
+      G[a][b] = v;
+    }
+}
+
+// H (D x D) and b at state z: each factor's record, then one thread per entry sums the records touching it
+__device__ void pgo_cov_normal(const double* z, const double* P, const double* Li, const double* V, int N, int fc,
+                               int E, double w_rx, double w_rq, double* rec, double* H, double* bv) {
+  const int D = 6 * N;
+  double* ru = rec;                       // [N][kUnaryRec]
+  double* re = rec + N * kUnaryRec;       // [E][kEdgeRec]
+  for (int c = threadIdx.x; c < N + E; c += blockDim.x) {
+    if (c < N) {
+      const int i = c;
+      const Q4 q = {z[7 * i + 3], z[7 * i + 4], z[7 * i + 5], z[7 * i + 6]};
+      double M[4][3], d[7], r[7], J[7][6];
+      m_rot(q, M);
+      for (int a = 0; a < 7; ++a) d[a] = z[7 * i + a] - P[7 * i + a];
+      const double* L = Li + 49 * i;      // C^-1, lower triangular
+      for (int a = 0; a < 7; ++a) {
+        double v = 0.0;
+        for (int b = 0; b <= a; ++b) v += L[7 * a + b] * d[b];
+        r[a] = v;
+        for (int cc = 0; cc < 3; ++cc) J[a][cc] = a >= cc ? L[7 * a + cc] : 0.0;
+        for (int cc = 0; cc < 3; ++cc) {
+          double s = 0.0;
+          for (int b = 3; b <= a; ++b) s += L[7 * a + b] * M[b - 3][cc];
+          J[a][3 + cc] = s;
+        }
+      }
+      double* o = ru + kUnaryRec * i;
+      for (int a = 0; a < 6; ++a) {
+        for (int b = 0; b < 6; ++b) {
+          double s = 0.0;
+          for (int k = 0; k < 7; ++k) s += J[k][a] * J[k][b];
+          o[6 * a + b] = s;
+        }
+        double s = 0.0;
+        for (int k = 0; k < 7; ++k) s += J[k][a] * r[k];
+        o[36 + a] = s;
+      }
+    } else {
+      const int e = c - N;
+      int i, j;
+      trackcore::vo_pair(e, N, fc, &i, &j);
+      const Q4 qi = {z[7 * i + 3], z[7 * i + 4], z[7 * i + 5], z[7 * i + 6]};
+      const Q4 qj = {z[7 * j + 3], z[7 * j + 4], z[7 * j + 5], z[7 * j + 6]};
+      double* o = re + kEdgeRec * e;
+      double Dt[3][3], rt[3];
+      dqstq_t(qi, Dt);
+      const double dv[3] = {z[7 * j] - z[7 * i], z[7 * j + 1] - z[7 * i + 1], z[7 * j + 2] - z[7 * i + 2]};
+      q_rotate(dv, q_inv(qi), rt);
+      for (int a = 0; a < 3; ++a) {
+        rt[a] = w_rx * (rt[a] - V[7 * e + a]);
+        for (int b = 0; b < 3; ++b) Dt[a][b] *= w_rx;
+      }
+      for (int a = 0; a < 3; ++a) {
+        double g = 0.0;
+        for (int k = 0; k < 3; ++k) g += Dt[k][a] * rt[k];
+        o[9 + a] = g;
+        for (int b = 0; b < 3; ++b) {
+          double s = 0.0;
+          for (int k = 0; k < 3; ++k) s += Dt[k][a] * Dt[k][b];
+          o[3 * a + b] = s;
+        }
+      }
+      double A4[4][4], B4[4][4], Mi[4][3], Mj[4][3], Ja[4][3], Jb[4][3], rq[4];
+      dpsq_p(qj, A4); dpsq_q(qi, B4); m_rot(qi, Mi); m_rot(qj, Mj);
+      for (int a = 0; a < 4; ++a)
+        for (int b = 0; b < 3; ++b) {
+          double sa = 0.0, sb = 0.0;
+          for (int k = 0; k < 4; ++k) { sa += A4[a][k] * Mi[k][b]; sb += B4[a][k] * Mj[k][b]; }
+          Ja[a][b] = w_rq * sa; Jb[a][b] = w_rq * sb;
+        }
+      const Q4 qvo = q_mul(q_inv(qi), qj);
+      rq[0] = w_rq * (qvo.w - V[7 * e + 3]); rq[1] = w_rq * (qvo.x - V[7 * e + 4]);
+      rq[2] = w_rq * (qvo.y - V[7 * e + 5]); rq[3] = w_rq * (qvo.z - V[7 * e + 6]);
+      for (int a = 0; a < 3; ++a) {
+        double ga = 0.0, gb = 0.0;
+        for (int k = 0; k < 4; ++k) { ga += Ja[k][a] * rq[k]; gb += Jb[k][a] * rq[k]; }
+        o[39 + a] = ga; o[42 + a] = gb;
+        for (int b = 0; b < 3; ++b) {
+          double saa = 0.0, sbb = 0.0, sab = 0.0;
+          for (int k = 0; k < 4; ++k) { saa += Ja[k][a] * Ja[k][b]; sbb += Jb[k][a] * Jb[k][b]; sab += Ja[k][a] * Jb[k][b]; }
+          o[12 + 3 * a + b] = saa; o[21 + 3 * a + b] = sbb; o[30 + 3 * a + b] = sab;
+        }
+      }
+    }
+  }
+  __syncthreads();
+  for (int idx = threadIdx.x; idx < D * D + D; idx += blockDim.x) {
+    if (idx < D * D) {
+      const int row = idx / D, col = idx % D, i = row / 6, a = row % 6, j = col / 6, b = col % 6;
+      const bool tt = a < 3 && b < 3, qq = a >= 3 && b >= 3;
+      double v;
+      if (i == j) {
+        v = ru[kUnaryRec * i + 6 * a + b];
+        for (int m = 0; m < N; ++m) {
+          const int e = m == i ? -1 : pgo_edge(i < m ? i : m, i < m ? m : i, N, fc);
+          if (e < 0) continue;
+          const double* o = re + kEdgeRec * e;
+          if (tt) v += o[3 * a + b];
+          else if (qq) v += o[(i < m ? 12 : 21) + 3 * (a - 3) + (b - 3)];
+        }
+      } else {
+        const int e = pgo_edge(i < j ? i : j, i < j ? j : i, N, fc);
+        const double* o = re + kEdgeRec * (e < 0 ? 0 : e);
+        v = 0.0;
+        if (e >= 0 && tt) v = -o[3 * a + b];
+        else if (e >= 0 && qq) v = i < j ? o[30 + 3 * (a - 3) + (b - 3)] : o[30 + 3 * (b - 3) + (a - 3)];
+      }
+      H[idx] = v;
+    } else {
+      const int row = idx - D * D, i = row / 6, a = row % 6;
+      double v = ru[kUnaryRec * i + 36 + a];
+      for (int m = 0; m < N; ++m) {
+        const int e = m == i ? -1 : pgo_edge(i < m ? i : m, i < m ? m : i, N, fc);
+        if (e < 0) continue;
+        const double* o = re + kEdgeRec * e;
+        if (a < 3) v += i < m ? -o[9 + a] : o[9 + a];
+        else v += o[(i < m ? 39 : 42) + a - 3];
+      }
+      bv[row] = v;
+    }
+  }
+  __syncthreads();
+}
+
+// H = R' R in place (upper R, row-major), right-looking over the block, as k_pgo factors; a pivot <= 0 sets *fail
+__device__ void pgo_cov_cholesky(double* H, int D, int* fail) {
+  for (int k = 0; k < D; ++k) {
+    if (threadIdx.x == 0) {
+      const double d = H[k * D + k];
+      if (!(d > 0.0)) *fail = 1;
+      H[k * D + k] = sqrt(d > 0.0 ? d : 1.0);
+    }
+    __syncthreads();
+    const double rkk = H[k * D + k];
+    for (int j = k + 1 + threadIdx.x; j < D; j += blockDim.x) H[k * D + j] /= rkk;
+    __syncthreads();
+    for (int idx = threadIdx.x; idx < (D - k - 1) * (D - k - 1); idx += blockDim.x) {
+      const int i = k + 1 + idx / (D - k - 1), j = k + 1 + idx % (D - k - 1);
+      if (j >= i) H[i * D + j] -= H[k * D + i] * H[k * D + j];
+    }
+    __syncthreads();
+  }
+}
+
+// warp 0: xs = -(R'R)^-1 b, rows lane, lane + 32, lane + 64 in registers
+__device__ void pgo_cov_solve(const double* R, const double* bv, int D, double* xs) {
+  if (threadIdx.x >= 32) return;
+  const int lane = threadIdx.x;
+  double y[3];
+#pragma unroll
+  for (int s = 0; s < 3; ++s) y[s] = lane + 32 * s < D ? -bv[lane + 32 * s] : 0.0;
+  for (int k = 0; k < D; ++k) {             // R' y = -b
+    const int ks = k >> 5;
+    double yk = ks == 0 ? y[0] : (ks == 1 ? y[1] : y[2]);
+    yk = __shfl_sync(0xffffffffu, yk, k & 31) / R[k * D + k];
+#pragma unroll
+    for (int s = 0; s < 3; ++s) {
+      const int i = lane + 32 * s;
+      if (i == k) y[s] = yk;
+      else if (i > k && i < D) y[s] -= R[k * D + i] * yk;
+    }
+  }
+  for (int k = D - 1; k >= 0; --k) {        // R x = y
+    const int ks = k >> 5;
+    double xk = ks == 0 ? y[0] : (ks == 1 ? y[1] : y[2]);
+    xk = __shfl_sync(0xffffffffu, xk, k & 31) / R[k * D + k];
+#pragma unroll
+    for (int s = 0; s < 3; ++s) {
+      const int i = lane + 32 * s;
+      if (i == k) y[s] = xk;
+      else if (i < k) y[s] -= R[i * D + k] * xk;
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < 3; ++s)
+    if (lane + 32 * s < D) xs[lane + 32 * s] = y[s];
+}
+
+// One window per block (kPgoThreads threads).  poses [W][N][7] (the absolute poses p), sig7 [W][N][7][7] (their
+// covariances), vos [W][E][7] -> out [W][N][7], cov [W][N][6][6]; n_win_dev, win_fail and status as for k_pgo.
+__global__ void __launch_bounds__(kPgoThreads)
+k_pgo_cov(const double* __restrict__ poses, const double* __restrict__ sig7, const double* __restrict__ vos,
+          double* __restrict__ out, double* __restrict__ cov, int N, int fc, double w_rx, double w_rq, int n_iters,
+          int* __restrict__ status, const int* __restrict__ n_win_dev, int* __restrict__ win_fail) {
+  pdl_prologue();
+  if (n_win_dev != nullptr && (int)blockIdx.x >= *n_win_dev) return;
+  extern __shared__ double sm[];
+  const int D = 6 * N, W = blockIdx.x;
+  const int E = fc ? N * (N - 1) / 2 : N - 1;
+  double* H = sm;                         // D x D
+  double* bv = H + D * D;                 // D
+  double* xs = bv + D;                    // D
+  double* z = xs + D;                     // 7 N
+  double* Li = z + 7 * N;                 // N x [7][7]: C^-1
+  double* rec = Li + 49 * N;              // factor records, then the posterior blocks [N][36]
+  const double* P = poses + (size_t)W * N * 7;
+  const double* V = vos + (size_t)W * E * 7;
+  __shared__ int s_fail;
+  if (threadIdx.x == 0) s_fail = 0;
+  for (int i = threadIdx.x; i < 7 * N; i += blockDim.x) z[i] = P[i];
+  // prologue: C = chol(S7) and C^-1 per slot
+  for (int i = threadIdx.x; i < N; i += blockDim.x) {
+    const double* S = sig7 + ((size_t)W * N + i) * 49;
+    double C[7][7];
+    bool ok = true;
+    for (int c = 0; c < 7; ++c) {
+      for (int r = c; r < 7; ++r) {
+        double v = S[7 * r + c];
+        for (int k = 0; k < c; ++k) v -= C[r][k] * C[c][k];
+        if (r == c) {
+          if (!(v > 0.0)) { ok = false; v = 1.0; }
+          C[c][c] = sqrt(v);
+        } else {
+          C[r][c] = v / C[c][c];
+        }
+      }
+    }
+    double* L = Li + 49 * i;
+    for (int c = 0; c < 7; ++c)             // C L = I, column by column
+      for (int r = 0; r < 7; ++r) {
+        double v = r == c ? 1.0 : 0.0;
+        for (int k = c; k < r; ++k) v -= C[r][k] * L[7 * k + c];
+        L[7 * r + c] = r < c ? 0.0 : v / C[r][r];
+      }
+    if (!ok) atomicExch(&s_fail, 1);
+  }
+  __syncthreads();
+  for (int it = 0; it <= n_iters; ++it) {
+    pgo_cov_normal(z, P, Li, V, N, fc, E, w_rx, w_rq, rec, H, bv);
+    pgo_cov_cholesky(H, D, &s_fail);
+    if (it == n_iters) break;               // the posterior's factor, at the returned state
+    pgo_cov_solve(H, bv, D, xs);
+    __syncthreads();
+    for (int i = threadIdx.x; i < N; i += blockDim.x) {
+      z[7 * i] += xs[6 * i]; z[7 * i + 1] += xs[6 * i + 1]; z[7 * i + 2] += xs[6 * i + 2];
+      const double mx = xs[6 * i + 3], my = xs[6 * i + 4], mz = xs[6 * i + 5];
+      const double n = sqrt(mx * mx + my * my + mz * mz);
+      const double sc = (n == 0.0) ? 1.0 : sin(n) / n;
+      const Q4 dq = {cos(n), sc * mx, sc * my, sc * mz};
+      const Q4 q = q_mul(Q4{z[7 * i + 3], z[7 * i + 4], z[7 * i + 5], z[7 * i + 6]}, dq);
+      z[7 * i + 3] = q.w; z[7 * i + 4] = q.x; z[7 * i + 5] = q.y; z[7 * i + 6] = q.z;
+    }
+    __syncthreads();
+  }
+  // Q = R^-1 (upper), right-looking from the last row: Q[a][c] (a < c) kept in H[c][a], its diagonal in xs
+  for (int idx = threadIdx.x; idx < D * D; idx += blockDim.x) {
+    const int r = idx / D, c = idx % D;
+    if (c < r) H[idx] = 0.0;
+  }
+  for (int i = threadIdx.x; i < D; i += blockDim.x) xs[i] = 1.0;
+  __syncthreads();
+  for (int m = D - 1; m >= 0; --m) {
+    const double rmm = H[m * D + m];
+    for (int c = m + threadIdx.x; c < D; c += blockDim.x) {
+      if (c == m) xs[m] /= rmm;
+      else H[c * D + m] /= rmm;
+    }
+    __syncthreads();
+    for (int idx = threadIdx.x; idx < m * (D - m); idx += blockDim.x) {
+      const int a = idx / (D - m), c = m + idx % (D - m);
+      const double qmc = c == m ? xs[m] : H[c * D + m];
+      H[c * D + a] -= H[a * D + m] * qmc;
+    }
+    __syncthreads();
+  }
+  // P = Q Q': the 6 x 6 diagonal block of each slot
+  double* Pb = rec;
+  for (int idx = threadIdx.x; idx < 36 * N; idx += blockDim.x) {
+    const int i = idx / 36, a = 6 * i + (idx % 36) / 6, b = 6 * i + idx % 6;
+    const int c0 = a > b ? a : b;
+    double v = (c0 == a ? xs[a] : H[c0 * D + a]) * (c0 == b ? xs[b] : H[c0 * D + b]);
+    for (int c = c0 + 1; c < D; ++c) v += H[c * D + a] * H[c * D + b];
+    Pb[idx] = v;
+  }
+  __syncthreads();
+  double* O = out + (size_t)W * N * 7;
+  for (int i = threadIdx.x; i < 7 * N; i += blockDim.x) O[i] = z[i];
+  for (int i = threadIdx.x; i < N; i += blockDim.x) {   // cov = B P B', B = blockdiag(I, G(q))
+    double G[3][3], B[6][6] = {};
+    qlog_jac(Q4{z[7 * i + 3], z[7 * i + 4], z[7 * i + 5], z[7 * i + 6]}, G);
+    for (int a = 0; a < 3; ++a) {
+      B[a][a] = 1.0;
+      for (int b = 0; b < 3; ++b) B[3 + a][3 + b] = G[a][b];
+    }
+    const double* Pi = Pb + 36 * i;
+    double BP[6][6];
+    for (int a = 0; a < 6; ++a)
+      for (int b = 0; b < 6; ++b) {
+        double v = 0.0;
+        for (int k = 0; k < 6; ++k) v += B[a][k] * Pi[6 * k + b];
+        BP[a][b] = v;
+      }
+    double* o = cov + ((size_t)W * N + i) * 36;
+    for (int a = 0; a < 6; ++a)
+      for (int b = 0; b < 6; ++b) {
+        double v = 0.0;
+        for (int k = 0; k < 6; ++k) v += BP[a][k] * B[b][k];
+        o[6 * a + b] = v;
+      }
+  }
+  if (threadIdx.x == 0 && s_fail && status != nullptr) atomicExch(status, 1);
+  if (threadIdx.x == 0 && win_fail != nullptr) win_fail[W] = s_fail;
+}
+
+static size_t pgo_cov_smem(int N) {
+  const int D = 6 * N, E = N * (N - 1) / 2;
+  const int rec = N * kUnaryRec + E * kEdgeRec;
+  return (size_t)(D * D + 2 * D + 7 * N + 49 * N + (rec > 36 * N ? rec : 36 * N)) * sizeof(double);
+}
+
+int pgo_cov_prepare() {
+  static bool attr = false;
+  if (!attr) {
+    MN_CUDA(cudaFuncSetAttribute(k_pgo_cov, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pgo_cov_smem(kPgoMaxN)));
+    attr = true;
+  }
+  return 0;
+}
+
+int launch_pgo_cov(const double* poses, const double* sig7, const double* vos, double* out, double* cov, int n_windows,
+                   int N, int fc, double w_rx, double w_rq, int n_iters, int* status, const int* n_win_dev,
+                   int* win_fail, cudaStream_t st) {
+  MN_TRY(pgo_cov_prepare());
+  MN_LAUNCH(k_pgo_cov, n_windows, kPgoThreads, pgo_cov_smem(N), st, poses, sig7, vos, out, cov, N, fc, w_rx, w_rq,
+            n_iters, status, n_win_dev, win_fail);
+  MN_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace mapnet
 
 using namespace mapnet;
@@ -284,6 +660,19 @@ extern "C" int mapnet_pgo_optimize(const double* poses, const double* vos, doubl
   pgo_weights(sax, saq, srx, srq, w4);
   return launch_pgo(poses, vos, out, n_windows, N, fc_vos ? 1 : 0, w4, n_iters, flags & 1, status_dev, nullptr,
                     (cudaStream_t)stream);
+}
+
+extern "C" int mapnet_pgo_optimize_cov(const double* poses, const double* sig7, const double* vos, double* out,
+                                       double* cov, int n_windows, int N, int fc_vos, double srx, double srq,
+                                       int n_iters, int* status_dev, void* stream) {
+  MN_CHECK(poses && sig7 && vos && out && cov && n_windows >= 1, "pgo_optimize_cov: bad argument");
+  MN_CHECK(N >= 2 && N <= kPgoMaxN, "pgo_optimize_cov: window of %d poses outside [2, %d]", N, kPgoMaxN);
+  MN_CHECK(srx > 0 && srq > 0 && n_iters >= 0, "pgo_optimize_cov: covariances must be positive");
+  int ndev = 0;
+  MN_CHECK(cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0,
+           "pgo_optimize_cov: no CUDA device (this library has no CPU fallback)");
+  return launch_pgo_cov(poses, sig7, vos, out, cov, n_windows, N, fc_vos ? 1 : 0, 1.0 / sqrt(srx), 1.0 / sqrt(srq),
+                        n_iters, status_dev, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 // qexp + un-normalisation of a batch of 6-vectors (scripts/eval.py:163-181): out[i] = (t * pose_s + pose_m, qexp(logq))
@@ -329,22 +718,9 @@ __global__ void k_sample_post(const double* __restrict__ mean, const double* __r
   if (pose7 != nullptr) {
     double* o = pose7 + 7 * i;
     for (int k = 0; k < 3; ++k) o[k] = mu[k] * d[k] + ms[k];
-    const double vx = mu[3], vy = mu[4], vz = mu[5];
-    const double nn = sqrt(vx * vx + vy * vy + vz * vz);
-    const double f = nn > 0.0 ? sin(nn) / nn : 0.0;
-    o[3] = nn > 0.0 ? cos(nn) : 1.0;
-    o[4] = f * vx; o[5] = f * vy; o[6] = f * vz;
+    sample_qexp(mu[3], mu[4], mu[5], o + 3);
   }
-  if (cov_out != nullptr)
-    for (int r = 0; r < 6; ++r)
-      for (int c = 0; c < 6; ++c) cov_out[36 * i + 6 * r + c] = d[r] * C[6 * r + c] * d[c];
-  double tt = 0.0, tq = 0.0;
-  for (int k = 0; k < 3; ++k) {
-    tt += d[k] * C[7 * k] * d[k];
-    tq += C[7 * (k + 3)];
-  }
-  t_std[i] = sqrt(tt);
-  q_std_deg[i] = 2.0 * sqrt(tq) * (180.0 / 3.14159265358979323846);
+  sample_stats(C, d, cov_out != nullptr ? cov_out + 36 * i : nullptr, t_std + i, q_std_deg + i);
 }
 }  // namespace mapnet
 

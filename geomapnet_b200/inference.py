@@ -23,7 +23,7 @@ from . import _lib
 from .common.pgo import optimize_pose_windows
 from .data.loader import SidePipeline
 
-__all__ = ["Predictor", "Localizer", "Tracker", "MultiTracker", "predict", "post", "pgo", "pose_errors", "evaluate_tuples", "evaluate_sequence", "validate"]
+__all__ = ["Predictor", "Localizer", "Tracker", "MultiTracker", "SampledTracker", "predict", "post", "pgo", "pose_errors", "evaluate_tuples", "evaluate_sequence", "validate"]
 
 
 class Predictor(object):
@@ -719,6 +719,174 @@ class Tracker(object):
             getattr(_lib.lib(), self._DESTROY)(self.h)
             self.h = ctypes.c_void_p()
         self._open = False
+
+
+class SampledTracker(Tracker):
+    """Tracker with Monte-Carlo dropout: each frame's S dropout draws weigh its pose in the pose graph, and every
+    tracked pose comes with a covariance.
+
+        st = SampledTracker(loc, S=32, steps=7, skip=10, vo_fc=True, sax=1e-4, saq=1e-4, srx=20, srq=20)
+        first, est = st(frames, vo_poses)       # est = dict(pose7 [n,7], cov [n,6,6], t_std [n], q_std_deg [n])
+        now, first, est = st.step(frames, vo_poses)     # now: the same dict, each given frame's zero-lag estimate
+        first, est = st.flush(); st.reset(); st.close(); st.lag; st.seen
+
+    Frames, VO poses, windows, lag, chunking and errors are Tracker's.  Per frame f, the S draws (Localizer.sample's,
+    in the model's normalised units) give a mean (mu_t, mu_v) and a covariance Sigma_f [6,6].  Its absolute pose is
+    p_f = (mu_t, qexp(mu_v)) (bit for bit Localizer.sample's pose7 without pose statistics), and its factor covariance
+        S7_f = A Sigma_f A' + diag(sax, sax, sax, saq, saq, saq, saq),  A = blockdiag(I3, d qexp(v) / dv at mu_v).
+    The absolute factor of slot k holding frame f has residual C^-1 (z_k - p_f), S7_f = C C'; the relative factors
+    (srx, srq), state and manifold update are the Tracker's, and each of the 10 iterations takes the exact Gauss-Newton
+    step (not eval.py's literal solve, whose end point has no posterior).  A window's posterior is the inverse of its
+    normal matrix at the returned state; slot k's 6 x 6 block, mapped to (t, log q), is cov_k, comparable with
+    Localizer.sample's cov.  est per emitted frame: pose7 (slot steps//2, un-normalised as Tracker's), cov = D cov_k D
+    with D = diag(pose_s, 1, 1, 1), t_std = sqrt(trace of its translation block), q_std_deg = 2 sqrt(trace of its log q
+    block) in degrees -- Localizer.sample's statistics.  All float64 on the device.
+
+    sax and saq keep the reference's meaning, the variance floor of the absolute factors (normalised units).  The
+    sampled covariance is added to them, so it matters only where the floors sit below the sampled variances: at the
+    reference's default of 1, the floors dominate and the weights barely move.
+
+    Each chunk of max_batch frames replays one CUDA graph, captured per (B, H, W): the Localizer's sampled engine
+    launches at the device dropout counter (S consecutive dropout steps per chunk, as Localizer.sample takes them), then
+    three tracking launches (csrc/loader.cu, mapnet_track_sample_*: gather, k_pgo_cov, emit).  The eager run before the
+    capture uses an explicit dropout step and runs no tracking launch, so it advances neither the dropout counter nor
+    the sequence.  Engines, snapshot, refresh(), precision and dropout counter are the Localizer's predictor's.  S as
+    Localizer.sample takes it: 2 <= S <= 1024, and a model without dropout raises ValueError."""
+
+    _DESTROY = "mapnet_track_sample_destroy"
+
+    def __init__(self, localizer, S, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0):
+        super(SampledTracker, self).__init__(localizer, steps, skip, vo_fc, sax, saq, srx, srq)
+        self.S = _check_draws(S, localizer.predictor.droprate)
+
+    def _handle(self):
+        if not self.h:
+            pr = self.loc.predictor
+            sig = (ctypes.c_double * 4)(*self.sigmas)
+            _lib.check(_lib.lib().mapnet_track_sample_create(ctypes.byref(self.h), self.steps, self.skip,
+                                                             int(self.vo_fc), pr.max_batch, sig, self.loc._m,
+                                                             self.loc._s), "mapnet_track_sample_create")
+        return self.h
+
+    def _graph(self, fb, now=False):
+        B, H, W = fb.shape[:3]
+        graphs = self._now_graphs if now else self._graphs
+        g = graphs.get((B, H, W))
+        if g is None:
+            loc, pr, L = self.loc, self.loc.predictor, _lib.lib()
+            dev, h, S = pr.device, self._handle(), self.S
+            eng, pre = pr._engine(*loc._resized(H, W)), loc._plan(H, W)
+            f64 = dict(dtype=torch.float64, device=dev)
+            xs = torch.empty((B, H, W, 3), dtype=torch.uint8, device=dev)
+            xs.copy_(fb)
+            vs = torch.zeros((B, 6), dtype=torch.float32, device=dev)
+            smp = torch.empty((B, S, 6), dtype=torch.float32, device=dev)
+            mean, cov = torch.empty((B, 6), **f64), torch.empty((B, 6, 6), **f64)
+            row = _lib.TRACK_SAMPLE_ROW
+            out = torch.empty((B, row), **f64)
+            nowb = torch.empty((B, row), **f64) if now else None
+            fp = ctypes.POINTER(ctypes.c_float)
+
+            def sample(step):
+                _lib.check(L.mapnet_infer_sample_frames(eng.h, pre, xs.data_ptr(), B, loc.mean.ctypes.data_as(fp),
+                                                        loc.std.ctypes.data_as(fp), S, pr.droprate, int(pr.seed), step,
+                                                        smp.data_ptr(), mean.data_ptr(), cov.data_ptr(),
+                                                        _lib.stream_ptr()), "mapnet_infer_sample_frames")
+
+            def track():
+                if now:
+                    _lib.check(L.mapnet_track_sample_step_now(h, mean.data_ptr(), cov.data_ptr(), vs.data_ptr(), B,
+                                                              out.data_ptr(), nowb.data_ptr(), _lib.stream_ptr()),
+                               "mapnet_track_sample_step_now")
+                else:
+                    _lib.check(L.mapnet_track_sample_step(h, mean.data_ptr(), cov.data_ptr(), vs.data_ptr(), B,
+                                                          out.data_ptr(), _lib.stream_ptr()), "mapnet_track_sample_step")
+
+            cur = torch.cuda.current_stream(dev)
+            side = torch.cuda.Stream(dev)
+            side.wait_stream(cur)
+            with torch.cuda.stream(side):        # eager run first, at an explicit dropout step: no state advances
+                sample(0)
+            cur.wait_stream(side)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                sample(_lib.UINT64_MAX)
+                track()
+            g = graphs[(B, H, W)] = (graph, xs, vs, out, smp, mean, cov, nowb)   # every buffer the graph reads
+        return g
+
+    @staticmethod
+    def _est(rows):
+        """the est dict of output rows [n,45]"""
+        return dict(pose7=rows[:, :7].contiguous(), cov=rows[:, 7:43].reshape(-1, 6, 6).contiguous(),
+                    t_std=rows[:, 43].contiguous(), q_std_deg=rows[:, 44].contiguous())
+
+    def _run(self, frames, vo_poses, now):
+        """(first, rows [n,45], now rows [B,45] or None): the chunks of max_batch frames, one graph replay each"""
+        self._check_open()
+        x, single = self.loc._frames(frames)
+        vo = self._vo(vo_poses, x.shape[0], single)
+        pr = self.loc.predictor
+        mb, first = pr.max_batch, _first_pending(self.seen, self.lag)
+        outs, nows = [], []
+        with torch.cuda.device(pr.device):
+            for lo in range(0, x.shape[0], mb):
+                fb = x[lo:lo + mb]
+                g = self._graph(fb, now)
+                graph, xs, vs, out = g[:4]
+                xs.copy_(fb, non_blocking=True)
+                vs.copy_(vo[lo:lo + mb], non_blocking=True)
+                graph.replay()
+                n = _first_pending(self.seen + fb.shape[0], self.lag) - _first_pending(self.seen, self.lag)
+                self.seen += fb.shape[0]
+                outs.append(out[:n].clone())
+                if now:
+                    nows.append(g[7].clone())
+        cat = lambda ts: ts[0] if len(ts) == 1 else torch.cat(ts, 0)
+        return first, cat(outs), (cat(nows) if now else None)
+
+    @torch.no_grad()
+    def __call__(self, frames, vo_poses):
+        """-> (first, est): the frames first .. first+n-1 whose windows this call completed (Tracker.__call__)"""
+        first, rows, _ = self._run(frames, vo_poses, False)
+        return first, self._est(rows)
+
+    @torch.no_grad()
+    def step(self, frames, vo_poses):
+        """-> (now, first, est): now holds each given frame's zero-lag estimate (Tracker.step's window), one row per
+        frame; (first, est) is what self(frames, vo_poses) returns"""
+        first, rows, nows = self._run(frames, vo_poses, True)
+        return self._est(nows), first, self._est(rows)
+
+    @torch.no_grad()
+    def flush(self):
+        """-> (first, est): the last n = min(lag, seen) frames, as Tracker.flush; raises np.linalg.LinAlgError after
+        resetting when a window's normal matrix or a frame's factor covariance was not positive definite"""
+        self._check_open()
+        pr = self.loc.predictor
+        first = _first_pending(self.seen, self.lag)
+        n, failed = self.seen - first, ctypes.c_int(0)
+        with torch.cuda.device(pr.device):
+            out = torch.empty((max(self.lag, 1), _lib.TRACK_SAMPLE_ROW), dtype=torch.float64, device=pr.device)
+            if self.h:
+                L = _lib.lib()
+                _lib.check(L.mapnet_track_sample_flush(self.h, out.data_ptr(), _lib.stream_ptr()),
+                           "mapnet_track_sample_flush")
+                _lib.check(L.mapnet_track_sample_status(self.h, None, ctypes.byref(failed), _lib.stream_ptr()),
+                           "mapnet_track_sample_status")
+        self.reset()
+        if failed.value:
+            raise np.linalg.LinAlgError("pose graph: the normal matrix of a window of the sequence is not positive "
+                                        "definite")
+        return first, self._est(out[:n])
+
+    def reset(self):
+        """Start a new sequence: the next frame is frame 0 (stream-ordered)."""
+        self._check_open()
+        if self.h:
+            with torch.cuda.device(self.loc.predictor.device):
+                _lib.check(_lib.lib().mapnet_track_sample_reset(self.h, _lib.stream_ptr()), "mapnet_track_sample_reset")
+        self.seen = 0
 
 
 def _stream_records(seen, streams, lag):

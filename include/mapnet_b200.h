@@ -223,6 +223,20 @@ int mapnet_pose_post(const float* pred6, double* out7, int64_t n, const double* 
 int mapnet_pgo_optimize(const double* poses, const double* vos, double* out, int n_windows, int N, int fc_vos,
                         double sax, double saq, double srx, double srq, int n_iters, int flags, int* status_dev, void* stream);
 
+/* mapnet_pgo_optimize_cov: covariance-weighted pose graph of n_windows windows of N <= 16 poses in one launch.  poses
+ * [n_windows][N][7] are the absolute poses p (t, q wxyz), sig7 [n_windows][N][7][7] their covariances S7 (symmetric
+ * positive definite; the lower triangle is read), vos [n_windows][E][7] as for mapnet_pgo_optimize.  With S7 = C C'
+ * (lower Cholesky factor) slot k's absolute factor has residual C^-1 (z_k - p_k) and Jacobian C^-1 blockdiag(I3,
+ * m_rot(q_k)); the relative factors (weights srx, srq), the state and its manifold update are mapnet_pgo_optimize's;
+ * each of the n_iters iterations takes the exact Gauss-Newton step.  Outputs: out [n_windows][N][7] and cov
+ * [n_windows][N][6][6], slot k's posterior covariance in (t, log q): the 6 x 6 diagonal block of H^-1 of the normal
+ * matrix at the returned state, mapped by blockdiag(I3, G(q_k)), G(q) = d qlog(q * dq(x)) / dx at x = 0.  Every output
+ * is a fixed-order sum (no atomics), so equal inputs give bitwise equal outputs.  *status_dev (may be NULL) is set to 1
+ * when a window's normal matrix or one of its S7 is not positive definite.  Device pointers, fp64. */
+int mapnet_pgo_optimize_cov(const double* poses, const double* sig7, const double* vos, double* out, double* cov,
+                            int n_windows, int N, int fc_vos, double srx, double srq, int n_iters, int* status_dev,
+                            void* stream);
+
 /* ---- streaming pose-graph tracker (csrc/loader.cu; geomapnet_b200.inference.Tracker): scripts/eval.py's MapNet+PGO
  * loop over frames as they arrive.  The window of frame c is eval.py's MF(steps=T, skip) tuple: slot k holds frame
  * clip(c + (k - T/2) * skip, 0, last), its VOs are calc_vos_safe of the VO-library poses of consecutive slots (or of
@@ -299,6 +313,40 @@ int mapnet_track_multi_flush(mapnet_track_multi_t* h, int s, double* out7, void*
 int mapnet_track_multi_reset(mapnet_track_multi_t* h, int s, void* stream);
 int mapnet_track_multi_status(mapnet_track_multi_t* h, int s, int64_t* frames_seen, int* failed, void* stream);
 int mapnet_track_multi_destroy(mapnet_track_multi_t* h);
+
+/* ---- Monte-Carlo tracker (csrc/loader.cu; geomapnet_b200.inference.SampledTracker): mapnet_track_t's windows, lag,
+ * counter and call semantics, with every frame's S-draw Monte-Carlo dropout statistics in place of its one draw and a
+ * covariance-weighted pose graph (mapnet_pgo_optimize_cov) in place of k_pgo.
+ *   mapnet_track_sample_create: mapnet_track_create's arguments and checks.  sax / saq are the floors of the absolute
+ *     factors' covariances, srx / srq the relative factors', in normalised units.
+ *   mapnet_track_sample_step: B new frames (1 <= B <= max_batch): mean6 [B][6] and cov36 [B][6][6] float64 (the
+ *     normalised (t, log q) mean and covariance of the draws, as mapnet_infer_sample_frames writes them) and vo6
+ *     [B][6] float32 as mapnet_track_step takes it.  Each new frame's p = (mean_t, qexp(mean_v)) (qexp as
+ *     mapnet_sample_post) and S7 = A cov A' + diag(sax I3, saq I4), A = blockdiag(I3, d qexp(v) / dv at mean_v), are
+ *     formed once into device rings.  out gets one row of 45 doubles per frame mapnet_track_step would emit:
+ *     pose7 [7] (slot T/2, translated as mapnet_track_step's out7), cov [6][6] = D cov_k D with D = diag(pose_s, 1, 1,
+ *     1) (the identity without pose statistics), t_std and q_std_deg (mapnet_sample_post's statistics of that cov).
+ *     Three launches (gather, k_pgo_cov, emit), graph-capturable, nothing read back.
+ *   mapnet_track_sample_step_now: also now [B][45], the same row for slot T-1 of the window that ends at each new
+ *     frame (mapnet_track_step_now's windows).
+ *   mapnet_track_sample_flush / _reset / _status / _destroy: as mapnet_track_*; the status is also set when a frame's
+ *     S7 is not positive definite.
+ * Pointers are device memory unless marked HOST.  Argument errors return non-zero before any launch. */
+typedef struct mapnet_track_sample mapnet_track_sample_t;
+int mapnet_track_sample_create(mapnet_track_sample_t** out, int T, int skip, int fc_vos, int max_batch,
+                               const double* sigmas4, const double* pose_m3, const double* pose_s3);
+int mapnet_track_sample_step(mapnet_track_sample_t* h, const double* mean6, const double* cov36, const float* vo6, int B,
+                             double* out, void* stream);
+int mapnet_track_sample_step_now(mapnet_track_sample_t* h, const double* mean6, const double* cov36, const float* vo6,
+                                 int B, double* out, double* now, void* stream);
+int mapnet_track_sample_flush(mapnet_track_sample_t* h, double* out, void* stream);
+int mapnet_track_sample_reset(mapnet_track_sample_t* h, void* stream);
+int mapnet_track_sample_status(mapnet_track_sample_t* h, int64_t* frames_seen, int* failed, void* stream);
+int mapnet_track_sample_destroy(mapnet_track_sample_t* h);
+/* mapnet_test_sample_factor: what mapnet_track_sample_step forms for each of n frames, with its arithmetic: p7 [n][7]
+ * and S7 [n][7][7] from mean6 [n][6] and cov36 [n][6][6] (device pointers, float64) and the floors sax, saq > 0. */
+int mapnet_test_sample_factor(const double* mean6, const double* cov36, int64_t n, double sax, double saq, double* p7,
+                              double* s7, void* stream);
 
 /* ---- eval-mode inference engine (csrc/infer.cu): a frozen snapshot of a PoseNet / MapNet trunk for
  * scripts/eval.py-style prediction.  mapnet_infer_load copies the weights (packed fprop operands only), the eval-mode
