@@ -508,6 +508,118 @@ k_track_multi_emit(const double* __restrict__ opt7, const int* __restrict__ win_
   if (win_fail[w]) atomicExch(&st[s].status, 1);
 }
 
+// ---- multi-stream Monte-Carlo tracker (mapnet_track_multi_sample_*, inference.SampledMultiTracker): the streams,
+// records and windows of mapnet_track_multi_* with the factors of mapnet_track_sample_*.  Per stream: its frame count,
+// its status word and rings of R frames of p7, S7 (float64) and VO poses (float32), [n_streams][R].
+
+// k_track_sample_gather for B frames of several streams (records rec) or a flush of stream flush_s: rows 0 .. B-1
+// form the new frames' p7 / S7 into their streams' rings, then slot (w, k) of window w < max_win, then VO (w, e), the
+// windows found as k_track_multi_gather finds them.  A slot that holds a frame of this call forms that frame's factor
+// itself, from the frame's input row: a multi-stream call has no cheap map from a frame to the slots that hold it (the
+// frame's row would scan every window of the call), and sample_factor is a pure function of the frame's mean and cov,
+// so each copy is bit for bit the ring's.  Thread 0 writes the count of windows k_pgo_cov and the emit read.
+__global__ void __launch_bounds__(128)
+k_track_multi_sample_gather(const double* __restrict__ mean, const double* __restrict__ cov,
+                            const float* __restrict__ vo6, const MTrackRec* __restrict__ rec, int B, int now,
+                            int flush_s, const MTrackDev* __restrict__ st, int n_streams, int* __restrict__ n_win_dev,
+                            double* __restrict__ ring7, double* __restrict__ ring49, float* __restrict__ ring_vo,
+                            long long R, int T, int skip, int fc, int max_win, double sax, double saq,
+                            double* __restrict__ win7, double* __restrict__ win49, double* __restrict__ vos7) {
+  pdl_prologue();
+  const long long lag = trackcore::lag(T, skip);
+  const int E = fc ? T * (T - 1) / 2 : T - 1;
+  long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r == 0) {
+    int n = 0;
+    if (flush_s >= 0) n = (int)(st[flush_s].seen - trackcore::first_pending(st[flush_s].seen, lag));
+    else if (now) n = B;
+    else while (n < B && rec[n].win >= 0) ++n;
+    *n_win_dev = n;
+  }
+  if (r < B) {
+    const MTrackRec q = rec[r];
+    if (q.stream < 0 || q.stream >= n_streams) return;
+    const long long k = q.stream * R + q.frame % R;
+    sample_factor(mean + 6 * r, cov + 36 * r, sax, saq, ring7 + 7 * k, ring49 + 49 * k);
+#pragma unroll
+    for (int c = 0; c < 6; ++c) ring_vo[6 * k + c] = vo6[6 * r + c];
+    return;
+  }
+  r -= B;
+  MWin m;
+  if (r < (long long)max_win * T) {
+    const int w = (int)(r / T), k = (int)(r % T);
+    if (!mtrack_window(rec, B, w, now, flush_s, st, n_streams, lag, &m)) return;
+    const long long f = trackcore::slot_frame(m.c, k, T, skip, m.last);
+    if (f >= m.f0) {
+      const int b = mtrack_input(rec, B, m, f);
+      if (b >= 0) {
+        sample_factor(mean + 6LL * b, cov + 36LL * b, sax, saq, win7 + 7 * r, win49 + 49 * r);
+      } else {                                      // an inconsistent record table: a visible NaN, no stray read
+        const double nan = __longlong_as_double(0x7ff8000000000000LL);
+        for (int c = 0; c < 7; ++c) win7[7 * r + c] = nan;
+        for (int c = 0; c < 49; ++c) win49[49 * r + c] = nan;
+      }
+    } else {
+      const long long q = m.s * R + f % R;
+      for (int c = 0; c < 7; ++c) win7[7 * r + c] = ring7[7 * q + c];
+      for (int c = 0; c < 49; ++c) win49[49 * r + c] = ring49[49 * q + c];
+    }
+    return;
+  }
+  r -= (long long)max_win * T;
+  if (r < (long long)max_win * E) {
+    const int w = (int)(r / E), e = (int)(r % E);
+    if (!mtrack_window(rec, B, w, now, flush_s, st, n_streams, lag, &m)) return;
+    int i, j;
+    trackcore::vo_pair(e, T, fc, &i, &j);
+    const long long fa = trackcore::slot_frame(m.c, i, T, skip, m.last);
+    const long long fb = trackcore::slot_frame(m.c, j, T, skip, m.last);
+    const posemath::Pose6 v = posemath::calc_vo_logq_safe(mtrack_vo(vo6, ring_vo, rec, B, m, fa, R),
+                                                          mtrack_vo(vo6, ring_vo, rec, B, m, fb, R));
+    const float v6[6] = {v.t.x, v.t.y, v.t.z, v.l.x, v.l.y, v.l.z};
+    st_pose7(v6, vos7 + 7 * r);
+  }
+}
+
+// k_track_multi_emit with k_track_sample_emit's rows: window w's middle slot into out row w (a zero-lag step: into
+// row rec[w].row when the window completed a frame, and its last slot into now row w); a window k_pgo_cov marked
+// failed (its normal matrix or a slot's S7 not positive definite) sets its own stream's status; the last record of
+// each stream in the call sets that stream's frame count.
+__global__ void __launch_bounds__(128)
+k_track_multi_sample_emit(const double* __restrict__ opt7, const double* __restrict__ cov36,
+                          const int* __restrict__ win_fail, const MTrackRec* __restrict__ rec, int B, int flush_s,
+                          MTrackDev* __restrict__ st, int n_streams, const int* __restrict__ n_win_dev, int T, int un,
+                          double m0, double m1, double m2, double s0, double s1, double s2, double* __restrict__ out,
+                          double* __restrict__ now) {
+  pdl_prologue();
+  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+  const double ms[3] = {m0, m1, m2}, ss[3] = {s0, s1, s2};
+  const long long mid = (long long)w * T + T / 2, last = (long long)w * T + T - 1;
+  if (w < B) {
+    const MTrackRec q = rec[w];
+    const bool ok = q.stream >= 0 && q.stream < n_streams;
+    if (ok && q.rank == q.count - 1) st[q.stream].seen = (long long)q.frame + 1;
+    if (now != nullptr) {
+      if (!ok) return;
+      track_sample_row(opt7 + 7 * last, cov36 + 36 * last, un, ms, ss, now + kTrackSampleRow * (long long)w);
+      if (q.row >= 0)
+        track_sample_row(opt7 + 7 * mid, cov36 + 36 * mid, un, ms, ss, out + kTrackSampleRow * (long long)q.row);
+      if (win_fail[w]) atomicExch(&st[q.stream].status, 1);
+      return;
+    }
+  }
+  if (now != nullptr || w >= *n_win_dev) return;
+  int s = flush_s;
+  if (s < 0) {
+    const int b = rec[w].win;
+    s = b >= 0 && b < B ? rec[b].stream : -1;
+    if (s < 0 || s >= n_streams) return;
+  }
+  track_sample_row(opt7 + 7 * mid, cov36 + 36 * mid, un, ms, ss, out + kTrackSampleRow * (long long)w);
+  if (win_fail[w]) atomicExch(&st[s].status, 1);
+}
+
 }  // namespace mapnet
 
 using namespace mapnet;
@@ -1030,6 +1142,134 @@ int mapnet_track_multi_destroy(mapnet_track_multi_t* h) {
   if (h == nullptr) return 0;
   cudaFree(h->st); cudaFree(h->n_win); cudaFree(h->ring7); cudaFree(h->ring_vo); cudaFree(h->win7); cudaFree(h->vos7);
   cudaFree(h->opt7);
+  delete h;
+  return 0;
+}
+
+}  // extern "C"
+
+struct mapnet_track_multi_sample : TrackCfg {
+  int n_streams;
+  double sax, saq;                          // the floors of the absolute factors' covariances
+  MTrackDev* st;                            // [n_streams]
+  int* n_win;                               // the windows of the current call, written by the gather
+  int* win_fail;                            // [max_win]: k_pgo_cov's per-window failure flags
+  double *ring7, *ring49;                   // [n_streams][R][7], [n_streams][R][7][7]
+  float* ring_vo;                           // [n_streams][R][6]
+  double *win7, *win49, *vos7, *opt7, *cov36;   // [max_win][T][7], [.][T][49], [.][E][7], [.][T][7], [.][T][36]
+};
+
+// the three launches of a multi-stream sampled call: B frames with records rec (a step; with now a zero-lag step,
+// which solves all B of its windows) or a flush of stream flush_s (B = 0); out [max_win][45], now [B][45] or null
+static int track_multi_sample_launch(mapnet_track_multi_sample_t* h, const double* mean, const double* cov,
+                                     const float* vo6, const MTrackRec* rec, int B, int flush_s, double* out,
+                                     double* now, cudaStream_t st) {
+  const int nw = flush_s >= 0 ? (int)(h->lag < h->max_win ? h->lag : h->max_win) : B;    // the grid's windows
+  const int zl = now != nullptr ? 1 : 0;
+  const long long rows = B + (long long)nw * (h->T + h->E);
+  MN_LAUNCH(k_track_multi_sample_gather, cdiv(rows, 128), 128, 0, st, mean, cov, vo6, rec, B, zl, flush_s,
+            (const MTrackDev*)h->st, h->n_streams, h->n_win, h->ring7, h->ring49, h->ring_vo, h->R, h->T, h->skip,
+            h->fc, nw, h->sax, h->saq, h->win7, h->win49, h->vos7);
+  MN_LAUNCH_CHECK();
+  MN_TRY(launch_pgo_cov(h->win7, h->win49, h->vos7, h->opt7, h->cov36, nw, h->T, h->fc, h->w4[2], h->w4[3], 10,
+                        nullptr, zl ? nullptr : h->n_win, h->win_fail, st));
+  MN_LAUNCH(k_track_multi_sample_emit, cdiv(nw > B ? nw : B, 128), 128, 0, st, (const double*)h->opt7,
+            (const double*)h->cov36, (const int*)h->win_fail, rec, B, flush_s, h->st, h->n_streams,
+            (const int*)h->n_win, h->T, h->un, h->m[0], h->m[1], h->m[2], h->s[0], h->s[1], h->s[2], out, now);
+  MN_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" {
+
+int mapnet_track_multi_sample_create(mapnet_track_multi_sample_t** out, int n_streams, int T, int skip, int fc_vos,
+                                     int max_batch, const double* sigmas4, const double* pose_m3,
+                                     const double* pose_s3) {
+  MN_CHECK(out != nullptr && sigmas4 != nullptr, "track_multi_sample_create: null argument");
+  *out = nullptr;
+  MN_CHECK(n_streams >= 1 && n_streams <= MAPNET_TRACK_MAX_STREAMS,
+           "track_multi_sample_create: %d streams outside [1, %d]", n_streams, MAPNET_TRACK_MAX_STREAMS);
+  TrackCfg c;
+  MN_TRY(track_config(&c, "track_multi_sample_create", T, skip, fc_vos, max_batch, sigmas4, pose_m3, pose_s3));
+  MN_TRY(pgo_cov_prepare());
+  const size_t W = (size_t)c.max_win, WT = W * c.T, ring = (size_t)n_streams * (size_t)c.R;
+  const size_t frame_bytes = (7 + 49) * sizeof(double) + 6 * sizeof(float);      // 472 B per ring frame
+  const size_t bytes = ring * frame_bytes + WT * (7 + 49 + 7 + 36) * sizeof(double) + W * c.E * 7 * sizeof(double) +
+                       (size_t)n_streams * sizeof(MTrackDev) + (W + 1) * sizeof(int);
+  MN_CHECK(ring < (1ull << 31), "track_multi_sample_create: %d streams x rings of %lld frames = %zu frames (%.3f GB) "
+           "exceed 2^31 ring frames", n_streams, c.R, ring, bytes / 1e9);
+  mapnet_track_multi_sample* h = new mapnet_track_multi_sample();
+  static_cast<TrackCfg&>(*h) = c;
+  h->n_streams = n_streams;
+  h->sax = sigmas4[0]; h->saq = sigmas4[1];
+  bool ok = cudaMalloc((void**)&h->st, (size_t)n_streams * sizeof(MTrackDev)) == cudaSuccess &&
+            cudaMalloc((void**)&h->n_win, (W + 1) * sizeof(int)) == cudaSuccess &&
+            cudaMalloc((void**)&h->ring7, ring * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->ring49, ring * 49 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->ring_vo, ring * 6 * sizeof(float)) == cudaSuccess &&
+            cudaMalloc((void**)&h->win7, WT * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->win49, WT * 49 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->vos7, W * c.E * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->opt7, WT * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->cov36, WT * 36 * sizeof(double)) == cudaSuccess &&
+            cudaMemset(h->st, 0, (size_t)n_streams * sizeof(MTrackDev)) == cudaSuccess &&
+            cudaMemset(h->n_win, 0, (W + 1) * sizeof(int)) == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess;
+  if (!ok) {
+    cudaGetLastError();
+    set_last_error("track_multi_sample_create: device allocation of %zu bytes (%d streams x rings of %lld frames of "
+                   "%zu B, %d windows) failed", bytes, n_streams, c.R, frame_bytes, c.max_win);
+    mapnet_track_multi_sample_destroy(h);
+    return 1;
+  }
+  h->win_fail = h->n_win + 1;
+  *out = h;
+  return 0;
+}
+
+int mapnet_track_multi_sample_step(mapnet_track_multi_sample_t* h, const double* mean6, const double* cov36,
+                                   const float* vo6, const int32_t* rec, int B, double* out, double* now,
+                                   void* stream) {
+  MN_CHECK(h != nullptr, "track_multi_sample_step: null handle");
+  MN_CHECK(mean6 != nullptr && cov36 != nullptr && vo6 != nullptr && rec != nullptr && out != nullptr,
+           "track_multi_sample_step: null argument");
+  MN_CHECK(B >= 1 && B <= h->max_batch, "track_multi_sample_step: %d frames outside [1, max_batch=%d]", B,
+           h->max_batch);
+  return track_multi_sample_launch(h, mean6, cov36, vo6, (const MTrackRec*)rec, B, -1, out, now,
+                                   (cudaStream_t)stream);
+}
+
+int mapnet_track_multi_sample_flush(mapnet_track_multi_sample_t* h, int s, double* out, void* stream) {
+  MN_CHECK(h != nullptr, "track_multi_sample_flush: null handle");
+  MN_CHECK(out != nullptr, "track_multi_sample_flush: null argument");
+  MN_CHECK(s >= 0 && s < h->n_streams, "track_multi_sample_flush: stream %d outside [0, %d)", s, h->n_streams);
+  if (h->lag == 0) return 0;                 // every window was complete when its last frame arrived
+  return track_multi_sample_launch(h, nullptr, nullptr, nullptr, nullptr, 0, s, out, nullptr, (cudaStream_t)stream);
+}
+
+int mapnet_track_multi_sample_reset(mapnet_track_multi_sample_t* h, int s, void* stream) {
+  MN_CHECK(h != nullptr, "track_multi_sample_reset: null handle");
+  MN_CHECK(s >= -1 && s < h->n_streams, "track_multi_sample_reset: stream %d outside [-1, %d)", s, h->n_streams);
+  const size_t n = s < 0 ? (size_t)h->n_streams : 1;
+  MN_CUDA(cudaMemsetAsync(h->st + (s < 0 ? 0 : s), 0, n * sizeof(MTrackDev), (cudaStream_t)stream));
+  return 0;
+}
+
+int mapnet_track_multi_sample_status(mapnet_track_multi_sample_t* h, int s, int64_t* frames_seen, int* failed,
+                                     void* stream) {
+  MN_CHECK(h != nullptr, "track_multi_sample_status: null handle");
+  MN_CHECK(s >= 0 && s < h->n_streams, "track_multi_sample_status: stream %d outside [0, %d)", s, h->n_streams);
+  MTrackDev d;
+  MN_CUDA(cudaMemcpyAsync(&d, h->st + s, sizeof(MTrackDev), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  MN_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+  if (frames_seen != nullptr) *frames_seen = d.seen;
+  if (failed != nullptr) *failed = d.status;
+  return 0;
+}
+
+int mapnet_track_multi_sample_destroy(mapnet_track_multi_sample_t* h) {
+  if (h == nullptr) return 0;
+  cudaFree(h->st); cudaFree(h->n_win); cudaFree(h->ring7); cudaFree(h->ring49); cudaFree(h->ring_vo);
+  cudaFree(h->win7); cudaFree(h->win49); cudaFree(h->vos7); cudaFree(h->opt7); cudaFree(h->cov36);
   delete h;
   return 0;
 }

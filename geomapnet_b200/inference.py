@@ -721,6 +721,42 @@ class Tracker(object):
         self._open = False
 
 
+def _sampled_capture(loc, S, fb, track):
+    """(CUDA graph, static uint8 input [B,H,W,3], (draws [B,S,6], mean [B,6], cov [B,6,6])) of frames shaped like fb:
+    the Localizer's sampled engine (mapnet_infer_sample_frames: S draws per frame, their normalised float64 mean and
+    covariance) at the device dropout counter, then track(mean, cov)'s launches.  Captured after an eager run of the
+    engine alone at an explicit dropout step, so building the graph advances neither the dropout counter nor any
+    tracked sequence."""
+    B, H, W = fb.shape[:3]
+    pr, L = loc.predictor, _lib.lib()
+    dev = pr.device
+    eng, pre = pr._engine(*loc._resized(H, W)), loc._plan(H, W)
+    f64 = dict(dtype=torch.float64, device=dev)
+    xs = torch.empty((B, H, W, 3), dtype=torch.uint8, device=dev)
+    xs.copy_(fb)
+    smp = torch.empty((B, S, 6), dtype=torch.float32, device=dev)
+    mean, cov = torch.empty((B, 6), **f64), torch.empty((B, 6, 6), **f64)
+    fp = ctypes.POINTER(ctypes.c_float)
+
+    def sample(step):
+        _lib.check(L.mapnet_infer_sample_frames(eng.h, pre, xs.data_ptr(), B, loc.mean.ctypes.data_as(fp),
+                                                loc.std.ctypes.data_as(fp), S, pr.droprate, int(pr.seed), step,
+                                                smp.data_ptr(), mean.data_ptr(), cov.data_ptr(), _lib.stream_ptr()),
+                   "mapnet_infer_sample_frames")
+
+    cur = torch.cuda.current_stream(dev)
+    side = torch.cuda.Stream(dev)
+    side.wait_stream(cur)
+    with torch.cuda.stream(side):        # eager run first, at an explicit dropout step: no state advances
+        sample(0)
+    cur.wait_stream(side)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        sample(_lib.UINT64_MAX)
+        track(mean, cov)
+    return graph, xs, (smp, mean, cov)
+
+
 class SampledTracker(Tracker):
     """Tracker with Monte-Carlo dropout: each frame's S dropout draws weigh its pose in the pose graph, and every
     tracked pose comes with a covariance.
@@ -773,27 +809,14 @@ class SampledTracker(Tracker):
         graphs = self._now_graphs if now else self._graphs
         g = graphs.get((B, H, W))
         if g is None:
-            loc, pr, L = self.loc, self.loc.predictor, _lib.lib()
-            dev, h, S = pr.device, self._handle(), self.S
-            eng, pre = pr._engine(*loc._resized(H, W)), loc._plan(H, W)
+            dev, h, L = self.loc.predictor.device, self._handle(), _lib.lib()
             f64 = dict(dtype=torch.float64, device=dev)
-            xs = torch.empty((B, H, W, 3), dtype=torch.uint8, device=dev)
-            xs.copy_(fb)
             vs = torch.zeros((B, 6), dtype=torch.float32, device=dev)
-            smp = torch.empty((B, S, 6), dtype=torch.float32, device=dev)
-            mean, cov = torch.empty((B, 6), **f64), torch.empty((B, 6, 6), **f64)
             row = _lib.TRACK_SAMPLE_ROW
             out = torch.empty((B, row), **f64)
             nowb = torch.empty((B, row), **f64) if now else None
-            fp = ctypes.POINTER(ctypes.c_float)
 
-            def sample(step):
-                _lib.check(L.mapnet_infer_sample_frames(eng.h, pre, xs.data_ptr(), B, loc.mean.ctypes.data_as(fp),
-                                                        loc.std.ctypes.data_as(fp), S, pr.droprate, int(pr.seed), step,
-                                                        smp.data_ptr(), mean.data_ptr(), cov.data_ptr(),
-                                                        _lib.stream_ptr()), "mapnet_infer_sample_frames")
-
-            def track():
+            def track(mean, cov):
                 if now:
                     _lib.check(L.mapnet_track_sample_step_now(h, mean.data_ptr(), cov.data_ptr(), vs.data_ptr(), B,
                                                               out.data_ptr(), nowb.data_ptr(), _lib.stream_ptr()),
@@ -802,17 +825,8 @@ class SampledTracker(Tracker):
                     _lib.check(L.mapnet_track_sample_step(h, mean.data_ptr(), cov.data_ptr(), vs.data_ptr(), B,
                                                           out.data_ptr(), _lib.stream_ptr()), "mapnet_track_sample_step")
 
-            cur = torch.cuda.current_stream(dev)
-            side = torch.cuda.Stream(dev)
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):        # eager run first, at an explicit dropout step: no state advances
-                sample(0)
-            cur.wait_stream(side)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                sample(_lib.UINT64_MAX)
-                track()
-            g = graphs[(B, H, W)] = (graph, xs, vs, out, smp, mean, cov, nowb)   # every buffer the graph reads
+            graph, xs, draws = _sampled_capture(self.loc, self.S, fb, track)
+            g = graphs[(B, H, W)] = (graph, xs, vs, out, draws, nowb)   # every buffer the graph reads
         return g
 
     @staticmethod
@@ -841,7 +855,7 @@ class SampledTracker(Tracker):
                 self.seen += fb.shape[0]
                 outs.append(out[:n].clone())
                 if now:
-                    nows.append(g[7].clone())
+                    nows.append(g[5].clone())
         cat = lambda ts: ts[0] if len(ts) == 1 else torch.cat(ts, 0)
         return first, cat(outs), (cat(nows) if now else None)
 
@@ -948,19 +962,26 @@ class MultiTracker(Tracker):
     it."""
 
     _DESTROY = "mapnet_track_multi_destroy"
+    _API = "mapnet_track_multi"     # the handle's C calls: _API + "_create", "_flush", "_status", "_reset"
+    _ROW = 7                        # doubles per output row
 
     def __init__(self, localizer, n_streams, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0):
         super(MultiTracker, self).__init__(localizer, steps, skip, vo_fc, sax, saq, srx, srq)
         self.n_streams = _int_arg(n_streams, "n_streams", 1, _lib.MAX_TRACK_STREAMS)
         self.seen = np.zeros(self.n_streams, dtype=np.int64)    # frames of each stream's sequence, mirrored on the device
 
+    @staticmethod
+    def _est(rows):
+        """what a caller gets for output rows [n, _ROW]: pose7 itself"""
+        return rows
+
     def _handle(self):
         if not self.h:
             pr = self.loc.predictor
             sig = (ctypes.c_double * 4)(*self.sigmas)
-            _lib.check(_lib.lib().mapnet_track_multi_create(ctypes.byref(self.h), self.n_streams, self.steps, self.skip,
-                                                            int(self.vo_fc), pr.max_batch, sig, self.loc._m,
-                                                            self.loc._s), "mapnet_track_multi_create")
+            _lib.check(getattr(_lib.lib(), self._API + "_create")(ctypes.byref(self.h), self.n_streams, self.steps,
+                                                                  self.skip, int(self.vo_fc), pr.max_batch, sig,
+                                                                  self.loc._m, self.loc._s), self._API + "_create")
         return self.h
 
     def _stream_ids(self, streams, B, single):
@@ -1050,18 +1071,18 @@ class MultiTracker(Tracker):
         first = _first_pending(int(self.seen[s]), self.lag)
         n, failed = int(self.seen[s]) - first, ctypes.c_int(0)
         with torch.cuda.device(pr.device):
-            out = torch.empty((max(self.lag, 1), 7), dtype=torch.float64, device=pr.device)
+            out = torch.empty((max(self.lag, 1), self._ROW), dtype=torch.float64, device=pr.device)
             if self.h:
                 L = _lib.lib()
-                _lib.check(L.mapnet_track_multi_flush(self.h, s, out.data_ptr(), _lib.stream_ptr()),
-                           "mapnet_track_multi_flush")
-                _lib.check(L.mapnet_track_multi_status(self.h, s, None, ctypes.byref(failed), _lib.stream_ptr()),
-                           "mapnet_track_multi_status")
+                _lib.check(getattr(L, self._API + "_flush")(self.h, s, out.data_ptr(), _lib.stream_ptr()),
+                           self._API + "_flush")
+                _lib.check(getattr(L, self._API + "_status")(self.h, s, None, ctypes.byref(failed), _lib.stream_ptr()),
+                           self._API + "_status")
         self.reset(s)
         if failed.value:
             raise np.linalg.LinAlgError("pose graph: the normal matrix of a window of stream %d's sequence is not "
                                         "positive definite" % s)
-        return first, out[:n]
+        return first, self._est(out[:n])
 
     def reset(self, s=None):
         """Start a new sequence on stream s, or on every stream when s is None (stream-ordered)."""
@@ -1069,11 +1090,84 @@ class MultiTracker(Tracker):
         s = -1 if s is None else _int_arg(s, "stream", 0, self.n_streams - 1)
         if self.h:
             with torch.cuda.device(self.loc.predictor.device):
-                _lib.check(_lib.lib().mapnet_track_multi_reset(self.h, s, _lib.stream_ptr()), "mapnet_track_multi_reset")
+                _lib.check(getattr(_lib.lib(), self._API + "_reset")(self.h, s, _lib.stream_ptr()),
+                           self._API + "_reset")
         if s < 0:
             self.seen[:] = 0
         else:
             self.seen[s] = 0
+
+
+class SampledMultiTracker(MultiTracker):
+    """MultiTracker with Monte-Carlo dropout: n_streams camera streams share one Localizer, each frame's S dropout
+    draws weigh its pose in its stream's pose graph, and every tracked pose comes with a covariance.
+
+        smt = SampledMultiTracker(loc, S=32, n_streams=64, steps=7, skip=10, vo_fc=True, sax=1e-4, saq=1e-4, srx=20,
+                                  srq=20)
+        sid, fid, est = smt(frames, vo_poses, streams)  # est = dict(pose7 [n,7], cov [n,6,6], t_std [n], q_std_deg [n])
+        now, sid, fid, est = smt.step(frames, vo_poses, streams)    # now: the same dict, one zero-lag row per frame
+        first, est = smt.flush(s)       # stream s alone: its last min(lag, seen[s]) frames; starts a new sequence
+        smt.reset(); smt.reset(s); smt.seen; smt.lag; smt.close()
+
+    Frames, VO poses, stream ids, the rows a call returns and their order, chunking, flush and reset are MultiTracker's;
+    the factor model, sax / saq, S and the est dict are SampledTracker's.  Each stream is tracked exactly as a
+    SampledTracker of the same arguments tracks it, given the same per-frame draws: a stream's estimates are bit for
+    bit those of a SampledTracker fed that stream's frames' means and covariances in order.  They are not those of a
+    SampledTracker fed the same frames, because dropout draws a frame's masks by its row in the engine batch (and by
+    the chunk's dropout steps), and a frame's row in a batch of many streams is not its row in a one-stream batch.
+
+    A call of more than max_batch frames runs in chunks of max_batch, in order, one CUDA graph replay each, captured per
+    (B, H, W): the Localizer's sampled engine launches at the device dropout counter (S consecutive dropout steps per
+    chunk, as SampledTracker takes them), then three tracking launches (csrc/loader.cu, mapnet_track_multi_sample_*:
+    gather, k_pgo_cov, emit) for all of the chunk's streams.  The per-frame records are built on the host and copied in
+    with the frames.  The eager run before a capture uses an explicit dropout step and makes no tracking launch, so it
+    advances neither the dropout counter nor any stream.  A window whose normal matrix or one of whose frames' factor
+    covariances is not positive definite marks its own stream only: flush(s) raises np.linalg.LinAlgError for stream s
+    after resetting it."""
+
+    _DESTROY = "mapnet_track_multi_sample_destroy"
+    _API = "mapnet_track_multi_sample"
+    _ROW = _lib.TRACK_SAMPLE_ROW
+    _est = staticmethod(SampledTracker._est)
+
+    def __init__(self, localizer, S, n_streams, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0):
+        super(SampledMultiTracker, self).__init__(localizer, n_streams, steps, skip, vo_fc, sax, saq, srx, srq)
+        self.S = _check_draws(S, localizer.predictor.droprate)
+
+    def _graph(self, fb, now=False):
+        B, H, W = fb.shape[:3]
+        graphs = self._now_graphs if now else self._graphs
+        g = graphs.get((B, H, W))
+        if g is None:
+            dev, h, L = self.loc.predictor.device, self._handle(), _lib.lib()
+            f64 = dict(dtype=torch.float64, device=dev)
+            vs = torch.zeros((B, 6), dtype=torch.float32, device=dev)
+            rs = torch.zeros((B, 6), dtype=torch.int32, device=dev)
+            out = torch.empty((B, self._ROW), **f64)
+            nowb = torch.empty((B, self._ROW), **f64) if now else None
+
+            def track(mean, cov):
+                _lib.check(L.mapnet_track_multi_sample_step(h, mean.data_ptr(), cov.data_ptr(), vs.data_ptr(),
+                                                            rs.data_ptr(), B, out.data_ptr(),
+                                                            nowb.data_ptr() if now else None, _lib.stream_ptr()),
+                           "mapnet_track_multi_sample_step")
+
+            graph, xs, draws = _sampled_capture(self.loc, self.S, fb, track)
+            g = graphs[(B, H, W)] = (graph, xs, vs, rs, out, draws, nowb)     # MultiTracker._run's layout
+        return g
+
+    @torch.no_grad()
+    def __call__(self, frames, vo_poses, streams):
+        """-> (sid int64 [n], fid int64 [n], est): the windows this call completes (MultiTracker.__call__)"""
+        sid, fid, rows, _ = self._run(frames, vo_poses, streams, False)
+        return sid, fid, self._est(rows)
+
+    @torch.no_grad()
+    def step(self, frames, vo_poses, streams):
+        """-> (now, sid, fid, est): now holds each given frame's zero-lag estimate, one row per frame in the order
+        given (MultiTracker.step's windows); (sid, fid, est) is what __call__ returns"""
+        sid, fid, rows, nows = self._run(frames, vo_poses, streams, True)
+        return self._est(nows), sid, fid, self._est(rows)
 
 
 def pgo(pred7, vos7, sax=1.0, saq=1.0, srx=1.0, srq=1.0, fc_vos=False):

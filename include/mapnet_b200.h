@@ -348,6 +348,40 @@ int mapnet_track_sample_destroy(mapnet_track_sample_t* h);
 int mapnet_test_sample_factor(const double* mean6, const double* cov36, int64_t n, double sax, double saq, double* p7,
                               double* s7, void* stream);
 
+/* ---- multi-stream Monte-Carlo tracker (csrc/loader.cu; geomapnet_b200.inference.SampledMultiTracker): n_streams
+ * independent sequences, each tracked exactly as a mapnet_track_sample_t of the same arguments would track it, with one
+ * set of launches per call for all of them.  Stream s's rows (out, now and flushes) are bit for bit those of a
+ * mapnet_track_sample_t of the same arguments fed stream s's rows in order.
+ *   mapnet_track_multi_sample_create: mapnet_track_multi_create's arguments and checks (sigmas4 as
+ *     mapnet_track_sample_create reads them).  Per stream a frame count, a status word and rings of
+ *     R = max_batch + (T-1)*skip frames of p7 (float64), S7 (float64 [7][7]) and VO poses (float32), R x 472 bytes;
+ *     the error of a failed allocation states its total bytes.
+ *   mapnet_track_multi_sample_step: B frames of any streams (1 <= B <= max_batch): mean6 [B][6], cov36 [B][6][6]
+ *     float64 and vo6 [B][6] float32 as mapnet_track_sample_step takes them, rec [B][6] int32 as mapnet_track_multi_step
+ *     takes it.  out [n][45] (room for B rows) gets the row of 45 doubles of mapnet_track_sample_step for each
+ *     completed window, in the order of mapnet_track_multi_step's out7; with now (may be NULL) [B][45] also the
+ *     zero-lag row of frame b (mapnet_track_sample_step_now's) in row b.  Three launches (gather, k_pgo_cov, emit),
+ *     graph-capturable, nothing read back.  A record whose stream is outside [0, n_streams) is skipped.
+ *   mapnet_track_multi_sample_flush: mapnet_track_sample_flush of stream s alone (0 <= s < n_streams), into out (room
+ *     for lag rows).  Three launches (none when lag = 0).
+ *   mapnet_track_multi_sample_reset: stream-ordered: stream s (or every stream when s = -1) starts a new sequence at
+ *     frame 0 and its status word is cleared.
+ *   mapnet_track_multi_sample_status: synchronises the stream and returns stream s's frames seen and status (1: a
+ *     window of s had a normal matrix or a frame's S7 that was not positive definite; other streams are not marked).
+ * Pointers are device memory unless marked HOST.  Argument errors return non-zero before any launch. */
+typedef struct mapnet_track_multi_sample mapnet_track_multi_sample_t;
+int mapnet_track_multi_sample_create(mapnet_track_multi_sample_t** out, int n_streams, int T, int skip, int fc_vos,
+                                     int max_batch, const double* sigmas4, const double* pose_m3,
+                                     const double* pose_s3);
+int mapnet_track_multi_sample_step(mapnet_track_multi_sample_t* h, const double* mean6, const double* cov36,
+                                   const float* vo6, const int32_t* rec, int B, double* out, double* now,
+                                   void* stream);
+int mapnet_track_multi_sample_flush(mapnet_track_multi_sample_t* h, int s, double* out, void* stream);
+int mapnet_track_multi_sample_reset(mapnet_track_multi_sample_t* h, int s, void* stream);
+int mapnet_track_multi_sample_status(mapnet_track_multi_sample_t* h, int s, int64_t* frames_seen, int* failed,
+                                     void* stream);
+int mapnet_track_multi_sample_destroy(mapnet_track_multi_sample_t* h);
+
 /* ---- eval-mode inference engine (csrc/infer.cu): a frozen snapshot of a PoseNet / MapNet trunk for
  * scripts/eval.py-style prediction.  mapnet_infer_load copies the weights (packed fprop operands only), the eval-mode
  * BatchNorm scale / shift (computed from the running statistics exactly as mapnet_forward(training = 0) does) and the
