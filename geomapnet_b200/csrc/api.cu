@@ -910,6 +910,88 @@ int mapnet_test_head(int B, int F, const float* feat, const float* params, float
   return r;
 }
 
+// The weight-pack table of a parameter-table-only trunk in one precision; fp8 uses the bf16 table, as InferNet::init.
+// im2col_stem: the tensor-core modes' fallback stem layout (the CUDA-core modes always have it; the fp8 engine never).
+static int pack_spec(Net* spec, int H, int W, int precision, int im2col_stem, const char* what) {
+  MN_CHECK(precision >= PREC_FP32 && precision <= PREC_FP8, "%s: precision %d outside [0, 4]", what, precision);
+  MN_CHECK(im2col_stem == 0 || im2col_stem == 1, "%s: im2col_stem %d is not 0 or 1", what, im2col_stem);
+  MN_CHECK(!(im2col_stem && precision == PREC_FP8), "%s: the fp8 engine has no im2col stem", what);
+  return spec->init(0, H, W, 2048, precision == PREC_FP8 ? PREC_BF16_TC : precision, im2col_stem);
+}
+
+int mapnet_test_weight_table(int H, int W, int precision, int im2col_stem, int64_t* out, int cap) {
+  MN_CHECK(out != nullptr, "test_weight_table: null out pointer");
+  Net* spec = new Net();
+  int r = pack_spec(spec, H, W, precision, im2col_stem, "test_weight_table");
+  const int n = (int)spec->convs.size();
+  if (r == 0 && cap < 2 + 9 * n) {
+    set_last_error("test_weight_table: cap %d < %d (2 + 9 per conv)", cap, 2 + 9 * n);
+    r = 2;
+  }
+  if (r == 0) {
+    out[0] = n;
+    out[1] = spec->wk_total;
+    for (int i = 0; i < n; ++i) {
+      const WeightDesc& d = spec->convs[i].wd;
+      const int64_t row[9] = {d.p_off, d.k_off, d.Co, d.Ci, d.Ci_real, d.KH, d.KW, d.im2col_k, d.s2d};
+      for (int k = 0; k < 9; ++k) out[2 + 9 * i + k] = row[k];
+    }
+  }
+  spec->destroy();
+  delete spec;
+  return r;
+}
+
+// The production pack of one precision: Net::forward_t's (fp32, bf16_simt, bf16, tc_split with its dgrad planes) or
+// InferNet::load's fp8 pair, over the descriptors of a parameter-table-only trunk.
+int mapnet_test_pack_weights(int precision, int im2col_stem, int H, int W, const float* params_flat, void* krsc_out, void* dg_out,
+                             float* s_w_out, void* stream) {
+  MN_CHECK(params_flat && krsc_out && dg_out, "test_pack_weights: null argument");
+  MN_CHECK((s_w_out != nullptr) == (precision == PREC_FP8), "test_pack_weights: s_w_out is given exactly for fp8 "
+           "(precision %d)", precision);
+  Net* spec = new Net();
+  int r = pack_spec(spec, H, W, precision, im2col_stem, "test_pack_weights");
+  WeightDesc* d_wd = nullptr;
+  float* f32 = nullptr;
+  auto body = [&]() -> int {
+    MN_TRY(require_device());
+    for (const void* p : {(const void*)params_flat, (const void*)krsc_out, (const void*)dg_out, (const void*)s_w_out}) {
+      if (p == nullptr) continue;
+      cudaPointerAttributes at;
+      MN_CUDA(cudaPointerGetAttributes(&at, p));
+      MN_CHECK(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged,
+               "test_pack_weights: params_flat and the outputs must be device memory");
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    const int nconv = (int)spec->convs.size();
+    const long long wk = spec->wk_total;
+    std::vector<WeightDesc> wd;
+    for (auto& c : spec->convs) wd.push_back(c.wd);
+    MN_CUDA(cudaMalloc((void**)&d_wd, wd.size() * sizeof(WeightDesc)));
+    MN_CUDA(cudaMemcpy(d_wd, wd.data(), wd.size() * sizeof(WeightDesc), cudaMemcpyHostToDevice));
+    if (precision == PREC_FP32 || precision == PREC_BF16_SIMT) {
+      MN_TRY(launch_pack_weights<float>(d_wd, nconv, params_flat, (float*)krsc_out, (float*)dg_out, spec->max_w_elems,
+                                        precision == PREC_BF16_SIMT, st));
+    } else if (precision == PREC_BF16_TC) {
+      MN_TRY(launch_pack_weights<bf16>(d_wd, nconv, params_flat, (bf16*)krsc_out, (bf16*)dg_out, spec->max_w_elems, 0, st));
+    } else if (precision == PREC_TC_SPLIT) {
+      MN_CUDA(cudaMalloc((void**)&f32, (size_t)wk * 2 * sizeof(float)));     // the fp32 K-major matrices (Net's w_*_f32)
+      MN_TRY(launch_pack_weights_split(d_wd, nconv, params_flat, f32, f32 + wk, krsc_out, dg_out, spec->max_w_elems, st));
+    } else {
+      MN_TRY(launch_pack_weights<bf16>(d_wd, 1, params_flat, (bf16*)dg_out, nullptr, spec->max_w_elems, 0, st));
+      MN_TRY(launch_pack_weights_fp8(d_wd, nconv, params_flat, (uint8_t*)krsc_out, s_w_out, st));
+    }
+    MN_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  };
+  if (r == 0) r = body();
+  cudaFree(f32);
+  cudaFree(d_wd);
+  spec->destroy();
+  delete spec;
+  return r;
+}
+
 // The stem operand of the inference engine from one of its two sources: uint8 frames through pre (the fused vertical
 // pass), or float32 images of pre's output size through k_stem_s2d (what mapnet_infer_forward writes).
 int mapnet_test_stem_operand(int precision, mapnet_preprocess_t* pre, const void* frames_nhwc_u8, const float* x_nchw,

@@ -140,7 +140,7 @@ void Net::build_table() {
   wpqr_b = table[add("fc_wpqr.bias", 0, {3})].offset;
 }
 
-int Net::init(int max_B_, int H_, int W_, int feat_dim_, int precision_) {
+int Net::init(int max_B_, int H_, int W_, int feat_dim_, int precision_, int im2col_stem) {
   max_B = max_B_; H = H_; W = W_; feat_dim = feat_dim_; precision = precision_;
   MN_CHECK(max_B >= 0 && H >= 32 && W >= 32, "create: need max_B>=0 and H,W>=32 (got %d,%d,%d)", max_B, H, W);
   MN_CHECK(precision >= 0 && precision <= 3, "create: bad precision %d", precision);
@@ -149,7 +149,7 @@ int Net::init(int max_B_, int H_, int W_, int feat_dim_, int precision_) {
   bwd_pre = false; bwd_next_part = 0;
   side = nullptr; ring_pos = 0; cur_grads = nullptr; dw_stem_elems = 0;
   for (int i = 0; i < 4; ++i) { ring[i] = nullptr; ring_ready[i] = ring_done[i] = nullptr; ring_pending[i] = false; }
-  stem_s2d = tc() && (max_B == 0 || tc_overlapped_view_supported());
+  stem_s2d = !im2col_stem && tc() && (max_B == 0 || tc_overlapped_view_supported());
   Hc = conv_out(H, 7, 2, 3); Wc = conv_out(W, 7, 2, 3);        // (build_table sets them again)
   stem_fuse = (Hc % 2 == 0) && (Wc % 2 == 0);
   { const char* e = getenv("MAPNET_TC_FUSE_BWD"); fuse_bwd = (precision == PREC_BF16_TC) && (e ? atoi(e) != 0 : 1); }

@@ -140,7 +140,9 @@ struct Net {
   size_t elt() const { return (precision == PREC_FP32 || precision == PREC_TC_SPLIT) ? 4 : 2; }
   bool tc() const { return precision == PREC_BF16_TC || precision == PREC_TC_SPLIT; }
 
-  int init(int max_B, int H, int W, int feat_dim, int precision);
+  // im2col_stem: the tensor-core modes' fallback stem (patch matrix instead of the space-to-depth view), as init picks
+  // it when the driver rejects overlapped tensor maps -- set by the pack tests so that layout is checked on any driver
+  int init(int max_B, int H, int W, int feat_dim, int precision, int im2col_stem = 0);
   void destroy();
   int forward(const float* x, const float* params, float* bufs, int B, int training, float droprate,
               unsigned long long seed, unsigned long long step, float* pred, cudaStream_t st);

@@ -576,6 +576,27 @@ int mapnet_test_head(int B, int F, const float* feat, const float* params, float
                      const float* dpred, int filter_nans, float* dh, float* dfeat, float* grads, float* scale2,
                      void* stream);
 
+/* host-only: the weight-pack table of the trunk of an H x W frame in one precision (MAPNET_PREC_FP32 ..
+ * MAPNET_PREC_FP8; the fp8 engine's table is the bf16 one, as mapnet_infer_create builds it), from a parameter-table-only
+ * trunk (max_B = 0).  im2col_stem = 1: the stem as the tensor-core training modes lay it out when the driver rejects
+ * overlapped tensor maps (the im2col row of 192; the CUDA-core modes always use it, fp8 never: an error there).  out [cap] int64: out[0] = number of convs n, out[1] = wk_total (packed elements of every conv,
+ * each conv's matrix 512-element aligned), then per conv i at out[2 + 9 i]: p_off, k_off, Co, Ci, Ci_real, KH, KW,
+ * im2col_k, s2d (the stem's K order: im2col_k > 0 and s2d = 1 for the space-to-depth row).  Needs cap >= 2 + 9 n. */
+int mapnet_test_weight_table(int H, int W, int precision, int im2col_stem, int64_t* out, int cap);
+/* the whole-network weight pack of one precision (im2col_stem as for mapnet_test_weight_table), the launches the training step (forward) or mapnet_infer_load runs,
+ * from params_flat (device, the trunk's parameter buffer) into caller-owned device buffers laid out by the table of
+ * mapnet_test_weight_table (conv i at element k_off):
+ *   fp32 / bf16_simt: fp32 krsc_out and dg_out [wk_total] (bf16_simt: values rounded to bf16);
+ *   bf16:             bf16 krsc_out and dg_out [wk_total];
+ *   tc_split:         fp16 hi / lo planes, uint16 krsc_out and dg_out [4 wk_total] (element offset 4 k_off);
+ *   fp8:              e4m3 krsc_out [wk_total] bytes (every conv but the stem), the stem's bf16 row matrix in dg_out
+ *                     [k_off of conv 1] (the fp8 engine has no dgrad operand) and s_w_out [n * 512] floats, conv i's
+ *                     output channel co at i * 512 + co.
+ * The stem has no dgrad operand: its dg_out range is not written.  s_w_out is given exactly for fp8.  Arguments are
+ * checked before the device is touched; the call returns after the launches complete. */
+int mapnet_test_pack_weights(int precision, int im2col_stem, int H, int W, const float* params_flat, void* krsc_out,
+                             void* dg_out, float* s_w_out, void* stream);
+
 /* micro-benchmark of one tensor-core conv configuration (tools/bench_conv.py): average ms per launch */
 int mapnet_bench_conv(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* in0,
                       const void* in1, const void* wmat, void* out, int iters, float* host_ms);
