@@ -106,70 +106,39 @@ k_eval_windows(const float* __restrict__ pred6, const float* __restrict__ poses,
 }
 
 // ---- streaming pose-graph tracker (mapnet_track_*, inference.Tracker): eval.py's windows over frames as they arrive.
-// Device state of one sequence: `seen` frames so far; n_win: the windows the current call completes, written by
-// k_track_gather for k_pgo and k_track_emit; status: 1 once a window's normal matrix was not positive definite.
+// Device state of one sequence (one per stream of a multi-stream tracker): `seen` frames so far; status: 1 once a
+// window's normal matrix was not positive definite.  The count of windows the current call solves sits apart, with the
+// per-window failure flags of a multi-stream call: written by the gather for the PGO launch and the emit.
 struct TrackDev {
   long long seen;
-  int n_win, status;
+  int status, pad;
+};
+
+// what a tracker handle is created with: window geometry, PGO weights, pose statistics (single and multi-stream)
+struct TrackCfg {
+  int T, skip, fc, max_batch, E, max_win;   // max_win: the most windows one call completes, max(max_batch, lag)
+  long long R, lag;
+  double w4[4];                             // PGO weights 1/sqrt(sigma) of sax, saq, srx, srq
+  int un;
+  double m[3], s[3];
+};
+
+// the device state of every tracker handle: n_streams sequences (1 for the single-stream trackers), their rings of R
+// frames and the windows of one call.  The sampled trackers' buffers (ring49, win49, cov36) are null for point factors.
+struct TrackHandle : TrackCfg {
+  int n_streams;
+  double sax, saq;                          // the floors of the absolute factors' covariances (sampled)
+  TrackDev* st;                             // [n_streams]
+  int* n_win;                               // the windows of the current call, written by the gather
+  int* win_fail;                            // [max_win]: the PGO's per-window failure flags (multi-stream)
+  double *ring7, *ring49;                   // [n_streams][R][7], [n_streams][R][7][7]: p and S7 of the last R frames
+  float* ring_vo;                           // [n_streams][R][6]: their VO-library poses
+  double *win7, *win49, *vos7, *opt7, *cov36;   // [max_win][T][7], [.][T][49], [.][E][7], [.][T][7], [.][T][36]
 };
 
 __device__ __forceinline__ const float* track_src(const float* fresh, const float* ring, long long f, long long seen,
                                                   long long R) {
   return f >= seen ? fresh + 6 * (f - seen) : ring + 6 * (f % R);
-}
-
-// One thread per row: the n new frames into the rings (pose7 of pred6, the VO-library pose as given), then slot
-// (w, k) of every completed window w < n_win (rows n .. n + max_win*T - 1), then VO (w, e) (the next max_win*E rows).
-// A slot's frame comes from this call's inputs when it is new, else from the ring: R = max_batch + (T-1)*skip frames
-// hold every older frame a window of this call reaches, none of them in a ring slot this call writes.  The values are
-// k_eval_windows': st_pose7 of the float32 pose, calc_vo_logq_safe of the float32 VO-library poses.  A zero-lag call
-// (now) gathers the n windows that end at its frames instead, from centre now_first(seen); st->n_win is the count of
-// completed windows either way.
-__global__ void __launch_bounds__(128)
-k_track_gather(const float* __restrict__ pred6, const float* __restrict__ vo6, int n, int flush, int now,
-               TrackDev* __restrict__ st, double* __restrict__ ring7, float* __restrict__ ring_vo, long long R, int T,
-               int skip, int fc, int max_win, double* __restrict__ win7, double* __restrict__ vos7) {
-  pdl_prologue();
-  const long long seen = st->seen, total = seen + n, lag = trackcore::lag(T, skip);
-  const long long pending = trackcore::first_pending(seen, lag);
-  const int n_done = (int)((flush ? total : trackcore::first_pending(total, lag)) - pending);
-  const long long first = now ? trackcore::now_first(seen, lag) : pending;
-  const int n_win = now ? n : n_done;
-  const int E = fc ? T * (T - 1) / 2 : T - 1;
-  long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r == 0) st->n_win = n_done;
-  if (r < n) {
-    const long long f = seen + r;
-    st_pose7(pred6 + 6 * r, ring7 + 7 * (f % R));
-#pragma unroll
-    for (int c = 0; c < 6; ++c) ring_vo[6 * (f % R) + c] = vo6[6 * r + c];
-    return;
-  }
-  r -= n;
-  if (r < (long long)max_win * T) {
-    const int w = (int)(r / T), k = (int)(r % T);
-    if (w >= n_win) return;
-    const long long f = trackcore::slot_frame(first + w, k, T, skip, total - 1);
-    if (f >= seen) st_pose7(pred6 + 6 * (f - seen), win7 + 7 * r);
-    else {
-#pragma unroll
-      for (int c = 0; c < 7; ++c) win7[7 * r + c] = ring7[7 * (f % R) + c];
-    }
-    return;
-  }
-  r -= (long long)max_win * T;
-  if (r < (long long)max_win * E) {
-    const int w = (int)(r / E), e = (int)(r % E);
-    if (w >= n_win) return;
-    int i, j;
-    trackcore::vo_pair(e, T, fc, &i, &j);
-    const long long fa = trackcore::slot_frame(first + w, i, T, skip, total - 1);
-    const long long fb = trackcore::slot_frame(first + w, j, T, skip, total - 1);
-    const posemath::Pose6 v = posemath::calc_vo_logq_safe(ld_pose6(track_src(vo6, ring_vo, fa, seen, R)),
-                                                          ld_pose6(track_src(vo6, ring_vo, fb, seen, R)));
-    const float v6[6] = {v.t.x, v.t.y, v.t.z, v.l.x, v.l.y, v.l.z};
-    st_pose7(v6, vos7 + 7 * r);
-  }
 }
 
 __device__ __forceinline__ void track_emit_pose(const double* p, int un, const double ms[3], const double ss[3],
@@ -180,34 +149,10 @@ __device__ __forceinline__ void track_emit_pose(const double* p, int un, const d
   for (int k = 3; k < 7; ++k) o[k] = p[k];
 }
 
-// One thread per completed window: its optimised middle slot, translations un-normalised as _window_errors does
-// (un = 0: kept), into out7 row w; thread 0 advances the frame counter by the call's n frames.  With now7 (a zero-lag
-// call: n windows, the last n_win of them completed) thread w also writes window w's last slot into now7 row w, and the
-// completed window n - n_win + j feeds out7 row j.
-__global__ void __launch_bounds__(128)
-k_track_emit(const double* __restrict__ opt7, TrackDev* __restrict__ st, int n, int T, int un, double m0,
-             double m1, double m2, double s0, double s1, double s2, double* __restrict__ out7,
-             double* __restrict__ now7) {
-  pdl_prologue();
-  const int w = blockIdx.x * blockDim.x + threadIdx.x;
-  const int n_win = st->n_win;
-  if (w == 0) st->seen += n;
-  const double ms[3] = {m0, m1, m2}, ss[3] = {s0, s1, s2};
-  const double* win = opt7 + 7LL * w * T;
-  if (now7 == nullptr) {
-    if (w < n_win) track_emit_pose(win + 7 * (T / 2), un, ms, ss, out7 + 7LL * w);
-    return;
-  }
-  if (w >= n) return;
-  track_emit_pose(win + 7 * (T - 1), un, ms, ss, now7 + 7LL * w);
-  const int lead = n - n_win;
-  if (w >= lead) track_emit_pose(win + 7 * (T / 2), un, ms, ss, out7 + 7LL * (w - lead));
-}
-
 // ---- Monte-Carlo tracker (mapnet_track_sample_*, inference.SampledTracker): mapnet_track_*'s windows, with each
 // frame's S-draw mean (t, log q) and covariance Sigma [6][6] (float64, mapnet_infer_sample_frames' outputs) in place of
 // its one draw.  A new frame's absolute pose p = (mean_t, qexp(mean_v)) (k_sample_post's qexp) and its factor covariance
-// S7 = A Sigma A' + diag(sax I3, saq I4), A = blockdiag(I3, E(mean_v)), are formed once, into rings of R frames; the
+// S7 = A Sigma A' + diag(sax I3, saq I4), A = blockdiag(I3, E(mean_v)), are formed into rings of R frames; the
 // windows gather them, k_pgo_cov solves them, and the emit writes per window row pose7 [7], cov [36] = D cov D,
 // t_std, q_std_deg (k_sample_post's statistics), kTrackSampleRow doubles.
 static constexpr int kTrackSampleRow = 45;
@@ -258,15 +203,98 @@ k_test_sample_factor(const double* __restrict__ mean, const double* __restrict__
   if (i < n) sample_factor(mean + 6 * i, cov + 36 * i, sax, saq, p7 + 7 * i, s7 + 49 * i);
 }
 
-// k_track_gather for the sampled tracker: rows 0 .. n-1 form the n new frames' p7 / S7 into the rings and into every
-// window slot of this call that holds them (each formed once); then slot (w, k) of window w < n_win for the frames
-// before this call, from the rings; then VO (w, e), as k_track_gather computes it.
+__device__ __forceinline__ void track_sample_row(const double* p7, const double* C, int un, const double ms[3],
+                                                 const double ss[3], double* o) {
+  track_emit_pose(p7, un, ms, ss, o);
+  const double d[6] = {ss[0], ss[1], ss[2], 1.0, 1.0, 1.0};
+  sample_stats(C, d, o + 7, o + 43, o + 44);
+}
+
+// ---- the factors a window slot holds: everything the point and the sampled trackers do differently.  A factor is
+// formed from input row b of a call into ring slot q or window slot q (a pure function of the row, so every copy is
+// bit for bit the ring's), copied from ring slot q into window slot r, and an optimised window slot becomes an
+// output row of kRow doubles; pgo launches the matching pose-graph optimisation of the call's windows.
+// Point factors: p7 = st_pose7 of the engine's float32 (t, log q); k_pgo.
+struct PointFactor {
+  static constexpr int kRow = 7;
+  const float* pred6;                       // [B][6], null for a flush
+  double *ring7, *win7;
+  const double* opt7;
+
+  PointFactor(const TrackHandle& h, const float* pred6_)
+      : pred6(pred6_), ring7(h.ring7), win7(h.win7), opt7(h.opt7) {}
+  __device__ __forceinline__ void form(long long b, bool ring, long long q) const {
+    st_pose7(pred6 + 6 * b, (ring ? ring7 : win7) + 7 * q);
+  }
+  __device__ __forceinline__ void nan_slot(long long r) const {
+    const float nan = __int_as_float(0x7fc00000);
+    const float v6[6] = {nan, nan, nan, nan, nan, nan};
+    st_pose7(v6, win7 + 7 * r);
+  }
+  __device__ __forceinline__ void copy(long long q, long long r) const {
+#pragma unroll
+    for (int c = 0; c < 7; ++c) win7[7 * r + c] = ring7[7 * q + c];
+  }
+  __device__ __forceinline__ void row(long long k, int un, const double ms[3], const double ss[3], double* o) const {
+    track_emit_pose(opt7 + 7 * k, un, ms, ss, o);
+  }
+  int pgo(const TrackHandle& h, int nw, int* status, const int* n_win_dev, int* win_fail, cudaStream_t st) const {
+    return launch_pgo(h.win7, h.vos7, h.opt7, nw, h.T, h.fc, h.w4, 10, 0, status, n_win_dev, st, win_fail);
+  }
+};
+
+// Sampled factors: p7 and S7 = sample_factor of the frame's float64 mean [6] and covariance [36]; k_pgo_cov, whose
+// posterior cov36 the output rows carry.
+struct SampleFactor {
+  static constexpr int kRow = kTrackSampleRow;
+  const double *mean, *cov;                 // [B][6], [B][36], null for a flush
+  double sax, saq;
+  double *ring7, *ring49, *win7, *win49;
+  const double *opt7, *cov36;
+
+  SampleFactor(const TrackHandle& h, const double* mean_, const double* cov_)
+      : mean(mean_), cov(cov_), sax(h.sax), saq(h.saq), ring7(h.ring7), ring49(h.ring49), win7(h.win7),
+        win49(h.win49), opt7(h.opt7), cov36(h.cov36) {}
+  // the frame's mean and covariance through the read-only path into registers first: the struct's pointers carry no
+  // restrict, so sample_factor reading them in place would reload the covariance after every store of S7
+  __device__ __forceinline__ void form(long long b, bool ring, long long q) const {
+    double mu[6], C[36];
+#pragma unroll
+    for (int c = 0; c < 6; ++c) mu[c] = __ldg(mean + 6 * b + c);
+#pragma unroll
+    for (int c = 0; c < 36; ++c) C[c] = __ldg(cov + 36 * b + c);
+    sample_factor(mu, C, sax, saq, (ring ? ring7 : win7) + 7 * q, (ring ? ring49 : win49) + 49 * q);
+  }
+  __device__ __forceinline__ void nan_slot(long long r) const {
+    const double nan = __longlong_as_double(0x7ff8000000000000LL);
+    for (int c = 0; c < 7; ++c) win7[7 * r + c] = nan;
+    for (int c = 0; c < 49; ++c) win49[49 * r + c] = nan;
+  }
+  __device__ __forceinline__ void copy(long long q, long long r) const {
+    for (int c = 0; c < 7; ++c) win7[7 * r + c] = ring7[7 * q + c];
+    for (int c = 0; c < 49; ++c) win49[49 * r + c] = ring49[49 * q + c];
+  }
+  __device__ __forceinline__ void row(long long k, int un, const double ms[3], const double ss[3], double* o) const {
+    track_sample_row(opt7 + 7 * k, cov36 + 36 * k, un, ms, ss, o);
+  }
+  int pgo(const TrackHandle& h, int nw, int* status, const int* n_win_dev, int* win_fail, cudaStream_t st) const {
+    return launch_pgo_cov(h.win7, h.win49, h.vos7, h.opt7, h.cov36, nw, h.T, h.fc, h.w4[2], h.w4[3], 10, status,
+                          n_win_dev, win_fail, st);
+  }
+};
+
+// One thread per row: the n new frames into the rings (their factors, the VO-library pose as given), then slot
+// (w, k) of every completed window w < n_win (rows n .. n + max_win*T - 1), then VO (w, e) (the next max_win*E rows).
+// A slot's frame comes from this call's inputs when it is new, else from the ring: R = max_batch + (T-1)*skip frames
+// hold every older frame a window of this call reaches, none of them in a ring slot this call writes.  The values are
+// k_eval_windows': the frame's factor (st_pose7 of the float32 pose for point factors), calc_vo_logq_safe of the
+// float32 VO-library poses.  A zero-lag call (now) gathers the n windows that end at its frames instead, from centre
+// now_first(seen); *n_win_dev is the count of completed windows either way.
+template <class F>
 __global__ void __launch_bounds__(128)
-k_track_sample_gather(const double* __restrict__ mean, const double* __restrict__ cov, const float* __restrict__ vo6,
-                      int n, int flush, int now, TrackDev* __restrict__ st, double* __restrict__ ring7,
-                      double* __restrict__ ring49, float* __restrict__ ring_vo, long long R, int T, int skip, int fc,
-                      int max_win, double sax, double saq, double* __restrict__ win7, double* __restrict__ win49,
-                      double* __restrict__ vos7) {
+k_track_gather(F fac, const float* __restrict__ vo6, int n, int flush, int now, const TrackDev* __restrict__ st,
+               int* __restrict__ n_win_dev, float* __restrict__ ring_vo, long long R, int T, int skip, int fc,
+               int max_win, double* __restrict__ vos7) {
   pdl_prologue();
   const long long seen = st->seen, total = seen + n, lag = trackcore::lag(T, skip);
   const long long pending = trackcore::first_pending(seen, lag);
@@ -275,37 +303,25 @@ k_track_sample_gather(const double* __restrict__ mean, const double* __restrict_
   const int n_win = now ? n : n_done;
   const int E = fc ? T * (T - 1) / 2 : T - 1;
   long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r == 0) st->n_win = n_done;
-  if (r < n) {
-    const long long f = seen + r, q = f % R;
-    double p7[7], S7[49];
-    sample_factor(mean + 6 * r, cov + 36 * r, sax, saq, p7, S7);
-    for (int c = 0; c < 7; ++c) ring7[7 * q + c] = p7[c];
-    for (int c = 0; c < 49; ++c) ring49[49 * q + c] = S7[c];
+  if (r == 0) *n_win_dev = n_done;
+  // the input row b whose factor this thread forms into ring slot q (a new frame) or window slot q: one call site,
+  // so the threads of a warp that form a frame's ring copy and its window copies run the formation together
+  const bool ring = r < n;
+  long long b, q;
+  if (ring) {
+    b = r; q = (seen + r) % R;
 #pragma unroll
     for (int c = 0; c < 6; ++c) ring_vo[6 * q + c] = vo6[6 * r + c];
-    for (int w = 0; w < n_win; ++w)
-      for (int k = 0; k < T; ++k) {
-        if (trackcore::slot_frame(first + w, k, T, skip, total - 1) != f) continue;
-        const long long s = (long long)w * T + k;
-        for (int c = 0; c < 7; ++c) win7[7 * s + c] = p7[c];
-        for (int c = 0; c < 49; ++c) win49[49 * s + c] = S7[c];
-      }
-    return;
-  }
-  r -= n;
-  if (r < (long long)max_win * T) {
+  } else if (r - n < (long long)max_win * T) {
+    r -= n;
     const int w = (int)(r / T), k = (int)(r % T);
     if (w >= n_win) return;
     const long long f = trackcore::slot_frame(first + w, k, T, skip, total - 1);
-    if (f >= seen) return;                 // a new frame: written by its own row
-    const long long q = f % R;
-    for (int c = 0; c < 7; ++c) win7[7 * r + c] = ring7[7 * q + c];
-    for (int c = 0; c < 49; ++c) win49[49 * r + c] = ring49[49 * q + c];
-    return;
-  }
-  r -= (long long)max_win * T;
-  if (r < (long long)max_win * E) {
+    if (f < seen) { fac.copy(f % R, r); return; }
+    b = f - seen; q = r;
+  } else {
+    r -= n + (long long)max_win * T;
+    if (r >= (long long)max_win * E) return;
     const int w = (int)(r / E), e = (int)(r % E);
     if (w >= n_win) return;
     int i, j;
@@ -316,48 +332,43 @@ k_track_sample_gather(const double* __restrict__ mean, const double* __restrict_
                                                           ld_pose6(track_src(vo6, ring_vo, fb, seen, R)));
     const float v6[6] = {v.t.x, v.t.y, v.t.z, v.l.x, v.l.y, v.l.z};
     st_pose7(v6, vos7 + 7 * r);
+    return;
   }
+  fac.form(b, ring, q);
 }
 
-__device__ __forceinline__ void track_sample_row(const double* p7, const double* C, int un, const double ms[3],
-                                                 const double ss[3], double* o) {
-  track_emit_pose(p7, un, ms, ss, o);
-  const double d[6] = {ss[0], ss[1], ss[2], 1.0, 1.0, 1.0};
-  sample_stats(C, d, o + 7, o + 43, o + 44);
-}
-
-// k_track_emit for the sampled tracker: window w's middle slot into out row w (a zero-lag call: its last slot into now
-// row w, and the completed window n - n_win + j into out row j); thread 0 advances the frame counter
+// One thread per completed window: its optimised middle slot, translations un-normalised as _window_errors does
+// (un = 0: kept), into out row w; thread 0 advances the frame counter by the call's n frames.  With now (a zero-lag
+// call: n windows, the last n_win of them completed) thread w also writes window w's last slot into now row w, and the
+// completed window n - n_win + j feeds out row j.
+template <class F>
 __global__ void __launch_bounds__(128)
-k_track_sample_emit(const double* __restrict__ opt7, const double* __restrict__ cov36, TrackDev* __restrict__ st, int n,
-                    int T, int un, double m0, double m1, double m2, double s0, double s1, double s2,
-                    double* __restrict__ out, double* __restrict__ now) {
+k_track_emit(F fac, TrackDev* __restrict__ st, const int* __restrict__ n_win_dev, int n, int T, int un, double m0,
+             double m1, double m2, double s0, double s1, double s2, double* __restrict__ out,
+             double* __restrict__ now) {
   pdl_prologue();
   const int w = blockIdx.x * blockDim.x + threadIdx.x;
-  const int n_win = st->n_win;
+  const int n_win = *n_win_dev;
   if (w == 0) st->seen += n;
   const double ms[3] = {m0, m1, m2}, ss[3] = {s0, s1, s2};
   const long long mid = (long long)w * T + T / 2, last = (long long)w * T + T - 1;
   if (now == nullptr) {
-    if (w < n_win) track_sample_row(opt7 + 7 * mid, cov36 + 36 * mid, un, ms, ss, out + kTrackSampleRow * (long long)w);
+    if (w < n_win) fac.row(mid, un, ms, ss, out + F::kRow * (long long)w);
     return;
   }
   if (w >= n) return;
-  track_sample_row(opt7 + 7 * last, cov36 + 36 * last, un, ms, ss, now + kTrackSampleRow * (long long)w);
+  fac.row(last, un, ms, ss, now + F::kRow * (long long)w);
   const int lead = n - n_win;
-  if (w >= lead) track_sample_row(opt7 + 7 * mid, cov36 + 36 * mid, un, ms, ss, out + kTrackSampleRow * (long long)(w - lead));
+  if (w >= lead) fac.row(mid, un, ms, ss, out + F::kRow * (long long)(w - lead));
 }
 
-// ---- multi-stream tracker (mapnet_track_multi_*, inference.MultiTracker): the same windows for n_streams independent
-// sequences, one set of launches per call.  Per stream: its frames so far and its status word; the rings are
-// [n_streams][R].  The host keeps count of every stream and builds one record per frame of a call, so the kernels
-// find every window without reading a counter: stream, rank among that stream's frames in the call, that stream's
-// frame count in the call, absolute frame index, the output row of the frame's completed window (-1: none yet), and
-// (a per-row field) the record whose completed window is output row b (-1 once the call's rows are done).
-struct MTrackDev {
-  long long seen;
-  int status, pad;
-};
+// ---- multi-stream trackers (mapnet_track_multi_*, inference.MultiTracker; mapnet_track_multi_sample_*,
+// inference.SampledMultiTracker): the same windows for n_streams independent sequences, one set of launches per call.
+// Per stream: its frames so far and its status word; the rings are [n_streams][R].  The host keeps count of every
+// stream and builds one record per frame of a call, so the kernels find every window without reading a counter:
+// stream, rank among that stream's frames in the call, that stream's frame count in the call, absolute frame index,
+// the output row of the frame's completed window (-1: none yet), and (a per-row field) the record whose completed
+// window is output row b (-1 once the call's rows are done).
 struct MTrackRec { int stream, rank, count, frame, row, win; };
 
 // one window of a multi-stream call: its stream, centre, the last frame its slots may reach and the stream's first
@@ -371,7 +382,7 @@ struct MWin {
 // order (rec[w].win), a zero-lag step's the one that ends at each record's frame (record w); a flush of stream
 // flush_s >= 0 solves that stream's pending windows, clipped at its last frame.
 __device__ __forceinline__ bool mtrack_window(const MTrackRec* rec, int B, int w, int now, int flush_s,
-                                              const MTrackDev* st, int n_streams, long long lag, MWin* o) {
+                                              const TrackDev* st, int n_streams, long long lag, MWin* o) {
   if (flush_s >= 0) {
     const long long seen = st[flush_s].seen, first = trackcore::first_pending(seen, lag);
     if (w >= seen - first) return false;
@@ -412,14 +423,15 @@ __device__ __forceinline__ posemath::Pose6 mtrack_vo(const float* vo6, const flo
 
 // k_track_gather for B frames of several streams (records rec) or a flush of stream flush_s: rows 0 .. B-1 write
 // the new frames into their streams' rings, then slot (w, k) of window w < max_win, then VO (w, e).  The values are
-// k_track_gather's (st_pose7, calc_vo_logq_safe), so each window is bit for bit the single-stream tracker's.  Thread
-// 0 writes the count of windows k_pgo and the emit read: the completed windows of a step (the records with a row), B
+// k_track_gather's (the factors, calc_vo_logq_safe), so each window is bit for bit the single-stream tracker's.  Thread
+// 0 writes the count of windows the PGO and the emit read: the completed windows of a step (the records with a row), B
 // for a zero-lag step, the stream's pending windows for a flush.
+template <class F>
 __global__ void __launch_bounds__(128)
-k_track_multi_gather(const float* __restrict__ pred6, const float* __restrict__ vo6, const MTrackRec* __restrict__ rec,
-                     int B, int now, int flush_s, const MTrackDev* __restrict__ st, int n_streams,
-                     int* __restrict__ n_win_dev, double* __restrict__ ring7, float* __restrict__ ring_vo, long long R,
-                     int T, int skip, int fc, int max_win, double* __restrict__ win7, double* __restrict__ vos7) {
+k_track_multi_gather(F fac, const float* __restrict__ vo6, const MTrackRec* __restrict__ rec, int B, int now,
+                     int flush_s, const TrackDev* __restrict__ st, int n_streams, int* __restrict__ n_win_dev,
+                     float* __restrict__ ring_vo, long long R, int T, int skip, int fc, int max_win,
+                     double* __restrict__ vos7) {
   pdl_prologue();
   const long long lag = trackcore::lag(T, skip);
   const int E = fc ? T * (T - 1) / 2 : T - 1;
@@ -431,36 +443,30 @@ k_track_multi_gather(const float* __restrict__ pred6, const float* __restrict__ 
     else while (n < B && rec[n].win >= 0) ++n;
     *n_win_dev = n;
   }
-  if (r < B) {
-    const MTrackRec q = rec[r];
-    if (q.stream < 0 || q.stream >= n_streams) return;
-    const long long k = q.stream * R + q.frame % R;
-    st_pose7(pred6 + 6 * r, ring7 + 7 * k);
+  // one formation call site for ring and window slots, as in k_track_gather
+  const bool ring = r < B;
+  long long b, q;
+  if (ring) {
+    const MTrackRec x = rec[r];
+    if (x.stream < 0 || x.stream >= n_streams) return;
+    b = r; q = x.stream * R + x.frame % R;
 #pragma unroll
-    for (int c = 0; c < 6; ++c) ring_vo[6 * k + c] = vo6[6 * r + c];
-    return;
-  }
-  r -= B;
-  MWin m;
-  if (r < (long long)max_win * T) {
+    for (int c = 0; c < 6; ++c) ring_vo[6 * q + c] = vo6[6 * r + c];
+  } else if (r - B < (long long)max_win * T) {
+    r -= B;
     const int w = (int)(r / T), k = (int)(r % T);
+    MWin m;
     if (!mtrack_window(rec, B, w, now, flush_s, st, n_streams, lag, &m)) return;
     const long long f = trackcore::slot_frame(m.c, k, T, skip, m.last);
-    if (f >= m.f0) {
-      const int b = mtrack_input(rec, B, m, f);
-      const float nan = __int_as_float(0x7fc00000);
-      const float v6[6] = {nan, nan, nan, nan, nan, nan};
-      st_pose7(b >= 0 ? pred6 + 6LL * b : v6, win7 + 7 * r);
-    } else {
-      const double* src = ring7 + 7 * (m.s * R + f % R);
-#pragma unroll
-      for (int c = 0; c < 7; ++c) win7[7 * r + c] = src[c];
-    }
-    return;
-  }
-  r -= (long long)max_win * T;
-  if (r < (long long)max_win * E) {
+    if (f < m.f0) { fac.copy(m.s * R + f % R, r); return; }
+    b = mtrack_input(rec, B, m, f);
+    if (b < 0) { fac.nan_slot(r); return; }         // an inconsistent record table: a visible NaN, no stray read
+    q = r;
+  } else {
+    r -= B + (long long)max_win * T;
+    if (r >= (long long)max_win * E) return;
     const int w = (int)(r / E), e = (int)(r % E);
+    MWin m;
     if (!mtrack_window(rec, B, w, now, flush_s, st, n_streams, lag, &m)) return;
     int i, j;
     trackcore::vo_pair(e, T, fc, &i, &j);
@@ -470,128 +476,21 @@ k_track_multi_gather(const float* __restrict__ pred6, const float* __restrict__ 
                                                           mtrack_vo(vo6, ring_vo, rec, B, m, fb, R));
     const float v6[6] = {v.t.x, v.t.y, v.t.z, v.l.x, v.l.y, v.l.z};
     st_pose7(v6, vos7 + 7 * r);
-  }
-}
-
-// k_track_emit for several streams: window w's middle slot into out7 row w (a zero-lag step: into row rec[w].row
-// when the window completed a frame, and its last slot into now7 row w); a window k_pgo marked failed sets its
-// stream's status; the last record of each stream in the call sets that stream's frame count.
-__global__ void __launch_bounds__(128)
-k_track_multi_emit(const double* __restrict__ opt7, const int* __restrict__ win_fail, const MTrackRec* __restrict__ rec,
-                   int B, int flush_s, MTrackDev* __restrict__ st, int n_streams, const int* __restrict__ n_win_dev,
-                   int T, int un, double m0, double m1, double m2, double s0, double s1, double s2,
-                   double* __restrict__ out7, double* __restrict__ now7) {
-  pdl_prologue();
-  const int w = blockIdx.x * blockDim.x + threadIdx.x;
-  const double ms[3] = {m0, m1, m2}, ss[3] = {s0, s1, s2};
-  const double* win = opt7 + 7LL * w * T;
-  if (w < B) {
-    const MTrackRec q = rec[w];
-    const bool ok = q.stream >= 0 && q.stream < n_streams;
-    if (ok && q.rank == q.count - 1) st[q.stream].seen = (long long)q.frame + 1;
-    if (now7 != nullptr) {
-      if (!ok) return;
-      track_emit_pose(win + 7 * (T - 1), un, ms, ss, now7 + 7LL * w);
-      if (q.row >= 0) track_emit_pose(win + 7 * (T / 2), un, ms, ss, out7 + 7LL * q.row);
-      if (win_fail[w]) atomicExch(&st[q.stream].status, 1);
-      return;
-    }
-  }
-  if (now7 != nullptr || w >= *n_win_dev) return;
-  int s = flush_s;
-  if (s < 0) {
-    const int b = rec[w].win;
-    s = b >= 0 && b < B ? rec[b].stream : -1;
-    if (s < 0 || s >= n_streams) return;
-  }
-  track_emit_pose(win + 7 * (T / 2), un, ms, ss, out7 + 7LL * w);
-  if (win_fail[w]) atomicExch(&st[s].status, 1);
-}
-
-// ---- multi-stream Monte-Carlo tracker (mapnet_track_multi_sample_*, inference.SampledMultiTracker): the streams,
-// records and windows of mapnet_track_multi_* with the factors of mapnet_track_sample_*.  Per stream: its frame count,
-// its status word and rings of R frames of p7, S7 (float64) and VO poses (float32), [n_streams][R].
-
-// k_track_sample_gather for B frames of several streams (records rec) or a flush of stream flush_s: rows 0 .. B-1
-// form the new frames' p7 / S7 into their streams' rings, then slot (w, k) of window w < max_win, then VO (w, e), the
-// windows found as k_track_multi_gather finds them.  A slot that holds a frame of this call forms that frame's factor
-// itself, from the frame's input row: a multi-stream call has no cheap map from a frame to the slots that hold it (the
-// frame's row would scan every window of the call), and sample_factor is a pure function of the frame's mean and cov,
-// so each copy is bit for bit the ring's.  Thread 0 writes the count of windows k_pgo_cov and the emit read.
-__global__ void __launch_bounds__(128)
-k_track_multi_sample_gather(const double* __restrict__ mean, const double* __restrict__ cov,
-                            const float* __restrict__ vo6, const MTrackRec* __restrict__ rec, int B, int now,
-                            int flush_s, const MTrackDev* __restrict__ st, int n_streams, int* __restrict__ n_win_dev,
-                            double* __restrict__ ring7, double* __restrict__ ring49, float* __restrict__ ring_vo,
-                            long long R, int T, int skip, int fc, int max_win, double sax, double saq,
-                            double* __restrict__ win7, double* __restrict__ win49, double* __restrict__ vos7) {
-  pdl_prologue();
-  const long long lag = trackcore::lag(T, skip);
-  const int E = fc ? T * (T - 1) / 2 : T - 1;
-  long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r == 0) {
-    int n = 0;
-    if (flush_s >= 0) n = (int)(st[flush_s].seen - trackcore::first_pending(st[flush_s].seen, lag));
-    else if (now) n = B;
-    else while (n < B && rec[n].win >= 0) ++n;
-    *n_win_dev = n;
-  }
-  if (r < B) {
-    const MTrackRec q = rec[r];
-    if (q.stream < 0 || q.stream >= n_streams) return;
-    const long long k = q.stream * R + q.frame % R;
-    sample_factor(mean + 6 * r, cov + 36 * r, sax, saq, ring7 + 7 * k, ring49 + 49 * k);
-#pragma unroll
-    for (int c = 0; c < 6; ++c) ring_vo[6 * k + c] = vo6[6 * r + c];
     return;
   }
-  r -= B;
-  MWin m;
-  if (r < (long long)max_win * T) {
-    const int w = (int)(r / T), k = (int)(r % T);
-    if (!mtrack_window(rec, B, w, now, flush_s, st, n_streams, lag, &m)) return;
-    const long long f = trackcore::slot_frame(m.c, k, T, skip, m.last);
-    if (f >= m.f0) {
-      const int b = mtrack_input(rec, B, m, f);
-      if (b >= 0) {
-        sample_factor(mean + 6LL * b, cov + 36LL * b, sax, saq, win7 + 7 * r, win49 + 49 * r);
-      } else {                                      // an inconsistent record table: a visible NaN, no stray read
-        const double nan = __longlong_as_double(0x7ff8000000000000LL);
-        for (int c = 0; c < 7; ++c) win7[7 * r + c] = nan;
-        for (int c = 0; c < 49; ++c) win49[49 * r + c] = nan;
-      }
-    } else {
-      const long long q = m.s * R + f % R;
-      for (int c = 0; c < 7; ++c) win7[7 * r + c] = ring7[7 * q + c];
-      for (int c = 0; c < 49; ++c) win49[49 * r + c] = ring49[49 * q + c];
-    }
-    return;
-  }
-  r -= (long long)max_win * T;
-  if (r < (long long)max_win * E) {
-    const int w = (int)(r / E), e = (int)(r % E);
-    if (!mtrack_window(rec, B, w, now, flush_s, st, n_streams, lag, &m)) return;
-    int i, j;
-    trackcore::vo_pair(e, T, fc, &i, &j);
-    const long long fa = trackcore::slot_frame(m.c, i, T, skip, m.last);
-    const long long fb = trackcore::slot_frame(m.c, j, T, skip, m.last);
-    const posemath::Pose6 v = posemath::calc_vo_logq_safe(mtrack_vo(vo6, ring_vo, rec, B, m, fa, R),
-                                                          mtrack_vo(vo6, ring_vo, rec, B, m, fb, R));
-    const float v6[6] = {v.t.x, v.t.y, v.t.z, v.l.x, v.l.y, v.l.z};
-    st_pose7(v6, vos7 + 7 * r);
-  }
+  fac.form(b, ring, q);
 }
 
-// k_track_multi_emit with k_track_sample_emit's rows: window w's middle slot into out row w (a zero-lag step: into
-// row rec[w].row when the window completed a frame, and its last slot into now row w); a window k_pgo_cov marked
-// failed (its normal matrix or a slot's S7 not positive definite) sets its own stream's status; the last record of
-// each stream in the call sets that stream's frame count.
+// k_track_emit for several streams: window w's middle slot into out row w (a zero-lag step: into row rec[w].row
+// when the window completed a frame, and its last slot into now row w); a window the PGO marked failed (its normal
+// matrix, or a slot's S7, not positive definite) sets its own stream's status; the last record of each stream in the
+// call sets that stream's frame count.
+template <class F>
 __global__ void __launch_bounds__(128)
-k_track_multi_sample_emit(const double* __restrict__ opt7, const double* __restrict__ cov36,
-                          const int* __restrict__ win_fail, const MTrackRec* __restrict__ rec, int B, int flush_s,
-                          MTrackDev* __restrict__ st, int n_streams, const int* __restrict__ n_win_dev, int T, int un,
-                          double m0, double m1, double m2, double s0, double s1, double s2, double* __restrict__ out,
-                          double* __restrict__ now) {
+k_track_multi_emit(F fac, const int* __restrict__ win_fail, const MTrackRec* __restrict__ rec, int B, int flush_s,
+                   TrackDev* __restrict__ st, int n_streams, const int* __restrict__ n_win_dev, int T, int un,
+                   double m0, double m1, double m2, double s0, double s1, double s2, double* __restrict__ out,
+                   double* __restrict__ now) {
   pdl_prologue();
   const int w = blockIdx.x * blockDim.x + threadIdx.x;
   const double ms[3] = {m0, m1, m2}, ss[3] = {s0, s1, s2};
@@ -602,9 +501,8 @@ k_track_multi_sample_emit(const double* __restrict__ opt7, const double* __restr
     if (ok && q.rank == q.count - 1) st[q.stream].seen = (long long)q.frame + 1;
     if (now != nullptr) {
       if (!ok) return;
-      track_sample_row(opt7 + 7 * last, cov36 + 36 * last, un, ms, ss, now + kTrackSampleRow * (long long)w);
-      if (q.row >= 0)
-        track_sample_row(opt7 + 7 * mid, cov36 + 36 * mid, un, ms, ss, out + kTrackSampleRow * (long long)q.row);
+      fac.row(last, un, ms, ss, now + F::kRow * (long long)w);
+      if (q.row >= 0) fac.row(mid, un, ms, ss, out + F::kRow * (long long)q.row);
       if (win_fail[w]) atomicExch(&st[q.stream].status, 1);
       return;
     }
@@ -616,7 +514,7 @@ k_track_multi_sample_emit(const double* __restrict__ opt7, const double* __restr
     s = b >= 0 && b < B ? rec[b].stream : -1;
     if (s < 0 || s >= n_streams) return;
   }
-  track_sample_row(opt7 + 7 * mid, cov36 + 36 * mid, un, ms, ss, out + kTrackSampleRow * (long long)w);
+  fac.row(mid, un, ms, ss, out + F::kRow * (long long)w);
   if (win_fail[w]) atomicExch(&st[s].status, 1);
 }
 
@@ -782,15 +680,6 @@ int mapnet_eval_windows(const float* pred6, int n_pred, const float* poses, cons
 
 }  // extern "C"
 
-// what a tracker handle is created with: window geometry, PGO weights, pose statistics (single and multi-stream)
-struct TrackCfg {
-  int T, skip, fc, max_batch, E, max_win;   // max_win: the most windows one call completes, max(max_batch, lag)
-  long long R, lag;
-  double w4[4];                             // PGO weights 1/sqrt(sigma) of sax, saq, srx, srq
-  int un;
-  double m[3], s[3];
-};
-
 // checks a tracker's arguments (messages prefixed with `who`) and fills c; nothing is allocated or launched
 static int track_config(TrackCfg* c, const char* who, int T, int skip, int fc_vos, int max_batch, const double* sigmas4,
                         const double* pose_m3, const double* pose_s3) {
@@ -814,26 +703,122 @@ static int track_config(TrackCfg* c, const char* who, int T, int skip, int fc_vo
   return 0;
 }
 
-struct mapnet_track : TrackCfg {
-  TrackDev* st;
-  double* ring7;                            // [R][7]: pose7 of the last R frames, normalised translations
-  float* ring_vo;                           // [R][6]: their VO-library poses
-  double *win7, *vos7, *opt7;               // [max_win][T][7], [max_win][E][7], [max_win][T][7]
-};
+struct mapnet_track : TrackHandle {};
+struct mapnet_track_sample : TrackHandle {};
+struct mapnet_track_multi : TrackHandle {};
+struct mapnet_track_multi_sample : TrackHandle {};
 
-// the three launches of one call: n new frames (a step) or none (flush), out7 [max_win][7]; with now7 [n][7] a
-// zero-lag step, which solves all n of its windows, so k_pgo needs no device count
-static int track_launch(mapnet_track_t* h, const float* pred6, const float* vo6, int n, int flush, double* out7,
-                        double* now7, cudaStream_t st) {
+template <class H>
+static int track_destroy(H* h) {
+  if (h == nullptr) return 0;
+  cudaFree(h->st); cudaFree(h->n_win); cudaFree(h->ring7); cudaFree(h->ring49); cudaFree(h->ring_vo);
+  cudaFree(h->win7); cudaFree(h->win49); cudaFree(h->vos7); cudaFree(h->opt7); cudaFree(h->cov36);
+  delete h;
+  return 0;
+}
+
+// every tracker's create: the checks, then one allocation per buffer, with the byte count in the failure message of
+// the multi-stream trackers (multi); sampled trackers also hold the p / S7 rings and the posterior covariances
+template <class H>
+static int track_create(H** out, const char* who, bool multi, bool sampled, int n_streams, int T, int skip,
+                        int fc_vos, int max_batch, const double* sigmas4, const double* pose_m3,
+                        const double* pose_s3) {
+  MN_CHECK(out != nullptr && sigmas4 != nullptr, "%s: null argument", who);
+  *out = nullptr;
+  MN_CHECK(n_streams >= 1 && n_streams <= MAPNET_TRACK_MAX_STREAMS, "%s: %d streams outside [1, %d]", who, n_streams,
+           MAPNET_TRACK_MAX_STREAMS);
+  TrackCfg c;
+  MN_TRY(track_config(&c, who, T, skip, fc_vos, max_batch, sigmas4, pose_m3, pose_s3));
+  if (sampled) MN_TRY(pgo_cov_prepare());
+  const size_t W = (size_t)c.max_win, WT = W * c.T, ring = (size_t)n_streams * (size_t)c.R;
+  const size_t P = sampled ? 7 + 49 : 7;                     // doubles per ring frame and window slot of the factors
+  const size_t frame_bytes = P * sizeof(double) + 6 * sizeof(float);       // 472 B per sampled ring frame
+  const size_t bytes = ring * frame_bytes + WT * (P + 7 + (sampled ? 36 : 0)) * sizeof(double) +
+                       W * c.E * 7 * sizeof(double) + (size_t)n_streams * sizeof(TrackDev) + (W + 1) * sizeof(int);
+  MN_CHECK(ring < (1ull << 31), "%s: %d streams x rings of %lld frames = %zu frames (%.3f GB) exceed 2^31 ring frames",
+           who, n_streams, c.R, ring, bytes / 1e9);
+  H* h = new H();
+  static_cast<TrackCfg&>(*h) = c;
+  h->n_streams = n_streams;
+  h->sax = sigmas4[0]; h->saq = sigmas4[1];
+  bool ok = cudaMalloc((void**)&h->st, (size_t)n_streams * sizeof(TrackDev)) == cudaSuccess &&
+            cudaMalloc((void**)&h->n_win, (W + 1) * sizeof(int)) == cudaSuccess &&
+            cudaMalloc((void**)&h->ring7, ring * 7 * sizeof(double)) == cudaSuccess &&
+            (!sampled || cudaMalloc((void**)&h->ring49, ring * 49 * sizeof(double)) == cudaSuccess) &&
+            cudaMalloc((void**)&h->ring_vo, ring * 6 * sizeof(float)) == cudaSuccess &&
+            cudaMalloc((void**)&h->win7, WT * 7 * sizeof(double)) == cudaSuccess &&
+            (!sampled || cudaMalloc((void**)&h->win49, WT * 49 * sizeof(double)) == cudaSuccess) &&
+            cudaMalloc((void**)&h->vos7, W * c.E * 7 * sizeof(double)) == cudaSuccess &&
+            cudaMalloc((void**)&h->opt7, WT * 7 * sizeof(double)) == cudaSuccess &&
+            (!sampled || cudaMalloc((void**)&h->cov36, WT * 36 * sizeof(double)) == cudaSuccess) &&
+            cudaMemset(h->st, 0, (size_t)n_streams * sizeof(TrackDev)) == cudaSuccess &&
+            cudaMemset(h->n_win, 0, (W + 1) * sizeof(int)) == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess;
+  if (!ok) {
+    cudaGetLastError();
+    if (!multi)
+      set_last_error("%s: device allocation of a ring of %lld frames and %d windows failed", who, c.R, c.max_win);
+    else if (!sampled)
+      set_last_error("%s: device allocation of %zu bytes (%d streams x rings of %lld frames, %d windows) failed", who,
+                     bytes, n_streams, c.R, c.max_win);
+    else
+      set_last_error("%s: device allocation of %zu bytes (%d streams x rings of %lld frames of %zu B, %d windows) "
+                     "failed", who, bytes, n_streams, c.R, frame_bytes, c.max_win);
+    track_destroy(h);
+    return 1;
+  }
+  h->win_fail = h->n_win + 1;
+  *out = h;
+  return 0;
+}
+
+// stream s (every stream when s = -1) starts a new sequence, stream-ordered
+static int track_reset(TrackHandle* h, int s, cudaStream_t stream) {
+  const size_t n = s < 0 ? (size_t)h->n_streams : 1;
+  MN_CUDA(cudaMemsetAsync(h->st + (s < 0 ? 0 : s), 0, n * sizeof(TrackDev), stream));
+  return 0;
+}
+
+static int track_status(TrackHandle* h, int s, int64_t* frames_seen, int* failed, cudaStream_t stream) {
+  TrackDev d;
+  MN_CUDA(cudaMemcpyAsync(&d, h->st + s, sizeof(TrackDev), cudaMemcpyDeviceToHost, stream));
+  MN_CUDA(cudaStreamSynchronize(stream));
+  if (frames_seen != nullptr) *frames_seen = d.seen;
+  if (failed != nullptr) *failed = d.status;
+  return 0;
+}
+
+// the three launches of a single-stream call: n new frames (a step) or none (flush), out [max_win][kRow]; with now
+// [n][kRow] a zero-lag step, which solves all n of its windows, so the PGO needs no device count
+template <class F>
+static int track_launch(TrackHandle* h, F fac, const float* vo6, int n, int flush, double* out, double* now,
+                        cudaStream_t st) {
   const int nw = flush ? (int)(h->lag < h->max_win ? h->lag : h->max_win) : n;   // the grid's windows
   const long long rows = n + (long long)nw * (h->T + h->E);
-  MN_LAUNCH(k_track_gather, cdiv(rows, 128), 128, 0, st, pred6, vo6, n, flush, now7 != nullptr ? 1 : 0, h->st, h->ring7,
-            h->ring_vo, h->R, h->T, h->skip, h->fc, nw, h->win7, h->vos7);
+  MN_LAUNCH(k_track_gather<F>, cdiv(rows, 128), 128, 0, st, fac, vo6, n, flush, now != nullptr ? 1 : 0,
+            (const TrackDev*)h->st, h->n_win, h->ring_vo, h->R, h->T, h->skip, h->fc, nw, h->vos7);
   MN_LAUNCH_CHECK();
-  MN_TRY(launch_pgo(h->win7, h->vos7, h->opt7, nw, h->T, h->fc, h->w4, 10, 0, &h->st->status,
-                    now7 != nullptr ? nullptr : &h->st->n_win, st));
-  MN_LAUNCH(k_track_emit, cdiv(nw, 128), 128, 0, st, (const double*)h->opt7, h->st, n, h->T, h->un, h->m[0], h->m[1],
-            h->m[2], h->s[0], h->s[1], h->s[2], out7, now7);
+  MN_TRY(fac.pgo(*h, nw, &h->st->status, now != nullptr ? nullptr : h->n_win, nullptr, st));
+  MN_LAUNCH(k_track_emit<F>, cdiv(nw, 128), 128, 0, st, fac, h->st, (const int*)h->n_win, n, h->T, h->un, h->m[0],
+            h->m[1], h->m[2], h->s[0], h->s[1], h->s[2], out, now);
+  MN_LAUNCH_CHECK();
+  return 0;
+}
+
+// the three launches of a multi-stream call: B frames with records rec (a step; with now a zero-lag step, which
+// solves all B of its windows) or a flush of stream flush_s (B = 0); out [max_win][kRow], now [B][kRow] or null
+template <class F>
+static int track_multi_launch(TrackHandle* h, F fac, const float* vo6, const MTrackRec* rec, int B, int flush_s,
+                              double* out, double* now, cudaStream_t st) {
+  const int nw = flush_s >= 0 ? (int)(h->lag < h->max_win ? h->lag : h->max_win) : B;    // the grid's windows
+  const int zl = now != nullptr ? 1 : 0;
+  const long long rows = B + (long long)nw * (h->T + h->E);
+  MN_LAUNCH(k_track_multi_gather<F>, cdiv(rows, 128), 128, 0, st, fac, vo6, rec, B, zl, flush_s,
+            (const TrackDev*)h->st, h->n_streams, h->n_win, h->ring_vo, h->R, h->T, h->skip, h->fc, nw, h->vos7);
+  MN_LAUNCH_CHECK();
+  MN_TRY(fac.pgo(*h, nw, nullptr, zl ? nullptr : h->n_win, h->win_fail, st));
+  MN_LAUNCH(k_track_multi_emit<F>, cdiv(nw > B ? nw : B, 128), 128, 0, st, fac, (const int*)h->win_fail, rec, B,
+            flush_s, h->st, h->n_streams, (const int*)h->n_win, h->T, h->un, h->m[0], h->m[1], h->m[2], h->s[0],
+            h->s[1], h->s[2], out, now);
   MN_LAUNCH_CHECK();
   return 0;
 }
@@ -842,36 +827,14 @@ extern "C" {
 
 int mapnet_track_create(mapnet_track_t** out, int T, int skip, int fc_vos, int max_batch, const double* sigmas4,
                         const double* pose_m3, const double* pose_s3) {
-  MN_CHECK(out != nullptr && sigmas4 != nullptr, "track_create: null argument");
-  *out = nullptr;
-  TrackCfg c;
-  MN_TRY(track_config(&c, "track_create", T, skip, fc_vos, max_batch, sigmas4, pose_m3, pose_s3));
-  const long long R = c.R;
-  mapnet_track* h = new mapnet_track();
-  static_cast<TrackCfg&>(*h) = c;
-  const size_t W = (size_t)h->max_win;
-  bool ok = cudaMalloc((void**)&h->st, sizeof(TrackDev)) == cudaSuccess &&
-            cudaMalloc((void**)&h->ring7, (size_t)R * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->ring_vo, (size_t)R * 6 * sizeof(float)) == cudaSuccess &&
-            cudaMalloc((void**)&h->win7, W * T * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->vos7, W * h->E * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->opt7, W * T * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMemset(h->st, 0, sizeof(TrackDev)) == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess;
-  if (!ok) {
-    cudaGetLastError();
-    set_last_error("track_create: device allocation of a ring of %lld frames and %d windows failed", R, h->max_win);
-    mapnet_track_destroy(h);
-    return 1;
-  }
-  *out = h;
-  return 0;
+  return track_create(out, "track_create", false, false, 1, T, skip, fc_vos, max_batch, sigmas4, pose_m3, pose_s3);
 }
 
 int mapnet_track_step(mapnet_track_t* h, const float* pred6, const float* vo6, int B, double* out7, void* stream) {
   MN_CHECK(h != nullptr, "track_step: null handle");
   MN_CHECK(pred6 != nullptr && vo6 != nullptr && out7 != nullptr, "track_step: null argument");
   MN_CHECK(B >= 1 && B <= h->max_batch, "track_step: %d frames outside [1, max_batch=%d]", B, h->max_batch);
-  return track_launch(h, pred6, vo6, B, 0, out7, nullptr, (cudaStream_t)stream);
+  return track_launch(h, PointFactor(*h, pred6), vo6, B, 0, out7, nullptr, (cudaStream_t)stream);
 }
 
 int mapnet_track_step_now(mapnet_track_t* h, const float* pred6, const float* vo6, int B, double* out7, double* now7,
@@ -879,98 +842,32 @@ int mapnet_track_step_now(mapnet_track_t* h, const float* pred6, const float* vo
   MN_CHECK(h != nullptr, "track_step_now: null handle");
   MN_CHECK(pred6 != nullptr && vo6 != nullptr && out7 != nullptr && now7 != nullptr, "track_step_now: null argument");
   MN_CHECK(B >= 1 && B <= h->max_batch, "track_step_now: %d frames outside [1, max_batch=%d]", B, h->max_batch);
-  return track_launch(h, pred6, vo6, B, 0, out7, now7, (cudaStream_t)stream);
+  return track_launch(h, PointFactor(*h, pred6), vo6, B, 0, out7, now7, (cudaStream_t)stream);
 }
 
 int mapnet_track_flush(mapnet_track_t* h, double* out7, void* stream) {
   MN_CHECK(h != nullptr, "track_flush: null handle");
   MN_CHECK(out7 != nullptr, "track_flush: null argument");
   if (h->lag == 0) return 0;                 // every window was complete when its last frame arrived
-  return track_launch(h, nullptr, nullptr, 0, 1, out7, nullptr, (cudaStream_t)stream);
+  return track_launch(h, PointFactor(*h, nullptr), nullptr, 0, 1, out7, nullptr, (cudaStream_t)stream);
 }
 
 int mapnet_track_reset(mapnet_track_t* h, void* stream) {
   MN_CHECK(h != nullptr, "track_reset: null handle");
-  MN_CUDA(cudaMemsetAsync(h->st, 0, sizeof(TrackDev), (cudaStream_t)stream));
-  return 0;
+  return track_reset(h, -1, (cudaStream_t)stream);
 }
 
 int mapnet_track_status(mapnet_track_t* h, int64_t* frames_seen, int* failed, void* stream) {
   MN_CHECK(h != nullptr, "track_status: null handle");
-  TrackDev d;
-  MN_CUDA(cudaMemcpyAsync(&d, h->st, sizeof(TrackDev), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  MN_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-  if (frames_seen != nullptr) *frames_seen = d.seen;
-  if (failed != nullptr) *failed = d.status;
-  return 0;
+  return track_status(h, 0, frames_seen, failed, (cudaStream_t)stream);
 }
 
-int mapnet_track_destroy(mapnet_track_t* h) {
-  if (h == nullptr) return 0;
-  cudaFree(h->st); cudaFree(h->ring7); cudaFree(h->ring_vo); cudaFree(h->win7); cudaFree(h->vos7); cudaFree(h->opt7);
-  delete h;
-  return 0;
-}
-
-}  // extern "C"
-
-struct mapnet_track_sample : TrackCfg {
-  TrackDev* st;
-  double sax, saq;                          // the floors of the absolute factors' covariances
-  double *ring7, *ring49;                   // [R][7], [R][7][7]: p and S7 of the last R frames
-  float* ring_vo;                           // [R][6]
-  double *win7, *win49, *vos7, *opt7, *cov36;   // [max_win][T][7], [.][T][49], [.][E][7], [.][T][7], [.][T][36]
-};
-
-// the three launches of a sampled call: n new frames (a step) or none (flush); out [max_win][45], now [n][45] or null
-static int track_sample_launch(mapnet_track_sample_t* h, const double* mean, const double* cov, const float* vo6, int n,
-                               int flush, double* out, double* now, cudaStream_t st) {
-  const int nw = flush ? (int)(h->lag < h->max_win ? h->lag : h->max_win) : n;
-  const long long rows = n + (long long)nw * (h->T + h->E);
-  MN_LAUNCH(k_track_sample_gather, cdiv(rows, 128), 128, 0, st, mean, cov, vo6, n, flush, now != nullptr ? 1 : 0, h->st,
-            h->ring7, h->ring49, h->ring_vo, h->R, h->T, h->skip, h->fc, nw, h->sax, h->saq, h->win7, h->win49,
-            h->vos7);
-  MN_LAUNCH_CHECK();
-  MN_TRY(launch_pgo_cov(h->win7, h->win49, h->vos7, h->opt7, h->cov36, nw, h->T, h->fc, h->w4[2], h->w4[3], 10,
-                        &h->st->status, now != nullptr ? nullptr : &h->st->n_win, nullptr, st));
-  MN_LAUNCH(k_track_sample_emit, cdiv(nw, 128), 128, 0, st, (const double*)h->opt7, (const double*)h->cov36, h->st, n,
-            h->T, h->un, h->m[0], h->m[1], h->m[2], h->s[0], h->s[1], h->s[2], out, now);
-  MN_LAUNCH_CHECK();
-  return 0;
-}
-
-extern "C" {
+int mapnet_track_destroy(mapnet_track_t* h) { return track_destroy(h); }
 
 int mapnet_track_sample_create(mapnet_track_sample_t** out, int T, int skip, int fc_vos, int max_batch,
                                const double* sigmas4, const double* pose_m3, const double* pose_s3) {
-  MN_CHECK(out != nullptr && sigmas4 != nullptr, "track_sample_create: null argument");
-  *out = nullptr;
-  TrackCfg c;
-  MN_TRY(track_config(&c, "track_sample_create", T, skip, fc_vos, max_batch, sigmas4, pose_m3, pose_s3));
-  MN_TRY(pgo_cov_prepare());
-  const size_t R = (size_t)c.R, W = (size_t)c.max_win, WT = W * T;
-  mapnet_track_sample* h = new mapnet_track_sample();
-  static_cast<TrackCfg&>(*h) = c;
-  h->sax = sigmas4[0]; h->saq = sigmas4[1];
-  bool ok = cudaMalloc((void**)&h->st, sizeof(TrackDev)) == cudaSuccess &&
-            cudaMalloc((void**)&h->ring7, R * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->ring49, R * 49 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->ring_vo, R * 6 * sizeof(float)) == cudaSuccess &&
-            cudaMalloc((void**)&h->win7, WT * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->win49, WT * 49 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->vos7, W * c.E * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->opt7, WT * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->cov36, WT * 36 * sizeof(double)) == cudaSuccess &&
-            cudaMemset(h->st, 0, sizeof(TrackDev)) == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess;
-  if (!ok) {
-    cudaGetLastError();
-    set_last_error("track_sample_create: device allocation of a ring of %lld frames and %d windows failed", c.R,
-                   c.max_win);
-    mapnet_track_sample_destroy(h);
-    return 1;
-  }
-  *out = h;
-  return 0;
+  return track_create(out, "track_sample_create", false, true, 1, T, skip, fc_vos, max_batch, sigmas4, pose_m3,
+                      pose_s3);
 }
 
 int mapnet_track_sample_step(mapnet_track_sample_t* h, const double* mean6, const double* cov36, const float* vo6, int B,
@@ -978,7 +875,7 @@ int mapnet_track_sample_step(mapnet_track_sample_t* h, const double* mean6, cons
   MN_CHECK(h != nullptr, "track_sample_step: null handle");
   MN_CHECK(mean6 != nullptr && cov36 != nullptr && vo6 != nullptr && out != nullptr, "track_sample_step: null argument");
   MN_CHECK(B >= 1 && B <= h->max_batch, "track_sample_step: %d frames outside [1, max_batch=%d]", B, h->max_batch);
-  return track_sample_launch(h, mean6, cov36, vo6, B, 0, out, nullptr, (cudaStream_t)stream);
+  return track_launch(h, SampleFactor(*h, mean6, cov36), vo6, B, 0, out, nullptr, (cudaStream_t)stream);
 }
 
 int mapnet_track_sample_step_now(mapnet_track_sample_t* h, const double* mean6, const double* cov36, const float* vo6,
@@ -987,30 +884,24 @@ int mapnet_track_sample_step_now(mapnet_track_sample_t* h, const double* mean6, 
   MN_CHECK(mean6 != nullptr && cov36 != nullptr && vo6 != nullptr && out != nullptr && now != nullptr,
            "track_sample_step_now: null argument");
   MN_CHECK(B >= 1 && B <= h->max_batch, "track_sample_step_now: %d frames outside [1, max_batch=%d]", B, h->max_batch);
-  return track_sample_launch(h, mean6, cov36, vo6, B, 0, out, now, (cudaStream_t)stream);
+  return track_launch(h, SampleFactor(*h, mean6, cov36), vo6, B, 0, out, now, (cudaStream_t)stream);
 }
 
 int mapnet_track_sample_flush(mapnet_track_sample_t* h, double* out, void* stream) {
   MN_CHECK(h != nullptr, "track_sample_flush: null handle");
   MN_CHECK(out != nullptr, "track_sample_flush: null argument");
   if (h->lag == 0) return 0;
-  return track_sample_launch(h, nullptr, nullptr, nullptr, 0, 1, out, nullptr, (cudaStream_t)stream);
+  return track_launch(h, SampleFactor(*h, nullptr, nullptr), nullptr, 0, 1, out, nullptr, (cudaStream_t)stream);
 }
 
 int mapnet_track_sample_reset(mapnet_track_sample_t* h, void* stream) {
   MN_CHECK(h != nullptr, "track_sample_reset: null handle");
-  MN_CUDA(cudaMemsetAsync(h->st, 0, sizeof(TrackDev), (cudaStream_t)stream));
-  return 0;
+  return track_reset(h, -1, (cudaStream_t)stream);
 }
 
 int mapnet_track_sample_status(mapnet_track_sample_t* h, int64_t* frames_seen, int* failed, void* stream) {
   MN_CHECK(h != nullptr, "track_sample_status: null handle");
-  TrackDev d;
-  MN_CUDA(cudaMemcpyAsync(&d, h->st, sizeof(TrackDev), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  MN_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-  if (frames_seen != nullptr) *frames_seen = d.seen;
-  if (failed != nullptr) *failed = d.status;
-  return 0;
+  return track_status(h, 0, frames_seen, failed, (cudaStream_t)stream);
 }
 
 int mapnet_test_sample_factor(const double* mean6, const double* cov36, int64_t n, double sax, double saq, double* p7,
@@ -1024,83 +915,12 @@ int mapnet_test_sample_factor(const double* mean6, const double* cov36, int64_t 
   return 0;
 }
 
-int mapnet_track_sample_destroy(mapnet_track_sample_t* h) {
-  if (h == nullptr) return 0;
-  cudaFree(h->st); cudaFree(h->ring7); cudaFree(h->ring49); cudaFree(h->ring_vo); cudaFree(h->win7);
-  cudaFree(h->win49); cudaFree(h->vos7); cudaFree(h->opt7); cudaFree(h->cov36);
-  delete h;
-  return 0;
-}
-
-}  // extern "C"
-
-struct mapnet_track_multi : TrackCfg {
-  int n_streams;
-  MTrackDev* st;                            // [n_streams]
-  int* n_win;                               // the windows of the current call, written by the gather
-  int* win_fail;                            // [max_win]: k_pgo's per-window failure flags
-  double* ring7;                            // [n_streams][R][7]
-  float* ring_vo;                           // [n_streams][R][6]
-  double *win7, *vos7, *opt7;               // [max_win][T][7], [max_win][E][7], [max_win][T][7]
-};
-
-// the three launches of a multi-stream call: B frames with records rec (a step; with now7 a zero-lag step, which
-// solves all B of its windows) or a flush of stream flush_s (B = 0)
-static int track_multi_launch(mapnet_track_multi_t* h, const float* pred6, const float* vo6, const MTrackRec* rec,
-                              int B, int flush_s, double* out7, double* now7, cudaStream_t st) {
-  const int nw = flush_s >= 0 ? (int)(h->lag < h->max_win ? h->lag : h->max_win) : B;    // the grid's windows
-  const int now = now7 != nullptr ? 1 : 0;
-  const long long rows = B + (long long)nw * (h->T + h->E);
-  MN_LAUNCH(k_track_multi_gather, cdiv(rows, 128), 128, 0, st, pred6, vo6, rec, B, now, flush_s,
-            (const MTrackDev*)h->st, h->n_streams, h->n_win, h->ring7, h->ring_vo, h->R, h->T, h->skip, h->fc, nw,
-            h->win7, h->vos7);
-  MN_LAUNCH_CHECK();
-  MN_TRY(launch_pgo(h->win7, h->vos7, h->opt7, nw, h->T, h->fc, h->w4, 10, 0, nullptr, now ? nullptr : h->n_win, st,
-                    h->win_fail));
-  MN_LAUNCH(k_track_multi_emit, cdiv(nw > B ? nw : B, 128), 128, 0, st, (const double*)h->opt7,
-            (const int*)h->win_fail, rec, B, flush_s, h->st, h->n_streams, (const int*)h->n_win, h->T, h->un, h->m[0],
-            h->m[1], h->m[2], h->s[0], h->s[1], h->s[2], out7, now7);
-  MN_LAUNCH_CHECK();
-  return 0;
-}
-
-extern "C" {
+int mapnet_track_sample_destroy(mapnet_track_sample_t* h) { return track_destroy(h); }
 
 int mapnet_track_multi_create(mapnet_track_multi_t** out, int n_streams, int T, int skip, int fc_vos, int max_batch,
                               const double* sigmas4, const double* pose_m3, const double* pose_s3) {
-  MN_CHECK(out != nullptr && sigmas4 != nullptr, "track_multi_create: null argument");
-  *out = nullptr;
-  MN_CHECK(n_streams >= 1 && n_streams <= MAPNET_TRACK_MAX_STREAMS, "track_multi_create: %d streams outside [1, %d]",
-           n_streams, MAPNET_TRACK_MAX_STREAMS);
-  TrackCfg c;
-  MN_TRY(track_config(&c, "track_multi_create", T, skip, fc_vos, max_batch, sigmas4, pose_m3, pose_s3));
-  const size_t W = (size_t)c.max_win, ring = (size_t)n_streams * (size_t)c.R;
-  const size_t bytes = ring * (7 * sizeof(double) + 6 * sizeof(float)) + W * (2 * c.T + c.E) * 7 * sizeof(double) +
-                       (size_t)n_streams * sizeof(MTrackDev) + (W + 1) * sizeof(int);
-  MN_CHECK(ring < (1ull << 31), "track_multi_create: %d streams x rings of %lld frames = %zu frames (%.3f GB) exceed "
-           "2^31 ring frames", n_streams, c.R, ring, bytes / 1e9);
-  mapnet_track_multi* h = new mapnet_track_multi();
-  static_cast<TrackCfg&>(*h) = c;
-  h->n_streams = n_streams;
-  bool ok = cudaMalloc((void**)&h->st, (size_t)n_streams * sizeof(MTrackDev)) == cudaSuccess &&
-            cudaMalloc((void**)&h->n_win, (W + 1) * sizeof(int)) == cudaSuccess &&
-            cudaMalloc((void**)&h->ring7, ring * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->ring_vo, ring * 6 * sizeof(float)) == cudaSuccess &&
-            cudaMalloc((void**)&h->win7, W * c.T * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->vos7, W * c.E * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->opt7, W * c.T * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMemset(h->st, 0, (size_t)n_streams * sizeof(MTrackDev)) == cudaSuccess &&
-            cudaMemset(h->n_win, 0, (W + 1) * sizeof(int)) == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess;
-  if (!ok) {
-    cudaGetLastError();
-    set_last_error("track_multi_create: device allocation of %zu bytes (%d streams x rings of %lld frames, %d windows) "
-                   "failed", bytes, n_streams, c.R, c.max_win);
-    mapnet_track_multi_destroy(h);
-    return 1;
-  }
-  h->win_fail = h->n_win + 1;
-  *out = h;
-  return 0;
+  return track_create(out, "track_multi_create", true, false, n_streams, T, skip, fc_vos, max_batch, sigmas4, pose_m3,
+                      pose_s3);
 }
 
 int mapnet_track_multi_step(mapnet_track_multi_t* h, const float* pred6, const float* vo6, const int32_t* rec, int B,
@@ -1108,7 +928,8 @@ int mapnet_track_multi_step(mapnet_track_multi_t* h, const float* pred6, const f
   MN_CHECK(h != nullptr, "track_multi_step: null handle");
   MN_CHECK(pred6 != nullptr && vo6 != nullptr && rec != nullptr && out7 != nullptr, "track_multi_step: null argument");
   MN_CHECK(B >= 1 && B <= h->max_batch, "track_multi_step: %d frames outside [1, max_batch=%d]", B, h->max_batch);
-  return track_multi_launch(h, pred6, vo6, (const MTrackRec*)rec, B, -1, out7, now7, (cudaStream_t)stream);
+  return track_multi_launch(h, PointFactor(*h, pred6), vo6, (const MTrackRec*)rec, B, -1, out7, now7,
+                            (cudaStream_t)stream);
 }
 
 int mapnet_track_multi_flush(mapnet_track_multi_t* h, int s, double* out7, void* stream) {
@@ -1116,114 +937,28 @@ int mapnet_track_multi_flush(mapnet_track_multi_t* h, int s, double* out7, void*
   MN_CHECK(out7 != nullptr, "track_multi_flush: null argument");
   MN_CHECK(s >= 0 && s < h->n_streams, "track_multi_flush: stream %d outside [0, %d)", s, h->n_streams);
   if (h->lag == 0) return 0;                 // every window was complete when its last frame arrived
-  return track_multi_launch(h, nullptr, nullptr, nullptr, 0, s, out7, nullptr, (cudaStream_t)stream);
+  return track_multi_launch(h, PointFactor(*h, nullptr), nullptr, nullptr, 0, s, out7, nullptr, (cudaStream_t)stream);
 }
 
 int mapnet_track_multi_reset(mapnet_track_multi_t* h, int s, void* stream) {
   MN_CHECK(h != nullptr, "track_multi_reset: null handle");
   MN_CHECK(s >= -1 && s < h->n_streams, "track_multi_reset: stream %d outside [-1, %d)", s, h->n_streams);
-  const size_t n = s < 0 ? (size_t)h->n_streams : 1;
-  MN_CUDA(cudaMemsetAsync(h->st + (s < 0 ? 0 : s), 0, n * sizeof(MTrackDev), (cudaStream_t)stream));
-  return 0;
+  return track_reset(h, s, (cudaStream_t)stream);
 }
 
 int mapnet_track_multi_status(mapnet_track_multi_t* h, int s, int64_t* frames_seen, int* failed, void* stream) {
   MN_CHECK(h != nullptr, "track_multi_status: null handle");
   MN_CHECK(s >= 0 && s < h->n_streams, "track_multi_status: stream %d outside [0, %d)", s, h->n_streams);
-  MTrackDev d;
-  MN_CUDA(cudaMemcpyAsync(&d, h->st + s, sizeof(MTrackDev), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  MN_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-  if (frames_seen != nullptr) *frames_seen = d.seen;
-  if (failed != nullptr) *failed = d.status;
-  return 0;
+  return track_status(h, s, frames_seen, failed, (cudaStream_t)stream);
 }
 
-int mapnet_track_multi_destroy(mapnet_track_multi_t* h) {
-  if (h == nullptr) return 0;
-  cudaFree(h->st); cudaFree(h->n_win); cudaFree(h->ring7); cudaFree(h->ring_vo); cudaFree(h->win7); cudaFree(h->vos7);
-  cudaFree(h->opt7);
-  delete h;
-  return 0;
-}
-
-}  // extern "C"
-
-struct mapnet_track_multi_sample : TrackCfg {
-  int n_streams;
-  double sax, saq;                          // the floors of the absolute factors' covariances
-  MTrackDev* st;                            // [n_streams]
-  int* n_win;                               // the windows of the current call, written by the gather
-  int* win_fail;                            // [max_win]: k_pgo_cov's per-window failure flags
-  double *ring7, *ring49;                   // [n_streams][R][7], [n_streams][R][7][7]
-  float* ring_vo;                           // [n_streams][R][6]
-  double *win7, *win49, *vos7, *opt7, *cov36;   // [max_win][T][7], [.][T][49], [.][E][7], [.][T][7], [.][T][36]
-};
-
-// the three launches of a multi-stream sampled call: B frames with records rec (a step; with now a zero-lag step,
-// which solves all B of its windows) or a flush of stream flush_s (B = 0); out [max_win][45], now [B][45] or null
-static int track_multi_sample_launch(mapnet_track_multi_sample_t* h, const double* mean, const double* cov,
-                                     const float* vo6, const MTrackRec* rec, int B, int flush_s, double* out,
-                                     double* now, cudaStream_t st) {
-  const int nw = flush_s >= 0 ? (int)(h->lag < h->max_win ? h->lag : h->max_win) : B;    // the grid's windows
-  const int zl = now != nullptr ? 1 : 0;
-  const long long rows = B + (long long)nw * (h->T + h->E);
-  MN_LAUNCH(k_track_multi_sample_gather, cdiv(rows, 128), 128, 0, st, mean, cov, vo6, rec, B, zl, flush_s,
-            (const MTrackDev*)h->st, h->n_streams, h->n_win, h->ring7, h->ring49, h->ring_vo, h->R, h->T, h->skip,
-            h->fc, nw, h->sax, h->saq, h->win7, h->win49, h->vos7);
-  MN_LAUNCH_CHECK();
-  MN_TRY(launch_pgo_cov(h->win7, h->win49, h->vos7, h->opt7, h->cov36, nw, h->T, h->fc, h->w4[2], h->w4[3], 10,
-                        nullptr, zl ? nullptr : h->n_win, h->win_fail, st));
-  MN_LAUNCH(k_track_multi_sample_emit, cdiv(nw > B ? nw : B, 128), 128, 0, st, (const double*)h->opt7,
-            (const double*)h->cov36, (const int*)h->win_fail, rec, B, flush_s, h->st, h->n_streams,
-            (const int*)h->n_win, h->T, h->un, h->m[0], h->m[1], h->m[2], h->s[0], h->s[1], h->s[2], out, now);
-  MN_LAUNCH_CHECK();
-  return 0;
-}
-
-extern "C" {
+int mapnet_track_multi_destroy(mapnet_track_multi_t* h) { return track_destroy(h); }
 
 int mapnet_track_multi_sample_create(mapnet_track_multi_sample_t** out, int n_streams, int T, int skip, int fc_vos,
                                      int max_batch, const double* sigmas4, const double* pose_m3,
                                      const double* pose_s3) {
-  MN_CHECK(out != nullptr && sigmas4 != nullptr, "track_multi_sample_create: null argument");
-  *out = nullptr;
-  MN_CHECK(n_streams >= 1 && n_streams <= MAPNET_TRACK_MAX_STREAMS,
-           "track_multi_sample_create: %d streams outside [1, %d]", n_streams, MAPNET_TRACK_MAX_STREAMS);
-  TrackCfg c;
-  MN_TRY(track_config(&c, "track_multi_sample_create", T, skip, fc_vos, max_batch, sigmas4, pose_m3, pose_s3));
-  MN_TRY(pgo_cov_prepare());
-  const size_t W = (size_t)c.max_win, WT = W * c.T, ring = (size_t)n_streams * (size_t)c.R;
-  const size_t frame_bytes = (7 + 49) * sizeof(double) + 6 * sizeof(float);      // 472 B per ring frame
-  const size_t bytes = ring * frame_bytes + WT * (7 + 49 + 7 + 36) * sizeof(double) + W * c.E * 7 * sizeof(double) +
-                       (size_t)n_streams * sizeof(MTrackDev) + (W + 1) * sizeof(int);
-  MN_CHECK(ring < (1ull << 31), "track_multi_sample_create: %d streams x rings of %lld frames = %zu frames (%.3f GB) "
-           "exceed 2^31 ring frames", n_streams, c.R, ring, bytes / 1e9);
-  mapnet_track_multi_sample* h = new mapnet_track_multi_sample();
-  static_cast<TrackCfg&>(*h) = c;
-  h->n_streams = n_streams;
-  h->sax = sigmas4[0]; h->saq = sigmas4[1];
-  bool ok = cudaMalloc((void**)&h->st, (size_t)n_streams * sizeof(MTrackDev)) == cudaSuccess &&
-            cudaMalloc((void**)&h->n_win, (W + 1) * sizeof(int)) == cudaSuccess &&
-            cudaMalloc((void**)&h->ring7, ring * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->ring49, ring * 49 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->ring_vo, ring * 6 * sizeof(float)) == cudaSuccess &&
-            cudaMalloc((void**)&h->win7, WT * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->win49, WT * 49 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->vos7, W * c.E * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->opt7, WT * 7 * sizeof(double)) == cudaSuccess &&
-            cudaMalloc((void**)&h->cov36, WT * 36 * sizeof(double)) == cudaSuccess &&
-            cudaMemset(h->st, 0, (size_t)n_streams * sizeof(MTrackDev)) == cudaSuccess &&
-            cudaMemset(h->n_win, 0, (W + 1) * sizeof(int)) == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess;
-  if (!ok) {
-    cudaGetLastError();
-    set_last_error("track_multi_sample_create: device allocation of %zu bytes (%d streams x rings of %lld frames of "
-                   "%zu B, %d windows) failed", bytes, n_streams, c.R, frame_bytes, c.max_win);
-    mapnet_track_multi_sample_destroy(h);
-    return 1;
-  }
-  h->win_fail = h->n_win + 1;
-  *out = h;
-  return 0;
+  return track_create(out, "track_multi_sample_create", true, true, n_streams, T, skip, fc_vos, max_batch, sigmas4,
+                      pose_m3, pose_s3);
 }
 
 int mapnet_track_multi_sample_step(mapnet_track_multi_sample_t* h, const double* mean6, const double* cov36,
@@ -1234,8 +969,8 @@ int mapnet_track_multi_sample_step(mapnet_track_multi_sample_t* h, const double*
            "track_multi_sample_step: null argument");
   MN_CHECK(B >= 1 && B <= h->max_batch, "track_multi_sample_step: %d frames outside [1, max_batch=%d]", B,
            h->max_batch);
-  return track_multi_sample_launch(h, mean6, cov36, vo6, (const MTrackRec*)rec, B, -1, out, now,
-                                   (cudaStream_t)stream);
+  return track_multi_launch(h, SampleFactor(*h, mean6, cov36), vo6, (const MTrackRec*)rec, B, -1, out, now,
+                            (cudaStream_t)stream);
 }
 
 int mapnet_track_multi_sample_flush(mapnet_track_multi_sample_t* h, int s, double* out, void* stream) {
@@ -1243,36 +978,24 @@ int mapnet_track_multi_sample_flush(mapnet_track_multi_sample_t* h, int s, doubl
   MN_CHECK(out != nullptr, "track_multi_sample_flush: null argument");
   MN_CHECK(s >= 0 && s < h->n_streams, "track_multi_sample_flush: stream %d outside [0, %d)", s, h->n_streams);
   if (h->lag == 0) return 0;                 // every window was complete when its last frame arrived
-  return track_multi_sample_launch(h, nullptr, nullptr, nullptr, nullptr, 0, s, out, nullptr, (cudaStream_t)stream);
+  return track_multi_launch(h, SampleFactor(*h, nullptr, nullptr), nullptr, nullptr, 0, s, out, nullptr,
+                            (cudaStream_t)stream);
 }
 
 int mapnet_track_multi_sample_reset(mapnet_track_multi_sample_t* h, int s, void* stream) {
   MN_CHECK(h != nullptr, "track_multi_sample_reset: null handle");
   MN_CHECK(s >= -1 && s < h->n_streams, "track_multi_sample_reset: stream %d outside [-1, %d)", s, h->n_streams);
-  const size_t n = s < 0 ? (size_t)h->n_streams : 1;
-  MN_CUDA(cudaMemsetAsync(h->st + (s < 0 ? 0 : s), 0, n * sizeof(MTrackDev), (cudaStream_t)stream));
-  return 0;
+  return track_reset(h, s, (cudaStream_t)stream);
 }
 
 int mapnet_track_multi_sample_status(mapnet_track_multi_sample_t* h, int s, int64_t* frames_seen, int* failed,
                                      void* stream) {
   MN_CHECK(h != nullptr, "track_multi_sample_status: null handle");
   MN_CHECK(s >= 0 && s < h->n_streams, "track_multi_sample_status: stream %d outside [0, %d)", s, h->n_streams);
-  MTrackDev d;
-  MN_CUDA(cudaMemcpyAsync(&d, h->st + s, sizeof(MTrackDev), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  MN_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-  if (frames_seen != nullptr) *frames_seen = d.seen;
-  if (failed != nullptr) *failed = d.status;
-  return 0;
+  return track_status(h, s, frames_seen, failed, (cudaStream_t)stream);
 }
 
-int mapnet_track_multi_sample_destroy(mapnet_track_multi_sample_t* h) {
-  if (h == nullptr) return 0;
-  cudaFree(h->st); cudaFree(h->n_win); cudaFree(h->ring7); cudaFree(h->ring49); cudaFree(h->ring_vo);
-  cudaFree(h->win7); cudaFree(h->win49); cudaFree(h->vos7); cudaFree(h->opt7); cudaFree(h->cov36);
-  delete h;
-  return 0;
-}
+int mapnet_track_multi_sample_destroy(mapnet_track_multi_sample_t* h) { return track_destroy(h); }
 
 int mapnet_frame_cache_destroy(mapnet_frame_cache_t* h) {
   if (h == nullptr) return 0;

@@ -571,7 +571,8 @@ class Tracker(object):
     sizes.  A window whose normal matrix is not positive definite (where scipy's cholesky raises) is reported by
     flush(), which raises np.linalg.LinAlgError after resetting."""
 
-    _DESTROY = "mapnet_track_destroy"      # the C call that frees the handle
+    _API = "mapnet_track"       # the handle's C calls: _API + "_create", "_step", "_step_now", "_flush", ...
+    _ROW = 7                    # doubles per output row
 
     def __init__(self, localizer, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0):
         if not isinstance(localizer, Localizer):
@@ -584,8 +585,8 @@ class Tracker(object):
         self.loc, self.vo_fc = localizer, bool(vo_fc)
         self.lag = (self.steps - 1 - self.steps // 2) * self.skip
         self.seen = 0           # frames of the current sequence, mirrored on the device
-        self._graphs = {}       # (B, H, W) -> (CUDAGraph, static uint8 input, vo [B,6], out [B,7], pred6 [B,6])
-        self._now_graphs = {}   # the same for step(), with now7 [B,7] last
+        self._graphs = {}       # (B, H, W) -> (CUDAGraph, static uint8 input, vo [B,6], out [B,_ROW], engine outputs)
+        self._now_graphs = {}   # the same for step(), with now [B,_ROW] last
         self.h = ctypes.c_void_p()      # mapnet_track_t, created with the first call
         self._open = True
 
@@ -607,13 +608,23 @@ class Tracker(object):
                 list(want), "one [H,W,3] frame" if single else "%d frames" % n, tuple(v.shape)))
         return v.reshape(n, 6)
 
+    @staticmethod
+    def _est(rows):
+        """what a caller gets for output rows [n, _ROW]: pose7 itself"""
+        return rows
+
+    def _capture(self, fb, track):
+        """(CUDA graph, static uint8 input, engine outputs) of frames shaped like fb: the Localizer's engine, then
+        track(*engine outputs)'s launches"""
+        return self.loc._capture(fb, track, eager_tail=False)  # the eager run must not advance the stream
+
     def _handle(self):
         if not self.h:
             pr = self.loc.predictor
             sig = (ctypes.c_double * 4)(*self.sigmas)
-            _lib.check(_lib.lib().mapnet_track_create(ctypes.byref(self.h), self.steps, self.skip, int(self.vo_fc),
-                                                      pr.max_batch, sig, self.loc._m, self.loc._s),
-                       "mapnet_track_create")
+            _lib.check(getattr(_lib.lib(), self._API + "_create")(ctypes.byref(self.h), self.steps, self.skip,
+                                                                  int(self.vo_fc), pr.max_batch, sig, self.loc._m,
+                                                                  self.loc._s), self._API + "_create")
         return self.h
 
     def _graph(self, fb, now=False):
@@ -623,25 +634,21 @@ class Tracker(object):
         if g is None:
             dev, h = self.loc.predictor.device, self._handle()
             vs = torch.zeros((B, 6), dtype=torch.float32, device=dev)
-            out = torch.empty((B, 7), dtype=torch.float64, device=dev)
-            now7 = torch.empty((B, 7), dtype=torch.float64, device=dev) if now else None
+            out = torch.empty((B, self._ROW), dtype=torch.float64, device=dev)
+            nows = (torch.empty((B, self._ROW), dtype=torch.float64, device=dev),) if now else ()
+            name = self._API + ("_step_now" if now else "_step")
 
-            def track(pred):
-                if now:
-                    _lib.check(_lib.lib().mapnet_track_step_now(h, pred.data_ptr(), vs.data_ptr(), B, out.data_ptr(),
-                                                                now7.data_ptr(), _lib.stream_ptr()),
-                               "mapnet_track_step_now")
-                else:
-                    _lib.check(_lib.lib().mapnet_track_step(h, pred.data_ptr(), vs.data_ptr(), B, out.data_ptr(),
-                                                            _lib.stream_ptr()), "mapnet_track_step")
+            def track(*ins):
+                _lib.check(getattr(_lib.lib(), name)(h, *[t.data_ptr() for t in ins], vs.data_ptr(), B, out.data_ptr(),
+                                                     *[t.data_ptr() for t in nows], _lib.stream_ptr()), name)
 
-            graph, xs, pred = self.loc._capture(fb, track, eager_tail=False)  # the eager run must not advance the stream
-            g = (graph, xs, vs, out, pred) + ((now7,) if now else ())     # every buffer the graph reads stays alive
+            graph, xs, ins = self._capture(fb, track)
+            g = (graph, xs, vs, out, ins) + nows        # every buffer the graph reads stays alive
             graphs[(B, H, W)] = g
         return g
 
     def _run(self, frames, vo_poses, now):
-        """(first, pose7 [n,7], now7 [B,7] or None): the chunks of max_batch frames, one graph replay each"""
+        """(first, rows [n,_ROW], now rows [B,_ROW] or None): the chunks of max_batch frames, one graph replay each"""
         self._check_open()
         x, single = self.loc._frames(frames)
         vo = self._vo(vo_poses, x.shape[0], single)
@@ -668,8 +675,8 @@ class Tracker(object):
     def __call__(self, frames, vo_poses):
         """-> (first, pose7 float64 [n,7] on the device): the frames first .. first+n-1 whose windows this call
         completed, n = max(seen + B - lag, 0) - max(seen - lag, 0) for the B frames given"""
-        first, pose7, _ = self._run(frames, vo_poses, False)
-        return first, pose7
+        first, rows, _ = self._run(frames, vo_poses, False)
+        return first, self._est(rows)
 
     @torch.no_grad()
     def step(self, frames, vo_poses):
@@ -677,8 +684,8 @@ class Tracker(object):
         frame given, f = seen + b: slot steps-1 of the optimised window that ends at f (frame (f - lag)'s window,
         clipped at 0), un-normalised as pose7; (first, pose7) is what self(frames, vo_poses) returns.  Takes what
         __call__ takes; each chunk replays a graph of its own, the same three tracking launches."""
-        first, pose7, now7 = self._run(frames, vo_poses, True)
-        return now7, first, pose7
+        first, rows, nows = self._run(frames, vo_poses, True)
+        return self._est(nows), first, self._est(rows)
 
     @torch.no_grad()
     def flush(self):
@@ -690,24 +697,25 @@ class Tracker(object):
         first = _first_pending(self.seen, self.lag)
         n, failed = self.seen - first, ctypes.c_int(0)
         with torch.cuda.device(pr.device):
-            out = torch.empty((max(self.lag, 1), 7), dtype=torch.float64, device=pr.device)
+            out = torch.empty((max(self.lag, 1), self._ROW), dtype=torch.float64, device=pr.device)
             if self.h:
                 L = _lib.lib()
-                _lib.check(L.mapnet_track_flush(self.h, out.data_ptr(), _lib.stream_ptr()), "mapnet_track_flush")
-                _lib.check(L.mapnet_track_status(self.h, None, ctypes.byref(failed), _lib.stream_ptr()),
-                           "mapnet_track_status")
+                _lib.check(getattr(L, self._API + "_flush")(self.h, out.data_ptr(), _lib.stream_ptr()),
+                           self._API + "_flush")
+                _lib.check(getattr(L, self._API + "_status")(self.h, None, ctypes.byref(failed), _lib.stream_ptr()),
+                           self._API + "_status")
         self.reset()
         if failed.value:
             raise np.linalg.LinAlgError("pose graph: the normal matrix of a window of the sequence is not positive "
                                         "definite")
-        return first, out[:n]
+        return first, self._est(out[:n])
 
     def reset(self):
         """Start a new sequence: the next frame is frame 0 (stream-ordered)."""
         self._check_open()
         if self.h:
             with torch.cuda.device(self.loc.predictor.device):
-                _lib.check(_lib.lib().mapnet_track_reset(self.h, _lib.stream_ptr()), "mapnet_track_reset")
+                _lib.check(getattr(_lib.lib(), self._API + "_reset")(self.h, _lib.stream_ptr()), self._API + "_reset")
         self.seen = 0
 
     def close(self):
@@ -716,7 +724,7 @@ class Tracker(object):
             torch.cuda.current_stream(self.loc.predictor.device).synchronize()
             self._graphs.clear()
             self._now_graphs.clear()
-            getattr(_lib.lib(), self._DESTROY)(self.h)
+            getattr(_lib.lib(), self._API + "_destroy")(self.h)
             self.h = ctypes.c_void_p()
         self._open = False
 
@@ -789,45 +797,12 @@ class SampledTracker(Tracker):
     the sequence.  Engines, snapshot, refresh(), precision and dropout counter are the Localizer's predictor's.  S as
     Localizer.sample takes it: 2 <= S <= 1024, and a model without dropout raises ValueError."""
 
-    _DESTROY = "mapnet_track_sample_destroy"
+    _API = "mapnet_track_sample"
+    _ROW = _lib.TRACK_SAMPLE_ROW
 
     def __init__(self, localizer, S, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0):
         super(SampledTracker, self).__init__(localizer, steps, skip, vo_fc, sax, saq, srx, srq)
         self.S = _check_draws(S, localizer.predictor.droprate)
-
-    def _handle(self):
-        if not self.h:
-            pr = self.loc.predictor
-            sig = (ctypes.c_double * 4)(*self.sigmas)
-            _lib.check(_lib.lib().mapnet_track_sample_create(ctypes.byref(self.h), self.steps, self.skip,
-                                                             int(self.vo_fc), pr.max_batch, sig, self.loc._m,
-                                                             self.loc._s), "mapnet_track_sample_create")
-        return self.h
-
-    def _graph(self, fb, now=False):
-        B, H, W = fb.shape[:3]
-        graphs = self._now_graphs if now else self._graphs
-        g = graphs.get((B, H, W))
-        if g is None:
-            dev, h, L = self.loc.predictor.device, self._handle(), _lib.lib()
-            f64 = dict(dtype=torch.float64, device=dev)
-            vs = torch.zeros((B, 6), dtype=torch.float32, device=dev)
-            row = _lib.TRACK_SAMPLE_ROW
-            out = torch.empty((B, row), **f64)
-            nowb = torch.empty((B, row), **f64) if now else None
-
-            def track(mean, cov):
-                if now:
-                    _lib.check(L.mapnet_track_sample_step_now(h, mean.data_ptr(), cov.data_ptr(), vs.data_ptr(), B,
-                                                              out.data_ptr(), nowb.data_ptr(), _lib.stream_ptr()),
-                               "mapnet_track_sample_step_now")
-                else:
-                    _lib.check(L.mapnet_track_sample_step(h, mean.data_ptr(), cov.data_ptr(), vs.data_ptr(), B,
-                                                          out.data_ptr(), _lib.stream_ptr()), "mapnet_track_sample_step")
-
-            graph, xs, draws = _sampled_capture(self.loc, self.S, fb, track)
-            g = graphs[(B, H, W)] = (graph, xs, vs, out, draws, nowb)   # every buffer the graph reads
-        return g
 
     @staticmethod
     def _est(rows):
@@ -835,72 +810,8 @@ class SampledTracker(Tracker):
         return dict(pose7=rows[:, :7].contiguous(), cov=rows[:, 7:43].reshape(-1, 6, 6).contiguous(),
                     t_std=rows[:, 43].contiguous(), q_std_deg=rows[:, 44].contiguous())
 
-    def _run(self, frames, vo_poses, now):
-        """(first, rows [n,45], now rows [B,45] or None): the chunks of max_batch frames, one graph replay each"""
-        self._check_open()
-        x, single = self.loc._frames(frames)
-        vo = self._vo(vo_poses, x.shape[0], single)
-        pr = self.loc.predictor
-        mb, first = pr.max_batch, _first_pending(self.seen, self.lag)
-        outs, nows = [], []
-        with torch.cuda.device(pr.device):
-            for lo in range(0, x.shape[0], mb):
-                fb = x[lo:lo + mb]
-                g = self._graph(fb, now)
-                graph, xs, vs, out = g[:4]
-                xs.copy_(fb, non_blocking=True)
-                vs.copy_(vo[lo:lo + mb], non_blocking=True)
-                graph.replay()
-                n = _first_pending(self.seen + fb.shape[0], self.lag) - _first_pending(self.seen, self.lag)
-                self.seen += fb.shape[0]
-                outs.append(out[:n].clone())
-                if now:
-                    nows.append(g[5].clone())
-        cat = lambda ts: ts[0] if len(ts) == 1 else torch.cat(ts, 0)
-        return first, cat(outs), (cat(nows) if now else None)
-
-    @torch.no_grad()
-    def __call__(self, frames, vo_poses):
-        """-> (first, est): the frames first .. first+n-1 whose windows this call completed (Tracker.__call__)"""
-        first, rows, _ = self._run(frames, vo_poses, False)
-        return first, self._est(rows)
-
-    @torch.no_grad()
-    def step(self, frames, vo_poses):
-        """-> (now, first, est): now holds each given frame's zero-lag estimate (Tracker.step's window), one row per
-        frame; (first, est) is what self(frames, vo_poses) returns"""
-        first, rows, nows = self._run(frames, vo_poses, True)
-        return self._est(nows), first, self._est(rows)
-
-    @torch.no_grad()
-    def flush(self):
-        """-> (first, est): the last n = min(lag, seen) frames, as Tracker.flush; raises np.linalg.LinAlgError after
-        resetting when a window's normal matrix or a frame's factor covariance was not positive definite"""
-        self._check_open()
-        pr = self.loc.predictor
-        first = _first_pending(self.seen, self.lag)
-        n, failed = self.seen - first, ctypes.c_int(0)
-        with torch.cuda.device(pr.device):
-            out = torch.empty((max(self.lag, 1), _lib.TRACK_SAMPLE_ROW), dtype=torch.float64, device=pr.device)
-            if self.h:
-                L = _lib.lib()
-                _lib.check(L.mapnet_track_sample_flush(self.h, out.data_ptr(), _lib.stream_ptr()),
-                           "mapnet_track_sample_flush")
-                _lib.check(L.mapnet_track_sample_status(self.h, None, ctypes.byref(failed), _lib.stream_ptr()),
-                           "mapnet_track_sample_status")
-        self.reset()
-        if failed.value:
-            raise np.linalg.LinAlgError("pose graph: the normal matrix of a window of the sequence is not positive "
-                                        "definite")
-        return first, self._est(out[:n])
-
-    def reset(self):
-        """Start a new sequence: the next frame is frame 0 (stream-ordered)."""
-        self._check_open()
-        if self.h:
-            with torch.cuda.device(self.loc.predictor.device):
-                _lib.check(_lib.lib().mapnet_track_sample_reset(self.h, _lib.stream_ptr()), "mapnet_track_sample_reset")
-        self.seen = 0
+    def _capture(self, fb, track):
+        return _sampled_capture(self.loc, self.S, fb, track)
 
 
 def _stream_records(seen, streams, lag):
@@ -961,19 +872,12 @@ class MultiTracker(Tracker):
     positive definite marks its own stream only: flush(s) raises np.linalg.LinAlgError for stream s after resetting
     it."""
 
-    _DESTROY = "mapnet_track_multi_destroy"
-    _API = "mapnet_track_multi"     # the handle's C calls: _API + "_create", "_flush", "_status", "_reset"
-    _ROW = 7                        # doubles per output row
+    _API = "mapnet_track_multi"
 
     def __init__(self, localizer, n_streams, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0):
         super(MultiTracker, self).__init__(localizer, steps, skip, vo_fc, sax, saq, srx, srq)
         self.n_streams = _int_arg(n_streams, "n_streams", 1, _lib.MAX_TRACK_STREAMS)
         self.seen = np.zeros(self.n_streams, dtype=np.int64)    # frames of each stream's sequence, mirrored on the device
-
-    @staticmethod
-    def _est(rows):
-        """what a caller gets for output rows [n, _ROW]: pose7 itself"""
-        return rows
 
     def _handle(self):
         if not self.h:
@@ -1007,23 +911,24 @@ class MultiTracker(Tracker):
         graphs = self._now_graphs if now else self._graphs
         g = graphs.get((B, H, W))
         if g is None:
-            dev, h = self.loc.predictor.device, self._handle()
+            dev, h, name = self.loc.predictor.device, self._handle(), self._API + "_step"
             vs = torch.zeros((B, 6), dtype=torch.float32, device=dev)
             rs = torch.zeros((B, 6), dtype=torch.int32, device=dev)
-            out = torch.empty((B, 7), dtype=torch.float64, device=dev)
-            now7 = torch.empty((B, 7), dtype=torch.float64, device=dev) if now else None
+            out = torch.empty((B, self._ROW), dtype=torch.float64, device=dev)
+            nowb = torch.empty((B, self._ROW), dtype=torch.float64, device=dev) if now else None
 
-            def track(pred):
-                _lib.check(_lib.lib().mapnet_track_multi_step(h, pred.data_ptr(), vs.data_ptr(), rs.data_ptr(), B,
-                                                              out.data_ptr(), now7.data_ptr() if now else None,
-                                                              _lib.stream_ptr()), "mapnet_track_multi_step")
+            def track(*ins):
+                _lib.check(getattr(_lib.lib(), name)(h, *[t.data_ptr() for t in ins], vs.data_ptr(), rs.data_ptr(), B,
+                                                     out.data_ptr(), nowb.data_ptr() if now else None,
+                                                     _lib.stream_ptr()), name)
 
-            graph, xs, pred = self.loc._capture(fb, track, eager_tail=False)  # the eager run must not advance a stream
-            g = graphs[(B, H, W)] = (graph, xs, vs, rs, out, pred, now7)     # every buffer the graph reads stays alive
+            graph, xs, ins = self._capture(fb, track)
+            g = graphs[(B, H, W)] = (graph, xs, vs, rs, out, ins, nowb)     # every buffer the graph reads stays alive
         return g
 
     def _run(self, frames, vo_poses, streams, now):
-        """(sid [n], fid [n], pose7 [n,7], now7 [B,7] or None): the chunks of max_batch frames, one graph replay each"""
+        """(sid [n], fid [n], rows [n,_ROW], now rows [B,_ROW] or None): the chunks of max_batch frames, one graph
+        replay each"""
         self._check_open()
         x, single = self.loc._frames(frames)
         vo = self._vo(vo_poses, x.shape[0], single)
@@ -1050,15 +955,15 @@ class MultiTracker(Tracker):
     @torch.no_grad()
     def __call__(self, frames, vo_poses, streams):
         """-> (sid int64 [n], fid int64 [n], pose7 float64 [n,7] on the device): the windows this call completes"""
-        sid, fid, pose7, _ = self._run(frames, vo_poses, streams, False)
-        return sid, fid, pose7
+        sid, fid, rows, _ = self._run(frames, vo_poses, streams, False)
+        return sid, fid, self._est(rows)
 
     @torch.no_grad()
     def step(self, frames, vo_poses, streams):
         """-> (now7 float64 [B,7] on the device, sid, fid, pose7): row b of now7 is the zero-lag pose of the b-th frame
         given, as Tracker.step defines it for that frame's stream; (sid, fid, pose7) is what __call__ returns"""
-        sid, fid, pose7, now7 = self._run(frames, vo_poses, streams, True)
-        return now7, sid, fid, pose7
+        sid, fid, rows, nows = self._run(frames, vo_poses, streams, True)
+        return self._est(nows), sid, fid, self._est(rows)
 
     @torch.no_grad()
     def flush(self, s):
@@ -1125,49 +1030,14 @@ class SampledMultiTracker(MultiTracker):
     covariances is not positive definite marks its own stream only: flush(s) raises np.linalg.LinAlgError for stream s
     after resetting it."""
 
-    _DESTROY = "mapnet_track_multi_sample_destroy"
     _API = "mapnet_track_multi_sample"
-    _ROW = _lib.TRACK_SAMPLE_ROW
+    _ROW = SampledTracker._ROW
     _est = staticmethod(SampledTracker._est)
+    _capture = SampledTracker._capture
 
     def __init__(self, localizer, S, n_streams, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0):
         super(SampledMultiTracker, self).__init__(localizer, n_streams, steps, skip, vo_fc, sax, saq, srx, srq)
         self.S = _check_draws(S, localizer.predictor.droprate)
-
-    def _graph(self, fb, now=False):
-        B, H, W = fb.shape[:3]
-        graphs = self._now_graphs if now else self._graphs
-        g = graphs.get((B, H, W))
-        if g is None:
-            dev, h, L = self.loc.predictor.device, self._handle(), _lib.lib()
-            f64 = dict(dtype=torch.float64, device=dev)
-            vs = torch.zeros((B, 6), dtype=torch.float32, device=dev)
-            rs = torch.zeros((B, 6), dtype=torch.int32, device=dev)
-            out = torch.empty((B, self._ROW), **f64)
-            nowb = torch.empty((B, self._ROW), **f64) if now else None
-
-            def track(mean, cov):
-                _lib.check(L.mapnet_track_multi_sample_step(h, mean.data_ptr(), cov.data_ptr(), vs.data_ptr(),
-                                                            rs.data_ptr(), B, out.data_ptr(),
-                                                            nowb.data_ptr() if now else None, _lib.stream_ptr()),
-                           "mapnet_track_multi_sample_step")
-
-            graph, xs, draws = _sampled_capture(self.loc, self.S, fb, track)
-            g = graphs[(B, H, W)] = (graph, xs, vs, rs, out, draws, nowb)     # MultiTracker._run's layout
-        return g
-
-    @torch.no_grad()
-    def __call__(self, frames, vo_poses, streams):
-        """-> (sid int64 [n], fid int64 [n], est): the windows this call completes (MultiTracker.__call__)"""
-        sid, fid, rows, _ = self._run(frames, vo_poses, streams, False)
-        return sid, fid, self._est(rows)
-
-    @torch.no_grad()
-    def step(self, frames, vo_poses, streams):
-        """-> (now, sid, fid, est): now holds each given frame's zero-lag estimate, one row per frame in the order
-        given (MultiTracker.step's windows); (sid, fid, est) is what __call__ returns"""
-        sid, fid, rows, nows = self._run(frames, vo_poses, streams, True)
-        return self._est(nows), sid, fid, self._est(rows)
 
 
 def pgo(pred7, vos7, sax=1.0, saq=1.0, srx=1.0, srq=1.0, fc_vos=False):

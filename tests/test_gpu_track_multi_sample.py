@@ -481,6 +481,6 @@ def test_one_replay_of_the_sampled_engine_and_three_tracking_launches_per_chunk(
         smt(fr[:4], vo[:4], [2, 1, 0, 2])
         torch.cuda.synchronize()
     names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-    for k in ("k_track_multi_sample_gather", "k_pgo_cov", "k_track_multi_sample_emit"):
+    for k in ("k_track_multi_gather<mapnet::SampleFactor>", "k_pgo_cov", "k_track_multi_emit<mapnet::SampleFactor>"):
         assert sum(k in n for n in names) == 1, (k, names)
     smt.close(); la.close(); lb.close(); pa.close(); pb.close()

@@ -371,6 +371,6 @@ def test_one_replay_of_the_sampled_engine_and_three_tracking_launches_per_chunk(
         st(frames[:4], vo[:4])
         torch.cuda.synchronize()
     names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-    for k in ("k_track_sample_gather", "k_pgo_cov", "k_track_sample_emit"):
+    for k in ("k_track_gather<mapnet::SampleFactor>", "k_pgo_cov", "k_track_emit<mapnet::SampleFactor>"):
         assert sum(k in n for n in names) == 1, (k, names)
     st.close(); loc.close(); pa.close()
