@@ -27,6 +27,7 @@ TRACK_SAMPLE_API = ["mapnet_track_sample_create", "mapnet_track_sample_step", "m
                     "mapnet_track_sample_flush", "mapnet_track_sample_reset", "mapnet_track_sample_status",
                     "mapnet_track_sample_destroy"]
 TRACK_SAMPLE_ROW = 45       # mapnet_track_sample_step: pose7 [7], cov [36], t_std, q_std_deg per output row
+EVAL_SAMPLE_API = ["mapnet_eval_sample_windows", "mapnet_eval_sample_emit"]
 TRACK_MULTI_SAMPLE_API = ["mapnet_track_multi_sample_create", "mapnet_track_multi_sample_step",
                           "mapnet_track_multi_sample_flush", "mapnet_track_multi_sample_reset",
                           "mapnet_track_multi_sample_status", "mapnet_track_multi_sample_destroy"]
@@ -114,6 +115,13 @@ def lib():
     L.mapnet_eval_windows.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int,
                                       c_void_p, c_void_p, c_void_p, c_void_p]
     L.mapnet_eval_windows.restype = c_int
+    L.mapnet_eval_sample_windows.argtypes = [c_void_p, c_void_p, c_int, ctypes.c_double, ctypes.c_double, c_void_p, c_int,
+                                             c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
+    L.mapnet_eval_sample_emit.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int,
+                                          c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_void_p, c_void_p, c_void_p]
+    for name in EVAL_SAMPLE_API:
+        getattr(L, name).restype = c_int
     L.mapnet_batch_losses.argtypes = [c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int,
                                       c_void_p, c_void_p, c_void_p]
     L.mapnet_batch_losses.restype = c_int
@@ -246,7 +254,7 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_batch_losses", "mapnet_infer_forward_frames", "mapnet_test_stem_operand", "mapnet_infer_sample",
             "mapnet_infer_sample_frames", "mapnet_sample_post", "mapnet_test_small_gemm_plan", "mapnet_test_stem_ex",
             "mapnet_test_head", "mapnet_pgo_optimize_cov",
-            "mapnet_test_sample_factor", "mapnet_test_weight_table", "mapnet_test_pack_weights"] + TRACK_API + TRACK_MULTI_API + TRACK_SAMPLE_API + TRACK_MULTI_SAMPLE_API
+            "mapnet_test_sample_factor", "mapnet_test_weight_table", "mapnet_test_pack_weights"] + TRACK_API + TRACK_MULTI_API + TRACK_SAMPLE_API + TRACK_MULTI_SAMPLE_API + EVAL_SAMPLE_API
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 MAX_SAMPLE_DRAWS = 1024      # mapnet_infer_sample: S in [2, MAX_SAMPLE_DRAWS] dropout draws per frame
 

@@ -13,6 +13,7 @@
 #include "pose_math.h"
 #include "pose_post.cuh"
 #include "track_core.h"
+#include "calib_core.h"
 
 #include "../../include/mapnet_b200.h"
 
@@ -85,6 +86,14 @@ __device__ __forceinline__ void st_pose7(const float* p6, double* o7) {
   post_qexp(p6[3], p6[4], p6[5], o7 + 3);
 }
 
+// calc_vos_safe / calc_vos_safe_fc (common/pose_utils.py:276-304) of VO pair p on the VO library's float32 poses, as the
+// MFOnline targets of k_loader_assemble
+__device__ __forceinline__ void eval_vo(const float* vo_poses, const TargRow p, double* o7) {
+  const posemath::Pose6 v = posemath::calc_vo_logq_safe(ld_pose6(vo_poses + 6LL * p.a), ld_pose6(vo_poses + 6LL * p.b));
+  const float v6[6] = {v.t.x, v.t.y, v.t.z, v.l.x, v.l.y, v.l.z};
+  st_pose7(v6, o7);
+}
+
 __global__ void __launch_bounds__(128)
 k_eval_windows(const float* __restrict__ pred6, const float* __restrict__ poses, const float* __restrict__ vo_poses,
                const int* __restrict__ frame, const int* __restrict__ slot, int n_rows, const TargRow* __restrict__ vo_rows,
@@ -96,12 +105,7 @@ k_eval_windows(const float* __restrict__ pred6, const float* __restrict__ poses,
     st_pose7(poses + 6LL * frame[r], targ7 + 7LL * r);
   } else if (r < n_rows + n_vo) {
     const int k = r - n_rows;
-    const TargRow p = vo_rows[k];
-    // calc_vos_safe / calc_vos_safe_fc (common/pose_utils.py:276-304) on the VO library's float32 poses, as the
-    // MFOnline targets of k_loader_assemble
-    const posemath::Pose6 v = posemath::calc_vo_logq_safe(ld_pose6(vo_poses + 6LL * p.a), ld_pose6(vo_poses + 6LL * p.b));
-    const float v6[6] = {v.t.x, v.t.y, v.t.z, v.l.x, v.l.y, v.l.z};
-    st_pose7(v6, vos7 + 7LL * k);
+    eval_vo(vo_poses, vo_rows[k], vos7 + 7LL * k);
   }
 }
 
@@ -171,11 +175,16 @@ __device__ __forceinline__ void qexp_jac(const double v[3], double Ej[4][3]) {
   }
 }
 
+// one frame's absolute pose p7 = (mean_t, qexp(mean_v)) from its draws' mean [6]
+__device__ __forceinline__ void sample_pose7(const double* mu, double p7[7]) {
+  p7[0] = mu[0]; p7[1] = mu[1]; p7[2] = mu[2];
+  sample_qexp(mu[3], mu[4], mu[5], p7 + 3);
+}
+
 // one frame's absolute pose p7 and factor covariance S7 [7][7] from its draws' mean [6] and covariance [36]
 __device__ __forceinline__ void sample_factor(const double* mu, const double* C, double sax, double saq, double p7[7],
                                               double S7[49]) {
-  p7[0] = mu[0]; p7[1] = mu[1]; p7[2] = mu[2];
-  sample_qexp(mu[3], mu[4], mu[5], p7 + 3);
+  sample_pose7(mu, p7);
   double Ej[4][3];
   qexp_jac(mu + 3, Ej);
   double A[7][6] = {};
@@ -255,6 +264,10 @@ struct SampleFactor {
   SampleFactor(const TrackHandle& h, const double* mean_, const double* cov_)
       : mean(mean_), cov(cov_), sax(h.sax), saq(h.saq), ring7(h.ring7), ring49(h.ring49), win7(h.win7),
         win49(h.win49), opt7(h.opt7), cov36(h.cov36) {}
+  // window slots alone, without a tracker (k_eval_sample_windows)
+  SampleFactor(const double* mean_, const double* cov_, double sax_, double saq_, double* win7_, double* win49_)
+      : mean(mean_), cov(cov_), sax(sax_), saq(saq_), ring7(nullptr), ring49(nullptr), win7(win7_), win49(win49_),
+        opt7(nullptr), cov36(nullptr) {}
   // the frame's mean and covariance through the read-only path into registers first: the struct's pointers carry no
   // restrict, so sample_factor reading them in place would reload the covariance after every store of S7
   __device__ __forceinline__ void form(long long b, bool ring, long long q) const {
@@ -518,6 +531,50 @@ k_track_multi_emit(F fac, const int* __restrict__ win_fail, const MTrackRec* __r
   if (win_fail[w]) atomicExch(&st[s].status, 1);
 }
 
+// ---- Monte-Carlo evaluation windows (mapnet_eval_sample_*, inference.evaluate_sequence(samples=S)): every frame's
+// S-draw mean [6] and covariance [36] once, shared by every window slot that holds it, as the sampled trackers share
+// them.  One thread per row: slot r < n_rows gets the factor (p7, S7) of frame row slot[r], formed by SampleFactor as
+// the tracker forms it into its rings (bit for bit), and VO k the row k_eval_windows writes.
+__global__ void __launch_bounds__(128)
+k_eval_sample_windows(SampleFactor fac, const float* __restrict__ vo_poses, const int* __restrict__ slot, int n_rows,
+                      const TargRow* __restrict__ vo_rows, int n_vo, double* __restrict__ vos7) {
+  pdl_prologue();
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < n_rows) fac.form(slot[r], false, r);
+  else if (r < n_rows + n_vo) eval_vo(vo_poses, vo_rows[r - n_rows], vos7 + 7LL * (r - n_rows));
+}
+
+// One thread per item i: its estimate as a kTrackSampleRow row (track_sample_row: pose7 un-normalised as
+// _window_errors does, D cov D, t_std, q_std_deg) -- slot `keep` of its optimised window (opt7 / post36 rows i*T + keep)
+// or, without a pose graph (opt7 null), the draws' own mean and covariance of frame row slot[i] -- its target (st_pose7
+// of poses[frame[i]], un-normalised alike) and calibcore::score of the row's pose7 and covariance against the target.
+__global__ void __launch_bounds__(128)
+k_eval_sample_emit(const double* __restrict__ mean, const double* __restrict__ cov, const double* __restrict__ opt7,
+                   const double* __restrict__ post36, int T, int keep, const float* __restrict__ poses,
+                   const int* __restrict__ frame, const int* __restrict__ slot, int n, int un, double m0, double m1,
+                   double m2, double s0, double s1, double s2, double* __restrict__ out, double* __restrict__ targ7,
+                   double* __restrict__ d2, double* __restrict__ u, double* __restrict__ nll) {
+  pdl_prologue();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double ms[3] = {m0, m1, m2}, ss[3] = {s0, s1, s2};
+  double* o = out + (long long)kTrackSampleRow * i;
+  if (opt7 != nullptr) {
+    const long long r = (long long)i * T + keep;
+    track_sample_row(opt7 + 7 * r, post36 + 36 * r, un, ms, ss, o);
+  } else {
+    double mu[6], p7[7];
+    for (int c = 0; c < 6; ++c) mu[c] = mean[6LL * slot[i] + c];
+    sample_pose7(mu, p7);
+    track_sample_row(p7, cov + 36LL * slot[i], un, ms, ss, o);
+  }
+  double t7[7];
+  st_pose7(poses + 6LL * frame[i], t7);
+  double* tg = targ7 + 7LL * i;
+  track_emit_pose(t7, un, ms, ss, tg);
+  calibcore::score(o, tg, o + 7, d2 + 3LL * i, u + 3LL * i, nll + i);
+}
+
 }  // namespace mapnet
 
 using namespace mapnet;
@@ -673,6 +730,89 @@ int mapnet_eval_windows(const float* pred6, int n_pred, const float* poses, cons
   if (n_vo > 0) MN_CUDA(cudaMemcpyAsync(d + 2 * n_rows, vo_rows, 2 * (size_t)n_vo * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   MN_LAUNCH(k_eval_windows, (int)cdiv((long long)n_rows + n_vo, 128), 128, 0, st, pred6, poses, vo_poses, (const int*)d,
             (const int*)(d + n_rows), n_rows, (const TargRow*)(d + 2 * n_rows), n_vo, pred7, targ7, vos7);
+  MN_LAUNCH_CHECK();
+  MN_CUDA(cudaFreeAsync(d, st));
+  return 0;
+}
+
+// the checks both Monte-Carlo evaluation entry points share: the frame rows' count, every slot row and every frame or
+// VO pose index inside its table
+static int eval_sample_rows(const char* who, int n_pred, int n_poses, const int32_t* frame, const int32_t* slot,
+                            int n_rows, const int32_t* vo_rows, int n_vo) {
+  for (int r = 0; r < n_rows; ++r) {
+    MN_CHECK((frame == nullptr || (frame[r] >= 0 && frame[r] < n_poses)) && slot[r] >= 0 && slot[r] < n_pred,
+             "%s: row %d = (frame %d, slot %d) outside the %d poses / %d frame rows", who, r,
+             frame != nullptr ? frame[r] : 0, slot[r], n_poses, n_pred);
+  }
+  for (int k = 0; k < 2 * n_vo; ++k)
+    MN_CHECK(vo_rows[k] >= 0 && vo_rows[k] < n_poses, "%s: VO row %d = (%d, %d) outside the %d poses", who, k / 2,
+             vo_rows[k & ~1], vo_rows[k | 1], n_poses);
+  return 0;
+}
+
+int mapnet_eval_sample_windows(const double* mean6, const double* cov36, int n_pred, double sax, double saq,
+                               const float* vo_poses, int n_poses, const int32_t* slot, int n_rows,
+                               const int32_t* vo_rows, int n_vo, double* p7, double* s7, double* vos7, void* stream) {
+  MN_CHECK(mean6 != nullptr && cov36 != nullptr && slot != nullptr && p7 != nullptr && s7 != nullptr,
+           "eval_sample_windows: null argument");
+  MN_CHECK(n_rows >= 1 && n_pred >= 1 && n_poses >= 1 && n_vo >= 0, "eval_sample_windows: bad count");
+  MN_CHECK(sax > 0 && saq > 0, "eval_sample_windows: sax = %g and saq = %g must be positive", sax, saq);
+  MN_CHECK(n_vo == 0 || (vo_poses != nullptr && vo_rows != nullptr && vos7 != nullptr),
+           "eval_sample_windows: %d VO rows need vo_poses, vo_rows and vos7", n_vo);
+  MN_CHECK((long long)n_rows + n_vo < (1LL << 31), "eval_sample_windows: %d + %d rows", n_rows, n_vo);
+  MN_TRY(eval_sample_rows("eval_sample_windows", n_pred, n_poses, nullptr, slot, n_rows, vo_rows, n_vo));
+  MN_CHECK(device_memory(mean6) && device_memory(cov36) && device_memory(p7) && device_memory(s7) &&
+           (n_vo == 0 || (device_memory(vo_poses) && device_memory(vos7))),
+           "eval_sample_windows: tensors must be device memory");
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t bytes = ((size_t)n_rows + 2 * (size_t)n_vo) * sizeof(int32_t);
+  int32_t* d = nullptr;                // the index tables, stream-ordered: freed once the kernel has read them
+  MN_CUDA(cudaMallocAsync((void**)&d, bytes, st));
+  MN_CUDA(cudaMemcpyAsync(d, slot, (size_t)n_rows * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (n_vo > 0) MN_CUDA(cudaMemcpyAsync(d + n_rows, vo_rows, 2 * (size_t)n_vo * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  MN_LAUNCH(k_eval_sample_windows, (int)cdiv((long long)n_rows + n_vo, 128), 128, 0, st,
+            SampleFactor(mean6, cov36, sax, saq, p7, s7), vo_poses, (const int*)d, n_rows,
+            (const TargRow*)(d + n_rows), n_vo, vos7);
+  MN_LAUNCH_CHECK();
+  MN_CUDA(cudaFreeAsync(d, st));
+  return 0;
+}
+
+int mapnet_eval_sample_emit(const double* mean6, const double* cov36, int n_pred, const double* opt7,
+                            const double* post36, int T, int keep, const float* poses, int n_poses,
+                            const int32_t* frame, const int32_t* slot, int n, const double* pose_m3,
+                            const double* pose_s3, double* out, double* targ7, double* d2, double* u, double* nll,
+                            void* stream) {
+  MN_CHECK(poses != nullptr && frame != nullptr && out != nullptr && targ7 != nullptr && d2 != nullptr &&
+           u != nullptr && nll != nullptr, "eval_sample_emit: null argument");
+  MN_CHECK(opt7 != nullptr ? post36 != nullptr : (mean6 != nullptr && cov36 != nullptr && slot != nullptr),
+           "eval_sample_emit: need opt7 and post36, or mean6, cov36 and slot");
+  MN_CHECK(n >= 1 && n_poses >= 1 && (opt7 != nullptr || n_pred >= 1), "eval_sample_emit: bad count");
+  MN_CHECK(T >= 1 && keep >= 0 && keep < T && (long long)n * T < (1LL << 31),
+           "eval_sample_emit: slot %d of windows of %d outside the window", keep, T);
+  MN_CHECK((pose_m3 == nullptr) == (pose_s3 == nullptr), "eval_sample_emit: pose_m3 and pose_s3 go together");
+  if (opt7 != nullptr) {
+    for (int i = 0; i < n; ++i)
+      MN_CHECK(frame[i] >= 0 && frame[i] < n_poses, "eval_sample_emit: item %d: frame %d outside the %d poses", i,
+               frame[i], n_poses);
+  } else {
+    MN_TRY(eval_sample_rows("eval_sample_emit", n_pred, n_poses, frame, slot, n, nullptr, 0));
+  }
+  MN_CHECK(device_memory(poses) && device_memory(out) && device_memory(targ7) && device_memory(d2) &&
+           device_memory(u) && device_memory(nll) &&
+           (opt7 != nullptr ? device_memory(opt7) && device_memory(post36) : device_memory(mean6) && device_memory(cov36)),
+           "eval_sample_emit: tensors must be device memory");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int un = pose_m3 != nullptr;
+  const size_t rows = opt7 != nullptr ? 1 : 2;
+  int32_t* d = nullptr;                // frame (and slot) of every item, stream-ordered as in mapnet_eval_windows
+  MN_CUDA(cudaMallocAsync((void**)&d, rows * (size_t)n * sizeof(int32_t), st));
+  MN_CUDA(cudaMemcpyAsync(d, frame, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (opt7 == nullptr) MN_CUDA(cudaMemcpyAsync(d + n, slot, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  MN_LAUNCH(k_eval_sample_emit, (int)cdiv(n, 128), 128, 0, st, mean6, cov36, opt7, post36, T, keep, poses,
+            (const int*)d, opt7 != nullptr ? nullptr : (const int*)(d + n), n, un, un ? pose_m3[0] : 0.0,
+            un ? pose_m3[1] : 0.0, un ? pose_m3[2] : 0.0, un ? pose_s3[0] : 1.0, un ? pose_s3[1] : 1.0,
+            un ? pose_s3[2] : 1.0, out, targ7, d2, u, nll);
   MN_LAUNCH_CHECK();
   MN_CUDA(cudaFreeAsync(d, st));
   return 0;

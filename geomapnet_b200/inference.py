@@ -173,10 +173,11 @@ class Predictor(object):
         out = torch.cat(outs, 0)
         return out.view(*x.shape[:-3], 6)
 
-    def _sample_graph(self, B, H, W, S):
+    def _sample_graph(self, B, H, W, S, slot=0):
         """(CUDA graph, static input [B,3,H,W], static outputs) of S dropout draws per frame for one batch shape,
-        captured after an eager run at an explicit dropout step, which leaves the engine's dropout counter alone"""
-        key = (B, H, W, S)
+        captured after an eager run at an explicit dropout step, which leaves the engine's dropout counter alone.
+        slot > 0: a further graph of the same shape with its own input and output buffers."""
+        key = (B, H, W, S) if slot == 0 else (B, H, W, S, slot)
         g = self._sample_graphs.get(key)
         if g is None:
             eng, dev, L = self._engine(H, W), self.device, _lib.lib()
@@ -1200,8 +1201,91 @@ def _predict_batches(pr, net, ds, batches, droprate, dev):
     return pred, targ
 
 
+def _sample_frames(pr, ds, frames, S, dev):
+    """(mean [F,6], cov [F,36]) float64 of the S dropout draws of each cache frame `frames` (host int32 [F]): chunks of
+    the Predictor's max_batch frames in order, each taking S consecutive dropout steps, as Predictor.sample on those
+    chunks.  The next chunk is assembled on a side stream (a second graph slot) while this one runs; a chunk larger
+    than the dataset's assembly is assembled in parts."""
+    F, B, cap = frames.shape[0], pr.max_batch, ds.max_batch * ds.frames_per_item
+    chunks = [(lo, min(lo + B, F)) for lo in range(0, F, B)]
+    n_slots = 2 if len(chunks) > 1 else 1
+    keys = [(hi - lo, k % n_slots) for k, (lo, hi) in enumerate(chunks)]
+    graphs = {key: pr._sample_graph(key[0], ds.Ho, ds.Wo, S, slot=key[1]) for key in dict.fromkeys(keys)}
+    pipe = SidePipeline(dev)
+    mean = torch.empty((F, 6), dtype=torch.float64, device=dev)
+    cov = torch.empty((F, 36), dtype=torch.float64, device=dev)
+
+    def fill(k):
+        lo, hi = chunks[k]
+        xs = graphs[keys[k]][1]
+        pipe.fill(keys[k], lambda: [ds.assemble_frames(frames[a:min(a + cap, hi)], xs[a - lo:min(a + cap, hi) - lo])
+                                    for a in range(lo, hi, cap)])
+
+    fill(0)
+    for k, (lo, hi) in enumerate(chunks):
+        graph, _, o = graphs[keys[k]]
+        pipe.take(keys[k])
+        graph.replay()
+        pipe.read(keys[k]).record(torch.cuda.current_stream(dev))
+        mean[lo:hi].copy_(o["mean"])
+        cov[lo:hi].copy_(o["cov"].view(-1, 36))
+        if k + 1 < len(chunks):
+            fill(k + 1)
+    return mean, cov
+
+
+def _evaluate_sampled(pr, ds, S, vo, vo_fc, zero_lag, pose_m, pose_s, sig, dev):
+    """evaluate_sequence(samples=S) once the arguments are checked: the draws of every frame, then one gather, one
+    k_pgo_cov and one emit (with VO poses) or one emit, and one host synchronisation for the PGO status"""
+    L_lib = _lib.lib()
+    # every frame of the sequence is the kept slot of its own window (the middle slot's offset is 0, and a zero-lag
+    # window ends at its frame), so the draws are queued first and the host builds the window tables after them
+    frames = np.arange(ds.L, dtype=np.int32)
+    mean, cov = _sample_frames(pr, ds, frames, S, dev)
+    tab = ds.eval_tables(unique=True, vo_fc=vo_fc, zero_lag=zero_lag)
+    if not np.array_equal(tab["frames"], frames):
+        raise RuntimeError("evaluate_sequence: the windows do not hold every frame of the sequence")
+    windows, slots = tab["windows"], tab["slots"]
+    L, T = windows.shape
+    F = frames.shape[0]
+    keep = T - 1 if zero_lag else T // 2
+    f64 = dict(dtype=torch.float64, device=dev)
+    opt7 = post36 = status = None
+    if vo:
+        E = tab["vo_rows"].shape[1]
+        p7, s7 = torch.empty((L * T, 7), **f64), torch.empty((L * T, 49), **f64)
+        vos7, opt7, post36 = torch.empty((L * E, 7), **f64), torch.empty((L * T, 7), **f64), torch.empty((L * T, 36), **f64)
+        status = torch.zeros(1, dtype=torch.int32, device=dev)
+        _lib.check(L_lib.mapnet_eval_sample_windows(
+            mean.data_ptr(), cov.data_ptr(), F, sig["sax"], sig["saq"], ds.vo_poses.data_ptr(), ds.poses.shape[0],
+            slots.ctypes.data, L * T, tab["vo_rows"].ctypes.data, L * E, p7.data_ptr(), s7.data_ptr(), vos7.data_ptr(),
+            _lib.stream_ptr()), "mapnet_eval_sample_windows")
+        _lib.check(L_lib.mapnet_pgo_optimize_cov(p7.data_ptr(), s7.data_ptr(), vos7.data_ptr(), opt7.data_ptr(),
+                                                 post36.data_ptr(), L, T, 1 if vo_fc else 0, sig["srx"], sig["srq"], 10,
+                                                 status.data_ptr(), _lib.stream_ptr()), "mapnet_pgo_optimize_cov")
+    m = s = None
+    if pose_m is not None:
+        m = (ctypes.c_double * 3)(*[float(v) for v in np.asarray(pose_m).reshape(3)])
+        s = (ctypes.c_double * 3)(*[float(v) for v in np.asarray(pose_s).reshape(3)])
+    out = torch.empty((L, SampledTracker._ROW), **f64)
+    targ7, d2, u, nll = torch.empty((L, 7), **f64), torch.empty((L, 3), **f64), torch.empty((L, 3), **f64), \
+        torch.empty(L, **f64)
+    frame_k = np.ascontiguousarray(windows[:, keep])
+    slot_k = np.ascontiguousarray(slots[:, keep])
+    _lib.check(L_lib.mapnet_eval_sample_emit(
+        mean.data_ptr(), cov.data_ptr(), F, opt7.data_ptr() if vo else None, post36.data_ptr() if vo else None, T, keep,
+        ds.poses.data_ptr(), ds.poses.shape[0], frame_k.ctypes.data, slot_k.ctypes.data, L, m, s, out.data_ptr(),
+        targ7.data_ptr(), d2.data_ptr(), u.data_ptr(), nll.data_ptr(), _lib.stream_ptr()), "mapnet_eval_sample_emit")
+    if vo and int(status.item()) != 0:                      # the sequence's one host synchronisation
+        raise np.linalg.LinAlgError("pose graph: the normal matrix of a window of the sequence is not positive definite")
+    est = SampledTracker._est(out)
+    t_err, q_err = pose_errors(est["pose7"], targ7)
+    return dict(pred7=est["pose7"], targ7=targ7, t_err=t_err, q_err=q_err, n_frames=F, cov=est["cov"],
+                t_std=est["t_std"], q_std_deg=est["q_std_deg"], d2=d2, u=u, nll=nll)
+
+
 @torch.no_grad()
-def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, zero_lag=False, **sigmas):
+def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, zero_lag=False, samples=None, **sigmas):
     """The whole loop of scripts/eval.py:117-199 over a device-resident sequence: the windows of MF(steps, skip,
     variable_skip, no_duplicates=False) -- or single frames when dataset.steps is None -- one per frame index, in index
     order.  Returns what evaluate_tuples returns (pred7 [L,7], targ7 [L,7], t_err, q_err: the middle frame of each
@@ -1221,7 +1305,28 @@ def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, zer
     and the windows are rebuilt from the per-frame poses.  With droprate > 0 (the reference's dropout is active at
     eval) each window's frames go through the network together, one window per forward, as in the reference's loop.
     Chunk k+1 is assembled on a side stream while chunk k runs.  variable_skip draws from np.random as the
-    reference's DataLoader(shuffle=False) does."""
+    reference's DataLoader(shuffle=False) does.
+
+    samples=S (an int, 2 <= S <= 1024; the model must have dropout) evaluates Monte-Carlo dropout, SampledTracker's
+    model, on the labelled sequence.  Every distinct frame goes through the sampled engine once, in frame order, in
+    chunks of the Predictor's max_batch frames, each chunk taking S consecutive dropout steps (Predictor.sample on
+    those chunks).  Each frame's S draws are shared by every window that holds it, as the sampled trackers share them,
+    where eval.py would draw each window's frames anew: with the same chunks, seed and dropout counter the estimates
+    are bit for bit those of a SampledTracker fed the same frames (its step() rows under zero_lag).  With
+    dataset.vo_poses each window slot gets the frame's factor (mean pose, S7 = A Sigma A' + the floors sax / saq) and
+    all windows are solved in one covariance-weighted PGO launch (srx / srq); the kept slot's posterior is the
+    estimate.  Without VO poses each item's estimate is its frame's own sampled mean and covariance.  The result
+    adds, per item, SampledTracker's cov [L,6,6] (D cov D with D = diag(pose_s, 1, 1, 1)), t_std and q_std_deg, and
+    the calibration of that covariance against the target: d2 [L,3], the squared Mahalanobis distances of the error
+    (t^ - t, qlog(q^) - qlog(sign(q^.q) q)) over all 6 DoF, the translation block and the log q block; u [L,3], their
+    chi-square CDFs (6, 3 and 3 degrees of freedom), each uniform on [0, 1] for a calibrated model, so the coverage at
+    level p is (u <= p).mean(0); and nll [L], the 6-DoF Gaussian negative log-likelihood.  A covariance (block) that is
+    not positive definite gives NaN there: without PGO the 6-DoF column always is for S <= 6, since S draws span at
+    most S - 1 dimensions.  A window whose normal matrix (or a slot's S7) is not positive definite raises
+    np.linalg.LinAlgError.  The model is a Predictor of any precision or a live bf16 / tc_split model (run by a
+    temporary Predictor); a live model without a sampled engine raises ValueError.  Launches past the per-chunk
+    assembly and engine replay: one gather, one k_pgo_cov and one emit (one emit without VO poses), and one host
+    synchronisation."""
     from .data.loader import DeviceDataset
     ds = dataset
     if not isinstance(ds, DeviceDataset):
@@ -1244,6 +1349,20 @@ def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, zer
         raise ValueError("vo_fc: the dataset has no vo_poses")
     droprate = pr.droprate if pr is not None else float(net.droprate)
     cap = ds.max_batch * ds.frames_per_item                  # frames the dataset's cache assembles per call
+    if samples is not None:
+        S = _check_draws(samples, droprate)
+        if pr is None and net.precision not in ("bf16", "tc_split"):
+            raise ValueError("evaluate_sequence: samples needs a Predictor or a bf16 / tc_split model (a %s model has "
+                             "no sampled engine)" % net.precision)
+        sig = dict(sax=1.0, saq=1.0, srx=1.0, srq=1.0)
+        for k, v in sigmas.items():
+            if k not in sig:
+                raise TypeError("evaluate_sequence: unknown covariance %r (sax, saq, srx, srq)" % k)
+            sig[k] = float(v)
+        if not all(v > 0 for v in sig.values()):
+            raise ValueError("sax, saq, srx, srq must be positive, got %s" % (sig,))
+        with _eval_pass(model, pr, net, dev, min(64, cap)) as pr:
+            return _evaluate_sampled(pr, ds, S, vo, vo_fc, zero_lag, pose_m, pose_s, sig, dev)
     B = min(pr.max_batch if pr is not None else 64, cap)
     if droprate > 0:
         if B < T:

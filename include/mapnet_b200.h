@@ -209,6 +209,33 @@ int mapnet_eval_windows(const float* pred6, int n_pred, const float* poses, cons
                         const int32_t* frame, const int32_t* slot, int n_rows, const int32_t* vo_rows, int n_vo,
                         double* pred7, double* targ7, double* vos7, void* stream);
 
+/* ---- Monte-Carlo evaluation windows (csrc/loader.cu; geomapnet_b200.inference.evaluate_sequence(samples=S)): each
+ * frame's S-draw mean and covariance, shared by every window slot that holds the frame, as mapnet_track_sample_t
+ * shares them.
+ * mapnet_eval_sample_windows: for every window slot r < n_rows, (p7[r], s7[r]) = the factor mapnet_track_sample_step
+ * forms of frame row slot[r] (mapnet_test_sample_factor's arithmetic, bit for bit) from mean6 [n_pred][6] and cov36
+ * [n_pred][6][6] with the floors sax, saq > 0; for every VO k < n_vo, vos7[k] as mapnet_eval_windows writes it from
+ * vo_poses [n_poses][6] and vo_rows.  p7 [n_rows][7], s7 [n_rows][7][7]: the inputs of mapnet_pgo_optimize_cov.
+ * mapnet_eval_sample_emit: for every item i < n, out[i] = the 45-double row of mapnet_track_sample_step (pose7, cov =
+ * D cov D, t_std, q_std_deg; D = diag(pose_s3, 1, 1, 1), translations un-normalised as the tracker does) of either
+ * slot `keep` of item i's optimised window (opt7 [n*T][7] and post36 [n*T][6][6], mapnet_pgo_optimize_cov's outputs)
+ * or, with opt7 = NULL, frame row slot[i]'s own mean6 / cov36; targ7[i] = (t, qexp(log q)) of poses[frame[i]]
+ * (mapnet_eval_windows' targ7, un-normalised alike); d2[i] [3] = the squared Mahalanobis distances of the error
+ * (t^ - t, qlog(q^) - qlog(sign(q^.q) q)) under the row's cov (6-DoF, translation block, log q block), u[i] [3] their
+ * chi-square CDFs (6, 3, 3 degrees of freedom) and nll[i] the 6-DoF Gaussian negative log-likelihood
+ * (csrc/calib_core.h); NaN where a covariance (block) is not positive definite.  pose_m3 / pose_s3 (HOST [3]) go
+ * together or are both NULL (translations stay normalised).
+ * Float arrays are device memory; slot, frame and vo_rows are HOST int32 arrays, checked and copied before the call
+ * returns.  One launch each; nothing is launched when a check fails. */
+int mapnet_eval_sample_windows(const double* mean6, const double* cov36, int n_pred, double sax, double saq,
+                               const float* vo_poses, int n_poses, const int32_t* slot, int n_rows,
+                               const int32_t* vo_rows, int n_vo, double* p7, double* s7, double* vos7, void* stream);
+int mapnet_eval_sample_emit(const double* mean6, const double* cov36, int n_pred, const double* opt7,
+                            const double* post36, int T, int keep, const float* poses, int n_poses,
+                            const int32_t* frame, const int32_t* slot, int n, const double* pose_m3,
+                            const double* pose_s3, double* out, double* targ7, double* d2, double* u, double* nll,
+                            void* stream);
+
 /* ---- batched inference post-processing + pose-graph optimisation (SURVEY.md section 8 row f3; csrc/pgo.cu).
  * mapnet_pose_post: scripts/eval.py:163-181 for n poses at once -- pred6 = (t, log q) float32 -> out7 = (t * pose_s +
  * pose_m, qexp(log q)) float64; pose_m3 / pose_s3 are HOST pointers (pose_stats.txt) or NULL (keep the translations).
