@@ -226,6 +226,11 @@ def lib():
     L.mapnet_test_pack_weights.argtypes = [c_int, c_int, c_int, c_int] + [c_void_p] * 5
     for name in ("mapnet_test_weight_table", "mapnet_test_pack_weights"):
         getattr(L, name).restype = c_int
+    L.mapnet_test_conv_simt.argtypes = [c_int] * 9 + [c_void_p] * 6
+    L.mapnet_test_stem_im2col.argtypes = [c_int] * 4 + [c_void_p] * 6 + [c_float, c_void_p, c_void_p]
+    L.mapnet_test_trunk_create.argtypes = [POINTER(c_void_p)] + [c_int] * 6
+    for name in ("mapnet_test_conv_simt", "mapnet_test_stem_im2col", "mapnet_test_trunk_create"):
+        getattr(L, name).restype = c_int
     for name in ("mapnet_infer_create", "mapnet_infer_load", "mapnet_infer_forward", "mapnet_infer_destroy",
                  "mapnet_infer_calibrate", "mapnet_infer_act_scales", "mapnet_infer_forward_frames"):
         getattr(L, name).restype = c_int
@@ -254,7 +259,8 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_batch_losses", "mapnet_infer_forward_frames", "mapnet_test_stem_operand", "mapnet_infer_sample",
             "mapnet_infer_sample_frames", "mapnet_sample_post", "mapnet_test_small_gemm_plan", "mapnet_test_stem_ex",
             "mapnet_test_head", "mapnet_pgo_optimize_cov",
-            "mapnet_test_sample_factor", "mapnet_test_weight_table", "mapnet_test_pack_weights"] + TRACK_API + TRACK_MULTI_API + TRACK_SAMPLE_API + TRACK_MULTI_SAMPLE_API + EVAL_SAMPLE_API
+            "mapnet_test_sample_factor", "mapnet_test_weight_table", "mapnet_test_pack_weights",
+            "mapnet_test_conv_simt", "mapnet_test_stem_im2col", "mapnet_test_trunk_create"] + TRACK_API + TRACK_MULTI_API + TRACK_SAMPLE_API + TRACK_MULTI_SAMPLE_API + EVAL_SAMPLE_API
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 MAX_SAMPLE_DRAWS = 1024      # mapnet_infer_sample: S in [2, MAX_SAMPLE_DRAWS] dropout draws per frame
 

@@ -39,6 +39,24 @@ int mapnet_trunk_create(mapnet_trunk_t** out, int max_B, int H, int W, int feat_
   return 0;
 }
 
+// mapnet_trunk_create with Net::init's im2col_stem: 1 gives the tensor-core modes the stem they fall back to when the
+// driver rejects overlapped tensor maps (the CUDA-core modes always run it)
+int mapnet_test_trunk_create(mapnet_trunk_t** out, int max_B, int H, int W, int feat_dim, int precision, int im2col_stem) {
+  MN_CHECK(out != nullptr, "test_trunk_create: null out pointer");
+  *out = nullptr;
+  MN_CHECK(im2col_stem == 0 || im2col_stem == 1, "test_trunk_create: im2col_stem %d is not 0 or 1", im2col_stem);
+  MN_CHECK(precision >= PREC_FP32 && precision <= PREC_TC_SPLIT, "test_trunk_create: precision %d is not a training "
+           "precision", precision);
+  MN_CHECK(max_B >= 0 && H >= 32 && W >= 32 && feat_dim >= 8 && feat_dim % 4 == 0, "test_trunk_create: bad shape "
+           "(max_B %d, %dx%d, feat_dim %d)", max_B, H, W, feat_dim);
+  if (max_B > 0) MN_TRY(require_device());
+  mapnet_trunk* h = new mapnet_trunk();
+  int r = h->net.init(max_B, H, W, feat_dim, precision, im2col_stem);
+  if (r != 0) { h->net.destroy(); delete h; return r; }
+  *out = h;
+  return 0;
+}
+
 int mapnet_trunk_destroy(mapnet_trunk_t* h) {
   if (h == nullptr) return 0;
   h->net.destroy();
@@ -442,6 +460,146 @@ int mapnet_test_stem_ex(int precision, int B, int H, int W, const float* x_nchw,
   if (pf) tc_plan_destroy(pf);
   if (pw) tc_plan_destroy(pw);
   cudaFree(S); cudaFree(wk); cudaFree(dwk); cudaFree(dys); cudaFree(f32); cudaFree(d_scale); cudaFree(acc);
+  cudaFree(d_wd);
+  return r;
+}
+
+// The CUDA-core engines (fp32 and bf16_simt) as Net::conv_fprop / conv_dgrad / conv_wgrad launch them: NHWC activations
+// and gradients of the mode's type, fp32 K-major weights, fp32 dW accumulated into `out`.  A residual (dgrad only, out's
+// type and shape) is added before the store; it may be `out` itself, as in Net::backward_t's conv_dgrad(conv1, S1, S0, S0).
+int mapnet_test_conv_simt(int precision, int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride,
+                          const void* in0, const void* in1, const void* wmat, const void* residual, void* out, void* stream) {
+  MN_CHECK(precision == PREC_FP32 || precision == PREC_BF16_SIMT, "test_conv_simt: precision %d is not a CUDA-core "
+           "precision (fp32 = %d or bf16_simt = %d)", precision, PREC_FP32, PREC_BF16_SIMT);
+  MN_CHECK(kind >= 0 && kind <= 2, "test_conv_simt: kind %d outside [0, 2]", kind);
+  MN_CHECK(B >= 1 && Hi >= 1 && Wi >= 1 && (k == 1 || k == 3) && (stride == 1 || stride == 2) && Ci > 0 && Co > 0 &&
+           Ci % 4 == 0 && Co % 4 == 0, "test_conv_simt: bad shape (B %d, %dx%d, Ci %d, Co %d, k %d, stride %d)", B, Hi,
+           Wi, Ci, Co, k, stride);
+  MN_CHECK(in0 && out && (kind == 2 ? in1 != nullptr : wmat != nullptr), "test_conv_simt: null argument");
+  MN_CHECK(residual == nullptr || kind == 1, "test_conv_simt: a residual is a dgrad feature");
+  MN_TRY(require_device());
+  ConvGeom g;
+  g.B = B; g.Hi = Hi; g.Wi = Wi; g.Ci = Ci; g.Co = Co; g.KH = g.KW = k; g.stride = stride; g.pad = (k - 1) / 2;
+  g.Ho = (Hi + 2 * g.pad - k) / stride + 1; g.Wo = (Wi + 2 * g.pad - k) / stride + 1;
+  cudaStream_t st = (cudaStream_t)stream;
+  const float* w = (const float*)wmat;
+  if (precision == PREC_FP32) {
+    if (kind == 0) MN_TRY(launch_conv_simt_fprop<float>(g, (const float*)in0, w, nullptr, (float*)out, st));
+    else if (kind == 1) MN_TRY(launch_conv_simt_dgrad<float>(g, (const float*)in0, w, (const float*)residual, (float*)out, st));
+    else MN_TRY(launch_conv_simt_wgrad<float>(g, (const float*)in0, (const float*)in1, (float*)out, st));
+  } else {
+    if (kind == 0) MN_TRY(launch_conv_simt_fprop<bf16>(g, (const bf16*)in0, w, nullptr, (bf16*)out, st));
+    else if (kind == 1) MN_TRY(launch_conv_simt_dgrad<bf16>(g, (const bf16*)in0, w, (const bf16*)residual, (bf16*)out, st));
+    else MN_TRY(launch_conv_simt_wgrad<bf16>(g, (const bf16*)in0, (const bf16*)in1, (float*)out, st));
+  }
+  MN_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// The training step's im2col stem (Net::forward_t / backward_t when stem_s2d is off: always in the CUDA-core modes, the
+// fallback of the tensor-core modes): k_stem_im2col's [B*Hc*Wc][192] patch matrix of the operand type, the mode's weight
+// pack into the [64][192] row, the 1x1 GEMM view (Ci = 192) fprop -- in the tensor-core modes with the BatchNorm-statistics
+// epilogue when host_sums != NULL -- and with dy the wgrad into the zeroed [64][192] accumulator, re-laid out into
+// dw_oihw [64,3,7,7] by k_unpack_wgrads.  a_out (optional) receives the patch matrix.  Types as mapnet_test_stem_ex, with
+// the CUDA-core modes' y_out / dy fp32 (fp32) or bf16 (bf16_simt).
+int mapnet_test_stem_im2col(int precision, int B, int H, int W, const float* x_nchw, const float* w_oihw, void* a_out,
+                            void* y_out, const void* dy, float* dw_oihw, float out_scale, double* host_sums, void* stream) {
+  MN_CHECK(precision >= PREC_FP32 && precision <= PREC_TC_SPLIT, "test_stem_im2col: precision %d is not a training "
+           "precision", precision);
+  MN_CHECK(B >= 1 && H >= 32 && W >= 32, "test_stem_im2col: bad shape (B %d, %dx%d)", B, H, W);
+  MN_TRY(stem_im2col_check(W, kStemIm2colK));
+  MN_CHECK(x_nchw && w_oihw && y_out, "test_stem_im2col: null argument");
+  MN_CHECK((dy == nullptr) == (dw_oihw == nullptr), "test_stem_im2col: dy and dw_oihw go together");
+  MN_CHECK(out_scale == 0.f || (precision == PREC_TC_SPLIT && dy != nullptr && isfinite(out_scale) && out_scale > 0.f),
+           "test_stem_im2col: out_scale %g: a positive gradient scale of the strict-mode wgrad, or 0", out_scale);
+  const bool tc = precision == PREC_BF16_TC || precision == PREC_TC_SPLIT;
+  MN_CHECK(host_sums == nullptr || tc, "test_stem_im2col: the BatchNorm-statistics epilogue is a tensor-core feature "
+           "(the CUDA-core modes take the statistics from k_channel_sums)");
+  MN_TRY(require_device());
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool sp = precision == PREC_TC_SPLIT;
+  const size_t ez = (precision == PREC_BF16_TC || precision == PREC_BF16_SIMT) ? 2 : 4;   // split: an fp16 hi / lo pair
+  const int K = kStemIm2colK;
+  const int Hc = (H - 1) / 2 + 1, Wc = (W - 1) / 2 + 1;
+  ConvGeom g;                                      // the GEMM view: a 1x1 conv over the patch matrix
+  g.B = B; g.Hi = g.Ho = Hc; g.Wi = g.Wo = Wc; g.Ci = K; g.Co = 64; g.KH = g.KW = 1; g.stride = 1; g.pad = 0;
+  if (sp) g.split = 1;
+  WeightDesc wd; memset(&wd, 0, sizeof(wd));
+  wd.Co = 64; wd.Ci = K; wd.Ci_real = 3; wd.KH = wd.KW = 1; wd.im2col_k = K;
+  const long long M = (long long)B * Hc * Wc, n_y = M * 64;
+  const size_t acc_doubles = (size_t)kBnAccReplicas * kBnAccStride;
+  void *A = nullptr, *wk = nullptr, *dys = nullptr; float *dwk = nullptr, *f32 = nullptr, *d_scale = nullptr;
+  double* acc = nullptr; WeightDesc* d_wd = nullptr;
+  TcConvPlan *pf = nullptr, *pw = nullptr;
+  std::vector<double> h;
+  auto body = [&]() -> int {
+    MN_CUDA(cudaMalloc(&A, (size_t)M * K * ez));
+    MN_CUDA(cudaMalloc(&wk, (size_t)64 * K * (sp ? 8 : (precision == PREC_BF16_TC ? 2 : 4))));
+    MN_CUDA(cudaMalloc(&dwk, (size_t)64 * K * sizeof(float)));
+    MN_CUDA(cudaMalloc(&d_wd, sizeof(WeightDesc)));
+    MN_CUDA(cudaMemcpyAsync(d_wd, &wd, sizeof(wd), cudaMemcpyHostToDevice, st));
+    MN_CUDA(cudaMemsetAsync(dwk, 0, (size_t)64 * K * sizeof(float), st));
+    if (precision == PREC_FP32 || precision == PREC_BF16_SIMT) {
+      if (precision == PREC_FP32) MN_TRY(launch_stem_im2col<float>(x_nchw, (float*)A, B, H, W, Hc, Wc, K, st));
+      else MN_TRY(launch_stem_im2col<bf16>(x_nchw, (bf16*)A, B, H, W, Hc, Wc, K, st));
+      MN_TRY(launch_pack_weights<float>(d_wd, 1, w_oihw, (float*)wk, nullptr, 64 * K, precision == PREC_BF16_SIMT, st));
+    } else if (sp) {
+      MN_CUDA(cudaMalloc(&f32, (size_t)64 * K * sizeof(float)));
+      MN_TRY(launch_stem_im2col<hsplit>(x_nchw, (hsplit*)A, B, H, W, Hc, Wc, K, st));
+      MN_TRY(launch_pack_weights_split(d_wd, 1, w_oihw, f32, nullptr, wk, nullptr, 64 * K, st));
+    } else {
+      MN_TRY(launch_stem_im2col<bf16>(x_nchw, (bf16*)A, B, H, W, Hc, Wc, K, st));
+      MN_TRY(launch_pack_weights<bf16>(d_wd, 1, w_oihw, (bf16*)wk, nullptr, 64 * K, 0, st));
+    }
+    if (a_out != nullptr) MN_CUDA(cudaMemcpyAsync(a_out, A, (size_t)M * K * ez, cudaMemcpyDeviceToDevice, st));
+    if (host_sums != nullptr) {
+      MN_CUDA(cudaMalloc((void**)&acc, acc_doubles * sizeof(double)));
+      MN_CUDA(cudaMemsetAsync(acc, 0, acc_doubles * sizeof(double), st));
+    }
+    if (precision == PREC_FP32) MN_TRY(launch_conv_simt_fprop<float>(g, (const float*)A, (const float*)wk, nullptr, (float*)y_out, st));
+    else if (precision == PREC_BF16_SIMT) MN_TRY(launch_conv_simt_fprop<bf16>(g, (const bf16*)A, (const float*)wk, nullptr, (bf16*)y_out, st));
+    else {
+      MN_TRY(tc_plan_create(&pf, g, 0, (const bf16*)wk));
+      MN_TRY(tc_conv_run(pf, (const bf16*)A, nullptr, nullptr, y_out, st, acc));
+    }
+    if (dy != nullptr) {
+      if (precision == PREC_FP32) MN_TRY(launch_conv_simt_wgrad<float>(g, (const float*)A, (const float*)dy, dwk, st));
+      else if (precision == PREC_BF16_SIMT) MN_TRY(launch_conv_simt_wgrad<bf16>(g, (const bf16*)A, (const bf16*)dy, dwk, st));
+      else {
+        const void* g_in = dy;
+        if (sp) {
+          MN_CUDA(cudaMalloc(&dys, (size_t)n_y * 4));
+          MN_TRY(launch_split_tensor((const float*)dy, dys, n_y, st));
+          g_in = dys;
+        }
+        MN_TRY(tc_plan_create(&pw, g, 2, nullptr));
+        if (out_scale != 0.f) {
+          MN_CUDA(cudaMalloc((void**)&d_scale, sizeof(float)));
+          MN_CUDA(cudaMemcpyAsync(d_scale, &out_scale, sizeof(float), cudaMemcpyHostToDevice, st));
+          tc_plan_set_out_scale(pw, d_scale);
+        }
+        MN_TRY(tc_conv_run(pw, (const bf16*)A, (const bf16*)g_in, nullptr, dwk, st));
+      }
+      MN_TRY(launch_unpack_wgrads(d_wd, 1, dwk, dw_oihw, 64 * K, st));
+    }
+    if (acc != nullptr) {
+      h.resize(acc_doubles);
+      MN_CUDA(cudaMemcpyAsync(h.data(), acc, acc_doubles * sizeof(double), cudaMemcpyDeviceToHost, st));
+    }
+    MN_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  };
+  const int r = body();
+  if (r == 0 && host_sums != nullptr)
+    for (int j = 0; j < 2; ++j)
+      for (int c = 0; c < 64; ++c) {
+        double s = 0.0;
+        for (int rep = 0; rep < kBnAccReplicas; ++rep) s += h[(size_t)rep * kBnAccStride + (size_t)j * 64 + c];
+        host_sums[(size_t)j * 64 + c] = s;
+      }
+  if (pf) tc_plan_destroy(pf);
+  if (pw) tc_plan_destroy(pw);
+  cudaFree(A); cudaFree(wk); cudaFree(dwk); cudaFree(dys); cudaFree(f32); cudaFree(d_scale); cudaFree(acc);
   cudaFree(d_wd);
   return r;
 }

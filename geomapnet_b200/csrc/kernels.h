@@ -160,6 +160,10 @@ int launch_stem_s2d(const float* x_nchw, TZ* S, int B, int H, int W, int Hs, int
 // geometry of the stem as the engines see it on that image (B left 0): 4 taps x 64 elements, overlapped view
 int stem_s2d_wsp(int wc);
 void stem_s2d_geometry(int H, int W, int Co, ConvGeom* g, WeightDesc* wd, int elt_bytes = 2);
+// the im2col stem's patch-matrix row: 7*7*3 = 147 padded to 192 (a multiple of the tensor-core K block)
+static constexpr int kStemIm2colK = 192;
+// host-side limits of launch_stem_im2col (it calls this first): Kpad a multiple of 8 in [147, kStemIm2colK], W <= 570
+int stem_im2col_check(int W, int Kpad);
 template <typename T>
 int launch_stem_im2col(const float* x_nchw, T* A, int B, int H, int W, int Ho, int Wo, int Kpad, cudaStream_t st);
 

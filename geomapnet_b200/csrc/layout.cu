@@ -310,10 +310,10 @@ __global__ void __launch_bounds__(256)
 k_stem_im2col(const float* __restrict__ x, T* __restrict__ A, int B, int H, int W, int Ho, int Wo, int Kpad) {
   pdl_prologue();
   extern __shared__ float sx[];          // [3*7][W + 6]
-  __shared__ int lut[192];               // k -> offset of (c,kh,kw) inside sx (-1: zero padding of K)
+  __shared__ int lut[kStemIm2colK];      // k -> offset of (c,kh,kw) inside sx (-1: zero padding of K)
   const int WP = W + 6;
   const int b = blockIdx.x / Ho, oh = blockIdx.x - b * Ho;
-  if (threadIdx.x < 192) {
+  if (threadIdx.x < kStemIm2colK) {
     const int k = threadIdx.x;
     int off = -1;
     if (k < 147) { const int t = k / 3, c = k - t * 3; const int kh = t / 7, kw = t - kh * 7; off = (c * 7 + kh) * WP + kw; }
@@ -342,11 +342,21 @@ k_stem_im2col(const float* __restrict__ x, T* __restrict__ A, int B, int H, int 
   }
 }
 
+// Kpad indexes k_stem_im2col's kStemIm2colK-entry k -> offset table.  The 21 staged input rows of W + 6 floats and that
+// table share the 48 KB of shared memory a launch gets without opting in, so W <= 570 (a wider frame used to pass a check
+// that left the table out and then failed at launch with "invalid argument").
+int stem_im2col_check(int W, int Kpad) {
+  MN_CHECK(Kpad % 8 == 0 && Kpad >= 147 && Kpad <= kStemIm2colK, "stem_im2col: Kpad %d is not a multiple of 8 in [147, %d]", Kpad,
+           kStemIm2colK);
+  MN_CHECK(W >= 1 && (size_t)21 * (W + 6) * sizeof(float) + kStemIm2colK * sizeof(int) <= 48 * 1024,
+           "stem_im2col: image width %d too large (at most 570)", W);
+  return 0;
+}
+
 template <typename T>
 int launch_stem_im2col(const float* x_nchw, T* A, int B, int H, int W, int Ho, int Wo, int Kpad, cudaStream_t st) {
-  MN_CHECK(Kpad % 8 == 0 && Kpad >= 147, "stem_im2col: bad Kpad");
+  MN_TRY(stem_im2col_check(W, Kpad));
   const size_t smem = (size_t)21 * (W + 6) * sizeof(float);
-  MN_CHECK(smem <= 48 * 1024, "stem_im2col: image width %d too large", W);
   MN_LAUNCH(k_stem_im2col<T>, B * Ho, 256, smem, st, x_nchw, A, B, H, W, Ho, Wo, Kpad);
   MN_LAUNCH_CHECK();
   return 0;

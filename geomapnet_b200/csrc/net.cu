@@ -33,7 +33,7 @@ void set_last_error(const char* fmt, ...) {
 const char* get_last_error() { return g_err; }
 
 static const int kStages[4][3] = {{64, 3, 1}, {128, 4, 2}, {256, 6, 2}, {512, 3, 2}};
-static const int kStemK = 192;   // 7*7*3 = 147 padded to a multiple of 64 (tensor-core K block)
+static const int kStemK = kStemIm2colK;
 
 static long long align_up(long long v, long long a) { return (v + a - 1) / a * a; }
 static int conv_out(int n, int k, int s, int p) { return (n + 2 * p - k) / s + 1; }

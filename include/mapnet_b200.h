@@ -591,6 +591,30 @@ int mapnet_test_small_gemm_plan(int epi, int M, int N, int K, int* splits, int* 
  * Arguments are checked before the device is touched.  mapnet_test_plan_describe(kind 0 / 2, k 7) gives its plans. */
 int mapnet_test_stem_ex(int precision, int B, int H, int W, const float* x_nchw, const float* w_oihw, void* y_out,
                         const void* dy, float* dw_oihw, float out_scale, double* host_sums, void* stream);
+/* the CUDA-core conv engines (precision fp32 or bf16_simt) as the training step launches them: in0 / in1 / out NHWC
+ * activations and gradients of the mode's type (fp32; bf16), wmat the fp32 K-major weights ([Co][k][k][Ci] fprop,
+ * [Ci][k][k][Co] dgrad; fp32 in both modes), wgrad: in0 = x, in1 = dy, out = fp32 [Co][k][k][Ci] accumulated.
+ * residual (dgrad only, out's type and shape; NULL = none) is added before the store and may be `out` itself.  Needs
+ * Ci and Co multiples of 4, k 1 or 3, stride 1 or 2.  Arguments are checked before the device is touched; the call
+ * returns after the launches complete. */
+int mapnet_test_conv_simt(int precision, int kind /*0 fprop 1 dgrad 2 wgrad*/, int B, int Hi, int Wi, int Ci, int Co,
+                          int k, int stride, const void* in0, const void* in1, const void* wmat, const void* residual,
+                          void* out, void* stream);
+/* the training step's im2col stem in any training precision, as Net runs it when the space-to-depth stem is off: the
+ * [B*Hc*Wc][192] patch matrix of x_nchw (k = (kh*7 + kw)*3 + c, columns 147..191 zero; fp32, bf16, or fp16 hi/lo planes
+ * in strict mode) copied to a_out when a_out != NULL, the mode's pack of w_oihw into the [64][192] row (bf16_simt: fp32
+ * values rounded to bf16), the 1x1 fprop over it into y_out ([B,Hc,Wc,64]; fp32 in fp32 and strict mode, else bf16) with,
+ * in the tensor-core modes and when host_sums != NULL, the BatchNorm-statistics epilogue (host_sums as for
+ * mapnet_test_stem_ex; NULL in the CUDA-core modes).  dy != NULL (y_out's type and shape; strict mode cut into fp16
+ * planes here): the wgrad into the zeroed [64][192] accumulator, with out_scale (strict mode; 0 = none), re-laid out
+ * into dw_oihw [64,3,7,7].  W at most 570.  Arguments are checked before the device is touched.
+ * mapnet_test_plan_describe(kind, B, Hc, Wc, 192, 64, 1, 1, flags) gives the tensor-core plans. */
+int mapnet_test_stem_im2col(int precision, int B, int H, int W, const float* x_nchw, const float* w_oihw, void* a_out,
+                            void* y_out, const void* dy, float* dw_oihw, float out_scale, double* host_sums, void* stream);
+/* mapnet_trunk_create with the stem layout chosen: im2col_stem = 1 gives the tensor-core training modes the im2col stem
+ * they fall back to when the driver rejects overlapped tensor maps (0: as mapnet_trunk_create).  The handle is an
+ * ordinary trunk handle (mapnet_trunk_destroy). */
+int mapnet_test_trunk_create(mapnet_trunk_t** out, int max_B, int H, int W, int feat_dim, int precision, int im2col_stem);
 /* the pose head's forward and backward launch sequences, the ones the training step runs, on caller-owned fp32 device
  * tensors: feat [B,512]; params (and grads) packed fc_w [F,512], fc_b [F], xyz_w [3,F], xyz_b [3], wpqr_w [3,F],
  * wpqr_b [3].  Forward: droprate > 0 writes the dropout mask [B,F] of flat offset step * stride (step == UINT64_MAX: of
