@@ -142,6 +142,8 @@ def lib():
     L.mapnet_bench_conv.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_int, POINTER(c_float)]
     L.mapnet_bench_conv.restype = c_int
+    L.mapnet_test_wgrad.argtypes = [c_int] * 9 + [c_void_p] * 3 + [c_int, POINTER(c_float)]
+    L.mapnet_test_wgrad.restype = c_int
     L.mapnet_test_conv_affine.argtypes = [c_int] * 8 + [c_void_p] * 5 + [c_int, c_void_p, c_void_p]
     L.mapnet_test_conv_affine.restype = c_int
     L.mapnet_infer_create.argtypes = [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int]
@@ -246,7 +248,7 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_param_count", "mapnet_param_info", "mapnet_param_layout", "mapnet_params_numel", "mapnet_bufs_numel",
             "mapnet_forward", "mapnet_backward", "mapnet_loss_fwd_bwd", "mapnet_sqnorm", "mapnet_adam_step",
             "mapnet_test_conv", "mapnet_launch_count", "mapnet_profile", "mapnet_profile_read",
-            "mapnet_adam_step_dev", "mapnet_bench_conv", "mapnet_test_stem",
+            "mapnet_adam_step_dev", "mapnet_bench_conv", "mapnet_test_wgrad", "mapnet_test_stem",
             "mapnet_test_dgrad_shortcut", "mapnet_test_plan_describe", "mapnet_preprocess_create",
             "mapnet_preprocess_output_size", "mapnet_preprocess_run", "mapnet_preprocess_destroy",
             "mapnet_backward_part", "mapnet_grad_part_range", "mapnet_preprocess_run_ex", "mapnet_test_conv_epilogue", "mapnet_pose_post", "mapnet_pgo_optimize",

@@ -1191,6 +1191,43 @@ int mapnet_infer_destroy(mapnet_infer_t* h) {
   return 0;
 }
 
+// wgrad of one stride-1 (or any) conv on a chosen engine, keeping the plan's K partition: taps -1 = the planner's
+// choice, 0 = the per-tap engine, 3 / 9 = the halo engine with that many filter taps per CTA at N tile bn.  dw is
+// accumulated onto (one split) or has the splits' sum added to it, as in the training step.  iters 0: one run;
+// iters > 0: 3 warm-up runs, then the average ms of `iters` runs into *host_ms (tools/bench_conv.py)
+int mapnet_test_wgrad(int taps, int bn, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* x,
+                      const void* dy, void* dw, int iters, float* host_ms) {
+  MN_TRY(require_device());
+  ConvGeom g;
+  g.B = B; g.Hi = Hi; g.Wi = Wi; g.Ci = Ci; g.Co = Co; g.KH = g.KW = k; g.stride = stride; g.pad = (k - 1) / 2;
+  g.Ho = (Hi + 2 * g.pad - k) / stride + 1; g.Wo = (Wi + 2 * g.pad - k) / stride + 1;
+  TcConvPlan* plan = nullptr;
+  MN_TRY(tc_plan_create(&plan, g, 2, nullptr));
+  cudaStream_t st = 0;
+  int r = taps >= 0 ? tc_plan_force_wgrad(plan, taps, bn) : 0;
+  auto run = [&]() { return tc_conv_run(plan, (const bf16*)x, (const bf16*)dy, nullptr, dw, st); };
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  if (r == 0 && iters <= 0) r = run();
+  if (r == 0 && iters > 0) {
+    for (int i = 0; i < 3 && r == 0; ++i) r = run();
+    cudaEventCreate(&e0); cudaEventCreate(&e1);
+    cudaEventRecord(e0, st);
+    for (int i = 0; i < iters && r == 0; ++i) r = run();
+    cudaEventRecord(e1, st);
+  }
+  const cudaError_t e = cudaStreamSynchronize(st);
+  if (r == 0 && e != cudaSuccess) { set_last_error("test_wgrad: %s", cudaGetErrorString(e)); r = 1; }
+  if (r == 0 && iters > 0 && host_ms != nullptr) {
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, e0, e1);
+    *host_ms = ms / iters;
+  }
+  if (e0) cudaEventDestroy(e0);
+  if (e1) cudaEventDestroy(e1);
+  tc_plan_destroy(plan);
+  return r;
+}
+
 // micro-benchmark of one wgmma conv launch configuration (plan built once, CUDA-event timing)
 int mapnet_bench_conv(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* in0,
                       const void* in1, const void* wmat, void* out, int iters, float* host_ms) {

@@ -19,6 +19,8 @@
 //       128 rows of A (one per consumer warpgroup), dY supplies up to 128 columns of B;
 //       split-K over pixel tiles, the splits' partial dW added up in a fixed order into the flat
 //       wgrad buffer (k_wgrad_reduce).
+//  k_halo_wgrad  the same dW for stride-1 3x3 convs with the same K partition: per k-block one X halo and one dY
+//     tile, 3 or 9 filter taps read from the halo by descriptor (tc_plan_create picks the engine per conv).
 #include <cudaTypedefs.h>
 
 #include <stdarg.h>
@@ -165,6 +167,14 @@ struct WgradParams {
   float* partial;          // splits > 1: split s stores its dW slice at partial + s * part_stride (no atomics), or null
   long long part_stride;   // Co * KK * Ci
   WgradTap taps[16];
+  // stride-1 3x3 convs run from a staged input halo (k_halo_wgrad) when halo_taps != 0; the K partition above
+  // (box, splits, tiles_per_split) is the per-tap engine's either way
+  int halo_taps;           // 3: one filter row per CTA (one consumer warpgroup), 9: all three rows (three warpgroups)
+  int halo_bn;             // its N tile (64 or 128; 9 taps: 64)
+  int RW, HR;              // halo box: RW = TW + 2 rounded up to 8 pixels wide, HR = TH + halo_taps / 3 - 1 rows high
+  int halo_bytes;          // 128 * RW * HR * TN
+  int halo_sbo;            // bytes between the two 8-pixel groups of a k16 step inside the halo
+  int step_row[4];         // halo row of the first pixel of k16 step j of a k-block (filter tap (0, 0) of the halo)
 };
 // chunk c = (tap c / cpt, 64-element block c % cpt)
 __device__ __forceinline__ WgradChunk wgrad_chunk(const WgradParams& P, int c) {
@@ -893,7 +903,7 @@ k_f8_conv(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUt
 // (r/16)*8 + r%8 of plane (r/8)%2, columns likewise -- so the four hi/lo products of one (co, ci) pair are the
 // cells (r, c), (r+8, c), (r, c+8), (r+8, c+8), all held by the same thread: summed in registers, one atomic.
 // ---------------------------------------------------------------------------------
-template <int BN>
+template <int BN, int JG = 4>
 __device__ __forceinline__ void wgrad_store(const WgradParams& P, float* __restrict__ dw, const float (&d)[BN / 2],
                                             const WgradChunk& ch, const int col0, const int wq, const int lane) {
   const int r = 16 * wq + (lane >> 2);
@@ -903,8 +913,8 @@ __device__ __forceinline__ void wgrad_store(const WgradParams& P, float* __restr
   if (!P.split) {
     // Adding into dw reads it first.  The compiler cannot tell that the addresses differ, so one `+=` at a time makes
     // every load wait for the previous store: BN / 2 dependent DRAM round trips per thread (measured on H100: more than
-    // half of a layer4 wgrad).  Groups of 16 loads are issued together before their adds and stores instead.
-    constexpr int JG = 4;                      // j values per group: 4 x 2 x 2 values
+    // half of a layer4 wgrad).  Groups of 4 * JG loads (JG j values x 2 x 2) are issued together before their adds and
+    // stores instead.
     // element (co = col0 + c + k, row r) is at p0 + k * cstride
     float* p0 = dw + ((long long)(col0 + c) * P.KK + ch.tap) * P.Ci + ch.c0 + r;
     const int cstride = P.KK * P.Ci;
@@ -1033,6 +1043,124 @@ k_tc_wgrad(const __grid_constant__ CUtensorMap mapX0, const __grid_constant__ CU
   }
 }
 
+// ---------------------------------------------------------------------------------
+// stride-1 3x3 wgrad from a staged input halo: one CTA per (64-channel X block, tap group, N tile of BN, K split)
+// ---------------------------------------------------------------------------------
+// k_tc_wgrad loads every filter tap's X box on its own, although the nine boxes of one pixel box are shifted views of
+// one halo, and loads the dY tile again for every M tile: its operand stream, not its MMAs, bounds it.  Here each
+// k-block loads the halo of the pixel box (NWG filter rows; zero outside the tensor, as the per-tap boxes are) and the
+// dY tile once.  Tap (kh0 + wg, kw) of k16 step j is a descriptor into the halo at row step_row[j] + wg * RW + kw: the
+// same pixels in the same order as the per-tap box, so every dW element sees the same wgmma k16 steps as in
+// k_tc_wgrad and comes out bit for bit the same.  NWG consumer warpgroups, one per filter row, hold three accumulators
+// each (one per filter column).  The 128B swizzle of a shifted start row follows from its address (the halo is
+// 1024-byte aligned, the descriptor's base offset stays 0).
+static constexpr uint32_t halo_max_bytes(int NWG) { return NWG == 3 ? 28672u : 16384u; }   // 224 / 128 halo rows
+static constexpr int halo_stages(int BN, int NWG) { return (NWG == 1 && BN == 64) ? 4 : 6; }
+static constexpr int halo_ctas_per_sm(int BN, int NWG) { return (NWG == 1 && BN == 64) ? 2 : 1; }
+static constexpr size_t halo_smem_bytes(int BN, int NWG) {
+  return (size_t)halo_stages(BN, NWG) * (halo_max_bytes(NWG) + BN * 128) + 1024;
+}
+
+template <int BN, int NWG>
+__global__ void __launch_bounds__(NWG * 128 + 32, halo_ctas_per_sm(BN, NWG))
+k_halo_wgrad(const __grid_constant__ CUtensorMap mapH, const __grid_constant__ CUtensorMap mapDY,
+                const __grid_constant__ WgradParams P, float* __restrict__ dw) {
+  static_assert(NWG == 1 || (NWG == 3 && BN == 64), "9 taps hold 3 x 64 x BN accumulators per warpgroup: BN 64 only");
+  constexpr int STAGES = halo_stages(BN, NWG);
+  constexpr uint32_t HALO_BYTES = halo_max_bytes(NWG);
+  constexpr uint32_t CHUNK_BYTES = 64 * 128;
+  constexpr uint32_t STAGE_BYTES = HALO_BYTES + BN * 128;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = __shfl_sync(0xffffffffu, (smem_u32(smem_raw) + 1023u) & ~1023u, 0);
+  __shared__ __align__(8) uint64_t bars[2 * STAGES];
+  const uint32_t full0 = __shfl_sync(0xffffffffu, smem_u32(&bars[0]), 0), empty0 = smem_u32(&bars[STAGES]);
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+
+  int u = blockIdx.x;
+  const int split = u % P.splits; u /= P.splits;
+  const int n_nt = P.Co / BN;
+  const int nt = u % n_nt; u /= n_nt;
+  const int kh0 = (u % (3 / NWG)) * NWG;      // first filter row of this CTA
+  const int cb = u / (3 / NWG);               // 64-channel X block
+  const int t_beg = split * P.tiles_per_split;
+  int t_end = t_beg + P.tiles_per_split; if (t_end > P.n_pix_tiles) t_end = P.n_pix_tiles;
+  const int ksteps = (t_end > t_beg) ? (t_end - t_beg) : 0;
+
+  if (warp == 4 * NWG && lane == 0) {
+    prefetch_tmap(&mapH); prefetch_tmap(&mapDY);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(full0 + 8 * i, 1); mbar_init(empty0 + 8 * i, NWG); }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_prologue();
+
+  if (warp == 4 * NWG) {
+    if (elect_one()) {
+      int stage = 0; uint32_t phase = 0;
+      const uint32_t tx = (uint32_t)P.halo_bytes + BN * 128;
+      for (int t = t_beg; t < t_end; ++t) {
+        int tt = t;
+        const int tw = tt % P.tiles_w; tt /= P.tiles_w;
+        const int th = tt % P.tiles_h;
+        const int tb = tt / P.tiles_h;
+        const int ow0 = tw * P.TW, oh0 = th * P.TH, n0 = tb * P.TN;
+        mbar_wait(empty0 + 8 * stage, phase ^ 1);
+        const uint32_t sa = smem_base + stage * STAGE_BYTES;
+        mbar_expect_tx(full0 + 8 * stage, tx);
+        tma_load_4d(sa, &mapH, full0 + 8 * stage, cb * 64, ow0 - 1, oh0 + kh0 - 1, n0);
+#pragma unroll
+        for (int j = 0; j < BN / 64; ++j)
+          tma_load_4d(sa + HALO_BYTES + j * CHUNK_BYTES, &mapDY, full0 + 8 * stage, nt * BN + j * 64, ow0, oh0, n0);
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+    }
+  } else {
+    const int wg = warp >> 2;                 // filter row kh0 + wg
+    const uint64_t adesc = make_smem_desc_base(CHUNK_BYTES, (uint32_t)P.halo_sbo);
+    constexpr uint64_t BDESC = make_smem_desc_base(CHUNK_BYTES, 1024);
+    uint32_t arow[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) arow[j] = (uint32_t)(P.step_row[j] + wg * P.RW) * 128u;
+    const bool arriver = (threadIdx.x & 127) == 0;
+    float d[3][BN / 2];
+    int stage = 0, prev = -1; uint32_t phase = 0;
+    for (int kb = 0; kb < ksteps; ++kb) {
+      mbar_wait(full0 + 8 * stage, phase);
+      const uint32_t sa = smem_base + stage * STAGE_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint64_t db = smem_desc(BDESC, sa + HALO_BYTES + j * 2048);
+#pragma unroll
+        for (int kw = 0; kw < 3; ++kw)
+          wgmma_k16<1, 1>(WgmmaTag<BN, 1>(), d[kw], smem_desc(adesc, sa + arow[j] + kw * 128), db,
+                          (kb > 0 || j > 0) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+#pragma unroll
+      for (int kw = 0; kw < 3; ++kw) wgmma_fence_acc(d[kw]);
+      if (prev >= 0) release_stage(empty0 + 8 * prev, arriver);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int kw = 0; kw < 3; ++kw) wgmma_fence_acc(d[kw]);
+    if (prev >= 0) release_stage(empty0 + 8 * prev, arriver);
+    float* dst = (P.partial != nullptr) ? P.partial + (long long)split * P.part_stride : dw;
+    if (ksteps > 0) {
+#pragma unroll
+      for (int kw = 0; kw < 3; ++kw) {
+        WgradChunk ch;
+        ch.tap = (kh0 + wg) * 3 + kw; ch.c0 = cb * 64; ch.dh = 0; ch.dw = 0; ch.map = 0;
+        wgrad_store<BN, NWG == 3 ? 2 : 4>(P, dst, d[kw], ch, nt * BN, warp & 3, lane);   // 9 taps: within 128 registers
+      }
+    }
+  }
+}
+
 // dw[i] += sum over splits s = 0, 1, ... of part[s * stride + i], added in that order (4 elements per thread).  The
 // loads of 8 splits are issued together before their adds: one dependent DRAM round trip per split would make the
 // kernel latency-bound (tens of splits, few elements per thread).
@@ -1143,6 +1271,64 @@ static int choose_bn(int Cout, long long Mpix, int kblocks) {
   const long long mtiles = (Mpix + 127) / 128;
   const int kb[1] = {kblocks};
   return choose_bn_classes(Cout, mtiles, 1, kb);
+}
+
+// Halo geometry of a stride-1 3x3 wgrad plan for `taps` (3 or 9) filter taps per CTA, into P.  False when the pixel
+// box does not suit k_halo_wgrad: every k16 step must be two runs of 8 consecutive halo rows, the same distance
+// apart in every step (that distance is the descriptor's SBO), and the halo must fit its stage slot.
+static bool wgrad_halo_geometry(WgradParams& P, int taps) {
+  const int RW = (P.TW + 2 + 7) / 8 * 8, HR = P.TH + taps / 3 - 1;
+  const long long bytes = 128LL * RW * HR * P.TN;
+  if (P.TW % 8 != 0 || bytes > (long long)halo_max_bytes(taps / 3)) return false;
+  auto row = [&](int q) { return ((q / (P.TW * P.TH)) * HR + (q / P.TW) % P.TH) * RW + q % P.TW; };
+  const int sbo = row(8) - row(0);
+  for (int j = 0; j < 4; ++j) {
+    for (int i = 1; i < 8; ++i)
+      if (row(16 * j + i) != row(16 * j) + i || row(16 * j + 8 + i) != row(16 * j + 8) + i) return false;
+    if (row(16 * j + 8) - row(16 * j) != sbo) return false;
+  }
+  P.RW = RW; P.HR = HR; P.halo_bytes = (int)bytes; P.halo_sbo = sbo * 128;
+  for (int j = 0; j < 4; ++j) P.step_row[j] = row(16 * j);
+  return true;
+}
+
+static bool wgrad_halo_allowed(const ConvGeom& g, const WgradParams& P, int taps, int bn) {
+  if (g.split || g.stride != 1 || g.KH != 3 || g.KW != 3 || g.pad != 1 || g.in_pix_stride != 0) return false;
+  if (!((taps == 3 && (bn == 64 || bn == 128)) || (taps == 9 && bn == 64)) || g.Co % bn != 0) return false;
+  WgradParams Q = P;
+  return wgrad_halo_geometry(Q, taps);
+}
+
+// Switch a wgrad plan to the halo engine (taps 3 / 9, N tile bn) or back to the per-tap engine (taps 0).  The K
+// partition stays as it is: only the units of the grid change.
+static void wgrad_use_engine(TcConvPlan* p, int taps, int bn) {
+  WgradParams& P = p->WP;
+  P.halo_taps = taps; P.halo_bn = taps ? bn : 0;
+  if (taps) wgrad_halo_geometry(P, taps);
+  p->c_in0 = p->c_in1 = nullptr;         // the X tensor map's box changes
+  p->smem_attr_set = false;
+}
+
+static int wgrad_units(const WgradParams& P, int taps, int bn) {
+  return taps ? (P.Ci / 64) * (9 / taps) * (P.Co / bn) : P.n_mtiles * P.n_ntiles;
+}
+
+// Cycles of the busiest SM for one wgrad engine: waves x CTAs sharing the SM x k-blocks per CTA x max(MMA clocks,
+// operand bytes / L2 rate) per k-block.  MMA clocks: m64nBNk16 is 64 * BN * 16 MACs at 2048 per clock per SM.  Operand
+// bytes: per-tap engine 2 X chunks + the dY tile; halo engine the halo + the dY tile.  CTAs per SM come from the
+// kernels' shared memory and registers (checked with -Xptxas -v): per-tap 2, halo 3 taps at BN 64 2, else 1.  The L2
+// rate is the operand stream the fprop / dgrad engines reach on H100 (20-47 B/clk/SM, profiles/h100_conv_bound.md).
+static constexpr double kWgradL2BytesPerClk = 40.0;
+static double wgrad_cost(const WgradParams& P0, int taps, int bn) {
+  WgradParams P = P0;
+  if (taps) wgrad_halo_geometry(P, taps);
+  const double mma = (taps ? taps : 2) * 4 * bn / 2.0;
+  const double bytes = (taps ? P.halo_bytes : 2 * 8192) + bn * 128.0;
+  const int cps = taps ? ((taps == 3 && bn == 64) ? halo_ctas_per_sm(64, 1) : 1) : 2;
+  const long long per_sm = cdiv((long long)wgrad_units(P, taps, bn) * P.splits, kNumSMs);
+  const long long waves = (per_sm + cps - 1) / cps, conc = per_sm < cps ? per_sm : cps;
+  const double per_kb = mma > bytes / kWgradL2BytesPerClk ? mma : bytes / kWgradL2BytesPerClk;
+  return (double)waves * conc * P.tiles_per_split * per_kb;
 }
 
 static int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
@@ -1306,6 +1492,16 @@ int tc_plan_create(TcConvPlan** out, const ConvGeom& g, int kind, const bf16* wm
     if (splits > P.n_pix_tiles) splits = P.n_pix_tiles;
     P.tiles_per_split = cdiv(P.n_pix_tiles, splits);
     P.splits = cdiv(P.n_pix_tiles, P.tiles_per_split);
+    // the engine with the lowest modelled cost; the per-tap engine unless a halo engine is strictly cheaper
+    static const int kHalo[3][2] = {{3, 64}, {3, 128}, {9, 64}};
+    int taps = 0, bn = p->BN;
+    double best = wgrad_cost(P, 0, p->BN);
+    for (const auto& v : kHalo) {
+      if (!wgrad_halo_allowed(g, P, v[0], v[1])) continue;
+      const double c = wgrad_cost(P, v[0], v[1]);
+      if (c < best) { best = c; taps = v[0]; bn = v[1]; }
+    }
+    wgrad_use_engine(p, taps, bn);
   }
   *out = p;
   return 0;
@@ -1316,6 +1512,14 @@ void tc_plan_destroy(TcConvPlan* p) {
   delete p;
 }
 void tc_plan_set_out_scale(TcConvPlan* p, const float* inv_scale) { if (p != nullptr) p->out_scale = inv_scale; }
+
+int tc_plan_force_wgrad(TcConvPlan* p, int taps, int bn) {
+  MN_CHECK(p != nullptr && p->kind == 2, "tc_plan_force_wgrad: not a wgrad plan");
+  MN_CHECK(taps == 0 || wgrad_halo_allowed(p->g, p->WP, taps, bn),
+           "tc_plan_force_wgrad: no halo engine with %d taps at BN %d for this conv", taps, bn);
+  wgrad_use_engine(p, taps, bn);
+  return 0;
+}
 
 // Fold the dgrad of the block's 1x1 / stride-2 downsample conv into the (merged) dgrad of its 3x3 / stride-2 conv1:
 // both produce d(block input), the shortcut only reaches the pixel class (0, 0), where it is one more filter tap
@@ -1365,7 +1569,13 @@ int tc_plan_describe(const TcConvPlan* p, char* buf, int cap) {
       const int tap = i / P.cpt, c0 = (i - tap * P.cpt) * 64;
       put("%s[%d,%d,%d,%d,%d]", i ? "," : "", P.taps[tap].dh, P.taps[tap].dw, P.taps[tap].map, c0, tap);
     }
-    put("]}");
+    // the engine that runs it: taps 0 = k_tc_wgrad (BN above), 3 / 9 = k_halo_wgrad
+    const int bn = P.halo_taps ? P.halo_bn : P.BN;
+    put("],\"engine\":{\"taps\":%d,\"BN\":%d,\"units\":%d,\"grid\":%d,\"RW\":%d,\"HR\":%d,\"halo_bytes\":%d,"
+        "\"sbo\":%d,\"step_row\":[%d,%d,%d,%d]}}",
+        P.halo_taps, bn, wgrad_units(P, P.halo_taps, bn), wgrad_units(P, P.halo_taps, bn) * P.splits,
+        P.halo_taps ? P.RW : 0, P.halo_taps ? P.HR : 0, P.halo_taps ? P.halo_bytes : 0, P.halo_taps ? P.halo_sbo : 0,
+        P.step_row[0], P.step_row[1], P.step_row[2], P.step_row[3]);
   } else {
     put(",\"launches\":[");
     for (size_t li = 0; li < p->launches.size(); ++li) {
@@ -1559,20 +1769,29 @@ int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* res
   WgradParams& P = p->WP;
   P.oscale = p->out_scale;
   if (p->c_in0 != in0 || p->c_in1 != in1) {
-    for (int i = 0; i < p->w_nmaps; ++i)
-      MN_TRY(encode_view(&p->mapX[i], in0, g.B, g.Hi, g.Wi, SP * g.Ci, g.stride, p->wpa[i], p->wpb[i], P.TW, P.TH, P.TN, &g));
+    if (P.halo_taps) {       // the halo box: RW x HR pixels per image
+      MN_TRY(encode_view(&p->mapX[0], in0, g.B, g.Hi, g.Wi, g.Ci, 1, 0, 0, P.RW, P.HR, P.TN));
+    } else {
+      for (int i = 0; i < p->w_nmaps; ++i)
+        MN_TRY(encode_view(&p->mapX[i], in0, g.B, g.Hi, g.Wi, SP * g.Ci, g.stride, p->wpa[i], p->wpb[i], P.TW, P.TH, P.TN, &g));
+    }
     for (int i = p->w_nmaps; i < 4; ++i) p->mapX[i] = p->mapX[0];
     MN_TRY(encode_view(&p->mapDY, in1, g.B, g.Ho, g.Wo, SP * g.Co, 1, 0, 0, P.TW, P.TH, P.TN));
     p->c_in0 = in0; p->c_in1 = in1;
   }
-  const size_t smem = (size_t)wgrad_stages(p->BN) * (2 * 8192 + (p->BN / 64) * 8192) + 1024;
   void (*k1)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, WgradParams, float*) =
       (p->BN == 64) ? k_tc_wgrad<64> : k_tc_wgrad<128>;
+  void (*kh)(CUtensorMap, CUtensorMap, WgradParams, float*) =
+      P.halo_taps == 9 ? k_halo_wgrad<64, 3> : P.halo_bn == 64 ? k_halo_wgrad<64, 1> : k_halo_wgrad<128, 1>;
+  const size_t smem = !P.halo_taps ? (size_t)wgrad_stages(p->BN) * (2 * 8192 + (p->BN / 64) * 8192) + 1024
+                      : P.halo_taps == 9 ? halo_smem_bytes(64, 3) : P.halo_bn == 64 ? halo_smem_bytes(64, 1)
+                                                                                    : halo_smem_bytes(128, 1);
   if (!p->smem_attr_set) {
-    MN_TRY(set_smem(k1, smem));
+    if (P.halo_taps) MN_TRY(set_smem(kh, smem));
+    else MN_TRY(set_smem(k1, smem));
     p->smem_attr_set = true;
   }
-  const int grid = P.n_mtiles * P.n_ntiles * P.splits;
+  const int grid = wgrad_units(P, P.halo_taps, P.halo_taps ? P.halo_bn : p->BN) * P.splits;
   P.part_stride = (long long)g.Co * P.KK * g.Ci;
   P.partial = nullptr;
   if (P.splits > 1) {
@@ -1581,7 +1800,10 @@ int tc_conv_run(TcConvPlan* p, const bf16* in0, const bf16* in1, const bf16* res
     if (p->ws == nullptr) MN_CUDA(cudaMalloc(&p->ws, (size_t)P.splits * P.part_stride * sizeof(float)));
     P.partial = p->ws;
   }
-  MN_LAUNCH(k1, grid, kConvThreads, smem, st, p->mapX[0], p->mapX[1], p->mapX[2], p->mapX[3], p->mapDY, P, (float*)out);
+  if (P.halo_taps)
+    MN_LAUNCH(kh, grid, (P.halo_taps / 3) * 128 + 32, smem, st, p->mapX[0], p->mapDY, P, (float*)out);
+  else
+    MN_LAUNCH(k1, grid, kConvThreads, smem, st, p->mapX[0], p->mapX[1], p->mapX[2], p->mapX[3], p->mapDY, P, (float*)out);
   MN_LAUNCH_CHECK();
   if (P.splits > 1) {
     MN_TRY(launch_split_reduce(p->ws, P.splits, P.part_stride, (float*)out, st));

@@ -71,6 +71,9 @@ int tc_plan_launches(const TcConvPlan* p);
 // dgrad / wgrad plans: multiply the accumulators by the device scalar *inv_scale before they are added to the residual /
 // the wgrad buffer (strict mode: the gradient operand planes carry a per-step power-of-two scale)
 void tc_plan_set_out_scale(TcConvPlan* p, const float* inv_scale);
+// tests and micro-benchmarks only: run a wgrad plan on the per-tap engine (taps 0) or the halo engine with 3 / 9
+// filter taps per CTA at N tile bn, keeping the plan's K partition
+int tc_plan_force_wgrad(TcConvPlan* p, int taps, int bn);
 int tc_plan_describe(const TcConvPlan* p, char* buf, int cap);      // JSON, host-only (CPU tests of the plan arithmetic)
 // fprop: in0 = x, out = y (bf16);  dgrad: in0 = dy [, in1 = the folded shortcut's dy], out = dx (bf16);
 // wgrad: in0 = x, in1 = dy, out = fp32 dW (accumulated)

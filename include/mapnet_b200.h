@@ -652,6 +652,14 @@ int mapnet_test_pack_weights(int precision, int im2col_stem, int H, int W, const
 int mapnet_bench_conv(int kind, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* in0,
                       const void* in1, const void* wmat, void* out, int iters, float* host_ms);
 
+/* tests and tools/bench_conv.py: the wgrad of one conv on a chosen engine with the plan's K partition -- taps -1 = the
+ * planner's choice, 0 = the per-tap engine, 3 / 9 = the stride-1 3x3 halo engine with that many filter taps per CTA at
+ * N tile bn (3: 64 or 128; 9: 64).  x [B,Hi,Wi,Ci] and dy [B,Ho,Wo,Co] bf16, dw [Co][k*k][Ci] fp32 is added onto.
+ * iters 0: one run; else the average ms of iters timed runs (after 3 warm-ups) into *host_ms.  Returns after the
+ * launches complete. */
+int mapnet_test_wgrad(int taps, int bn, int B, int Hi, int Wi, int Ci, int Co, int k, int stride, const void* x,
+                      const void* dy, void* dw, int iters, float* host_ms);
+
 #ifdef __cplusplus
 }
 #endif
