@@ -19,6 +19,9 @@ LOSS_MODE = {"posenet": 0, "mapnet": 1, "online": 2, "online_gps": 3}
 
 TRACK_API = ["mapnet_track_create", "mapnet_track_step", "mapnet_track_flush", "mapnet_track_reset", "mapnet_track_status",
              "mapnet_track_destroy", "mapnet_track_step_now"]
+# the Cauchy-weighted pose graphs and each tracker handle's way to take one (csrc/pgo.cu, csrc/loader.cu)
+ROBUST_API = ["mapnet_pgo_optimize_robust", "mapnet_pgo_optimize_cov_robust", "mapnet_track_set_robust",
+              "mapnet_track_multi_set_robust", "mapnet_track_sample_set_robust", "mapnet_track_multi_sample_set_robust"]
 MAX_TRACK_STEPS = 16    # mapnet_track_create: windows of at most 16 frames (the PGO kernel's limit)
 TRACK_MULTI_API = ["mapnet_track_multi_create", "mapnet_track_multi_step", "mapnet_track_multi_flush",
                    "mapnet_track_multi_reset", "mapnet_track_multi_status", "mapnet_track_multi_destroy"]
@@ -209,6 +212,14 @@ def lib():
     L.mapnet_track_multi_sample_destroy.argtypes = [c_void_p]
     for name in TRACK_MULTI_SAMPLE_API:
         getattr(L, name).restype = c_int
+    L.mapnet_pgo_optimize_robust.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int] + \
+        [ctypes.c_double] * 4 + [c_int, c_int, ctypes.c_double, c_void_p, c_void_p, c_void_p]
+    L.mapnet_pgo_optimize_cov_robust.argtypes = [c_void_p] * 5 + [c_int, c_int, c_int, ctypes.c_double, ctypes.c_double,
+                                                                  c_int, ctypes.c_double, c_void_p, c_void_p, c_void_p]
+    for name in ROBUST_API[2:]:
+        getattr(L, name).argtypes = [c_void_p, ctypes.c_double]
+    for name in ROBUST_API:
+        getattr(L, name).restype = c_int
     L.mapnet_test_sample_factor.argtypes = [c_void_p, c_void_p, c_int64, ctypes.c_double, ctypes.c_double, c_void_p,
                                             c_void_p, c_void_p]
     L.mapnet_test_sample_factor.restype = c_int
@@ -262,7 +273,7 @@ EXPORTED = ["mapnet_last_error", "mapnet_abi_version", "mapnet_trunk_create", "m
             "mapnet_infer_sample_frames", "mapnet_sample_post", "mapnet_test_small_gemm_plan", "mapnet_test_stem_ex",
             "mapnet_test_head", "mapnet_pgo_optimize_cov",
             "mapnet_test_sample_factor", "mapnet_test_weight_table", "mapnet_test_pack_weights",
-            "mapnet_test_conv_simt", "mapnet_test_stem_im2col", "mapnet_test_trunk_create"] + TRACK_API + TRACK_MULTI_API + TRACK_SAMPLE_API + TRACK_MULTI_SAMPLE_API + EVAL_SAMPLE_API
+            "mapnet_test_conv_simt", "mapnet_test_stem_im2col", "mapnet_test_trunk_create"] + TRACK_API + TRACK_MULTI_API + TRACK_SAMPLE_API + TRACK_MULTI_SAMPLE_API + EVAL_SAMPLE_API + ROBUST_API
 UINT64_MAX = 0xFFFFFFFFFFFFFFFF
 MAX_SAMPLE_DRAWS = 1024      # mapnet_infer_sample: S in [2, MAX_SAMPLE_DRAWS] dropout draws per frame
 

@@ -260,18 +260,22 @@ int launch_rmsprop(float* p, const float* g, float* square_avg, float* grad_avg,
 // ---- pgo.cu: pose-graph optimisation of n_windows windows of N poses (k_pgo) --------------------------------------
 // w4 = (1/sqrt(sax), 1/sqrt(saq), 1/sqrt(srx), 1/sqrt(srq)) from pgo_weights; n_win_dev (may be null): a device count
 // of windows, the blocks beyond it exit; win_fail (may be null): per window 1 / 0, whether its normal matrix was not
-// positive definite.  pgo_prepare sets k_pgo's shared-memory limit once (not graph-capturable).
+// positive definite.  pgo_prepare sets k_pgo's shared-memory limit once (not graph-capturable).  robust_c > 0: the
+// absolute factors take the Cauchy loss of scale robust_c (whitened units, iteratively reweighted; k_pgo<true>), and
+// w_out (may be null) [n_windows][N] gets each slot's weight at the returned state; 0: the plain k_pgo<false>.
 int pgo_prepare();
 void pgo_weights(double sax, double saq, double srx, double srq, double w4[4]);
 int launch_pgo(const double* poses, const double* vos, double* out, int n_windows, int N, int fc, const double w4[4],
-               int n_iters, int exact, int* status, const int* n_win_dev, cudaStream_t st, int* win_fail = nullptr);
+               int n_iters, int exact, int* status, const int* n_win_dev, cudaStream_t st, int* win_fail = nullptr,
+               double robust_c = 0.0, double* w_out = nullptr);
 // k_pgo_cov: sig7 [n_windows][N][7][7] covariances of the absolute factors, relative weights w_rx = 1/sqrt(srx) and
 // w_rq = 1/sqrt(srq), the exact Gauss-Newton step; out [n_windows][N][7] and the posterior cov [n_windows][N][6][6]
-// in (t, log q).  n_win_dev, win_fail, status as launch_pgo's.  pgo_cov_prepare sets its shared-memory limit once.
+// in (t, log q).  n_win_dev, win_fail, status, robust_c and w_out as launch_pgo's (the posterior is taken with the
+// weights at the returned state).  pgo_cov_prepare sets its shared-memory limit once.
 int pgo_cov_prepare();
 int launch_pgo_cov(const double* poses, const double* sig7, const double* vos, double* out, double* cov, int n_windows,
                    int N, int fc, double w_rx, double w_rq, int n_iters, int* status, const int* n_win_dev,
-                   int* win_fail, cudaStream_t st);
+                   int* win_fail, cudaStream_t st, double robust_c = 0.0, double* w_out = nullptr);
 
 // input pipeline internals shared by preprocess.cu and the frame cache (loader.cu)
 struct JitterParams;

@@ -138,6 +138,8 @@ struct TrackHandle : TrackCfg {
   double *ring7, *ring49;                   // [n_streams][R][7], [n_streams][R][7][7]: p and S7 of the last R frames
   float* ring_vo;                           // [n_streams][R][6]: their VO-library poses
   double *win7, *win49, *vos7, *opt7, *cov36;   // [max_win][T][7], [.][T][49], [.][E][7], [.][T][7], [.][T][36]
+  double robust_c;                          // > 0: the Cauchy scale of the absolute factors (fixed before the first step)
+  bool started;                             // a step or flush has been enqueued: robust_c is fixed
 };
 
 __device__ __forceinline__ const float* track_src(const float* fresh, const float* ring, long long f, long long seen,
@@ -248,7 +250,8 @@ struct PointFactor {
     track_emit_pose(opt7 + 7 * k, un, ms, ss, o);
   }
   int pgo(const TrackHandle& h, int nw, int* status, const int* n_win_dev, int* win_fail, cudaStream_t st) const {
-    return launch_pgo(h.win7, h.vos7, h.opt7, nw, h.T, h.fc, h.w4, 10, 0, status, n_win_dev, st, win_fail);
+    return launch_pgo(h.win7, h.vos7, h.opt7, nw, h.T, h.fc, h.w4, 10, 0, status, n_win_dev, st, win_fail,
+                      h.robust_c);
   }
 };
 
@@ -292,7 +295,7 @@ struct SampleFactor {
   }
   int pgo(const TrackHandle& h, int nw, int* status, const int* n_win_dev, int* win_fail, cudaStream_t st) const {
     return launch_pgo_cov(h.win7, h.win49, h.vos7, h.opt7, h.cov36, nw, h.T, h.fc, h.w4[2], h.w4[3], 10, status,
-                          n_win_dev, win_fail, st);
+                          n_win_dev, win_fail, st, h.robust_c);
   }
 };
 
@@ -918,6 +921,16 @@ static int track_reset(TrackHandle* h, int s, cudaStream_t stream) {
   return 0;
 }
 
+// the Cauchy scale c of every window's absolute factors from now on; refused once the handle has enqueued a step or
+// a flush, so every window of the handle's life (and every graph that captured its launches) has the same loss
+static int track_set_robust(TrackHandle* h, const char* who, double c) {
+  MN_CHECK(h != nullptr, "%s: null handle", who);
+  MN_CHECK(c > 0 && isfinite(c), "%s: the Cauchy scale c = %g must be finite and positive", who, c);
+  MN_CHECK(!h->started, "%s: the handle has already stepped; set the robust loss before the first step", who);
+  h->robust_c = c;
+  return 0;
+}
+
 static int track_status(TrackHandle* h, int s, int64_t* frames_seen, int* failed, cudaStream_t stream) {
   TrackDev d;
   MN_CUDA(cudaMemcpyAsync(&d, h->st + s, sizeof(TrackDev), cudaMemcpyDeviceToHost, stream));
@@ -934,6 +947,7 @@ static int track_launch(TrackHandle* h, F fac, const float* vo6, int n, int flus
                         cudaStream_t st) {
   const int nw = flush ? (int)(h->lag < h->max_win ? h->lag : h->max_win) : n;   // the grid's windows
   const long long rows = n + (long long)nw * (h->T + h->E);
+  h->started = true;
   MN_LAUNCH(k_track_gather<F>, cdiv(rows, 128), 128, 0, st, fac, vo6, n, flush, now != nullptr ? 1 : 0,
             (const TrackDev*)h->st, h->n_win, h->ring_vo, h->R, h->T, h->skip, h->fc, nw, h->vos7);
   MN_LAUNCH_CHECK();
@@ -952,6 +966,7 @@ static int track_multi_launch(TrackHandle* h, F fac, const float* vo6, const MTr
   const int nw = flush_s >= 0 ? (int)(h->lag < h->max_win ? h->lag : h->max_win) : B;    // the grid's windows
   const int zl = now != nullptr ? 1 : 0;
   const long long rows = B + (long long)nw * (h->T + h->E);
+  h->started = true;
   MN_LAUNCH(k_track_multi_gather<F>, cdiv(rows, 128), 128, 0, st, fac, vo6, rec, B, zl, flush_s,
             (const TrackDev*)h->st, h->n_streams, h->n_win, h->ring_vo, h->R, h->T, h->skip, h->fc, nw, h->vos7);
   MN_LAUNCH_CHECK();
@@ -1001,6 +1016,8 @@ int mapnet_track_status(mapnet_track_t* h, int64_t* frames_seen, int* failed, vo
   MN_CHECK(h != nullptr, "track_status: null handle");
   return track_status(h, 0, frames_seen, failed, (cudaStream_t)stream);
 }
+
+int mapnet_track_set_robust(mapnet_track_t* h, double c) { return track_set_robust(h, "track_set_robust", c); }
 
 int mapnet_track_destroy(mapnet_track_t* h) { return track_destroy(h); }
 
@@ -1055,6 +1072,8 @@ int mapnet_test_sample_factor(const double* mean6, const double* cov36, int64_t 
   return 0;
 }
 
+int mapnet_track_sample_set_robust(mapnet_track_sample_t* h, double c) { return track_set_robust(h, "track_sample_set_robust", c); }
+
 int mapnet_track_sample_destroy(mapnet_track_sample_t* h) { return track_destroy(h); }
 
 int mapnet_track_multi_create(mapnet_track_multi_t** out, int n_streams, int T, int skip, int fc_vos, int max_batch,
@@ -1091,6 +1110,8 @@ int mapnet_track_multi_status(mapnet_track_multi_t* h, int s, int64_t* frames_se
   MN_CHECK(s >= 0 && s < h->n_streams, "track_multi_status: stream %d outside [0, %d)", s, h->n_streams);
   return track_status(h, s, frames_seen, failed, (cudaStream_t)stream);
 }
+
+int mapnet_track_multi_set_robust(mapnet_track_multi_t* h, double c) { return track_set_robust(h, "track_multi_set_robust", c); }
 
 int mapnet_track_multi_destroy(mapnet_track_multi_t* h) { return track_destroy(h); }
 
@@ -1134,6 +1155,8 @@ int mapnet_track_multi_sample_status(mapnet_track_multi_sample_t* h, int s, int6
   MN_CHECK(s >= 0 && s < h->n_streams, "track_multi_sample_status: stream %d outside [0, %d)", s, h->n_streams);
   return track_status(h, s, frames_seen, failed, (cudaStream_t)stream);
 }
+
+int mapnet_track_multi_sample_set_robust(mapnet_track_multi_sample_t* h, double c) { return track_set_robust(h, "track_multi_sample_set_robust", c); }
 
 int mapnet_track_multi_sample_destroy(mapnet_track_multi_sample_t* h) { return track_destroy(h); }
 

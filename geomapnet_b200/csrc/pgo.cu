@@ -78,15 +78,42 @@ __device__ __forceinline__ void dqstq_t(const Q4& q, double D[3][3]) {
     for (int b = 0; b < 3; ++b) D[a][b] = (a == b ? c : 0.0) + 2.0 * v[a] * v[b] - 2.0 * q.w * S[a][b];
 }
 
+// Cauchy weight of an absolute factor whose whitened residual is r [7]: omega = 1 / (1 + |r|^2 / c^2), the IRLS
+// weight of rho(s) = c^2 log(1 + s / c^2) (rho'(s) = omega).  s / c^2 is summed as (r_k / c)^2, so a zero residual gives
+// omega = 1 and an overflowing one omega = 0 for every finite c > 0, never 0 / 0.
+__device__ __forceinline__ double cauchy_weight(const double r[7], double c) {
+  double u = 0.0;
+#pragma unroll
+  for (int a = 0; a < 7; ++a) {
+    const double e = r[a] / c;
+    u += e * e;
+  }
+  return 1.0 / (1.0 + u);
+}
+
+// k_pgo's absolute factor of slot i at state z: its Cauchy weight at scale c (residual (w_ax (t - t0), w_aq (q - q0)))
+__device__ __forceinline__ double pgo_point_weight(const double* z, const double* P, int i, double w_ax, double w_aq,
+                                                   double c) {
+  double r[7];
+#pragma unroll
+  for (int a = 0; a < 7; ++a) r[a] = (a < 3 ? w_ax : w_aq) * (z[7 * i + a] - P[7 * i + a]);
+  return cauchy_weight(r, c);
+}
+
 // One window per block.  Constraints are dealt to threads; each thread accumulates into the shared H / b with
 // double atomics (a few hundred constraints x <= 144 entries: contention is irrelevant next to the Cholesky).
 // n_win_dev (may be null): the device count of windows to optimise; the blocks beyond it exit, so a captured graph can
 // keep a fixed grid while the count changes from replay to replay.  win_fail (may be null): per window, 1 when its
 // normal matrix was not positive definite, else 0, so a caller can tell which windows failed.
+// kRobust: iteratively reweighted Gauss-Newton for the Cauchy loss on the absolute factors -- in every iteration the
+// unary work item of slot i weighs its H and b contributions by omega_i = cauchy_weight at the iteration's starting
+// state (scale c, whitened units); w_out (may be null) [W][N] gets omega at the returned state.  The step rule (exact)
+// is unchanged.  Without kRobust, c and w_out are not read.
+template <bool kRobust>
 __global__ void __launch_bounds__(kPgoThreads)
 k_pgo(const double* __restrict__ poses, const double* __restrict__ vos, double* __restrict__ out, int N, int fc,
       double w_ax, double w_aq, double w_rx, double w_rq, int n_iters, int exact, int* __restrict__ status,
-      const int* __restrict__ n_win_dev, int* __restrict__ win_fail) {
+      const int* __restrict__ n_win_dev, int* __restrict__ win_fail, double c, double* __restrict__ w_out) {
   pdl_prologue();
   if (n_win_dev != nullptr && (int)blockIdx.x >= *n_win_dev) return;
   extern __shared__ double sm[];
@@ -107,14 +134,17 @@ k_pgo(const double* __restrict__ poses, const double* __restrict__ vos, double* 
     for (int i = threadIdx.x; i < D * D + D; i += blockDim.x) H[i] = 0.0;
     __syncthreads();
     // ---- unary constraints + pairwise constraints: work items 0..N-1 unary, N..N+E-1 edges ----
-    for (int c = threadIdx.x; c < N + E; c += blockDim.x) {
-      if (c < N) {
-        const int i = c;
+    for (int f = threadIdx.x; f < N + E; f += blockDim.x) {
+      if (f < N) {
+        const int i = f;
         const Q4 q = {z[7 * i + 3], z[7 * i + 4], z[7 * i + 5], z[7 * i + 6]};
+        double om = 1.0;                         // the slot's Cauchy weight (1: plain least squares)
+        if constexpr (kRobust) om = pgo_point_weight(z, P, i, w_ax, w_aq, c);
+        const double wx2 = kRobust ? om * (w_ax * w_ax) : w_ax * w_ax;
         // translation: J = w_ax I, r = w_ax (t - t0)
         for (int a = 0; a < 3; ++a) {
-          atomicAdd(&H[(6 * i + a) * D + 6 * i + a], w_ax * w_ax);
-          atomicAdd(&bv[6 * i + a], w_ax * w_ax * (z[7 * i + a] - P[7 * i + a]));
+          atomicAdd(&H[(6 * i + a) * D + 6 * i + a], wx2);
+          atomicAdd(&bv[6 * i + a], wx2 * (z[7 * i + a] - P[7 * i + a]));
         }
         double M[4][3], r[4];
         m_rot(q, M);
@@ -126,14 +156,14 @@ k_pgo(const double* __restrict__ poses, const double* __restrict__ vos, double* 
           for (int b = 0; b < 3; ++b) {
             double s = 0.0;
             for (int k = 0; k < 4; ++k) s += M[k][a] * M[k][b];
-            atomicAdd(&H[(6 * i + 3 + a) * D + 6 * i + 3 + b], s);
+            atomicAdd(&H[(6 * i + 3 + a) * D + 6 * i + 3 + b], kRobust ? om * s : s);
           }
           double s = 0.0;
           for (int k = 0; k < 4; ++k) s += M[k][a] * r[k];
-          atomicAdd(&bv[6 * i + 3 + a], s);
+          atomicAdd(&bv[6 * i + 3 + a], kRobust ? om * s : s);
         }
       } else {
-        int e = c - N, i, j;
+        int e = f - N, i, j;
         if (!fc) { i = e; j = e + 1; }
         else {                                   // row-major enumeration of the pairs i < j
           i = 0;
@@ -244,23 +274,38 @@ k_pgo(const double* __restrict__ poses, const double* __restrict__ vos, double* 
   }
   double* O = out + (size_t)W * N * 7;
   for (int i = threadIdx.x; i < 7 * N; i += blockDim.x) O[i] = z[i];
+  if constexpr (kRobust) {
+    if (w_out != nullptr)
+      for (int i = threadIdx.x; i < N; i += blockDim.x) w_out[(size_t)W * N + i] = pgo_point_weight(z, P, i, w_ax, w_aq, c);
+  }
   if (threadIdx.x == 0 && s_fail && status != nullptr) atomicExch(status, 1);
   if (threadIdx.x == 0 && win_fail != nullptr) win_fail[W] = s_fail;
 }
 
 int pgo_prepare() {
   static bool attr = false;
-  if (!attr) { MN_CUDA(cudaFuncSetAttribute(k_pgo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(96 * 96 + 96 * 2 + 7 * 16) * 8)); attr = true; }
+  if (!attr) {
+    const int smem = (int)(96 * 96 + 96 * 2 + 7 * 16) * 8;
+    MN_CUDA(cudaFuncSetAttribute(k_pgo<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    MN_CUDA(cudaFuncSetAttribute(k_pgo<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attr = true;
+  }
   return 0;
 }
 
 int launch_pgo(const double* poses, const double* vos, double* out, int n_windows, int N, int fc, const double w4[4],
-               int n_iters, int exact, int* status, const int* n_win_dev, cudaStream_t st, int* win_fail) {
+               int n_iters, int exact, int* status, const int* n_win_dev, cudaStream_t st, int* win_fail,
+               double robust_c, double* w_out) {
   MN_TRY(pgo_prepare());
   const int D = 6 * N;
   const size_t smem = (size_t)(D * D + D + 7 * N + D) * sizeof(double);
-  MN_LAUNCH(k_pgo, n_windows, kPgoThreads, smem, st, poses, vos, out, N, fc, w4[0], w4[1], w4[2], w4[3], n_iters, exact,
-            status, n_win_dev, win_fail);
+  if (robust_c > 0.0) {
+    MN_LAUNCH(k_pgo<true>, n_windows, kPgoThreads, smem, st, poses, vos, out, N, fc, w4[0], w4[1], w4[2], w4[3],
+              n_iters, exact, status, n_win_dev, win_fail, robust_c, w_out);
+  } else {
+    MN_LAUNCH(k_pgo<false>, n_windows, kPgoThreads, smem, st, poses, vos, out, N, fc, w4[0], w4[1], w4[2], w4[3],
+              n_iters, exact, status, n_win_dev, win_fail, 0.0, (double*)nullptr);
+  }
   MN_LAUNCH_CHECK();
   return 0;
 }
@@ -316,15 +361,19 @@ __device__ __forceinline__ void qlog_jac(const Q4& q, double G[3][3]) {
     }
 }
 
-// H (D x D) and b at state z: each factor's record, then one thread per entry sums the records touching it
+// H (D x D) and b at state z: each factor's record, then one thread per entry sums the records touching it.
+// kRobust: slot i's record is weighed by its Cauchy weight at z (scale c), which it also writes to w_out[i] when
+// w_out is not null.
+template <bool kRobust>
 __device__ void pgo_cov_normal(const double* z, const double* P, const double* Li, const double* V, int N, int fc,
-                               int E, double w_rx, double w_rq, double* rec, double* H, double* bv) {
+                               int E, double w_rx, double w_rq, double* rec, double* H, double* bv, double c,
+                               double* w_out) {
   const int D = 6 * N;
   double* ru = rec;                       // [N][kUnaryRec]
   double* re = rec + N * kUnaryRec;       // [E][kEdgeRec]
-  for (int c = threadIdx.x; c < N + E; c += blockDim.x) {
-    if (c < N) {
-      const int i = c;
+  for (int f = threadIdx.x; f < N + E; f += blockDim.x) {
+    if (f < N) {
+      const int i = f;
       const Q4 q = {z[7 * i + 3], z[7 * i + 4], z[7 * i + 5], z[7 * i + 6]};
       double M[4][3], d[7], r[7], J[7][6];
       m_rot(q, M);
@@ -341,19 +390,24 @@ __device__ void pgo_cov_normal(const double* z, const double* P, const double* L
           J[a][3 + cc] = s;
         }
       }
+      double om = 1.0;                      // the slot's Cauchy weight (1: plain least squares)
+      if constexpr (kRobust) {
+        om = cauchy_weight(r, c);
+        if (w_out != nullptr) w_out[i] = om;
+      }
       double* o = ru + kUnaryRec * i;
       for (int a = 0; a < 6; ++a) {
         for (int b = 0; b < 6; ++b) {
           double s = 0.0;
           for (int k = 0; k < 7; ++k) s += J[k][a] * J[k][b];
-          o[6 * a + b] = s;
+          o[6 * a + b] = kRobust ? om * s : s;
         }
         double s = 0.0;
         for (int k = 0; k < 7; ++k) s += J[k][a] * r[k];
-        o[36 + a] = s;
+        o[36 + a] = kRobust ? om * s : s;
       }
     } else {
-      const int e = c - N;
+      const int e = f - N;
       int i, j;
       trackcore::vo_pair(e, N, fc, &i, &j);
       const Q4 qi = {z[7 * i + 3], z[7 * i + 4], z[7 * i + 5], z[7 * i + 6]};
@@ -495,10 +549,15 @@ __device__ void pgo_cov_solve(const double* R, const double* bv, int D, double* 
 
 // One window per block (kPgoThreads threads).  poses [W][N][7] (the absolute poses p), sig7 [W][N][7][7] (their
 // covariances), vos [W][E][7] -> out [W][N][7], cov [W][N][6][6]; n_win_dev, win_fail and status as for k_pgo.
+// kRobust: the absolute factors are Cauchy-weighted as in k_pgo<true>, each iteration's weights taken at its starting
+// state; the posterior's normal matrix is built at the returned state with the weights at that state, which w_out
+// (may be null) [W][N] gets.  Without kRobust, c and w_out are not read.
+template <bool kRobust>
 __global__ void __launch_bounds__(kPgoThreads)
 k_pgo_cov(const double* __restrict__ poses, const double* __restrict__ sig7, const double* __restrict__ vos,
           double* __restrict__ out, double* __restrict__ cov, int N, int fc, double w_rx, double w_rq, int n_iters,
-          int* __restrict__ status, const int* __restrict__ n_win_dev, int* __restrict__ win_fail) {
+          int* __restrict__ status, const int* __restrict__ n_win_dev, int* __restrict__ win_fail, double c,
+          double* __restrict__ w_out) {
   pdl_prologue();
   if (n_win_dev != nullptr && (int)blockIdx.x >= *n_win_dev) return;
   extern __shared__ double sm[];
@@ -543,7 +602,8 @@ k_pgo_cov(const double* __restrict__ poses, const double* __restrict__ sig7, con
   }
   __syncthreads();
   for (int it = 0; it <= n_iters; ++it) {
-    pgo_cov_normal(z, P, Li, V, N, fc, E, w_rx, w_rq, rec, H, bv);
+    pgo_cov_normal<kRobust>(z, P, Li, V, N, fc, E, w_rx, w_rq, rec, H, bv, c,
+                            kRobust && it == n_iters && w_out != nullptr ? w_out + (size_t)W * N : nullptr);
     pgo_cov_cholesky(H, D, &s_fail);
     if (it == n_iters) break;               // the posterior's factor, at the returned state
     pgo_cov_solve(H, bv, D, xs);
@@ -628,7 +688,10 @@ static size_t pgo_cov_smem(int N) {
 int pgo_cov_prepare() {
   static bool attr = false;
   if (!attr) {
-    MN_CUDA(cudaFuncSetAttribute(k_pgo_cov, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pgo_cov_smem(kPgoMaxN)));
+    MN_CUDA(cudaFuncSetAttribute(k_pgo_cov<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)pgo_cov_smem(kPgoMaxN)));
+    MN_CUDA(cudaFuncSetAttribute(k_pgo_cov<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)pgo_cov_smem(kPgoMaxN)));
     attr = true;
   }
   return 0;
@@ -636,10 +699,15 @@ int pgo_cov_prepare() {
 
 int launch_pgo_cov(const double* poses, const double* sig7, const double* vos, double* out, double* cov, int n_windows,
                    int N, int fc, double w_rx, double w_rq, int n_iters, int* status, const int* n_win_dev,
-                   int* win_fail, cudaStream_t st) {
+                   int* win_fail, cudaStream_t st, double robust_c, double* w_out) {
   MN_TRY(pgo_cov_prepare());
-  MN_LAUNCH(k_pgo_cov, n_windows, kPgoThreads, pgo_cov_smem(N), st, poses, sig7, vos, out, cov, N, fc, w_rx, w_rq,
-            n_iters, status, n_win_dev, win_fail);
+  if (robust_c > 0.0) {
+    MN_LAUNCH(k_pgo_cov<true>, n_windows, kPgoThreads, pgo_cov_smem(N), st, poses, sig7, vos, out, cov, N, fc, w_rx,
+              w_rq, n_iters, status, n_win_dev, win_fail, robust_c, w_out);
+  } else {
+    MN_LAUNCH(k_pgo_cov<false>, n_windows, kPgoThreads, pgo_cov_smem(N), st, poses, sig7, vos, out, cov, N, fc, w_rx,
+              w_rq, n_iters, status, n_win_dev, win_fail, 0.0, (double*)nullptr);
+  }
   MN_LAUNCH_CHECK();
   return 0;
 }
@@ -673,6 +741,37 @@ extern "C" int mapnet_pgo_optimize_cov(const double* poses, const double* sig7, 
            "pgo_optimize_cov: no CUDA device (this library has no CPU fallback)");
   return launch_pgo_cov(poses, sig7, vos, out, cov, n_windows, N, fc_vos ? 1 : 0, 1.0 / sqrt(srx), 1.0 / sqrt(srq),
                         n_iters, status_dev, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int mapnet_pgo_optimize_robust(const double* poses, const double* vos, double* out, int n_windows, int N,
+                                          int fc_vos, double sax, double saq, double srx, double srq, int n_iters,
+                                          int flags, double c, double* w, int* status_dev, void* stream) {
+  MN_CHECK(poses && vos && out && n_windows >= 1, "pgo_optimize_robust: bad argument");
+  MN_CHECK(N >= 2 && N <= kPgoMaxN, "pgo_optimize_robust: window of %d poses outside [2, %d]", N, kPgoMaxN);
+  MN_CHECK(sax > 0 && saq > 0 && srx > 0 && srq > 0 && n_iters >= 0,
+           "pgo_optimize_robust: covariances must be positive");
+  MN_CHECK(c > 0 && isfinite(c), "pgo_optimize_robust: the Cauchy scale c = %g must be finite and positive", c);
+  int ndev = 0;
+  MN_CHECK(cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0,
+           "pgo_optimize_robust: no CUDA device (this library has no CPU fallback)");
+  double w4[4];
+  pgo_weights(sax, saq, srx, srq, w4);
+  return launch_pgo(poses, vos, out, n_windows, N, fc_vos ? 1 : 0, w4, n_iters, flags & 1, status_dev, nullptr,
+                    (cudaStream_t)stream, nullptr, c, w);
+}
+
+extern "C" int mapnet_pgo_optimize_cov_robust(const double* poses, const double* sig7, const double* vos, double* out,
+                                              double* cov, int n_windows, int N, int fc_vos, double srx, double srq,
+                                              int n_iters, double c, double* w, int* status_dev, void* stream) {
+  MN_CHECK(poses && sig7 && vos && out && cov && n_windows >= 1, "pgo_optimize_cov_robust: bad argument");
+  MN_CHECK(N >= 2 && N <= kPgoMaxN, "pgo_optimize_cov_robust: window of %d poses outside [2, %d]", N, kPgoMaxN);
+  MN_CHECK(srx > 0 && srq > 0 && n_iters >= 0, "pgo_optimize_cov_robust: covariances must be positive");
+  MN_CHECK(c > 0 && isfinite(c), "pgo_optimize_cov_robust: the Cauchy scale c = %g must be finite and positive", c);
+  int ndev = 0;
+  MN_CHECK(cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0,
+           "pgo_optimize_cov_robust: no CUDA device (this library has no CPU fallback)");
+  return launch_pgo_cov(poses, sig7, vos, out, cov, n_windows, N, fc_vos ? 1 : 0, 1.0 / sqrt(srx), 1.0 / sqrt(srq),
+                        n_iters, status_dev, nullptr, nullptr, (cudaStream_t)stream, c, w);
 }
 
 // qexp + un-normalisation of a batch of 6-vectors (scripts/eval.py:163-181): out[i] = (t * pose_s + pose_m, qexp(logq))

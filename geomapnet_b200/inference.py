@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .common.pgo import optimize_pose_windows
+from .common.pgo import check_robust_c, optimize_pose_windows
 from .data.loader import SidePipeline
 
 __all__ = ["Predictor", "Localizer", "Tracker", "MultiTracker", "SampledTracker", "predict", "post", "pgo", "pose_errors", "evaluate_tuples", "evaluate_sequence", "validate"]
@@ -570,12 +570,18 @@ class Tracker(object):
     gather the windows from device rings of recent poses, k_pgo, emit), with the frame counter in device memory; a
     call never waits for the device.  The host counts frames too, so the frames a call emits follow from the call
     sizes.  A window whose normal matrix is not positive definite (where scipy's cholesky raises) is reported by
-    flush(), which raises np.linalg.LinAlgError after resetting."""
+    flush(), which raises np.linalg.LinAlgError after resetting.
+
+    robust_c=c (a finite number > 0, in sigmas) gives every window's absolute factors the Cauchy loss of scale c
+    (common.pgo.optimize_pose_windows(robust_c=c)): a frame whose prediction is far off -- glare, occlusion -- is
+    down-weighted in each window that holds it instead of pulling on all of them.  The output formats, launches and
+    chunking stay; the poses are bit for bit evaluate_sequence(..., robust_c=c)'s.  A bad robust_c raises ValueError
+    here, before anything is launched."""
 
     _API = "mapnet_track"       # the handle's C calls: _API + "_create", "_step", "_step_now", "_flush", ...
     _ROW = 7                    # doubles per output row
 
-    def __init__(self, localizer, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0):
+    def __init__(self, localizer, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0, robust_c=None):
         if not isinstance(localizer, Localizer):
             raise TypeError("Tracker wraps a geomapnet_b200.inference.Localizer, got %s" % type(localizer).__name__)
         self.steps = _int_arg(steps, "steps", 2, _lib.MAX_TRACK_STEPS)
@@ -583,6 +589,7 @@ class Tracker(object):
         self.sigmas = [float(v) for v in (sax, saq, srx, srq)]
         if not all(v > 0 for v in self.sigmas):
             raise ValueError("sax, saq, srx, srq must be positive, got %s" % (self.sigmas,))
+        self.robust_c = check_robust_c(robust_c)
         self.loc, self.vo_fc = localizer, bool(vo_fc)
         self.lag = (self.steps - 1 - self.steps // 2) * self.skip
         self.seen = 0           # frames of the current sequence, mirrored on the device
@@ -626,7 +633,13 @@ class Tracker(object):
             _lib.check(getattr(_lib.lib(), self._API + "_create")(ctypes.byref(self.h), self.steps, self.skip,
                                                                   int(self.vo_fc), pr.max_batch, sig, self.loc._m,
                                                                   self.loc._s), self._API + "_create")
+            self._set_robust()
         return self.h
+
+    def _set_robust(self):
+        """the new handle's Cauchy scale, before its first step (nothing is launched)"""
+        if self.robust_c is not None:
+            _lib.check(getattr(_lib.lib(), self._API + "_set_robust")(self.h, self.robust_c), self._API + "_set_robust")
 
     def _graph(self, fb, now=False):
         B, H, W = fb.shape[:3]
@@ -796,13 +809,15 @@ class SampledTracker(Tracker):
     three tracking launches (csrc/loader.cu, mapnet_track_sample_*: gather, k_pgo_cov, emit).  The eager run before the
     capture uses an explicit dropout step and runs no tracking launch, so it advances neither the dropout counter nor
     the sequence.  Engines, snapshot, refresh(), precision and dropout counter are the Localizer's predictor's.  S as
-    Localizer.sample takes it: 2 <= S <= 1024, and a model without dropout raises ValueError."""
+    Localizer.sample takes it: 2 <= S <= 1024, and a model without dropout raises ValueError.  robust_c as Tracker's, on
+    the whitened residual C^-1 (z - p): a frame that is wrong and confident (small Sigma_f) is down-weighted too, and
+    each posterior is taken with the weights at the returned state."""
 
     _API = "mapnet_track_sample"
     _ROW = _lib.TRACK_SAMPLE_ROW
 
-    def __init__(self, localizer, S, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0):
-        super(SampledTracker, self).__init__(localizer, steps, skip, vo_fc, sax, saq, srx, srq)
+    def __init__(self, localizer, S, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0, robust_c=None):
+        super(SampledTracker, self).__init__(localizer, steps, skip, vo_fc, sax, saq, srx, srq, robust_c)
         self.S = _check_draws(S, localizer.predictor.droprate)
 
     @staticmethod
@@ -871,12 +886,13 @@ class MultiTracker(Tracker):
     captures; the per-frame records (stream, rank, counts, frame index, output row) are built on the host from its own
     counts and copied in with the frames.  All frames of a call share one H x W.  A window whose normal matrix is not
     positive definite marks its own stream only: flush(s) raises np.linalg.LinAlgError for stream s after resetting
-    it."""
+    it.  robust_c as Tracker's, for every stream."""
 
     _API = "mapnet_track_multi"
 
-    def __init__(self, localizer, n_streams, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0):
-        super(MultiTracker, self).__init__(localizer, steps, skip, vo_fc, sax, saq, srx, srq)
+    def __init__(self, localizer, n_streams, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0,
+                 robust_c=None):
+        super(MultiTracker, self).__init__(localizer, steps, skip, vo_fc, sax, saq, srx, srq, robust_c)
         self.n_streams = _int_arg(n_streams, "n_streams", 1, _lib.MAX_TRACK_STREAMS)
         self.seen = np.zeros(self.n_streams, dtype=np.int64)    # frames of each stream's sequence, mirrored on the device
 
@@ -887,6 +903,7 @@ class MultiTracker(Tracker):
             _lib.check(getattr(_lib.lib(), self._API + "_create")(ctypes.byref(self.h), self.n_streams, self.steps,
                                                                   self.skip, int(self.vo_fc), pr.max_batch, sig,
                                                                   self.loc._m, self.loc._s), self._API + "_create")
+            self._set_robust()
         return self.h
 
     def _stream_ids(self, streams, B, single):
@@ -1029,21 +1046,24 @@ class SampledMultiTracker(MultiTracker):
     with the frames.  The eager run before a capture uses an explicit dropout step and makes no tracking launch, so it
     advances neither the dropout counter nor any stream.  A window whose normal matrix or one of whose frames' factor
     covariances is not positive definite marks its own stream only: flush(s) raises np.linalg.LinAlgError for stream s
-    after resetting it."""
+    after resetting it.  robust_c as SampledTracker's, for every stream."""
 
     _API = "mapnet_track_multi_sample"
     _ROW = SampledTracker._ROW
     _est = staticmethod(SampledTracker._est)
     _capture = SampledTracker._capture
 
-    def __init__(self, localizer, S, n_streams, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0):
-        super(SampledMultiTracker, self).__init__(localizer, n_streams, steps, skip, vo_fc, sax, saq, srx, srq)
+    def __init__(self, localizer, S, n_streams, steps, skip=1, vo_fc=False, sax=1.0, saq=1.0, srx=1.0, srq=1.0,
+                 robust_c=None):
+        super(SampledMultiTracker, self).__init__(localizer, n_streams, steps, skip, vo_fc, sax, saq, srx, srq,
+                                                  robust_c)
         self.S = _check_draws(S, localizer.predictor.droprate)
 
 
-def pgo(pred7, vos7, sax=1.0, saq=1.0, srx=1.0, srq=1.0, fc_vos=False):
-    """eval.py:172-178 for all windows at once: pred7 [W,N,7], vos7 [W,N-1,7] -> [W,N,7]"""
-    return optimize_pose_windows(pred7, vos7, fc_vos=fc_vos, sax=sax, saq=saq, srx=srx, srq=srq)
+def pgo(pred7, vos7, sax=1.0, saq=1.0, srx=1.0, srq=1.0, fc_vos=False, robust_c=None):
+    """eval.py:172-178 for all windows at once: pred7 [W,N,7], vos7 [W,N-1,7] -> [W,N,7]; with robust_c, (poses,
+    w [W,N]) of the Cauchy-weighted graph (optimize_pose_windows)"""
+    return optimize_pose_windows(pred7, vos7, fc_vos=fc_vos, sax=sax, saq=saq, srx=srx, srq=srq, robust_c=robust_c)
 
 
 def pose_errors(pred7, targ7):
@@ -1234,7 +1254,7 @@ def _sample_frames(pr, ds, frames, S, dev):
     return mean, cov
 
 
-def _evaluate_sampled(pr, ds, S, vo, vo_fc, zero_lag, pose_m, pose_s, sig, dev):
+def _evaluate_sampled(pr, ds, S, vo, vo_fc, zero_lag, pose_m, pose_s, sig, dev, robust_c=None):
     """evaluate_sequence(samples=S) once the arguments are checked: the draws of every frame, then one gather, one
     k_pgo_cov and one emit (with VO poses) or one emit, and one host synchronisation for the PGO status"""
     L_lib = _lib.lib()
@@ -1260,9 +1280,16 @@ def _evaluate_sampled(pr, ds, S, vo, vo_fc, zero_lag, pose_m, pose_s, sig, dev):
             mean.data_ptr(), cov.data_ptr(), F, sig["sax"], sig["saq"], ds.vo_poses.data_ptr(), ds.poses.shape[0],
             slots.ctypes.data, L * T, tab["vo_rows"].ctypes.data, L * E, p7.data_ptr(), s7.data_ptr(), vos7.data_ptr(),
             _lib.stream_ptr()), "mapnet_eval_sample_windows")
-        _lib.check(L_lib.mapnet_pgo_optimize_cov(p7.data_ptr(), s7.data_ptr(), vos7.data_ptr(), opt7.data_ptr(),
-                                                 post36.data_ptr(), L, T, 1 if vo_fc else 0, sig["srx"], sig["srq"], 10,
-                                                 status.data_ptr(), _lib.stream_ptr()), "mapnet_pgo_optimize_cov")
+        if robust_c is None:
+            _lib.check(L_lib.mapnet_pgo_optimize_cov(p7.data_ptr(), s7.data_ptr(), vos7.data_ptr(), opt7.data_ptr(),
+                                                     post36.data_ptr(), L, T, 1 if vo_fc else 0, sig["srx"], sig["srq"],
+                                                     10, status.data_ptr(), _lib.stream_ptr()), "mapnet_pgo_optimize_cov")
+        else:
+            w = torch.empty((L, T), **f64)
+            _lib.check(L_lib.mapnet_pgo_optimize_cov_robust(
+                p7.data_ptr(), s7.data_ptr(), vos7.data_ptr(), opt7.data_ptr(), post36.data_ptr(), L, T,
+                1 if vo_fc else 0, sig["srx"], sig["srq"], 10, robust_c, w.data_ptr(), status.data_ptr(),
+                _lib.stream_ptr()), "mapnet_pgo_optimize_cov_robust")
     m = s = None
     if pose_m is not None:
         m = (ctypes.c_double * 3)(*[float(v) for v in np.asarray(pose_m).reshape(3)])
@@ -1280,12 +1307,16 @@ def _evaluate_sampled(pr, ds, S, vo, vo_fc, zero_lag, pose_m, pose_s, sig, dev):
         raise np.linalg.LinAlgError("pose graph: the normal matrix of a window of the sequence is not positive definite")
     est = SampledTracker._est(out)
     t_err, q_err = pose_errors(est["pose7"], targ7)
-    return dict(pred7=est["pose7"], targ7=targ7, t_err=t_err, q_err=q_err, n_frames=F, cov=est["cov"],
-                t_std=est["t_std"], q_std_deg=est["q_std_deg"], d2=d2, u=u, nll=nll)
+    res = dict(pred7=est["pose7"], targ7=targ7, t_err=t_err, q_err=q_err, n_frames=F, cov=est["cov"],
+               t_std=est["t_std"], q_std_deg=est["q_std_deg"], d2=d2, u=u, nll=nll)
+    if robust_c is not None:
+        res["w"] = w[:, keep].contiguous()
+    return res
 
 
 @torch.no_grad()
-def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, zero_lag=False, samples=None, **sigmas):
+def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, zero_lag=False, samples=None,
+                      robust_c=None, **sigmas):
     """The whole loop of scripts/eval.py:117-199 over a device-resident sequence: the windows of MF(steps, skip,
     variable_skip, no_duplicates=False) -- or single frames when dataset.steps is None -- one per frame index, in index
     order.  Returns what evaluate_tuples returns (pred7 [L,7], targ7 [L,7], t_err, q_err: the middle frame of each
@@ -1326,8 +1357,15 @@ def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, zer
     np.linalg.LinAlgError.  The model is a Predictor of any precision or a live bf16 / tc_split model (run by a
     temporary Predictor); a live model without a sampled engine raises ValueError.  Launches past the per-chunk
     assembly and engine replay: one gather, one k_pgo_cov and one emit (one emit without VO poses), and one host
-    synchronisation."""
+    synchronisation.
+
+    robust_c=c (a finite number > 0, in sigmas; needs dataset.vo_poses) gives the absolute factors of every window the
+    Cauchy loss of scale c (common.pgo: optimize_pose_windows / optimize_pose_windows_cov with robust_c), on the point
+    path and with samples, zero_lag and variable skips alike, and the result gains w [L], the final weight of each
+    item's kept slot: near 1 for a frame its window agrees with, near 0 for one it overrules.  The trackers given the
+    same robust_c produce these poses bit for bit.  A bad robust_c raises ValueError before anything is launched."""
     from .data.loader import DeviceDataset
+    robust_c = check_robust_c(robust_c)
     ds = dataset
     if not isinstance(ds, DeviceDataset):
         raise TypeError("evaluate_sequence needs a geomapnet_b200.data.DeviceDataset, got %s" % type(ds).__name__)
@@ -1347,6 +1385,8 @@ def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, zer
         raise ValueError("pose-graph optimisation needs windows of >= 2 frames (dataset.steps)")
     if vo_fc and not vo:
         raise ValueError("vo_fc: the dataset has no vo_poses")
+    if robust_c is not None and not vo:
+        raise ValueError("robust_c weighs the absolute factors of a pose graph: the dataset has no vo_poses")
     droprate = pr.droprate if pr is not None else float(net.droprate)
     cap = ds.max_batch * ds.frames_per_item                  # frames the dataset's cache assembles per call
     if samples is not None:
@@ -1362,7 +1402,7 @@ def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, zer
         if not all(v > 0 for v in sig.values()):
             raise ValueError("sax, saq, srx, srq must be positive, got %s" % (sig,))
         with _eval_pass(model, pr, net, dev, min(64, cap)) as pr:
-            return _evaluate_sampled(pr, ds, S, vo, vo_fc, zero_lag, pose_m, pose_s, sig, dev)
+            return _evaluate_sampled(pr, ds, S, vo, vo_fc, zero_lag, pose_m, pose_s, sig, dev, robust_c)
     B = min(pr.max_batch if pr is not None else 64, cap)
     if droprate > 0:
         if B < T:
@@ -1384,8 +1424,13 @@ def evaluate_sequence(model, dataset, pose_m=None, pose_s=None, vo_fc=False, zer
             tab["windows"].ctypes.data, tab["slots"].ctypes.data, L * T,
             tab["vo_rows"].ctypes.data if vo else None, L * E if vo else 0, pred7.data_ptr(), targ7.data_ptr(),
             vos7.data_ptr() if vo else None, _lib.stream_ptr()), "mapnet_eval_windows")
-        out = _window_errors(pgo(pred7, vos7, fc_vos=vo_fc, **sigmas) if vo else pred7, targ7, pose_m, pose_s,
-                             last=zero_lag)
+        if robust_c is None:
+            out = _window_errors(pgo(pred7, vos7, fc_vos=vo_fc, **sigmas) if vo else pred7, targ7, pose_m, pose_s,
+                                 last=zero_lag)
+        else:
+            opt, w = pgo(pred7, vos7, fc_vos=vo_fc, robust_c=robust_c, **sigmas)
+            out = _window_errors(opt, targ7, pose_m, pose_s, last=zero_lag)
+            out["w"] = w[:, T - 1 if zero_lag else T // 2].contiguous()
     return dict(out, n_frames=F)
 
 

@@ -264,6 +264,24 @@ int mapnet_pgo_optimize_cov(const double* poses, const double* sig7, const doubl
                             int n_windows, int N, int fc_vos, double srx, double srq, int n_iters, int* status_dev,
                             void* stream);
 
+/* mapnet_pgo_optimize_robust / mapnet_pgo_optimize_cov_robust: mapnet_pgo_optimize / mapnet_pgo_optimize_cov with the
+ * Cauchy loss rho(s) = c^2 log(1 + s / c^2) on the absolute factors (the relative ones stay squared errors), solved by
+ * iteratively reweighted Gauss-Newton.  Slot k's whitened absolute residual r_k is (sax^-1/2 (t_k - t^_k), saq^-1/2
+ * (q_k - q^_k)) for mapnet_pgo_optimize_robust and C^-1 (z_k - p_k) for mapnet_pgo_optimize_cov_robust; in every
+ * iteration its weight w_k = 1 / (1 + |r_k|^2 / c^2), taken at the iteration's starting state, multiplies the slot's
+ * contributions to H and b.  The step rule is the plain call's (flags bit 0; the exact step for _cov), and
+ * mapnet_pgo_optimize_cov_robust's posterior is taken at the returned state with the weights at that state.  c (HOST
+ * value) is in whitened units, multiples of sigma: finite and > 0.  w (may be NULL) [n_windows][N] float64 gets each
+ * slot's weight at the returned state.  A slot 20 sigma off at c = 2 weighs 1/101.  Other arguments, outputs, checks
+ * and the status word are the plain call's; the plain calls are unchanged.  (Added in ABI version 2, backward
+ * compatible.) */
+int mapnet_pgo_optimize_robust(const double* poses, const double* vos, double* out, int n_windows, int N, int fc_vos,
+                               double sax, double saq, double srx, double srq, int n_iters, int flags, double c,
+                               double* w, int* status_dev, void* stream);
+int mapnet_pgo_optimize_cov_robust(const double* poses, const double* sig7, const double* vos, double* out,
+                                   double* cov, int n_windows, int N, int fc_vos, double srx, double srq, int n_iters,
+                                   double c, double* w, int* status_dev, void* stream);
+
 /* ---- streaming pose-graph tracker (csrc/loader.cu; geomapnet_b200.inference.Tracker): scripts/eval.py's MapNet+PGO
  * loop over frames as they arrive.  The window of frame c is eval.py's MF(steps=T, skip) tuple: slot k holds frame
  * clip(c + (k - T/2) * skip, 0, last), its VOs are calc_vos_safe of the VO-library poses of consecutive slots (or of
@@ -292,6 +310,11 @@ int mapnet_pgo_optimize_cov(const double* poses, const double* sig7, const doubl
  *   mapnet_track_reset: stream-ordered: the next step is frame 0 of a new sequence, the status word is cleared.
  *   mapnet_track_status: synchronises the stream and returns the frames seen and the status (1: a window's normal
  *     matrix was not positive definite, where scipy's cholesky raises).
+ *   mapnet_track_set_robust: every window of the handle takes the Cauchy loss of scale c on its absolute factors
+ *     (mapnet_pgo_optimize_robust with flags 0).  Only before the handle's first step or flush, so a handle keeps one
+ *     loss for its lifetime; c finite and > 0.  Host-only: nothing is launched, and the three launches per call stay.
+ *     The same call exists for the three other tracker handles (mapnet_track_sample_set_robust, ...).  (Added in ABI
+ *     version 2, backward compatible.)
  * Pointers are device memory unless marked HOST.  Argument errors return non-zero before any launch. */
 typedef struct mapnet_track mapnet_track_t;
 int mapnet_track_create(mapnet_track_t** out, int T, int skip, int fc_vos, int max_batch, const double* sigmas4,
@@ -302,6 +325,7 @@ int mapnet_track_step_now(mapnet_track_t* h, const float* pred6, const float* vo
 int mapnet_track_flush(mapnet_track_t* h, double* out7, void* stream);
 int mapnet_track_reset(mapnet_track_t* h, void* stream);
 int mapnet_track_status(mapnet_track_t* h, int64_t* frames_seen, int* failed, void* stream);
+int mapnet_track_set_robust(mapnet_track_t* h, double c);
 int mapnet_track_destroy(mapnet_track_t* h);
 
 /* ---- multi-stream tracker (csrc/loader.cu; geomapnet_b200.inference.MultiTracker): n_streams independent sequences,
@@ -329,6 +353,7 @@ int mapnet_track_destroy(mapnet_track_t* h);
  *   mapnet_track_multi_status: synchronises the stream and returns stream s's frames seen and status (1: a window of s
  *     had a normal matrix that was not positive definite; k_pgo flags windows one by one, so other streams are not
  *     marked).
+ *   mapnet_track_multi_set_robust: mapnet_track_set_robust for every stream of the handle.
  * Pointers are device memory unless marked HOST.  Argument errors return non-zero before any launch. */
 #define MAPNET_TRACK_MAX_STREAMS 65536
 typedef struct mapnet_track_multi mapnet_track_multi_t;
@@ -339,6 +364,7 @@ int mapnet_track_multi_step(mapnet_track_multi_t* h, const float* pred6, const f
 int mapnet_track_multi_flush(mapnet_track_multi_t* h, int s, double* out7, void* stream);
 int mapnet_track_multi_reset(mapnet_track_multi_t* h, int s, void* stream);
 int mapnet_track_multi_status(mapnet_track_multi_t* h, int s, int64_t* frames_seen, int* failed, void* stream);
+int mapnet_track_multi_set_robust(mapnet_track_multi_t* h, double c);
 int mapnet_track_multi_destroy(mapnet_track_multi_t* h);
 
 /* ---- Monte-Carlo tracker (csrc/loader.cu; geomapnet_b200.inference.SampledTracker): mapnet_track_t's windows, lag,
@@ -358,6 +384,7 @@ int mapnet_track_multi_destroy(mapnet_track_multi_t* h);
  *     frame (mapnet_track_step_now's windows).
  *   mapnet_track_sample_flush / _reset / _status / _destroy: as mapnet_track_*; the status is also set when a frame's
  *     S7 is not positive definite.
+ *   mapnet_track_sample_set_robust: mapnet_track_set_robust, with mapnet_pgo_optimize_cov_robust's weights.
  * Pointers are device memory unless marked HOST.  Argument errors return non-zero before any launch. */
 typedef struct mapnet_track_sample mapnet_track_sample_t;
 int mapnet_track_sample_create(mapnet_track_sample_t** out, int T, int skip, int fc_vos, int max_batch,
@@ -369,6 +396,7 @@ int mapnet_track_sample_step_now(mapnet_track_sample_t* h, const double* mean6, 
 int mapnet_track_sample_flush(mapnet_track_sample_t* h, double* out, void* stream);
 int mapnet_track_sample_reset(mapnet_track_sample_t* h, void* stream);
 int mapnet_track_sample_status(mapnet_track_sample_t* h, int64_t* frames_seen, int* failed, void* stream);
+int mapnet_track_sample_set_robust(mapnet_track_sample_t* h, double c);
 int mapnet_track_sample_destroy(mapnet_track_sample_t* h);
 /* mapnet_test_sample_factor: what mapnet_track_sample_step forms for each of n frames, with its arithmetic: p7 [n][7]
  * and S7 [n][7][7] from mean6 [n][6] and cov36 [n][6][6] (device pointers, float64) and the floors sax, saq > 0. */
@@ -395,6 +423,7 @@ int mapnet_test_sample_factor(const double* mean6, const double* cov36, int64_t 
  *     frame 0 and its status word is cleared.
  *   mapnet_track_multi_sample_status: synchronises the stream and returns stream s's frames seen and status (1: a
  *     window of s had a normal matrix or a frame's S7 that was not positive definite; other streams are not marked).
+ *   mapnet_track_multi_sample_set_robust: mapnet_track_sample_set_robust for every stream of the handle.
  * Pointers are device memory unless marked HOST.  Argument errors return non-zero before any launch. */
 typedef struct mapnet_track_multi_sample mapnet_track_multi_sample_t;
 int mapnet_track_multi_sample_create(mapnet_track_multi_sample_t** out, int n_streams, int T, int skip, int fc_vos,
@@ -407,6 +436,7 @@ int mapnet_track_multi_sample_flush(mapnet_track_multi_sample_t* h, int s, doubl
 int mapnet_track_multi_sample_reset(mapnet_track_multi_sample_t* h, int s, void* stream);
 int mapnet_track_multi_sample_status(mapnet_track_multi_sample_t* h, int s, int64_t* frames_seen, int* failed,
                                      void* stream);
+int mapnet_track_multi_sample_set_robust(mapnet_track_multi_sample_t* h, double c);
 int mapnet_track_multi_sample_destroy(mapnet_track_multi_sample_t* h);
 
 /* ---- eval-mode inference engine (csrc/infer.cu): a frozen snapshot of a PoseNet / MapNet trunk for
